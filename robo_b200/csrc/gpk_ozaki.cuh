@@ -9,7 +9,11 @@
 // operand relative to its row maximum and the triangle s + t < 7 has 28 slice pairs (tools/ozaki_study.py prints the
 // error of this split against 7-bit truncated digits).  The pairs of one level share one int32 accumulator
 // ((lvl + 1) K 128^2 < 2^31 for K <= 16384), so a tile keeps 7 accumulators.  Per 64-byte k-block the CTA stages all
-// 7 + 7 slice tiles (TMA, 64B swizzle) once and issues 56 MMAs per warpgroup on them.
+// 7 + 7 slice tiles (TMA, 64B swizzle) once and issues 56 MMAs per warpgroup on them.  The L^-1 slice is the A operand
+// and comes from registers (ldmatrix once per slice and k-block, reused by its 7 - s levels); only the K* slice is read
+// from shared memory by every MMA.  With both operands in shared memory the 56 MMAs read 168 KB per warpgroup and
+// k-block, more than the SM's shared-memory bandwidth delivers at the tensor pipe's issue rate; in registers, 84 KB
+// (tools/microbench/int8_operand_rates.cu measures both forms).
 // Accuracy (tools/ozaki_study.py): the split is exact to 2^-57 of the row maximum per operand; the handle falls back to
 // the fp64 DMMA kernel when the factor is worse conditioned than max |L^-1| < 64 (eP > OZ_MAX_EXP) or N > 16384.
 //
@@ -23,8 +27,7 @@
 constexpr int OZ_S = 7;                       // slices (balanced base-256 digits) per operand
 constexpr int OZ_PAIRS = OZ_S * (OZ_S + 1) / 2;   // slice pairs with s + t < OZ_S
 // Tile: 128 rows of L^-1 x 32 candidates.  Each of the two consumer warpgroups owns 64 rows and keeps the 7 level
-// accumulators of its 64 x 32 share in registers (7 x 16 = 112 int32 per thread): a wider tile would not fit the
-// register file next to the epilogue.
+// accumulators of its 64 x 32 share in registers (7 x 16 = 112 int32 per thread), next to two 8-register A fragments.
 constexpr int OZ_TM = 128, OZ_TN = 32;
 constexpr int OZ_KB = 64;                     // k-block: 64 int8 = one 64-byte swizzle row
 constexpr int OZ_UK = 32;                     // K of one wgmma m64n32k32 s8
@@ -70,17 +73,33 @@ __device__ __forceinline__ uint64_t oz_desc(uint32_t smem_addr) {
 }
 #define OZ_ACC16(d) "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), \
                     "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
-// d (64 x 32 s32, wgmma accumulator layout) (+)= A (64 x 32 s8, K-major) * B (32 x 32 s8, K-major)^T
-__device__ __forceinline__ void oz_wgmma(uint32_t (&d)[16], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
-                 "wgmma.mma_async.sync.aligned.m64n32k32.s32.s8.s8 "
-                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p;\n\t}"
-                 : OZ_ACC16(d) : "l"(a_desc), "l"(b_desc), "r"(accumulate));
+// d (64 x 32 s32, wgmma accumulator layout) += A (64 x 32 s8, from registers: one fragment of oz_lda_frag) *
+// B (32 x 32 s8, K-major in shared memory)^T
+__device__ __forceinline__ void oz_wgmma_rs(uint32_t (&d)[16], const uint32_t (&a)[4], uint64_t b_desc) {
+    asm volatile("wgmma.mma_async.sync.aligned.m64n32k32.s32.s8.s8 "
+                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, 1;"
+                 : OZ_ACC16(d) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc));
+}
+// A fragments of one 64-byte k-block (two k32 halves) of a 64-row, 64B-swizzled K-major slice tile at `tile`, for the
+// warp's 16 rows starting at row0.  The wgmma register layout of an s8 A fragment (reg 0: row lane/4, k 4 (lane%4) ..
+// + 3; reg 1: row + 8; regs 2, 3: the same at k + 16) is what ldmatrix.x4 of four 8-row x 16-byte matrices delivers.
+// Lane L addresses row L % 8 + 8 ((L / 8) & 1), 16-byte chunk L / 16 of the half; SWIZZLE_64B XORs the chunk index
+// (address bits 4-5) with bits 7-8, i.e. with (row / 2) % 4 for 64-byte rows.
+__device__ __forceinline__ void oz_lda_frag(uint32_t (&a)[2][4], uint32_t tile, int row0, int lane) {
+    const int r = row0 + (lane & 7) + ((lane >> 3) & 1) * 8;
+#pragma unroll
+    for (int k = 0; k < OZ_KB / OZ_UK; ++k) {
+        const int chunk = 2 * k + (lane >> 4);
+        const uint32_t addr = tile + (uint32_t)(r * OZ_KB + ((chunk ^ ((r >> 1) & 3)) << 4));
+        asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+                     : "=r"(a[k][0]), "=r"(a[k][1]), "=r"(a[k][2]), "=r"(a[k][3]) : "r"(addr) : "memory");
+    }
 }
 __device__ __forceinline__ void oz_wgmma_fence(uint32_t (&d)[16]) { asm volatile("" : OZ_ACC16(d) :: "memory"); }
 __device__ __forceinline__ void wgmma_arrive() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_one() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
 
 // exact int32 -> fp64 without the quarter-rate I2F.F64: 2^52 + 2^31 + d as bit pattern, minus the constant
 __device__ __forceinline__ double oz_i2d(uint32_t d) {
@@ -141,9 +160,10 @@ struct OzArgs {
 // The contraction: tile t of the L2-grouped, longest-first order (oz_tile_of) for t = blockIdx.x, + gridDim.x, ...
 // A grid of one CTA per tile does one tile each; a grid of one CTA per SM ("ozpersist" = 1) walks the list, so
 // barriers and the pipeline fill are paid once and the producer runs ahead into the next tile during the epilogue.
-// Warpgroup 0 (one thread) streams the 7 + 7 slice tiles of each 64-byte k-block into a 3-stage ring with TMA;
-// warpgroups 1 and 2 each issue the 56 wgmma m64n32k32 of their 64 rows per stage, then fold the 7 level accumulators
-// to fp64 (least significant level first), scale by the row exponent, square and reduce over the tile's 128 rows.
+// Warpgroup 0 (one thread, 40 registers after setmaxnreg) streams the 7 + 7 slice tiles of each 64-byte k-block into a
+// 3-stage ring with TMA; warpgroups 1 and 2 (232 registers) each issue the 56 wgmma m64n32k32 of their 64 rows per
+// stage with the L^-1 slice in registers, then fold the 7 level accumulators to fp64 (least significant level first),
+// scale by the row exponent, square and reduce over the tile's 128 rows.
 // ---------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(OZ_THREADS, 1)
 gpk_oz_vargemm_kernel(const __grid_constant__ CUtensorMap mapP, const __grid_constant__ CUtensorMap mapK, const OzArgs g)
@@ -163,6 +183,7 @@ gpk_oz_vargemm_kernel(const __grid_constant__ CUtensorMap mapP, const __grid_con
     __syncthreads();
 
     if (wg == 0) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
         if (tid == 0) {
             int it = 0;
             for (int t = blockIdx.x; t < total; t += gridDim.x) {
@@ -187,38 +208,52 @@ gpk_oz_vargemm_kernel(const __grid_constant__ CUtensorMap mapP, const __grid_con
     }
     // consumers: warpgroup c = wg - 1 owns tile rows 64 c .. 64 c + 63; accumulator element e of a thread sits at row
     // 16 w + lane / 4 + 8 ((e >> 1) & 1), column 8 (e >> 2) + 2 (lane % 4) + (e & 1)   (w = warp within the warpgroup)
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
     const int c = wg - 1, cw = (tid - 128) >> 5;                     // cw: consumer warp 0..7
     const int r0 = c * 64 + (cw & 3) * 16 + (lane >> 2);
     int it = 0, tl = 0;
     for (int t = blockIdx.x; t < total; t += gridDim.x, ++tl) {
         int ib, cb;
         oz_tile_of(t, g.nb, g.ncb, g.group, ib, cb);
-        const int nkb = (ib + 1) * OZ_TM / OZ_KB;
+        const int nkb = (ib + 1) * OZ_TM / OZ_KB;                    // even: the k-loop takes two stages per pass
         uint32_t acc[OZ_S][16];
 #pragma unroll
         for (int l = 0; l < OZ_S; ++l)
 #pragma unroll
             for (int e = 0; e < 16; ++e) acc[l][e] = 0u;
-        for (int kb = 0; kb < nkb; ++kb, ++it) {
-            const int s = it % OZ_NSTG;
-            oz_mbar_wait(bar_full + 8 * s, (uint32_t)((it / OZ_NSTG) & 1));
-            const uint32_t st = base + s * OZ_STAGE;
-            wgmma_arrive();
+        // Slice s of L^-1 is loaded into registers once per k-block and multiplies the K* slices t = 0 .. 6 - s into
+        // acc[s + t]: one commit group per slice.  The fragment is double-buffered over the global slice sequence (two
+        // stages = 14 slices per pass keep the buffer index static); wait_group 1 after each commit retires the group
+        // two slices back, so its buffer can be reloaded, and after slice 0 of a stage, the previous stage's last group,
+        // so that stage is handed back to the producer while this one runs.
+        uint32_t fa[2][2][4];
+        for (int kb = 0; kb < nkb; kb += 2) {
 #pragma unroll
-            for (int lvl = 0; lvl < OZ_S; ++lvl)
+            for (int h = 0; h < 2; ++h, ++it) {
+                const int s = it % OZ_NSTG;
+                oz_mbar_wait(bar_full + 8 * s, (uint32_t)((it / OZ_NSTG) & 1));
+                const uint32_t st = base + s * OZ_STAGE;
 #pragma unroll
-                for (int a = 0; a <= lvl; ++a)
+                for (int a = 0; a < OZ_S; ++a) {
+                    uint32_t (&f)[2][4] = fa[(h * OZ_S + a) & 1];
+                    oz_lda_frag(f, st + a * OZ_A_SLICE, c * 64 + (cw & 3) * 16, lane);
+                    wgmma_arrive();
 #pragma unroll
-                    for (int k = 0; k < OZ_KB / OZ_UK; ++k)
-                        oz_wgmma(acc[lvl], oz_desc(st + a * OZ_A_SLICE + c * 64 * OZ_KB + k * OZ_UK),
-                                 oz_desc(st + OZ_S * OZ_A_SLICE + (lvl - a) * OZ_B_SLICE + k * OZ_UK),
-                                 (uint32_t)((kb | a | k) != 0));
-            wgmma_commit();
-            wgmma_wait_all();
+                    for (int tk = 0; tk < OZ_S - a; ++tk)
 #pragma unroll
-            for (int l = 0; l < OZ_S; ++l) oz_wgmma_fence(acc[l]);
-            if ((tid & 127) == 0) mbar_arrive(bar_empty + 8 * s);    // this warpgroup no longer reads stage s
+                        for (int k = 0; k < OZ_KB / OZ_UK; ++k)
+                            oz_wgmma_rs(acc[a + tk], f[k], oz_desc(st + OZ_S * OZ_A_SLICE + tk * OZ_B_SLICE + k * OZ_UK));
+                    wgmma_commit();
+                    wgmma_wait_one();
+                    if (a == 0 && (h == 1 || kb > 0) && (tid & 127) == 0)
+                        mbar_arrive(bar_empty + 8 * ((it + OZ_NSTG - 1) % OZ_NSTG));   // previous stage fully read
+                }
+            }
         }
+        wgmma_wait_all();
+#pragma unroll
+        for (int l = 0; l < OZ_S; ++l) oz_wgmma_fence(acc[l]);
+        if ((tid & 127) == 0) mbar_arrive(bar_empty + 8 * ((it + OZ_NSTG - 1) % OZ_NSTG));
         const double rs0 = ldexp(1.0, g.eP[ib * OZ_TM + r0] + g.eK), rs1 = ldexp(1.0, g.eP[ib * OZ_TM + r0 + 8] + g.eK);
         // per thread 8 columns x 2 rows; column sums over the warp's 16 rows (lanes with equal lane % 4), then over warps
         double col[8];
