@@ -73,9 +73,11 @@ const char* gpk_version(void);
  *               (gpk_ozaki.cuh); used while max |L^-1| < 64 and N <= 16384, otherwise the fp64 kernel runs [default;
  *               batches of >= 2048 candidates]; 0 = always fp64 DMMA.  The posterior mean never goes through the digits
  *               (fp64 K* alpha)
- *   "ozpersist" 0 = one CTA per tile; 1 = one CTA per SM walks the tile list; 3 = automatic [default]: persistent for
- *               N <= 3072, one CTA per tile above (on an H100 the walk shortens a scoring pass up to N = 2048, is even at
- *               3072 and costs 10 % at 4096: tools/persist_threshold.py)
+ *   "ozpersist" 0 = one CTA per tile; 1 = one CTA per SM walks the tile list (by clusters); 3 = automatic [default]:
+ *               persistent for N <= 4096, one CTA per tile above (tools/persist_threshold.py, DESIGN.md 9.5)
+ *   "ozcluster" 1, 2 or 4 [default 4] = CTAs per cluster of the int8 contraction: they take adjacent candidate blocks of
+ *               one row block and share its L^-1 digit slices by TMA multicast, so each CTA reads 1 / CS of them from L2.
+ *               Every value gives bit-identical results
  *   "ozpdl"     1 = the look-ahead K* builder runs as a small resident grid ("covctas" CTAs per SM) that triggers a
  *               programmatic dependent launch of the contraction behind it on the same stream (the two really co-run);
  *               0 = builder on the side stream (the block scheduler places it in the contraction's tail) [default: the
@@ -302,7 +304,7 @@ int gpk_get_z(gpk_handle* h, double* z /* n */);
  * out[10] = of those, launches of the int8 (Ozaki) contraction; out[11] = largest row exponent of L^-1 seen by it
  * (option "ozaki"); out[12] = option "persist"; out[13] = int8 slice-pair products the int8 contraction spends per
  * fp64 product (28: 7 balanced base-256 digits per operand); out[14] = which int8 kernel ran last (1 gpk_oz_vargemm_kernel;
- * + 8: persistent tile walk); out[15] reserved (zero). */
+ * + 8: persistent tile walk; + 16 / + 32: clusters of 2 / 4 CTAs); out[15] reserved (zero). */
 int gpk_get_timings(gpk_handle* h, double* out16);
 /* diagnostics of the blocked diagonal-block kernel (option "diagprof" = 1): clock64() stamps of the last
  * launched block: out[0] start, out[1] tiles loaded, out[2+2p] panel p factorised + solved, out[3+2p] panel p's

@@ -146,7 +146,8 @@ class Handle(object):
         # implementation switches (all default-on variants have a cross-check twin): GPK_COV=1|2, GPK_PERSIST=0|1,
         # GPK_CHAINSPLIT=0|1, GPK_OZAKI=0|1
         for env, key in (("GPK_COV", "cov"), ("GPK_PERSIST", "persist"), ("GPK_CHAINSPLIT", "chainsplit"),
-                         ("GPK_OZAKI", "ozaki"), ("GPK_GRAPH", "graph"), ("GPK_DEPTH2", "depth2"), ("GPK_OZFUSED", "ozfused"), ("GPK_OZPERSIST", "ozpersist"), ("GPK_OZPDL", "ozpdl"), ("GPK_COVCTAS", "covctas")):
+                         ("GPK_OZAKI", "ozaki"), ("GPK_GRAPH", "graph"), ("GPK_DEPTH2", "depth2"), ("GPK_OZFUSED", "ozfused"), ("GPK_OZPERSIST", "ozpersist"), ("GPK_OZPDL", "ozpdl"), ("GPK_COVCTAS", "covctas"),
+                         ("GPK_OZCLUSTER", "ozcluster")):
             if os.environ.get(env):
                 self.set_option(key, int(os.environ[env]))
 

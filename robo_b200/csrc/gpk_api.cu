@@ -54,10 +54,14 @@ struct gpk_handle {
                                     //    contraction behind it on the SAME stream (real overlap); 0: side stream (tail overlap only)
     int cov_ctas = 2;               // CTAs per SM of that resident builder grid
     int oz_last_variant = 0;        // contraction of the last int8 launch: 1 = gpk_oz_vargemm_kernel, + 8 when it walked the tile
-                                    // list persistently
+                                    // list persistently, + 16 / + 32 in clusters of 2 / 4 CTAs
+    int oz_cluster = 4;             // CTAs per cluster of the int8 contraction (1, 2 or 4): they share the L^-1 slices by TMA
+                                    // multicast [default 4: tools/persist_threshold.py and bench.py on an H100, DESIGN 9.5]
+    int oz_map_cs = 0;              // cluster size mapOzP's box was encoded for (0: not encoded)
+    int oz_max_clusters[5] = {0, 0, 0, 0, 0};   // co-resident clusters of the contraction per cluster size (0: not queried)
     int oz_persist = 3;             // 1: one CTA per SM walks the tile list; 0: one CTA per tile; 3 = automatic [default]: persistent
-                                    // for N <= 3072 (tools/persist_threshold.py on an H100: a scoring pass 2-12 % shorter up to
-                                    // N = 2048, equal at 3072, 10 % longer at 4096 and 6144)
+                                    // for N <= 4096 (tools/persist_threshold.py and bench.py on an H100 with 4-CTA clusters: the
+                                    // walk is as fast or faster up to N = 4096, one CTA per tile is faster at 6144)
     int oz_fused = 1;               // 1: K* leaves the covariance builder as int8 digits (gpk_cov_oz_kernel); 0: fp64 K* + split + dot
     long oz_linv_serial = -1;       // linv_serial the slices of L^-1 were made for
     long linv_serial = 0;           // bumped whenever L^-1 is (re)built
@@ -324,26 +328,62 @@ cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t s
     return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
 }
 
-// int8 contraction launch with an optional programmatic dependency on the kernel launched just before it on the stream
-// (the resident look-ahead K* builder, which triggers at its start)
+// int8 contraction launch in clusters of cs CTAs (grid a multiple of cs), with an optional programmatic dependency on the
+// kernel launched just before it on the stream (the resident look-ahead K* builder, which triggers at its start)
 template <typename... KArgs, typename... Args>
-cudaError_t launch_oz(void (*kernel)(KArgs...), unsigned grid, size_t smem, cudaStream_t stream, bool dependent, Args... args) {
+cudaError_t launch_oz(void (*kernel)(KArgs...), unsigned grid, int cs, size_t smem, cudaStream_t stream, bool dependent,
+                      Args... args) {
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = dim3(grid);
     cfg.blockDim = dim3(OZ_THREADS);
     cfg.dynamicSmemBytes = smem;
     cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
+    cudaLaunchAttribute attr[2];
     int na = 0;
     if (dependent) {
         attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
         attr[na].val.programmaticStreamSerializationAllowed = 1;
         ++na;
     }
+    if (cs > 1) {
+        attr[na].id = cudaLaunchAttributeClusterDimension;
+        attr[na].val.clusterDim.x = (unsigned)cs;
+        attr[na].val.clusterDim.y = 1;
+        attr[na].val.clusterDim.z = 1;
+        ++na;
+    }
     cfg.attrs = attr;
     cfg.numAttrs = na;
     return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
+}
+
+// How many clusters of cs contraction CTAs fit on the device at once (the grid of the persistent walk), once per handle
+int oz_max_clusters(gpk_handle* h, int cs, int* out) {
+    if (h->oz_max_clusters[cs] == 0) {
+        if (cs == 1) {
+            h->oz_max_clusters[cs] = std::max(h->n_sm, 1);
+        } else {
+            cudaLaunchConfig_t cfg;
+            memset(&cfg, 0, sizeof(cfg));
+            cfg.gridDim = dim3((unsigned)cs);
+            cfg.blockDim = dim3(OZ_THREADS);
+            cfg.dynamicSmemBytes = OZ_SMEM;
+            cudaLaunchAttribute attr[1];
+            attr[0].id = cudaLaunchAttributeClusterDimension;
+            attr[0].val.clusterDim.x = (unsigned)cs;
+            attr[0].val.clusterDim.y = 1;
+            attr[0].val.clusterDim.z = 1;
+            cfg.attrs = attr;
+            cfg.numAttrs = 1;
+            int n = 0;
+            CK(cudaOccupancyMaxActiveClusters(&n, gpk_oz_vargemm_kernel, &cfg));
+            if (n < 1) { set_err(h, "no cluster of %d int8 contraction CTAs fits on this device", cs); return GPK_CUDA_ERROR; }
+            h->oz_max_clusters[cs] = n;
+        }
+    }
+    *out = h->oz_max_clusters[cs];
+    return GPK_OK;
 }
 
 template <int EPI, int MI = 8>
@@ -766,8 +806,15 @@ int prepare_ozaki(gpk_handle* h, bool* usable) {
         CKL();
         CK(cudaMemcpyAsync(&h->oz_emax_host, h->oz_emax.p, 4, cudaMemcpyDeviceToHost, h->stream));
         CK(cudaStreamSynchronize(h->stream));
-        if ((rc = make_oz_map(h, &h->mapOzP, h->oz_Pq.p, (long)OZ_S * NP, NP, OZ_TM))) return rc;
+        h->oz_map_cs = 0;
         h->oz_linv_serial = h->linv_serial;
+    }
+    // each CTA of a cluster loads 128 / CS rows of every L^-1 slice; 64-row (CS = 2) and 32-row (CS = 4) offsets are
+    // multiples of the 512-byte SWIZZLE_64B atom, so the multicast pieces form the same swizzled 128-row tile
+    if (h->oz_map_cs != h->oz_cluster) {
+        int rc;
+        if ((rc = make_oz_map(h, &h->mapOzP, h->oz_Pq.p, (long)OZ_S * NP, NP, OZ_TM / h->oz_cluster))) return rc;
+        h->oz_map_cs = h->oz_cluster;
     }
     *usable = h->oz_emax_host <= OZ_MAX_EXP;
     return GPK_OK;
@@ -946,18 +993,25 @@ int score_dev(gpk_handle* h, const double* dX, long m, int kind, double eta, dou
             if (last) CK(cudaEventRecord(h->ev[10], h->stream));
             CK(cudaEventRecord(h->ev_g0[ci], h->stream));
         }
-        const int oz_persist = h->oz_persist == 3 ? (h->nb <= 24 ? 1 : 0) : h->oz_persist;
+        const int oz_persist = h->oz_persist == 3 ? (h->nb <= 32 ? 1 : 0) : h->oz_persist;
         if (use_oz) {
             OzArgs o;
             o.nb = h->nb; o.ncb = (int)(mcp / OZ_TN); o.NP = (int)NP; o.rows = (int)cap;
-            // a group's K* slices take about 24 MB, half of the L2
-            o.group = (int)std::min<long>(512, std::max<long>(4, ((long)24 << 20) / ((long)OZ_TN * NP * OZ_S)));
+            // a group's K* slices take about 24 MB, half of the L2; whole clusters of candidate blocks (ncb = mcp / 32 is a
+            // multiple of 4, so of every cluster size)
+            const int cs = h->oz_cluster;
+            o.group = (int)std::min<long>(512, std::max<long>(4, ((long)24 << 20) / ((long)OZ_TN * NP * OZ_S))) / cs * cs;
             o.eP = ptr<int>(h->oz_eP); o.eK = oz_eK;
             o.part_ssq = a.part_ssq; o.ldpart = a.ldpart;
             const int tiles = o.nb * o.ncb;
-            const int grid = oz_persist == 1 ? std::min(tiles, std::max(h->n_sm, 1)) : tiles;
-            h->oz_last_variant = 1 + (oz_persist == 1 ? 8 : 0);
-            CK(launch_oz(gpk_oz_vargemm_kernel, (unsigned)grid, (size_t)OZ_SMEM, h->stream, dependent, h->mapOzP,
+            int grid = tiles;
+            if (oz_persist == 1) {
+                int nclusters = 0;
+                if ((rc = oz_max_clusters(h, cs, &nclusters))) return rc;
+                grid = cs * std::min(tiles / cs, nclusters);
+            }
+            h->oz_last_variant = 1 + (oz_persist == 1 ? 8 : 0) + (cs == 2 ? 16 : cs == 4 ? 32 : 0);
+            CK(launch_oz(gpk_oz_vargemm_kernel, (unsigned)grid, cs, (size_t)OZ_SMEM, h->stream, dependent, h->mapOzP,
                          second ? h->mapOzK2 : h->mapOzK, o));
             CKL();
             h->oz_launches += 1;
@@ -1114,6 +1168,11 @@ int gpk_set_option(gpk_handle* h, const char* key, long value) {
     if (!strcmp(key, "ozpersist")) {
         if (value != 0 && value != 1 && value != 3) BAD("ozpersist must be 0, 1 or 3");
         h->oz_persist = (int)value;
+        return GPK_OK;
+    }
+    if (!strcmp(key, "ozcluster")) {
+        if (value != 1 && value != 2 && value != 4) BAD("ozcluster must be 1, 2 or 4");
+        h->oz_cluster = (int)value;
         return GPK_OK;
     }
     if (!strcmp(key, "ozpdl")) {

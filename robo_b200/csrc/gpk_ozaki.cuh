@@ -9,7 +9,8 @@
 // operand relative to its row maximum and the triangle s + t < 7 has 28 slice pairs (tools/ozaki_study.py prints the
 // error of this split against 7-bit truncated digits).  The pairs of one level share one int32 accumulator
 // ((lvl + 1) K 128^2 < 2^31 for K <= 16384), so a tile keeps 7 accumulators.  Per 64-byte k-block the CTA stages all
-// 7 + 7 slice tiles (TMA, 64B swizzle) once and issues 56 MMAs per warpgroup on them.  The L^-1 slice is the A operand
+// 7 + 7 slice tiles (TMA, 64B swizzle) once and issues 56 MMAs per warpgroup on them; the CTAs of a cluster share the
+// L^-1 slices by TMA multicast (option "ozcluster").  The L^-1 slice is the A operand
 // and comes from registers (ldmatrix once per slice and k-block, reused by its 7 - s levels); only the K* slice is read
 // from shared memory by every MMA.  With both operands in shared memory the 56 MMAs read 168 KB per warpgroup and
 // k-block, more than the SM's shared-memory bandwidth delivers at the tensor pipe's issue rate; in registers, 84 KB
@@ -60,6 +61,41 @@ __device__ __forceinline__ int oz_digit_of(unsigned long long y, int s) { return
 
 __device__ __forceinline__ void oz_mbar_wait(uint32_t bar, uint32_t parity) {
     while (!mbar_try_wait(bar, parity)) { }
+}
+// ---- CTA clusters -------------------------------------------------------------------------------------------------
+// A launch without a cluster attribute is a cluster of one CTA: rank 0 of 1.
+__device__ __forceinline__ uint32_t oz_cluster_size() {
+    uint32_t n;
+    asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(n));
+    return n;
+}
+__device__ __forceinline__ uint32_t oz_cluster_rank() {
+    uint32_t r;
+    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+    return r;
+}
+// every thread of every CTA of the cluster; orders shared-memory and mbarrier operations across the cluster
+__device__ __forceinline__ void oz_cluster_sync() {
+    asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
+// TMA 2D load whose box lands at the same shared-memory offset in every CTA of cta_mask, and completes bytes on the
+// mbarrier at the same offset in each of them
+__device__ __forceinline__ void tma_load_2d_multicast(uint32_t smem_dst, const CUtensorMap* map, int c_inner, int c_outer,
+                                                      uint32_t bar, uint16_t cta_mask) {
+    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+                 " [%0], [%1, {%3, %4}], [%2], %5;"
+                 :: "r"(smem_dst), "l"((uint64_t)map), "r"(bar), "r"(c_inner), "r"(c_outer), "h"(cta_mask)
+                 : "memory");
+}
+// Hands a ring stage back to the producers: one arrival on the empty barrier at offset `bar` of every CTA of the
+// cluster, since each of their producers multicasts into this CTA's copy of the stage.  Called by threads 0 .. cs - 1
+// of a consumer warpgroup, thread r arriving for CTA r: the cs arrivals go out as one warp instruction.  The reads they
+// release are complete (ldmatrix into registers, wgmma retired by wait_group), so the default .cta release suffices.
+__device__ __forceinline__ void oz_release_stage(uint32_t bar, uint32_t cs, uint32_t r) {
+    if (cs == 1) { mbar_arrive(bar); return; }
+    uint32_t remote;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(bar), "r"(r));
+    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" :: "r"(remote) : "memory");
 }
 // K-major SWIZZLE_64B shared-memory matrix descriptor of wgmma: start address >> 4, leading byte offset (unused for
 // swizzled K-major layouts) 1, stride byte offset 512 (8 rows x 64 bytes), layout type 2 = SWIZZLE_64B in bits [62,64)
@@ -138,7 +174,8 @@ __global__ void gpk_oz_split_kernel(const double* __restrict__ A, long rows, lon
 // ---- the contraction ----------------------------------------------------------------------------------------------
 // Tile order: candidate blocks are taken in groups of `group` blocks whose K* slices (group x TN x NP x 7 bytes, about
 // half of the 50 MB L2, see score_dev) stay L2-resident while the group walks all row blocks of L^-1, longest
-// contraction first; without the grouping every row block re-reads the whole chunk's slices from HBM.
+// contraction first; without the grouping every row block re-reads the whole chunk's slices from HBM.  The kernel
+// calls it in units of cluster tiles (CS adjacent candidate blocks of one row block): ncb and group divided by CS.
 __device__ __forceinline__ void oz_tile_of(int id, int nb, int ncb, int group, int& ib, int& cb) {
     const int full = ncb / group;
     int grp = id / (nb * group), gsz = group;
@@ -150,7 +187,7 @@ __device__ __forceinline__ void oz_tile_of(int id, int nb, int ncb, int group, i
 
 struct OzArgs {
     int nb, ncb;                        // row blocks of L^-1 (128 rows), candidate blocks of the chunk (32 candidates)
-    int group;                          // candidate blocks per L2-resident group
+    int group;                          // candidate blocks per L2-resident group (a multiple of the cluster size)
     int NP, rows;                       // L^-1 is NP x NP; the K* slices have `rows` rows each
     const int* eP; int eK;
     double* part_ssq; long ldpart;
@@ -158,12 +195,18 @@ struct OzArgs {
 
 // ---------------------------------------------------------------------------------------
 // The contraction: tile t of the L2-grouped, longest-first order (oz_tile_of) for t = blockIdx.x, + gridDim.x, ...
-// A grid of one CTA per tile does one tile each; a grid of one CTA per SM ("ozpersist" = 1) walks the list, so
+// A grid of one CTA per tile does one tile each; a grid of as many clusters as fit at once ("ozpersist" = 1) walks the list, so
 // barriers and the pipeline fill are paid once and the producer runs ahead into the next tile during the epilogue.
 // Warpgroup 0 (one thread, 40 registers after setmaxnreg) streams the 7 + 7 slice tiles of each 64-byte k-block into a
 // 3-stage ring with TMA; warpgroups 1 and 2 (232 registers) each issue the 56 wgmma m64n32k32 of their 64 rows per
 // stage with the L^-1 slice in registers, then fold the 7 level accumulators to fp64 (least significant level first),
 // scale by the row exponent, square and reduce over the tile's 128 rows.
+// Launched in clusters of CS = 1, 2 or 4 CTAs (cluster size = the launch's cluster dimension): the CTAs of a cluster
+// take the same row block ib and the adjacent candidate blocks cb = CS p + rank, so they stage the same L^-1 slices.
+// Each producer loads 128 / CS rows of every L^-1 slice (mapP has a box of 128 / CS rows) and multicasts them into
+// the same stage of all CTAs of the cluster, and loads its own K* slices alone.  A stage is refilled only when the
+// consumers of every CTA of the cluster have released it: the empty barriers count 2 CS arrivals.  The persistent
+// walk goes by cluster tiles, so the CTAs of a cluster run the same k-block sequence.
 // ---------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(OZ_THREADS, 1)
 gpk_oz_vargemm_kernel(const __grid_constant__ CUtensorMap mapP, const __grid_constant__ CUtensorMap mapK, const OzArgs g)
@@ -173,37 +216,48 @@ gpk_oz_vargemm_kernel(const __grid_constant__ CUtensorMap mapP, const __grid_con
     const uint32_t bar_full = base + OZ_NSTG * OZ_STAGE, bar_empty = bar_full + 8 * OZ_NSTG;
     const uint32_t red = base + OZ_NSTG * OZ_STAGE + 256;            // 2 x [8 consumer warps][32 columns] partial sums of V^2
     const int tid = threadIdx.x, wg = tid >> 7, lane = tid & 31;
-    const int total = g.nb * g.ncb;
+    const uint32_t cs = oz_cluster_size(), rank = oz_cluster_rank();
+    const int ncl = (int)(gridDim.x / cs), cid = (int)(blockIdx.x / cs);     // clusters of the grid, this CTA's cluster
+    const int ncbc = g.ncb / (int)cs, gc = g.group / (int)cs;                // ... and the tile list in cluster tiles
+    const int total = g.nb * ncbc;
 
     if (tid == 0) {
-        for (int s = 0; s < OZ_NSTG; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 2); }
+        for (int s = 0; s < OZ_NSTG; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 2 * cs); }
         fence_barrier_init();
         fence_proxy_async();
     }
-    __syncthreads();
+    // peers multicast into this CTA's stages and arrive on its empty barriers only after they are initialised
+    if (cs > 1) oz_cluster_sync(); else __syncthreads();
 
     if (wg == 0) {
         asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
         if (tid == 0) {
+            const int prow = OZ_TM / (int)cs;                                         // L^-1 rows this CTA loads
+            const uint16_t mask = (uint16_t)((1u << cs) - 1u);
             int it = 0;
-            for (int t = blockIdx.x; t < total; t += gridDim.x) {
-                int ib, cb;
-                oz_tile_of(t, g.nb, g.ncb, g.group, ib, cb);
+            for (int t = cid; t < total; t += ncl) {
+                int ib, cbc;
+                oz_tile_of(t, g.nb, ncbc, gc, ib, cbc);
+                const int cb = cbc * (int)cs + (int)rank;
                 const int nkb = (ib + 1) * OZ_TM / OZ_KB;                                 // lower triangle only
                 for (int kb = 0; kb < nkb; ++kb, ++it) {
                     const int s = it % OZ_NSTG;
                     if (it >= OZ_NSTG) oz_mbar_wait(bar_empty + 8 * s, (uint32_t)((it / OZ_NSTG - 1) & 1));
                     const uint32_t st = base + s * OZ_STAGE;
-                    mbar_arrive_expect_tx(bar_full + 8 * s, OZ_STAGE);
+                    mbar_arrive_expect_tx(bar_full + 8 * s, OZ_STAGE);               // every byte of the stage lands here
 #pragma unroll
                     for (int q = 0; q < OZ_S; ++q) {
-                        tma_load_2d(st + q * OZ_A_SLICE, &mapP, kb * OZ_KB, q * g.NP + ib * OZ_TM, bar_full + 8 * s);
+                        const uint32_t pdst = st + q * OZ_A_SLICE + rank * prow * OZ_KB;
+                        const int prow0 = q * g.NP + ib * OZ_TM + (int)rank * prow;
+                        if (cs == 1) tma_load_2d(pdst, &mapP, kb * OZ_KB, prow0, bar_full + 8 * s);
+                        else tma_load_2d_multicast(pdst, &mapP, kb * OZ_KB, prow0, bar_full + 8 * s, mask);
                         tma_load_2d(st + OZ_S * OZ_A_SLICE + q * OZ_B_SLICE, &mapK, kb * OZ_KB, q * g.rows + cb * OZ_TN,
                                     bar_full + 8 * s);
                     }
                 }
             }
         }
+        if (cs > 1) oz_cluster_sync();              // pairs with the consumers' cluster barrier at the end
         return;
     }
     // consumers: warpgroup c = wg - 1 owns tile rows 64 c .. 64 c + 63; accumulator element e of a thread sits at row
@@ -212,9 +266,10 @@ gpk_oz_vargemm_kernel(const __grid_constant__ CUtensorMap mapP, const __grid_con
     const int c = wg - 1, cw = (tid - 128) >> 5;                     // cw: consumer warp 0..7
     const int r0 = c * 64 + (cw & 3) * 16 + (lane >> 2);
     int it = 0, tl = 0;
-    for (int t = blockIdx.x; t < total; t += gridDim.x, ++tl) {
-        int ib, cb;
-        oz_tile_of(t, g.nb, g.ncb, g.group, ib, cb);
+    for (int t = cid; t < total; t += ncl, ++tl) {
+        int ib, cbc;
+        oz_tile_of(t, g.nb, ncbc, gc, ib, cbc);
+        const int cb = cbc * (int)cs + (int)rank;
         const int nkb = (ib + 1) * OZ_TM / OZ_KB;                    // even: the k-loop takes two stages per pass
         uint32_t acc[OZ_S][16];
 #pragma unroll
@@ -245,15 +300,15 @@ gpk_oz_vargemm_kernel(const __grid_constant__ CUtensorMap mapP, const __grid_con
                             oz_wgmma_rs(acc[a + tk], f[k], oz_desc(st + OZ_S * OZ_A_SLICE + tk * OZ_B_SLICE + k * OZ_UK));
                     wgmma_commit();
                     wgmma_wait_one();
-                    if (a == 0 && (h == 1 || kb > 0) && (tid & 127) == 0)
-                        mbar_arrive(bar_empty + 8 * ((it + OZ_NSTG - 1) % OZ_NSTG));   // previous stage fully read
+                    if (a == 0 && (h == 1 || kb > 0) && (uint32_t)(tid & 127) < cs)       // previous stage fully read
+                        oz_release_stage(bar_empty + 8 * ((it + OZ_NSTG - 1) % OZ_NSTG), cs, (uint32_t)(tid & 127));
                 }
             }
         }
         wgmma_wait_all();
 #pragma unroll
         for (int l = 0; l < OZ_S; ++l) oz_wgmma_fence(acc[l]);
-        if ((tid & 127) == 0) mbar_arrive(bar_empty + 8 * ((it + OZ_NSTG - 1) % OZ_NSTG));
+        if ((uint32_t)(tid & 127) < cs) oz_release_stage(bar_empty + 8 * ((it + OZ_NSTG - 1) % OZ_NSTG), cs, (uint32_t)(tid & 127));
         const double rs0 = ldexp(1.0, g.eP[ib * OZ_TM + r0] + g.eK), rs1 = ldexp(1.0, g.eP[ib * OZ_TM + r0 + 8] + g.eK);
         // per thread 8 columns x 2 rows; column sums over the warp's 16 rows (lanes with equal lane % 4), then over warps
         double col[8];
@@ -285,6 +340,8 @@ gpk_oz_vargemm_kernel(const __grid_constant__ CUtensorMap mapP, const __grid_con
             g.part_ssq[(long)ib * g.ldpart + cb * OZ_TN + et] = s2;
         }
     }
+    // no CTA leaves while a peer may still arrive on its empty barriers
+    if (cs > 1) oz_cluster_sync();
 }
 
 // ---------------------------------------------------------------------------------------
