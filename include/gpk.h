@@ -78,6 +78,9 @@ const char* gpk_version(void);
  *   "ozcluster" 1, 2 or 4 [default 4] = CTAs per cluster of the int8 contraction: they take adjacent candidate blocks of
  *               one row block and share its L^-1 digit slices by TMA multicast, so each CTA reads 1 / CS of them from L2.
  *               Every value gives bit-identical results
+ *   "ozgrid"    >= 0: most clusters the persistent walk of the int8 contraction launches; 0 = as many as fit at once
+ *               [default].  Tests and diagnostics: with "ozpersist" = 1 and "ozgrid" = 1 one cluster walks every tile in
+ *               the L2-grouped, longest-first order.  Results are bit-identical for every value
  *   "ozpdl"     1 = the look-ahead K* builder runs as a small resident grid ("covctas" CTAs per SM) that triggers a
  *               programmatic dependent launch of the contraction behind it on the same stream (the two really co-run);
  *               0 = builder on the side stream (the block scheduler places it in the contraction's tail) [default: the
@@ -295,6 +298,16 @@ int gpk_measure_int8_peak_sustained(gpk_handle* h, double seconds, int random_op
 int gpk_get_factor(gpk_handle* h, double* L /* n x n row-major, lower */);
 int gpk_get_linv(gpk_handle* h, double* Linv /* n x n row-major, lower */);
 int gpk_get_z(gpk_handle* h, double* z /* n */);
+/* The int8 variance contraction alone, on caller-supplied operands (tests: tests/ozaki_model.py restates it exactly).
+ * P: n x n row-major, lower triangular (the stand-in for L^-1; only its block-lower triangle is read by the contraction,
+ * its row maxima by the row exponents).  Ks: m x n row-major, every |entry| <= amp.  Both are zero-padded to NP =
+ * round_up(n, 128) columns and to NP / round_up(m, 128) rows, split into 7 balanced base-256 digits (row exponents eP of
+ * P, one exponent eK = oz_exponent(amp) for Ks) and contracted with the handle's "ozcluster", "ozpersist" and "ozgrid",
+ * whatever "ozaki" says.  Out: part_ssq (nb x m row-major, nb = NP / 128) = sum over the rows of row block ib of V^2,
+ * V = P Ks^T; eP (n) and eK.  Uses its own scratch: a fitted model is left untouched.  GPK_BAD_ARG when an entry of Ks
+ * exceeds amp or NP > 16384.  Updates out[14] of gpk_get_timings. */
+int gpk_oz_contract(gpk_handle* h, const double* P, int n, const double* Ks, long m, double amp,
+                    double* part_ssq /* nb x m */, int* eP /* n */, int* eK);
 /* last fit/score timings measured with CUDA events on the handle's stream, milliseconds:
  * out[0] fit total, [1] K build, [2] Cholesky, [3] L^-1, [4] last score call total,
  * [5] K* build and [7] epilogue of the last candidate chunk, [6] variance GEMM averaged over the

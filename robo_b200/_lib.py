@@ -68,6 +68,7 @@ _SIGNATURES = {
     "gpk_get_factor": [_vp, _dp],
     "gpk_get_linv": [_vp, _dp],
     "gpk_get_z": [_vp, _dp],
+    "gpk_oz_contract": [_vp, _dp, C.c_int, _dp, C.c_long, C.c_double, _dp, _ip, _ip],
     "gpk_get_timings": [_vp, _dp],
     "gpk_get_diag_profile": [_vp, C.POINTER(C.c_longlong)],
 }
@@ -147,7 +148,7 @@ class Handle(object):
         # GPK_CHAINSPLIT=0|1, GPK_OZAKI=0|1
         for env, key in (("GPK_COV", "cov"), ("GPK_PERSIST", "persist"), ("GPK_CHAINSPLIT", "chainsplit"),
                          ("GPK_OZAKI", "ozaki"), ("GPK_GRAPH", "graph"), ("GPK_DEPTH2", "depth2"), ("GPK_OZFUSED", "ozfused"), ("GPK_OZPERSIST", "ozpersist"), ("GPK_OZPDL", "ozpdl"), ("GPK_COVCTAS", "covctas"),
-                         ("GPK_OZCLUSTER", "ozcluster")):
+                         ("GPK_OZCLUSTER", "ozcluster"), ("GPK_OZGRID", "ozgrid")):
             if os.environ.get(env):
                 self.set_option(key, int(os.environ[env]))
 
@@ -417,6 +418,21 @@ class Handle(object):
         z = np.empty(n)
         self._check(self.lib.gpk_get_z(self._h, _as_dp(z)))
         return z
+
+    def oz_contract(self, P, Ks, amp):
+        """The int8 variance contraction alone (gpk_oz_contract) on P (n x n, lower triangular) and Ks (m x n,
+        |entries| <= amp) -> dict(part_ssq (nb x m), eP (n,) int32, eK)."""
+        P, Ks = f64(P), f64(Ks)
+        n = P.shape[0]
+        if P.ndim != 2 or P.shape[1] != n or Ks.ndim != 2 or Ks.shape[1] != n:
+            raise ValueError("oz_contract: P must be n x n and Ks m x n")
+        m = Ks.shape[0]
+        part = np.empty(((n + 127) // 128, m))
+        eP = np.empty(n, dtype=np.int32)
+        eK = C.c_int()
+        self._check(self.lib.gpk_oz_contract(self._h, _as_dp(P), n, _as_dp(Ks), m, float(amp), _as_dp(part),
+                                             eP.ctypes.data_as(_ip), C.byref(eK)))
+        return dict(part_ssq=part, eP=eP, eK=eK.value)
 
     def diag_profile(self):
         t = np.zeros(64, dtype=np.int64)

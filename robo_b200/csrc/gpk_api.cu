@@ -62,7 +62,9 @@ struct gpk_handle {
     int oz_persist = 3;             // 1: one CTA per SM walks the tile list; 0: one CTA per tile; 3 = automatic [default]: persistent
                                     // for N <= 4096 (tools/persist_threshold.py and bench.py on an H100 with 4-CTA clusters: the
                                     // walk is as fast or faster up to N = 4096, one CTA per tile is faster at 6144)
-    int oz_fused = 1;               // 1: K* leaves the covariance builder as int8 digits (gpk_cov_oz_kernel); 0: fp64 K* + split + dot
+    int oz_grid = 0;                // most clusters the persistent walk launches (0: as many as fit at once [default])
+    DevBuf oz_probe;                // scratch of gpk_oz_contract (operands, slices, exponents, partial sums)
+    int oz_fused = 1;              // 1: K* leaves the covariance builder as int8 digits (gpk_cov_oz_kernel); 0: fp64 K* + split + dot
     long oz_linv_serial = -1;       // linv_serial the slices of L^-1 were made for
     long linv_serial = 0;           // bumped whenever L^-1 is (re)built
     int oz_emax_host = 0;
@@ -383,6 +385,34 @@ int oz_max_clusters(gpk_handle* h, int cs, int* out) {
         }
     }
     *out = h->oz_max_clusters[cs];
+    return GPK_OK;
+}
+
+// One launch of the int8 contraction over nb row blocks of L^-1 and the ncb = rows_padded / 32 candidate blocks whose
+// slices mapK covers (stacked [7][rows][NP]), with the handle's "ozcluster", "ozpersist" and "ozgrid": L2 group,
+// persistent grid and the variant code timings() reports.  Shared by score_dev and gpk_oz_contract.
+int launch_oz_contraction(gpk_handle* h, const CUtensorMap& mapP, const CUtensorMap& mapK, int nb, long rows_padded,
+                          long NP, long rows, const int* eP, int eK, double* part_ssq, long ldpart, bool dependent) {
+    OzArgs o;
+    o.nb = nb; o.ncb = (int)(rows_padded / OZ_TN); o.NP = (int)NP; o.rows = (int)rows;
+    // a group's K* slices take about 24 MB, half of the L2; whole clusters of candidate blocks (ncb = rows_padded / 32 is
+    // a multiple of 4, so of every cluster size)
+    const int cs = h->oz_cluster;
+    o.group = (int)std::min<long>(512, std::max<long>(4, ((long)24 << 20) / ((long)OZ_TN * NP * OZ_S))) / cs * cs;
+    o.eP = eP; o.eK = eK;
+    o.part_ssq = part_ssq; o.ldpart = ldpart;
+    const int persist = h->oz_persist == 3 ? (nb <= 32 ? 1 : 0) : h->oz_persist;
+    const int tiles = o.nb * o.ncb;
+    int grid = tiles;
+    if (persist == 1) {
+        int nclusters = 0, rc;
+        if ((rc = oz_max_clusters(h, cs, &nclusters))) return rc;
+        if (h->oz_grid > 0) nclusters = std::min(nclusters, h->oz_grid);
+        grid = cs * std::min(tiles / cs, nclusters);
+    }
+    h->oz_last_variant = 1 + (persist == 1 ? 8 : 0) + (cs == 2 ? 16 : cs == 4 ? 32 : 0);
+    CK(launch_oz(gpk_oz_vargemm_kernel, (unsigned)grid, cs, (size_t)OZ_SMEM, h->stream, dependent, mapP, mapK, o));
+    CKL();
     return GPK_OK;
 }
 
@@ -993,27 +1023,10 @@ int score_dev(gpk_handle* h, const double* dX, long m, int kind, double eta, dou
             if (last) CK(cudaEventRecord(h->ev[10], h->stream));
             CK(cudaEventRecord(h->ev_g0[ci], h->stream));
         }
-        const int oz_persist = h->oz_persist == 3 ? (h->nb <= 32 ? 1 : 0) : h->oz_persist;
         if (use_oz) {
-            OzArgs o;
-            o.nb = h->nb; o.ncb = (int)(mcp / OZ_TN); o.NP = (int)NP; o.rows = (int)cap;
-            // a group's K* slices take about 24 MB, half of the L2; whole clusters of candidate blocks (ncb = mcp / 32 is a
-            // multiple of 4, so of every cluster size)
-            const int cs = h->oz_cluster;
-            o.group = (int)std::min<long>(512, std::max<long>(4, ((long)24 << 20) / ((long)OZ_TN * NP * OZ_S))) / cs * cs;
-            o.eP = ptr<int>(h->oz_eP); o.eK = oz_eK;
-            o.part_ssq = a.part_ssq; o.ldpart = a.ldpart;
-            const int tiles = o.nb * o.ncb;
-            int grid = tiles;
-            if (oz_persist == 1) {
-                int nclusters = 0;
-                if ((rc = oz_max_clusters(h, cs, &nclusters))) return rc;
-                grid = cs * std::min(tiles / cs, nclusters);
-            }
-            h->oz_last_variant = 1 + (oz_persist == 1 ? 8 : 0) + (cs == 2 ? 16 : cs == 4 ? 32 : 0);
-            CK(launch_oz(gpk_oz_vargemm_kernel, (unsigned)grid, cs, (size_t)OZ_SMEM, h->stream, dependent, h->mapOzP,
-                         second ? h->mapOzK2 : h->mapOzK, o));
-            CKL();
+            if ((rc = launch_oz_contraction(h, h->mapOzP, second ? h->mapOzK2 : h->mapOzK, h->nb, mcp, NP, cap,
+                                            ptr<int>(h->oz_eP), oz_eK, a.part_ssq, a.ldpart, dependent)))
+                return rc;
             h->oz_launches += 1;
         } else if (h->persist && h->loader == LOADER_TMA_WS) {
             // one CTA per SM, tiles handed out by a counter (zeroed in stream order before every launch)
@@ -1121,7 +1134,7 @@ int gpk_destroy(gpk_handle* h) {
     DevBuf* bufs[] = {&h->Xrow, &h->Xt, &h->y, &h->Kbuf, &h->P, &h->Q, &h->W, &h->lower, &h->upper, &h->logdet_part,
                       &h->scal, &h->status, &h->jobs, &h->cand, &h->Kstar, &h->Kstar2, &h->cand2, &h->part_mu, &h->part_ssq, &h->out_mu,
                       &h->out_var, &h->out_acq, &h->block_best, &h->best, &h->nneg, &h->Vt, &h->cov, &h->XsT,
-                      &h->tmpjobs, &h->alpha, &h->tmp1, &h->tmp2, &h->tmp3, &h->chain_cnt, &h->dprof, &h->Xts, &h->tile_cnt, &h->oz_Pq, &h->oz_Kq, &h->oz_Kq2, &h->oz_eP, &h->oz_emax, &h->oz_mu, &h->oz_mu2, &h->oz_pmu2,
+                      &h->tmpjobs, &h->alpha, &h->tmp1, &h->tmp2, &h->tmp3, &h->chain_cnt, &h->dprof, &h->Xts, &h->tile_cnt, &h->oz_Pq, &h->oz_Kq, &h->oz_Kq2, &h->oz_eP, &h->oz_emax, &h->oz_mu, &h->oz_mu2, &h->oz_pmu2, &h->oz_probe,
                       &h->multi_cand, &h->multi_A, &h->multi_B, &h->multi_out, &h->multi_bb, &h->gather, &h->best_global};
     for (DevBuf* b : bufs)
         if (b->p) cudaFree(b->p);
@@ -1173,6 +1186,11 @@ int gpk_set_option(gpk_handle* h, const char* key, long value) {
     if (!strcmp(key, "ozcluster")) {
         if (value != 1 && value != 2 && value != 4) BAD("ozcluster must be 1, 2 or 4");
         h->oz_cluster = (int)value;
+        return GPK_OK;
+    }
+    if (!strcmp(key, "ozgrid")) {
+        if (value < 0 || value > (1L << 20)) BAD("ozgrid must be >= 0 (0: as many clusters as fit)");
+        h->oz_grid = (int)value;
         return GPK_OK;
     }
     if (!strcmp(key, "ozpdl")) {
@@ -2512,6 +2530,54 @@ int gpk_get_z(gpk_handle* h, double* z) {
     CK(cudaSetDevice(h->device));
     CK(cudaMemcpyAsync(z, ptr<double>(h->Kbuf) + (long)h->NP * h->NP, (size_t)h->n * 8, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
+    return GPK_OK;
+}
+
+int gpk_oz_contract(gpk_handle* h, const double* P, int n, const double* Ks, long m, double amp, double* part_ssq,
+                    int* eP, int* eK) {
+    if (!h) return GPK_BAD_ARG;
+    if (!P || !Ks || !part_ssq || !eP || !eK || n <= 0 || m <= 0 || !(amp > 0.0) || !std::isfinite(amp))
+        BAD("gpk_oz_contract: bad arguments");
+    const long NP = round_up(n, OZ_TM), MP = round_up(m, OZ_TM), nb = NP / OZ_TM;
+    if (NP > 16384) BAD("gpk_oz_contract: n = %d pads to %ld > 16384 (the int32 level sums hold K <= 16384)", n, NP);
+    for (long i = 0; i < m * (long)n; ++i)
+        if (!(std::fabs(Ks[i]) <= amp)) BAD("gpk_oz_contract: |Ks| exceeds amp at entry %ld", i);
+    CK(cudaSetDevice(h->device));
+    // scratch, every piece a multiple of 512 bytes: P, Ks (zero-padded to NP x NP and MP x NP), their slices, the
+    // partial sums, the row exponents and the exponent maximum the row-exponent kernel also writes
+    const size_t oK = (size_t)NP * NP * 8, oPq = oK + (size_t)MP * NP * 8, oKq = oPq + (size_t)OZ_S * NP * NP;
+    const size_t opart = oKq + (size_t)OZ_S * MP * NP, oe = opart + (size_t)nb * MP * 8, oemax = oe + (size_t)NP * 4;
+    int rc;
+    if ((rc = ensure(h, h->oz_probe, oemax + 4))) return rc;
+    char* b = (char*)h->oz_probe.p;
+    double* dP = (double*)b;
+    double* dK = (double*)(b + oK);
+    int8_t* dPq = (int8_t*)(b + oPq);
+    int8_t* dKq = (int8_t*)(b + oKq);
+    double* dpart = (double*)(b + opart);
+    int* de = (int*)(b + oe);
+    cudaStream_t st = h->stream;
+    CK(cudaMemsetAsync(dP, 0, (size_t)NP * NP * 8, st));
+    CK(cudaMemcpy2DAsync(dP, (size_t)NP * 8, P, (size_t)n * 8, (size_t)n * 8, (size_t)n, cudaMemcpyHostToDevice, st));
+    CK(cudaMemsetAsync(dK, 0, (size_t)MP * NP * 8, st));
+    CK(cudaMemcpy2DAsync(dK, (size_t)NP * 8, Ks, (size_t)n * 8, (size_t)n * 8, (size_t)m, cudaMemcpyHostToDevice, st));
+    CK(cudaMemsetAsync(b + oemax, 0, 4, st));
+    CK(cudaMemsetAsync(dpart, 0xFF, (size_t)nb * MP * 8, st));      // NaN: a tile that is never written shows
+    gpk_oz_rowexp_kernel<<<(unsigned)NP, 256, 0, st>>>(dP, NP, (int)NP, de, (int*)(b + oemax));
+    CKL();
+    gpk_oz_split_kernel<<<(unsigned)((NP * NP + 255) / 256), 256, 0, st>>>(dP, NP, NP, de, 0, dPq, NP * NP);
+    CKL();
+    const int ek = oz_exponent(amp);
+    gpk_oz_split_kernel<<<(unsigned)((MP * NP + 255) / 256), 256, 0, st>>>(dK, MP, NP, nullptr, ek, dKq, MP * NP);
+    CKL();
+    CUtensorMap mapP, mapK;
+    if ((rc = make_oz_map(h, &mapP, dPq, (long)OZ_S * NP, NP, OZ_TM / h->oz_cluster))) return rc;
+    if ((rc = make_oz_map(h, &mapK, dKq, (long)OZ_S * MP, NP, OZ_TN))) return rc;
+    if ((rc = launch_oz_contraction(h, mapP, mapK, (int)nb, MP, NP, MP, de, ek, dpart, MP, false))) return rc;
+    CK(cudaMemcpy2DAsync(part_ssq, (size_t)m * 8, dpart, (size_t)MP * 8, (size_t)m * 8, (size_t)nb, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(eP, de, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    *eK = ek;
     return GPK_OK;
 }
 

@@ -310,7 +310,12 @@ gpk_oz_vargemm_kernel(const __grid_constant__ CUtensorMap mapP, const __grid_con
         for (int l = 0; l < OZ_S; ++l) oz_wgmma_fence(acc[l]);
         if ((uint32_t)(tid & 127) < cs) oz_release_stage(bar_empty + 8 * ((it + OZ_NSTG - 1) % OZ_NSTG), cs, (uint32_t)(tid & 127));
         const double rs0 = ldexp(1.0, g.eP[ib * OZ_TM + r0] + g.eK), rs1 = ldexp(1.0, g.eP[ib * OZ_TM + r0 + 8] + g.eK);
-        // per thread 8 columns x 2 rows; column sums over the warp's 16 rows (lanes with equal lane % 4), then over warps
+        // per thread 8 columns x 2 rows; column sums over the warp's 16 rows (lanes with equal lane % 4), then over warps.
+        // The rounding sequence is a contract that tests/ozaki_model.py restates bit for bit (change both together):
+        //   v = 0, v = fma(acc[lvl], 2^(-8 (lvl + 2)), v) for lvl = 6 .. 0;  x = v 2^(eP[row] + eK);
+        //   warp w (rows 16 w .. 16 w + 15), row pair g: c_g = fma(x(16 w + g + 8), x(16 w + g + 8), x(16 w + g)^2)
+        //   (nvcc contracts col += x * x);  butterfly ((c0 + c1) + (c2 + c3)) + ((c4 + c5) + (c6 + c7));
+        //   tile column sum = (((0 + w0) + w1) + ...) + w7;  gpk_finish_kernel then adds part_ssq over ib = 0 .. nb - 1.
         double col[8];
 #pragma unroll
         for (int j = 0; j < 8; ++j) col[j] = 0.0;
