@@ -238,6 +238,32 @@ int gpk_acq_multi(gpk_handle* const* models, int n_models, const double* Xs, lon
                   const double* eta, double par, double* out1, double* out2, long* n_negative, double* best_val,
                   long* best_idx);
 
+/* DifferentialEvolution.maximize (robo/maximizers/differential_evolution.py:27-51) on the device: scipy's
+ * differential_evolution with strategy 'best1bin' and Latin-hypercube initialisation
+ * (scipy/optimize/_differentialevolution.py) minimising the energy -acq(x), x = clip(scaled member, lower, upper),
+ * acq = mean over the n_models handles (the value gpk_acq_multi mode 0 returns; one handle: gpk_acq's value), an
+ * infinite energy replaced by DBL_MAX as the reference's wrapper does.  Population, trials, energies, selection and the
+ * convergence test std(E) <= atol + tol |mean(E)| stay on the device; each generation is one scoring pass of pop rows
+ * over all models, and only a 16-byte status record crosses PCIe per generation.
+ * Two deviations from the reference:
+ *   - updating='deferred' (a whole generation is scored at once) instead of scipy's default 'immediate', which is
+ *     serial by construction;
+ *   - the random stream is Philox4x32-10 keyed by `seed`, counter (member, generation, word, tag) with a tag disjoint
+ *     from gpk_maximize_random's counters (gpk_de.cuh).  The reference never passes an rng to scipy, so its stream
+ *     cannot be reproduced anyway.  Results depend on nothing but the arguments: not on chunking or n_models' order of
+ *     completion.
+ * The order of every rounding step, the sums of mean and std included, is documented in gpk_de.cuh.
+ * pop: 5 <= pop <= 2^24 (scipy: max(5, popsize * d)).  maxiter >= 0 generations (0: score the initial population
+ * only); 0 <= mut_lo <= mut_hi < 2 (dither F ~ U[mut_lo, mut_hi) per generation); 0 <= recombination <= 1;
+ * lower < upper (d each); acq_kind EI ... LCB; eta[n_models]; the handles as for gpk_acq_multi.  Out: best_x (d) =
+ * the scaled winner, best_energy = its energy, nit = generations run, nfev = pop * (nit + 1), n_negative = EI values
+ * < 0 over all evaluations; population (pop x d unit cube, row-major, slot 0 = winner) and energies (pop) may be NULL. */
+int gpk_maximize_de(gpk_handle* const* models, int n_models, unsigned long long seed, long pop, int maxiter,
+                    double mut_lo, double mut_hi, double recombination, double tol, double atol,
+                    const double* lower, const double* upper, int acq_kind, const double* eta, double par,
+                    double* best_x, double* best_energy, int* nit, long* nfev, long* n_negative,
+                    double* population, double* energies);
+
 /* kernel.get_value(X1, X2) (test/test_models/test_gaussian_process.py:44-46) with the
  * handle's current kernel; no input scaling.  out is (n1, n2) row-major. */
 int gpk_kernel_matrix(gpk_handle* h, const double* X1, long n1, const double* X2, long n2,

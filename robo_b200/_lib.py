@@ -51,6 +51,8 @@ _SIGNATURES = {
     "gpk_kernel_matrix": [_vp, _dp, C.c_long, _dp, C.c_long, C.c_int, _dp],
     "gpk_reduce_models": [_vp, _dp, _dp, C.c_int, C.c_long, C.c_int, _dp, _dp],
     "gpk_acq_multi": [C.POINTER(_vp), C.c_int, _dp, C.c_long, C.c_int, C.c_int, _dp, C.c_double, _dp, _dp, _lp, _dp, _lp],
+    "gpk_maximize_de": [C.POINTER(_vp), C.c_int, C.c_ulonglong, C.c_long, C.c_int, C.c_double, C.c_double, C.c_double,
+                        C.c_double, C.c_double, _dp, _dp, C.c_int, _dp, C.c_double, _dp, _dp, _ip, _lp, _lp, _dp, _dp],
     "gpk_comm_unique_id": [_vp],
     "gpk_comm_init": [_vp, C.c_int, C.c_int, _vp],
     "gpk_comm_destroy": [_vp],
@@ -483,6 +485,30 @@ def acq_multi(handles, Xs, mode, kind=ACQ_NONE, eta=None, par=0.0, want_argmax=F
     if mode == 1:
         return dict(mean=out1, var=out2)
     return dict(values=out1, n_negative=nn.value, best_val=bv.value, best_idx=bi.value)
+
+
+def maximize_de(handles, seed, pop, maxiter, mutation, recombination, tol, atol, lower, upper, kind, eta, par=0.0,
+                want_population=False):
+    """gpk_maximize_de over ``handles`` (all fitted, same device): differential evolution minimising -acq, acq the
+    mean over the handles.  -> dict(x (D,), energy, nit, nfev, n_negative[, population (pop, D), energies (pop,)])."""
+    h0 = handles[0]
+    lo, up = f64(lower).ravel(), f64(upper).ravel()
+    arr = (_vp * len(handles))(*[h._h for h in handles])
+    etas = f64(np.broadcast_to(np.asarray(eta, dtype=np.float64), (len(handles),)))
+    x = np.empty(lo.size)
+    pop = int(pop)
+    P = np.empty((pop, lo.size)) if want_population and pop > 0 else None
+    E = np.empty(pop) if want_population and pop > 0 else None
+    be, nit, nfev, nn = C.c_double(), C.c_int(), C.c_long(), C.c_long()
+    h0._check(h0.lib.gpk_maximize_de(arr, len(handles), int(seed) & 0xFFFFFFFFFFFFFFFF, pop, int(maxiter),
+                                     float(mutation[0]), float(mutation[1]), float(recombination), float(tol),
+                                     float(atol), _as_dp(lo), _as_dp(up), int(kind), _as_dp(etas), float(par),
+                                     _as_dp(x), C.byref(be), C.byref(nit), C.byref(nfev), C.byref(nn),
+                                     _as_dp(P) if P is not None else None, _as_dp(E) if E is not None else None))
+    r = dict(x=x, energy=be.value, nit=nit.value, nfev=nfev.value, n_negative=nn.value)
+    if want_population:
+        r.update(population=P, energies=E)
+    return r
 
 
 _moments_handle = {}

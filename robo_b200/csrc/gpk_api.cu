@@ -25,6 +25,7 @@
 #include "gpk_diag16.cuh"
 #include "gpk_chain.cuh"
 #include "gpk_ozaki.cuh"
+#include "gpk_de.cuh"
 
 namespace {
 
@@ -148,6 +149,9 @@ struct gpk_handle {
     // several models, one batch (gpk_acq_multi): buffers owned by the first handle of the call
     DevBuf multi_cand, multi_A, multi_B, multi_out, multi_bb;
     cudaEvent_t ev_multi = nullptr;
+    // differential evolution (gpk_maximize_de): population, trials, scaled batch, energies, {status, limits, winner},
+    // radix-sort scratch of the LHS initialisation; owned by the first handle of the call
+    DevBuf de_pop, de_trial, de_param, de_E, de_small, de_sort;
     // multi-GPU (gpk_comm_*): NCCL communicator bound at run time, one 16-byte pair per rank
     void* comm = nullptr;
     int rank = 0, world = 1;
@@ -1135,7 +1139,8 @@ int gpk_destroy(gpk_handle* h) {
                       &h->scal, &h->status, &h->jobs, &h->cand, &h->Kstar, &h->Kstar2, &h->cand2, &h->part_mu, &h->part_ssq, &h->out_mu,
                       &h->out_var, &h->out_acq, &h->block_best, &h->best, &h->nneg, &h->Vt, &h->cov, &h->XsT,
                       &h->tmpjobs, &h->alpha, &h->tmp1, &h->tmp2, &h->tmp3, &h->chain_cnt, &h->dprof, &h->Xts, &h->tile_cnt, &h->oz_Pq, &h->oz_Kq, &h->oz_Kq2, &h->oz_eP, &h->oz_emax, &h->oz_mu, &h->oz_mu2, &h->oz_pmu2, &h->oz_probe,
-                      &h->multi_cand, &h->multi_A, &h->multi_B, &h->multi_out, &h->multi_bb, &h->gather, &h->best_global};
+                      &h->multi_cand, &h->multi_A, &h->multi_B, &h->multi_out, &h->multi_bb, &h->gather, &h->best_global,
+                      &h->de_pop, &h->de_trial, &h->de_param, &h->de_E, &h->de_small, &h->de_sort};
     for (DevBuf* b : bufs)
         if (b->p) cudaFree(b->p);
     if (h->ev_ok)

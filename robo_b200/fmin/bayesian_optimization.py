@@ -8,7 +8,7 @@ import numpy as np
 from robo_b200 import kernels
 from robo_b200.acquisition_functions import EI, LCB, PI, LogEI, MarginalizationGPMCMC
 from robo_b200.initial_design import init_latin_hypercube_sampling
-from robo_b200.maximizers import RandomSampling
+from robo_b200.maximizers import DifferentialEvolution, RandomSampling
 from robo_b200.models import GaussianProcess, GaussianProcessMCMC
 from robo_b200.priors import DefaultPrior
 from robo_b200.solver import BayesianOptimization
@@ -50,8 +50,10 @@ def bayesian_optimization(objective_function, lower, upper, num_iterations=30, X
 
     if maximizer == "random":
         max_func = RandomSampling(acq, lower, upper, n_samples=n_candidates, rng=rng)
+    elif maximizer == "differential_evolution":
+        max_func = DifferentialEvolution(acq, lower, upper, rng=rng)
     else:
-        raise ValueError("'{}' is not accelerated on the GPU path; use 'random' or pass the robo_b200 "
+        raise ValueError("'{}' is not accelerated on the GPU path; use 'random', 'differential_evolution' or pass the robo_b200 "
                          "objects to the reference's own maximizers".format(maximizer))
 
     bo = BayesianOptimization(objective_function, lower, upper, acq, model, max_func, initial_points=n_init,

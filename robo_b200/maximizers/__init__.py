@@ -1,2 +1,3 @@
 from .random_sampling import RandomSampling  # noqa: F401
 from .device_random_sampling import DeviceRandomSampling  # noqa: F401
+from .differential_evolution import DifferentialEvolution  # noqa: F401
