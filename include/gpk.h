@@ -34,7 +34,9 @@ typedef enum {
     GPK_BAD_ARG = 2,
     GPK_CUDA_ERROR = 3,
     GPK_NOT_FITTED = 4,
-    GPK_NOT_APPLICABLE = 5 /* gpk_fit_append: preconditions not met, nothing was changed; do a full fit */
+    GPK_NOT_APPLICABLE = 5, /* gpk_fit_append: preconditions not met, nothing was changed; do a full fit */
+    GPK_EP_FAILED = 6      /* gpk_ep_joint_min: an EP update produced a NaN variance (the reference raises Exception,
+                              robo/util/epmgp.py:204-207) */
 } gpk_status;
 
 /* stationary radial families, george names (oracle/george_oracle.py) */
@@ -263,6 +265,37 @@ int gpk_maximize_de(gpk_handle* const* models, int n_models, unsigned long long 
                     const double* lower, const double* upper, int acq_kind, const double* eta, double par,
                     double* best_x, double* best_energy, int* nit, long* nfev, long* n_negative,
                     double* population, double* energies);
+
+/* epmgp.joint_min(mu, V, with_derivatives=True) (robo/util/epmgp.py:11-250): the EPMGP approximation of p_min, the
+ * probability of each of nb points to be the minimum of a Gaussian N(mu, V), on caller operands.  One CTA per point k
+ * runs the EP problem of k (at most 50 sweeps, stop when sum |d| < 0.001, float32 epsilon in the message clamps), then
+ * joint_min's renormalisation runs on the device (gpk_es.cuh).  2 <= nb <= 64; mu (nb), V (nb x nb row-major).
+ * Out: logP (nb) = log p_min; dlogPdMu (nb x nb), dlogPdSigma (nb x nb (nb + 1) / 2: row k is the lower triangle of the
+ * symmetrised derivative in row-major order), dlogPdMudMu (nb x nb x nb), sweeps (nb: EP sweeps of problem k); each of
+ * these four may be NULL.  Uses its own scratch: a fitted model is left untouched, and no fit is needed.
+ * GPK_EP_FAILED when an EP update yields a NaN variance; GPK_NOT_PD when IRSR is not positive definite even with
+ * +1e-6 I (numpy.linalg.LinAlgError in the reference). */
+int gpk_ep_joint_min(gpk_handle* h, const double* mu, const double* V, int nb, double* logP, double* dlogPdMu,
+                     double* dlogPdSigma, double* dlogPdMudMu, int* sweeps);
+
+/* InformationGain.update after the representer points are sampled (robo/acquisition_functions/information_gain.py:
+ * 153-167): Mb, Vb = predict(zb, full_cov=True) on the handle (clipped like the reference), EP for p_min
+ * (gpk_ep_joint_min), and U = K^-1 K(X, zb) (N x Nb, fp64, from the handle's L^-1) for the cross-covariance of the
+ * candidates; everything stays on the device.  zb (nb x d raw inputs), lmb (nb, the log-probabilities of zb under the
+ * sampling acquisition: GPK_BAD_ARG "lmb should not be infinite." when one is not finite, :207-211), sn2 = the model's
+ * noise, W (np) the quantiles of the hallucinated observations, lower / upper (d) the acquisition's bounds.
+ * logP (nb), dlogPdMu, dlogPdSigma, dlogPdMudMu (shapes as gpk_ep_joint_min) may be NULL.  2 <= nb <= 64, np >= 1. */
+int gpk_es_update(gpk_handle* h, const double* zb, int nb, const double* lmb, double sn2, const double* W, int np,
+                  const double* lower, const double* upper, double* logP, double* dlogPdMu, double* dlogPdSigma,
+                  double* dlogPdMudMu);
+/* InformationGain.compute (information_gain.py:87-125, 169-203) over m candidates Xs (m x d raw inputs): the
+ * predictive variance v from the scoring pass, the covariance sigma to zb, the innovations and the entropy change dH
+ * per candidate (gpk_es.cuh).  A candidate outside [lower, upper] gives DBL_EPSILON, NaN or +inf gives -DBL_MAX, -inf is
+ * kept.  Each candidate is computed on its own, so the values do not depend on "chunk" or on how a batch is split.
+ * GPK_BAD_ARG before gpk_es_update or after the model changed since. */
+int gpk_es_compute(gpk_handle* h, const double* Xs, long m, double* out);
+/* the same on device pointers (d_Xs: m x d, d_out: m doubles), asynchronous on the handle's stream */
+int gpk_es_compute_dev(gpk_handle* h, const void* d_Xs, long m, void* d_out);
 
 /* kernel.get_value(X1, X2) (test/test_models/test_gaussian_process.py:44-46) with the
  * handle's current kernel; no input scaling.  out is (n1, n2) row-major. */

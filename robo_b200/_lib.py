@@ -6,6 +6,7 @@ callers already handle (SURVEY.md section 8b "Error conventions"):
     GPK_NOT_PD     -> numpy.linalg.LinAlgError   (gaussian_process.py:120,156)
     GPK_BAD_ARG    -> ValueError
     GPK_CUDA_ERROR -> RuntimeError
+    GPK_EP_FAILED  -> Exception with the reference's message (robo/util/epmgp.py:204-207)
 """
 import ctypes as C
 import os
@@ -14,7 +15,7 @@ import numpy as np
 
 from . import _build
 
-GPK_OK, GPK_NOT_PD, GPK_BAD_ARG, GPK_CUDA_ERROR, GPK_NOT_FITTED, GPK_NOT_APPLICABLE = range(6)
+GPK_OK, GPK_NOT_PD, GPK_BAD_ARG, GPK_CUDA_ERROR, GPK_NOT_FITTED, GPK_NOT_APPLICABLE, GPK_EP_FAILED = range(7)
 MATERN52, EXPSQUARED, MATERN32 = 0, 1, 2
 ACQ_NONE, ACQ_EI, ACQ_LOG_EI, ACQ_PI, ACQ_LCB = range(5)
 ACQ_KIND = {"ei": ACQ_EI, "log_ei": ACQ_LOG_EI, "pi": ACQ_PI, "lcb": ACQ_LCB, "none": ACQ_NONE}
@@ -71,6 +72,10 @@ _SIGNATURES = {
     "gpk_get_linv": [_vp, _dp],
     "gpk_get_z": [_vp, _dp],
     "gpk_oz_contract": [_vp, _dp, C.c_int, _dp, C.c_long, C.c_double, _dp, _ip, _ip],
+    "gpk_ep_joint_min": [_vp, _dp, _dp, C.c_int, _dp, _dp, _dp, _dp, _ip],
+    "gpk_es_update": [_vp, _dp, C.c_int, _dp, C.c_double, _dp, C.c_int, _dp, _dp, _dp, _dp, _dp, _dp],
+    "gpk_es_compute": [_vp, _dp, C.c_long, _dp],
+    "gpk_es_compute_dev": [_vp, _vp, C.c_long, _vp],
     "gpk_get_timings": [_vp, _dp],
     "gpk_get_diag_profile": [_vp, C.POINTER(C.c_longlong)],
 }
@@ -177,6 +182,8 @@ class Handle(object):
             raise ValueError(msg)
         if rc == GPK_NOT_FITTED:
             raise RuntimeError(msg or "model not fitted")
+        if rc == GPK_EP_FAILED:
+            raise Exception(msg)
         raise RuntimeError("gpk: " + msg)
 
     def set_option(self, key, value):
@@ -435,6 +442,50 @@ class Handle(object):
         self._check(self.lib.gpk_oz_contract(self._h, _as_dp(P), n, _as_dp(Ks), m, float(amp), _as_dp(part),
                                              eP.ctypes.data_as(_ip), C.byref(eK)))
         return dict(part_ssq=part, eP=eP, eK=eK.value)
+
+    def ep_joint_min(self, mu, V, derivatives=True):
+        """EPMGP p_min on caller operands (gpk_ep_joint_min) -> dict(logP (nb,)[, dlogPdMu (nb, nb), dlogPdSigma
+        (nb, nb (nb + 1) / 2), dlogPdMudMu (nb, nb, nb), sweeps (nb,) int32])."""
+        mu, V = f64(mu).ravel(), f64(V)
+        nb = mu.size
+        if V.shape != (nb, nb):
+            raise ValueError("ep_joint_min: V must be %d x %d" % (nb, nb))
+        logP = np.empty(nb)
+        if not derivatives or not 2 <= nb <= 64:          # nb is checked by the library before any buffer is used
+            self._check(self.lib.gpk_ep_joint_min(self._h, _as_dp(mu), _as_dp(V), nb, _as_dp(logP), None, None, None, None))
+            return dict(logP=logP)
+        dMu, dSig, dMuMu = np.empty((nb, nb)), np.empty((nb, nb * (nb + 1) // 2)), np.empty((nb, nb, nb))
+        sweeps = np.empty(nb, dtype=np.int32)
+        self._check(self.lib.gpk_ep_joint_min(self._h, _as_dp(mu), _as_dp(V), nb, _as_dp(logP), _as_dp(dMu), _as_dp(dSig),
+                                              _as_dp(dMuMu), sweeps.ctypes.data_as(_ip)))
+        return dict(logP=logP, dlogPdMu=dMu, dlogPdSigma=dSig, dlogPdMudMu=dMuMu, sweeps=sweeps)
+
+    def es_update(self, zb, lmb, sn2, W, lower, upper):
+        """gpk_es_update -> dict(logP (nb,), dlogPdMu, dlogPdSigma, dlogPdMudMu)."""
+        zb, lmb, W = f64(zb), f64(lmb).ravel(), f64(W).ravel()
+        lo, up = f64(lower).ravel(), f64(upper).ravel()
+        nb = zb.shape[0]
+        if lmb.size != nb:
+            raise ValueError("es_update: lmb needs one value per representer point")
+        if not 2 <= nb <= 64:
+            self._check(self.lib.gpk_es_update(self._h, _as_dp(zb), nb, _as_dp(lmb), float(sn2), _as_dp(W), W.size,
+                                               _as_dp(lo), _as_dp(up), None, None, None, None))
+        logP = np.empty(nb)
+        dMu, dSig, dMuMu = np.empty((nb, nb)), np.empty((nb, nb * (nb + 1) // 2)), np.empty((nb, nb, nb))
+        self._check(self.lib.gpk_es_update(self._h, _as_dp(zb), nb, _as_dp(lmb), float(sn2), _as_dp(W), W.size,
+                                           _as_dp(lo), _as_dp(up), _as_dp(logP), _as_dp(dMu), _as_dp(dSig),
+                                           _as_dp(dMuMu)))
+        return dict(logP=logP, dlogPdMu=dMu, dlogPdSigma=dSig, dlogPdMudMu=dMuMu)
+
+    def es_compute(self, Xs):
+        """gpk_es_compute: the entropy change of every row of Xs (m, d) -> (m,)."""
+        Xs = f64(Xs)
+        out = np.empty(Xs.shape[0])
+        self._check(self.lib.gpk_es_compute(self._h, _as_dp(Xs), Xs.shape[0], _as_dp(out)))
+        return out
+
+    def es_compute_dev(self, d_Xs_ptr, m, d_out_ptr):
+        self._check(self.lib.gpk_es_compute_dev(self._h, _vp(d_Xs_ptr), int(m), _vp(d_out_ptr)))
 
     def diag_profile(self):
         t = np.zeros(64, dtype=np.int64)

@@ -1,0 +1,126 @@
+"""InformationGain — the entropy-search acquisition of robo/acquisition_functions/information_gain.py:19-272 (Hennig
+and Schuler, JMLR 2012) with its numerical work on the GPU.
+
+update(): the representer points zb are drawn by the ensemble sampler from the sampling acquisition (each
+half-ensemble scored in ONE call of the fused acquisition); p_min over zb by EP, the derivatives of log p_min and
+U = K^-1 K(X, zb) are computed and kept on the device (gpk_es_update).  compute(): the entropy change of every
+candidate in one batched call (gpk_es_compute): the reference loops over candidates with one predict and one
+(Nb + 1)-point predict(full_cov=True) each.  innovations() stays a host method, as in the reference.
+
+Serves robo_b200 GaussianProcess models whose inputs go to the device untransformed; marginalised over a GP-MCMC
+ensemble by MarginalizationGPMCMC (one estimator, with its own representer points, per sub-model).
+"""
+import logging
+
+import numpy as np
+import scipy.stats
+
+from robo_b200.acquisition_functions.base_acquisition import BaseAcquisitionFunction
+from robo_b200.acquisition_functions.log_ei import LogEI
+from robo_b200.util.ensemble_sampler import EnsembleSampler
+
+logger = logging.getLogger(__name__)
+
+
+def _device_model(model):
+    from robo_b200.maximizers.differential_evolution import _raw_inputs
+    if not _raw_inputs(model) or not hasattr(getattr(model, "gp", None), "handle"):
+        raise TypeError("InformationGain runs on robo_b200 GaussianProcess models whose inputs go to the device "
+                        "untransformed")
+    model.gp._restore()
+    model.gp._push_cfg()
+    return model.gp.handle
+
+
+class InformationGain(BaseAcquisitionFunction):
+
+    def __init__(self, model, lower, upper, Nb=50, Np=400, sampling_acquisition=None,
+                 sampling_acquisition_kw={"par": 0.0}, rng=None, **kwargs):
+        self.Nb = Nb
+        super(InformationGain, self).__init__(model)
+        self.lower = lower
+        self.upper = upper
+        self.D = self.lower.shape[0]
+        self.sn2 = None
+        if sampling_acquisition is None:
+            sampling_acquisition = LogEI
+        self.sampling_acquisition = sampling_acquisition(model, **sampling_acquisition_kw)
+        self.Np = Np
+        if rng is None:
+            self.rng = np.random.RandomState(np.random.randint(0, 10000))
+        else:
+            self.rng = rng
+        self.zb = self.lmb = None
+
+    def sampling_acquisition_wrapper(self, x):
+        if np.any(x < self.lower) or np.any(x > self.upper):
+            return -np.inf
+        return self.sampling_acquisition(np.array([x]))[0]
+
+    def _sampling_batch(self, X):
+        """The wrapper's one-point semantics over a whole half-ensemble, scored in one call."""
+        out = np.full(X.shape[0], -np.inf)
+        inside = np.all((X >= self.lower) & (X <= self.upper), axis=1)
+        if np.any(inside):
+            out[inside] = np.asarray(self.sampling_acquisition(X[inside]), dtype=np.float64).ravel()
+        return out
+
+    def sample_representer_points(self):
+        self.sampling_acquisition.update(self.model)
+        for i in range(5):
+            restarts = self.lower + (self.upper - self.lower) * self.rng.uniform(size=(self.Nb, self.D))
+            sampler = EnsembleSampler(self.Nb, self.D, self.sampling_acquisition_wrapper,
+                                      batch_lnpostfn=self._sampling_batch)
+            self.zb, self.lmb, _ = sampler.run_mcmc(restarts, 50, rstate0=self.rng)
+            if not np.any(np.isinf(self.lmb)):
+                break
+            logger.info("infinite log-probability among the representer points, resampling")
+        if len(self.zb.shape) == 1:
+            self.zb = self.zb[:, None]
+        if len(self.lmb.shape) == 1:
+            self.lmb = self.lmb[:, None]
+
+    def update(self, model):
+        self.model = model
+        handle = _device_model(model)
+        self.sn2 = self.model.get_noise()
+        self.sample_representer_points()
+        self.W = scipy.stats.norm.ppf(np.linspace(1. / (self.Np + 1), 1 - 1. / (self.Np + 1), self.Np))[np.newaxis, :]
+        r = handle.es_update(self.zb, self.lmb, self.sn2, self.W, self.lower, self.upper)
+        self.logP = np.reshape(r["logP"], (self.Nb, 1))
+        self.dlogPdMu, self.dlogPdSigma, self.dlogPdMudMu = r["dlogPdMu"], r["dlogPdSigma"], r["dlogPdMudMu"]
+
+    def compute(self, X_test, derivative=False, **kwargs):
+        """Entropy change of every row of X_test -> (N,).  derivative=True is not implemented (the reference's finite
+        differences are marked "Not tested!")."""
+        if derivative:
+            raise NotImplementedError("InformationGain has no derivative on the GPU path")
+        if self.zb is None:
+            raise ValueError("InformationGain.compute needs update() first")
+        if not np.all(np.isfinite(self.lmb)):
+            raise ValueError("lmb should not be infinite.")
+        return _device_model(self.model).es_compute(np.asarray(X_test, dtype=np.float64))
+
+    def argmax(self, X_test):
+        return int(np.argmax(self.compute(X_test)))
+
+    def dh_fun(self, x, derivative=False):
+        if derivative:
+            raise NotImplementedError("InformationGain has no derivative on the GPU path")
+        if not np.all(np.isfinite(self.lmb)):
+            raise ValueError("lmb should not be infinite.")
+        if len(x.shape) == 1:
+            x = x[np.newaxis]
+        if np.any(x < self.lower) or np.any(x > self.upper):
+            return np.array([[np.spacing(1)]]), np.array([[np.zeros((x.shape[1], 1))]])
+        return self.compute(x[:1])
+
+    def innovations(self, x, rep):
+        _, v = self.model.predict(x)
+        v = v.reshape(-1, 1)
+        v_ = v - self.sn2
+        sigma_x_rep = self.model.predict_variance(rep, x)
+        norm_cov = np.dot(sigma_x_rep, np.linalg.inv(v_))
+        dm_rep = np.dot(norm_cov, np.linalg.cholesky(v + 1e-10))
+        dv_rep = -norm_cov.dot(sigma_x_rep.T)
+        return dm_rep, dv_rep

@@ -26,6 +26,7 @@
 #include "gpk_chain.cuh"
 #include "gpk_ozaki.cuh"
 #include "gpk_de.cuh"
+#include "gpk_es.cuh"
 
 namespace {
 
@@ -152,6 +153,12 @@ struct gpk_handle {
     // differential evolution (gpk_maximize_de): population, trials, scaled batch, energies, {status, limits, winner},
     // radix-sort scratch of the LHS initialisation; owned by the first handle of the call
     DevBuf de_pop, de_trial, de_param, de_E, de_small, de_sort;
+    DevBuf ep_buf;                  // scratch of gpk_ep_joint_min (operands, raw and renormalised outputs, status)
+    // entropy search (gpk_es_update / gpk_es_compute): EP state, W, bounds, scaled zb, U = K^-1 K(X, zb), per-chunk v, sigma
+    DevBuf es_state, es_U, es_work, es_in;
+    int es_nb = 0, es_np = 0;
+    double es_sn2 = 0.0, es_H = 0.0;
+    long es_linv_serial = -1;       // linv_serial U was built for (-1: no update yet)
     // multi-GPU (gpk_comm_*): NCCL communicator bound at run time, one 16-byte pair per rank
     void* comm = nullptr;
     int rank = 0, world = 1;
@@ -1140,7 +1147,7 @@ int gpk_destroy(gpk_handle* h) {
                       &h->out_var, &h->out_acq, &h->block_best, &h->best, &h->nneg, &h->Vt, &h->cov, &h->XsT,
                       &h->tmpjobs, &h->alpha, &h->tmp1, &h->tmp2, &h->tmp3, &h->chain_cnt, &h->dprof, &h->Xts, &h->tile_cnt, &h->oz_Pq, &h->oz_Kq, &h->oz_Kq2, &h->oz_eP, &h->oz_emax, &h->oz_mu, &h->oz_mu2, &h->oz_pmu2, &h->oz_probe,
                       &h->multi_cand, &h->multi_A, &h->multi_B, &h->multi_out, &h->multi_bb, &h->gather, &h->best_global,
-                      &h->de_pop, &h->de_trial, &h->de_param, &h->de_E, &h->de_small, &h->de_sort};
+                      &h->de_pop, &h->de_trial, &h->de_param, &h->de_E, &h->de_small, &h->de_sort, &h->ep_buf, &h->es_state, &h->es_U, &h->es_work, &h->es_in};
     for (DevBuf* b : bufs)
         if (b->p) cudaFree(b->p);
     if (h->ev_ok)
@@ -2583,6 +2590,186 @@ int gpk_oz_contract(gpk_handle* h, const double* P, int n, const double* Ks, lon
     CK(cudaMemcpyAsync(eP, de, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     *eK = ek;
+    return GPK_OK;
+}
+
+int gpk_ep_joint_min(gpk_handle* h, const double* mu, const double* V, int nb, double* logP, double* dlogPdMu,
+                     double* dlogPdSigma, double* dlogPdMudMu, int* sweeps) {
+    if (!h) return GPK_BAD_ARG;
+    if (!mu || !V || !logP) BAD("gpk_ep_joint_min: need mu, V and logP");
+    if (nb < 2 || nb > GPK_EP_MAX_NB) BAD("gpk_ep_joint_min: nb = %d outside 2 .. %d", nb, GPK_EP_MAX_NB);
+    CK(cudaSetDevice(h->device));
+    const size_t D = (size_t)nb, T = D * (D + 1) / 2;
+    // scratch in doubles: mu, V, logP, dMu, dMuMu, dSigma, Zm, Zs, adds, then 2 nb ints (sweeps, status)
+    const size_t omu = 0, oV = omu + D, oP = oV + D * D, odM = oP + D, odMM = odM + D * D, odS = odMM + D * D * D;
+    const size_t oZm = odS + D * T, oZs = oZm + D, oad = oZs + T, oint = oad + D * D;
+    int rc;
+    if ((rc = ensure(h, h->ep_buf, oint * 8 + 2 * D * 4))) return rc;
+    double* b = ptr<double>(h->ep_buf);
+    int* dsw = (int*)(b + oint);
+    int* dst = dsw + D;
+    cudaStream_t st = h->stream;
+    CK(cudaMemcpyAsync(b + omu, mu, D * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(b + oV, V, D * D * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaFuncSetAttribute(gpk_ep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GPK_EP_SMEM));
+    gpk_ep_kernel<<<nb, GPK_EP_THREADS, GPK_EP_SMEM, st>>>(b + omu, b + oV, nb, b + oP, b + odM, b + odMM, b + odS, dsw, dst);
+    CKL();
+    std::vector<int> status(D);
+    CK(cudaMemcpyAsync(status.data(), dst, D * 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    // the reference solves the problems in order k = 0, 1, ...: the first failing one decides the error
+    for (size_t k = 0; k < D; ++k) {
+        if (status[k] == GPK_EP_NAN_VARIANCE) {
+            set_err(h, "an error occurs while running expectation propagation in entropy search. "
+                       "Resulting variance contains NaN");
+            return GPK_EP_FAILED;
+        }
+        if (status[k] == GPK_EP_IRSR_NOT_PD) {
+            set_err(h, "gpk_ep_joint_min: IRSR of problem %zu is not positive definite", k);
+            return GPK_NOT_PD;
+        }
+    }
+    gpk_ep_norm_kernel<<<1, GPK_EP_THREADS, 0, st>>>(nb, b + oP, b + odM, b + odMM, b + odS, b + oZm, b + oZs, b + oad);
+    CKL();
+    gpk_ep_apply_kernel<<<nb, GPK_EP_THREADS, 0, st>>>(nb, b + odM, b + odMM, b + odS, b + oZm, b + oZs, b + oad);
+    CKL();
+    CK(cudaMemcpyAsync(logP, b + oP, D * 8, cudaMemcpyDeviceToHost, st));
+    if (dlogPdMu) CK(cudaMemcpyAsync(dlogPdMu, b + odM, D * D * 8, cudaMemcpyDeviceToHost, st));
+    if (dlogPdSigma) CK(cudaMemcpyAsync(dlogPdSigma, b + odS, D * T * 8, cudaMemcpyDeviceToHost, st));
+    if (dlogPdMudMu) CK(cudaMemcpyAsync(dlogPdMudMu, b + odMM, D * D * D * 8, cudaMemcpyDeviceToHost, st));
+    if (sweeps) CK(cudaMemcpyAsync(sweeps, dsw, D * 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    return GPK_OK;
+}
+
+// layout of h->es_state (doubles): logP (nb), lmb (nb), dMu (nb x nb), dSig (nb x T), Hs (nb x T), W (np), lower (d),
+// upper (d), scaled zb (nb x d)
+struct EsLayout {
+    size_t logP, lmb, dMu, dSig, Hs, W, lo, up, zb, total;
+    EsLayout(int nb, int np_, int d) {
+        const size_t T = (size_t)nb * (nb + 1) / 2;
+        logP = 0; lmb = logP + nb; dMu = lmb + nb; dSig = dMu + (size_t)nb * nb; Hs = dSig + nb * T; W = Hs + nb * T;
+        lo = W + np_; up = lo + d; zb = up + d; total = zb + (size_t)nb * d;
+    }
+};
+
+int gpk_es_update(gpk_handle* h, const double* zb, int nb, const double* lmb, double sn2, const double* W, int np_,
+                  const double* lower, const double* upper, double* logP, double* dlogPdMu, double* dlogPdSigma,
+                  double* dlogPdMudMu) {
+    int rc = require(h, true, true, true);
+    if (rc) return rc;
+    if (!zb || !lmb || !W || !lower || !upper) BAD("gpk_es_update: need zb, lmb, W, lower and upper");
+    if (nb < 2 || nb > GPK_EP_MAX_NB) BAD("gpk_es_update: Nb = %d outside 2 .. %d", nb, GPK_EP_MAX_NB);
+    if (np_ < 1) BAD("gpk_es_update: Np = %d < 1", np_);
+    for (int i = 0; i < nb; ++i)
+        if (!std::isfinite(lmb[i])) BAD("lmb should not be infinite.");
+    const int d = h->d, n = h->n, NP = h->NP;
+    const size_t D = (size_t)nb, T = D * (D + 1) / 2;
+    std::vector<double> mu(D), V(D * D), lp(D), dMu(D * D), dSig(D * T), dMuMu(D * D * D);
+    if ((rc = gpk_predict_cov(h, zb, nb, mu.data(), V.data()))) return rc;          // predict(zb, full_cov=True)
+    if ((rc = gpk_ep_joint_min(h, mu.data(), V.data(), nb, lp.data(), dMu.data(), dSig.data(), dMuMu.data(), nullptr)))
+        return rc;
+    // H of the loss (information_gain.py:82) and dlogPdMudMu folded to its lower triangle
+    double H = 0.0;
+    for (size_t i = 0; i < D; ++i) H += std::exp(lp[i]) * (lp[i] + lmb[i]);
+    H = -H;
+    std::vector<double> Hs(D * T);
+    for (size_t i = 0; i < D; ++i)
+        for (size_t a = 0; a < D; ++a)
+            for (size_t b = 0; b <= a; ++b)
+                Hs[i * T + a * (a + 1) / 2 + b] = a == b ? dMuMu[(i * D + a) * D + a]
+                                                         : dMuMu[(i * D + a) * D + b] + dMuMu[(i * D + b) * D + a];
+    EsLayout L(nb, np_, d);
+    if ((rc = ensure(h, h->es_state, L.total * 8))) return rc;
+    double* st = ptr<double>(h->es_state);
+    cudaStream_t s = h->stream;
+    CK(cudaMemcpyAsync(st + L.logP, lp.data(), D * 8, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(st + L.lmb, lmb, D * 8, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(st + L.dMu, dMu.data(), D * D * 8, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(st + L.dSig, dSig.data(), D * T * 8, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(st + L.Hs, Hs.data(), D * T * 8, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(st + L.W, W, (size_t)np_ * 8, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(st + L.lo, lower, (size_t)d * 8, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(st + L.up, upper, (size_t)d * 8, cudaMemcpyHostToDevice, s));
+    // scaled zb, then U = L^-T (L^-1 K(X, zb)) in fp64 from the handle's L^-1
+    if ((rc = ensure(h, h->tmp1, D * d * 8))) return rc;
+    CK(cudaMemcpyAsync(h->tmp1.p, zb, D * d * 8, cudaMemcpyHostToDevice, s));
+    const double* lo = h->has_bounds ? ptr<double>(h->lower) : nullptr;
+    const double* up = h->has_bounds ? ptr<double>(h->upper) : nullptr;
+    gpk_es_scale_kernel<<<(unsigned)((D * d + 255) / 256), 256, 0, s>>>(ptr<double>(h->tmp1), nb, d, lo, up, st + L.zb);
+    CKL();
+    if (!h->linv_ready && (rc = build_linv(h))) return rc;
+    if ((rc = ensure(h, h->es_U, (size_t)NP * D * 8 * 2))) return rc;
+    double* U = ptr<double>(h->es_U);
+    double* tmp = U + (size_t)NP * D;
+    CK(cudaMemsetAsync(tmp, 0, (size_t)NP * D * 8, s));
+    gpk_es_kxz_kernel<<<(unsigned)(((long)n * nb + 255) / 256), 256, 0, s>>>(h->spec, ptr<double>(h->Xrow), n, d, st + L.zb,
+                                                                              nb, tmp);
+    CKL();
+    gpk_es_trmm_kernel<<<(unsigned)(((long)NP * nb + 255) / 256), 256, 0, s>>>(ptr<double>(h->P), NP, tmp, nb, 0, U);
+    CKL();
+    gpk_es_trmm_kernel<<<(unsigned)(((long)NP * nb + 255) / 256), 256, 0, s>>>(ptr<double>(h->P), NP, U, nb, 1, tmp);
+    CKL();
+    CK(cudaMemcpyAsync(U, tmp, (size_t)NP * D * 8, cudaMemcpyDeviceToDevice, s));
+    CK(cudaStreamSynchronize(s));
+    h->es_nb = nb;
+    h->es_np = np_;
+    h->es_sn2 = sn2;
+    h->es_H = H;
+    h->es_linv_serial = h->linv_serial;
+    if (logP) std::copy(lp.begin(), lp.end(), logP);
+    if (dlogPdMu) std::copy(dMu.begin(), dMu.end(), dlogPdMu);
+    if (dlogPdSigma) std::copy(dSig.begin(), dSig.end(), dlogPdSigma);
+    if (dlogPdMudMu) std::copy(dMuMu.begin(), dMuMu.end(), dlogPdMudMu);
+    return GPK_OK;
+}
+
+int gpk_es_compute_dev(gpk_handle* h, const void* d_Xs, long m, void* d_out) {
+    int rc = require(h, true, true, true);
+    if (rc) return rc;
+    if (!d_Xs || !d_out || m <= 0) BAD("gpk_es_compute_dev: need candidates and out");
+    if (h->es_linv_serial < 0) BAD("gpk_es_compute: call gpk_es_update first");
+    if (!h->linv_ready || h->es_linv_serial != h->linv_serial) BAD("gpk_es_compute: the model changed since gpk_es_update");
+    CK(cudaSetDevice(h->device));
+    const int nb = h->es_nb, d = h->d;
+    EsLayout L(nb, h->es_np, d);
+    const double* st = ptr<double>(h->es_state);
+    const long CH = 16384;                  // candidates per pass; every candidate is independent of the others
+    if ((rc = ensure(h, h->es_work, (size_t)CH * (nb + 1) * 8))) return rc;
+    double* var = ptr<double>(h->es_work);
+    double* sig = var + CH;
+    const double* lo = h->has_bounds ? ptr<double>(h->lower) : nullptr;
+    const double* up = h->has_bounds ? ptr<double>(h->upper) : nullptr;
+    const double out_scale = h->norm_out ? h->y_std * h->y_std : 1.0;
+    for (long c0 = 0; c0 < m; c0 += CH) {
+        const long rows = std::min(CH, m - c0);
+        const double* X = (const double*)d_Xs + c0 * d;
+        if ((rc = score_dev(h, X, rows, GPK_ACQ_NONE, 0.0, 0.0, nullptr, nullptr, var, nullptr, nullptr))) return rc;
+        gpk_es_sigma_kernel<<<(unsigned)rows, GPK_ES_THREADS, 0, h->stream>>>(h->spec, X, rows, d, lo, up,
+                                                                              ptr<double>(h->Xrow), h->n,
+                                                                              ptr<double>(h->es_U), st + L.zb, nb,
+                                                                              out_scale, sig);
+        CKL();
+        gpk_es_dh_kernel<<<(unsigned)rows, GPK_ES_THREADS, 0, h->stream>>>(
+            X, rows, d, st + L.lo, st + L.up, var, sig, nb, h->es_np, h->es_sn2, h->es_H, st + L.logP, st + L.lmb,
+            st + L.dMu, st + L.dSig, st + L.Hs, st + L.W, (double*)d_out + c0);
+        CKL();
+    }
+    return GPK_OK;
+}
+
+int gpk_es_compute(gpk_handle* h, const double* Xs, long m, double* out) {
+    int rc = require(h, true, true, true);
+    if (rc) return rc;
+    if (!Xs || !out || m <= 0) BAD("gpk_es_compute: need candidates and out");
+    CK(cudaSetDevice(h->device));
+    if ((rc = ensure(h, h->es_in, (size_t)m * (h->d + 1) * 8))) return rc;
+    double* dX = ptr<double>(h->es_in);
+    double* dout = dX + (size_t)m * h->d;
+    CK(cudaMemcpyAsync(dX, Xs, (size_t)m * h->d * 8, cudaMemcpyHostToDevice, h->stream));
+    if ((rc = gpk_es_compute_dev(h, dX, m, dout))) return rc;
+    CK(cudaMemcpyAsync(out, dout, (size_t)m * 8, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
     return GPK_OK;
 }
 
