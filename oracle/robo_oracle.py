@@ -220,6 +220,77 @@ def gp_predict_var_only_fast(st, X_test, chunk=8192):
     return mu, np.clip(var, EPS, np.inf)
 
 
+def _kernel_input_grad(k, Xs, X):
+    """(k(Xs, X) (m, n), d k(Xs, X) / d Xs (m, n, ndim)) of a george_oracle kernel, by the product rule over its tree:
+    ConstantKernel -> 0; radial kernel f(r2) -> f'(r2) * 2 (x*_a - x_a) / metric_a on each of its axes."""
+    if isinstance(k, G.Product):
+        v1, g1 = _kernel_input_grad(k.k1, Xs, X)
+        v2, g2 = _kernel_input_grad(k.k2, Xs, X)
+        return v1 * v2, g1 * v2[:, :, None] + g2 * v1[:, :, None]
+    if isinstance(k, G.ConstantKernel):
+        return k._value(Xs, X), np.zeros((len(Xs), len(X), Xs.shape[1]))
+    if isinstance(k, G._RadialKernel):
+        r2 = k._r2(Xs, X)
+        dfdr2 = k._dfdr2(r2)
+        g = np.zeros((len(Xs), len(X), Xs.shape[1]))
+        for a, md in zip(k.axes, k._axis_metric()):
+            g[:, :, a] += dfdr2 * (2.0 * (Xs[:, a][:, None] - X[:, a][None, :]) / md)
+        return k._f(r2), g
+    raise TypeError("gp_predictive_gradients: unsupported kernel %r" % type(k))
+
+
+def gp_predictive_gradients(st, X_test, chunk_elems=1 << 22):
+    """Input gradients of GaussianProcess.predict's moments at the rows of X_test, in raw input coordinates:
+        d mu / d x   = dk* . alpha                      (alpha = K^-1 (y - mean))
+        d var / d x  = -2 dk* . w,   w = K^-1 k*        (k** is constant: stationary kernels)
+    dk* from the george kernel tree (_kernel_input_grad), then the chain rules of zero_one_normalization
+    (1 / (upper - lower)) and of the output un-normalisation (y_std, y_std^2).  The clip of var at DBL_EPSILON is not
+    differentiated.  Returns dict(dmu, dvar, s_mu, s_var), each (m, D): s_mu = sum_j |dk_j| |alpha_j| and
+    s_var = 2 sum_j |dk_j| |w_j| (same chain factors) are the magnitudes the sums cancel from, the natural error scale
+    of any floating-point evaluation of them."""
+    X_test = np.asarray(X_test, dtype=np.float64)
+    if st["normalize_input"]:
+        Xs, _, _ = zero_one_normalization(X_test, st["lower"], st["upper"])
+        chain = 1.0 / (np.asarray(st["upper"], dtype=np.float64) - np.asarray(st["lower"], dtype=np.float64))
+    else:
+        Xs, chain = X_test, np.ones(X_test.shape[1])
+    gp = st["gp"]
+    alpha = gp._compute_alpha(st["y"])
+    X = gp._x
+    m, D = Xs.shape
+    out = {k: np.empty((m, D)) for k in ("dmu", "dvar", "s_mu", "s_var")}
+    step = max(1, chunk_elems // max(1, len(X) * D))
+    for lo in range(0, m, step):
+        Ks, dK = _kernel_input_grad(gp.kernel, Xs[lo:lo + step], X)
+        W = gp.solver.apply_inverse(Ks.T)                                  # (n, mc)
+        sl = slice(lo, lo + step)
+        out["dmu"][sl] = np.einsum("cja,j->ca", dK, alpha)
+        out["dvar"][sl] = -2.0 * np.einsum("cja,jc->ca", dK, W)
+        out["s_mu"][sl] = np.einsum("cja,j->ca", np.abs(dK), np.abs(alpha))
+        out["s_var"][sl] = 2.0 * np.einsum("cja,jc->ca", np.abs(dK), np.abs(W))
+    ys = st["y_std"] if st["normalize_output"] else 1.0
+    for k, f in (("dmu", ys), ("s_mu", ys), ("dvar", ys * ys), ("s_var", ys * ys)):
+        out[k] *= chain[None, :] * f
+    return out
+
+
+def acq_gradients(mu, var, dmu, dvar, kind, eta=0.0, par=0.0):
+    """(f (m,), df (m, D)): value and input gradient of EI / PI / LCB from the moments and their gradients, as the
+    reference writes them with derivative=True (ei.py:80-85, pi.py:65-71, lcb.py:66-69); ds = dvar / (2 s)."""
+    mu, var = np.asarray(mu, dtype=np.float64), np.asarray(var, dtype=np.float64)
+    s = np.sqrt(var)
+    dm, ds = np.asarray(dmu), np.asarray(dvar) / (2.0 * s[:, None])
+    if kind == "lcb":
+        return acq_lcb(mu, var, par), -(dm - par * ds)
+    z = (eta - mu - par) / s
+    if kind == "ei":
+        f = s * (z * ndtr(z) + _pdf(z))
+        return f, -dm * ndtr(z)[:, None] + ds * _pdf(z)[:, None]
+    if kind == "pi":
+        return ndtr(z), (-_pdf(z) / s)[:, None] * (dm + ds * z[:, None])
+    raise ValueError("acq_gradients: %r has no input gradient" % kind)
+
+
 def gp_predict_variance(st, x1, X2):
     """GaussianProcess.predict_variance: gaussian_process.py:221-248."""
     x_ = np.concatenate((x1, X2))
