@@ -98,13 +98,7 @@ const char* gpk_version(void);
  *               four 32-row tiles), the rows below run on a second high-priority stream, trailing update with
  *               look-ahead 2;
  *               0 = plain look-ahead schedule [default] (bit-identical factor)
- *   "diag"      diagonal-block Cholesky + inverse kernel: 4 = 16-column panels, square-root-free pivot chain in one warp,
- *               substitutions in four, rank-16 updates on the fp64 tensor pipe [default]; 3 = the same with DFMA register
- *               tiles; 2 = column-by-column register-tiled kernel; 0 = simple shared-memory version (cross-checks)
- *   "diagprof"  1 = the blocked diagonal kernels record clock64() stamps per phase (gpk_get_diag_profile)
- *   "lookahead" 1 = trailing updates on a side stream, overlapped with the next diag/panel [default]
- *   "smalltile" 1 = 32-row tiles for the panel solve / next-panel update [default], 2 = 16-row tiles, 0 = 128-row tiles
- *   "fusechain" 1 = panel solve + next-panel update of a step in one launch (default 0)
+ *   "diagprof"  1 = the diagonal-block kernel records clock64() stamps per phase (gpk_get_diag_profile)
  *   "pdl"       1 = programmatic dependent launch for the kernels of the Cholesky chain [default]
  *   "overlap"   1 = build K* of chunk i+1 on the side stream while chunk i contracts [default] */
 int gpk_set_option(gpk_handle* h, const char* key, long value);

@@ -147,8 +147,6 @@ class Handle(object):
         # test/diagnostic overrides: GPK_LOADER=0|1 (cp.async | TMA staging), GPK_CHUNK=<multiple of 128>
         if os.environ.get("GPK_LOADER"):
             self.set_option("loader", int(os.environ["GPK_LOADER"]))
-        if os.environ.get("GPK_DIAG"):
-            self.set_option("diag", int(os.environ["GPK_DIAG"]))
         if os.environ.get("GPK_CHUNK"):
             self.set_option("chunk", int(os.environ["GPK_CHUNK"]))
         # implementation switches (all default-on variants have a cross-check twin): GPK_COV=1|2, GPK_PERSIST=0|1,

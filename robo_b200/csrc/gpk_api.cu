@@ -81,16 +81,12 @@ struct gpk_handle {
     cudaGraphExec_t fit_graph = nullptr;
     double fit_graph_launches = 0;
     int chainsplit = 0;             // 1: diag(k+1) waits only for block row k+1 of step k (gpk_chain_step_kernel on 4 CTAs)
-    int lookahead = 1;
-    int smalltile = 1;              // 32-row tiles for the panel solve / next-panel update
     int pdl = 1;                    // programmatic dependent launch on the Cholesky chain
-    int fusechain = 0;              // 1: panel solve + next-panel update of a step in one launch (gpk_chain.cuh)
     DevBuf chain_cnt;
     char err[1024] = {0};
     int loader = LOADER_TMA_WS;
     long chunk = 16384;
     bool chunk_user = false;        // false: candidates per scoring pass chosen from N (chunk_rows)
-    int diag_kernel = 4;          // 4 = blocked 16-column panels, DMMA updates (default); 3 = same with DFMA register tiles, 2 = column-by-column register-tiled, 0 = simple shared-memory version
     int diag_prof = 0;            // 1: the blocked diagonal kernel records clock64() stamps per phase (diagnostics)
     DevBuf dprof;
 
@@ -119,7 +115,7 @@ struct gpk_handle {
     int jobs_nb = -1;
 
     // job tables
-    std::vector<Range> trsm_r, syrk_r, tri1_r, tri2_r, trsm32_r, pu32_r, trsm16_r, pu16_r;
+    std::vector<Range> syrk_r, tri1_r, tri2_r, trsm32_r, pu32_r;
     std::vector<Range> syrk2_r;     // depth-2 trailing update: columns >= k+2 with panels k-1 and k in one contraction (K = 256)
     int depth2 = 2;                 // 0 / 1, or 2 = automatic: on for nb >= 48 (trailing updates gate the fit only there)
     Range kinv_r;
@@ -128,10 +124,10 @@ struct gpk_handle {
 
     // tensor maps
     CUtensorMap mapK, mapP, mapQ, mapW, mapKs, mapVt;
-    CUtensorMap mapK32, mapK16, mapKs2;
+    CUtensorMap mapK32, mapKs2;     // mapK32: Kbuf with a 32-row box, A operand of the 32-row chain GEMMs
     long mapKs2_rows = 0;
     std::vector<cudaEvent_t> ev_cov, ev_gemm;
-    int overlap = 1;                // build K* of chunk i+1 on the side stream while chunk i contracts            // Kbuf with a 32-row box: A operand of the small-tile chain GEMMs
+    int overlap = 1;                // build K* of chunk i+1 on the side stream while chunk i contracts
     bool maps_ok = false;
     long mapKs_rows = 0, mapVt_rows = 0;
 
@@ -432,7 +428,7 @@ int launch_gemm(gpk_handle* h, const CUtensorMap& mA, const CUtensorMap& mB, con
                 cudaStream_t stream = nullptr, bool pdl = false) {
     if (njobs <= 0) return GPK_OK;
     if (stream == nullptr) stream = h->stream;
-    if (pdl && h->pdl && h->loader != LOADER_CPASYNC && MI <= 2) {
+    if (pdl && h->pdl && h->loader != LOADER_CPASYNC && MI == 2) {
         CK(launch_pdl(gpk_gemm_nt_kernel<EPI, LOADER_TMA, MI>, dim3(njobs), dim3(GEMM_THREADS),
                       (size_t)gemm_smem_bytes(LOADER_TMA, MI), stream, mA, mB, a));
         h->launches_total += 1;
@@ -457,8 +453,6 @@ int set_kernel_attrs(gpk_handle* h) {
     CK(cudaFuncSetAttribute(gpk_gemm_ws_kernel<EPI_COLREDUCE>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM_TMA));
     CK(cudaFuncSetAttribute(gpk_gemm_nt_kernel<EPI_STORE, LOADER_TMA, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm_smem_bytes(LOADER_TMA, 2)));
     CK(cudaFuncSetAttribute(gpk_gemm_nt_kernel<EPI_STORE, LOADER_CPASYNC, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm_smem_bytes(LOADER_CPASYNC, 2)));
-    CK(cudaFuncSetAttribute(gpk_gemm_nt_kernel<EPI_STORE, LOADER_CPASYNC, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm_smem_bytes(LOADER_CPASYNC, 1)));
-    CK(cudaFuncSetAttribute(gpk_gemm_nt_kernel<EPI_STORE, LOADER_TMA, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm_smem_bytes(LOADER_TMA, 1)));
     CK(cudaFuncSetAttribute(gpk_oz_vargemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, OZ_SMEM));
     CK(cudaFuncSetAttribute(gpk_cov_oz_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cov_oz_smem_bytes(GPK_MAX_TERMS, 8)));
     CK(cudaFuncSetAttribute(gpk_cov_oz_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cov_oz_smem_bytes(GPK_MAX_TERMS, 4)));
@@ -470,11 +464,8 @@ int set_kernel_attrs(gpk_handle* h) {
     }
     CK(cudaFuncSetAttribute(gpk_cov_tma_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cov_tma_smem_bytes(GPK_MAX_TERMS, 8)));
     CK(cudaFuncSetAttribute(gpk_cov_tma_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cov_tma_smem_bytes(GPK_MAX_TERMS, 4)));
-    CK(cudaFuncSetAttribute(gpk_potrf_diag_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DIAG_SMEM));
-    CK(cudaFuncSetAttribute(gpk_potrf_diag_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DIAG2_SMEM));
     CK(cudaFuncSetAttribute(gpk_chain_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, CH_SMEM));
-    CK(cudaFuncSetAttribute(gpk_potrf_diag_blocked_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DIAG3_SMEM));
-    CK(cudaFuncSetAttribute(gpk_potrf_diag_dmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DIAG4_SMEM));
+    CK(cudaFuncSetAttribute(gpk_potrf_diag_dmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DIAG_SMEM));
     return GPK_OK;
 }
 
@@ -495,13 +486,8 @@ int build_job_tables(gpk_handle* h) {
     const int nb = h->nb;
     if (h->jobs_nb == nb) return GPK_OK;
     std::vector<GemmJob> jobs;
-    h->trsm_r.assign(nb, Range());
     h->syrk_r.assign(nb, Range());
     for (int k = 0; k < nb; ++k) {
-        h->trsm_r[k].off = (int)jobs.size();
-        for (int i = k + 1; i <= nb; ++i)          // i == nb: augmented rhs block row
-            jobs.push_back({i * BM, k * BM, k * BM, (k + 1) * BM, i * BM, k * BM, 0, 0});
-        h->trsm_r[k].cnt = (int)jobs.size() - h->trsm_r[k].off;
         h->syrk_r[k].off = (int)jobs.size();
         for (int j = k + 1; j < nb; ++j)
             for (int i = j; i <= nb; ++i)
@@ -538,26 +524,6 @@ int build_job_tables(gpk_handle* h) {
                     jobs.push_back({i * BM + 32 * q, (k + 1) * BM, k * BM, (k + 1) * BM, i * BM + 32 * q, (k + 1) * BM, 0, 0});
                 }
         h->pu32_r[k].cnt = (int)jobs.size() - h->pu32_r[k].off;
-    }
-    // 16-row versions (option smalltile = 2): twice the CTAs, half the arithmetic per CTA on the chain
-    h->trsm16_r.assign(nb, Range());
-    h->pu16_r.assign(nb, Range());
-    for (int k = 0; k < nb; ++k) {
-        h->trsm16_r[k].off = (int)jobs.size();
-        for (int i = k + 1; i <= nb; ++i)
-            for (int q = 0; q < 8; ++q) {
-                if (i == nb && q > 0) break;
-                jobs.push_back({i * BM + 16 * q, k * BM, k * BM, (k + 1) * BM, i * BM + 16 * q, k * BM, 0, 0});
-            }
-        h->trsm16_r[k].cnt = (int)jobs.size() - h->trsm16_r[k].off;
-        h->pu16_r[k].off = (int)jobs.size();
-        if (k + 1 < nb)
-            for (int i = k + 1; i <= nb; ++i)
-                for (int q = 0; q < 8; ++q) {
-                    if (i == nb && q > 0) break;
-                    jobs.push_back({i * BM + 16 * q, (k + 1) * BM, k * BM, (k + 1) * BM, i * BM + 16 * q, (k + 1) * BM, 0, 0});
-                }
-        h->pu16_r[k].cnt = (int)jobs.size() - h->pu16_r[k].off;
     }
     std::vector<Node> nodes;
     int hmax = build_nodes(0, nb, nodes);
@@ -646,7 +612,6 @@ int rebuild_maps(gpk_handle* h) {
     int rc;
     if ((rc = make_map(h, &h->mapK, h->Kbuf.p, NP + BM, NP, NP))) return rc;
     if ((rc = make_map(h, &h->mapK32, h->Kbuf.p, NP + BM, NP, NP, 32))) return rc;
-    if ((rc = make_map(h, &h->mapK16, h->Kbuf.p, NP + BM, NP, NP, 16))) return rc;
     if ((rc = make_map(h, &h->mapP, h->P.p, NP, NP, NP))) return rc;
     if ((rc = make_map(h, &h->mapQ, h->Q.p, NP, NP, NP))) return rc;
     if ((rc = make_map(h, &h->mapW, h->W.p, NP, NP, NP))) return rc;
@@ -1239,11 +1204,6 @@ int gpk_set_option(gpk_handle* h, const char* key, long value) {
         h->chainsplit = (int)value;
         return GPK_OK;
     }
-    if (!strcmp(key, "fusechain")) {
-        if (value != 0 && value != 1) BAD("fusechain must be 0 or 1");
-        h->fusechain = (int)value;
-        return GPK_OK;
-    }
     if (!strcmp(key, "pdl")) {
         if (value != 0 && value != 1) BAD("pdl must be 0 or 1");
         h->pdl = (int)value;
@@ -1252,16 +1212,6 @@ int gpk_set_option(gpk_handle* h, const char* key, long value) {
     if (!strcmp(key, "overlap")) {
         if (value != 0 && value != 1) BAD("overlap must be 0 or 1");
         h->overlap = (int)value;
-        return GPK_OK;
-    }
-    if (!strcmp(key, "smalltile")) {
-        if (value < 0 || value > 2) BAD("smalltile must be 0 (128-row chain tiles), 1 (32 rows) or 2 (16 rows)");
-        h->smalltile = (int)value;
-        return GPK_OK;
-    }
-    if (!strcmp(key, "lookahead")) {
-        if (value != 0 && value != 1) BAD("lookahead must be 0 or 1");
-        h->lookahead = (int)value;
         return GPK_OK;
     }
     if (!strcmp(key, "diagprof")) {                 // 1: stamps; 2: stamps + skip the kernel's global stores (timing only)
@@ -1275,13 +1225,6 @@ int gpk_set_option(gpk_handle* h, const char* key, long value) {
                 CK(cudaMemcpy((char*)h->dprof.p + 63 * 8, &one, 8, cudaMemcpyHostToDevice));
             }
         }
-        return GPK_OK;
-    }
-    if (!strcmp(key, "diag")) {
-        if (value != 0 && value != 2 && value != 3 && value != 4)
-            BAD("diag must be 4 (blocked panels, DMMA updates), 3 (blocked panels, DFMA register tiles), 2 (column-by-column "
-                "register-tiled kernel) or 0 (simple shared-memory kernel)");
-        h->diag_kernel = (int)value;
         return GPK_OK;
     }
     if (!strcmp(key, "cov")) {
@@ -1454,23 +1397,17 @@ int gpk_fit_begin(gpk_handle* h, double diag_add, double mean) {
         h->ev_rest.push_back(e2);
     }
     std::vector<char> rest_recorded(nb, 0);
-    const bool fuse = h->fusechain && h->smalltile == 1 && h->lookahead;
-    if (fuse) {
-        if ((rc = ensure(h, h->chain_cnt, (size_t)nb * 4))) return rc;
-        CK(cudaMemsetAsync(h->chain_cnt.p, 0, (size_t)nb * 4, h->stream));
-    }
-    // ---- split chain (default): only block row k+1 of step k stays between diag(k) and diag(k+1) ----------------
-    // Step k of the right-looking factorisation used to put diag(k) -> panel solve (all rows) -> update of block column
+    // ---- split chain (option "chainsplit" = 1): only block row k+1 of step k stays between diag(k) and diag(k+1) ---
+    // Step k of the plain look-ahead schedule (below) puts diag(k) -> panel solve (all rows) -> update of block column
     // k+1 (all rows) on the critical chain.  diag(k+1) only needs A[k+1,k+1] -= L[k+1,k] L[k+1,k]^T with
     // L[k+1,k] = A[k+1,k] inv(L_kk)^T: one launch of gpk_chain_step_kernel on the four 32-row tiles of block row k+1
     // ("X(k)").  The rows below go to a second high-priority stream and overlap diag(k+1); the trailing update is cut
     // in two (block column k+2 first) so that the chain waits for one column, not for the whole update (look-ahead 2).
-    // Every tile still receives its panels in increasing order: the factor is bit-identical to the other schedules.
+    // Every tile still receives its panels in increasing order: the factor is bit-identical to the plain schedule.
     //   C (h->stream)     diag(k) . X(k) . diag(k+1) ...
     //   P (panel_stream)  solve'(k) [rows > k+1] . update'(k) [block column k+1, rows > k+1]
     //   R (side_stream)   rest_a(k) [block column k+2] . rest_b(k) [block columns >= k+3]
-    const bool split = h->chainsplit && h->smalltile == 1 && h->lookahead && !fuse && h->diag_kernel >= 3 &&
-                       h->loader != LOADER_CPASYNC && nb >= 3;
+    const bool split = h->chainsplit && h->loader != LOADER_CPASYNC && nb >= 3;
     if (split) {
         if ((rc = ensure(h, h->chain_cnt, (size_t)nb * 4))) return rc;
         while ((int)h->ev_cs.size() < 5 * nb + 3) {
@@ -1498,12 +1435,8 @@ int gpk_fit_begin(gpk_handle* h, double diag_add, double mean) {
         for (int k = 0; k < nb; ++k) {
             long long* dprof = h->diag_prof ? ptr<long long>(h->dprof) : nullptr;
             // ---- C: diag(k)
-            if (h->diag_kernel == 4)
-                gpk_potrf_diag_dmma_kernel<<<1, 256, DIAG4_SMEM, C>>>(K, NP, k, ptr<double>(h->P), ptr<double>(h->Q), NP,
-                                                                     ptr<int>(h->status), ptr<double>(h->logdet_part), dprof);
-            else
-                gpk_potrf_diag_blocked_kernel<<<1, 256, DIAG3_SMEM, C>>>(K, NP, k, ptr<double>(h->P), ptr<double>(h->Q), NP,
-                                                                        ptr<int>(h->status), ptr<double>(h->logdet_part), dprof);
+            gpk_potrf_diag_dmma_kernel<<<1, 256, DIAG_SMEM, C>>>(K, NP, k, ptr<double>(h->P), ptr<double>(h->Q), NP,
+                                                                 ptr<int>(h->status), ptr<double>(h->logdet_part), dprof);
             CKL();
             CK(cudaEventRecord(evD(k), C));
             const int nsolve = h->trsm32_r[k].cnt, nupd = h->pu32_r[k].cnt;
@@ -1607,67 +1540,21 @@ int gpk_fit_begin(gpk_handle* h, double diag_add, double mean) {
             return rc;
         }
     }
-    if (!split && h->diag_kernel >= 3) {
+    // ---- plain look-ahead schedule [default]: diag(k), then the panel solve and the update of block column k+1 in
+    // 32-row tiles on the critical stream; the rest of the trailing update on the side stream
+    if (!split) {
         gpk_diag_prezero_kernel<<<nb, 256, 0, h->stream>>>(K, (long)NP, ptr<double>(h->P), (long)NP);
         CKL();
     }
     for (int k = 0; k < nb && !split; ++k) {
         long long* dprof = h->diag_prof ? ptr<long long>(h->dprof) : nullptr;
-        if (h->diag_kernel == 4 && h->pdl && k > 0)
-            CK(launch_pdl(gpk_potrf_diag_dmma_kernel, dim3(1), dim3(256), (size_t)DIAG4_SMEM, h->stream, K, (long)NP, k,
+        if (h->pdl && k > 0)
+            CK(launch_pdl(gpk_potrf_diag_dmma_kernel, dim3(1), dim3(256), (size_t)DIAG_SMEM, h->stream, K, (long)NP, k,
                           ptr<double>(h->P), ptr<double>(h->Q), (long)NP, ptr<int>(h->status), ptr<double>(h->logdet_part), dprof));
-        else if (h->diag_kernel == 4)
-            gpk_potrf_diag_dmma_kernel<<<1, 256, DIAG4_SMEM, h->stream>>>(K, NP, k, ptr<double>(h->P), ptr<double>(h->Q), NP,
-                                                                          ptr<int>(h->status), ptr<double>(h->logdet_part), dprof);
-        else if (h->diag_kernel == 3 && h->pdl && k > 0)
-            CK(launch_pdl(gpk_potrf_diag_blocked_kernel, dim3(1), dim3(256), (size_t)DIAG3_SMEM, h->stream, K, (long)NP, k,
-                          ptr<double>(h->P), ptr<double>(h->Q), (long)NP, ptr<int>(h->status), ptr<double>(h->logdet_part), dprof));
-        else if (h->diag_kernel == 3)
-            gpk_potrf_diag_blocked_kernel<<<1, 256, DIAG3_SMEM, h->stream>>>(K, NP, k, ptr<double>(h->P), ptr<double>(h->Q), NP,
-                                                                             ptr<int>(h->status), ptr<double>(h->logdet_part), dprof);
-        else if (h->diag_kernel == 2 && h->pdl && k > 0)
-            CK(launch_pdl(gpk_potrf_diag_fused_kernel, dim3(1), dim3(256), (size_t)DIAG2_SMEM, h->stream, K, (long)NP, k,
-                          ptr<double>(h->P), ptr<double>(h->Q), (long)NP, ptr<int>(h->status), ptr<double>(h->logdet_part)));
-        else if (h->diag_kernel == 2)
-            gpk_potrf_diag_fused_kernel<<<1, 256, DIAG2_SMEM, h->stream>>>(K, NP, k, ptr<double>(h->P), ptr<double>(h->Q), NP,
-                                                                           ptr<int>(h->status), ptr<double>(h->logdet_part));
         else
-            gpk_potrf_diag_kernel<<<1, 256, DIAG_SMEM, h->stream>>>(K, NP, k, ptr<double>(h->P), ptr<double>(h->Q), NP,
-                                                                    ptr<int>(h->status), ptr<double>(h->logdet_part));
+            gpk_potrf_diag_dmma_kernel<<<1, 256, DIAG_SMEM, h->stream>>>(K, NP, k, ptr<double>(h->P), ptr<double>(h->Q), NP,
+                                                                         ptr<int>(h->status), ptr<double>(h->logdet_part), dprof);
         CKL();
-        if (fuse) {
-            // one launch for panel solve + next-panel update (gpk_chain.cuh).  Its second pass writes block column
-            // k+1, which the rest of step k-1 (side stream) also updates: wait for that first.
-            const int npu = nb - k;
-            if (k >= 1 && rest_recorded[k - 1]) CK(cudaStreamWaitEvent(h->stream, h->ev_rest[k - 1], 0));
-            ChainArgs c;
-            c.K = K; c.ld = NP; c.P = ptr<double>(h->P); c.ldp = NP;
-            c.solve_jobs = ptr<GemmJob>(h->jobs) + h->trsm32_r[k].off;
-            c.update_jobs = h->pu32_r[k].cnt > 0 ? ptr<GemmJob>(h->jobs) + h->pu32_r[k].off : nullptr;
-            c.counter = ptr<int>(h->chain_cnt) + k;
-            c.status = ptr<int>(h->status);
-            if (h->pdl)
-                CK(launch_pdl(gpk_chain_step_kernel, dim3((unsigned)h->trsm32_r[k].cnt), dim3(GEMM_THREADS), (size_t)CH_SMEM,
-                              h->stream, c));
-            else
-                gpk_chain_step_kernel<<<(unsigned)h->trsm32_r[k].cnt, GEMM_THREADS, CH_SMEM, h->stream>>>(c);
-            CKL();
-            h->launches_total += 1;
-            const int off = h->syrk_r[k].off, cnt = h->syrk_r[k].cnt;
-            if (cnt > npu) {
-                CK(cudaEventRecord(h->ev_panel[k], h->stream));
-                CK(cudaStreamWaitEvent(h->side_stream, h->ev_panel[k], 0));
-                GemmArgs s2;
-                memset(&s2, 0, sizeof(s2));
-                s2.A = K; s2.lda = NP; s2.B = K; s2.ldb = NP; s2.C = K; s2.ldc = NP;
-                s2.alpha = -1.0; s2.beta = 1; s2.job_mode = JOBS_TABLE; s2.status = ptr<int>(h->status);
-                s2.jobs = ptr<GemmJob>(h->jobs) + off + npu;
-                if ((rc = launch_gemm<EPI_STORE>(h, h->mapK, h->mapK, s2, cnt - npu, h->side_stream))) return rc;
-                CK(cudaEventRecord(h->ev_rest[k], h->side_stream));
-                rest_recorded[k] = 1;
-            }
-            continue;
-        }
         GemmArgs a;
         memset(&a, 0, sizeof(a));
         a.A = K; a.lda = NP;
@@ -1676,16 +1563,8 @@ int gpk_fit_begin(gpk_handle* h, double diag_add, double mean) {
         a.alpha = 1.0; a.beta = 0;
         a.job_mode = JOBS_TABLE;
         a.status = ptr<int>(h->status);
-        if (h->smalltile == 2) {
-            a.jobs = ptr<GemmJob>(h->jobs) + h->trsm16_r[k].off;
-            if ((rc = launch_gemm<EPI_STORE, 1>(h, h->mapK16, h->mapP, a, h->trsm16_r[k].cnt, nullptr, true))) return rc;
-        } else if (h->smalltile) {
-            a.jobs = ptr<GemmJob>(h->jobs) + h->trsm32_r[k].off;
-            if ((rc = launch_gemm<EPI_STORE, 2>(h, h->mapK32, h->mapP, a, h->trsm32_r[k].cnt, nullptr, true))) return rc;
-        } else {
-            a.jobs = ptr<GemmJob>(h->jobs) + h->trsm_r[k].off;
-            if ((rc = launch_gemm<EPI_STORE>(h, h->mapK, h->mapP, a, h->trsm_r[k].cnt))) return rc;
-        }
+        a.jobs = ptr<GemmJob>(h->jobs) + h->trsm32_r[k].off;
+        if ((rc = launch_gemm<EPI_STORE, 2>(h, h->mapK32, h->mapP, a, h->trsm32_r[k].cnt, nullptr, true))) return rc;
         GemmArgs s;
         memset(&s, 0, sizeof(s));
         s.A = K; s.lda = NP;
@@ -1695,27 +1574,16 @@ int gpk_fit_begin(gpk_handle* h, double diag_add, double mean) {
         s.job_mode = JOBS_TABLE;
         s.status = ptr<int>(h->status);
         const int off = h->syrk_r[k].off, cnt = h->syrk_r[k].cnt;
-        if (!h->lookahead) {
-            s.jobs = ptr<GemmJob>(h->jobs) + off;
-            if ((rc = launch_gemm<EPI_STORE>(h, h->mapK, h->mapK, s, cnt))) return rc;
-        } else if (cnt > 0) {
+        if (cnt > 0) {
             // Look-ahead: the first nb-k jobs update column block k+1 (what the next diagonal block
             // and panel solve need) and stay on the critical stream; the rest of the trailing update
             // runs on the low-priority side stream, overlapped with diag(k+1) / panel(k+1).
             const int npu = nb - k;
             CK(cudaEventRecord(h->ev_panel[k], h->stream));                       // panel k solved
             if (k >= 1 && rest_recorded[k - 1]) CK(cudaStreamWaitEvent(h->stream, h->ev_rest[k - 1], 0));
-            if (h->smalltile == 2) {
-                s.jobs = ptr<GemmJob>(h->jobs) + h->pu16_r[k].off;
-                if ((rc = launch_gemm<EPI_STORE, 1>(h, h->mapK16, h->mapK, s, h->pu16_r[k].cnt, nullptr, true))) return rc;
-            } else if (h->smalltile) {
-                s.jobs = ptr<GemmJob>(h->jobs) + h->pu32_r[k].off;
-                if ((rc = launch_gemm<EPI_STORE, 2>(h, h->mapK32, h->mapK, s, h->pu32_r[k].cnt, nullptr, true))) return rc;
-            } else {
-                s.jobs = ptr<GemmJob>(h->jobs) + off;
-                if ((rc = launch_gemm<EPI_STORE>(h, h->mapK, h->mapK, s, npu))) return rc;
-            }
-            const bool d2 = h->smalltile && (h->depth2 == 1 || (h->depth2 == 2 && nb >= 48));
+            s.jobs = ptr<GemmJob>(h->jobs) + h->pu32_r[k].off;
+            if ((rc = launch_gemm<EPI_STORE, 2>(h, h->mapK32, h->mapK, s, h->pu32_r[k].cnt, nullptr, true))) return rc;
+            const bool d2 = h->depth2 == 1 || (h->depth2 == 2 && nb >= 48);
             if (cnt > npu && !d2) {
                 CK(cudaStreamWaitEvent(h->side_stream, h->ev_panel[k], 0));
                 s.jobs = ptr<GemmJob>(h->jobs) + off + npu;
@@ -1739,7 +1607,7 @@ int gpk_fit_begin(gpk_handle* h, double diag_add, double mean) {
             }
         }
     }
-    if (!split && h->diag_kernel >= 3) {
+    if (!split) {
         gpk_diag_qfill_kernel<<<nb, 256, 0, h->stream>>>(ptr<double>(h->P), ptr<double>(h->Q), (long)NP, ptr<int>(h->status));
         CKL();
     }
@@ -1862,25 +1730,13 @@ int gpk_fit_append(gpk_handle* h, const double* X, const double* y, int n, int d
     CK(cudaMemcpy2DAsync(K + (long)N1 * NP, (size_t)NP * 8, W + (long)N1 * NP, (size_t)NP * 8, (size_t)N1 * 8, BM,
                          cudaMemcpyDeviceToDevice, h->stream));
     // factor + invert the last diagonal block
-    if (h->diag_kernel >= 3) {
-        gpk_diag_prezero_kernel<<<1, 256, 0, h->stream>>>(K + (long)N1 * NP + N1, (long)NP, P + (long)N1 * NP + N1, (long)NP);
-        CKL();
-        if (h->diag_kernel == 4)
-            gpk_potrf_diag_dmma_kernel<<<1, 256, DIAG4_SMEM, h->stream>>>(K, NP, b, P, Q, NP, ptr<int>(h->status),
-                                                                          ptr<double>(h->logdet_part), nullptr);
-        else
-            gpk_potrf_diag_blocked_kernel<<<1, 256, DIAG3_SMEM, h->stream>>>(K, NP, b, P, Q, NP, ptr<int>(h->status),
-                                                                             ptr<double>(h->logdet_part), nullptr);
-        CKL();
-        gpk_diag_qfill_kernel<<<1, 256, 0, h->stream>>>(P + (long)N1 * NP + N1, Q + (long)N1 * NP + N1, (long)NP,
-                                                         ptr<int>(h->status));
-    } else if (h->diag_kernel == 2) {
-        gpk_potrf_diag_fused_kernel<<<1, 256, DIAG2_SMEM, h->stream>>>(K, NP, b, P, Q, NP, ptr<int>(h->status),
-                                                                       ptr<double>(h->logdet_part));
-    } else {
-        gpk_potrf_diag_kernel<<<1, 256, DIAG_SMEM, h->stream>>>(K, NP, b, P, Q, NP, ptr<int>(h->status),
-                                                                ptr<double>(h->logdet_part));
-    }
+    gpk_diag_prezero_kernel<<<1, 256, 0, h->stream>>>(K + (long)N1 * NP + N1, (long)NP, P + (long)N1 * NP + N1, (long)NP);
+    CKL();
+    gpk_potrf_diag_dmma_kernel<<<1, 256, DIAG_SMEM, h->stream>>>(K, NP, b, P, Q, NP, ptr<int>(h->status),
+                                                                 ptr<double>(h->logdet_part), nullptr);
+    CKL();
+    gpk_diag_qfill_kernel<<<1, 256, 0, h->stream>>>(P + (long)N1 * NP + N1, Q + (long)N1 * NP + N1, (long)NP,
+                                                     ptr<int>(h->status));
     CKL();
     // T = L_row P11 -> P[b, 0:N1], T^T -> Q[0:N1, b]   (split-K like L_row; the Gram partials in W(s, b) are consumed)
     memset(&a, 0, sizeof(a));

@@ -1,14 +1,14 @@
-// gpk_chain.cuh — fused chain step of the blocked Cholesky (option "fusechain" = 1).
+// gpk_chain.cuh — step X(k) of the split Cholesky chain (option "chainsplit" = 1, see gpk_fit_begin).
 //
-// Step k of the factorisation puts three dependent launches on the critical chain: diag(k), the panel solve
-// L_ik = A_ik inv(L_kk)^T and the update of block column k+1 with that panel (what diag(k+1) and the next panel solve
-// need).  The two GEMM launches contract over K = 128 only: ~11 us each of which 4 us is arithmetic, plus a dependent
-// launch gap.  Here ONE launch does both: CTA b solves its 32-row tile of the panel, publishes it (store, __threadfence,
-// the four tiles of block row k+1 bump a counter), waits until those four have arrived and then applies
+// diag(k+1) needs only A[k+1,k+1] -= L[k+1,k] L[k+1,k]^T with L[k+1,k] = A[k+1,k] inv(L_kk)^T.  As two GEMM launches
+// the panel solve and this update contract over K = 128 only: ~11 us each of which 4 us is arithmetic, plus a dependent
+// launch gap.  Here ONE launch of four CTAs does both for the four 32-row tiles of block row k+1: CTA b solves its tile
+// of the panel, publishes it (store, __threadfence, bump a counter), waits until all four tiles have arrived and then
+// applies
 //   A[rows, k+1] -= L[rows, k] L[k+1, k]^T
-// to its own rows of block column k+1.  CTAs are dispatched in order and the four producers never wait on a later
-// CTA, so the spin cannot deadlock even when the grid exceeds the number of SMs.  All operands of both passes come in
-// through cp.async (generic proxy, L2): the second pass reads what other CTAs of the same launch stored moments ago.
+// to its own rows of block column k+1.  Each CTA needs one SM and waits only for the other three, which get SMs as
+// other work drains, so the spin cannot deadlock.  All operands of both passes come in through cp.async (generic proxy,
+// L2): the second pass reads what other CTAs of the same launch stored moments ago.
 #pragma once
 #include "gpk_gemm.cuh"
 
@@ -22,8 +22,8 @@ constexpr int CH_SMEM = CH_STAGES * CH_STAGE_BYTES + 256;          // 205056
 struct ChainArgs {
     double* K; long ld;              // factor buffer (in place)
     const double* P; long ldp;       // inverse diagonal blocks
-    const GemmJob* solve_jobs;       // 32-row panel-solve jobs of step k
-    const GemmJob* update_jobs;      // 32-row next-panel-update jobs of step k (same order); NULL at the last step
+    const GemmJob* solve_jobs;       // 32-row panel-solve jobs of block row k+1, one per CTA
+    const GemmJob* update_jobs;      // 32-row update jobs of tile (k+1, k+1), same order
     int* counter;                    // arrivals of the four tiles of block row k+1 (zeroed before the factorisation)
     const int* status;
 };
@@ -116,13 +116,12 @@ gpk_chain_step_kernel(const ChainArgs g)
 
     // pass 1: L[rows, k] = A[rows, k] inv(L_kk)^T   (in place: the whole tile is staged before anything is stored)
     chain_tile(smem, g.K, g.ld, g.P, g.ldp, g.K, g.ld, g.solve_jobs[blockIdx.x], 1.0, 0, tid);
-    if (g.update_jobs == nullptr) return;
 
     // publish; the four tiles of block row k+1 are the B operand of everybody's pass 2
     __threadfence();
     __syncthreads();
     if (tid == 0) {
-        if (blockIdx.x < 4) atomicAdd(g.counter, 1);
+        atomicAdd(g.counter, 1);
         while (atomicAdd(g.counter, 0) < 4) __nanosleep(64);
         __threadfence();
     }

@@ -1,10 +1,13 @@
-// Blocked diagonal-block kernels (option diag = 3: DFMA register tiles, this part of the file; diag = 4, the default:
-// DMMA fragments, second part; same contract as gpk_potrf_diag_fused_kernel):
+// gpk_diag16.cuh — diagonal block of the blocked Cholesky (gpk_potrf_diag_dmma_kernel):
 //   L_kk = chol(A_kk) and inv(L_kk) of one 128 x 128 diagonal block, one CTA of 256 threads.
+// It writes L_kk (lower) back to K, the rows of inv(L_kk) up to their diagonal 16-block to P, sum log diag(L_kk) to
+// logdet_part[kb], and flags a non-positive pivot in *status (1 + global pivot index), which is what
+// scipy.linalg.cholesky reports as LinAlgError.  The zeros right of the 16 x 16 sub-blocks and Q = P^T are written off
+// the critical chain by gpk_diag_prezero_kernel and gpk_diag_qfill_kernel.
 //
-// The column-by-column kernel pays one block-wide barrier per pivot (128 intervals of ~950 cycles; 3/4 of its
-// issued instructions are not arithmetic).  Here the block is processed in 8 panels of 16 columns with two
-// barriers per panel:
+// A column-by-column kernel pays one block-wide barrier per pivot (128 intervals of ~950 cycles; 3/4 of its issued
+// instructions are not arithmetic).  Here the block is processed in 8 panels of 16 columns with two barriers per
+// panel:
 //   S  "factor + solve": warp 0 eliminates the published 16 x 16 diagonal sub-block in registers (lane & 15 = row)
 //      in square-root-free form (L' D L'^T): the serial chain per pivot is mul -> fma -> reciprocal, the raw column goes
 //      through a warp-private shared vector before its pivot's reciprocal is known, and the 16 rsqrt that give the factor
@@ -15,21 +18,19 @@
 //      always 128 vectors -- then scale by D^-1/2.  (Alternatives with more cycles per panel: all 8 warps
 //      factorising redundantly with the substitutions in the same loop, DP-issue bound; one warp carrying the sqrt
 //      chain AND 32 substitutions.)
-//   U  "update + publish": rank-16 update of the 8 x 8 cyclic register tiles of the trailing matrix and of the
-//      inverse's residual (kept in shared memory, staged through registers for the panel's k loop), operands read
-//      with conflict-free / broadcast 64-bit shared loads; then the next panel's sub-block and rows are published.
-// The arithmetic order per element (pivots subtracted in increasing order) is the one of the column-by-column
-// kernel, so the factors agree to rounding.  The panel loop is rolled and only U is specialised per panel (static
-// register indices): the kernel runs once per launch on one SM, i.e. out of a cold instruction cache, and a first
-// fully unrolled version (38k instructions) was fetch-bound and slower than the kernel it replaces.
+//   U  "update + publish": rank-16 update of the trailing matrix and of the inverse's residual (kept in shared
+//      memory) on the fp64 tensor pipe (see gpk_potrf_diag_dmma_kernel); then the next panel's sub-block and rows
+//      are published.
+// Every element receives the pivots in increasing order, as in the column-by-column algorithm, so the factor agrees
+// with an unblocked Cholesky to rounding.  The panel loop is rolled: the kernel runs once per launch on one SM, i.e.
+// out of a cold instruction cache, and a fully unrolled blocked kernel (38k instructions) was fetch-bound.
 #pragma once
 
 constexpr int D3PS = 17;      // row stride (doubles) of the panel staging array: odd -> thread-per-row and
                               // 16-rows-per-half-warp 64-bit loads are bank-conflict-free
-template <int XS_>
-struct __align__(16) D3SmemT {
-    static constexpr int XS = XS_;    // row stride of the inverse's residual
-    double xs[128 * XS_];         // Xtilde / finished rows of inv(L_kk), row-major
+struct __align__(16) DiagSmem {
+    static constexpr int XS = 129;    // row stride of the inverse's residual: odd -> conflict-free B fragments out of it
+    double xs[128 * XS];          // Xtilde / finished rows of inv(L_kk), row-major
     double pan[2][128 * D3PS];    // pan[i][k]: column 16 kb + k of the current panel, row i (raw, then solved)
     double din[2][16 * 17];       // the 16 x 16 diagonal sub-block as published
     double colp[16][16];          // colp[j][c] = L'_D[c][j]: column j as published by the factorising warp
@@ -37,11 +38,7 @@ struct __align__(16) D3SmemT {
     double ub[2][16];             // raw column of the sub-block about to be eliminated (factorising warp only)
     double ldd[2][16 * 17];       // the factorised sub-block (lower) by panel parity, for the coalesced store
 };
-using D3Smem = D3SmemT<130>;      // register-tile (DFMA) kernel
-using D4Smem = D3SmemT<129>;      // DMMA kernel: odd stride -> conflict-free B fragments out of the residual
-constexpr int D3XS = D3Smem::XS;
-constexpr int DIAG3_SMEM = (int)sizeof(D3Smem);
-constexpr int DIAG4_SMEM = (int)sizeof(D4Smem);
+constexpr int DIAG_SMEM = (int)sizeof(DiagSmem);
 
 __device__ __forceinline__ double d3_shfl(double v, int src) { return __shfl_sync(0xffffffffu, v, src); }
 
@@ -71,69 +68,13 @@ __device__ __forceinline__ double d3_rcp(double p)
 __device__ __forceinline__ void d3_bar_arrive(int id) { asm volatile("bar.arrive %0, 160;" :: "r"(id) : "memory"); }
 __device__ __forceinline__ void d3_bar_sync(int id) { asm volatile("bar.sync %0, 160;" :: "r"(id) : "memory"); }
 
-__device__ __forceinline__ void d3_store16(double* __restrict__ dst, const double (&v)[16])
-{
-#pragma unroll
-    for (int q = 0; q < 8; ++q) *reinterpret_cast<double2*>(dst + 2 * q) = make_double2(v[2 * q], v[2 * q + 1]);
-}
-
-// ---- publish the raw sub-block and the panel below it (register indices are static)
-template <int KB>
-__device__ __forceinline__ void d3_publish(const double (&A)[8][8], D3Smem& sm, int ty, int tx)
-{
-    constexpr int PB = KB & 1;
-    sm.din[PB][ty * 17 + tx] = A[KB][KB];
-#pragma unroll
-    for (int a = KB + 1; a < 8; ++a) sm.pan[PB][(ty + 16 * a) * D3PS + tx] = A[a][KB];
-}
-
-// ---- U: rank-16 updates after panel KB, then publish panel KB + 1
-template <int KB>
-__device__ __forceinline__ void d3_update(double (&A)[8][8], D3Smem& sm, int ty, int tx)
-{
-    constexpr int PB = KB & 1;
-    const double* pr = sm.pan[PB] + ty * D3PS;
-    const double* pc = sm.pan[PB] + tx * D3PS;
-    const double* xrow = sm.xs + (16 * KB) * D3XS + tx;
-    double* xown = sm.xs + ty * D3XS + tx;
-    double xa[8][8];
-#pragma unroll
-    for (int a = KB + 1; a < 8; ++a)
-#pragma unroll
-        for (int b = 0; b <= KB; ++b) xa[a][b] = xown[16 * a * D3XS + 16 * b];
-#pragma unroll 2
-    for (int k = 0; k < 16; ++k) {
-        double lr[8], lc[8], xc[8];
-#pragma unroll
-        for (int a = KB + 1; a < 8; ++a) lr[a] = pr[16 * a * D3PS + k];
-#pragma unroll
-        for (int b = KB + 1; b < 8; ++b) lc[b] = pc[16 * b * D3PS + k];
-#pragma unroll
-        for (int b = 0; b <= KB; ++b) xc[b] = xrow[k * D3XS + 16 * b];
-#pragma unroll
-        for (int b = KB + 1; b < 8; ++b)
-#pragma unroll
-            for (int a = b; a < 8; ++a) A[a][b] = fma(-lr[a], lc[b], A[a][b]);
-#pragma unroll
-        for (int b = 0; b <= KB; ++b)
-#pragma unroll
-            for (int a = KB + 1; a < 8; ++a) xa[a][b] = fma(-lr[a], xc[b], xa[a][b]);
-    }
-#pragma unroll
-    for (int a = KB + 1; a < 8; ++a)
-#pragma unroll
-        for (int b = 0; b <= KB; ++b) xown[16 * a * D3XS + 16 * b] = xa[a][b];
-    d3_publish<KB + 1>(A, sm, ty, tx);
-}
-
 // ---- coalesced 128-bit stores of what panel kp finished: the factorised sub-block, the solved panel rows below it
 // (final L values) and the row block of the inverse up to its diagonal (what lies right of it is zeroed off the
-// chain by gpk_diag_prezero_kernel).  Executed by threads t = 0..nth-1.  Measured: issued at the start of U by all
-// threads they cost the issuing warps ~1.4k cycles per panel; issued by the three warps that idle during phase S of
-// the NEXT panel the DMMA kernel went from 69.2k to 64.3k cycles per block (a run with the stores disabled takes the
-// same time: they are hidden), while the DFMA kernel got slower (70.8k -> 77.8k) and keeps them at the start of U.
-template <class SM>
-__device__ __forceinline__ void d3_store_panel(const SM& sm, const int kp, const int t, const int nth,
+// chain by gpk_diag_prezero_kernel).  Executed by threads t = 0..nth-1.  Measured on a B200: issued at the start of U
+// by all threads they cost the issuing warps ~1.4k cycles per panel; issued by the three warps that idle during phase
+// S of the NEXT panel the kernel went from 69.2k to 64.3k cycles per block (a run with the stores disabled takes the
+// same time: they are hidden).
+__device__ __forceinline__ void d3_store_panel(const DiagSmem& sm, const int kp, const int t, const int nth,
                                                double* __restrict__ Kt, const long ld, double* __restrict__ Pt, const long ldp)
 {
     const double* pan = sm.pan[kp & 1];
@@ -152,15 +93,14 @@ __device__ __forceinline__ void d3_store_panel(const SM& sm, const int kp, const
     const int npair = 8 * (kp + 1);                               // inverse rows 16 kp .. +15, columns 0 .. 16 (kp + 1)
     for (int it = t; it < 16 * npair; it += nth) {
         const int r16 = it / npair, c = (it - r16 * npair) * 2;
-        const double* xr = sm.xs + (16 * kp + r16) * SM::XS;
+        const double* xr = sm.xs + (16 * kp + r16) * DiagSmem::XS;
         *reinterpret_cast<double2*>(Pt + (long)(16 * kp + r16) * ldp + c) = make_double2(xr[c], xr[c + 1]);
     }
 }
 
 // ---- S: warp 0 factorises the published 16 x 16 sub-block, warps 1..4 run the 128 forward substitutions of panel
-// kbp (shared by the DFMA and the DMMA kernel)
-template <class SM>
-__device__ __forceinline__ void d3_phase_s(SM& sm, const int kbp, const int kb, const int tid, int* s_bad, double& lsum,
+// kbp
+__device__ __forceinline__ void d3_phase_s(DiagSmem& sm, const int kbp, const int kb, const int tid, int* s_bad, double& lsum,
                                            long long* __restrict__ prof, const bool fine)
 {
     const int lane = tid & 31, r = lane & 15;
@@ -241,8 +181,8 @@ __device__ __forceinline__ void d3_phase_s(SM& sm, const int kbp, const int kb, 
         // -- one forward substitution per thread against the unit-lower factor, column by column as published
         double v[16];
         {
-            const double* src = is_pan ? pan + irow * D3PS : sm.xs + (16 * kbp) * SM::XS + ccol;
-            const int step = is_pan ? 1 : SM::XS;
+            const double* src = is_pan ? pan + irow * D3PS : sm.xs + (16 * kbp) * DiagSmem::XS + ccol;
+            const int step = is_pan ? 1 : DiagSmem::XS;
 #pragma unroll
             for (int k = 0; k < 16; ++k) v[k] = src[k * step];
         }
@@ -268,99 +208,26 @@ __device__ __forceinline__ void d3_phase_s(SM& sm, const int kbp, const int kb, 
             for (int k = 0; k < 16; ++k) pan[irow * D3PS + k] = v[k];
         } else {                                      // finished column of the inverse's row block
 #pragma unroll
-            for (int k = 0; k < 16; ++k) sm.xs[(16 * kbp + k) * SM::XS + ccol] = v[k];
+            for (int k = 0; k < 16; ++k) sm.xs[(16 * kbp + k) * DiagSmem::XS + ccol] = v[k];
         }
     }
-}
-
-#define D3_CASES7(F, ...) switch (kbp) { case 0: F<0>(__VA_ARGS__); break; case 1: F<1>(__VA_ARGS__); break; \
-    case 2: F<2>(__VA_ARGS__); break; case 3: F<3>(__VA_ARGS__); break; case 4: F<4>(__VA_ARGS__); break; \
-    case 5: F<5>(__VA_ARGS__); break; default: F<6>(__VA_ARGS__); break; }
-
-__global__ void __launch_bounds__(256, 1)
-gpk_potrf_diag_blocked_kernel(double* __restrict__ K, long ld, int kb,
-                              double* __restrict__ P, double* __restrict__ Q, long ldp,
-                              int* __restrict__ status, double* __restrict__ logdet_part,
-                              long long* __restrict__ prof)
-{
-    extern __shared__ __align__(16) unsigned char d3_raw[];
-    D3Smem& sm = *reinterpret_cast<D3Smem*>(d3_raw);
-    __shared__ int s_bad;
-
-    const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
-    cudaGridDependencySynchronize();      // programmatic dependent launch (see gpk_gemm_nt_kernel)
-    if (*status != 0) return;
-    if (tid == 0) s_bad = 0;
-    const bool stamp = prof != nullptr && tid == 159;      // last substitution thread
-    const bool nostore = prof != nullptr && prof[63] != 0;  // timing experiment: results are not written
-    if (stamp) prof[0] = clock64();
-
-    double* Kt = K + (long)kb * 128 * ld + (long)kb * 128;
-    double* Pt = P + (long)kb * 128 * ldp + (long)kb * 128;
-    double A[8][8];
-#pragma unroll
-    for (int a = 0; a < 8; ++a)
-#pragma unroll
-        for (int b = 0; b < 8; ++b) {
-            const int i = ty + 16 * a, c = tx + 16 * b;
-            A[a][b] = (b <= a && c <= i) ? Kt[(long)i * ld + c] : 0.0;
-        }
-    for (int e = tid; e < 128 * D3XS; e += 256) {          // Xtilde = I
-        const int i = e / D3XS, c = e - i * D3XS;
-        sm.xs[e] = (i == c) ? 1.0 : 0.0;
-    }
-    d3_publish<0>(A, sm, ty, tx);
-    double lsum = 0.0;
-    __syncthreads();
-    if (stamp) prof[1] = clock64();
-
-#pragma unroll 1
-    for (int kbp = 0; kbp < 8; ++kbp) {   // panel loop rolled: phase S exists once in the binary
-        const bool fine = stamp && kbp == 3;
-        d3_phase_s(sm, kbp, kb, tid, &s_bad, lsum, prof, fine);
-        if (fine) prof[39] = clock64();
-        __syncthreads();
-        if (stamp) prof[2 + 2 * kbp] = clock64();
-        // ---- U: coalesced stores of what panel kbp finished (all threads; letting the idle warps of phase S issue them
-        // as the DMMA kernel does made THIS kernel slower: 77.8k vs 70.8k cycles), rank-16 updates, publish the next
-        // panel.  (The zeros right of the sub-block and Q = P^T are written off the critical chain.)
-        if (!nostore) d3_store_panel(sm, kbp, tid, 256, Kt, ld, Pt, ldp);
-        if (kbp == 7) break;
-        if (fine) prof[40] = clock64();
-        D3_CASES7(d3_update, A, sm, ty, tx)
-        if (fine) prof[41] = clock64();
-        __syncthreads();
-        if (stamp) prof[3 + 2 * kbp] = clock64();
-    }
-
-    if (tid < 32) {                       // log-det partial: sum over the 16 rows of the 8 panels
-        double s = (tid < 16) ? lsum : 0.0;
-#pragma unroll
-        for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
-        if (tid == 0) {
-            logdet_part[kb] = s;
-            if (s_bad != 0) atomicCAS(status, 0, s_bad);
-        }
-    }
-    if (stamp) prof[33] = clock64();
 }
 
 // ---------------------------------------------------------------------------------------
-// DMMA variant (option diag = 4): same S phase, but the rank-16 updates of phase U run on the fp64 tensor pipe.
-// The DFMA kernel's 8 x 8 cyclic register tiles need one 64-bit shared load per 2.3 FMAs, and LDS.64 occupies the
-// LSU for 2 cycles per warp whatever the broadcast degree: its U phase is LSU-bound at ~2.4x the DP-pipe time.
-// Here the trailing matrix lives in m8n8k4 accumulator fragments: the block is cut into 16 x 16 "tiles" of 8 rows x
+// Phase U on the fp64 tensor pipe.  With DFMA on 8 x 8 cyclic register tiles the rank-16 update needs one 64-bit
+// shared load per 2.3 FMAs, and LDS.64 occupies the LSU for 2 cycles per warp whatever the broadcast degree: such a
+// U phase is LSU-bound at ~2.4x the DP-pipe time.  Here the trailing matrix lives in m8n8k4 accumulator fragments: the block is cut into 16 x 16 "tiles" of 8 rows x
 // 8 columns, tile t = rows 16 (t/2) + 2 (t%2) + {0,4,8,12,1,5,9,13} (the interleave makes the 34-word row stride of
 // the panel array bank-conflict-free for fragment loads AND for the thread-per-row substitutions of phase S);
 // warp w owns tile rows w and 15 - w (18 tiles, all tiles (I, J) with J/2 <= I/2, so that the A fragment of a tile row is
 // loaded once per k-chunk and reused along the row).  Per panel and warp: <= 8 + 72 fragment loads for <= 72 DMMA
-// (the DFMA kernel: 190 loads), and the inverse's residual is updated in shared memory through the same fragments.
+// (DFMA register tiles: 190 loads), and the inverse's residual is updated in shared memory through the same fragments.
 // ---------------------------------------------------------------------------------------
 __device__ __forceinline__ int d4_row(int t, int idx) { return 16 * (t >> 1) + 2 * (t & 1) + 4 * (idx & 3) + (idx >> 2); }
 
 // write the elements of the tiles in tile columns 2 kp, 2 kp + 1 (the next panel) to din / pan
 template <int NS>
-__device__ __forceinline__ void d4_publish_row(const double (&c)[NS][2], const int I, const int kp, D4Smem& sm, const int g,
+__device__ __forceinline__ void d4_publish_row(const double (&c)[NS][2], const int I, const int kp, DiagSmem& sm, const int g,
                                                const int q)
 {
     if ((I >> 1) < kp) return;
@@ -381,7 +248,7 @@ __device__ __forceinline__ void d4_publish_row(const double (&c)[NS][2], const i
 
 // rank-16 update of one owned tile row: trailing-matrix tiles (registers) and the inverse's residual (shared memory)
 template <int NS>
-__device__ __forceinline__ void d4_update_row(double (&c)[NS][2], const int I, const int kbp, D4Smem& sm, const int g,
+__device__ __forceinline__ void d4_update_row(double (&c)[NS][2], const int I, const int kbp, DiagSmem& sm, const int g,
                                               const int q)
 {
     const int c0 = 2 * (kbp + 1);                    // first tile row / column behind the panel
@@ -408,8 +275,8 @@ __device__ __forceinline__ void d4_update_row(double (&c)[NS][2], const int I, c
         }
     }
     // Xtilde[I-rows, 0 : 16 (kbp+1)) -= L_panel[I-rows, :] X[panel rows, :]
-    double* xrow = sm.xs + row * D4Smem::XS;
-    const double* xb = sm.xs + (16 * kbp + q) * D4Smem::XS;
+    double* xrow = sm.xs + row * DiagSmem::XS;
+    const double* xb = sm.xs + (16 * kbp + q) * DiagSmem::XS;
 #pragma unroll 1
     for (int Jc = 0; Jc < c0; Jc += 2) {                 // c0 is even: two tiles (independent chains) per iteration
         int col[2][2], colb[2];
@@ -422,7 +289,7 @@ __device__ __forceinline__ void d4_update_row(double (&c)[NS][2], const int I, c
             x[t][0] = xrow[col[t][0]];
             x[t][1] = xrow[col[t][1]];
 #pragma unroll
-            for (int ch = 0; ch < 4; ++ch) bx[t][ch] = xb[4 * ch * D4Smem::XS + colb[t]];
+            for (int ch = 0; ch < 4; ++ch) bx[t][ch] = xb[4 * ch * DiagSmem::XS + colb[t]];
         }
 #pragma unroll
         for (int ch = 0; ch < 4; ++ch) {
@@ -444,8 +311,8 @@ gpk_potrf_diag_dmma_kernel(double* __restrict__ K, long ld, int kb,
                            long long* __restrict__ prof)
 {
     extern __shared__ __align__(16) unsigned char d3_raw[];
-    D4Smem& sm = *reinterpret_cast<D4Smem*>(d3_raw);
-    constexpr int XS = D4Smem::XS;
+    DiagSmem& sm = *reinterpret_cast<DiagSmem*>(d3_raw);
+    constexpr int XS = DiagSmem::XS;
     __shared__ int s_bad;
 
     const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
@@ -524,7 +391,7 @@ gpk_potrf_diag_dmma_kernel(double* __restrict__ K, long ld, int kb,
 
 // Off-chain helpers of the blocked kernel: zero what lies right of the 16 x 16 sub-blocks in every diagonal tile of
 // K (the covariance builder leaves the symmetric values there; later GEMMs read the tile as a lower-triangular
-// operand), likewise in P (the kernels store the inverse's rows only up to their diagonal 16-block); Q's diagonal tiles =
+// operand), likewise in P (the kernel stores the inverse's rows only up to their diagonal 16-block); Q's diagonal tiles =
 // transposed diagonal tiles of P.  One CTA per diagonal tile.
 __global__ void __launch_bounds__(256) gpk_diag_prezero_kernel(double* __restrict__ K, long ld, double* __restrict__ P,
                                                                long ldp)

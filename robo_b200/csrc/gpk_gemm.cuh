@@ -152,7 +152,7 @@ gpk_gemm_nt_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
     // start while the producing kernel drains; nothing is read before the dependency is resolved.
     cudaGridDependencySynchronize();
     if (g.status != nullptr && *g.status != 0) return;
-    static_assert(MI == 8 || MI == 4 || MI == 2 || MI == 1, "tile height 128, 64, 32 or 16");
+    static_assert(MI == 8 || MI == 2, "tile height 128 or 32");
     static_assert(EPI == EPI_STORE || MI == 8, "column-reduce epilogue uses full tiles");
     constexpr int TM = 16 * MI;                                          // tile rows (A rows)
     constexpr int NS = gemm_nstage(MI);                                  // ring depth
@@ -167,7 +167,7 @@ gpk_gemm_nt_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
     constexpr int RING_MIN = NS * STAGE_BYTES;
     constexpr int CT_NEED = ((TM * CT_STRIDE * 8 + 1023) / 1024) * 1024;
     constexpr int RING = MI == 8 ? (LOADER == LOADER_TMA ? RING_TMA : RING_PAD)
-                                 : RING_MIN;                            // (32/64-row tiles: CT tile fits the ring)
+                                 : RING_MIN;                            // (32-row tiles: CT tile fits the ring)
     static_assert(RING >= CT_NEED, "epilogue staging tile must fit the operand ring");
     const uint32_t full_bar = smem + RING;                              // NSTAGE x 8 bytes
     const uint32_t red = smem + RING + 64;                              // 2 x 128 doubles

@@ -215,308 +215,6 @@ __global__ void gpk_kfix_kernel(double* __restrict__ K, long ld, int n, int NP, 
 }
 
 // ---------------------------------------------------------------------------------------
-// Diagonal block: L_kk = chol(A_kk) in shared memory, then inv(L_kk) in place.
-//   writes L_kk (lower, upper zeroed) back to K,
-//   inv(L_kk) to the diagonal block of P (lower) and its transpose to Q (upper),
-//   sum log diag(L_kk) to logdet_part[kb], and flags a non-positive pivot in *status
-//   (1 + global pivot index), which is what scipy.linalg.cholesky reports as LinAlgError.
-// One CTA, 256 threads, dynamic smem 128 x 129 doubles + 3 x 128.
-// ---------------------------------------------------------------------------------------
-constexpr int DIAG_SMEM = (128 * 129 + 2 * 128) * 8;
-
-__global__ void __launch_bounds__(256)
-gpk_potrf_diag_kernel(double* __restrict__ K, long ld, int kb,
-                      double* __restrict__ P, double* __restrict__ Q, long ldp,
-                      int* __restrict__ status, double* __restrict__ logdet_part)
-{
-    extern __shared__ double dsm[];
-    double (*A)[129] = (double (*)[129])dsm;
-    double* dsq = dsm + 128 * 129;       // sqrt of pivots
-    double* vbuf = dsq + 128;
-    __shared__ double pb2[256];
-    __shared__ int s_bad;
-
-    const int tid = threadIdx.x;
-    if (*status != 0) return;
-    if (tid == 0) s_bad = 0;
-
-    double* Kt = K + (long)kb * 128 * ld + (long)kb * 128;
-    for (int e = tid; e < 128 * 128; e += 256) {
-        int r = e >> 7, c = e & 127;
-        A[r][c] = Kt[(long)r * ld + c];
-    }
-    __syncthreads();
-
-    const int i = tid & 127, h = tid >> 7;
-    // ---- elimination: after step j, column j holds the un-scaled column, A[j][j] = pivot d_j
-    for (int j = 0; j < 128; ++j) {
-        double d = A[j][j];
-        if (!(d > 0.0) || isinf(d)) {
-            if (tid == 0 && s_bad == 0) s_bad = kb * 128 + j + 1;
-            d = 1.0;
-        }
-        const double invd = 1.0 / d;
-        if (i > j) {
-            const double lij = A[i][j] * invd;
-            for (int c = j + 1 + h; c <= i; c += 2) A[i][c] -= lij * A[c][j];
-        }
-        __syncthreads();
-    }
-    if (tid < 128) {
-        double d = A[tid][tid];
-        if (!(d > 0.0) || isinf(d)) d = 1.0;
-        dsq[tid] = sqrt(d);
-    }
-    __syncthreads();
-    // ---- finalise L and write it back
-    for (int e = tid; e < 128 * 128; e += 256) {
-        int r = e >> 7, c = e & 127;
-        double v = 0.0;
-        if (c < r) { v = A[r][c] / dsq[c]; }
-        else if (c == r) v = dsq[c];
-        Kt[(long)r * ld + c] = v;
-    }
-    __syncthreads();
-    for (int e = tid; e < 128 * 128; e += 256) {
-        int r = e >> 7, c = e & 127;
-        if (c < r) A[r][c] = A[r][c] / dsq[c];
-    }
-    if (tid < 32) {
-        double s = 0.0;
-        for (int q = tid; q < 128; q += 32) s += log(dsq[q]);
-#pragma unroll
-        for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
-        if (tid == 0) logdet_part[kb] = s;
-    }
-    __syncthreads();
-    if (tid == 0 && s_bad != 0) atomicCAS(status, 0, s_bad);
-
-    // ---- in-place inverse of the lower-triangular block, right to left (LAPACK dtrti2 order)
-    for (int j = 127; j >= 0; --j) {
-        const double ajj = 1.0 / dsq[j];
-        if (tid < 128 && tid > j) vbuf[tid] = A[tid][j];
-        __syncthreads();
-        double part = 0.0;
-        if (i > j) {
-            for (int c = j + 1 + h; c <= i; c += 2) part = fma(A[i][c], vbuf[c], part);
-        }
-        pb2[tid] = part;
-        __syncthreads();
-        if (h == 0 && i > j) A[i][j] = -(pb2[i] + pb2[128 + i]) * ajj;
-        if (tid == 0) A[j][j] = ajj;
-    }
-    __syncthreads();
-    double* Pt = P + (long)kb * 128 * ldp + (long)kb * 128;
-    double* Qt = Q + (long)kb * 128 * ldp + (long)kb * 128;
-    for (int e = tid; e < 128 * 128; e += 256) {
-        int r = e >> 7, c = e & 127;
-        Pt[(long)r * ldp + c] = (c <= r) ? A[r][c] : 0.0;
-        Qt[(long)r * ldp + c] = (c >= r) ? A[c][r] : 0.0;
-    }
-}
-
-constexpr int DIAG2_SMEM = (128 * 129 + 5 * 128) * 8;
-
-// ---------------------------------------------------------------------------------------
-// Diagonal block, register-tiled fused version (default; same contract as gpk_potrf_diag_kernel).
-// Thread (ty, tx) = (tid / 16, tid % 16) keeps the 8 x 8 cyclic sub-tile A[ty + 16a][tx + 16b] in registers; per
-// column j the 16 owner threads publish the column through a double-buffered shared vector, everyone
-// scales it by rsqrt(pivot) and applies the rank-1 update to its registers.  The forward substitution L X = I runs one column behind the
-// factorisation inside the SAME barrier interval (row j-1 of X and column j of A are published
-// before the one __syncthreads of step j), so the block costs 128 barrier intervals instead of 256.
-// L columns reach the substitution through registers (the scaled column every thread already
-// computed for the rank-1 update), not through shared memory.
-// ---------------------------------------------------------------------------------------
-template <int JBP>
-__device__ __forceinline__ void diag_x_publish(double (&X)[8][8], double* rb, double rs_prev, int ty, int tx, int jjp)
-{
-    if (ty == jjp) {              // owners of row jm = 16*JBP + jjp finish it: X[jm][c] *= 1/L[jm][jm]
-#pragma unroll
-        for (int b = 0; b <= JBP; ++b) {
-            const double x = X[JBP][b] * rs_prev;
-            X[JBP][b] = x;
-            rb[tx + 16 * b] = x;
-        }
-    }
-}
-
-template <int JBP>
-__device__ __forceinline__ void diag_x_update(double (&X)[8][8], const double (&lr)[8], const double* rb,
-                                              int ty, int tx, int jjp)
-{
-    // X[i][c] -= L[i][jm] X[jm][c] for the rows below jm = 16 JBP + jjp.  No per-element predicates: the rows of
-    // block JBP that are not below jm get a zero multiplier (one select), columns right of jm hold zeros in rb.
-    double xr[8], lx[8];
-    const double* rbc = rb + tx;
-#pragma unroll
-    for (int b = 0; b <= JBP; ++b) xr[b] = rbc[16 * b];
-#pragma unroll
-    for (int a = JBP; a < 8; ++a) lx[a] = lr[a];
-    lx[JBP] = (ty > jjp) ? lr[JBP] : 0.0;
-#pragma unroll
-    for (int a = JBP; a < 8; ++a)
-#pragma unroll
-        for (int b = 0; b <= JBP; ++b) X[a][b] = fma(-lx[a], xr[b], X[a][b]);
-}
-
-template <int JB>
-__device__ __forceinline__ void diag_fused_block(double (&A)[8][8], double (&X)[8][8], double (&lr)[8], double& rs_prev,
-                                                 double& rs_cur, double* colbuf, double* rowbuf, double* dnext,
-                                                 int ty, int tx, int tid, int kb, int* s_bad)
-{
-    // Invariants.  lr[] enters holding the scaled column j-1 of L (this thread's rows) and leaves holding column j.
-    // rs_cur = rsqrt(pivot j) was computed during the previous step from the published diagonal element.
-    // Entries above the diagonal inside the diagonal blocks (row < column) are never read by valid entries and
-    // are left to hold garbage (this removes the per-element predicates; the final store masks them).
-    for (int jj = 0; jj < 16; ++jj) {
-        const int j = JB * 16 + jj;
-        double* cb = colbuf + (j & 1) * 128;
-        double* rb = rowbuf + ((j + 1) & 1) * 128;       // parity of jm = j - 1
-        if (tx == jj) {
-            double* cbw = cb + ty;
-#pragma unroll
-            for (int a = JB; a < 8; ++a) cbw[16 * a] = A[a][JB];
-        }
-        if (jj < 15) {
-            if (ty == jj + 1 && tx == jj + 1) dnext[j & 1] = A[JB][JB];
-        } else if (JB < 7) {
-            if (ty == 0 && tx == 0) dnext[j & 1] = A[JB < 7 ? JB + 1 : 7][JB < 7 ? JB + 1 : 7];
-        }
-        if (jj > 0) diag_x_publish<JB>(X, rb, rs_prev, ty, tx, jj - 1);
-        else if (JB > 0) diag_x_publish<(JB > 0 ? JB - 1 : 0)>(X, rb, rs_prev, ty, tx, 15);
-        __syncthreads();
-        double d = cb[j];
-        if (!(d > 0.0) || isinf(d)) {
-            if (tid == 0 && *s_bad == 0) *s_bad = kb * 128 + j + 1;
-            d = 1.0;
-        }
-        const double rs = rs_cur;            // == rsqrt(d)
-        const double sq = d * rs;
-        double rs_next = 1.0;
-        if (j < 127) {                       // next pivot: the same fma its owner applies below
-            const double ln = cb[j + 1] * rs;
-            const double dn = fma(-ln, ln, dnext[j & 1]);
-            rs_next = (dn > 0.0 && !isinf(dn)) ? rsqrt(dn) : 1.0;
-        }
-        // forward-substitution step for row j-1, with the previous column of L still in lr[]
-        if (jj > 0) diag_x_update<JB>(X, lr, rb, ty, tx, jj - 1);
-        else if (JB > 0) diag_x_update<(JB > 0 ? JB - 1 : 0)>(X, lr, rb, ty, tx, 15);
-        // column j of L, scaled
-        double lc[8];
-        const double* cbr = cb + ty;
-        const double* cbc = cb + tx;
-#pragma unroll
-        for (int a = JB; a < 8; ++a) lr[a] = cbr[16 * a] * rs;
-#pragma unroll
-        for (int b = JB; b < 8; ++b) lc[b] = cbc[16 * b] * rs;
-        if (tx == jj) {                      // owners keep the finished column (rows above the diagonal: don't care)
-#pragma unroll
-            for (int a = JB + 1; a < 8; ++a) A[a][JB] = lr[a];
-            A[JB][JB] = (ty == jj) ? sq : lr[JB];
-        }
-        // rank-1 update; only the column block that contains finished columns needs a predicate
-        if (tx > jj) {
-#pragma unroll
-            for (int a = JB; a < 8; ++a) A[a][JB] = fma(-lr[a], lc[JB], A[a][JB]);
-        }
-#pragma unroll
-        for (int b = JB + 1; b < 8; ++b)
-#pragma unroll
-            for (int a = b; a < 8; ++a) A[a][b] = fma(-lr[a], lc[b], A[a][b]);
-        rs_prev = rs;
-        rs_cur = rs_next;
-    }
-}
-
-__global__ void __launch_bounds__(256, 1)
-gpk_potrf_diag_fused_kernel(double* __restrict__ K, long ld, int kb,
-                            double* __restrict__ P, double* __restrict__ Q, long ldp,
-                            int* __restrict__ status, double* __restrict__ logdet_part)
-{
-    extern __shared__ double dsm[];
-    double (*Ls)[129] = (double (*)[129])dsm;
-    double* colbuf = dsm + 128 * 129;     // 2 x 128
-    double* rowbuf = colbuf + 256;        // 2 x 128
-    double* dnext = rowbuf + 256;         // 2: diagonal element of the next pivot
-    __shared__ int s_bad;
-
-    const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
-    cudaGridDependencySynchronize();      // programmatic dependent launch (see gpk_gemm_nt_kernel)
-    if (*status != 0) return;
-    if (tid == 0) s_bad = 0;
-
-    double* Kt = K + (long)kb * 128 * ld + (long)kb * 128;
-    double A[8][8], X[8][8], lrp[8];          // lrp: the scaled column of L of the previous step
-    double rs_prev = 1.0, rs_cur = 1.0;
-#pragma unroll
-    for (int a = 0; a < 8; ++a) {
-        lrp[a] = 0.0;
-#pragma unroll
-        for (int b = 0; b < 8; ++b) {
-            const int i = ty + 16 * a, c = tx + 16 * b;
-            A[a][b] = (c <= i) ? Kt[(long)i * ld + c] : 0.0;
-            X[a][b] = (i == c) ? 1.0 : 0.0;
-        }
-    }
-    if (tid == 0) dnext[1] = A[0][0];     // first pivot (slot 1: step 0 publishes the next one into slot 0)
-    __syncthreads();
-    {
-        const double d0 = dnext[1];
-        rs_cur = (d0 > 0.0 && !isinf(d0)) ? rsqrt(d0) : 1.0;
-    }
-    diag_fused_block<0>(A, X, lrp, rs_prev, rs_cur, colbuf, rowbuf, dnext, ty, tx, tid, kb, &s_bad);
-    diag_fused_block<1>(A, X, lrp, rs_prev, rs_cur, colbuf, rowbuf, dnext, ty, tx, tid, kb, &s_bad);
-    diag_fused_block<2>(A, X, lrp, rs_prev, rs_cur, colbuf, rowbuf, dnext, ty, tx, tid, kb, &s_bad);
-    diag_fused_block<3>(A, X, lrp, rs_prev, rs_cur, colbuf, rowbuf, dnext, ty, tx, tid, kb, &s_bad);
-    diag_fused_block<4>(A, X, lrp, rs_prev, rs_cur, colbuf, rowbuf, dnext, ty, tx, tid, kb, &s_bad);
-    diag_fused_block<5>(A, X, lrp, rs_prev, rs_cur, colbuf, rowbuf, dnext, ty, tx, tid, kb, &s_bad);
-    diag_fused_block<6>(A, X, lrp, rs_prev, rs_cur, colbuf, rowbuf, dnext, ty, tx, tid, kb, &s_bad);
-    diag_fused_block<7>(A, X, lrp, rs_prev, rs_cur, colbuf, rowbuf, dnext, ty, tx, tid, kb, &s_bad);
-    // last row of X (row 127) only needs its scaling; nobody reads the broadcast copy, but slower threads may still be
-    // reading this buffer for the update of step 127 (racecheck): write the copy to the other parity buffer
-    diag_x_publish<7>(X, rowbuf + 128, rs_prev, ty, tx, 15);
-
-    // ---------------- publish L, log-det, status ----------------
-#pragma unroll
-    for (int a = 0; a < 8; ++a)
-#pragma unroll
-        for (int b = 0; b < 8; ++b) {
-            const int i = ty + 16 * a, c = tx + 16 * b;
-            const double v = (c <= i) ? A[a][b] : 0.0;
-            if (i == c) colbuf[i] = v;                     // diagonal of L for the log-det
-            Kt[(long)i * ld + c] = v;
-        }
-    __syncthreads();
-    if (tid < 32) {
-        double s = 0.0;
-        for (int q = tid; q < 128; q += 32) s += log(colbuf[q]);
-#pragma unroll
-        for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
-        if (tid == 0) {
-            logdet_part[kb] = s;
-            if (s_bad != 0) atomicCAS(status, 0, s_bad);
-        }
-    }
-    // ---------------- publish L^-1 (P lower) and its transpose (Q upper) ----------------
-    double* Pt = P + (long)kb * 128 * ldp + (long)kb * 128;
-    double* Qt = Q + (long)kb * 128 * ldp + (long)kb * 128;
-#pragma unroll
-    for (int a = 0; a < 8; ++a)
-#pragma unroll
-        for (int b = 0; b < 8; ++b) {
-            const int i = ty + 16 * a, c = tx + 16 * b;
-            const double v = (c <= i) ? X[a][b] : 0.0;
-            Ls[i][c] = v;
-            Pt[(long)i * ldp + c] = v;
-        }
-    __syncthreads();
-    for (int e = tid; e < 128 * 128; e += 256) {
-        const int r = e >> 7, c = e & 127;
-        Qt[(long)r * ldp + c] = (c >= r) ? Ls[c][r] : 0.0;
-    }
-}
-
-// ---------------------------------------------------------------------------------------
 // Scoring epilogue: sum the per-row-block partials in fixed order, finish mean / variance,
 // apply the output transform + clip (gaussian_process.py:282-294), the acquisition closed form,
 // and a per-block arg-max with numpy.argmax tie-breaking.

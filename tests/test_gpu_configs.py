@@ -27,7 +27,7 @@ def _need_gpu():
     import torch
     if not torch.cuda.is_available():
         pytest.skip("no CUDA device")
-    for k in ("GPK_LOADER", "GPK_CHUNK", "GPK_DIAG"):
+    for k in ("GPK_LOADER", "GPK_CHUNK"):
         os.environ.pop(k, None)
 
 

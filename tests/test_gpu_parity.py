@@ -120,22 +120,14 @@ def test_cholesky_forward_solve_logdet(N, D, loader):
     assert np.abs(np.triu(Linv, 1)).max() == 0.0
 
 
-def test_cholesky_variants_agree():
-    """every implementation switch (diagonal-block kernel, look-ahead, 128 / 32 / 16-row chain tiles, fused chain
-    step, split chain with look-ahead 2) yields the same factor to rounding; the round-1 covariance builder (other
-    rounding of K itself) agrees to the conditioning of the problem"""
+def test_cholesky_schedules_agree():
+    """the plain look-ahead schedule and the split chain with look-ahead 2 yield the same factor to rounding; the
+    round-1 covariance builder (other rounding of K itself) agrees to the conditioning of the problem"""
     from robo_b200 import _lib
     X, y, _, theta, noise = O.synthetic_problem(600, 5, 1, seed_train=11)
     ref = None
-    for diag, la, st, fuse, split, cov in ((3, 1, 1, 0, 0, 2), (4, 1, 1, 0, 1, 2), (3, 1, 1, 0, 1, 2), (4, 1, 1, 0, 0, 2),
-                                           (4, 1, 1, 1, 0, 2), (4, 1, 0, 0, 0, 2), (4, 1, 2, 0, 0, 2), (2, 1, 1, 0, 0, 2),
-                                           (0, 1, 1, 0, 0, 2), (3, 0, 1, 0, 0, 2), (2, 0, 1, 0, 0, 2), (3, 1, 0, 0, 0, 2),
-                                           (0, 0, 0, 0, 0, 2), (4, 1, 1, 0, 1, 1)):
+    for split, cov in ((0, 2), (1, 2), (1, 1)):
         h = _lib.Handle(0)
-        h.set_option("diag", diag)
-        h.set_option("lookahead", la)
-        h.set_option("smalltile", st)
-        h.set_option("fusechain", fuse)
         h.set_option("chainsplit", split)
         h.set_option("cov", cov)
         h.set_data(X, y)
@@ -599,8 +591,9 @@ def test_bad_arguments_raise_value_errors():
     h.fit(1e-3, 0.0)
     with pytest.raises(ValueError):
         h.set_option("chunk", 100)
-    with pytest.raises(ValueError):
-        h.set_option("nonsense", 1)
+    for key in ("nonsense", "diag", "smalltile", "fusechain", "lookahead"):
+        with pytest.raises(ValueError):
+            h.set_option(key, 1)
 
 
 def test_device_candidate_generation_and_fused_maximize():
@@ -846,8 +839,7 @@ def test_full_size_properties():
 
 
 # --------------------------------------------------------------------------- incremental refit (SURVEY 8f-4)
-@pytest.mark.parametrize("diag", [3, 4, 2])
-def test_fit_append_matches_full_refit_and_oracle(diag):
+def test_fit_append_matches_full_refit_and_oracle():
     """gpk_fit_append: rows appended inside the last 128-row block.  Against a full refit on the device (factor,
     inverse, z, log-likelihood) and against the CPU oracle (posterior moments + EI at the north_star tolerances);
     not-applicable cases leave the model untouched."""
@@ -859,7 +851,6 @@ def test_fit_append_matches_full_refit_and_oracle(diag):
 
     def full(n, d_add=da):
         hh = _lib.Handle(0)
-        hh.set_option("diag", diag)
         hh.set_data(X[:n], y[:n])
         hh.set_kernel(f["family"], f["log_amp"], f["axis"], f["group"], f["log_metric"])
         return hh, hh.fit(d_add, float(np.mean(y[:n])))
