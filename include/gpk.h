@@ -63,10 +63,11 @@ const char* gpk_last_error(gpk_handle* h);
 const char* gpk_version(void);
 /* key in
  *   "loader"    operand staging of the GEMM tile engine: 2 = TMA with a dedicated producer warp and
- *               full/empty mbarriers [default], 1 = TMA issued by a consumer thread, 0 = cp.async (cross-check)
+ *               full/empty mbarriers [default], 1 = TMA issued by a consumer thread, 0 = cp.async (cross-check).
+ *               The covariance builder follows it: TMA-staged, pre-scaled term-major operands under 1 and 2; one
+ *               broadcast load per pair and term from an axis-major operand under 0
  *   "chunk"     candidates per scoring pass (multiple of 128); 0 = automatic [default]: the K* buffer is kept near
  *               512 MB (16384 candidates at N = 4096, 65536 at N <= 1024)
- *   "cov"       covariance builder: 2 = TMA-staged, pre-scaled term-major operands [default], 1 = round-1 kernel
  *   "graph"     1 = the split-chain schedule of a factorisation (~600 launches / event records / stream waits at
  *               N = 4096) is captured once per layout into a CUDA graph and replayed per fit [default]; 0 = enqueue
  *               every call directly
@@ -74,7 +75,8 @@ const char* gpk_version(void);
  *               error-free split of L^-1 and K* into 7 balanced base-256 digits each, 28 digit-pair products
  *               (gpk_ozaki.cuh); used while max |L^-1| < 64 and N <= 16384, otherwise the fp64 kernel runs [default;
  *               batches of >= 2048 candidates]; 0 = always fp64 DMMA.  The posterior mean never goes through the digits
- *               (fp64 K* alpha)
+ *               (fp64 K* alpha); the covariance builder writes the digits and the mean partials itself, no fp64 K*
+ *               in HBM
  *   "ozpersist" 0 = one CTA per tile; 1 = one CTA per SM walks the tile list (by clusters); 3 = automatic [default]:
  *               persistent for N <= 4096, one CTA per tile above (tools/persist_threshold.py, DESIGN.md 9.5)
  *   "ozcluster" 1, 2 or 4 [default 4] = CTAs per cluster of the int8 contraction: they take adjacent candidate blocks of
@@ -83,14 +85,6 @@ const char* gpk_version(void);
  *   "ozgrid"    >= 0: most clusters the persistent walk of the int8 contraction launches; 0 = as many as fit at once
  *               [default].  Tests and diagnostics: with "ozpersist" = 1 and "ozgrid" = 1 one cluster walks every tile in
  *               the L2-grouped, longest-first order.  Results are bit-identical for every value
- *   "ozpdl"     1 = the look-ahead K* builder runs as a small resident grid ("covctas" CTAs per SM) that triggers a
- *               programmatic dependent launch of the contraction behind it on the same stream (the two really co-run);
- *               0 = builder on the side stream (the block scheduler places it in the contraction's tail) [default: the
- *               co-running contraction loses more than the builder costs]
- *   "ozfused"   1 = with "ozaki": the covariance builder writes the int8 digits and the mean partials itself, no fp64
- *               K* in HBM [default]; 0 = fp64 K* + split kernel + mean dot
- *   "persist"   1 = persistent fp64 variance contraction (one CTA per SM, dynamic tile counter); 0 = one CTA per tile
- *               [default: on an H100 the two are within 2 % of each other for N = 512 .. 6144]
  *   "depth2"    1 = trailing updates of two consecutive panels in one K = 256 contraction (odd steps; even steps update
  *               only the next-but-one block column); 0 = one K = 128 update per step (bit-identical factor);
  *               2 = automatic [default]: on for N >= 6144, where the trailing updates gate the fit
@@ -368,7 +362,7 @@ int gpk_oz_contract(gpk_handle* h, const double* P, int n, const double* Ks, lon
  * out[8] = variance-GEMM launches so far,
  * out[9] = total kernel launches so far,
  * out[10] = of those, launches of the int8 (Ozaki) contraction; out[11] = largest row exponent of L^-1 seen by it
- * (option "ozaki"); out[12] = option "persist"; out[13] = int8 slice-pair products the int8 contraction spends per
+ * (option "ozaki"); out[12] reserved (zero); out[13] = int8 slice-pair products the int8 contraction spends per
  * fp64 product (28: 7 balanced base-256 digits per operand); out[14] = which int8 kernel ran last (1 gpk_oz_vargemm_kernel;
  * + 8: persistent tile walk; + 16 / + 32: clusters of 2 / 4 CTAs); out[15] reserved (zero). */
 int gpk_get_timings(gpk_handle* h, double* out16);

@@ -149,11 +149,11 @@ class Handle(object):
             self.set_option("loader", int(os.environ["GPK_LOADER"]))
         if os.environ.get("GPK_CHUNK"):
             self.set_option("chunk", int(os.environ["GPK_CHUNK"]))
-        # implementation switches (all default-on variants have a cross-check twin): GPK_COV=1|2, GPK_PERSIST=0|1,
-        # GPK_CHAINSPLIT=0|1, GPK_OZAKI=0|1
-        for env, key in (("GPK_COV", "cov"), ("GPK_PERSIST", "persist"), ("GPK_CHAINSPLIT", "chainsplit"),
-                         ("GPK_OZAKI", "ozaki"), ("GPK_GRAPH", "graph"), ("GPK_DEPTH2", "depth2"), ("GPK_OZFUSED", "ozfused"), ("GPK_OZPERSIST", "ozpersist"), ("GPK_OZPDL", "ozpdl"), ("GPK_COVCTAS", "covctas"),
-                         ("GPK_OZCLUSTER", "ozcluster"), ("GPK_OZGRID", "ozgrid")):
+        # schedule and contraction switches: GPK_CHAINSPLIT=0|1, GPK_OZAKI=0|1 (fp64 | int8 variance contraction),
+        # GPK_GRAPH, GPK_DEPTH2, GPK_OZPERSIST, GPK_OZCLUSTER, GPK_OZGRID (see gpk_set_option in include/gpk.h)
+        for env, key in (("GPK_CHAINSPLIT", "chainsplit"), ("GPK_OZAKI", "ozaki"), ("GPK_GRAPH", "graph"),
+                         ("GPK_DEPTH2", "depth2"), ("GPK_OZPERSIST", "ozpersist"), ("GPK_OZCLUSTER", "ozcluster"),
+                         ("GPK_OZGRID", "ozgrid")):
             if os.environ.get(env):
                 self.set_option(key, int(os.environ[env]))
 
@@ -494,7 +494,7 @@ class Handle(object):
         t = np.zeros(16)
         self._check(self.lib.gpk_get_timings(self._h, _as_dp(t)))
         keys = ["fit_ms", "kbuild_ms", "potrf_ms", "linv_ms", "score_ms", "kstar_ms", "vargemm_ms", "finish_ms",
-                "launches_vargemm", "launches_total", "launches_ozaki", "ozaki_max_row_exponent", "persist",
+                "launches_vargemm", "launches_total", "launches_ozaki", "ozaki_max_row_exponent", "reserved",
                 "ozaki_slice_pairs", "ozaki_kernel_variant"]
         return dict(zip(keys, t.tolist()))
 

@@ -51,10 +51,7 @@ struct gpk_handle {
     std::vector<cudaEvent_t> ev_cs;         // split chain: 5 events per step (diag, X, trsm', pu', rest_a)
     // variance contraction on the int8 tensor pipe (gpk_ozaki.cuh); 0 = fp64 DMMA kernels
     int ozaki = 1;
-    DevBuf oz_Pq, oz_Kq, oz_Kq2, oz_eP, oz_emax, oz_mu, oz_mu2, oz_pmu2;
-    int oz_pdl = 0;                 // 1: look-ahead K* builder = small resident grid that triggers the dependent launch of the
-                                    //    contraction behind it on the SAME stream (real overlap); 0: side stream (tail overlap only)
-    int cov_ctas = 2;               // CTAs per SM of that resident builder grid
+    DevBuf oz_Pq, oz_Kq, oz_Kq2, oz_eP, oz_emax, oz_pmu2;
     int oz_last_variant = 0;        // contraction of the last int8 launch: 1 = gpk_oz_vargemm_kernel, + 8 when it walked the tile
                                     // list persistently, + 16 / + 32 in clusters of 2 / 4 CTAs
     int oz_cluster = 4;             // CTAs per cluster of the int8 contraction (1, 2 or 4): they share the L^-1 slices by TMA
@@ -66,16 +63,12 @@ struct gpk_handle {
                                     // walk is as fast or faster up to N = 4096, one CTA per tile is faster at 6144)
     int oz_grid = 0;                // most clusters the persistent walk launches (0: as many as fit at once [default])
     DevBuf oz_probe;                // scratch of gpk_oz_contract (operands, slices, exponents, partial sums)
-    int oz_fused = 1;              // 1: K* leaves the covariance builder as int8 digits (gpk_cov_oz_kernel); 0: fp64 K* + split + dot
     long oz_linv_serial = -1;       // linv_serial the slices of L^-1 were made for
     long linv_serial = 0;           // bumped whenever L^-1 is (re)built
     int oz_emax_host = 0;
     long oz_rows = 0, oz_rows2 = 0;
     CUtensorMap mapOzP, mapOzK, mapOzK2;
     double oz_launches = 0;
-    int persist = 0;                // 1: persistent variance contraction (gpk_vargemm_persistent_kernel); 0: one CTA per tile
-                                    // (tools/persist_threshold.py on an H100: within 2 % of each other for N = 512 .. 6144)
-    DevBuf tile_cnt;
     int n_sm = 0;
     int use_graph = 1;              // split chain: one CUDA graph per layout, replayed per fit
     cudaGraphExec_t fit_graph = nullptr;
@@ -104,7 +97,6 @@ struct gpk_handle {
     DevBuf Xrow, Xt, y, Kbuf, P, Q, W, lower, upper, logdet_part, scal, status, jobs;
     DevBuf Kstar2, cand2;
     DevBuf Xts;                     // training inputs, term-major and pre-scaled (operand of gpk_cov_tma_kernel)
-    int cov_kernel = 2;             // 2 = TMA-staged, pre-scaled operands [default]; 1 = the round-1 kernel (cross-check)
     cudaStream_t copy_stream = nullptr;
     std::vector<cudaEvent_t> ev_copied, ev_scored;
     std::vector<cudaEvent_t> ev_g0, ev_g1;    // timed pairs around every variance-GEMM launch of the last scoring call
@@ -273,10 +265,12 @@ int make_cov_map(gpk_handle* h, CUtensorMap* map, void* base, int n_terms, long 
     return GPK_OK;
 }
 
-inline bool cov_tma(const gpk_handle* h) { return h->cov_kernel == 2 && h->loader != LOADER_CPASYNC; }
+// The covariance builder follows the tile engine's loader: gpk_cov_tma_kernel with TMA, gpk_cov_kernel under cp.async
+// (loader 0, also what gpk_create falls back to when the driver has no cuTensorMapEncodeTiled)
+inline bool cov_tma(const gpk_handle* h) { return h->loader != LOADER_CPASYNC; }
 
 // "Transposed" operand of the covariance builder for n points X (row-major, n x d) into dst with ld columns:
-// term-major + pre-scaled for the TMA kernel (dst needs n_terms x ld doubles), axis-major for the round-1 kernel
+// term-major + pre-scaled for the TMA kernel (dst needs n_terms x ld doubles), axis-major for gpk_cov_kernel
 // (d x ld doubles).  lo / up: input bounds to apply first (NULL: none).
 int build_cov_operand(gpk_handle* h, cudaStream_t st, const double* X, long n, int d, const double* lo, const double* up,
                       double* dst, long ld) {
@@ -337,33 +331,22 @@ cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t s
     return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
 }
 
-// int8 contraction launch in clusters of cs CTAs (grid a multiple of cs), with an optional programmatic dependency on the
-// kernel launched just before it on the stream (the resident look-ahead K* builder, which triggers at its start)
+// int8 contraction launch in clusters of cs CTAs (grid a multiple of cs)
 template <typename... KArgs, typename... Args>
-cudaError_t launch_oz(void (*kernel)(KArgs...), unsigned grid, int cs, size_t smem, cudaStream_t stream, bool dependent,
-                      Args... args) {
+cudaError_t launch_oz(void (*kernel)(KArgs...), unsigned grid, int cs, size_t smem, cudaStream_t stream, Args... args) {
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = dim3(grid);
     cfg.blockDim = dim3(OZ_THREADS);
     cfg.dynamicSmemBytes = smem;
     cfg.stream = stream;
-    cudaLaunchAttribute attr[2];
-    int na = 0;
-    if (dependent) {
-        attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[na].val.programmaticStreamSerializationAllowed = 1;
-        ++na;
-    }
-    if (cs > 1) {
-        attr[na].id = cudaLaunchAttributeClusterDimension;
-        attr[na].val.clusterDim.x = (unsigned)cs;
-        attr[na].val.clusterDim.y = 1;
-        attr[na].val.clusterDim.z = 1;
-        ++na;
-    }
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = (unsigned)cs;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = na;
+    cfg.numAttrs = cs > 1 ? 1 : 0;
     return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
 }
 
@@ -399,7 +382,7 @@ int oz_max_clusters(gpk_handle* h, int cs, int* out) {
 // slices mapK covers (stacked [7][rows][NP]), with the handle's "ozcluster", "ozpersist" and "ozgrid": L2 group,
 // persistent grid and the variant code timings() reports.  Shared by score_dev and gpk_oz_contract.
 int launch_oz_contraction(gpk_handle* h, const CUtensorMap& mapP, const CUtensorMap& mapK, int nb, long rows_padded,
-                          long NP, long rows, const int* eP, int eK, double* part_ssq, long ldpart, bool dependent) {
+                          long NP, long rows, const int* eP, int eK, double* part_ssq, long ldpart) {
     OzArgs o;
     o.nb = nb; o.ncb = (int)(rows_padded / OZ_TN); o.NP = (int)NP; o.rows = (int)rows;
     // a group's K* slices take about 24 MB, half of the L2; whole clusters of candidate blocks (ncb = rows_padded / 32 is
@@ -418,7 +401,7 @@ int launch_oz_contraction(gpk_handle* h, const CUtensorMap& mapP, const CUtensor
         grid = cs * std::min(tiles / cs, nclusters);
     }
     h->oz_last_variant = 1 + (persist == 1 ? 8 : 0) + (cs == 2 ? 16 : cs == 4 ? 32 : 0);
-    CK(launch_oz(gpk_oz_vargemm_kernel, (unsigned)grid, cs, (size_t)OZ_SMEM, h->stream, dependent, mapP, mapK, o));
+    CK(launch_oz(gpk_oz_vargemm_kernel, (unsigned)grid, cs, (size_t)OZ_SMEM, h->stream, mapP, mapK, o));
     CKL();
     return GPK_OK;
 }
@@ -456,7 +439,6 @@ int set_kernel_attrs(gpk_handle* h) {
     CK(cudaFuncSetAttribute(gpk_oz_vargemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, OZ_SMEM));
     CK(cudaFuncSetAttribute(gpk_cov_oz_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cov_oz_smem_bytes(GPK_MAX_TERMS, 8)));
     CK(cudaFuncSetAttribute(gpk_cov_oz_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cov_oz_smem_bytes(GPK_MAX_TERMS, 4)));
-    CK(cudaFuncSetAttribute(gpk_vargemm_persistent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PV_SMEM));
     {
         cudaDeviceProp prop;
         CK(cudaGetDeviceProperties(&prop, h->device));
@@ -858,7 +840,6 @@ int score_dev(gpk_handle* h, const double* dX, long m, int kind, double eta, dou
     bool use_oz = false;
     if (m >= 2048 && (rc = prepare_ozaki(h, &use_oz))) return rc;
     int oz_eK = 0;
-    const bool oz_fused = use_oz && h->oz_fused && cov_tma(h);
     if (use_oz) {
         // slices of K* per chunk buffer: [S][cap][NP] int8; one exponent for the whole matrix (0 < k <= amp)
         // (the tensor maps are re-encoded per call: a few microseconds, and they depend on the buffer, cap and NP)
@@ -866,8 +847,6 @@ int score_dev(gpk_handle* h, const double* dX, long m, int kind, double eta, dou
         if (h->overlap && (rc = ensure(h, h->oz_Kq2, (size_t)OZ_S * cap * NP))) return rc;
         if ((rc = make_oz_map(h, &h->mapOzK, h->oz_Kq.p, (long)OZ_S * cap, NP, OZ_TN))) return rc;
         if (h->overlap && (rc = make_oz_map(h, &h->mapOzK2, h->oz_Kq2.p, (long)OZ_S * cap, NP, OZ_TN))) return rc;
-        if ((rc = ensure(h, h->oz_mu, (size_t)cap * 8))) return rc;
-        if (h->overlap && (rc = ensure(h, h->oz_mu2, (size_t)cap * 8))) return rc;
         if (h->overlap && (rc = ensure(h, h->oz_pmu2, (size_t)h->nb * cap * 8))) return rc;
         oz_eK = oz_exponent(h->spec.amp);
     }
@@ -900,60 +879,37 @@ int score_dev(gpk_handle* h, const double* dX, long m, int kind, double eta, dou
         h->ev_g1.push_back(e2);
     }
     h->last_nchunks = nchunks;
-    auto launch_cov = [&](int ci, cudaStream_t st, bool small, bool resident = false) -> int {
+    auto launch_cov = [&](int ci, cudaStream_t st, bool small) -> int {
         const long base = (long)ci * cap;
         const long mc = std::min(cap, m - base);
         const long mcp = round_up(mc, BM);
-        double* dst = (pipelined && (ci & 1)) ? ptr<double>(h->Kstar2) : ptr<double>(h->Kstar);
+        const bool second = pipelined && (ci & 1);
         if (feeder) {
             int frc = feeder->ready(base, base + mc, st);
             if (frc) return frc;
         }
         const double* lo = h->has_bounds ? ptr<double>(h->lower) : nullptr;
         const double* up = h->has_bounds ? ptr<double>(h->upper) : nullptr;
-        int8_t* qdst = (pipelined && (ci & 1)) ? ptr<int8_t>(h->oz_Kq2) : ptr<int8_t>(h->oz_Kq);
-        if (use_oz && oz_fused) {
-            // K* never reaches HBM in fp64: digits + this tile's share of the mean straight out of the builder
-            CUtensorMap map;
-            int mrc = make_cov_map(h, &map, (void*)train_operand(h), h->spec.n_terms, NP);
-            if (mrc) return mrc;
-            double* pmu = (pipelined && (ci & 1)) ? ptr<double>(h->oz_pmu2) : ptr<double>(h->part_mu);
-            const int gx = (int)(NP / 128);
-            if (small) {
-                const int gy = (int)(mcp / 16);
-                const long items = (long)gx * gy;
-                const unsigned grid = resident ? (unsigned)std::min<long>(items, (long)std::max(h->n_sm, 1) * h->cov_ctas) : (unsigned)items;
-                gpk_cov_oz_kernel<4><<<grid, 256, cov_oz_smem_bytes(h->spec.n_terms, 4), st>>>(
-                    map, h->spec, h->n, dX + base * h->d, h->d, mc, lo, up, ptr<double>(h->alpha), oz_eK, qdst, NP, cap * NP, pmu, cap,
-                    gx, gy, resident ? 1 : 0);
-            } else {
-                const int gy = (int)(mcp / 32);
-                gpk_cov_oz_kernel<8><<<(unsigned)((long)gx * gy), 256, cov_oz_smem_bytes(h->spec.n_terms, 8), st>>>(
-                    map, h->spec, h->n, dX + base * h->d, h->d, mc, lo, up, ptr<double>(h->alpha), oz_eK, qdst, NP, cap * NP, pmu, cap,
-                    gx, gy, 0);
-            }
-            CKL();
-            return GPK_OK;
-        }
-        int crc = launch_cov_tiles(h, st, train_operand(h), NP, h->n, dX + base * h->d, h->d, mc, mcp, lo, up, dst, NP, 0, small);
-        if (crc || !use_oz) return crc;
-        // int8 slices of this chunk's K* (rows beyond mc are exact zeros in K*, so are their digits)
-        gpk_oz_split_kernel<<<(unsigned)((mcp * NP + 255) / 256), 256, 0, st>>>(dst, mcp, NP, nullptr, oz_eK, qdst, cap * NP);
-        CKL();
-        // the mean of this chunk in fp64: one warp per candidate, K*[c, :] . alpha
-        double* mdst = (pipelined && (ci & 1)) ? ptr<double>(h->oz_mu2) : ptr<double>(h->oz_mu);
-        gpk_rowdot_kernel<<<(unsigned)((mcp + 7) / 8), 256, 0, st>>>(dst, NP, mcp, (int)NP, 0, ptr<double>(h->alpha), mdst);
+        if (!use_oz)
+            return launch_cov_tiles(h, st, train_operand(h), NP, h->n, dX + base * h->d, h->d, mc, mcp, lo, up,
+                                    second ? ptr<double>(h->Kstar2) : ptr<double>(h->Kstar), NP, 0, small);
+        // K* never reaches HBM in fp64: digits + this tile's share of the mean straight out of the builder
+        CUtensorMap map;
+        int mrc = make_cov_map(h, &map, (void*)train_operand(h), h->spec.n_terms, NP);
+        if (mrc) return mrc;
+        int8_t* qdst = second ? ptr<int8_t>(h->oz_Kq2) : ptr<int8_t>(h->oz_Kq);
+        double* pmu = second ? ptr<double>(h->oz_pmu2) : ptr<double>(h->part_mu);
+        const int gx = (int)(NP / 128);
+        if (small)
+            gpk_cov_oz_kernel<4><<<(unsigned)(gx * (mcp / 16)), 256, cov_oz_smem_bytes(h->spec.n_terms, 4), st>>>(
+                map, h->spec, h->n, dX + base * h->d, h->d, mc, lo, up, ptr<double>(h->alpha), oz_eK, qdst, NP, cap * NP, pmu, cap, gx);
+        else
+            gpk_cov_oz_kernel<8><<<(unsigned)(gx * (mcp / 32)), 256, cov_oz_smem_bytes(h->spec.n_terms, 8), st>>>(
+                map, h->spec, h->n, dX + base * h->d, h->d, mc, lo, up, ptr<double>(h->alpha), oz_eK, qdst, NP, cap * NP, pmu, cap, gx);
         CKL();
         return GPK_OK;
     };
-    // int8 path with the fused builder: everything on ONE stream.  The builder of chunk i+1 is a small resident grid
-    // (cov_ctas CTAs per SM) that triggers its dependents at once; the contraction of chunk i behind it is launched with
-    // the programmatic-stream-serialization attribute, so it starts while the builder runs and the two share the SMs
-    // (FP64 ALU + tensor pipe).  With two streams the block scheduler only placed the builder in the contraction's tail.
-    const bool chained = pipelined && oz_fused && h->oz_pdl;
-    if (chained) {
-        if ((rc = launch_cov(0, h->stream, false))) return rc;
-    } else if (pipelined) {
+    if (pipelined) {
         CK(cudaEventRecord(h->ev_order, h->stream));          // side stream starts after all prior work
         CK(cudaStreamWaitEvent(h->side_stream, h->ev_order, 0));
         if ((rc = launch_cov(0, h->side_stream, false))) return rc;
@@ -965,15 +921,7 @@ int score_dev(gpk_handle* h, const double* dX, long m, int kind, double eta, dou
         const long mcp = round_up(mc, BM);
         const bool last = ci == nchunks - 1;
         if (last) CK(cudaEventRecord(h->ev[8], h->stream));
-        bool dependent = false;                                 // the contraction below is the dependent of a resident builder
-        if (chained) {
-            if (last) CK(cudaEventRecord(h->ev[10], h->stream));
-            CK(cudaEventRecord(h->ev_g0[ci], h->stream));       // nothing may sit between the builder and its dependent
-            if (ci + 1 < nchunks) {
-                if ((rc = launch_cov(ci + 1, h->stream, true, true))) return rc;
-                dependent = true;
-            }
-        } else if (pipelined) {
+        if (pipelined) {
             CK(cudaStreamWaitEvent(h->stream, h->ev_cov[ci], 0));
             if (ci + 1 < nchunks) {
                 if (ci >= 1) CK(cudaStreamWaitEvent(h->side_stream, h->ev_gemm[ci - 1], 0));   // buffer (ci+1)&1 is free
@@ -995,29 +943,18 @@ int score_dev(gpk_handle* h, const double* dX, long m, int kind, double eta, dou
         a.part_mu = ptr<double>(h->part_mu);
         a.part_ssq = ptr<double>(h->part_ssq);
         a.ldpart = cap;
-        if (!chained) {
-            if (last) CK(cudaEventRecord(h->ev[10], h->stream));
-            CK(cudaEventRecord(h->ev_g0[ci], h->stream));
-        }
+        if (last) CK(cudaEventRecord(h->ev[10], h->stream));
+        CK(cudaEventRecord(h->ev_g0[ci], h->stream));
         if (use_oz) {
             if ((rc = launch_oz_contraction(h, h->mapOzP, second ? h->mapOzK2 : h->mapOzK, h->nb, mcp, NP, cap,
-                                            ptr<int>(h->oz_eP), oz_eK, a.part_ssq, a.ldpart, dependent)))
+                                            ptr<int>(h->oz_eP), oz_eK, a.part_ssq, a.ldpart)))
                 return rc;
             h->oz_launches += 1;
-        } else if (h->persist && h->loader == LOADER_TMA_WS) {
-            // one CTA per SM, tiles handed out by a counter (zeroed in stream order before every launch)
-            if ((rc = ensure(h, h->tile_cnt, 4))) return rc;
-            CK(cudaMemsetAsync(h->tile_cnt.p, 0, 4, h->stream));
-            VarArgs v;
-            v.nb = a.nb; v.mcb = a.mcb; v.z = a.z; v.part_mu = a.part_mu; v.part_ssq = a.part_ssq; v.ldpart = a.ldpart;
-            v.counter = ptr<int>(h->tile_cnt);
-            const int grid = std::min(h->nb * a.mcb, std::max(h->n_sm, 1));
-            gpk_vargemm_persistent_kernel<<<grid, WS_THREADS, PV_SMEM, h->stream>>>(h->mapP, second ? h->mapKs2 : h->mapKs, v);
-            CKL();
         } else if ((rc = launch_gemm<EPI_COLREDUCE>(h, h->mapP, second ? h->mapKs2 : h->mapKs, a, h->nb * a.mcb))) return rc;
         CK(cudaEventRecord(h->ev_g1[ci], h->stream));
         if (last) CK(cudaEventRecord(h->ev[11], h->stream));
-        if (pipelined && !chained && !oz_fused) CK(cudaEventRecord(h->ev_gemm[ci], h->stream));
+        // fp64 path: this parity's K* buffer is free once the contraction has read it
+        if (pipelined && !use_oz) CK(cudaEventRecord(h->ev_gemm[ci], h->stream));
         h->launches_var += 1;
         h->last_chunk_rows = mcp;
         FinishArgs f;
@@ -1032,8 +969,7 @@ int score_dev(gpk_handle* h, const double* dX, long m, int kind, double eta, dou
         f.out_acq = d_out ? d_out + index_offset + base : nullptr;
         f.block_best = ptr<BestPair>(h->block_best);
         f.n_negative = d_nneg;
-        f.mu_direct = (use_oz && !oz_fused) ? (second ? ptr<double>(h->oz_mu2) : ptr<double>(h->oz_mu)) : nullptr;
-        if (oz_fused && second) f.part_mu = ptr<double>(h->oz_pmu2);
+        if (use_oz && second) f.part_mu = ptr<double>(h->oz_pmu2);
         const int fb = (int)((mc + 255) / 256);
         gpk_finish_kernel<<<fb, 256, 0, h->stream>>>(f);
         CKL();
@@ -1041,8 +977,8 @@ int score_dev(gpk_handle* h, const double* dX, long m, int kind, double eta, dou
             gpk_argmax_final_kernel<<<1, 256, 0, h->stream>>>(ptr<BestPair>(h->block_best), fb, d_best);
             CKL();
         }
-        // fused int8 builder: it also writes this parity's mean partials, which the finish kernel above still reads
-        if (pipelined && !chained && oz_fused) CK(cudaEventRecord(h->ev_gemm[ci], h->stream));
+        // int8 path: the builder also writes this parity's mean partials, which the finish kernel above still reads
+        if (pipelined && use_oz) CK(cudaEventRecord(h->ev_gemm[ci], h->stream));
         if (last) CK(cudaEventRecord(h->ev[12], h->stream));
     }
     CK(cudaEventRecord(h->ev[7], h->stream));
@@ -1110,7 +1046,7 @@ int gpk_destroy(gpk_handle* h) {
     DevBuf* bufs[] = {&h->Xrow, &h->Xt, &h->y, &h->Kbuf, &h->P, &h->Q, &h->W, &h->lower, &h->upper, &h->logdet_part,
                       &h->scal, &h->status, &h->jobs, &h->cand, &h->Kstar, &h->Kstar2, &h->cand2, &h->part_mu, &h->part_ssq, &h->out_mu,
                       &h->out_var, &h->out_acq, &h->block_best, &h->best, &h->nneg, &h->Vt, &h->cov, &h->XsT,
-                      &h->tmpjobs, &h->alpha, &h->tmp1, &h->tmp2, &h->tmp3, &h->chain_cnt, &h->dprof, &h->Xts, &h->tile_cnt, &h->oz_Pq, &h->oz_Kq, &h->oz_Kq2, &h->oz_eP, &h->oz_emax, &h->oz_mu, &h->oz_mu2, &h->oz_pmu2, &h->oz_probe,
+                      &h->tmpjobs, &h->alpha, &h->tmp1, &h->tmp2, &h->tmp3, &h->chain_cnt, &h->dprof, &h->Xts, &h->oz_Pq, &h->oz_Kq, &h->oz_Kq2, &h->oz_eP, &h->oz_emax, &h->oz_pmu2, &h->oz_probe,
                       &h->multi_cand, &h->multi_A, &h->multi_B, &h->multi_out, &h->multi_bb, &h->gather, &h->best_global,
                       &h->de_pop, &h->de_trial, &h->de_param, &h->de_E, &h->de_small, &h->de_sort, &h->ep_buf, &h->es_state, &h->es_U, &h->es_work, &h->es_in};
     for (DevBuf* b : bufs)
@@ -1170,28 +1106,9 @@ int gpk_set_option(gpk_handle* h, const char* key, long value) {
         h->oz_grid = (int)value;
         return GPK_OK;
     }
-    if (!strcmp(key, "ozpdl")) {
-        h->oz_pdl = (int)value;
-        return GPK_OK;
-    }
-    if (!strcmp(key, "covctas")) {
-        if (value < 1 || value > 8) BAD("covctas must be 1..8");
-        h->cov_ctas = (int)value;
-        return GPK_OK;
-    }
-    if (!strcmp(key, "ozfused")) {
-        if (value != 0 && value != 1) BAD("ozfused must be 0 or 1");
-        h->oz_fused = (int)value;
-        return GPK_OK;
-    }
     if (!strcmp(key, "ozaki")) {
         if (value != 0 && value != 1) BAD("ozaki must be 0 (fp64 DMMA) or 1 (int8 tensor pipe, error-free split)");
         h->ozaki = (int)value;
-        return GPK_OK;
-    }
-    if (!strcmp(key, "persist")) {
-        if (value != 0 && value != 1) BAD("persist must be 0 or 1");
-        h->persist = (int)value;
         return GPK_OK;
     }
     if (!strcmp(key, "depth2")) {
@@ -1225,13 +1142,6 @@ int gpk_set_option(gpk_handle* h, const char* key, long value) {
                 CK(cudaMemcpy((char*)h->dprof.p + 63 * 8, &one, 8, cudaMemcpyHostToDevice));
             }
         }
-        return GPK_OK;
-    }
-    if (!strcmp(key, "cov")) {
-        if (value != 1 && value != 2) BAD("cov must be 2 (TMA-staged covariance builder, pre-scaled operands) or 1 (round-1 kernel)");
-        h->cov_kernel = (int)value;
-        h->fitted = false;
-        h->linv_ready = false;
         return GPK_OK;
     }
     if (!strcmp(key, "chunk")) {
@@ -2441,7 +2351,7 @@ int gpk_oz_contract(gpk_handle* h, const double* P, int n, const double* Ks, lon
     CUtensorMap mapP, mapK;
     if ((rc = make_oz_map(h, &mapP, dPq, (long)OZ_S * NP, NP, OZ_TM / h->oz_cluster))) return rc;
     if ((rc = make_oz_map(h, &mapK, dKq, (long)OZ_S * MP, NP, OZ_TN))) return rc;
-    if ((rc = launch_oz_contraction(h, mapP, mapK, (int)nb, MP, NP, MP, de, ek, dpart, MP, false))) return rc;
+    if ((rc = launch_oz_contraction(h, mapP, mapK, (int)nb, MP, NP, MP, de, ek, dpart, MP))) return rc;
     CK(cudaMemcpy2DAsync(part_ssq, (size_t)m * 8, dpart, (size_t)MP * 8, (size_t)m * 8, (size_t)nb, cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(eP, de, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
@@ -2668,7 +2578,6 @@ int gpk_get_timings(gpk_handle* h, double* out /* 16 */) {
     out[9] = h->launches_total;
     out[10] = h->oz_launches;
     out[11] = (double)h->oz_emax_host;
-    out[12] = (double)h->persist;
     out[13] = (double)OZ_PAIRS;
     out[14] = (double)h->oz_last_variant;
     return GPK_OK;

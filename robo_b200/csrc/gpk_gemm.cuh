@@ -573,184 +573,3 @@ gpk_gemm_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
             g.part_mu[(long)job.aux * g.ldpart + job.c_col + tid] = lds64(red + 8 * tid) + lds64(red + 8 * (128 + tid));
     }
 }
-
-// ---------------------------------------------------------------------------------------
-// Persistent variance contraction (default scoring kernel): one CTA per SM walks the tile list of a candidate chunk
-// (same tiles, same order as JOBS_VARIANCE above: groups of VAR_GROUP candidate blocks, longest contraction first)
-// taking the next tile from a global counter.  The TMA producer warp runs ahead ACROSS tile boundaries, so the operand
-// ring stays full while the consumers reduce and store a finished tile: no pipeline fill / drain per tile (a 128-long
-// contraction is only 8 k-steps), no launch tail per wave, and the load balance is dynamic.  Same fragment layout,
-// accumulation order and column-reduction order as gpk_gemm_ws_kernel<EPI_COLREDUCE>: bit-identical partial sums.
-//   smem: PV_STAGES x 32 KB operand ring | full / empty mbarriers | 2 tile slots | 2 x (4 x 128) reduction scratch
-// ---------------------------------------------------------------------------------------
-constexpr int PV_STAGES = 6;
-constexpr int PV_RED_BYTES = 4 * 128 * 8;          // {ssq, mu} x {wm = 0, 1} x 128 columns, per tile parity
-constexpr int PV_SMEM = PV_STAGES * STAGE_BYTES_TMA + 1024 /*align*/ + 128 /*barriers + tile slots*/ + 2 * PV_RED_BYTES;
-
-struct VarArgs {
-    int nb, mcb;                       // row blocks of L^-1 x candidate blocks of the chunk
-    const double* z;                   // z = L^-1 (y - mean): row weights of the mean
-    double* part_mu; double* part_ssq; long ldpart;
-    int* counter;                      // tile counter, zeroed before the launch
-};
-
-__device__ __forceinline__ void var_tile(const VarArgs& g, int id, int& ib, int& cb) {
-    const int full = g.mcb / VAR_GROUP;
-    int grp = id / (g.nb * VAR_GROUP), gsz = VAR_GROUP;
-    if (grp >= full) { grp = full; gsz = g.mcb - full * VAR_GROUP; }
-    id -= grp * g.nb * VAR_GROUP;
-    ib = g.nb - 1 - id / gsz;
-    cb = grp * VAR_GROUP + id % gsz;
-}
-
-__global__ void __launch_bounds__(WS_THREADS, 1)
-gpk_vargemm_persistent_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
-                              const VarArgs g)
-{
-    constexpr int LOADER = LOADER_TMA;
-    constexpr int MI = 8, HM = 64;
-    extern __shared__ unsigned char smem_raw[];
-    const uint32_t smem = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    constexpr int ROWB = BK * 8;
-    constexpr int A_BYTES = BM * ROWB;
-    constexpr int STAGE_BYTES = STAGE_BYTES_TMA;
-    constexpr int RING = PV_STAGES * STAGE_BYTES;
-    const uint32_t full_bar = smem + RING;                       // PV_STAGES x 8 bytes
-    const uint32_t empty_bar = smem + RING + 48;                 // PV_STAGES x 8 bytes
-    const uint32_t slot = smem + RING + 96;                      // 2 x int: tile id of tile parity 0 / 1
-    const uint32_t red0 = smem + RING + 128;                     // 2 tile parities x (4 x 128 doubles)
-    const int total = g.nb * g.mcb;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-
-    if (tid == 0) {
-#pragma unroll
-        for (int s = 0; s < PV_STAGES; ++s) { mbar_init(full_bar + 8 * s, 1); mbar_init(empty_bar + 8 * s, 8); }
-        fence_barrier_init();
-        fence_proxy_async();
-    }
-    __syncthreads();
-
-    if (warp == 8) {
-        // ---------------- producer ----------------
-        if (lane == 0) {
-            int s = 0;                       // ring slot of the next k-step
-            uint32_t use = 0;                // how many times the ring has wrapped (slot s is in its use-th use)
-            for (int t = 0;; ++t) {
-                const int id = atomicAdd(g.counter, 1);
-                asm volatile("st.shared.s32 [%0], %1;" :: "r"(slot + 4u * (uint32_t)(t & 1)), "r"(id) : "memory");
-                if (id >= total) {
-                    // wake the consumers once more: they read the slot and leave
-                    if (use > 0) while (!mbar_try_wait(empty_bar + 8 * s, (use - 1) & 1)) { }
-                    mbar_arrive(full_bar + 8 * s);
-                    break;
-                }
-                int ib, cb;
-                var_tile(g, id, ib, cb);
-                const int KT = (ib + 1) * (BM / BK);
-                for (int kt = 0; kt < KT; ++kt) {
-                    if (use > 0) while (!mbar_try_wait(empty_bar + 8 * s, (use - 1) & 1)) { }
-                    const uint32_t st = smem + s * STAGE_BYTES;
-                    fence_proxy_async();
-                    mbar_arrive_expect_tx(full_bar + 8 * s, STAGE_BYTES);
-                    tma_load_2d(st, &mapA, kt * BK, ib * BM, full_bar + 8 * s);
-                    tma_load_2d(st + A_BYTES, &mapB, kt * BK, cb * BN, full_bar + 8 * s);
-                    if (++s == PV_STAGES) { s = 0; ++use; }
-                }
-            }
-        }
-        return;
-    }
-
-    // ---------------- consumers (warps 0-7) ----------------
-    const int gq = lane >> 2, tq = lane & 3;
-    const int wm = warp >> 2, wn = warp & 3;
-    constexpr int BLK = 8 * ROWB;
-    // fragment offsets inside a stage.  A rows wm*64 + r, B rows wn*32 + r with the same r = rowmap(gq) < 8, so the
-    // swizzle term ((k >> 1) ^ r) << 4 is common: four A offsets and one A -> B distance are all the state needed
-    // (tile_off(row, ks*4 + tq) = row*128 + (((2 ks + (tq >> 1)) ^ r) << 4) + ((tq & 1) << 3))
-    const int rA = wm * HM + rowmap<LOADER>(gq);
-    int kxA[4];
-#pragma unroll
-    for (int ks = 0; ks < 4; ++ks) kxA[ks] = tile_off<LOADER>(rA, ks * 4 + tq);
-    const int dB = A_BYTES + (wn * 32 - wm * HM) * ROWB;
-    int s = 0;
-    uint32_t use = 0;
-    for (int t = 0;; ++t) {
-        // the first stage of the tile (or the producer's final wake-up) carries the tile id
-        while (!mbar_try_wait(full_bar + 8 * s, use & 1)) { }
-        int id;
-        asm volatile("ld.shared.s32 %0, [%1];" : "=r"(id) : "r"(slot + 4u * (uint32_t)(t & 1)) : "memory");
-        if (id >= total) break;
-        int ib, cb;
-        var_tile(g, id, ib, cb);
-        const int KT = (ib + 1) * (BM / BK);
-        double acc[MI][4][2];
-#pragma unroll
-        for (int mi = 0; mi < MI; ++mi)
-#pragma unroll
-            for (int ni = 0; ni < 4; ++ni) { acc[mi][ni][0] = 0.0; acc[mi][ni][1] = 0.0; }
-        for (int kt = 0; kt < KT; ++kt) {
-            while (!mbar_try_wait(full_bar + 8 * s, use & 1)) { }
-            const uint32_t st = smem + s * STAGE_BYTES;
-#pragma unroll
-            for (int ks = 0; ks < 4; ++ks) {
-                double a[MI], b[4];
-#pragma unroll
-                for (int mi = 0; mi < MI; ++mi) a[mi] = lds64(st + kxA[ks] + mi * BLK);
-#pragma unroll
-                for (int ni = 0; ni < 4; ++ni) b[ni] = lds64(st + kxA[ks] + dB + ni * BLK);
-#pragma unroll
-                for (int mi = 0; mi < MI; ++mi)
-#pragma unroll
-                    for (int ni = 0; ni < 4; ++ni) dmma884(acc[mi][ni][0], acc[mi][ni][1], a[mi], b[ni]);
-            }
-            __syncwarp();
-            if (lane == 0) mbar_arrive(empty_bar + 8 * s);
-            if (++s == PV_STAGES) { s = 0; ++use; }
-        }
-        // ---- epilogue: column reductions over the tile's 128 rows (same order as gpk_gemm_ws_kernel<EPI_COLREDUCE>)
-        const uint32_t red = red0 + (uint32_t)(t & 1) * (uint32_t)PV_RED_BYTES;
-        const int c_row = ib * BM, c_col = cb * BN;
-        double zr[MI];
-#pragma unroll
-        for (int mi = 0; mi < MI; ++mi) zr[mi] = g.z[c_row + wm * HM + mi * 8 + rowmap<LOADER>(gq)];
-        double ssq[4][2], smu[4][2];
-#pragma unroll
-        for (int ni = 0; ni < 4; ++ni)
-#pragma unroll
-            for (int j = 0; j < 2; ++j) {
-                double s2 = 0.0, sm = 0.0;
-#pragma unroll
-                for (int mi = 0; mi < MI; ++mi) {
-                    double v = acc[mi][ni][j];
-                    s2 = fma(v, v, s2);
-                    sm = fma(v, zr[mi], sm);
-                }
-#pragma unroll
-                for (int off = 4; off < 32; off <<= 1) {
-                    s2 += __shfl_xor_sync(0xffffffffu, s2, off);
-                    sm += __shfl_xor_sync(0xffffffffu, sm, off);
-                }
-                ssq[ni][j] = s2; smu[ni][j] = sm;
-            }
-        if (gq == 0) {
-#pragma unroll
-            for (int ni = 0; ni < 4; ++ni)
-#pragma unroll
-                for (int j = 0; j < 2; ++j) {
-                    const int c = wn * 32 + ni * 8 + rowmap<LOADER>(2 * tq + j);
-                    sts64(red + 8 * (wm * 128 + c), ssq[ni][j]);
-                    sts64(red + 8 * (256 + wm * 128 + c), smu[ni][j]);
-                }
-        }
-        named_bar_sync(1, GEMM_THREADS);
-        if (tid < 128) {
-            g.part_ssq[(long)ib * g.ldpart + c_col + tid] = lds64(red + 8 * tid) + lds64(red + 8 * (128 + tid));
-        } else {
-            const int c = tid - 128;
-            g.part_mu[(long)ib * g.ldpart + c_col + c] = lds64(red + 8 * (256 + c)) + lds64(red + 8 * (384 + c));
-        }
-        // `red` is double-buffered by tile parity: the barrier of the next tile's epilogue orders this tile's reads
-        // before the writes of the tile after next
-    }
-}

@@ -230,7 +230,6 @@ struct FinishArgs {
     double* out_mu; double* out_var; double* out_acq;    // chunk-local device arrays, may be NULL
     BestPair* block_best;   // one per block
     unsigned long long* n_negative;
-    const double* mu_direct; // when set: mean - f.mean = K* alpha computed in fp64 beside the int8 variance contraction
 };
 
 __global__ void __launch_bounds__(256) gpk_finish_kernel(const FinishArgs f)
@@ -240,14 +239,9 @@ __global__ void __launch_bounds__(256) gpk_finish_kernel(const FinishArgs f)
     long long idx = -1;
     if (c < f.m) {
         double ssq = 0.0, mu = 0.0;
-        if (f.mu_direct != nullptr) {
-            for (int p = 0; p < f.nparts; ++p) ssq += f.part_ssq[(long)p * f.ldpart + c];
-            mu = f.mu_direct[c];
-        } else {
-            for (int p = 0; p < f.nparts; ++p) {
-                ssq += f.part_ssq[(long)p * f.ldpart + c];
-                mu += f.part_mu[(long)p * f.ldpart + c];
-            }
+        for (int p = 0; p < f.nparts; ++p) {
+            ssq += f.part_ssq[(long)p * f.ldpart + c];
+            mu += f.part_mu[(long)p * f.ldpart + c];
         }
         double var = f.kss - ssq;
         mu += f.mean;

@@ -363,17 +363,15 @@ gpk_cov_oz_kernel(const __grid_constant__ CUtensorMap mapX, const KSpec ks, int 
                   const double* __restrict__ cand, int dc, long m,
                   const double* __restrict__ lower, const double* __restrict__ upper,
                   const double* __restrict__ alpha, int eK, int8_t* __restrict__ Kq, long ldq, long slice_stride,
-                  double* __restrict__ part_mu, long ldpart, int gx, int gy, int trigger)
+                  double* __restrict__ part_mu, long ldpart, int gx)
 {
-    // trigger: this grid is the PRIMARY of a programmatic dependent launch (score_dev): all its CTAs are resident, so the
-    // int8 contraction of the previous chunk, launched right behind it on the same stream, may start now and run beside it
-    if (trigger) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-    // Work items (train tile bx of 128 columns, candidate group by of 4 CC rows) are walked with stride gridDim.x: a grid of
-    // gx * gy CTAs does one item each; the look-ahead launch uses one or two CTAs per SM (see score_dev: they are
-    // resident before the contraction's CTAs arrive, which is what lets the two kernels overlap).
+    // one CTA per (train tile bx of 128 columns, candidate group of 4 CC rows): a 1-D grid of gx x (candidate groups)
     constexpr int TC = 4 * CC;
     extern __shared__ unsigned char cov_raw[];
     const int tid = threadIdx.x;
+    const long w = blockIdx.x;
+    const int bx = (int)(w % gx);
+    const long c0 = (w / gx) * TC;
     const int nt = ks.n_terms;
     const uint32_t base = (cov_smem_u32(cov_raw) + 127u) & ~127u;
     const uint32_t xs = base;                                   // nt x 128 doubles
@@ -384,93 +382,84 @@ gpk_cov_oz_kernel(const __grid_constant__ CUtensorMap mapX, const KSpec ks, int 
         asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(bar) : "memory");
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(bar), "r"((uint32_t)nt * 1024u) : "memory");
+        asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
+                     :: "r"(xs), "l"((uint64_t)&mapX), "r"(bar), "r"(bx * 128), "r"(0) : "memory");
     }
-    __syncthreads();
     const int jp = tid & 63, cgp = tid >> 6, lane = tid & 31;
     const double sc = ldexp(1.0, -eK);
-    uint32_t phase = 0;
-    for (long w = blockIdx.x; w < (long)gx * gy; w += gridDim.x, phase ^= 1u) {
-        const int bx = (int)(w % gx);
-        const long c0 = (w / gx) * TC;
-        if (tid == 0) {
-            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(bar), "r"((uint32_t)nt * 1024u) : "memory");
-            asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-                         :: "r"(xs), "l"((uint64_t)&mapX), "r"(bar), "r"(bx * 128), "r"(0) : "memory");
+    for (int e = tid; e < TC * nt; e += 256) {
+        const int c = e / nt, t = e - c * nt;
+        const long ci = c0 + c;
+        double v = 0.0;
+        if (ci < m) {
+            const int a = ks.axis[t];
+            v = cand[ci * dc + a];
+            if (lower != nullptr) v = (v - lower[a]) / (upper[a] - lower[a]);
+            v *= ks.scale[t];
         }
-        for (int e = tid; e < TC * nt; e += 256) {
-            const int c = e / nt, t = e - c * nt;
-            const long ci = c0 + c;
-            double v = 0.0;
-            if (ci < m) {
-                const int a = ks.axis[t];
-                v = cand[ci * dc + a];
-                if (lower != nullptr) v = (v - lower[a]) / (upper[a] - lower[a]);
-                v *= ks.scale[t];
-            }
-            asm volatile("st.shared.f64 [%0], %1;" :: "r"(scb + (uint32_t)e * 8u), "d"(v) : "memory");
-        }
-        __syncthreads();
-        {
-            uint32_t ok = 0;
-            while (!ok)
-                asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                             : "=r"(ok) : "r"(bar), "r"(phase) : "memory");
-        }
-        double q[CC][2], pr[CC][2];
+        asm volatile("st.shared.f64 [%0], %1;" :: "r"(scb + (uint32_t)e * 8u), "d"(v) : "memory");
+    }
+    __syncthreads();
+    {
+        uint32_t ok = 0;
+        while (!ok)
+            asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], 0;\n\tselp.u32 %0, 1, 0, p;\n\t}"
+                         : "=r"(ok) : "r"(bar) : "memory");
+    }
+    double q[CC][2], pr[CC][2];
 #pragma unroll
-        for (int c = 0; c < CC; ++c) { q[c][0] = q[c][1] = 0.0; pr[c][0] = pr[c][1] = 1.0; }
-        const uint32_t xrow = xs + (uint32_t)jp * 16u;
-        const uint32_t srow = scb + (uint32_t)(cgp * CC * nt) * 8u;
-        for (int t = 0; t < nt; ++t) {
-            double x0, x1;
-            asm volatile("ld.shared.v2.f64 {%0, %1}, [%2];" : "=d"(x0), "=d"(x1) : "r"(xrow + (uint32_t)t * 1024u));
-#pragma unroll
-            for (int c = 0; c < CC; ++c) {
-                double sv;
-                asm volatile("ld.shared.f64 %0, [%1];" : "=d"(sv) : "r"(srow + (uint32_t)(c * nt + t) * 8u));
-                const double d0 = sv - x0, d1 = sv - x1;
-                q[c][0] = fma(d0, d0, q[c][0]);
-                q[c][1] = fma(d1, d1, q[c][1]);
-            }
-            if (ks.last[t]) {
-#pragma unroll
-                for (int c = 0; c < CC; ++c) {
-                    pr[c][0] *= gpk_radial_q(ks.family, q[c][0]);
-                    pr[c][1] *= gpk_radial_q(ks.family, q[c][1]);
-                    q[c][0] = q[c][1] = 0.0;
-                }
-            }
-        }
-        const int j0 = bx * 128 + 2 * jp;
-        const bool v0 = j0 < n, v1 = j0 + 1 < n;
-        const double a0 = v0 ? alpha[j0] : 0.0, a1 = v1 ? alpha[j0 + 1] : 0.0;
+    for (int c = 0; c < CC; ++c) { q[c][0] = q[c][1] = 0.0; pr[c][0] = pr[c][1] = 1.0; }
+    const uint32_t xrow = xs + (uint32_t)jp * 16u;
+    const uint32_t srow = scb + (uint32_t)(cgp * CC * nt) * 8u;
+    for (int t = 0; t < nt; ++t) {
+        double x0, x1;
+        asm volatile("ld.shared.v2.f64 {%0, %1}, [%2];" : "=d"(x0), "=d"(x1) : "r"(xrow + (uint32_t)t * 1024u));
 #pragma unroll
         for (int c = 0; c < CC; ++c) {
-            const long ci = c0 + cgp * CC + c;
-            const bool cv = ci < m;
-            const double k0 = (cv && v0) ? ks.amp * pr[c][0] : 0.0;
-            const double k1 = (cv && v1) ? ks.amp * pr[c][1] : 0.0;
-            // digits: two adjacent int8 per slice
-            const unsigned long long y0 = oz_digits(k0 * sc), y1 = oz_digits(k1 * sc);
-            int8_t* dst = Kq + ci * ldq + j0;
-#pragma unroll
-            for (int s2 = 0; s2 < OZ_S; ++s2)
-                *reinterpret_cast<uint16_t*>(dst + (long)s2 * slice_stride) = (uint16_t)(oz_digit_of(y0, s2) | (oz_digit_of(y1, s2) << 8));
-            // mean share of this tile: reduce over the 64 threads (2 warps) of the candidate group, fixed order
-            double pm = fma(k0, a0, k1 * a1);
-#pragma unroll
-            for (int off = 16; off > 0; off >>= 1) pm += __shfl_xor_sync(0xffffffffu, pm, off);
-            if (lane == 0) asm volatile("st.shared.f64 [%0], %1;" :: "r"(mred + (uint32_t)(((tid >> 5) * CC + c) * 8)), "d"(pm) : "memory");
+            double sv;
+            asm volatile("ld.shared.f64 %0, [%1];" : "=d"(sv) : "r"(srow + (uint32_t)(c * nt + t) * 8u));
+            const double d0 = sv - x0, d1 = sv - x1;
+            q[c][0] = fma(d0, d0, q[c][0]);
+            q[c][1] = fma(d1, d1, q[c][1]);
         }
-        __syncthreads();
-        if (tid < TC) {
-            const int g = tid / CC, c = tid - g * CC;           // candidate group g = warps 2g, 2g + 1
-            double lo2, hi2;
-            asm volatile("ld.shared.f64 %0, [%1];" : "=d"(lo2) : "r"(mred + (uint32_t)(((2 * g) * CC + c) * 8)));
-            asm volatile("ld.shared.f64 %0, [%1];" : "=d"(hi2) : "r"(mred + (uint32_t)(((2 * g + 1) * CC + c) * 8)));
-            part_mu[(long)bx * ldpart + c0 + tid] = lo2 + hi2;
+        if (ks.last[t]) {
+#pragma unroll
+            for (int c = 0; c < CC; ++c) {
+                pr[c][0] *= gpk_radial_q(ks.family, q[c][0]);
+                pr[c][1] *= gpk_radial_q(ks.family, q[c][1]);
+                q[c][0] = q[c][1] = 0.0;
+            }
         }
-        __syncthreads();                                        // the next item overwrites the operand tiles and mred
+    }
+    const int j0 = bx * 128 + 2 * jp;
+    const bool v0 = j0 < n, v1 = j0 + 1 < n;
+    const double a0 = v0 ? alpha[j0] : 0.0, a1 = v1 ? alpha[j0 + 1] : 0.0;
+#pragma unroll
+    for (int c = 0; c < CC; ++c) {
+        const long ci = c0 + cgp * CC + c;
+        const bool cv = ci < m;
+        const double k0 = (cv && v0) ? ks.amp * pr[c][0] : 0.0;
+        const double k1 = (cv && v1) ? ks.amp * pr[c][1] : 0.0;
+        // digits: two adjacent int8 per slice
+        const unsigned long long y0 = oz_digits(k0 * sc), y1 = oz_digits(k1 * sc);
+        int8_t* dst = Kq + ci * ldq + j0;
+#pragma unroll
+        for (int s2 = 0; s2 < OZ_S; ++s2)
+            *reinterpret_cast<uint16_t*>(dst + (long)s2 * slice_stride) = (uint16_t)(oz_digit_of(y0, s2) | (oz_digit_of(y1, s2) << 8));
+        // mean share of this tile: reduce over the 64 threads (2 warps) of the candidate group, fixed order
+        double pm = fma(k0, a0, k1 * a1);
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) pm += __shfl_xor_sync(0xffffffffu, pm, off);
+        if (lane == 0) asm volatile("st.shared.f64 [%0], %1;" :: "r"(mred + (uint32_t)(((tid >> 5) * CC + c) * 8)), "d"(pm) : "memory");
+    }
+    __syncthreads();
+    if (tid < TC) {
+        const int g = tid / CC, c = tid - g * CC;               // candidate group g = warps 2g, 2g + 1
+        double lo2, hi2;
+        asm volatile("ld.shared.f64 %0, [%1];" : "=d"(lo2) : "r"(mred + (uint32_t)(((2 * g) * CC + c) * 8)));
+        asm volatile("ld.shared.f64 %0, [%1];" : "=d"(hi2) : "r"(mred + (uint32_t)(((2 * g + 1) * CC + c) * 8)));
+        part_mu[(long)bx * ldpart + c0 + tid] = lo2 + hi2;
     }
 }
 inline size_t cov_oz_smem_bytes(int n_terms, int cc) { return (size_t)n_terms * 1024 + (size_t)4 * cc * n_terms * 8 + 8 + 8 * cc * 8 + 128; }

@@ -202,10 +202,11 @@ def test_contract_leaves_a_fitted_model_untouched():
 
 @pytest.mark.skipif(os.environ.get("GPK_OZAKI") == "0", reason="GPK_OZAKI=0 runs the fp64 contraction in gpk_acq")
 @pytest.mark.parametrize("transform", [False, True])
-def test_acq_variance_equals_model(transform):
+def test_acq_variance_equals_model_with_and_without_lookahead(transform):
     """The production path: L^-1 from get_linv and K* from kernel_matrix (the same covariance builder and train operand
-    as scoring; the fused builder's digits equal the un-fused ones) through the model give gpk_acq's variances bit for
-    bit, over several chunks with both K* buffers, every builder / launch arrangement and the output transform."""
+    as scoring; the model splits that fp64 K* into the digits the int8 builder writes itself) through the model give
+    gpk_acq's variances bit for bit, over several chunks with both K* buffers, the look-ahead builder on the side stream
+    and the serial schedule, and the output transform."""
     from robo_b200 import _lib
     N, D, m, chunk = 640, 5, 10000, 2048
     h, X, y, rng, amp = _fitted(N, D, 640 + transform, transform)
@@ -216,15 +217,11 @@ def test_acq_variance_equals_model(transform):
     var_ref = M.finish(M.contract(Linv, Ks[cols], amp)["part_ssq"], amp, 1.7 if transform else None)
     h.set_option("chunk", chunk)
     launches = 0
-    for fused in (0, 1):
-        for pdl in (0, 1):
-            for overlap in (0, 1):
-                h.set_option("ozfused", fused)
-                h.set_option("ozpdl", pdl)
-                h.set_option("overlap", overlap)
-                r = h.acq(Xs, _lib.ACQ_EI, float(np.min(y)), 0.0, want_values=True, want_moments=True)
-                t = h.timings()
-                assert t["launches_ozaki"] >= launches + 5, t                # one int8 launch per chunk, no fall-back
-                launches = t["launches_ozaki"]
-                np.testing.assert_array_equal(r["var"][cols], var_ref, err_msg=str((fused, pdl, overlap)))
+    for overlap in (0, 1):
+        h.set_option("overlap", overlap)
+        r = h.acq(Xs, _lib.ACQ_EI, float(np.min(y)), 0.0, want_values=True, want_moments=True)
+        t = h.timings()
+        assert t["launches_ozaki"] >= launches + 5, t                        # one int8 launch per chunk, no fall-back
+        launches = t["launches_ozaki"]
+        np.testing.assert_array_equal(r["var"][cols], var_ref, err_msg="overlap %d" % overlap)
     h.close()

@@ -21,7 +21,7 @@ y = np.sinc(X * 10 - 5).sum(axis=1) + 0.01 * rng.randn(N)
 theta = np.concatenate(([0.0], np.full(D, np.log(D / 4.0))))
 dX = torch.rand(M, D, dtype=torch.float64, device="cuda")
 out = {}
-for label, opts in (("overlap", {}), ("no_overlap", {"overlap": 0}), ("overlap_unfused", {"ozfused": 0}),
+for label, opts in (("overlap", {}), ("no_overlap", {"overlap": 0}),
                     ("fp64_overlap", {"ozaki": 0}), ("fp64_no_overlap", {"ozaki": 0, "overlap": 0})):
     h = _lib.Handle(0)
     for k, v in opts.items():

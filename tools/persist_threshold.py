@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Scoring time per pass with and without the persistent tile walk, per training-set size: options "ozpersist" and
-"ozcluster" of the int8 contraction (which N should the automatic mode switch at, for which cluster size?) and option
-"persist" of the fp64 contraction ("ozaki" = 0).    python tools/persist_threshold.py"""
+"ozcluster" of the int8 contraction (which N should the automatic mode switch at, for which cluster size?), next to
+the fp64 contraction ("ozaki" = 0, one CTA per tile).    python tools/persist_threshold.py"""
 import json
 import os
 import sys
@@ -26,7 +26,7 @@ for N, M in ((512, 524288), (1024, 524288), (1536, 262144), (2048, 262144), (307
     row = {}
     configs = [("int8_cluster%d_%s" % (cs, "persistent" if p else "one_tile_per_cta"), {"ozcluster": cs, "ozpersist": p})
                for cs in (1, 2, 4) for p in (0, 1)]
-    configs += [("fp64_one_tile_per_cta", {"ozaki": 0, "persist": 0}), ("fp64_persistent", {"ozaki": 0, "persist": 1})]
+    configs += [("fp64_one_tile_per_cta", {"ozaki": 0})]
     for name, opts in configs:
         h = _lib.Handle(0)
         for k, v in opts.items():

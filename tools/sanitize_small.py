@@ -33,19 +33,18 @@ for loader in (2, 1, 0):
     X2, y2 = np.vstack([X, rng.rand(10, D)]), np.concatenate([y, rng.rand(10)])
     print(" append", h.fit_append(X2, y2, 1e-3 + 1.25e-12, float(y2.mean())), h.predict(Xs[:64])[0][:2])
     h.close()
-# round-2 kernels: int8 contraction (fused and unfused digit builders, several chunks), persistent fp64 contraction,
-# split chain replayed from a CUDA graph, depth-2 trailing updates, fused multi-model scoring, raw posterior covariance
+# round-2 kernels: int8 contraction (digit builder, several chunks), split chain replayed from a CUDA graph, depth-2
+# trailing updates, fused multi-model scoring, raw posterior covariance
 Xb = rng.rand(2304, D)
 hs = []
-for opts in ({"ozaki": 1, "ozfused": 1}, {"ozaki": 1, "ozfused": 0}, {"ozaki": 0, "persist": 1},
-             {"ozaki": 0, "chainsplit": 1, "graph": 1, "depth2": 1},
-             # int8 contraction variants: one tile per CTA / persistent walk / resident builder + dependent launch
-             {"ozaki": 1, "ozpersist": 0}, {"ozaki": 1, "ozpersist": 1}, {"ozaki": 1, "ozpdl": 1}):
+for opts in ({"ozaki": 1}, {"ozaki": 0, "chainsplit": 1, "graph": 1, "depth2": 1},
+             # int8 contraction variants: one tile per CTA / persistent walk
+             {"ozaki": 1, "ozpersist": 0}, {"ozaki": 1, "ozpersist": 1}):
     h = _lib.Handle(0)
     for k, v in opts.items():
         h.set_option(k, v)
     h.set_option("chunk", 1024)
-    Xt, yt = (X, y) if len(hs) < 4 else (X[:250], y[:250])       # 250 rows = 2 row blocks: the CTA-pair kernels apply
+    Xt, yt = (X, y) if len(hs) < 2 else (X[:250], y[:250])       # 250 rows = 2 row blocks: the CTA-pair kernels apply
     h.set_data(Xt, yt)
     h.set_kernel(f["family"], f["log_amp"], f["axis"], f["group"], f["log_metric"])
     for _ in range(2):
@@ -55,8 +54,8 @@ for opts in ({"ozaki": 1, "ozfused": 1}, {"ozaki": 1, "ozfused": 0}, {"ozaki": 0
     print(opts, "fit", ll, "best", r["best_idx"], "oz launches", t["launches_ozaki"], "variant", t["ozaki_kernel_variant"])
     mu, cov = h.posterior_cov(Xs[:100])
     hs.append(h)
-rm = _lib.acq_multi(hs[:3], Xs[:300], 0, _lib.ACQ_EI, [float(y.min())] * 3, 0.0, want_argmax=True)
-rp = _lib.acq_multi(hs[:3], Xs[:300], 1)
+rm = _lib.acq_multi(hs[:2], Xs[:300], 0, _lib.ACQ_EI, [float(y.min())] * 2, 0.0, want_argmax=True)
+rp = _lib.acq_multi(hs[:2], Xs[:300], 1)
 print("multi", rm["best_idx"], rp["var"][:2])
 for h in hs:
     h.close()
