@@ -94,7 +94,10 @@ const char* gpk_version(void);
  *               0 = plain look-ahead schedule [default] (bit-identical factor)
  *   "diagprof"  1 = the diagonal-block kernel records clock64() stamps per phase (gpk_get_diag_profile)
  *   "pdl"       1 = programmatic dependent launch for the kernels of the Cholesky chain [default]
- *   "overlap"   1 = build K* of chunk i+1 on the side stream while chunk i contracts [default] */
+ *   "overlap"   1 = build K* of chunk i+1 on the side stream while chunk i contracts [default]
+ *   "meanonly"  1 = gpk_predict_mean (and the cost models of gpk_es_cost_multi) run the mean-only builder pass [default];
+ *               0 = they take the mean of the full scoring pass, variance contraction included (tools/fabolas_acq_bench.py
+ *               compares the two) */
 int gpk_set_option(gpk_handle* h, const char* key, long value);
 /* run on an existing CUDA stream (cudaStream_t passed as void*); NULL = the handle's own.  The handle's own stream has
  * the highest priority and its side stream (trailing updates, K* look-ahead) the lowest: give an external stream a high
@@ -153,6 +156,16 @@ int gpk_fit_append(gpk_handle* h, const double* X, const double* y, int n, int d
 /* Replaces george GP.predict + np.diag + clip (gaussian_process.py:276-294):
  * mu[m], var[m] (var clipped to >= DBL_EPSILON).  Xs is (m, d) row-major, raw (un-scaled). */
 int gpk_predict(gpk_handle* h, const double* Xs, long m, double* mu, double* var);
+
+/* The predictive mean alone: predict(X)[0], as the cost model of InformationGainPerUnitCost uses it
+ * (robo/acquisition_functions/information_gain_per_unit_cost.py:91).  Runs the int8 path's covariance builder with its
+ * digit stores compiled out and sums the per-tile shares of K* alpha in the same fixed order, alpha = L^-T z built once
+ * per fit: mu is bit-identical to gpk_predict's wherever gpk_predict takes the int8 path (option "ozaki", m >= 2048),
+ * and within rounding of its fp64 path elsewhere; no variance work.  Xs (m, d) raw inputs, m >= 1; mu (m).
+ * GPK_BAD_ARG under option "loader" = 0 (the builder needs TMA), GPK_NOT_FITTED before gpk_fit. */
+int gpk_predict_mean(gpk_handle* h, const double* Xs, long m, double* mu);
+/* the same on device pointers (d_Xs: m x d, d_mu: m doubles), asynchronous on the handle's stream */
+int gpk_predict_mean_dev(gpk_handle* h, const void* d_Xs, long m, void* d_mu);
 
 /* full_cov=True path (gaussian_process.py:280-294): cov is (m, m) row-major, every entry
  * clipped to >= DBL_EPSILON like the reference does. */
@@ -284,6 +297,48 @@ int gpk_es_update(gpk_handle* h, const double* zb, int nb, const double* lmb, do
 int gpk_es_compute(gpk_handle* h, const double* Xs, long m, double* out);
 /* the same on device pointers (d_Xs: m x d, d_out: m doubles), asynchronous on the handle's stream */
 int gpk_es_compute_dev(gpk_handle* h, const void* d_Xs, long m, void* d_out);
+
+/* basis functions of the environment column of Fabolas models (robo/fmin/fabolas.py:96-102) */
+typedef enum {
+    GPK_BASIS_S = 0,           /* basis(s) = s          (the cost model)      */
+    GPK_BASIS_ONE_MINUS_S_SQ = 1   /* basis(s) = (1 - s)^2  (the objective model) */
+} gpk_basis;
+
+/* InformationGainPerUnitCost.compute (robo/acquisition_functions/information_gain_per_unit_cost.py:67-106) over n
+ * (objective, cost) pairs of Fabolas models, averaged as MarginalizationGPMCMC.compute does (marginalization.py:115-121):
+ *   out[c] = mean_i dh_i(x_c) / (exp(mu_i(x_c)) + overhead)
+ * Xs (m x d) raw candidates: d - 1 configuration columns and the environment column last.  On the device the batch is
+ * mapped as FabolasGP.normalize maps it (fabolas_gp.py:122-126): configuration columns to (x - lower) / (upper - lower),
+ * the environment column through the family's basis (basis_objective / basis_cost, gpk_basis), bit-identical to numpy.
+ * dh_i is gpk_es_compute of objective[i] on the transformed batch, except that its bounds test sees the RAW candidate
+ * against the [lower, upper] given to gpk_es_update (DBL_EPSILON outside, NaN / +inf -> -DBL_MAX); mu_i is
+ * gpk_predict_mean of cost[i] on the transformed batch.  -DBL_MAX / c overflows to -inf for c < 1, as in numpy.  The mean
+ * over pairs is summed in index order (gpk_reduce_models mode 0); n = 1 returns the ratio itself.  Every handle runs on
+ * its own stream; the values do not depend on "chunk", on stream timing or on whether the batch came from the host.
+ * lower / upper (n_bounds = d - 1 entries each): the configuration bounds of the models' transform.  out (m) and best_val / best_idx
+ * (numpy.argmax of out) may be NULL.  GPK_BAD_ARG: n < 1, m < 1, a basis code out of range, lower >= upper, handles on
+ * different devices or with different input dimensions, a handle listed twice (objective and cost lists together), an
+ * objective handle without a current gpk_es_update (or changed since), a cost handle under option "loader" = 0. */
+int gpk_es_cost_multi(gpk_handle* const* objective, gpk_handle* const* cost, int n, const double* Xs, long m,
+                      const double* lower, const double* upper, int n_bounds, int basis_objective, int basis_cost,
+                      double overhead,
+                      double* out, double* best_val, long* best_idx);
+/* the same on a device batch (d_Xs: m x d), asynchronous on objective[0]'s stream: d_out (m doubles) is required,
+ * d_best (16 bytes {double value; long long index}) may be NULL.  lower / upper are host arrays. */
+int gpk_es_cost_multi_dev(gpk_handle* const* objective, gpk_handle* const* cost, int n, const void* d_Xs, long m,
+                          const double* lower, const double* upper, int n_bounds, int basis_objective, int basis_cost,
+                          double overhead,
+                          void* d_out, void* d_best);
+/* RandomSampling.maximize of that acquisition (robo/maximizers/random_sampling.py:38-50) on one GPU: count candidates
+ * from gpk_generate_candidates's Philox stream in [box_lower, box_upper] (d each; the first n_uniform uniform, the rest
+ * clip(incumbent + scale N(0, 1)^d)), scored by gpk_es_cost_multi; only the winner (best_x, d), its value and its index
+ * cross PCIe.  The arguments otherwise as for gpk_es_cost_multi; GPK_BAD_ARG when any objective or cost handle has a
+ * multi-rank communicator. */
+int gpk_maximize_random_es_cost(gpk_handle* const* objective, gpk_handle* const* cost, int n, unsigned long long seed,
+                                long count, long n_uniform, const double* box_lower, const double* box_upper,
+                                const double* incumbent, double scale, const double* lower, const double* upper,
+                                int n_bounds, int basis_objective, int basis_cost, double overhead, double* best_x, double* best_val,
+                                long* best_idx);
 
 /* kernel.get_value(X1, X2) (test/test_models/test_gaussian_process.py:44-46) with the
  * handle's current kernel; no input scaling.  out is (n1, n2) row-major. */

@@ -19,6 +19,7 @@ GPK_OK, GPK_NOT_PD, GPK_BAD_ARG, GPK_CUDA_ERROR, GPK_NOT_FITTED, GPK_NOT_APPLICA
 MATERN52, EXPSQUARED, MATERN32 = 0, 1, 2
 ACQ_NONE, ACQ_EI, ACQ_LOG_EI, ACQ_PI, ACQ_LCB = range(5)
 ACQ_KIND = {"ei": ACQ_EI, "log_ei": ACQ_LOG_EI, "pi": ACQ_PI, "lcb": ACQ_LCB, "none": ACQ_NONE}
+BASIS_S, BASIS_ONE_MINUS_S_SQ = range(2)      # gpk_basis: the environment column's basis of a Fabolas model
 
 _dp = C.POINTER(C.c_double)
 _ip = C.POINTER(C.c_int)
@@ -76,6 +77,14 @@ _SIGNATURES = {
     "gpk_es_update": [_vp, _dp, C.c_int, _dp, C.c_double, _dp, C.c_int, _dp, _dp, _dp, _dp, _dp, _dp],
     "gpk_es_compute": [_vp, _dp, C.c_long, _dp],
     "gpk_es_compute_dev": [_vp, _vp, C.c_long, _vp],
+    "gpk_predict_mean": [_vp, _dp, C.c_long, _dp],
+    "gpk_predict_mean_dev": [_vp, _vp, C.c_long, _vp],
+    "gpk_es_cost_multi": [C.POINTER(_vp), C.POINTER(_vp), C.c_int, _dp, C.c_long, _dp, _dp, C.c_int, C.c_int, C.c_int,
+                          C.c_double, _dp, _dp, _lp],
+    "gpk_es_cost_multi_dev": [C.POINTER(_vp), C.POINTER(_vp), C.c_int, _vp, C.c_long, _dp, _dp, C.c_int, C.c_int, C.c_int,
+                              C.c_double, _vp, _vp],
+    "gpk_maximize_random_es_cost": [C.POINTER(_vp), C.POINTER(_vp), C.c_int, C.c_ulonglong, C.c_long, C.c_long, _dp, _dp,
+                                    _dp, C.c_double, _dp, _dp, C.c_int, C.c_int, C.c_int, C.c_double, _dp, _dp, _lp],
     "gpk_get_timings": [_vp, _dp],
     "gpk_get_diag_profile": [_vp, C.POINTER(C.c_longlong)],
 }
@@ -485,6 +494,16 @@ class Handle(object):
     def es_compute_dev(self, d_Xs_ptr, m, d_out_ptr):
         self._check(self.lib.gpk_es_compute_dev(self._h, _vp(d_Xs_ptr), int(m), _vp(d_out_ptr)))
 
+    def predict_mean(self, Xs):
+        """gpk_predict_mean: the predictive mean alone of every row of Xs (m, d) -> (m,)."""
+        Xs = f64(Xs)
+        mu = np.empty(Xs.shape[0])
+        self._check(self.lib.gpk_predict_mean(self._h, _as_dp(Xs), Xs.shape[0], _as_dp(mu)))
+        return mu
+
+    def predict_mean_dev(self, d_Xs_ptr, m, d_mu_ptr):
+        self._check(self.lib.gpk_predict_mean_dev(self._h, _vp(d_Xs_ptr), int(m), _vp(d_mu_ptr)))
+
     def diag_profile(self):
         t = np.zeros(64, dtype=np.int64)
         self._check(self.lib.gpk_get_diag_profile(self._h, t.ctypes.data_as(C.POINTER(C.c_longlong))))
@@ -558,6 +577,59 @@ def maximize_de(handles, seed, pop, maxiter, mutation, recombination, tol, atol,
     if want_population:
         r.update(population=P, energies=E)
     return r
+
+
+def _es_cost_args(objective, cost, lower, upper):
+    if len(objective) == 0 or len(objective) != len(cost):
+        raise ValueError("information gain per unit cost: need as many cost handles as objective handles (>= 1)")
+    ho = (_vp * len(objective))(*[h._h for h in objective])
+    hc = (_vp * len(cost))(*[h._h for h in cost])
+    lo, up = f64(lower).ravel(), f64(upper).ravel()
+    if lo.size != up.size:
+        raise ValueError("information gain per unit cost: lower and upper differ in length")
+    return ho, hc, lo, up
+
+
+def es_cost_multi(objective, cost, Xs, lower, upper, basis_objective, basis_cost, overhead, want_values=True):
+    """gpk_es_cost_multi over the (objective[i], cost[i]) pairs: raw candidates Xs (m, d), configuration bounds
+    lower / upper (d - 1) -> dict(values (m,) or None, best_val, best_idx)."""
+    ho, hc, lo, up = _es_cost_args(objective, cost, lower, upper)
+    h0 = objective[0]
+    Xs = f64(Xs)
+    m = Xs.shape[0]
+    out = np.empty(m) if want_values else None
+    bv, bi = C.c_double(), C.c_long(-1)
+    h0._check(h0.lib.gpk_es_cost_multi(ho, hc, len(objective), _as_dp(Xs), m, _as_dp(lo), _as_dp(up), lo.size,
+                                       int(basis_objective), int(basis_cost), float(overhead),
+                                       _as_dp(out) if want_values else None, C.byref(bv), C.byref(bi)))
+    return dict(values=out, best_val=bv.value, best_idx=bi.value)
+
+
+def es_cost_multi_dev(objective, cost, d_Xs_ptr, m, lower, upper, basis_objective, basis_cost, overhead, d_out_ptr,
+                      d_best_ptr=0):
+    """Device-batch variant, asynchronous on objective[0]'s stream."""
+    ho, hc, lo, up = _es_cost_args(objective, cost, lower, upper)
+    h0 = objective[0]
+    h0._check(h0.lib.gpk_es_cost_multi_dev(ho, hc, len(objective), _vp(d_Xs_ptr), int(m), _as_dp(lo), _as_dp(up),
+                                           lo.size, int(basis_objective), int(basis_cost), float(overhead), _vp(d_out_ptr or 0),
+                                           _vp(d_best_ptr or 0)))
+
+
+def maximize_random_es_cost(objective, cost, seed, count, n_uniform, box_lower, box_upper, incumbent, scale, lower,
+                            upper, basis_objective, basis_cost, overhead):
+    """gpk_maximize_random_es_cost -> (best_x (d,), best_val, best_idx)."""
+    ho, hc, lo, up = _es_cost_args(objective, cost, lower, upper)
+    h0 = objective[0]
+    blo, bup, inc = f64(box_lower).ravel(), f64(box_upper).ravel(), f64(incumbent).ravel()
+    if not blo.size == bup.size == inc.size == lo.size + 1:
+        raise ValueError("maximize_random_es_cost: the box and the incumbent need d entries, the configuration bounds d - 1")
+    bx = np.empty(blo.size)
+    bv, bi = C.c_double(), C.c_long(-1)
+    h0._check(h0.lib.gpk_maximize_random_es_cost(ho, hc, len(objective), int(seed) & 0xFFFFFFFFFFFFFFFF, int(count),
+                                                 int(n_uniform), _as_dp(blo), _as_dp(bup), _as_dp(inc), float(scale),
+                                                 _as_dp(lo), _as_dp(up), lo.size, int(basis_objective), int(basis_cost),
+                                                 float(overhead), _as_dp(bx), C.byref(bv), C.byref(bi)))
+    return bx, bv.value, bi.value
 
 
 _moments_handle = {}

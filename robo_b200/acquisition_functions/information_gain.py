@@ -80,13 +80,20 @@ class InformationGain(BaseAcquisitionFunction):
         if len(self.lmb.shape) == 1:
             self.lmb = self.lmb[:, None]
 
+    # the model's device handle, and zb as that handle takes its inputs (InformationGainPerUnitCost: FabolasGP models)
+    def _device_handle(self, model):
+        return _device_model(model)
+
+    def _device_zb(self):
+        return self.zb
+
     def update(self, model):
         self.model = model
-        handle = _device_model(model)
+        handle = self._device_handle(model)
         self.sn2 = self.model.get_noise()
         self.sample_representer_points()
         self.W = scipy.stats.norm.ppf(np.linspace(1. / (self.Np + 1), 1 - 1. / (self.Np + 1), self.Np))[np.newaxis, :]
-        r = handle.es_update(self.zb, self.lmb, self.sn2, self.W, self.lower, self.upper)
+        r = handle.es_update(self._device_zb(), self.lmb, self.sn2, self.W, self.lower, self.upper)
         self.logP = np.reshape(r["logP"], (self.Nb, 1))
         self.dlogPdMu, self.dlogPdSigma, self.dlogPdMudMu = r["dlogPdMu"], r["dlogPdSigma"], r["dlogPdMudMu"]
 

@@ -45,6 +45,11 @@ class MarginalizationGPMCMC(BaseAcquisitionFunction):
 
     def compute(self, X_test, derivative=False):
         n = len(self.model.models)
+        es = self._es_cost_spec() if not derivative else None
+        if es is not None:
+            # information gain per unit cost over the (objective, cost) sub-model pairs as ONE call (gpk_es_cost_multi)
+            ho, hc, lo, up, bo, bc, oh = es
+            return _lib.es_cost_multi(ho, hc, np.asarray(X_test, dtype=np.float64), lo, up, bo, bc, oh)["values"]
         fused = self._fused_spec() if not derivative else None
         if fused is not None:
             # marginalization.py:115-121 as ONE call: the batch goes to the device once, the n sub-models score it
@@ -62,6 +67,11 @@ class MarginalizationGPMCMC(BaseAcquisitionFunction):
 
     def argmax(self, X_test):
         """numpy.argmax of compute(X_test) taken on the device when the fused path applies."""
+        es = self._es_cost_spec()
+        if es is not None:
+            ho, hc, lo, up, bo, bc, oh = es
+            r = _lib.es_cost_multi(ho, hc, np.asarray(X_test, dtype=np.float64), lo, up, bo, bc, oh, want_values=False)
+            return int(r["best_idx"])
         fused = self._fused_spec()
         if fused is None:
             return int(np.argmax(self.compute(X_test)))
@@ -71,6 +81,16 @@ class MarginalizationGPMCMC(BaseAcquisitionFunction):
         if kind == "ei" and r["n_negative"] > 0:
             raise ValueError("Expected Improvement is smaller than 0!")
         return int(r["best_idx"])
+
+    def _es_cost_spec(self):
+        """The fused call's arguments (information_gain_per_unit_cost.device_spec) when every estimator is an
+        InformationGainPerUnitCost; estimator i pairs objective sub-model i with cost sub-model i."""
+        from robo_b200.acquisition_functions.information_gain_per_unit_cost import (InformationGainPerUnitCost,
+                                                                                    device_spec)
+        if self.cost_model is None or len(self.estimators) == 0 or \
+                not all(isinstance(e, InformationGainPerUnitCost) for e in self.estimators):
+            return None
+        return device_spec(self.estimators)
 
     def _fused_spec(self):
         """(kind, eta per model, par, handles) when every estimator is a closed-form acquisition on a device GP."""

@@ -120,6 +120,7 @@ struct gpk_handle {
     long mapKs2_rows = 0;
     std::vector<cudaEvent_t> ev_cov, ev_gemm;
     int overlap = 1;                // build K* of chunk i+1 on the side stream while chunk i contracts
+    int mean_only = 1;              // gpk_predict_mean: 1 = mean-only builder pass [default]; 0 = the full scoring pass
     bool maps_ok = false;
     long mapKs_rows = 0, mapVt_rows = 0;
 
@@ -144,6 +145,9 @@ struct gpk_handle {
     DevBuf ep_buf;                  // scratch of gpk_ep_joint_min (operands, raw and renormalised outputs, status)
     // entropy search (gpk_es_update / gpk_es_compute): EP state, W, bounds, scaled zb, U = K^-1 K(X, zb), per-chunk v, sigma
     DevBuf es_state, es_U, es_work, es_in;
+    // information gain per unit cost (gpk_es_cost_multi): the batch under the objective's and the cost's Fabolas
+    // transform and the configuration bounds; owned by the first objective handle of the call
+    DevBuf fab_in;
     int es_nb = 0, es_np = 0;
     double es_sn2 = 0.0, es_H = 0.0;
     long es_linv_serial = -1;       // linv_serial U was built for (-1: no update yet)
@@ -439,6 +443,7 @@ int set_kernel_attrs(gpk_handle* h) {
     CK(cudaFuncSetAttribute(gpk_oz_vargemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, OZ_SMEM));
     CK(cudaFuncSetAttribute(gpk_cov_oz_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cov_oz_smem_bytes(GPK_MAX_TERMS, 8)));
     CK(cudaFuncSetAttribute(gpk_cov_oz_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cov_oz_smem_bytes(GPK_MAX_TERMS, 4)));
+    CK(cudaFuncSetAttribute(gpk_cov_oz_kernel<8, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cov_oz_smem_bytes(GPK_MAX_TERMS, 8)));
     {
         cudaDeviceProp prop;
         CK(cudaGetDeviceProperties(&prop, h->device));
@@ -751,6 +756,21 @@ int build_linv(gpk_handle* h) {
     CK(cudaEventRecord(h->ev[5], h->stream));
     h->linv_ready = true;
     h->linv_serial += 1;
+    h->alpha_ready = false;
+    return GPK_OK;
+}
+
+// alpha = L^-T z (Q = L^-T is upper triangular), once per factorisation: the posterior mean is mu - mean = K* alpha.
+// Needs L^-1 (build_linv).
+int ensure_alpha(gpk_handle* h) {
+    if (h->alpha_ready) return GPK_OK;
+    const long NP = h->NP;
+    int rc;
+    if ((rc = ensure(h, h->alpha, (size_t)NP * 8))) return rc;
+    gpk_rowdot_kernel<<<(unsigned)((NP + 7) / 8), 256, 0, h->stream>>>(ptr<double>(h->Q), NP, NP, (int)NP, 1,
+                                                                       ptr<double>(h->Kbuf) + NP * NP, ptr<double>(h->alpha));
+    CKL();
+    h->alpha_ready = true;
     return GPK_OK;
 }
 
@@ -787,11 +807,8 @@ int prepare_ozaki(gpk_handle* h, bool* usable) {
         gpk_oz_split_kernel<<<(unsigned)((NP * NP + 255) / 256), 256, 0, h->stream>>>(ptr<double>(h->P), NP, NP, ptr<int>(h->oz_eP), 0,
                                                                                    ptr<int8_t>(h->oz_Pq), NP * NP);
         CKL();
-        // alpha = L^-T z (Q = L^-T is upper triangular): the mean goes through fp64, mu - mean = K* alpha
-        if ((rc = ensure(h, h->alpha, (size_t)NP * 8))) return rc;
-        gpk_rowdot_kernel<<<(unsigned)((NP + 7) / 8), 256, 0, h->stream>>>(ptr<double>(h->Q), NP, NP, (int)NP, 1,
-                                                                           ptr<double>(h->Kbuf) + NP * NP, ptr<double>(h->alpha));
-        CKL();
+        // the mean goes through fp64, mu - mean = K* alpha
+        if ((rc = ensure_alpha(h))) return rc;
         CK(cudaMemcpyAsync(&h->oz_emax_host, h->oz_emax.p, 4, cudaMemcpyDeviceToHost, h->stream));
         CK(cudaStreamSynchronize(h->stream));
         h->oz_map_cs = 0;
@@ -986,6 +1003,94 @@ int score_dev(gpk_handle* h, const double* dX, long m, int kind, double eta, dou
     return GPK_OK;
 }
 
+// layout of h->es_state (doubles): logP (nb), lmb (nb), dMu (nb x nb), dSig (nb x T), Hs (nb x T), W (np), lower (d),
+// upper (d), scaled zb (nb x d)
+struct EsLayout {
+    size_t logP, lmb, dMu, dSig, Hs, W, lo, up, zb, total;
+    EsLayout(int nb, int np_, int d) {
+        const size_t T = (size_t)nb * (nb + 1) / 2;
+        logP = 0; lmb = logP + nb; dMu = lmb + nb; dSig = dMu + (size_t)nb * nb; Hs = dSig + nb * T; W = Hs + nb * T;
+        lo = W + np_; up = lo + d; zb = up + d; total = zb + (size_t)nb * d;
+    }
+};
+
+// Posterior mean alone of m candidates resident on the device (d_mu: m doubles), asynchronous on the handle's stream.
+// The int8 path's covariance builder with its digit stores compiled out writes each 128-column tile's share of K* alpha,
+// and gpk_mu_parts_finish_kernel sums the shares in tile order: no K* in HBM, no L^-1 slices, no contraction.  Every
+// candidate is independent, so the values depend neither on "chunk" nor on how a batch is split, and equal the mean of
+// score_dev's int8 path bit for bit.
+int predict_mean_dev(gpk_handle* h, const double* dX, long m, double* d_mu) {
+    if (!h->mean_only)                      // option "meanonly" = 0: the mean of the full scoring pass (comparisons)
+        return score_dev(h, dX, m, GPK_ACQ_NONE, 0.0, 0.0, nullptr, d_mu, nullptr, nullptr, nullptr);
+    if (!cov_tma(h)) BAD("gpk_predict_mean: needs the TMA covariance builder (option loader 1 or 2)");
+    int rc;
+    if ((rc = build_linv(h))) return rc;
+    if ((rc = ensure_alpha(h))) return rc;
+    const long NP = h->NP;
+    const long cap = std::min<long>(chunk_rows(h), round_up(m, BM));
+    if ((rc = ensure(h, h->part_mu, (size_t)h->nb * cap * 8))) return rc;
+    CUtensorMap map;
+    if ((rc = make_cov_map(h, &map, (void*)train_operand(h), h->spec.n_terms, NP))) return rc;
+    const double* lo = h->has_bounds ? ptr<double>(h->lower) : nullptr;
+    const double* up = h->has_bounds ? ptr<double>(h->upper) : nullptr;
+    const int gx = (int)(NP / 128);
+    for (long base = 0; base < m; base += cap) {
+        const long mc = std::min(cap, m - base);
+        const long mcp = round_up(mc, BM);
+        gpk_cov_oz_kernel<8, false><<<(unsigned)(gx * (mcp / 32)), 256, cov_oz_smem_bytes(h->spec.n_terms, 8), h->stream>>>(
+            map, h->spec, h->n, dX + base * h->d, h->d, mc, lo, up, ptr<double>(h->alpha), 0, nullptr, NP, 0,
+            ptr<double>(h->part_mu), cap, gx);
+        CKL();
+        gpk_mu_parts_finish_kernel<<<(unsigned)((mc + 255) / 256), 256, 0, h->stream>>>(
+            ptr<double>(h->part_mu), cap, h->nb, mc, h->mean, h->norm_out, h->y_mean, h->y_std, d_mu + base);
+        CKL();
+    }
+    return GPK_OK;
+}
+
+// Entropy change of m candidates on the device (InformationGain.compute): Xm are the inputs the model's scoring pass and
+// covariance to zb take, Xb the ones the bounds test of gpk_es_update's [lower, upper] sees (the same array unless the
+// model's inputs were transformed).  Asynchronous on the handle's stream; needs a current gpk_es_update.
+int es_dh_dev(gpk_handle* h, const double* Xm, const double* Xb, long m, double* d_out) {
+    const int nb = h->es_nb, d = h->d;
+    EsLayout L(nb, h->es_np, d);
+    const double* st = ptr<double>(h->es_state);
+    const long CH = 16384;                  // candidates per pass; every candidate is independent of the others
+    int rc;
+    if ((rc = ensure(h, h->es_work, (size_t)CH * (nb + 1) * 8))) return rc;
+    double* var = ptr<double>(h->es_work);
+    double* sig = var + CH;
+    const double* lo = h->has_bounds ? ptr<double>(h->lower) : nullptr;
+    const double* up = h->has_bounds ? ptr<double>(h->upper) : nullptr;
+    const double out_scale = h->norm_out ? h->y_std * h->y_std : 1.0;
+    for (long c0 = 0; c0 < m; c0 += CH) {
+        const long rows = std::min(CH, m - c0);
+        const double* X = Xm + c0 * d;
+        if ((rc = score_dev(h, X, rows, GPK_ACQ_NONE, 0.0, 0.0, nullptr, nullptr, var, nullptr, nullptr))) return rc;
+        gpk_es_sigma_kernel<<<(unsigned)rows, GPK_ES_THREADS, 0, h->stream>>>(h->spec, X, rows, d, lo, up,
+                                                                              ptr<double>(h->Xrow), h->n,
+                                                                              ptr<double>(h->es_U), st + L.zb, nb,
+                                                                              out_scale, sig);
+        CKL();
+        gpk_es_dh_kernel<<<(unsigned)rows, GPK_ES_THREADS, 0, h->stream>>>(
+            Xb + c0 * d, rows, d, st + L.lo, st + L.up, var, sig, nb, h->es_np, h->es_sn2, h->es_H, st + L.logP,
+            st + L.lmb, st + L.dMu, st + L.dSig, st + L.Hs, st + L.W, d_out + c0);
+        CKL();
+    }
+    return GPK_OK;
+}
+
+// the checks gpk_es_compute makes before it runs: a current gpk_es_update on an unchanged model
+int es_ready(gpk_handle* h, gpk_handle* report, const char* who) {
+    gpk_handle* r = report ? report : h;
+    if (h->es_linv_serial < 0) { set_err(r, "%s: call gpk_es_update first", who); return GPK_BAD_ARG; }
+    if (!h->linv_ready || h->es_linv_serial != h->linv_serial) {
+        set_err(r, "%s: the model changed since gpk_es_update", who);
+        return GPK_BAD_ARG;
+    }
+    return GPK_OK;
+}
+
 }  // namespace
 
 // =============================================================================================
@@ -1048,7 +1153,7 @@ int gpk_destroy(gpk_handle* h) {
                       &h->out_var, &h->out_acq, &h->block_best, &h->best, &h->nneg, &h->Vt, &h->cov, &h->XsT,
                       &h->tmpjobs, &h->alpha, &h->tmp1, &h->tmp2, &h->tmp3, &h->chain_cnt, &h->dprof, &h->Xts, &h->oz_Pq, &h->oz_Kq, &h->oz_Kq2, &h->oz_eP, &h->oz_emax, &h->oz_pmu2, &h->oz_probe,
                       &h->multi_cand, &h->multi_A, &h->multi_B, &h->multi_out, &h->multi_bb, &h->gather, &h->best_global,
-                      &h->de_pop, &h->de_trial, &h->de_param, &h->de_E, &h->de_small, &h->de_sort, &h->ep_buf, &h->es_state, &h->es_U, &h->es_work, &h->es_in};
+                      &h->de_pop, &h->de_trial, &h->de_param, &h->de_E, &h->de_small, &h->de_sort, &h->ep_buf, &h->es_state, &h->es_U, &h->es_work, &h->es_in, &h->fab_in};
     for (DevBuf* b : bufs)
         if (b->p) cudaFree(b->p);
     if (h->ev_ok)
@@ -1124,6 +1229,11 @@ int gpk_set_option(gpk_handle* h, const char* key, long value) {
     if (!strcmp(key, "pdl")) {
         if (value != 0 && value != 1) BAD("pdl must be 0 or 1");
         h->pdl = (int)value;
+        return GPK_OK;
+    }
+    if (!strcmp(key, "meanonly")) {
+        if (value != 0 && value != 1) BAD("meanonly must be 0 or 1");
+        h->mean_only = (int)value;
         return GPK_OK;
     }
     if (!strcmp(key, "overlap")) {
@@ -1880,6 +1990,28 @@ int gpk_predict(gpk_handle* h, const double* Xs, long m, double* mu, double* var
     return gpk_acq(h, Xs, m, GPK_ACQ_NONE, 0.0, 0.0, nullptr, mu, var, nullptr, nullptr, nullptr);
 }
 
+int gpk_predict_mean_dev(gpk_handle* h, const void* d_Xs, long m, void* d_mu) {
+    int rc = require(h, true, true, true);
+    if (rc) return rc;
+    if (!d_Xs || !d_mu || m <= 0) BAD("gpk_predict_mean_dev: need candidates and mu");
+    CK(cudaSetDevice(h->device));
+    return predict_mean_dev(h, (const double*)d_Xs, m, (double*)d_mu);
+}
+
+int gpk_predict_mean(gpk_handle* h, const double* Xs, long m, double* mu) {
+    int rc = require(h, true, true, true);
+    if (rc) return rc;
+    if (!Xs || !mu || m <= 0) BAD("gpk_predict_mean: need candidates and mu");
+    CK(cudaSetDevice(h->device));
+    if ((rc = ensure(h, h->cand, (size_t)m * h->d * 8))) return rc;
+    if ((rc = ensure(h, h->out_mu, (size_t)m * 8))) return rc;
+    CK(cudaMemcpyAsync(h->cand.p, Xs, (size_t)m * h->d * 8, cudaMemcpyHostToDevice, h->stream));
+    if ((rc = predict_mean_dev(h, ptr<double>(h->cand), m, ptr<double>(h->out_mu)))) return rc;
+    CK(cudaMemcpyAsync(mu, h->out_mu.p, (size_t)m * 8, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    return GPK_OK;
+}
+
 static int predict_cov_impl(gpk_handle* h, const double* Xs, long m, double* mu, double* cov, int clip) {
     int rc = require(h, true, true, true);
     if (rc) return rc;
@@ -2408,17 +2540,6 @@ int gpk_ep_joint_min(gpk_handle* h, const double* mu, const double* V, int nb, d
     return GPK_OK;
 }
 
-// layout of h->es_state (doubles): logP (nb), lmb (nb), dMu (nb x nb), dSig (nb x T), Hs (nb x T), W (np), lower (d),
-// upper (d), scaled zb (nb x d)
-struct EsLayout {
-    size_t logP, lmb, dMu, dSig, Hs, W, lo, up, zb, total;
-    EsLayout(int nb, int np_, int d) {
-        const size_t T = (size_t)nb * (nb + 1) / 2;
-        logP = 0; lmb = logP + nb; dMu = lmb + nb; dSig = dMu + (size_t)nb * nb; Hs = dSig + nb * T; W = Hs + nb * T;
-        lo = W + np_; up = lo + d; zb = up + d; total = zb + (size_t)nb * d;
-    }
-};
-
 int gpk_es_update(gpk_handle* h, const double* zb, int nb, const double* lmb, double sn2, const double* W, int np_,
                   const double* lower, const double* upper, double* logP, double* dlogPdMu, double* dlogPdSigma,
                   double* dlogPdMudMu) {
@@ -2494,34 +2615,9 @@ int gpk_es_compute_dev(gpk_handle* h, const void* d_Xs, long m, void* d_out) {
     int rc = require(h, true, true, true);
     if (rc) return rc;
     if (!d_Xs || !d_out || m <= 0) BAD("gpk_es_compute_dev: need candidates and out");
-    if (h->es_linv_serial < 0) BAD("gpk_es_compute: call gpk_es_update first");
-    if (!h->linv_ready || h->es_linv_serial != h->linv_serial) BAD("gpk_es_compute: the model changed since gpk_es_update");
+    if ((rc = es_ready(h, nullptr, "gpk_es_compute"))) return rc;
     CK(cudaSetDevice(h->device));
-    const int nb = h->es_nb, d = h->d;
-    EsLayout L(nb, h->es_np, d);
-    const double* st = ptr<double>(h->es_state);
-    const long CH = 16384;                  // candidates per pass; every candidate is independent of the others
-    if ((rc = ensure(h, h->es_work, (size_t)CH * (nb + 1) * 8))) return rc;
-    double* var = ptr<double>(h->es_work);
-    double* sig = var + CH;
-    const double* lo = h->has_bounds ? ptr<double>(h->lower) : nullptr;
-    const double* up = h->has_bounds ? ptr<double>(h->upper) : nullptr;
-    const double out_scale = h->norm_out ? h->y_std * h->y_std : 1.0;
-    for (long c0 = 0; c0 < m; c0 += CH) {
-        const long rows = std::min(CH, m - c0);
-        const double* X = (const double*)d_Xs + c0 * d;
-        if ((rc = score_dev(h, X, rows, GPK_ACQ_NONE, 0.0, 0.0, nullptr, nullptr, var, nullptr, nullptr))) return rc;
-        gpk_es_sigma_kernel<<<(unsigned)rows, GPK_ES_THREADS, 0, h->stream>>>(h->spec, X, rows, d, lo, up,
-                                                                              ptr<double>(h->Xrow), h->n,
-                                                                              ptr<double>(h->es_U), st + L.zb, nb,
-                                                                              out_scale, sig);
-        CKL();
-        gpk_es_dh_kernel<<<(unsigned)rows, GPK_ES_THREADS, 0, h->stream>>>(
-            X, rows, d, st + L.lo, st + L.up, var, sig, nb, h->es_np, h->es_sn2, h->es_H, st + L.logP, st + L.lmb,
-            st + L.dMu, st + L.dSig, st + L.Hs, st + L.W, (double*)d_out + c0);
-        CKL();
-    }
-    return GPK_OK;
+    return es_dh_dev(h, (const double*)d_Xs, (const double*)d_Xs, m, (double*)d_out);
 }
 
 int gpk_es_compute(gpk_handle* h, const double* Xs, long m, double* out) {

@@ -560,3 +560,36 @@ __global__ void __launch_bounds__(GPK_ES_THREADS) gpk_es_dh_kernel(const double*
         out[c] = (isnan(dH) || dH == INFINITY) ? -1.7976931348623157e308 : dH;
     }
 }
+
+// ---------------------------------------------------------------------------------------
+// Information gain per unit cost (robo/acquisition_functions/information_gain_per_unit_cost.py) over Fabolas models
+// ---------------------------------------------------------------------------------------
+// FabolasGP.normalize on the device (robo/models/fabolas_gp.py:122-126): out[c][j] = (x_j - lo_j) / (up_j - lo_j) for
+// the d - 1 configuration columns, basis(x_{d-1}) for the last (environment) column.  numpy's (1 - s) ** 2 on an array
+// is one multiply t * t, and its true division is IEEE: the result is bit-identical to the host transform.
+__global__ void gpk_fabolas_transform_kernel(const double* __restrict__ X, long m, int d, const double* __restrict__ lo,
+                                             const double* __restrict__ up, int basis, double* __restrict__ out) {
+    const long e = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= m * d) return;
+    const int j = (int)(e % d);
+    const double x = X[e];
+    double v;
+    if (j < d - 1) {
+        v = (x - lo[j]) / (up[j] - lo[j]);
+    } else if (basis == GPK_BASIS_ONE_MINUS_S_SQ) {
+        const double t = 1.0 - x;
+        v = t * t;
+    } else {
+        v = x;
+    }
+    out[e] = v;
+}
+
+// out = dh / (exp(log_cost) + overhead) per model and candidate (information_gain_per_unit_cost.py:91-104) over the
+// n x m values (out may be dh); -DBL_MAX / c overflows to -inf for c < 1 exactly as numpy does
+__global__ void gpk_es_cost_ratio_kernel(const double* dh, const double* __restrict__ log_cost, long total,
+                                         double overhead, double* out) {
+    const long e = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= total) return;
+    out[e] = dh[e] / (exp(log_cost[e]) + overhead);
+}

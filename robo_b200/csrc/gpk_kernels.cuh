@@ -276,6 +276,21 @@ __global__ void __launch_bounds__(256) gpk_finish_kernel(const FinishArgs f)
     }
 }
 
+// Mean-only epilogue (gpk_predict_mean): gpk_finish_kernel's mean, with the same fixed-order sum of the per-tile
+// partials, constant mean and output transform, and no variance partials.
+__global__ void __launch_bounds__(256) gpk_mu_parts_finish_kernel(const double* __restrict__ part_mu, long ldpart,
+                                                                  int nparts, long m, double mean, int norm_out,
+                                                                  double y_mean, double y_std, double* __restrict__ out)
+{
+    const long c = (long)blockIdx.x * 256 + threadIdx.x;
+    if (c >= m) return;
+    double mu = 0.0;
+    for (int p = 0; p < nparts; ++p) mu += part_mu[(long)p * ldpart + c];
+    mu += mean;
+    if (norm_out) mu = mu * y_std + y_mean;
+    out[c] = mu;
+}
+
 // Final arg-max over block results, merged into *best (which may hold the running best of
 // earlier chunks; idx < 0 means empty).
 __global__ void __launch_bounds__(256) gpk_argmax_final_kernel(const BestPair* __restrict__ bb, int nblocks,

@@ -356,8 +356,10 @@ gpk_oz_vargemm_kernel(const __grid_constant__ CUtensorMap mapP, const __grid_con
 // sum_j k(c, j) alpha_j of this 128-column tile is reduced over the 64 threads of a candidate group and written to
 // part_mu[tile][cand] (summed in fixed order by gpk_finish_kernel: deterministic).  Replaces K* store (8 B / element)
 // + split kernel (8 B read, 8 B written) + mean dot (8 B read) by 8 B written per element.
+// DIGITS = false compiles the digit stores out (Kq unused): the mean-only prediction (gpk_predict_mean) writes nothing
+// but part_mu, with the same arithmetic and reduction order, so its mean is bit-identical to the int8 scoring pass's.
 // ---------------------------------------------------------------------------------------
-template <int CC>
+template <int CC, bool DIGITS = true>
 __global__ void __launch_bounds__(256, CC == 8 ? 2 : 4)
 gpk_cov_oz_kernel(const __grid_constant__ CUtensorMap mapX, const KSpec ks, int n,
                   const double* __restrict__ cand, int dc, long m,
@@ -441,12 +443,14 @@ gpk_cov_oz_kernel(const __grid_constant__ CUtensorMap mapX, const KSpec ks, int 
         const bool cv = ci < m;
         const double k0 = (cv && v0) ? ks.amp * pr[c][0] : 0.0;
         const double k1 = (cv && v1) ? ks.amp * pr[c][1] : 0.0;
-        // digits: two adjacent int8 per slice
-        const unsigned long long y0 = oz_digits(k0 * sc), y1 = oz_digits(k1 * sc);
-        int8_t* dst = Kq + ci * ldq + j0;
+        if (DIGITS) {
+            // digits: two adjacent int8 per slice
+            const unsigned long long y0 = oz_digits(k0 * sc), y1 = oz_digits(k1 * sc);
+            int8_t* dst = Kq + ci * ldq + j0;
 #pragma unroll
-        for (int s2 = 0; s2 < OZ_S; ++s2)
-            *reinterpret_cast<uint16_t*>(dst + (long)s2 * slice_stride) = (uint16_t)(oz_digit_of(y0, s2) | (oz_digit_of(y1, s2) << 8));
+            for (int s2 = 0; s2 < OZ_S; ++s2)
+                *reinterpret_cast<uint16_t*>(dst + (long)s2 * slice_stride) = (uint16_t)(oz_digit_of(y0, s2) | (oz_digit_of(y1, s2) << 8));
+        }
         // mean share of this tile: reduce over the 64 threads (2 warps) of the candidate group, fixed order
         double pm = fma(k0, a0, k1 * a1);
 #pragma unroll

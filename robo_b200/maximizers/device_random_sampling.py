@@ -28,6 +28,9 @@ class DeviceRandomSampling(BaseMaximizer):
     def maximize(self):
         acq = self.objective_func
         model = acq.model
+        es = self._es_cost_spec(acq)
+        if es is not None:
+            return self._maximize_es_cost(acq, es)
         if not hasattr(model, "gp") or not hasattr(model.gp, "handle"):
             raise TypeError("DeviceRandomSampling needs a robo_b200 GaussianProcess model")
         kind = _lib.ACQ_KIND[acq.kind]
@@ -57,5 +60,36 @@ class DeviceRandomSampling(BaseMaximizer):
                 dev = "cuda:%d" % torch.cuda.current_device() if torch.cuda.is_available() else "cpu"
                 val, idx = allgather_best(pack_pair(val, idx, dev), self.group)
                 x = handle.generate_candidates(seed, idx, 1, n_uniform, self.lower, self.upper, inc_x, 0.1)[0]
+        self.last = dict(seed=seed, best_idx=idx, best_val=val)
+        return x
+
+    def _next_seed(self):
+        seed = (self.seed + 0x9E3779B97F4A7C15 * self.calls) & 0xFFFFFFFFFFFFFFFF
+        self.calls += 1
+        return seed
+
+    @staticmethod
+    def _es_cost_spec(acq):
+        """The fused call's arguments when acq is an InformationGainPerUnitCost, or a MarginalizationGPMCMC of them."""
+        from robo_b200.acquisition_functions.information_gain_per_unit_cost import (InformationGainPerUnitCost,
+                                                                                    device_spec)
+        if isinstance(acq, InformationGainPerUnitCost):
+            return device_spec([acq])
+        if hasattr(acq, "_es_cost_spec"):
+            return acq._es_cost_spec()
+        return None
+
+    def _maximize_es_cost(self, acq, es):
+        """Candidates, information gain per unit cost, mean over the model pairs and arg-max in one device call
+        (gpk_maximize_random_es_cost); the incumbent as random_sampling.py:42 takes it.  One GPU only."""
+        if self.world > 1:
+            raise ValueError("DeviceRandomSampling of InformationGainPerUnitCost runs on one GPU")
+        ho, hc, lo, up, bo, bc, oh = es
+        inc_x = acq.model.get_incumbent()[0]
+        seed = self._next_seed()
+        n_uniform = int(self.n_samples * .7)
+        n_total = n_uniform + int(self.n_samples * .3)
+        x, val, idx = _lib.maximize_random_es_cost(ho, hc, seed, n_total, n_uniform, self.lower, self.upper, inc_x, 0.1,
+                                                   lo, up, bo, bc, oh)
         self.last = dict(seed=seed, best_idx=idx, best_val=val)
         return x

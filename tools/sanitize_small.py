@@ -59,6 +59,28 @@ rp = _lib.acq_multi(hs[:2], Xs[:300], 1)
 print("multi", rm["best_idx"], rp["var"][:2])
 for h in hs:
     h.close()
+# information gain per unit cost: mean-only prediction, Fabolas transform, entropy change on two objective / cost pairs,
+# the ratio, the mean over pairs and the device arg-max
+pairs = []
+for i in range(4):
+    h = _lib.Handle(0)
+    h.set_data(X, y if i < 2 else 0.1 * y)
+    h.set_kernel(f["family"], f["log_amp"], f["axis"], f["group"], f["log_metric"])
+    h.fit(1e-3 + 1.25e-12, float(y.mean()))
+    pairs.append(h)
+print("mean only", pairs[2].predict_mean(Xb)[:2], pairs[2].predict_mean(Xs[:70])[:2])
+zb = np.hstack([rng.rand(20, D - 1), np.ones((20, 1))])
+W = np.linspace(-2.0, 2.0, 40)
+for h in pairs[:2]:
+    h.es_update(zb, rng.rand(20), 1e-3, W, np.zeros(D), np.ones(D))
+Xc = np.vstack([Xb, -np.ones((1, D))])
+for bo, bc in ((_lib.BASIS_ONE_MINUS_S_SQ, _lib.BASIS_S), (_lib.BASIS_S, _lib.BASIS_ONE_MINUS_S_SQ)):
+    r = _lib.es_cost_multi(pairs[:2], pairs[2:], Xc, np.zeros(D - 1), np.ones(D - 1), bo, bc, 0.1)
+    print("es cost", r["best_idx"], r["values"][-1])
+print("es cost random", _lib.maximize_random_es_cost(pairs[:1], pairs[2:3], 7, 1000, 700, np.zeros(D), np.ones(D), X[0],
+                                                     0.1, np.zeros(D - 1), np.ones(D - 1), 1, 0, 0.0)[2])
+for h in pairs:
+    h.close()
 h = _lib.moments_handle()
 print(h.acq_moments(rng.randn(100), rng.rand(100) + 0.1, _lib.ACQ_LOG_EI, 0.0, 0.0)[0][:3])
 print(h.reduce_models(rng.rand(4, 50), rng.rand(4, 50))[1][:3])
