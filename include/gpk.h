@@ -298,6 +298,18 @@ int gpk_es_compute(gpk_handle* h, const double* Xs, long m, double* out);
 /* the same on device pointers (d_Xs: m x d, d_out: m doubles), asynchronous on the handle's stream */
 int gpk_es_compute_dev(gpk_handle* h, const void* d_Xs, long m, void* d_out);
 
+/* MarginalizationGPMCMC.compute over InformationGain estimators (robo/acquisition_functions/marginalization.py:115-121)
+ * as one call: gpk_es_compute of every objective[i] on Xs (m x d raw inputs), each handle on its own stream, then the
+ * mean over the n handles summed in index order (gpk_reduce_models mode 0, also for n = 1).  Bit-identical to the n
+ * gpk_es_compute values reduced by gpk_reduce_models.  out (m) and best_val / best_idx (numpy.argmax of out) may be
+ * NULL.  GPK_BAD_ARG: n < 1, m < 1, handles on different devices or with different input dimensions, a handle listed
+ * twice, a handle without a current gpk_es_update (or changed since). */
+int gpk_es_multi(gpk_handle* const* objective, int n, const double* Xs, long m, double* out, double* best_val,
+                 long* best_idx);
+/* the same on a device batch (d_Xs: m x d), asynchronous on objective[0]'s stream: d_out (m doubles) is required,
+ * d_best (16 bytes {double value; long long index}) may be NULL. */
+int gpk_es_multi_dev(gpk_handle* const* objective, int n, const void* d_Xs, long m, void* d_out, void* d_best);
+
 /* basis functions of the environment column of Fabolas models (robo/fmin/fabolas.py:96-102) */
 typedef enum {
     GPK_BASIS_S = 0,           /* basis(s) = s          (the cost model)      */
@@ -339,6 +351,28 @@ int gpk_maximize_random_es_cost(gpk_handle* const* objective, gpk_handle* const*
                                 const double* incumbent, double scale, const double* lower, const double* upper,
                                 int n_bounds, int basis_objective, int basis_cost, double overhead, double* best_x, double* best_val,
                                 long* best_idx);
+
+/* gpk_maximize_de over the entropy change: the same evolution, kernels and Philox stream, with the same two deviations
+ * from the reference (updating='deferred'; the counter-based Philox stream keyed by `seed`), minimising
+ *   gpk_maximize_de_es:      -(gpk_es_multi's value of the member over objective[0 .. n-1]); n = 1: -(gpk_es_compute's
+ *                            value), no reduction;
+ *   gpk_maximize_de_es_cost: -(gpk_es_cost_multi's value of the member over the (objective[i], cost[i]) pairs); the
+ *                            members live in the extended box lower / upper (d each, the environment column last) and
+ *                            are scored raw; cfg_lower / cfg_upper (n_bounds = d - 1), the basis codes and the overhead
+ *                            as for gpk_es_cost_multi.
+ * pop, maxiter, mut_lo / mut_hi, recombination, tol, atol, lower / upper and the outputs as for gpk_maximize_de (there is
+ * no n_negative).  GPK_BAD_ARG as for gpk_maximize_de and gpk_es_multi / gpk_es_cost_multi, and when a handle has a
+ * multi-rank communicator: both run on one GPU. */
+int gpk_maximize_de_es(gpk_handle* const* objective, int n, unsigned long long seed, long pop, int maxiter,
+                       double mut_lo, double mut_hi, double recombination, double tol, double atol,
+                       const double* lower, const double* upper, double* best_x, double* best_energy, int* nit,
+                       long* nfev, double* population, double* energies);
+int gpk_maximize_de_es_cost(gpk_handle* const* objective, gpk_handle* const* cost, int n, unsigned long long seed,
+                            long pop, int maxiter, double mut_lo, double mut_hi, double recombination, double tol,
+                            double atol, const double* lower, const double* upper, const double* cfg_lower,
+                            const double* cfg_upper, int n_bounds, int basis_objective, int basis_cost, double overhead,
+                            double* best_x, double* best_energy, int* nit, long* nfev, double* population,
+                            double* energies);
 
 /* kernel.get_value(X1, X2) (test/test_models/test_gaussian_process.py:44-46) with the
  * handle's current kernel; no input scaling.  out is (n1, n2) row-major. */

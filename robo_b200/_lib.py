@@ -85,6 +85,13 @@ _SIGNATURES = {
                               C.c_double, _vp, _vp],
     "gpk_maximize_random_es_cost": [C.POINTER(_vp), C.POINTER(_vp), C.c_int, C.c_ulonglong, C.c_long, C.c_long, _dp, _dp,
                                     _dp, C.c_double, _dp, _dp, C.c_int, C.c_int, C.c_int, C.c_double, _dp, _dp, _lp],
+    "gpk_es_multi": [C.POINTER(_vp), C.c_int, _dp, C.c_long, _dp, _dp, _lp],
+    "gpk_es_multi_dev": [C.POINTER(_vp), C.c_int, _vp, C.c_long, _vp, _vp],
+    "gpk_maximize_de_es": [C.POINTER(_vp), C.c_int, C.c_ulonglong, C.c_long, C.c_int, C.c_double, C.c_double, C.c_double,
+                           C.c_double, C.c_double, _dp, _dp, _dp, _dp, _ip, _lp, _dp, _dp],
+    "gpk_maximize_de_es_cost": [C.POINTER(_vp), C.POINTER(_vp), C.c_int, C.c_ulonglong, C.c_long, C.c_int, C.c_double,
+                                C.c_double, C.c_double, C.c_double, C.c_double, _dp, _dp, _dp, _dp, C.c_int, C.c_int,
+                                C.c_int, C.c_double, _dp, _dp, _ip, _lp, _dp, _dp],
     "gpk_get_timings": [_vp, _dp],
     "gpk_get_diag_profile": [_vp, C.POINTER(C.c_longlong)],
 }
@@ -630,6 +637,79 @@ def maximize_random_es_cost(objective, cost, seed, count, n_uniform, box_lower, 
                                                  _as_dp(lo), _as_dp(up), lo.size, int(basis_objective), int(basis_cost),
                                                  float(overhead), _as_dp(bx), C.byref(bv), C.byref(bi)))
     return bx, bv.value, bi.value
+
+
+def es_multi(objective, Xs, want_values=True):
+    """gpk_es_multi: the entropy change of every row of Xs (m, d) under each handle, averaged over the handles ->
+    dict(values (m,) or None, best_val, best_idx)."""
+    h0 = objective[0]
+    ho = (_vp * len(objective))(*[h._h for h in objective])
+    Xs = f64(Xs)
+    m = Xs.shape[0]
+    out = np.empty(m) if want_values else None
+    bv, bi = C.c_double(), C.c_long(-1)
+    h0._check(h0.lib.gpk_es_multi(ho, len(objective), _as_dp(Xs), m, _as_dp(out) if want_values else None,
+                                  C.byref(bv), C.byref(bi)))
+    return dict(values=out, best_val=bv.value, best_idx=bi.value)
+
+
+def es_multi_dev(objective, d_Xs_ptr, m, d_out_ptr, d_best_ptr=0):
+    """Device-batch variant, asynchronous on objective[0]'s stream."""
+    h0 = objective[0]
+    ho = (_vp * len(objective))(*[h._h for h in objective])
+    h0._check(h0.lib.gpk_es_multi_dev(ho, len(objective), _vp(d_Xs_ptr), int(m), _vp(d_out_ptr or 0),
+                                      _vp(d_best_ptr or 0)))
+
+
+def _de_result(x, be, nit, nfev, P, E, want_population):
+    r = dict(x=x, energy=be.value, nit=nit.value, nfev=nfev.value)
+    if want_population:
+        r.update(population=P, energies=E)
+    return r
+
+
+def maximize_de_es(objective, seed, pop, maxiter, mutation, recombination, tol, atol, lower, upper,
+                   want_population=False):
+    """gpk_maximize_de_es: differential evolution minimising minus the entropy change (one handle: gpk_es_compute's
+    value; several: gpk_es_multi's mean) -> dict(x (D,), energy, nit, nfev[, population (pop, D), energies (pop,)])."""
+    h0 = objective[0]
+    ho = (_vp * len(objective))(*[h._h for h in objective])
+    lo, up = f64(lower).ravel(), f64(upper).ravel()
+    x = np.empty(lo.size)
+    pop = int(pop)
+    P = np.empty((pop, lo.size)) if want_population and pop > 0 else None
+    E = np.empty(pop) if want_population and pop > 0 else None
+    be, nit, nfev = C.c_double(), C.c_int(), C.c_long()
+    h0._check(h0.lib.gpk_maximize_de_es(ho, len(objective), int(seed) & 0xFFFFFFFFFFFFFFFF, pop, int(maxiter),
+                                        float(mutation[0]), float(mutation[1]), float(recombination), float(tol),
+                                        float(atol), _as_dp(lo), _as_dp(up), _as_dp(x), C.byref(be), C.byref(nit),
+                                        C.byref(nfev), _as_dp(P) if P is not None else None,
+                                        _as_dp(E) if E is not None else None))
+    return _de_result(x, be, nit, nfev, P, E, want_population)
+
+
+def maximize_de_es_cost(objective, cost, seed, pop, maxiter, mutation, recombination, tol, atol, lower, upper,
+                        cfg_lower, cfg_upper, basis_objective, basis_cost, overhead, want_population=False):
+    """gpk_maximize_de_es_cost: differential evolution over the extended box lower / upper (d) minimising minus the
+    information gain per unit cost of gpk_es_cost_multi (configuration bounds cfg_lower / cfg_upper, d - 1) -> as
+    maximize_de_es."""
+    ho, hc, clo, cup = _es_cost_args(objective, cost, cfg_lower, cfg_upper)
+    h0 = objective[0]
+    lo, up = f64(lower).ravel(), f64(upper).ravel()
+    if not lo.size == up.size == clo.size + 1:
+        raise ValueError("maximize_de_es_cost: the box needs d entries, the configuration bounds d - 1")
+    x = np.empty(lo.size)
+    pop = int(pop)
+    P = np.empty((pop, lo.size)) if want_population and pop > 0 else None
+    E = np.empty(pop) if want_population and pop > 0 else None
+    be, nit, nfev = C.c_double(), C.c_int(), C.c_long()
+    h0._check(h0.lib.gpk_maximize_de_es_cost(ho, hc, len(objective), int(seed) & 0xFFFFFFFFFFFFFFFF, pop, int(maxiter),
+                                             float(mutation[0]), float(mutation[1]), float(recombination), float(tol),
+                                             float(atol), _as_dp(lo), _as_dp(up), _as_dp(clo), _as_dp(cup), clo.size,
+                                             int(basis_objective), int(basis_cost), float(overhead), _as_dp(x),
+                                             C.byref(be), C.byref(nit), C.byref(nfev),
+                                             _as_dp(P) if P is not None else None, _as_dp(E) if E is not None else None))
+    return _de_result(x, be, nit, nfev, P, E, want_population)
 
 
 _moments_handle = {}

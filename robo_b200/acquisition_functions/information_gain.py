@@ -102,11 +102,16 @@ class InformationGain(BaseAcquisitionFunction):
         differences are marked "Not tested!")."""
         if derivative:
             raise NotImplementedError("InformationGain has no derivative on the GPU path")
+        return self._ready_handle().es_compute(np.asarray(X_test, dtype=np.float64))
+
+    def _ready_handle(self):
+        """The device handle compute() scores on, after compute()'s checks (ValueError before update() or with an
+        infinite lmb)."""
         if self.zb is None:
             raise ValueError("InformationGain.compute needs update() first")
         if not np.all(np.isfinite(self.lmb)):
             raise ValueError("lmb should not be infinite.")
-        return _device_model(self.model).es_compute(np.asarray(X_test, dtype=np.float64))
+        return _device_model(self.model)
 
     def argmax(self, X_test):
         return int(np.argmax(self.compute(X_test)))

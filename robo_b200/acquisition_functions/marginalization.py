@@ -50,6 +50,10 @@ class MarginalizationGPMCMC(BaseAcquisitionFunction):
             # information gain per unit cost over the (objective, cost) sub-model pairs as ONE call (gpk_es_cost_multi)
             ho, hc, lo, up, bo, bc, oh = es
             return _lib.es_cost_multi(ho, hc, np.asarray(X_test, dtype=np.float64), lo, up, bo, bc, oh)["values"]
+        handles = self._es_spec() if not derivative else None
+        if handles is not None:
+            # the information gain of every estimator and the mean over them as ONE call (gpk_es_multi)
+            return _lib.es_multi(handles, np.asarray(X_test, dtype=np.float64))["values"]
         fused = self._fused_spec() if not derivative else None
         if fused is not None:
             # marginalization.py:115-121 as ONE call: the batch goes to the device once, the n sub-models score it
@@ -72,6 +76,9 @@ class MarginalizationGPMCMC(BaseAcquisitionFunction):
             ho, hc, lo, up, bo, bc, oh = es
             r = _lib.es_cost_multi(ho, hc, np.asarray(X_test, dtype=np.float64), lo, up, bo, bc, oh, want_values=False)
             return int(r["best_idx"])
+        handles = self._es_spec()
+        if handles is not None:
+            return int(_lib.es_multi(handles, np.asarray(X_test, dtype=np.float64), want_values=False)["best_idx"])
         fused = self._fused_spec()
         if fused is None:
             return int(np.argmax(self.compute(X_test)))
@@ -91,6 +98,19 @@ class MarginalizationGPMCMC(BaseAcquisitionFunction):
                 not all(isinstance(e, InformationGainPerUnitCost) for e in self.estimators):
             return None
         return device_spec(self.estimators)
+
+    def _es_spec(self):
+        """The objective handles of the fused call (gpk_es_multi) when every estimator is an InformationGain, not per
+        unit cost, on a device GaussianProcess sub-model; raises the estimators' own ValueErrors (before update(), an
+        infinite lmb)."""
+        from robo_b200.acquisition_functions.information_gain import InformationGain
+        from robo_b200.acquisition_functions.information_gain_per_unit_cost import InformationGainPerUnitCost
+        from robo_b200.maximizers.differential_evolution import _raw_inputs
+        if len(self.estimators) == 0 or not all(isinstance(e, InformationGain) and
+                                                not isinstance(e, InformationGainPerUnitCost) and _raw_inputs(e.model)
+                                                for e in self.estimators):
+            return None
+        return [e._ready_handle() for e in self.estimators]
 
     def _fused_spec(self):
         """(kind, eta per model, par, handles) when every estimator is a closed-form acquisition on a device GP."""

@@ -1048,6 +1048,13 @@ int predict_mean_dev(gpk_handle* h, const double* dX, long m, double* d_mu) {
     return GPK_OK;
 }
 
+const long ES_CH = 16384;                   // candidates per pass of es_dh_dev; every candidate is independent of the others
+
+// es_dh_dev's scratch (variance and sigma of one pass), sized for the handle's current gpk_es_update
+int es_reserve(gpk_handle* h) {
+    return ensure(h, h->es_work, (size_t)ES_CH * (h->es_nb + 1) * 8);
+}
+
 // Entropy change of m candidates on the device (InformationGain.compute): Xm are the inputs the model's scoring pass and
 // covariance to zb take, Xb the ones the bounds test of gpk_es_update's [lower, upper] sees (the same array unless the
 // model's inputs were transformed).  Asynchronous on the handle's stream; needs a current gpk_es_update.
@@ -1055,9 +1062,9 @@ int es_dh_dev(gpk_handle* h, const double* Xm, const double* Xb, long m, double*
     const int nb = h->es_nb, d = h->d;
     EsLayout L(nb, h->es_np, d);
     const double* st = ptr<double>(h->es_state);
-    const long CH = 16384;                  // candidates per pass; every candidate is independent of the others
+    const long CH = ES_CH;
     int rc;
-    if ((rc = ensure(h, h->es_work, (size_t)CH * (nb + 1) * 8))) return rc;
+    if ((rc = es_reserve(h))) return rc;
     double* var = ptr<double>(h->es_work);
     double* sig = var + CH;
     const double* lo = h->has_bounds ? ptr<double>(h->lower) : nullptr;

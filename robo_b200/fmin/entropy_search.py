@@ -1,13 +1,15 @@
 """``entropy_search`` facade with the signature and object wiring of robo/fmin/entropy_search.py:20-131: same kernel
 (cov_amp * Matern52), DefaultPrior, n_hypers rule, ``InformationGain(gp, lower, upper, sampling_acquisition=EI)``,
-MarginalizationGPMCMC wrapping for ``gp_mcmc`` and result dict, built from the robo_b200 classes.  The only maximizer
-is "random"."""
+MarginalizationGPMCMC wrapping for ``gp_mcmc`` and result dict, built from the robo_b200 classes.  Maximizers:
+"random" (RandomSampling) and "differential_evolution" (the evolution on the device, gpk_maximize_de_es, with the
+reference's L-BFGS-B polish on the host); "scipy" needs a derivative of the entropy change, which the device path does
+not have."""
 import numpy as np
 
 from robo_b200 import kernels
 from robo_b200.acquisition_functions import EI, InformationGain, MarginalizationGPMCMC
 from robo_b200.initial_design import init_latin_hypercube_sampling
-from robo_b200.maximizers import RandomSampling
+from robo_b200.maximizers import DifferentialEvolution, RandomSampling
 from robo_b200.models import GaussianProcess, GaussianProcessMCMC
 from robo_b200.priors import DefaultPrior
 from robo_b200.solver import BayesianOptimization
@@ -20,10 +22,9 @@ def entropy_search(objective_function, lower, upper, num_iterations=30, maximize
     assert n_init <= num_iterations, "Number of initial design point has to be <= than the number of iterations"
     if rng is None:
         rng = np.random.RandomState(np.random.randint(0, 10000))
-    if maximizer != "random":
+    if maximizer not in ("random", "differential_evolution"):
         raise ValueError("'{}' is not a maximizer of entropy search on the GPU path: InformationGain has no device "
-                         "derivative for 'scipy', and 'differential_evolution' serves only EI / LogEI / PI / LCB; "
-                         "use 'random'".format(maximizer))
+                         "derivative for 'scipy'; use 'random' or 'differential_evolution'".format(maximizer))
 
     cov_amp = 2
     n_dims = lower.shape[0]
@@ -44,7 +45,10 @@ def entropy_search(objective_function, lower, upper, num_iterations=30, maximize
 
     a = InformationGain(gp, lower=lower, upper=upper, sampling_acquisition=EI)
     acquisition_func = a if model == "gp" else MarginalizationGPMCMC(a)
-    max_func = RandomSampling(acquisition_func, lower, upper, rng=rng)
+    if maximizer == "random":
+        max_func = RandomSampling(acquisition_func, lower, upper, rng=rng)
+    else:
+        max_func = DifferentialEvolution(acquisition_func, lower, upper, rng=rng)
 
     bo = BayesianOptimization(objective_function, lower, upper, acquisition_func, gp, max_func,
                               initial_design=init_latin_hypercube_sampling, initial_points=n_init, rng=rng,

@@ -12,6 +12,10 @@ the counter-based Philox stream keyed by the seed.  The reference never passes i
 cannot be reproduced by anyone; here the seed is drawn from ``rng`` at construction and advanced per call, as in
 DeviceRandomSampling.
 
+The acquisition may be EI / LogEI / PI / LCB (gpk_maximize_de), InformationGain (gpk_maximize_de_es: the entropy
+change, marginalised by gpk_es_multi over a GP-MCMC ensemble) or InformationGainPerUnitCost, Fabolas's acquisition
+(gpk_maximize_de_es_cost over the extended box), each alone or under MarginalizationGPMCMC.
+
 With ``polish=True`` (scipy's default, which the reference uses) L-BFGS-B refines the device winner on the host
 through the reference's single-point objective, and scipy's acceptance rule applies: lower energy, success, inside
 the bounds.  The polish stays per point by design.
@@ -44,6 +48,26 @@ class DifferentialEvolution(BaseMaximizer):
         self.seed = int(self.rng.randint(0, 2 ** 31 - 1))
 
     def _device_spec(self):
+        """What scores the population on the device, by acquisition:
+            ("es_cost", device_spec's tuple)   InformationGainPerUnitCost, alone or marginalised (gpk_es_cost_multi)
+            ("es", handles)                    InformationGain, alone or marginalised (gpk_es_compute / gpk_es_multi)
+            ("acq", (kind, etas, par, handles)) EI / LogEI / PI / LCB (gpk_acq_multi)
+        TypeError when the acquisition does not run on device models."""
+        from robo_b200.acquisition_functions.information_gain import InformationGain
+        from robo_b200.acquisition_functions.information_gain_per_unit_cost import (InformationGainPerUnitCost,
+                                                                                    device_spec)
+        acq = self.objective_func
+        estimators = acq.estimators if hasattr(acq, "_fused_spec") else [acq]
+        # InformationGainPerUnitCost is an InformationGain: it is recognised first
+        if estimators and all(isinstance(e, InformationGainPerUnitCost) for e in estimators):
+            return "es_cost", device_spec(estimators)
+        if estimators and all(isinstance(e, InformationGain) for e in estimators):
+            if not all(_raw_inputs(e.model) for e in estimators):
+                raise TypeError("DifferentialEvolution needs InformationGain on robo_b200 GaussianProcess models")
+            return "es", [e._ready_handle() for e in estimators]
+        return "acq", self._acq_spec()
+
+    def _acq_spec(self):
         """(kind, eta per model, par, handles) of the acquisition, or TypeError when it does not run on device GPs
         whose inputs go to the handle untransformed."""
         acq = self.objective_func
@@ -72,15 +96,23 @@ class DifferentialEvolution(BaseMaximizer):
         return float(a.ravel()[0])
 
     def maximize(self):
-        kind, etas, par, handles = self._device_spec()
+        which, spec = self._device_spec()
         lower, upper = np.asarray(self.lower, dtype=np.float64), np.asarray(self.upper, dtype=np.float64)
         seed = (self.seed + 0x9E3779B97F4A7C15 * self.calls) & 0xFFFFFFFFFFFFFFFF
         self.calls += 1
         pop = max(5, int(self.popsize) * lower.size)                 # scipy: max(5, popsize * D)
-        r = _lib.maximize_de(handles, seed, pop, int(self.n_iters), self.mutation, self.recombination, self.tol,
-                             self.atol, lower, upper, _lib.ACQ_KIND[kind], etas, par)
-        if kind == "ei" and r["n_negative"] > 0:
-            raise ValueError("Expected Improvement is smaller than 0!")          # ei.py:86-88
+        args = (seed, pop, int(self.n_iters), self.mutation, self.recombination, self.tol, self.atol, lower, upper)
+        if which == "es_cost":
+            ho, hc, lo, up, bo, bc, oh = spec
+            r = _lib.maximize_de_es_cost(ho, hc, *args, cfg_lower=lo, cfg_upper=up, basis_objective=bo, basis_cost=bc,
+                                         overhead=oh)
+        elif which == "es":
+            r = _lib.maximize_de_es(spec, *args)
+        else:
+            kind, etas, par, handles = spec
+            r = _lib.maximize_de(handles, *args, kind=_lib.ACQ_KIND[kind], eta=etas, par=par)
+            if kind == "ei" and r["n_negative"] > 0:
+                raise ValueError("Expected Improvement is smaller than 0!")      # ei.py:86-88
         x, fun, nfev, polished = r["x"], r["energy"], r["nfev"], False
         if self.polish:
             res = scipy.optimize.minimize(self._objective, np.copy(x), method="L-BFGS-B",
