@@ -374,6 +374,29 @@ int gpk_maximize_de_es_cost(gpk_handle* const* objective, gpk_handle* const* cos
                             double* best_x, double* best_energy, int* nit, long* nfev, double* population,
                             double* energies);
 
+/* The representer points of n entropy-search estimators in one call: the emcee 2.x stretch move (a = 2) of
+ * robo_b200/util/ensemble_sampler.py, replacing the host loops of information_gain.py:68-81 and
+ * information_gain_per_unit_cost.py:152-172.  Estimator i walks nb walkers of dimension dw on models[i], seeded by
+ * seeds[i] alone (Philox4x32-10; the counter layout and every rounding step are in robo_b200/csrc/gpk_rs.cuh): walkers
+ * start uniformly in [lower, upper] (dw each), each half of the ensemble proposes in turn, and each model scores its own
+ * half-batch of nb / 2 rows on its own stream with the closed form acq_kind (EI / LogEI / PI / LCB, eta[i], par), as
+ * gpk_acq would.  The log-density is -inf outside [lower, upper] and where the acquisition is NaN.
+ *   fabolas = 0: dw = d, the walker is the scored row.
+ *   fabolas = 1: dw = d - 1, the scored row is [walker, env_value] mapped as FabolasGP.normalize maps it
+ *                (cfg_lower / cfg_upper: d - 1 entries, basis: gpk_basis), bit-identical to numpy.
+ * A run is `steps` steps; an estimator whose final log-probabilities are not all finite runs again (run index + 1) up to
+ * max_runs runs, the others keep their result.  Each run ends in one 4-byte-per-estimator device-to-host copy.
+ * Out: zb (n x nb x dw) and lmb (n x nb) of the last run of each estimator, runs (n), n_accepted (n x nb, accepted moves
+ * of that run per walker; may be NULL), n_negative (may be NULL): the number of in-box EI values < 0 met (ei.py:86-88
+ * raises on them).  GPK_BAD_ARG: n < 1, nb odd, nb < 2 dw or nb > 64, steps < 1, max_runs < 1, acq_kind out of range,
+ * lower >= upper, dw != d (fabolas = 0) or d - 1 (fabolas = 1), an unknown basis code or cfg_lower >= cfg_upper,
+ * handles on different devices, with different d, listed twice, not fitted, or with a multi-rank communicator. */
+int gpk_sample_representers(gpk_handle* const* models, int n, const unsigned long long* seeds, int nb, int steps,
+                            int max_runs, int acq_kind, const double* eta, double par,
+                            const double* lower, const double* upper, int dw,
+                            int fabolas, const double* cfg_lower, const double* cfg_upper, int basis, double env_value,
+                            double* zb, double* lmb, int* runs, long* n_accepted, long* n_negative);
+
 /* kernel.get_value(X1, X2) (test/test_models/test_gaussian_process.py:44-46) with the
  * handle's current kernel; no input scaling.  out is (n1, n2) row-major. */
 int gpk_kernel_matrix(gpk_handle* h, const double* X1, long n1, const double* X2, long n2,

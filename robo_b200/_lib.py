@@ -92,6 +92,9 @@ _SIGNATURES = {
     "gpk_maximize_de_es_cost": [C.POINTER(_vp), C.POINTER(_vp), C.c_int, C.c_ulonglong, C.c_long, C.c_int, C.c_double,
                                 C.c_double, C.c_double, C.c_double, C.c_double, _dp, _dp, _dp, _dp, C.c_int, C.c_int,
                                 C.c_int, C.c_double, _dp, _dp, _ip, _lp, _dp, _dp],
+    "gpk_sample_representers": [C.POINTER(_vp), C.c_int, C.POINTER(C.c_ulonglong), C.c_int, C.c_int, C.c_int, C.c_int,
+                                _dp, C.c_double, _dp, _dp, C.c_int, C.c_int, _dp, _dp, C.c_int, C.c_double, _dp, _dp,
+                                _ip, _lp, _lp],
     "gpk_get_timings": [_vp, _dp],
     "gpk_get_diag_profile": [_vp, C.POINTER(C.c_longlong)],
 }
@@ -710,6 +713,44 @@ def maximize_de_es_cost(objective, cost, seed, pop, maxiter, mutation, recombina
                                              C.byref(be), C.byref(nit), C.byref(nfev),
                                              _as_dp(P) if P is not None else None, _as_dp(E) if E is not None else None))
     return _de_result(x, be, nit, nfev, P, E, want_population)
+
+
+def sample_representers(models, seeds, nb, steps, max_runs, kind, eta, par, lower, upper, fabolas=None):
+    """gpk_sample_representers: the stretch-move representer points of one estimator per handle in ``models``.
+    seeds (n,) 64-bit, eta (n,), lower / upper (dw,) the walker box; fabolas = None or dict(cfg_lower, cfg_upper, basis,
+    env_value) (the scored row is [walker, env_value] under the model's Fabolas transform) -> dict(zb (n, nb, dw),
+    lmb (n, nb), runs (n,), n_accepted (n, nb), n_negative)."""
+    n = len(models)
+    if n < 1:
+        raise ValueError("sample_representers: need at least one model")
+    h0 = models[0]
+    hs = (_vp * n)(*[h._h for h in models])
+    sd = np.ascontiguousarray(np.asarray(seeds, dtype=np.uint64).ravel())
+    etas = f64(np.broadcast_to(np.asarray(eta, dtype=np.float64), (n,)))
+    lo, up = f64(lower).ravel(), f64(upper).ravel()
+    if sd.size != n or lo.size != up.size:
+        raise ValueError("sample_representers: need one seed per model and lower / upper of one length")
+    dw, nb = lo.size, int(nb)
+    if fabolas is not None:
+        clo, cup = f64(fabolas["cfg_lower"]).ravel(), f64(fabolas["cfg_upper"]).ravel()
+        if clo.size != dw or cup.size != dw:
+            raise ValueError("sample_representers: the configuration bounds need dw = d - 1 entries")
+        basis, env = int(fabolas["basis"]), float(fabolas["env_value"])
+    else:
+        clo = cup = None
+        basis, env = 0, 0.0
+    zb = np.empty((n, max(nb, 0), dw))
+    lmb = np.empty((n, max(nb, 0)))
+    acc = np.zeros((n, max(nb, 0)), dtype=np.int64)
+    runs = np.zeros(n, dtype=np.int32)
+    nn = C.c_long(0)
+    h0._check(h0.lib.gpk_sample_representers(hs, n, sd.ctypes.data_as(C.POINTER(C.c_ulonglong)), nb, int(steps),
+                                             int(max_runs), int(kind), _as_dp(etas), float(par), _as_dp(lo), _as_dp(up),
+                                             dw, int(fabolas is not None), _as_dp(clo) if clo is not None else None,
+                                             _as_dp(cup) if cup is not None else None, basis, env, _as_dp(zb),
+                                             _as_dp(lmb), runs.ctypes.data_as(_ip), acc.ctypes.data_as(_lp),
+                                             C.byref(nn)))
+    return dict(zb=zb, lmb=lmb, runs=runs, n_accepted=acc, n_negative=nn.value)
 
 
 _moments_handle = {}

@@ -2,7 +2,8 @@
 and Schuler, JMLR 2012) with its numerical work on the GPU.
 
 update(): the representer points zb are drawn by the ensemble sampler from the sampling acquisition (each
-half-ensemble scored in ONE call of the fused acquisition); p_min over zb by EP, the derivatives of log p_min and
+half-ensemble scored in ONE call of the fused acquisition), or with representer_sampler="device" by the stretch move on
+the device (gpk_sample_representers: the same algorithm, a Philox stream, equal in law only); p_min over zb by EP, the derivatives of log p_min and
 U = K^-1 K(X, zb) are computed and kept on the device (gpk_es_update).  compute(): the entropy change of every
 candidate in one batched call (gpk_es_compute): the reference loops over candidates with one predict and one
 (Nb + 1)-point predict(full_cov=True) each.  innovations() stays a host method, as in the reference.
@@ -32,10 +33,46 @@ def _device_model(model):
     return model.gp.handle
 
 
+_DEVICE_KINDS = ("ei", "log_ei", "pi", "lcb")
+
+
+def sample_representers_device(estimators):
+    """The representer points of every estimator (InformationGain or InformationGainPerUnitCost) drawn on the device by
+    the stretch move (gpk_sample_representers), one call for all estimators that share the sampler's arguments.  Each
+    estimator draws its seed from its own rng (one draw per update); eta is its sampling acquisition's incumbent value
+    (0 for LCB).  Raises TypeError when an estimator cannot sample on the device, and the reference's ValueErrors:
+    ei.py's on a negative EI value, and InformationGainPerUnitCost's when -inf remains after 5 runs."""
+    from robo_b200 import _lib
+    calls = {}
+    for e in estimators:
+        sa = e.sampling_acquisition
+        kind = getattr(sa, "kind", None)
+        if kind not in _DEVICE_KINDS or not hasattr(sa, "par"):
+            raise TypeError("representer_sampler='device' needs EI, LogEI, PI or LCB as the sampling acquisition")
+        sa.update(e.model)
+        handle, lower, upper, fabolas = e._representer_spec()
+        eta = 0.0 if kind == "lcb" else float(e.model.get_incumbent()[1])
+        seed = int(e.rng.randint(0, 2 ** 63, dtype=np.int64))
+        key = (kind, float(sa.par), int(e.Nb), lower.tobytes(), upper.tobytes(),
+               None if fabolas is None else tuple((k, np.asarray(v).tobytes()) for k, v in sorted(fabolas.items())))
+        calls.setdefault(key, (kind, float(sa.par), int(e.Nb), lower, upper, fabolas, []))[-1].append(
+            (e, handle, seed, eta))
+    for kind, par, nb, lower, upper, fabolas, members in calls.values():
+        r = _lib.sample_representers([m[1] for m in members], [m[2] for m in members], nb, 50, 5, _lib.ACQ_KIND[kind],
+                                     [m[3] for m in members], par, lower, upper, fabolas=fabolas)
+        if kind == "ei" and r["n_negative"] > 0:
+            raise ValueError("Expected Improvement is smaller than 0!")      # ei.py:86-88
+        for i, (e, _, _, _) in enumerate(members):
+            e._set_representers(r["zb"][i], r["lmb"][i])
+
+
 class InformationGain(BaseAcquisitionFunction):
 
     def __init__(self, model, lower, upper, Nb=50, Np=400, sampling_acquisition=None,
-                 sampling_acquisition_kw={"par": 0.0}, rng=None, **kwargs):
+                 sampling_acquisition_kw={"par": 0.0}, rng=None, representer_sampler="host", **kwargs):
+        if representer_sampler not in ("host", "device"):
+            raise ValueError("representer_sampler must be 'host' or 'device', not %r" % (representer_sampler,))
+        self.representer_sampler = representer_sampler
         self.Nb = Nb
         super(InformationGain, self).__init__(model)
         self.lower = lower
@@ -66,6 +103,9 @@ class InformationGain(BaseAcquisitionFunction):
         return out
 
     def sample_representer_points(self):
+        if self.representer_sampler == "device":
+            sample_representers_device([self])
+            return
         self.sampling_acquisition.update(self.model)
         for i in range(5):
             restarts = self.lower + (self.upper - self.lower) * self.rng.uniform(size=(self.Nb, self.D))
@@ -87,11 +127,27 @@ class InformationGain(BaseAcquisitionFunction):
     def _device_zb(self):
         return self.zb
 
+    # the device sampler's view of this estimator: its handle, the walker box and the Fabolas arguments (None here)
+    def _representer_spec(self):
+        return self._device_handle(self.model), np.asarray(self.lower, dtype=np.float64), \
+            np.asarray(self.upper, dtype=np.float64), None
+
+    def _set_representers(self, zb, lmb):
+        self.zb, self.lmb = zb, lmb[:, None]
+
     def update(self, model):
+        handle = self._begin_update(model)
+        self.sample_representer_points()
+        self._end_update(handle)
+
+    # update() around the representer points, so that MarginalizationGPMCMC can draw those of all estimators in one call
+    def _begin_update(self, model):
         self.model = model
         handle = self._device_handle(model)
         self.sn2 = self.model.get_noise()
-        self.sample_representer_points()
+        return handle
+
+    def _end_update(self, handle):
         self.W = scipy.stats.norm.ppf(np.linspace(1. / (self.Np + 1), 1 - 1. / (self.Np + 1), self.Np))[np.newaxis, :]
         r = handle.es_update(self._device_zb(), self.lmb, self.sn2, self.W, self.lower, self.upper)
         self.logP = np.reshape(r["logP"], (self.Nb, 1))

@@ -20,7 +20,7 @@ import logging
 import numpy as np
 
 from robo_b200 import _lib
-from robo_b200.acquisition_functions.information_gain import InformationGain
+from robo_b200.acquisition_functions.information_gain import InformationGain, sample_representers_device
 from robo_b200.util.ensemble_sampler import EnsembleSampler
 
 logger = logging.getLogger(__name__)
@@ -90,21 +90,50 @@ def device_spec(pairs):
 class InformationGainPerUnitCost(InformationGain):
 
     def __init__(self, model, cost_model, lower, upper, is_env_variable, sampling_acquisition=None, n_representer=50,
-                 rng=None):
+                 rng=None, representer_sampler="host"):
         self.cost_model = cost_model
         self.n_dims = lower.shape[0]
         self.is_env = is_env_variable
         self.overhead = 0
         super(InformationGainPerUnitCost, self).__init__(model, lower, upper, sampling_acquisition=sampling_acquisition,
-                                                         Nb=n_representer, rng=rng)
+                                                         Nb=n_representer, rng=rng,
+                                                         representer_sampler=representer_sampler)
 
     def update(self, model, cost_model, overhead=None):
+        self._set_cost(cost_model, overhead)
+        super(InformationGainPerUnitCost, self).update(model)
+
+    def _set_cost(self, cost_model, overhead=None):
         self.cost_model = cost_model
         if overhead is None:
             self.overhead = 0
         else:
             self.overhead = overhead
-        super(InformationGainPerUnitCost, self).update(model)
+
+    # the device sampler's view: walkers in the configuration columns, scored at the environment's upper bound through
+    # the objective's Fabolas transform (sampling_acquisition_wrapper); one environment column, the last one
+    def _representer_spec(self):
+        is_env = np.asarray(self.is_env).ravel()
+        if int(np.sum(is_env == 1)) != 1 or is_env[-1] != 1 or is_env.size != self.lower.shape[0]:
+            raise TypeError("representer_sampler='device' needs exactly one environment column, the last one")
+        handle = self._device_handle(self.model)
+        lower, upper = self._config_bounds()
+        fabolas = dict(cfg_lower=np.asarray(self.model.lower, dtype=np.float64).ravel(),
+                       cfg_upper=np.asarray(self.model.upper, dtype=np.float64).ravel(),
+                       basis=basis_code(self.model.basis_function), env_value=float(self.upper[is_env == 1][0]))
+        return handle, np.asarray(lower, dtype=np.float64), np.asarray(upper, dtype=np.float64), fabolas
+
+    def _set_representers(self, zb, lmb):
+        if np.any(np.isinf(lmb)):
+            raise ValueError("Could not sample valid representer points! LogEI is -infinity")
+        self.zb, self.lmb = zb, lmb[:, None]
+        self._append_env_column()
+
+    def _append_env_column(self):
+        # information_gain_per_unit_cost.py:151-153: the environment coordinate is the number of environment dimensions
+        proj = np.ones([self.zb.shape[0], self.upper[self.is_env == 1].shape[0]])
+        proj *= self.upper[self.is_env == 1].shape[0]
+        self.zb = np.concatenate((self.zb, proj), axis=1)
 
     # InformationGain.update's device hooks: FabolasGP handle; zb transformed on the host as the model maps its inputs
     def _device_handle(self, model):
@@ -150,6 +179,9 @@ class InformationGainPerUnitCost(InformationGain):
         return out
 
     def sample_representer_points(self):
+        if self.representer_sampler == "device":
+            sample_representers_device([self])
+            return
         D = np.where(self.is_env == 0)[0].shape[0]
         lower, upper = self._config_bounds()
         self.sampling_acquisition.update(self.model)
@@ -166,7 +198,4 @@ class InformationGainPerUnitCost(InformationGain):
             self.zb = self.zb[:, None]
         if len(self.lmb.shape) == 1:
             self.lmb = self.lmb[:, None]
-        # information_gain_per_unit_cost.py:151-153: the environment coordinate is the number of environment dimensions
-        proj = np.ones([self.zb.shape[0], self.upper[self.is_env == 1].shape[0]])
-        proj *= self.upper[self.is_env == 1].shape[0]
-        self.zb = np.concatenate((self.zb, proj), axis=1)
+        self._append_env_column()

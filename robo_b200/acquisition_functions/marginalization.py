@@ -37,6 +37,19 @@ class MarginalizationGPMCMC(BaseAcquisitionFunction):
         if len(self.estimators) != len(self.model.models):
             self.estimators = []
             self._make_estimators()
+        from robo_b200.acquisition_functions.information_gain import InformationGain, sample_representers_device
+        if all(isinstance(e, InformationGain) and e.representer_sampler == "device" for e in self.estimators):
+            # the representer points of every estimator in one device call (gpk_sample_representers), then each
+            # estimator's EP and U as in its own update()
+            handles = []
+            for i, e in enumerate(self.estimators):
+                if cost_model is not None:
+                    e._set_cost(self.cost_model.models[i], **kwargs)
+                handles.append(e._begin_update(self.model.models[i]))
+            sample_representers_device(self.estimators)
+            for e, h in zip(self.estimators, handles):
+                e._end_update(h)
+            return
         for i in range(len(self.model.models)):
             if cost_model is not None:
                 self.estimators[i].update(self.model.models[i], self.cost_model.models[i], **kwargs)

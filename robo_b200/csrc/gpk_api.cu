@@ -27,6 +27,7 @@
 #include "gpk_ozaki.cuh"
 #include "gpk_de.cuh"
 #include "gpk_es.cuh"
+#include "gpk_rs.cuh"
 
 namespace {
 
@@ -148,6 +149,9 @@ struct gpk_handle {
     // information gain per unit cost (gpk_es_cost_multi): the batch under the objective's and the cost's Fabolas
     // transform and the configuration bounds; owned by the first objective handle of the call
     DevBuf fab_in;
+    // representer sampling (gpk_sample_representers): walkers, log-probabilities, proposals, scored batches, bounds,
+    // accept counts, seeds, slots; owned by the first handle of the call
+    DevBuf rs_buf;
     int es_nb = 0, es_np = 0;
     double es_sn2 = 0.0, es_H = 0.0;
     long es_linv_serial = -1;       // linv_serial U was built for (-1: no update yet)
@@ -1160,7 +1164,7 @@ int gpk_destroy(gpk_handle* h) {
                       &h->out_var, &h->out_acq, &h->block_best, &h->best, &h->nneg, &h->Vt, &h->cov, &h->XsT,
                       &h->tmpjobs, &h->alpha, &h->tmp1, &h->tmp2, &h->tmp3, &h->chain_cnt, &h->dprof, &h->Xts, &h->oz_Pq, &h->oz_Kq, &h->oz_Kq2, &h->oz_eP, &h->oz_emax, &h->oz_pmu2, &h->oz_probe,
                       &h->multi_cand, &h->multi_A, &h->multi_B, &h->multi_out, &h->multi_bb, &h->gather, &h->best_global,
-                      &h->de_pop, &h->de_trial, &h->de_param, &h->de_E, &h->de_small, &h->de_sort, &h->ep_buf, &h->es_state, &h->es_U, &h->es_work, &h->es_in, &h->fab_in};
+                      &h->de_pop, &h->de_trial, &h->de_param, &h->de_E, &h->de_small, &h->de_sort, &h->ep_buf, &h->es_state, &h->es_U, &h->es_work, &h->es_in, &h->fab_in, &h->rs_buf};
     for (DevBuf* b : bufs)
         if (b->p) cudaFree(b->p);
     if (h->ev_ok)

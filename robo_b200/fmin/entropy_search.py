@@ -16,7 +16,7 @@ from robo_b200.solver import BayesianOptimization
 
 
 def entropy_search(objective_function, lower, upper, num_iterations=30, maximizer="random", model="gp_mcmc",
-                   X_init=None, Y_init=None, n_init=3, output_path=None, rng=None):
+                   X_init=None, Y_init=None, n_init=3, output_path=None, rng=None, representer_sampler="host"):
     assert upper.shape[0] == lower.shape[0], "Dimension miss match"
     assert np.all(lower < upper), "Lower bound >= upper bound"
     assert n_init <= num_iterations, "Number of initial design point has to be <= than the number of iterations"
@@ -43,7 +43,8 @@ def entropy_search(objective_function, lower, upper, num_iterations=30, maximize
     else:
         raise ValueError("'{}' is not a valid model on the GPU path (gp, gp_mcmc)".format(model))
 
-    a = InformationGain(gp, lower=lower, upper=upper, sampling_acquisition=EI)
+    # representer_sampler="device" draws the representer points on the device (gpk_sample_representers)
+    a = InformationGain(gp, lower=lower, upper=upper, sampling_acquisition=EI, representer_sampler=representer_sampler)
     acquisition_func = a if model == "gp" else MarginalizationGPMCMC(a)
     if maximizer == "random":
         max_func = RandomSampling(acquisition_func, lower, upper, rng=rng)
