@@ -56,6 +56,18 @@ typedef enum {
 
 #define GPK_MAX_TERMS 64   /* metric entries (input dims x product factors) per kernel */
 
+/* hyper-parameter sampling (gpk_sample_hypers): the factor of one theta lives in one SM's shared memory as a packed fp64
+ * lower triangle, which bounds the training points; theta holds at most GPK_HYPER_MAX_DIM entries (noise included) */
+#define GPK_HYPER_MAX_N 232
+#define GPK_HYPER_MAX_DIM 96
+
+/* hyper-priors the device restates (robo/priors/default_priors.py, robo/priors/env_priors.py) */
+typedef enum {
+    GPK_PRIOR_NONE = 0,
+    GPK_PRIOR_DEFAULT = 1,     /* DefaultPrior */
+    GPK_PRIOR_ENV = 2          /* EnvPrior     */
+} gpk_prior_kind;
+
 /* ---- lifetime ---------------------------------------------------------------------- */
 int gpk_create(gpk_handle** h, int device);
 int gpk_destroy(gpk_handle* h);
@@ -396,6 +408,34 @@ int gpk_sample_representers(gpk_handle* const* models, int n, const unsigned lon
                             const double* lower, const double* upper, int dw,
                             int fabolas, const double* cfg_lower, const double* cfg_upper, int basis, double env_value,
                             double* zb, double* lmb, int* runs, long* n_accepted, long* n_negative);
+
+/* ---- GP-MCMC hyper-parameters on the device (robo_b200/csrc/gpk_hyper.cuh) ---------------------------------------
+ * GaussianProcessMCMC.train's stretch-move chain over theta = (kernel parameters, log noise) with every walker's
+ * log-posterior computed on chip: the kernel built from theta on the inputs of gpk_set_data, a Cholesky factor in shared
+ * memory (n <= GPK_HYPER_MAX_N), the prior restated on the device.
+ *
+ * gpk_set_hyper_model: how theta maps to the handle's kernel structure (family, axes, groups of the last gpk_set_kernel;
+ *   its parameter values are not used).  n_params = len(kernel) (theta has n_params + 1 entries, the log noise last);
+ *   amp_slot[p] = 1 when parameter p is an amplitude slot (log_amp = 0.0 + those entries in order), 0 for a metric slot;
+ *   term_param[t] (n_terms entries) = the metric slot that sets term t (kernels.py flatten()["slots"]).  The diagonal is
+ *   fl(sqrt(fl(yerr^2 + tiny)))^2 with yerr = sqrt(exp(theta[-1])), the constant mean `mean`.  prior_kind: gpk_prior_kind;
+ *   prior_par (7 entries, NULL for GPK_PRIOR_NONE) = lognormal sigma, lognormal mean (scipy's loc), tophat lower, tophat
+ *   upper, horseshoe scale, normal sigma, normal mean (the last two for GPK_PRIOR_ENV); n_ls, n_lr: EnvPrior's slices.
+ * gpk_hyper_lnpost: the log-likelihood ll (-inf for any |theta_j| > 20, a pivot that is not > 0 or a non-finite result)
+ *   and the log-prior lp (0 without a prior) of count thetas (count x dim); the sampler's log-posterior is lp + ll where
+ *   ll is finite (ll alone without a prior), -inf otherwise, NaN -> -inf.  The same device routine and block shape as
+ *   gpk_sample_hypers: the values are the ones the sampler sees, bit for bit.
+ * gpk_sample_hypers: one EnsembleSampler.run_mcmc(p0, steps): nwalkers x dim walkers from p0, the initial
+ *   log-posteriors, then `steps` steps of two half-steps (one launch each, no host synchronisation), keyed by `seed`
+ *   (Philox4x32-10; the counter layout and the rounding are in gpk_hyper.cuh).  Out: pos (nwalkers x dim), lnpost
+ *   (nwalkers), n_accepted (nwalkers, may be NULL), copied back in one transfer at the end.
+ * GPK_BAD_ARG: no data or kernel, no hyper model, n > GPK_HYPER_MAX_N, dim != n_params + 1, an odd number of walkers or
+ * fewer than 2 dim, steps < 0, a slot table that does not cover the kernel's terms, an unknown prior kind. */
+int gpk_set_hyper_model(gpk_handle* h, int n_params, const int* amp_slot, const int* term_param, int n_terms,
+                        double mean, double tiny, int prior_kind, const double* prior_par, int n_ls, int n_lr);
+int gpk_hyper_lnpost(gpk_handle* h, const double* theta, int count, int dim, double* ll, double* lp);
+int gpk_sample_hypers(gpk_handle* h, const double* p0, int nwalkers, int dim, int steps, unsigned long long seed,
+                      double* pos, double* lnpost, long* n_accepted);
 
 /* kernel.get_value(X1, X2) (test/test_models/test_gaussian_process.py:44-46) with the
  * handle's current kernel; no input scaling.  out is (n1, n2) row-major. */

@@ -20,6 +20,9 @@ MATERN52, EXPSQUARED, MATERN32 = 0, 1, 2
 ACQ_NONE, ACQ_EI, ACQ_LOG_EI, ACQ_PI, ACQ_LCB = range(5)
 ACQ_KIND = {"ei": ACQ_EI, "log_ei": ACQ_LOG_EI, "pi": ACQ_PI, "lcb": ACQ_LCB, "none": ACQ_NONE}
 BASIS_S, BASIS_ONE_MINUS_S_SQ = range(2)      # gpk_basis: the environment column's basis of a Fabolas model
+PRIOR_NONE, PRIOR_DEFAULT, PRIOR_ENV = range(3)   # gpk_prior_kind: the hyper-priors gpk_sample_hypers restates
+HYPER_MAX_N = 232                              # GPK_HYPER_MAX_N: most training points of gpk_sample_hypers
+HYPER_MAX_DIM = 96                             # GPK_HYPER_MAX_DIM: most entries of theta (log noise included)
 
 _dp = C.POINTER(C.c_double)
 _ip = C.POINTER(C.c_int)
@@ -95,6 +98,9 @@ _SIGNATURES = {
     "gpk_sample_representers": [C.POINTER(_vp), C.c_int, C.POINTER(C.c_ulonglong), C.c_int, C.c_int, C.c_int, C.c_int,
                                 _dp, C.c_double, _dp, _dp, C.c_int, C.c_int, _dp, _dp, C.c_int, C.c_double, _dp, _dp,
                                 _ip, _lp, _lp],
+    "gpk_set_hyper_model": [_vp, C.c_int, _ip, _ip, C.c_int, C.c_double, C.c_double, C.c_int, _dp, C.c_int, C.c_int],
+    "gpk_hyper_lnpost": [_vp, _dp, C.c_int, C.c_int, _dp, _dp],
+    "gpk_sample_hypers": [_vp, _dp, C.c_int, C.c_int, C.c_int, C.c_ulonglong, _dp, _dp, _lp],
     "gpk_get_timings": [_vp, _dp],
     "gpk_get_diag_profile": [_vp, C.POINTER(C.c_longlong)],
 }
@@ -751,6 +757,49 @@ def sample_representers(models, seeds, nb, steps, max_runs, kind, eta, par, lowe
                                              _as_dp(lmb), runs.ctypes.data_as(_ip), acc.ctypes.data_as(_lp),
                                              C.byref(nn)))
     return dict(zb=zb, lmb=lmb, runs=runs, n_accepted=acc, n_negative=nn.value)
+
+
+def set_hyper_model(handle, slots, n_terms, mean, tiny, prior_kind=PRIOR_NONE, prior_par=None, n_ls=0, n_lr=0):
+    """gpk_set_hyper_model: theta -> the handle's kernel (set_kernel first; its structure is used, not its values).
+    slots: kernels.py flatten()["slots"] (one ("amp", None) or ("metric", [terms]) per kernel parameter); n_terms: the
+    kernel's metric terms; mean / tiny: the constant mean and the jitter added to yerr^2; prior_par: the 7 constants of
+    include/gpk.h (None without a prior)."""
+    amp = np.array([1 if kind == "amp" else 0 for kind, _ in slots], dtype=np.int32)
+    term = np.full(int(n_terms), -1, dtype=np.int32)
+    for p, (kind, terms) in enumerate(slots):
+        if kind == "metric":
+            for t in terms:
+                if not 0 <= t < n_terms:
+                    raise ValueError("set_hyper_model: slot %d names term %d of %d" % (p, t, n_terms))
+                term[t] = p
+    par = f64(prior_par).ravel() if prior_par is not None else None
+    if par is not None and par.size != 7:
+        raise ValueError("set_hyper_model: the prior needs 7 constants")
+    handle._check(handle.lib.gpk_set_hyper_model(handle._h, amp.size, amp.ctypes.data_as(_ip), term.ctypes.data_as(_ip),
+                                                 term.size, float(mean), float(tiny), int(prior_kind),
+                                                 _as_dp(par) if par is not None else None, int(n_ls), int(n_lr)))
+
+
+def hyper_lnpost(handle, thetas):
+    """gpk_hyper_lnpost: (log-likelihood, log-prior) of every row of thetas (count, dim), as gpk_sample_hypers computes
+    them."""
+    T = f64(np.atleast_2d(thetas))
+    count, dim = T.shape
+    ll, lp = np.empty(count), np.empty(count)
+    handle._check(handle.lib.gpk_hyper_lnpost(handle._h, _as_dp(T), count, dim, _as_dp(ll), _as_dp(lp)))
+    return ll, lp
+
+
+def sample_hypers(handle, p0, steps, seed):
+    """gpk_sample_hypers: one stretch-move run of the walkers p0 (nwalkers, dim) for `steps` steps ->
+    dict(pos (nwalkers, dim), lnpost (nwalkers,), n_accepted (nwalkers,))."""
+    P = f64(np.atleast_2d(p0))
+    nw, dim = P.shape
+    pos, lnp = np.empty((nw, dim)), np.empty(nw)
+    acc = np.zeros(nw, dtype=np.int64)
+    handle._check(handle.lib.gpk_sample_hypers(handle._h, _as_dp(P), nw, dim, int(steps), int(seed) & 0xFFFFFFFFFFFFFFFF,
+                                               _as_dp(pos), _as_dp(lnp), acc.ctypes.data_as(_lp)))
+    return dict(pos=pos, lnpost=lnp, n_accepted=acc)
 
 
 _moments_handle = {}

@@ -28,6 +28,7 @@
 #include "gpk_de.cuh"
 #include "gpk_es.cuh"
 #include "gpk_rs.cuh"
+#include "gpk_hyper.cuh"
 
 namespace {
 
@@ -152,6 +153,10 @@ struct gpk_handle {
     // representer sampling (gpk_sample_representers): walkers, log-probabilities, proposals, scored batches, bounds,
     // accept counts, seeds, slots; owned by the first handle of the call
     DevBuf rs_buf;
+    // hyper-parameter sampling (gpk_sample_hypers): theta -> kernel map and prior, walkers / log-posteriors / accepts
+    bool has_hyper = false;
+    HyperModel hyper;
+    DevBuf hy_buf;
     int es_nb = 0, es_np = 0;
     double es_sn2 = 0.0, es_H = 0.0;
     long es_linv_serial = -1;       // linv_serial U was built for (-1: no update yet)
@@ -1164,7 +1169,7 @@ int gpk_destroy(gpk_handle* h) {
                       &h->out_var, &h->out_acq, &h->block_best, &h->best, &h->nneg, &h->Vt, &h->cov, &h->XsT,
                       &h->tmpjobs, &h->alpha, &h->tmp1, &h->tmp2, &h->tmp3, &h->chain_cnt, &h->dprof, &h->Xts, &h->oz_Pq, &h->oz_Kq, &h->oz_Kq2, &h->oz_eP, &h->oz_emax, &h->oz_pmu2, &h->oz_probe,
                       &h->multi_cand, &h->multi_A, &h->multi_B, &h->multi_out, &h->multi_bb, &h->gather, &h->best_global,
-                      &h->de_pop, &h->de_trial, &h->de_param, &h->de_E, &h->de_small, &h->de_sort, &h->ep_buf, &h->es_state, &h->es_U, &h->es_work, &h->es_in, &h->fab_in, &h->rs_buf};
+                      &h->de_pop, &h->de_trial, &h->de_param, &h->de_E, &h->de_small, &h->de_sort, &h->ep_buf, &h->es_state, &h->es_U, &h->es_work, &h->es_in, &h->fab_in, &h->rs_buf, &h->hy_buf};
     for (DevBuf* b : bufs)
         if (b->p) cudaFree(b->p);
     if (h->ev_ok)
@@ -2252,6 +2257,138 @@ int gpk_reduce_models(gpk_handle* h, const double* A, const double* B, int n_mod
     CK(cudaMemcpyAsync(out1, o1, (size_t)m * 8, cudaMemcpyDeviceToHost, h->stream));
     if (mode == 1) CK(cudaMemcpyAsync(out2, o2, (size_t)m * 8, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
+    return GPK_OK;
+}
+
+// ---------------------------------------------------------------------------------------
+// GP-MCMC hyper-parameters on the device (gpk_hyper.cuh; GaussianProcessMCMC.train, gaussian_process_mcmc.py:114-142)
+// ---------------------------------------------------------------------------------------
+int gpk_set_hyper_model(gpk_handle* h, int n_params, const int* amp_slot, const int* term_param, int n_terms,
+                        double mean, double tiny, int prior_kind, const double* prior_par, int n_ls, int n_lr) {
+    if (!h) return GPK_BAD_ARG;
+    const char* who = "gpk_set_hyper_model";
+    h->has_hyper = false;
+    if (!h->has_spec) BAD("%s: gpk_set_kernel has not been called", who);
+    if (n_params < 1 || n_params + 1 > GPK_HYPER_MAX_DIM || !amp_slot || !term_param)
+        BAD("%s: need 1 <= n_params <= %d and the slot table", who, GPK_HYPER_MAX_DIM - 1);
+    if (n_terms != h->spec.n_terms) BAD("%s: %d terms in the slot table, the kernel has %d", who, n_terms, h->spec.n_terms);
+    if (prior_kind < GPK_PRIOR_NONE || prior_kind > GPK_PRIOR_ENV) BAD("%s: unknown prior kind %d", who, prior_kind);
+    if (prior_kind != GPK_PRIOR_NONE && !prior_par) BAD("%s: the prior needs its constants", who);
+    if (prior_kind == GPK_PRIOR_ENV && (n_ls < 0 || n_lr < 0)) BAD("%s: need n_ls >= 0 and n_lr >= 0", who);
+    HyperModel m;
+    memset(&m, 0, sizeof(m));
+    m.family = h->spec.family;
+    m.n_terms = n_terms;
+    m.n_params = n_params;
+    std::vector<int> used(n_params, 0);
+    for (int p = 0; p < n_params; ++p) m.amp[p] = amp_slot[p] ? 1 : 0;
+    for (int t = 0; t < n_terms; ++t) {
+        const int p = term_param[t];
+        if (p < 0 || p >= n_params || m.amp[p]) BAD("%s: term %d is not set by a metric slot", who, t);
+        m.axis[t] = h->spec.axis[t];
+        m.last[t] = h->spec.last[t];
+        m.term_param[t] = p;
+        used[p] = 1;
+    }
+    for (int p = 0; p < n_params; ++p)
+        if (!m.amp[p] && !used[p]) BAD("%s: metric slot %d sets no term", who, p);
+    m.mean = mean;
+    m.tiny = tiny;
+    m.prior = prior_kind;
+    m.n_ls = n_ls;
+    m.n_lr = n_lr;
+    if (prior_kind != GPK_PRIOR_NONE) {
+        m.ln_sigma = prior_par[0]; m.ln_loc = prior_par[1]; m.th_lo = prior_par[2]; m.th_hi = prior_par[3];
+        m.hs_scale = prior_par[4]; m.nrm_sigma = prior_par[5]; m.nrm_mean = prior_par[6];
+    }
+    h->hyper = m;
+    h->has_hyper = true;
+    return GPK_OK;
+}
+
+namespace {
+// the preconditions of gpk_hyper_lnpost / gpk_sample_hypers, and the kernels' shared-memory opt-in
+int hyper_ready(gpk_handle* h, int dim, const char* who) {
+    int rc = require(h, true, true, false);
+    if (rc) return rc;
+    if (!h->has_hyper) BAD("%s: gpk_set_hyper_model has not been called", who);
+    const HyperModel& m = h->hyper;
+    if (m.n_terms != h->spec.n_terms || m.family != h->spec.family)
+        BAD("%s: the kernel structure changed since gpk_set_hyper_model", who);
+    for (int t = 0; t < m.n_terms; ++t) {
+        if (m.axis[t] != h->spec.axis[t] || m.last[t] != h->spec.last[t])
+            BAD("%s: the kernel structure changed since gpk_set_hyper_model", who);
+        if (m.axis[t] >= h->d) BAD("%s: kernel axis %d >= d = %d", who, m.axis[t], h->d);
+    }
+    if (h->n > GPK_HYPER_MAX_N) BAD("%s: n = %d exceeds GPK_HYPER_MAX_N = %d", who, h->n, GPK_HYPER_MAX_N);
+    if (dim != m.n_params + 1) BAD("%s: dim = %d, the slot table needs %d", who, dim, m.n_params + 1);
+    CK(cudaSetDevice(h->device));
+    const int smem = (int)(gpk_hy_smem_doubles(h->n) * 8);
+    CK(cudaFuncSetAttribute(gpk_hy_eval_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    CK(cudaFuncSetAttribute(gpk_hy_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    return GPK_OK;
+}
+}  // namespace
+
+int gpk_hyper_lnpost(gpk_handle* h, const double* theta, int count, int dim, double* ll, double* lp) {
+    if (!h) return GPK_BAD_ARG;
+    const char* who = "gpk_hyper_lnpost";
+    if (count < 1 || !theta || !ll || !lp) BAD("%s: need count >= 1, theta, ll and lp", who);
+    int rc = hyper_ready(h, dim, who);
+    if (rc) return rc;
+    const size_t nT = (size_t)count * dim;
+    if ((rc = ensure(h, h->hy_buf, (nT + 2 * (size_t)count) * 8))) return rc;
+    double* dT = ptr<double>(h->hy_buf);
+    double* dll = dT + nT;
+    double* dlp = dll + count;
+    CK(cudaMemcpyAsync(dT, theta, nT * 8, cudaMemcpyHostToDevice, h->stream));
+    gpk_hy_eval_kernel<<<count, GPK_HY_THREADS, gpk_hy_smem_doubles(h->n) * 8, h->stream>>>(
+        h->hyper, ptr<double>(h->Xt), h->NP, ptr<double>(h->y), h->n, dT, dll, dlp, nullptr);
+    CKL();
+    CK(cudaMemcpyAsync(ll, dll, (size_t)count * 8, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaMemcpyAsync(lp, dlp, (size_t)count * 8, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    return GPK_OK;
+}
+
+int gpk_sample_hypers(gpk_handle* h, const double* p0, int nwalkers, int dim, int steps, unsigned long long seed,
+                      double* pos, double* lnpost, long* n_accepted) {
+    static_assert(sizeof(long) == sizeof(long long) && sizeof(long long) == sizeof(double),
+                  "the accept counts travel in the walkers' transfer");
+    if (!h) return GPK_BAD_ARG;
+    const char* who = "gpk_sample_hypers";
+    if (!p0 || !pos || !lnpost) BAD("%s: need p0, pos and lnpost", who);
+    if (nwalkers % 2 != 0 || nwalkers < 2 * dim || nwalkers < 2)
+        BAD("%s: need an even number of walkers >= 2 dim (nwalkers = %d, dim = %d)", who, nwalkers, dim);
+    if (steps < 0) BAD("%s: need steps >= 0", who);
+    int rc = hyper_ready(h, dim, who);
+    if (rc) return rc;
+    // P (nwalkers x dim), L (nwalkers), accept counts (nwalkers): contiguous, so that one copy brings the run back
+    const size_t nP = (size_t)nwalkers * dim, total = nP + 2 * (size_t)nwalkers;
+    if ((rc = ensure(h, h->hy_buf, total * 8))) return rc;
+    double* P = ptr<double>(h->hy_buf);
+    double* L = P + nP;
+    long long* acc = (long long*)(L + nwalkers);
+    const size_t smem = gpk_hy_smem_doubles(h->n) * 8;
+    const double* Xt = ptr<double>(h->Xt);
+    const double* y = ptr<double>(h->y);
+    CK(cudaMemcpyAsync(P, p0, nP * 8, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemsetAsync(acc, 0, (size_t)nwalkers * 8, h->stream));
+    gpk_hy_eval_kernel<<<nwalkers, GPK_HY_THREADS, smem, h->stream>>>(h->hyper, Xt, h->NP, y, h->n, P, nullptr,
+                                                                      nullptr, L);
+    CKL();
+    for (int s = 0; s < steps; ++s)
+        for (int half = 0; half < 2; ++half) {
+            gpk_hy_step_kernel<<<nwalkers / 2, GPK_HY_THREADS, smem, h->stream>>>(h->hyper, Xt, h->NP, y, h->n,
+                                                                                nwalkers, s, half, seed, P, L, acc);
+            CKL();
+        }
+    std::vector<double> out(total);
+    CK(cudaMemcpyAsync(out.data(), P, total * 8, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    memcpy(pos, out.data(), nP * 8);
+    memcpy(lnpost, out.data() + nP, (size_t)nwalkers * 8);
+    if (n_accepted) memcpy(n_accepted, out.data() + nP + nwalkers, (size_t)nwalkers * 8);
     return GPK_OK;
 }
 

@@ -21,7 +21,7 @@
 //                      TAG_ACC); a NaN lnpdiff (-inf - -inf) rejects.  Accepted moves are counted per walker and run.
 // Counter (c0, c1, c2, c3) = (walker, step or run, 2 run + half or coordinate, tag), key = the estimator's 64-bit seed:
 // an estimator's draws depend on its seed alone, not on n, its position in the list or stream timing.  The tags are
-// disjoint from GPK_DE_TAG_* and from gpk_candidates_kernel's c3 = 0.
+// disjoint from GPK_DE_TAG_*, GPK_HY_TAG_* and from gpk_candidates_kernel's c3 = 0.
 //
 // Estimators are addressed by their index i in the call; slot[i] >= 0 is the position of an estimator that runs in the
 // current run in the compact scoring batch (n_active x nb/2 rows), slot[i] < 0 an estimator that is done.
@@ -35,6 +35,33 @@
 
 // the stretch factor's parameter a of emcee (ensemble_sampler.py: a = 2.0)
 #define GPK_RS_A 2.0
+
+// The stretch move's arithmetic, shared by this sampler and the hyper-parameter sampler (gpk_hyper.cuh); every step is
+// rounded explicitly.  z = fl(fl(t t) / a), t = fl(fl((a - 1) u01(w0, w1)) + 1)
+__device__ __forceinline__ double gpk_stretch_z(uint32_t w0, uint32_t w1)
+{
+    const double tz = __dadd_rn(__dmul_rn(GPK_RS_A - 1.0, gpk_u01(w0, w1)), 1.0);
+    return __ddiv_rn(__dmul_rn(tz, tz), GPK_RS_A);
+}
+
+// the partner of a walker of half h: walker (r2 * (hb)) >> 32 of the other half
+__device__ __forceinline__ int gpk_stretch_partner(uint32_t w2, int half, int hb)
+{
+    return (1 - half) * hb + (int)__umulhi(w2, (uint32_t)hb);
+}
+
+// q_j = fl(c_j - fl(z fl(c_j - s_j)))
+__device__ __forceinline__ double gpk_stretch_coord(double c, double s, double z)
+{
+    return __dsub_rn(c, __dmul_rn(z, __dsub_rn(c, s)));
+}
+
+// fl(fl(fl((dw - 1) log z) + new) - old) > log u01(r0, r1); a NaN difference (-inf - -inf) rejects
+__device__ __forceinline__ bool gpk_stretch_accept(int dw, double z, double v, double old, uint32_t r0, uint32_t r1)
+{
+    const double lnpdiff = __dsub_rn(__dadd_rn(__dmul_rn((double)(dw - 1), log(z)), v), old);
+    return lnpdiff > log(gpk_u01(r0, r1));
+}
 
 // init rows of run r: one thread per (estimator, walker, coordinate)
 __global__ void gpk_rs_init_kernel(int n, int nb, int dw, int run, const unsigned long long* __restrict__ seeds,
@@ -80,12 +107,11 @@ __global__ void gpk_rs_propose_kernel(int n, int nb, int dw, int d, int run, int
         uint32_t w[4];
         gpk_philox4x32_10((uint32_t)k, (uint32_t)step, (uint32_t)(2 * run + half), GPK_RS_TAG_MOVE, (uint32_t)seed,
                           (uint32_t)(seed >> 32), w);
-        const double tz = __dadd_rn(__dmul_rn(GPK_RS_A - 1.0, gpk_u01(w[0], w[1])), 1.0);
-        const double z = __ddiv_rn(__dmul_rn(tz, tz), GPK_RS_A);
-        const int c = (1 - half) * hb + (int)__umulhi(w[2], (uint32_t)hb);
+        const double z = gpk_stretch_z(w[0], w[1]);
+        const int c = gpk_stretch_partner(w[2], half, hb);
         const double* cp = P + ((long)i * nb + c) * dw;
         for (int j = 0; j < dw; ++j) {
-            const double v = __dsub_rn(cp[j], __dmul_rn(z, __dsub_rn(cp[j], s[j])));
+            const double v = gpk_stretch_coord(cp[j], s[j], z);
             q[j] = v;
             x[j] = v;
         }
@@ -122,8 +148,7 @@ __global__ void gpk_rs_accept_kernel(int n, int nb, int dw, int run, int step, i
     uint32_t r[4];
     gpk_philox4x32_10((uint32_t)k, (uint32_t)step, (uint32_t)(2 * run + half), GPK_RS_TAG_ACC, (uint32_t)seed,
                       (uint32_t)(seed >> 32), r);
-    const double lnpdiff = __dsub_rn(__dadd_rn(__dmul_rn((double)(dw - 1), log(Z[t])), v), L[w]);
-    if (lnpdiff > log(gpk_u01(r[0], r[1]))) {
+    if (gpk_stretch_accept(dw, Z[t], v, L[w], r[0], r[1])) {
         for (int j = 0; j < dw; ++j) P[w * dw + j] = q[j];
         L[w] = v;
         acc[w] += 1;

@@ -17,7 +17,7 @@ from robo_b200.solver import BayesianOptimization
 def bayesian_optimization(objective_function, lower, upper, num_iterations=30, X_init=None, Y_init=None,
                           maximizer="random", acquisition_func="log_ei", model_type="gp_mcmc",
                           n_init=3, rng=None, output_path=None, n_candidates=500,
-                          chain_length=200, burnin_steps=100):
+                          chain_length=200, burnin_steps=100, hyper_sampler="host"):
     assert upper.shape[0] == lower.shape[0], "Dimension miss match"
     assert np.all(lower < upper), "Lower bound >= upper bound"
     assert n_init <= num_iterations, "Number of initial design point has to be <= than the number of iterations"
@@ -36,9 +36,11 @@ def bayesian_optimization(objective_function, lower, upper, num_iterations=30, X
         model = GaussianProcess(kernel, prior=prior, rng=rng, normalize_output=False, normalize_input=True,
                                 lower=lower, upper=upper)
     elif model_type == "gp_mcmc":
+        # hyper_sampler="device" samples the hyper-parameters on the device (gpk_sample_hypers), "host" with
+        # EnsembleSampler; the two agree in law, not bit for bit
         model = GaussianProcessMCMC(kernel, prior=prior, n_hypers=n_hypers, chain_length=chain_length,
                                     burnin_steps=burnin_steps, normalize_input=True, normalize_output=False,
-                                    rng=rng, lower=lower, upper=upper)
+                                    rng=rng, lower=lower, upper=upper, hyper_sampler=hyper_sampler)
     else:
         raise ValueError("'{}' is not a valid model on the GPU path (gp, gp_mcmc)".format(model_type))
 

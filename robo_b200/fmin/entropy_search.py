@@ -16,7 +16,8 @@ from robo_b200.solver import BayesianOptimization
 
 
 def entropy_search(objective_function, lower, upper, num_iterations=30, maximizer="random", model="gp_mcmc",
-                   X_init=None, Y_init=None, n_init=3, output_path=None, rng=None, representer_sampler="host"):
+                   X_init=None, Y_init=None, n_init=3, output_path=None, rng=None, representer_sampler="host",
+                   hyper_sampler="host"):
     assert upper.shape[0] == lower.shape[0], "Dimension miss match"
     assert np.all(lower < upper), "Lower bound >= upper bound"
     assert n_init <= num_iterations, "Number of initial design point has to be <= than the number of iterations"
@@ -38,8 +39,11 @@ def entropy_search(objective_function, lower, upper, num_iterations=30, maximize
         gp = GaussianProcess(kernel, prior=prior, rng=rng, normalize_output=False, normalize_input=True,
                              lower=lower, upper=upper)
     elif model == "gp_mcmc":
+        # hyper_sampler="device" samples the hyper-parameters on the device (gpk_sample_hypers), "host" with
+        # EnsembleSampler; the two agree in law, not bit for bit
         gp = GaussianProcessMCMC(kernel, prior=prior, n_hypers=n_hypers, chain_length=200, burnin_steps=100,
-                                 normalize_input=True, normalize_output=False, rng=rng, lower=lower, upper=upper)
+                                 normalize_input=True, normalize_output=False, rng=rng, lower=lower, upper=upper,
+                                 hyper_sampler=hyper_sampler)
     else:
         raise ValueError("'{}' is not a valid model on the GPU path (gp, gp_mcmc)".format(model))
 

@@ -72,11 +72,12 @@ class FabolasGP(GaussianProcess):
 class FabolasGPMCMC(GaussianProcessMCMC):
 
     def __init__(self, kernel, basis_func, prior=None, n_hypers=20, chain_length=2000, burnin_steps=2000,
-                 normalize_output=False, rng=None, lower=None, upper=None, noise=-8, device=0):
+                 normalize_output=False, rng=None, lower=None, upper=None, noise=-8, device=0, hyper_sampler="host"):
         self.basis_func = basis_func
         super(FabolasGPMCMC, self).__init__(kernel, prior, n_hypers, chain_length, burnin_steps,
                                             normalize_output=normalize_output, normalize_input=False, rng=rng,
-                                            lower=lower, upper=upper, noise=noise, device=device)
+                                            lower=lower, upper=upper, noise=noise, device=device,
+                                            hyper_sampler=hyper_sampler)
 
     # fabolas_gp.py:33-100 is GaussianProcessMCMC.train with these two differences: the MCMC phase sees the transformed
     # inputs (:34-36), and every hyper-parameter sample becomes a FabolasGP trained on the raw inputs (:91-99).

@@ -7,13 +7,19 @@ reference.  The cost of `train` is `n_hypers x (burnin + chain)` evaluations of
 on the CPU.  Here every half-ensemble of walkers is evaluated together: one gpk handle (own CUDA
 stream) per proposal, `gpk_fit_begin` on all of them, then `gpk_fit_end` — the latency-bound
 factorisation chains overlap on the GPU (SURVEY.md section 8f rank 1).
+
+``hyper_sampler="device"`` runs each ``run_mcmc`` of ``train`` (burn-in, then chain) as one device call instead
+(gpk_sample_hypers, robo_b200/csrc/gpk_hyper.cuh): one launch evaluates the initial walkers, one launch per half-step
+proposes, evaluates the log-posteriors on chip (kernel, Cholesky and prior in one CTA per walker) and accepts; the
+final positions come back in one copy.  It draws from a counter-based Philox stream seeded from ``self.rng`` once per
+run, not from numpy's stream: the two samplers agree in law, not bit for bit, which is why ``"host"`` stays the default.
 """
 import logging
 from copy import deepcopy
 
 import numpy as np
 
-from robo_b200 import _lib
+from robo_b200 import _lib, priors
 from robo_b200.device_gp import DeviceGP, TINY
 from robo_b200.models.base_model import BaseModel
 from robo_b200.models.gaussian_process import GaussianProcess
@@ -70,12 +76,51 @@ class _LikelihoodPool(object):
         self.handles = []
 
 
+def _hyper_prior(prior):
+    """(gpk_prior_kind, the 7 constants, n_ls, n_lr) of a prior the device restates: None, DefaultPrior or EnvPrior
+    (the reference's classes or robo_b200.priors'); TypeError for any other."""
+    if prior is None:
+        return _lib.PRIOR_NONE, None, 0, 0
+    cls = type(prior)
+    mod = cls.__module__ or ""
+    ours = mod == priors.__name__ or mod.startswith("robo.priors")
+    if ours and cls.__name__ in ("DefaultPrior", "EnvPrior"):
+        par = [prior.ln_prior.sigma, prior.ln_prior.mean, prior.tophat.min, prior.tophat.max, prior.horseshoe.scale,
+               0.0, 0.0]
+        if cls.__name__ == "DefaultPrior":
+            return _lib.PRIOR_DEFAULT, par, 0, 0
+        par[5:] = [prior.bayes_lin_prior.sigma, prior.bayes_lin_prior.mean]
+        return _lib.PRIOR_ENV, par, int(prior.n_ls), int(prior.n_lr)
+    raise TypeError("hyper_sampler='device' restates None, DefaultPrior and EnvPrior only, not %s.%s"
+                    % (mod, cls.__name__))
+
+
+def _hyper_kernel(kernel):
+    """kernel.flatten(), or TypeError when the device cannot represent the kernel."""
+    try:
+        return kernel.flatten()
+    except Exception as e:
+        raise TypeError("hyper_sampler='device' cannot represent this kernel: %s" % e)
+
+
 class GaussianProcessMCMC(BaseModel):
 
     def __init__(self, kernel, prior=None, n_hypers=20, chain_length=2000, burnin_steps=2000,
                  normalize_output=False, normalize_input=True,
-                 rng=None, lower=None, upper=None, noise=-8, device=0):
-        """Arguments as in gaussian_process_mcmc.py:17-70, plus ``device``."""
+                 rng=None, lower=None, upper=None, noise=-8, device=0, hyper_sampler="host"):
+        """Arguments as in gaussian_process_mcmc.py:17-70, plus ``device`` and ``hyper_sampler``: "host" (default)
+        runs EnsembleSampler with numpy's stream, as before; "device" runs each run_mcmc on the device
+        (gpk_sample_hypers) with its own Philox stream, so the two agree in law, not bit for bit.  A train whose N
+        exceeds GPK_HYPER_MAX_N falls back to the host sampler.  "device" raises TypeError for a prior other than
+        None / DefaultPrior / EnvPrior or a kernel the device cannot represent."""
+        if hyper_sampler not in ("host", "device"):
+            raise ValueError("hyper_sampler must be 'host' or 'device', not %r" % (hyper_sampler,))
+        if hyper_sampler == "device":
+            _hyper_prior(prior)
+            _hyper_kernel(kernel)
+        self.hyper_sampler = hyper_sampler
+        self._hyper_handle = None
+        self._hyper_fallback_logged = False
         if rng is None:
             self.rng = np.random.RandomState(np.random.randint(0, 10000))
         else:
@@ -101,6 +146,7 @@ class GaussianProcessMCMC(BaseModel):
     def __getstate__(self):
         st = self.__dict__.copy()
         st["_pool"] = None
+        st["_hyper_handle"] = None
         return st
 
     @BaseModel._check_shapes_train
@@ -117,7 +163,17 @@ class GaussianProcessMCMC(BaseModel):
         self.gp = DeviceGP(self.kernel, mean=self.mean, device=self.device)
         self.gp.set_data(self.X, self.y)
 
-        if do_optimize:
+        on_device = do_optimize and self.hyper_sampler == "device"
+        if on_device and len(self.X) > _lib.HYPER_MAX_N:
+            # the device keeps one factor per SM in shared memory: larger N samples on the host for this train
+            if not self._hyper_fallback_logged:
+                logger.info("N = %d exceeds GPK_HYPER_MAX_N = %d: the hyper-parameters are sampled on the host",
+                            len(self.X), _lib.HYPER_MAX_N)
+                self._hyper_fallback_logged = True
+            on_device = False
+        if on_device:
+            self._sample_hypers_device()
+        elif do_optimize:
             if self._pool is not None:
                 self._pool.close()
             self._pool = _LikelihoodPool(self.kernel, self.X, self.y, self.mean, self.n_hypers // 2, self.device)
@@ -152,6 +208,36 @@ class GaussianProcessMCMC(BaseModel):
         for model in self.models:
             model.train_end()
         self.is_trained = True
+
+    def _sample_hypers_device(self):
+        """train's MCMC phase on the device: the same p0 / burn-in / chain bookkeeping as the host path, each run_mcmc
+        one gpk_sample_hypers call seeded from self.rng."""
+        prior_kind, prior_par, n_ls, n_lr = _hyper_prior(self.prior)
+        f = _hyper_kernel(self.kernel)
+        dim = len(self.kernel) + 1
+        if self._hyper_handle is None:
+            self._hyper_handle = _lib.Handle(self.device)
+        h = self._hyper_handle
+        h.set_data(self.X, self.y)
+        h.set_kernel(f["family"], f["log_amp"], f["axis"], f["group"], f["log_metric"])
+        _lib.set_hyper_model(h, f["slots"], len(f["axis"]), float(self.mean), TINY, prior_kind, prior_par, n_ls, n_lr)
+
+        def run(p0, steps):
+            seed = int(self.rng.randint(0, 2 ** 63, dtype=np.int64))
+            return _lib.sample_hypers(h, p0, steps, seed)["pos"]
+        calls = 0
+        if not self.burned:
+            if self.prior is None:
+                self.p0 = self.rng.rand(self.n_hypers, dim)
+            else:
+                self.p0 = self.prior.sample_from_prior(self.n_hypers)
+            self.p0 = run(self.p0, self.burnin_steps)
+            calls += self.n_hypers * (self.burnin_steps + 1)
+            self.burned = True
+        self.p0 = run(self.p0, self.chain_length)
+        calls += self.n_hypers * (self.chain_length + 1)
+        self.hypers = self.p0.copy()
+        self.n_lnprob_calls = calls
 
     # hooks for FabolasGPMCMC (robo/models/fabolas_gp.py), which differs only in how inputs are prepared
     def _likelihood_inputs(self, X):

@@ -1,6 +1,6 @@
 """Hyper-priors used by the fmin facade: O(H) scalar host math added to the GPU log-likelihood
 (SURVEY.md section 2 row 19: out of the hot path, stays Python).  Semantics — including the quirks —
-follow robo/priors/base_prior.py and robo/priors/default_priors.py."""
+follow robo/priors/base_prior.py, robo/priors/default_priors.py and robo/priors/env_priors.py."""
 import numpy as np
 import scipy.stats as sps
 
@@ -69,6 +69,21 @@ class LognormalPrior(object):
         return None
 
 
+class NormalPrior(object):
+    """base_prior.py:318-378 (lnprob returns the pdf, not its log, like the reference, :341-357)."""
+
+    def __init__(self, sigma, mean=0, rng=None):
+        self.rng = np.random.RandomState(np.random.randint(0, 10000)) if rng is None else rng
+        self.sigma, self.mean = sigma, mean
+
+    def lnprob(self, theta):
+        return sps.norm.pdf(theta, scale=self.sigma, loc=self.mean)
+
+    def sample_from_prior(self, n_samples):
+        p0 = self.rng.normal(loc=self.mean, scale=self.sigma, size=n_samples)
+        return p0[:, np.newaxis]
+
+
 class DefaultPrior(object):
     """default_priors.py:8-53: lognormal on the amplitude, tophat(-10, 2) on the length scales,
     horseshoe(0.1) on the noise; gradient identically zero (:51-53)."""
@@ -98,3 +113,38 @@ class DefaultPrior(object):
 
     def gradient(self, theta):
         return np.zeros([theta.shape[0]])
+
+
+class EnvPrior(object):
+    """env_priors.py:8-81 (the Fabolas prior): lognormal(mean -2) on the amplitude, tophat(-10, 2) on the n_ls length
+    scales, NormalPrior(0, 1) on the n_lr parameters of the environment kernel (the pdf is added, as the reference
+    does), horseshoe(0.001) on the noise."""
+
+    def __init__(self, n_dims, n_ls, n_lr, rng=None):
+        self.rng = np.random.RandomState(np.random.randint(0, 10000)) if rng is None else rng
+        self.n_dims, self.n_ls, self.n_lr = n_dims, n_ls, n_lr
+        self.bayes_lin_prior = NormalPrior(sigma=1, mean=0, rng=self.rng)
+        self.tophat = TophatPrior(-10, 2, rng=self.rng)
+        self.ln_prior = LognormalPrior(mean=-2, sigma=1.0, rng=self.rng)
+        self.horseshoe = HorseshoePrior(scale=0.001, rng=self.rng)
+
+    def lnprob(self, theta):
+        lp = 0
+        lp += self.ln_prior.lnprob(theta[0])
+        lp += self.tophat.lnprob(theta[1:self.n_ls + 1])
+        pos, end = self.n_ls + 1, self.n_ls + self.n_lr + 1
+        for t in theta[pos:end]:
+            lp += self.bayes_lin_prior.lnprob(t)
+        lp += self.horseshoe.lnprob(theta[-1])
+        return lp
+
+    def sample_from_prior(self, n_samples):
+        p0 = np.zeros([n_samples, self.n_dims])
+        p0[:, 0] = self.ln_prior.sample_from_prior(n_samples)[:, 0]
+        ls_sample = np.array([self.tophat.sample_from_prior(n_samples)[:, 0] for _ in range(0, self.n_ls)]).T
+        p0[:, 1:(self.n_ls + 1)] = ls_sample
+        pos, end = self.n_ls + 1, self.n_ls + self.n_lr + 1
+        samples = np.array([self.bayes_lin_prior.sample_from_prior(n_samples)[:, 0] for _ in range(0, self.n_lr)]).T
+        p0[:, pos:end] = samples
+        p0[:, -1] = self.horseshoe.sample_from_prior(n_samples)[:, 0]
+        return p0

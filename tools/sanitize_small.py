@@ -81,6 +81,16 @@ print("es cost random", _lib.maximize_random_es_cost(pairs[:1], pairs[2:3], 7, 1
                                                      0.1, np.zeros(D - 1), np.ones(D - 1), 1, 0, 0.0)[2])
 for h in pairs:
     h.close()
+# hyper-parameter sampling: the per-theta log-posterior (kernel, Cholesky, prior in one CTA) and a short stretch-move run
+from robo_b200.priors import DefaultPrior
+h = _lib.Handle(0)
+h.set_data(X[:150], y[:150])
+h.set_kernel(f["family"], f["log_amp"], f["axis"], f["group"], f["log_metric"])
+_lib.set_hyper_model(h, f["slots"], len(f["axis"]), float(y.mean()), 1.25e-12, _lib.PRIOR_DEFAULT,
+                     [1.0, 0.0, -10.0, 2.0, 0.1, 0.0, 0.0])
+p0 = DefaultPrior(D + 2, rng=np.random.RandomState(0)).sample_from_prior(10)
+print("hyper lnpost", _lib.hyper_lnpost(h, p0)[0][:3], "run", _lib.sample_hypers(h, p0, 5, 3)["n_accepted"])
+h.close()
 h = _lib.moments_handle()
 print(h.acq_moments(rng.randn(100), rng.rand(100) + 0.1, _lib.ACQ_LOG_EI, 0.0, 0.0)[0][:3])
 print(h.reduce_models(rng.rand(4, 50), rng.rand(4, 50))[1][:3])
