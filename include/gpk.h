@@ -497,6 +497,17 @@ int gpk_measure_int8_peak_sustained(gpk_handle* h, double seconds, int random_op
 int gpk_get_factor(gpk_handle* h, double* L /* n x n row-major, lower */);
 int gpk_get_linv(gpk_handle* h, double* Linv /* n x n row-major, lower */);
 int gpk_get_z(gpk_handle* h, double* z /* n */);
+/* The two inputs of the entropy change that gpk_es_compute derives per candidate, read back from the buffers its dH
+ * kernel reads (the same passes of ES_CH = 16384 candidates, the same launches): var (m) the predictive variance of the
+ * scoring pass, sigma (m x nb row-major) the covariance to the representer points, (k(zb_j, x) - K(x, X) U[:, j]) *
+ * y_std^2 (output transform) clipped at DBL_EPSILON.  Xs: m x d raw inputs.  GPK_BAD_ARG before gpk_es_update or after
+ * the model changed since. */
+int gpk_es_moments(gpk_handle* h, const double* Xs, long m, double* var, double* sigma);
+/* U = K^-1 K(X, zb) of the last gpk_es_update (n x nb row-major, fp64, built from L^-1); GPK_BAD_ARG as above. */
+int gpk_es_get_u(gpk_handle* h, double* U);
+/* n and nb of the last gpk_es_update: the shapes of gpk_es_get_u's U and of gpk_es_moments' sigma rows; GPK_BAD_ARG
+ * as above. */
+int gpk_es_dims(gpk_handle* h, int* n, int* nb);
 /* The int8 variance contraction alone, on caller-supplied operands (tests: tests/ozaki_model.py restates it exactly).
  * P: n x n row-major, lower triangular (the stand-in for L^-1; only its block-lower triangle is read by the contraction,
  * its row maxima by the row exponents).  Ks: m x n row-major, every |entry| <= amp.  Both are zero-padded to NP =

@@ -80,6 +80,9 @@ _SIGNATURES = {
     "gpk_es_update": [_vp, _dp, C.c_int, _dp, C.c_double, _dp, C.c_int, _dp, _dp, _dp, _dp, _dp, _dp],
     "gpk_es_compute": [_vp, _dp, C.c_long, _dp],
     "gpk_es_compute_dev": [_vp, _vp, C.c_long, _vp],
+    "gpk_es_moments": [_vp, _dp, C.c_long, _dp, _dp],
+    "gpk_es_get_u": [_vp, _dp],
+    "gpk_es_dims": [_vp, _ip, _ip],
     "gpk_predict_mean": [_vp, _dp, C.c_long, _dp],
     "gpk_predict_mean_dev": [_vp, _vp, C.c_long, _vp],
     "gpk_es_cost_multi": [C.POINTER(_vp), C.POINTER(_vp), C.c_int, _dp, C.c_long, _dp, _dp, C.c_int, C.c_int, C.c_int,
@@ -509,6 +512,28 @@ class Handle(object):
 
     def es_compute_dev(self, d_Xs_ptr, m, d_out_ptr):
         self._check(self.lib.gpk_es_compute_dev(self._h, _vp(d_Xs_ptr), int(m), _vp(d_out_ptr)))
+
+    def es_dims(self):
+        """gpk_es_dims: (n, nb) of the last es_update."""
+        n, nb = C.c_int(), C.c_int()
+        self._check(self.lib.gpk_es_dims(self._h, C.byref(n), C.byref(nb)))
+        return n.value, nb.value
+
+    def es_moments(self, Xs):
+        """gpk_es_moments (diagnostic): what gpk_es_compute's dH kernel reads for the rows of Xs (m, d) -> (var (m,),
+        sigma (m, nb))."""
+        Xs = f64(Xs)
+        m = Xs.shape[0]
+        _, nb = self.es_dims()
+        var, sigma = np.empty(m), np.empty((m, nb))
+        self._check(self.lib.gpk_es_moments(self._h, _as_dp(Xs), m, _as_dp(var), _as_dp(sigma)))
+        return var, sigma
+
+    def es_get_u(self):
+        """gpk_es_get_u (diagnostic): U = K^-1 K(X, zb) of the last es_update -> (n, nb)."""
+        U = np.empty(self.es_dims())
+        self._check(self.lib.gpk_es_get_u(self._h, _as_dp(U)))
+        return U
 
     def predict_mean(self, Xs):
         """gpk_predict_mean: the predictive mean alone of every row of Xs (m, d) -> (m,)."""

@@ -1064,6 +1064,28 @@ int es_reserve(gpk_handle* h) {
     return ensure(h, h->es_work, (size_t)ES_CH * (h->es_nb + 1) * 8);
 }
 
+// One pass of es_dh_dev's first half: the predictive variance of rows <= ES_CH candidates X (the scoring pass) into
+// es_work's var (rows) and their clipped covariance to zb into its sig (rows x nb), the two buffers gpk_es_dh_kernel
+// reads.  Asynchronous on the handle's stream; needs es_reserve and a current gpk_es_update.
+int es_moments_pass(gpk_handle* h, const double* X, long rows) {
+    const int nb = h->es_nb, d = h->d;
+    EsLayout L(nb, h->es_np, d);
+    const double* st = ptr<double>(h->es_state);
+    double* var = ptr<double>(h->es_work);
+    double* sig = var + ES_CH;
+    const double* lo = h->has_bounds ? ptr<double>(h->lower) : nullptr;
+    const double* up = h->has_bounds ? ptr<double>(h->upper) : nullptr;
+    const double out_scale = h->norm_out ? h->y_std * h->y_std : 1.0;
+    int rc;
+    if ((rc = score_dev(h, X, rows, GPK_ACQ_NONE, 0.0, 0.0, nullptr, nullptr, var, nullptr, nullptr))) return rc;
+    gpk_es_sigma_kernel<<<(unsigned)rows, GPK_ES_THREADS, 0, h->stream>>>(h->spec, X, rows, d, lo, up,
+                                                                          ptr<double>(h->Xrow), h->n,
+                                                                          ptr<double>(h->es_U), st + L.zb, nb,
+                                                                          out_scale, sig);
+    CKL();
+    return GPK_OK;
+}
+
 // Entropy change of m candidates on the device (InformationGain.compute): Xm are the inputs the model's scoring pass and
 // covariance to zb take, Xb the ones the bounds test of gpk_es_update's [lower, upper] sees (the same array unless the
 // model's inputs were transformed).  Asynchronous on the handle's stream; needs a current gpk_es_update.
@@ -1074,20 +1096,11 @@ int es_dh_dev(gpk_handle* h, const double* Xm, const double* Xb, long m, double*
     const long CH = ES_CH;
     int rc;
     if ((rc = es_reserve(h))) return rc;
-    double* var = ptr<double>(h->es_work);
-    double* sig = var + CH;
-    const double* lo = h->has_bounds ? ptr<double>(h->lower) : nullptr;
-    const double* up = h->has_bounds ? ptr<double>(h->upper) : nullptr;
-    const double out_scale = h->norm_out ? h->y_std * h->y_std : 1.0;
+    const double* var = ptr<double>(h->es_work);
+    const double* sig = var + CH;
     for (long c0 = 0; c0 < m; c0 += CH) {
         const long rows = std::min(CH, m - c0);
-        const double* X = Xm + c0 * d;
-        if ((rc = score_dev(h, X, rows, GPK_ACQ_NONE, 0.0, 0.0, nullptr, nullptr, var, nullptr, nullptr))) return rc;
-        gpk_es_sigma_kernel<<<(unsigned)rows, GPK_ES_THREADS, 0, h->stream>>>(h->spec, X, rows, d, lo, up,
-                                                                              ptr<double>(h->Xrow), h->n,
-                                                                              ptr<double>(h->es_U), st + L.zb, nb,
-                                                                              out_scale, sig);
-        CKL();
+        if ((rc = es_moments_pass(h, Xm + c0 * d, rows))) return rc;
         gpk_es_dh_kernel<<<(unsigned)rows, GPK_ES_THREADS, 0, h->stream>>>(
             Xb + c0 * d, rows, d, st + L.lo, st + L.up, var, sig, nb, h->es_np, h->es_sn2, h->es_H, st + L.logP,
             st + L.lmb, st + L.dMu, st + L.dSig, st + L.Hs, st + L.W, d_out + c0);
@@ -2779,6 +2792,50 @@ int gpk_es_compute(gpk_handle* h, const double* Xs, long m, double* out) {
     CK(cudaMemcpyAsync(dX, Xs, (size_t)m * h->d * 8, cudaMemcpyHostToDevice, h->stream));
     if ((rc = gpk_es_compute_dev(h, dX, m, dout))) return rc;
     CK(cudaMemcpyAsync(out, dout, (size_t)m * 8, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    return GPK_OK;
+}
+
+int gpk_es_moments(gpk_handle* h, const double* Xs, long m, double* var, double* sigma) {
+    int rc = require(h, true, true, true);
+    if (rc) return rc;
+    if (!Xs || !var || !sigma || m <= 0) BAD("gpk_es_moments: need candidates, var and sigma");
+    if ((rc = es_ready(h, nullptr, "gpk_es_moments"))) return rc;
+    CK(cudaSetDevice(h->device));
+    const int nb = h->es_nb, d = h->d;
+    if ((rc = es_reserve(h))) return rc;
+    if ((rc = ensure(h, h->es_in, (size_t)m * d * 8))) return rc;
+    double* dX = ptr<double>(h->es_in);
+    const double* dvar = ptr<double>(h->es_work);
+    const double* dsig = dvar + ES_CH;
+    CK(cudaMemcpyAsync(dX, Xs, (size_t)m * d * 8, cudaMemcpyHostToDevice, h->stream));
+    for (long c0 = 0; c0 < m; c0 += ES_CH) {          // the passes of es_dh_dev, each read back before the next
+        const long rows = std::min(ES_CH, m - c0);
+        if ((rc = es_moments_pass(h, dX + c0 * d, rows))) return rc;
+        CK(cudaMemcpyAsync(var + c0, dvar, (size_t)rows * 8, cudaMemcpyDeviceToHost, h->stream));
+        CK(cudaMemcpyAsync(sigma + c0 * nb, dsig, (size_t)rows * nb * 8, cudaMemcpyDeviceToHost, h->stream));
+        CK(cudaStreamSynchronize(h->stream));
+    }
+    return GPK_OK;
+}
+
+int gpk_es_dims(gpk_handle* h, int* n, int* nb) {
+    int rc = require(h, true, true, true);
+    if (rc) return rc;
+    if (!n || !nb) BAD("gpk_es_dims: null output");
+    if ((rc = es_ready(h, nullptr, "gpk_es_dims"))) return rc;
+    *n = h->n;
+    *nb = h->es_nb;
+    return GPK_OK;
+}
+
+int gpk_es_get_u(gpk_handle* h, double* U) {
+    int rc = require(h, true, true, true);
+    if (rc) return rc;
+    if (!U) BAD("gpk_es_get_u: null output");
+    if ((rc = es_ready(h, nullptr, "gpk_es_get_u"))) return rc;
+    CK(cudaSetDevice(h->device));
+    CK(cudaMemcpyAsync(U, h->es_U.p, (size_t)h->n * h->es_nb * 8, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
     return GPK_OK;
 }

@@ -81,6 +81,16 @@ print("es cost random", _lib.maximize_random_es_cost(pairs[:1], pairs[2:3], 7, 1
                                                      0.1, np.zeros(D - 1), np.ones(D - 1), 1, 0, 0.0)[2])
 for h in pairs:
     h.close()
+# entropy search at N = 257 (two 256-row tiles of the sigma kernel) and Nb = 64: the read-back of var, sigma and U, and
+# the entropy change itself (the dH kernel's full lane loop and all eight warps over the representer points)
+h = _lib.Handle(0)
+h.set_data(X[:257], y[:257])
+h.set_kernel(f["family"], f["log_amp"], f["axis"], f["group"], f["log_metric"])
+h.fit(1e-3 + 1.25e-12, float(y[:257].mean()))
+h.es_update(rng.rand(64, D), rng.rand(64), 1e-3, W, np.zeros(D), np.ones(D))
+var, sig = h.es_moments(Xs[:50])
+print("es moments", var[:2], sig.shape, h.es_get_u().shape, "dH", h.es_compute(Xs[:50])[:2])
+h.close()
 # hyper-parameter sampling: the per-theta log-posterior (kernel, Cholesky, prior in one CTA) and a short stretch-move run
 from robo_b200.priors import DefaultPrior
 h = _lib.Handle(0)
