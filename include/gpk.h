@@ -54,6 +54,10 @@ typedef enum {
     GPK_ACQ_LCB = 4        /* robo/acquisition_functions/lcb.py:62-65             */
 } gpk_acq_kind;
 
+/* posterior objectives of gpk_maximize_lbfgs (robo/util/posterior_optimization.py), minimised: */
+#define GPK_OBJ_MEAN 5         /* mu(x)                                                */
+#define GPK_OBJ_MEAN_STD 6     /* mu(x) + sqrt(v(x))                                   */
+
 #define GPK_MAX_TERMS 64   /* metric entries (input dims x product factors) per kernel */
 
 /* hyper-parameter sampling (gpk_sample_hypers): the factor of one theta lives in one SM's shared memory as a packed fp64
@@ -385,6 +389,55 @@ int gpk_maximize_de_es_cost(gpk_handle* const* objective, gpk_handle* const* cos
                             const double* cfg_upper, int n_bounds, int basis_objective, int basis_cost, double overhead,
                             double* best_x, double* best_energy, int* nit, long* nfev, double* population,
                             double* energies);
+
+/* SciPyOptimizer.maximize (robo/maximizers/scipy_optimizer.py) and posterior_mean(_plus_std)_optimization
+ * (robo/util/posterior_optimization.py) on the device: multi-start bounded L-BFGS, the n_starts starts run
+ * independently and in lockstep.  Each round scores, for every start still running, its trial point and the d
+ * forward-difference neighbours of it in one batched pass (n_active (d + 1) rows); the iteration (free set, two-loop
+ * recursion over the last maxcor pairs, projected Armijo backtracking, the stopping tests) runs in one warp per start,
+ * and only a 16-byte status record crosses PCIe per round.  The energy minimised is
+ *   acquisitions and information gain: -value of the row, x clipped into the box (scipy_optimizer.py:39-49);
+ *   GPK_OBJ_MEAN: mu(x); GPK_OBJ_MEAN_STD: mu(x) + sqrt(v(x)) (the mixture moments of gpk_acq_multi mode 1);
+ * a value that is not finite becomes DBL_MAX.  The gradient is scipy's 2-point forward difference with the relative
+ * step sqrt(DBL_EPSILON) max(1, |x_j|), turned inwards at a bound; there is no analytic gradient in the loop (the
+ * reference's with_gradients=True calls predictive_gradients, which no reference model has).
+ * Deviation from the reference: this is projected L-BFGS (steepest descent on the free set through the two-loop
+ * recursion, projected backtracking from alpha0 = min(1, 1 / ||d||) on the first iteration and 1 afterwards, at most 20
+ * halvings), not L-BFGS-B's Cauchy point, subspace minimisation and More-Thuente line search.  Every rounding step is
+ * fixed (gpk_lbfgs.cuh states the algorithm and the order), so a host model can restate a run bit for bit.
+ * Stopping per start, scipy's tests and defaults: (f_k - f_k+1) / max(|f_k|, |f_k+1|, 1) <= ftol (2.220446049250313e-09),
+ * ||P(x - g) - x||_inf <= pgtol (1e-5), nit >= maxiter (15000), nfev >= maxfun (15000 rows scored for the start).
+ * x0 (n_starts x d) finite starts, clipped into [lower, upper] before the first round; 1 <= n_starts <= 2^20;
+ * 1 <= maxcor <= 32 (scipy: 10).  Out per start: x_out (n_starts x d) the last accepted iterate, energy its energy, nit
+ * accepted steps, nfev rows scored, status (gpk_lb_status); energy, nit, nfev and status may be NULL.  n_negative:
+ * EI values < 0 over all rows.  GPK_BAD_ARG: d > GPK_LB_MAX_D, maxcor out of range, lower >= upper, a start that is
+ * not finite, a handle with a multi-rank communicator, and as for gpk_acq_multi / gpk_es_multi / gpk_es_cost_multi. */
+#define GPK_LB_MAX_D 64
+typedef enum {
+    GPK_LB_FTOL = 0,           /* relative reduction of f <= ftol (scipy: CONVERGENCE, success)        */
+    GPK_LB_PGTOL = 1,          /* projected gradient <= pgtol (scipy: CONVERGENCE, success)            */
+    GPK_LB_MAXITER = 2,        /* nit reached maxiter (scipy status 1)                                 */
+    GPK_LB_MAXFUN = 3,         /* nfev reached maxfun (scipy status 1)                                 */
+    GPK_LB_ABNORMAL = 4,       /* no sufficient decrease in 21 trials (ABNORMAL_TERMINATION_IN_LNSRCH) */
+    GPK_LB_INVALID = 5         /* the start's energy is DBL_MAX: stopped at once                       */
+} gpk_lb_status;
+/* acq_kind: GPK_ACQ_EI ... GPK_ACQ_LCB over the mean of the n_models handles (one handle: gpk_acq's value; eta[n_models]
+ * and par as for gpk_acq_multi), or GPK_OBJ_MEAN / GPK_OBJ_MEAN_STD (eta and par ignored). */
+int gpk_maximize_lbfgs(gpk_handle* const* models, int n_models, int acq_kind, const double* eta, double par,
+                       long n_starts, const double* x0, const double* lower, const double* upper, int maxcor,
+                       int maxiter, long maxfun, double ftol, double pgtol, double* x_out, double* energy, int* nit,
+                       long* nfev, int* status, long* n_negative);
+/* -(gpk_es_multi's value over objective[0 .. n-1]); n = 1: -(gpk_es_compute's value) */
+int gpk_maximize_lbfgs_es(gpk_handle* const* objective, int n, long n_starts, const double* x0, const double* lower,
+                          const double* upper, int maxcor, int maxiter, long maxfun, double ftol, double pgtol,
+                          double* x_out, double* energy, int* nit, long* nfev, int* status);
+/* -(gpk_es_cost_multi's value over the (objective[i], cost[i]) pairs) in the extended box lower / upper (d each);
+ * cfg_lower / cfg_upper (n_bounds = d - 1), the basis codes and the overhead as for gpk_es_cost_multi */
+int gpk_maximize_lbfgs_es_cost(gpk_handle* const* objective, gpk_handle* const* cost, int n, long n_starts,
+                               const double* x0, const double* lower, const double* upper, const double* cfg_lower,
+                               const double* cfg_upper, int n_bounds, int basis_objective, int basis_cost,
+                               double overhead, int maxcor, int maxiter, long maxfun, double ftol, double pgtol,
+                               double* x_out, double* energy, int* nit, long* nfev, int* status);
 
 /* The representer points of n entropy-search estimators in one call: the emcee 2.x stretch move (a = 2) of
  * robo_b200/util/ensemble_sampler.py, replacing the host loops of information_gain.py:68-81 and

@@ -19,6 +19,10 @@ GPK_OK, GPK_NOT_PD, GPK_BAD_ARG, GPK_CUDA_ERROR, GPK_NOT_FITTED, GPK_NOT_APPLICA
 MATERN52, EXPSQUARED, MATERN32 = 0, 1, 2
 ACQ_NONE, ACQ_EI, ACQ_LOG_EI, ACQ_PI, ACQ_LCB = range(5)
 ACQ_KIND = {"ei": ACQ_EI, "log_ei": ACQ_LOG_EI, "pi": ACQ_PI, "lcb": ACQ_LCB, "none": ACQ_NONE}
+OBJ_MEAN, OBJ_MEAN_STD = 5, 6                  # GPK_OBJ_MEAN / GPK_OBJ_MEAN_STD: posterior objectives of gpk_maximize_lbfgs
+LB_MAX_D = 64                                  # GPK_LB_MAX_D: largest input dimension of gpk_maximize_lbfgs*
+# gpk_lb_status: why a start of gpk_maximize_lbfgs* stopped (FTOL and PGTOL are scipy's success)
+LB_FTOL, LB_PGTOL, LB_MAXITER, LB_MAXFUN, LB_ABNORMAL, LB_INVALID = range(6)
 BASIS_S, BASIS_ONE_MINUS_S_SQ = range(2)      # gpk_basis: the environment column's basis of a Fabolas model
 PRIOR_NONE, PRIOR_DEFAULT, PRIOR_ENV = range(3)   # gpk_prior_kind: the hyper-priors gpk_sample_hypers restates
 HYPER_MAX_N = 232                              # GPK_HYPER_MAX_N: most training points of gpk_sample_hypers
@@ -98,6 +102,13 @@ _SIGNATURES = {
     "gpk_maximize_de_es_cost": [C.POINTER(_vp), C.POINTER(_vp), C.c_int, C.c_ulonglong, C.c_long, C.c_int, C.c_double,
                                 C.c_double, C.c_double, C.c_double, C.c_double, _dp, _dp, _dp, _dp, C.c_int, C.c_int,
                                 C.c_int, C.c_double, _dp, _dp, _ip, _lp, _dp, _dp],
+    "gpk_maximize_lbfgs": [C.POINTER(_vp), C.c_int, C.c_int, _dp, C.c_double, C.c_long, _dp, _dp, _dp, C.c_int, C.c_int,
+                           C.c_long, C.c_double, C.c_double, _dp, _dp, _ip, _lp, _ip, _lp],
+    "gpk_maximize_lbfgs_es": [C.POINTER(_vp), C.c_int, C.c_long, _dp, _dp, _dp, C.c_int, C.c_int, C.c_long, C.c_double,
+                              C.c_double, _dp, _dp, _ip, _lp, _ip],
+    "gpk_maximize_lbfgs_es_cost": [C.POINTER(_vp), C.POINTER(_vp), C.c_int, C.c_long, _dp, _dp, _dp, _dp, _dp, C.c_int,
+                                   C.c_int, C.c_int, C.c_double, C.c_int, C.c_int, C.c_long, C.c_double, C.c_double,
+                                   _dp, _dp, _ip, _lp, _ip],
     "gpk_sample_representers": [C.POINTER(_vp), C.c_int, C.POINTER(C.c_ulonglong), C.c_int, C.c_int, C.c_int, C.c_int,
                                 _dp, C.c_double, _dp, _dp, C.c_int, C.c_int, _dp, _dp, C.c_int, C.c_double, _dp, _dp,
                                 _ip, _lp, _lp],
@@ -744,6 +755,81 @@ def maximize_de_es_cost(objective, cost, seed, pop, maxiter, mutation, recombina
                                              C.byref(be), C.byref(nit), C.byref(nfev),
                                              _as_dp(P) if P is not None else None, _as_dp(E) if E is not None else None))
     return _de_result(x, be, nit, nfev, P, E, want_population)
+
+
+LB_DEFAULTS = dict(maxcor=10, maxiter=15000, maxfun=15000, ftol=2.220446049250313e-09, pgtol=1e-5)   # scipy's
+
+
+def _lb_io(x0, lower, upper):
+    lo, up = f64(lower).ravel(), f64(upper).ravel()
+    x0 = f64(np.atleast_2d(x0))
+    if lo.size != up.size or x0.ndim != 2 or x0.shape[1] != lo.size:
+        raise ValueError("maximize_lbfgs: x0 needs shape (n_starts, d) with d = len(lower) = len(upper)")
+    R = x0.shape[0]
+    outs = (np.empty((R, lo.size)), np.empty(R), np.empty(R, dtype=np.intc), np.empty(R, dtype=np.int_),
+            np.empty(R, dtype=np.intc))
+    return x0, lo, up, outs
+
+
+def _lb_opts(kw):
+    o = dict(LB_DEFAULTS, **kw)
+    return int(o["maxcor"]), int(o["maxiter"]), int(o["maxfun"]), float(o["ftol"]), float(o["pgtol"])
+
+
+def _lb_out_ptrs(outs):
+    x, e, nit, nfev, st = outs
+    return _as_dp(x), _as_dp(e), nit.ctypes.data_as(_ip), nfev.ctypes.data_as(_lp), st.ctypes.data_as(_ip)
+
+
+def _lb_result(outs):
+    x, e, nit, nfev, st = outs
+    return dict(x=x, energy=e, nit=nit.astype(np.int64), nfev=nfev.astype(np.int64), status=st.astype(np.int64))
+
+
+def maximize_lbfgs(handles, kind, eta, par, x0, lower, upper, **options):
+    """gpk_maximize_lbfgs over ``handles`` (all fitted, same device): multi-start bounded L-BFGS from the rows of x0
+    (n_starts, d) minimising -acq (kind ACQ_EI ... ACQ_LCB, acq the mean over the handles) or the posterior objective
+    (OBJ_MEAN, OBJ_MEAN_STD; eta ignored).  options: maxcor, maxiter, maxfun, ftol, pgtol (scipy's defaults) ->
+    dict(x (n_starts, d), energy, nit, nfev, status (n_starts each), n_negative)."""
+    h0 = handles[0]
+    x0, lo, up, outs = _lb_io(x0, lower, upper)
+    arr = (_vp * len(handles))(*[h._h for h in handles])
+    etas = f64(np.zeros(len(handles)) if eta is None else np.broadcast_to(np.asarray(eta, dtype=np.float64),
+                                                                           (len(handles),)))
+    nn = C.c_long()
+    h0._check(h0.lib.gpk_maximize_lbfgs(arr, len(handles), int(kind), _as_dp(etas), float(par), x0.shape[0], _as_dp(x0),
+                                        _as_dp(lo), _as_dp(up), *_lb_opts(options), *_lb_out_ptrs(outs), C.byref(nn)))
+    r = _lb_result(outs)
+    r["n_negative"] = nn.value
+    return r
+
+
+def maximize_lbfgs_es(objective, x0, lower, upper, **options):
+    """gpk_maximize_lbfgs_es: the same minimising minus the entropy change (one handle: gpk_es_compute's value;
+    several: gpk_es_multi's mean) -> dict(x, energy, nit, nfev, status)."""
+    h0 = objective[0]
+    ho = (_vp * len(objective))(*[h._h for h in objective])
+    x0, lo, up, outs = _lb_io(x0, lower, upper)
+    h0._check(h0.lib.gpk_maximize_lbfgs_es(ho, len(objective), x0.shape[0], _as_dp(x0), _as_dp(lo), _as_dp(up),
+                                           *_lb_opts(options), *_lb_out_ptrs(outs)))
+    return _lb_result(outs)
+
+
+def maximize_lbfgs_es_cost(objective, cost, x0, lower, upper, cfg_lower, cfg_upper, basis_objective, basis_cost,
+                           overhead, **options):
+    """gpk_maximize_lbfgs_es_cost: the same over the extended box lower / upper (d) minimising minus the information
+    gain per unit cost of gpk_es_cost_multi (configuration bounds cfg_lower / cfg_upper, d - 1) -> as
+    maximize_lbfgs_es."""
+    ho, hc, clo, cup = _es_cost_args(objective, cost, cfg_lower, cfg_upper)
+    h0 = objective[0]
+    x0, lo, up, outs = _lb_io(x0, lower, upper)
+    if lo.size != clo.size + 1:
+        raise ValueError("maximize_lbfgs_es_cost: the box needs d entries, the configuration bounds d - 1")
+    h0._check(h0.lib.gpk_maximize_lbfgs_es_cost(ho, hc, len(objective), x0.shape[0], _as_dp(x0), _as_dp(lo),
+                                                _as_dp(up), _as_dp(clo), _as_dp(cup), clo.size, int(basis_objective),
+                                                int(basis_cost), float(overhead), *_lb_opts(options),
+                                                *_lb_out_ptrs(outs)))
+    return _lb_result(outs)
 
 
 def sample_representers(models, seeds, nb, steps, max_runs, kind, eta, par, lower, upper, fabolas=None):

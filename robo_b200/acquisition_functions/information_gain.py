@@ -24,7 +24,7 @@ logger = logging.getLogger(__name__)
 
 
 def _device_model(model):
-    from robo_b200.maximizers.differential_evolution import _raw_inputs
+    from robo_b200.maximizers.device_spec import raw_inputs as _raw_inputs
     if not _raw_inputs(model) or not hasattr(getattr(model, "gp", None), "handle"):
         raise TypeError("InformationGain runs on robo_b200 GaussianProcess models whose inputs go to the device "
                         "untransformed")

@@ -118,7 +118,7 @@ class MarginalizationGPMCMC(BaseAcquisitionFunction):
         infinite lmb)."""
         from robo_b200.acquisition_functions.information_gain import InformationGain
         from robo_b200.acquisition_functions.information_gain_per_unit_cost import InformationGainPerUnitCost
-        from robo_b200.maximizers.differential_evolution import _raw_inputs
+        from robo_b200.maximizers.device_spec import raw_inputs as _raw_inputs
         if len(self.estimators) == 0 or not all(isinstance(e, InformationGain) and
                                                 not isinstance(e, InformationGainPerUnitCost) and _raw_inputs(e.model)
                                                 for e in self.estimators):

@@ -1,0 +1,75 @@
+"""What scores an acquisition on the device, shared by the device maximizers (DifferentialEvolution, SciPyOptimizer),
+and the multi-start L-BFGS call over it (gpk_maximize_lbfgs*)."""
+import numpy as np
+
+from robo_b200 import _lib
+from robo_b200.models.gaussian_process import GaussianProcess
+
+KINDS = ("ei", "log_ei", "pi", "lcb")
+
+
+def raw_inputs(model):
+    """The model hands its raw inputs to the handle (no host-side transform such as FabolasGP's)."""
+    return model is not None and getattr(type(model), "device_inputs", None) is GaussianProcess.device_inputs
+
+
+def device_spec(acq, who):
+    """What scores the acquisition ``acq`` on the device:
+        ("es_cost", device_spec's tuple)   InformationGainPerUnitCost, alone or marginalised (gpk_es_cost_multi)
+        ("es", handles)                    InformationGain, alone or marginalised (gpk_es_compute / gpk_es_multi)
+        ("acq", (kind, etas, par, handles)) EI / LogEI / PI / LCB (gpk_acq_multi)
+    TypeError, naming the maximizer ``who``, when the acquisition does not run on device models."""
+    from robo_b200.acquisition_functions.information_gain import InformationGain
+    from robo_b200.acquisition_functions.information_gain_per_unit_cost import (InformationGainPerUnitCost,
+                                                                                device_spec as es_cost_spec)
+    estimators = acq.estimators if hasattr(acq, "_fused_spec") else [acq]
+    # InformationGainPerUnitCost is an InformationGain: it is recognised first
+    if estimators and all(isinstance(e, InformationGainPerUnitCost) for e in estimators):
+        return "es_cost", es_cost_spec(estimators)
+    if estimators and all(isinstance(e, InformationGain) for e in estimators):
+        if not all(raw_inputs(e.model) for e in estimators):
+            raise TypeError("%s needs InformationGain on robo_b200 GaussianProcess models" % who)
+        return "es", [e._ready_handle() for e in estimators]
+    return "acq", acq_spec(acq, who)
+
+
+def acq_spec(acq, who):
+    """(kind, eta per model, par, handles) of the acquisition, or TypeError when it does not run on device GPs whose
+    inputs go to the handle untransformed."""
+    if hasattr(acq, "_fused_spec"):                          # MarginalizationGPMCMC
+        fused = acq._fused_spec()
+        if fused is None or not all(raw_inputs(m) for m in acq.model.models):
+            raise TypeError("%s needs a marginalised EI / LogEI / PI / LCB over device GaussianProcess sub-models" % who)
+        kind, etas, par, handles = fused
+        return kind, etas, par, handles
+    model = getattr(acq, "model", None)
+    kind = getattr(acq, "kind", None)
+    if kind not in KINDS or getattr(acq, "cost_model", None) is not None or not raw_inputs(model) \
+            or not hasattr(getattr(model, "gp", None), "handle"):
+        raise TypeError("%s needs EI / LogEI / PI / LCB on a robo_b200 GaussianProcess model" % who)
+    eta = 0.0 if kind == "lcb" else float(model.get_incumbent()[1])
+    model.gp._restore()
+    model.gp._push_cfg()
+    return kind, [eta], float(acq.par), [model.gp.handle]
+
+
+def maximize_lbfgs(which, spec, x0, lower, upper):
+    """Multi-start L-BFGS on the device from the rows of x0 over what ``device_spec`` returned, scipy's L-BFGS-B
+    defaults -> _lib's result dict (x, energy, nit, nfev, status per start).  ValueError as ei.py:86-88 when EI came
+    out negative."""
+    if which == "es_cost":
+        ho, hc, lo, up, bo, bc, oh = spec
+        return _lib.maximize_lbfgs_es_cost(ho, hc, x0, lower, upper, cfg_lower=lo, cfg_upper=up, basis_objective=bo,
+                                           basis_cost=bc, overhead=oh)
+    if which == "es":
+        return _lib.maximize_lbfgs_es(spec, x0, lower, upper)
+    kind, etas, par, handles = spec
+    r = _lib.maximize_lbfgs(handles, _lib.ACQ_KIND[kind], etas, par, x0, lower, upper)
+    if kind == "ei" and r["n_negative"] > 0:
+        raise ValueError("Expected Improvement is smaller than 0!")
+    return r
+
+
+def lbfgs_success(status):
+    """scipy's ``res.success`` for a gpk_lb_status: converged by ftol or pgtol."""
+    return np.isin(status, (_lib.LB_FTOL, _lib.LB_PGTOL))

@@ -18,7 +18,9 @@ change, marginalised by gpk_es_multi over a GP-MCMC ensemble) or InformationGain
 
 With ``polish=True`` (scipy's default, which the reference uses) L-BFGS-B refines the device winner on the host
 through the reference's single-point objective, and scipy's acceptance rule applies: lower energy, success, inside
-the bounds.  The polish stays per point by design.
+the bounds.  With ``polish="device"`` the same refinement runs as one start of the device's multi-start L-BFGS
+(gpk_maximize_lbfgs*, the engine of SciPyOptimizer) over the same scoring path as the evolution, under the same
+acceptance rule.
 """
 import sys
 
@@ -27,9 +29,7 @@ import scipy.optimize
 
 from robo_b200 import _lib
 from robo_b200.maximizers.base_maximizer import BaseMaximizer
-from robo_b200.models.gaussian_process import GaussianProcess
-
-KINDS = ("ei", "log_ei", "pi", "lcb")
+from robo_b200.maximizers.device_spec import device_spec, lbfgs_success, maximize_lbfgs
 
 
 class DifferentialEvolution(BaseMaximizer):
@@ -48,45 +48,8 @@ class DifferentialEvolution(BaseMaximizer):
         self.seed = int(self.rng.randint(0, 2 ** 31 - 1))
 
     def _device_spec(self):
-        """What scores the population on the device, by acquisition:
-            ("es_cost", device_spec's tuple)   InformationGainPerUnitCost, alone or marginalised (gpk_es_cost_multi)
-            ("es", handles)                    InformationGain, alone or marginalised (gpk_es_compute / gpk_es_multi)
-            ("acq", (kind, etas, par, handles)) EI / LogEI / PI / LCB (gpk_acq_multi)
-        TypeError when the acquisition does not run on device models."""
-        from robo_b200.acquisition_functions.information_gain import InformationGain
-        from robo_b200.acquisition_functions.information_gain_per_unit_cost import (InformationGainPerUnitCost,
-                                                                                    device_spec)
-        acq = self.objective_func
-        estimators = acq.estimators if hasattr(acq, "_fused_spec") else [acq]
-        # InformationGainPerUnitCost is an InformationGain: it is recognised first
-        if estimators and all(isinstance(e, InformationGainPerUnitCost) for e in estimators):
-            return "es_cost", device_spec(estimators)
-        if estimators and all(isinstance(e, InformationGain) for e in estimators):
-            if not all(_raw_inputs(e.model) for e in estimators):
-                raise TypeError("DifferentialEvolution needs InformationGain on robo_b200 GaussianProcess models")
-            return "es", [e._ready_handle() for e in estimators]
-        return "acq", self._acq_spec()
-
-    def _acq_spec(self):
-        """(kind, eta per model, par, handles) of the acquisition, or TypeError when it does not run on device GPs
-        whose inputs go to the handle untransformed."""
-        acq = self.objective_func
-        if hasattr(acq, "_fused_spec"):                          # MarginalizationGPMCMC
-            fused = acq._fused_spec()
-            if fused is None or not all(_raw_inputs(m) for m in acq.model.models):
-                raise TypeError("DifferentialEvolution needs a marginalised EI / LogEI / PI / LCB over device "
-                                "GaussianProcess sub-models")
-            kind, etas, par, handles = fused
-            return kind, etas, par, handles
-        model = getattr(acq, "model", None)
-        kind = getattr(acq, "kind", None)
-        if kind not in KINDS or getattr(acq, "cost_model", None) is not None or not _raw_inputs(model) \
-                or not hasattr(getattr(model, "gp", None), "handle"):
-            raise TypeError("DifferentialEvolution needs EI / LogEI / PI / LCB on a robo_b200 GaussianProcess model")
-        eta = 0.0 if kind == "lcb" else float(model.get_incumbent()[1])
-        model.gp._restore()
-        model.gp._push_cfg()
-        return kind, [eta], float(acq.par), [model.gp.handle]
+        """device_spec.device_spec of the acquisition: what scores the population on the device."""
+        return device_spec(self.objective_func, "DifferentialEvolution")
 
     def _objective(self, x):
         """The reference's single-point objective (differential_evolution.py:27-34)."""
@@ -114,7 +77,13 @@ class DifferentialEvolution(BaseMaximizer):
             if kind == "ei" and r["n_negative"] > 0:
                 raise ValueError("Expected Improvement is smaller than 0!")      # ei.py:86-88
         x, fun, nfev, polished = r["x"], r["energy"], r["nfev"], False
-        if self.polish:
+        if self.polish == "device":
+            res = maximize_lbfgs(which, spec, x[None, :], lower, upper)
+            nfev += int(res["nfev"][0])
+            xp, ep = res["x"][0], float(res["energy"][0])
+            if ep < fun and lbfgs_success(res["status"][0]) and np.all(xp <= upper) and np.all(lower <= xp):
+                x, fun, polished = xp, ep, True
+        elif self.polish:
             res = scipy.optimize.minimize(self._objective, np.copy(x), method="L-BFGS-B",
                                           bounds=scipy.optimize.Bounds(lower, upper))
             nfev += int(res.get("nfev", 0))
@@ -123,8 +92,3 @@ class DifferentialEvolution(BaseMaximizer):
         self.last = dict(seed=seed, nit=r["nit"], nfev=nfev, best_energy=fun, device_energy=r["energy"],
                          polished=polished)
         return np.clip(x, lower, upper)
-
-
-def _raw_inputs(model):
-    """The model hands its raw inputs to the handle (no host-side transform such as FabolasGP's)."""
-    return model is not None and getattr(type(model), "device_inputs", None) is GaussianProcess.device_inputs

@@ -101,6 +101,19 @@ _lib.set_hyper_model(h, f["slots"], len(f["axis"]), float(y.mean()), 1.25e-12, _
 p0 = DefaultPrior(D + 2, rng=np.random.RandomState(0)).sample_from_prior(10)
 print("hyper lnpost", _lib.hyper_lnpost(h, p0)[0][:3], "run", _lib.sample_hypers(h, p0, 5, 3)["n_accepted"])
 h.close()
+# multi-start L-BFGS: the stencil and step kernels over three starts (one clipped onto a corner), with maxcor = 2 so the
+# pair ring wraps, on an acquisition and on the posterior objective
+h = _lib.Handle(0)
+h.set_data(X[:100], y[:100])
+h.set_kernel(f["family"], f["log_amp"], f["axis"], f["group"], f["log_metric"])
+h.fit(1e-3 + 1.25e-12, float(y[:100].mean()))
+x0 = rng.rand(3, D)
+x0[1] = 2.0
+r = _lib.maximize_lbfgs([h], _lib.ACQ_LOG_EI, [float(y[:100].min())], 0.0, x0, np.zeros(D), np.ones(D), maxcor=2,
+                        maxiter=8)
+print("lbfgs", r["nfev"], r["status"],
+      _lib.maximize_lbfgs([h], _lib.OBJ_MEAN_STD, None, 0.0, x0, np.zeros(D), np.ones(D), maxiter=8)["status"])
+h.close()
 h = _lib.moments_handle()
 print(h.acq_moments(rng.randn(100), rng.rand(100) + 0.1, _lib.ACQ_LOG_EI, 0.0, 0.0)[0][:3])
 print(h.reduce_models(rng.rand(4, 50), rng.rand(4, 50))[1][:3])
