@@ -588,16 +588,26 @@ def shard_bounds(m, rank, world):
     return lo.value, hi.value
 
 
+def _handles(handles):
+    """The C array of the handles' pointers, the first argument of every entry point over several models."""
+    return (_vp * len(handles))(*[h._h for h in handles])
+
+
+def _etas(eta, n):
+    """eta (a scalar or one value per model; None: zeros) as n contiguous doubles."""
+    return f64(np.zeros(n) if eta is None else np.broadcast_to(np.asarray(eta, dtype=np.float64), (n,)))
+
+
 def acq_multi(handles, Xs, mode, kind=ACQ_NONE, eta=None, par=0.0, want_argmax=False):
     """gpk_acq_multi over ``handles`` (all fitted, same device).  mode 0 -> dict(values, n_negative, best_val,
     best_idx); mode 1 -> dict(mean, var)."""
     h0 = handles[0]
     Xs = f64(Xs)
     m = Xs.shape[0]
-    arr = (_vp * len(handles))(*[h._h for h in handles])
+    arr = _handles(handles)
     out1 = np.empty(m)
     out2 = np.empty(m) if mode == 1 else None
-    etas = f64(np.zeros(len(handles)) if eta is None else np.broadcast_to(np.asarray(eta, dtype=np.float64), (len(handles),)))
+    etas = _etas(eta, len(handles))
     nn, bv, bi = C.c_long(0), C.c_double(), C.c_long(-1)
     h0._check(h0.lib.gpk_acq_multi(arr, len(handles), _as_dp(Xs), m, int(mode), int(kind), _as_dp(etas), float(par),
                                    _as_dp(out1), _as_dp(out2) if out2 is not None else None, C.byref(nn),
@@ -613,8 +623,8 @@ def maximize_de(handles, seed, pop, maxiter, mutation, recombination, tol, atol,
     mean over the handles.  -> dict(x (D,), energy, nit, nfev, n_negative[, population (pop, D), energies (pop,)])."""
     h0 = handles[0]
     lo, up = f64(lower).ravel(), f64(upper).ravel()
-    arr = (_vp * len(handles))(*[h._h for h in handles])
-    etas = f64(np.broadcast_to(np.asarray(eta, dtype=np.float64), (len(handles),)))
+    arr = _handles(handles)
+    etas = _etas(eta, len(handles))
     x = np.empty(lo.size)
     pop = int(pop)
     P = np.empty((pop, lo.size)) if want_population and pop > 0 else None
@@ -625,17 +635,16 @@ def maximize_de(handles, seed, pop, maxiter, mutation, recombination, tol, atol,
                                      float(atol), _as_dp(lo), _as_dp(up), int(kind), _as_dp(etas), float(par),
                                      _as_dp(x), C.byref(be), C.byref(nit), C.byref(nfev), C.byref(nn),
                                      _as_dp(P) if P is not None else None, _as_dp(E) if E is not None else None))
-    r = dict(x=x, energy=be.value, nit=nit.value, nfev=nfev.value, n_negative=nn.value)
-    if want_population:
-        r.update(population=P, energies=E)
+    r = _de_result(x, be, nit, nfev, P, E, want_population)
+    r["n_negative"] = nn.value
     return r
 
 
 def _es_cost_args(objective, cost, lower, upper):
     if len(objective) == 0 or len(objective) != len(cost):
         raise ValueError("information gain per unit cost: need as many cost handles as objective handles (>= 1)")
-    ho = (_vp * len(objective))(*[h._h for h in objective])
-    hc = (_vp * len(cost))(*[h._h for h in cost])
+    ho = _handles(objective)
+    hc = _handles(cost)
     lo, up = f64(lower).ravel(), f64(upper).ravel()
     if lo.size != up.size:
         raise ValueError("information gain per unit cost: lower and upper differ in length")
@@ -688,7 +697,7 @@ def es_multi(objective, Xs, want_values=True):
     """gpk_es_multi: the entropy change of every row of Xs (m, d) under each handle, averaged over the handles ->
     dict(values (m,) or None, best_val, best_idx)."""
     h0 = objective[0]
-    ho = (_vp * len(objective))(*[h._h for h in objective])
+    ho = _handles(objective)
     Xs = f64(Xs)
     m = Xs.shape[0]
     out = np.empty(m) if want_values else None
@@ -701,7 +710,7 @@ def es_multi(objective, Xs, want_values=True):
 def es_multi_dev(objective, d_Xs_ptr, m, d_out_ptr, d_best_ptr=0):
     """Device-batch variant, asynchronous on objective[0]'s stream."""
     h0 = objective[0]
-    ho = (_vp * len(objective))(*[h._h for h in objective])
+    ho = _handles(objective)
     h0._check(h0.lib.gpk_es_multi_dev(ho, len(objective), _vp(d_Xs_ptr), int(m), _vp(d_out_ptr or 0),
                                       _vp(d_best_ptr or 0)))
 
@@ -718,7 +727,7 @@ def maximize_de_es(objective, seed, pop, maxiter, mutation, recombination, tol, 
     """gpk_maximize_de_es: differential evolution minimising minus the entropy change (one handle: gpk_es_compute's
     value; several: gpk_es_multi's mean) -> dict(x (D,), energy, nit, nfev[, population (pop, D), energies (pop,)])."""
     h0 = objective[0]
-    ho = (_vp * len(objective))(*[h._h for h in objective])
+    ho = _handles(objective)
     lo, up = f64(lower).ravel(), f64(upper).ravel()
     x = np.empty(lo.size)
     pop = int(pop)
@@ -793,9 +802,8 @@ def maximize_lbfgs(handles, kind, eta, par, x0, lower, upper, **options):
     dict(x (n_starts, d), energy, nit, nfev, status (n_starts each), n_negative)."""
     h0 = handles[0]
     x0, lo, up, outs = _lb_io(x0, lower, upper)
-    arr = (_vp * len(handles))(*[h._h for h in handles])
-    etas = f64(np.zeros(len(handles)) if eta is None else np.broadcast_to(np.asarray(eta, dtype=np.float64),
-                                                                           (len(handles),)))
+    arr = _handles(handles)
+    etas = _etas(eta, len(handles))
     nn = C.c_long()
     h0._check(h0.lib.gpk_maximize_lbfgs(arr, len(handles), int(kind), _as_dp(etas), float(par), x0.shape[0], _as_dp(x0),
                                         _as_dp(lo), _as_dp(up), *_lb_opts(options), *_lb_out_ptrs(outs), C.byref(nn)))
@@ -808,7 +816,7 @@ def maximize_lbfgs_es(objective, x0, lower, upper, **options):
     """gpk_maximize_lbfgs_es: the same minimising minus the entropy change (one handle: gpk_es_compute's value;
     several: gpk_es_multi's mean) -> dict(x, energy, nit, nfev, status)."""
     h0 = objective[0]
-    ho = (_vp * len(objective))(*[h._h for h in objective])
+    ho = _handles(objective)
     x0, lo, up, outs = _lb_io(x0, lower, upper)
     h0._check(h0.lib.gpk_maximize_lbfgs_es(ho, len(objective), x0.shape[0], _as_dp(x0), _as_dp(lo), _as_dp(up),
                                            *_lb_opts(options), *_lb_out_ptrs(outs)))
@@ -841,9 +849,9 @@ def sample_representers(models, seeds, nb, steps, max_runs, kind, eta, par, lowe
     if n < 1:
         raise ValueError("sample_representers: need at least one model")
     h0 = models[0]
-    hs = (_vp * n)(*[h._h for h in models])
+    hs = _handles(models)
     sd = np.ascontiguousarray(np.asarray(seeds, dtype=np.uint64).ravel())
-    etas = f64(np.broadcast_to(np.asarray(eta, dtype=np.float64), (n,)))
+    etas = _etas(eta, n)
     lo, up = f64(lower).ravel(), f64(upper).ravel()
     if sd.size != n or lo.size != up.size:
         raise ValueError("sample_representers: need one seed per model and lower / upper of one length")

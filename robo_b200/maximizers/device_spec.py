@@ -1,5 +1,5 @@
 """What scores an acquisition on the device, shared by the device maximizers (DifferentialEvolution, SciPyOptimizer),
-and the multi-start L-BFGS call over it (gpk_maximize_lbfgs*)."""
+and the differential-evolution and multi-start L-BFGS calls over it (gpk_maximize_de*, gpk_maximize_lbfgs*)."""
 import numpy as np
 
 from robo_b200 import _lib
@@ -53,21 +53,38 @@ def acq_spec(acq, who):
     return kind, [eta], float(acq.par), [model.gp.handle]
 
 
-def maximize_lbfgs(which, spec, x0, lower, upper):
-    """Multi-start L-BFGS on the device from the rows of x0 over what ``device_spec`` returned, scipy's L-BFGS-B
-    defaults -> _lib's result dict (x, energy, nit, nfev, status per start).  ValueError as ei.py:86-88 when EI came
-    out negative."""
+def _run(which, spec, es_cost, es, acq):
+    """Calls the maximizer of ``which`` over ``spec`` (what ``device_spec`` returned): es_cost(ho, hc, **configuration),
+    es(handles) or acq(handles, kind code, etas, par).  ValueError as ei.py:86-88 when EI came out negative."""
     if which == "es_cost":
         ho, hc, lo, up, bo, bc, oh = spec
-        return _lib.maximize_lbfgs_es_cost(ho, hc, x0, lower, upper, cfg_lower=lo, cfg_upper=up, basis_objective=bo,
-                                           basis_cost=bc, overhead=oh)
+        return es_cost(ho, hc, cfg_lower=lo, cfg_upper=up, basis_objective=bo, basis_cost=bc, overhead=oh)
     if which == "es":
-        return _lib.maximize_lbfgs_es(spec, x0, lower, upper)
+        return es(spec)
     kind, etas, par, handles = spec
-    r = _lib.maximize_lbfgs(handles, _lib.ACQ_KIND[kind], etas, par, x0, lower, upper)
+    r = acq(handles, _lib.ACQ_KIND[kind], etas, par)
     if kind == "ei" and r["n_negative"] > 0:
         raise ValueError("Expected Improvement is smaller than 0!")
     return r
+
+
+def maximize_de(which, spec, seed, pop, maxiter, mutation, recombination, tol, atol, lower, upper):
+    """Differential evolution on the device over what ``device_spec`` returned -> _lib's result dict (x, energy, nit,
+    nfev)."""
+    args = (seed, pop, maxiter, mutation, recombination, tol, atol, lower, upper)
+    return _run(which, spec,
+                lambda ho, hc, **cfg: _lib.maximize_de_es_cost(ho, hc, *args, **cfg),
+                lambda hs: _lib.maximize_de_es(hs, *args),
+                lambda hs, kind, etas, par: _lib.maximize_de(hs, *args, kind=kind, eta=etas, par=par))
+
+
+def maximize_lbfgs(which, spec, x0, lower, upper):
+    """Multi-start L-BFGS on the device from the rows of x0 over what ``device_spec`` returned, scipy's L-BFGS-B
+    defaults -> _lib's result dict (x, energy, nit, nfev, status per start)."""
+    return _run(which, spec,
+                lambda ho, hc, **cfg: _lib.maximize_lbfgs_es_cost(ho, hc, x0, lower, upper, **cfg),
+                lambda hs: _lib.maximize_lbfgs_es(hs, x0, lower, upper),
+                lambda hs, kind, etas, par: _lib.maximize_lbfgs(hs, kind, etas, par, x0, lower, upper))
 
 
 def lbfgs_success(status):

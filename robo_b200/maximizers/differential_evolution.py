@@ -27,9 +27,8 @@ import sys
 import numpy as np
 import scipy.optimize
 
-from robo_b200 import _lib
 from robo_b200.maximizers.base_maximizer import BaseMaximizer
-from robo_b200.maximizers.device_spec import device_spec, lbfgs_success, maximize_lbfgs
+from robo_b200.maximizers.device_spec import device_spec, lbfgs_success, maximize_de, maximize_lbfgs
 
 
 class DifferentialEvolution(BaseMaximizer):
@@ -64,18 +63,8 @@ class DifferentialEvolution(BaseMaximizer):
         seed = (self.seed + 0x9E3779B97F4A7C15 * self.calls) & 0xFFFFFFFFFFFFFFFF
         self.calls += 1
         pop = max(5, int(self.popsize) * lower.size)                 # scipy: max(5, popsize * D)
-        args = (seed, pop, int(self.n_iters), self.mutation, self.recombination, self.tol, self.atol, lower, upper)
-        if which == "es_cost":
-            ho, hc, lo, up, bo, bc, oh = spec
-            r = _lib.maximize_de_es_cost(ho, hc, *args, cfg_lower=lo, cfg_upper=up, basis_objective=bo, basis_cost=bc,
-                                         overhead=oh)
-        elif which == "es":
-            r = _lib.maximize_de_es(spec, *args)
-        else:
-            kind, etas, par, handles = spec
-            r = _lib.maximize_de(handles, *args, kind=_lib.ACQ_KIND[kind], eta=etas, par=par)
-            if kind == "ei" and r["n_negative"] > 0:
-                raise ValueError("Expected Improvement is smaller than 0!")      # ei.py:86-88
+        r = maximize_de(which, spec, seed, pop, int(self.n_iters), self.mutation, self.recombination, self.tol,
+                        self.atol, lower, upper)
         x, fun, nfev, polished = r["x"], r["energy"], r["nfev"], False
         if self.polish == "device":
             res = maximize_lbfgs(which, spec, x[None, :], lower, upper)
