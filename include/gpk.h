@@ -326,6 +326,69 @@ int gpk_es_multi(gpk_handle* const* objective, int n, const double* Xs, long m, 
  * d_best (16 bytes {double value; long long index}) may be NULL. */
 int gpk_es_multi_dev(gpk_handle* const* objective, int n, const void* d_Xs, long m, void* d_out, void* d_best);
 
+/* The sampling-based entropy search, InformationGainMC (robo/acquisition_functions/information_gain_mc.py) with its
+ * p_min estimator joint_pmin (robo/util/mc_part.py), on the device (robo_b200/csrc/gpk_esmc.cuh states every rounding
+ * step and summation order).  The reference draws F ~ N(0, I) (Nf x Nb) afresh on every joint_pmin call; here F (nb x
+ * nf) comes from Philox4x32-10 keyed by `seed` and Box-Muller, and one F serves an update and every candidate until the
+ * next update (common random numbers): each value has the reference's marginal law, compute(x) is a deterministic
+ * function of x between updates, and no value depends on its position in a batch, on "chunk" or on how a batch is split.
+ * The factorisation of V + noise I climbs the reference's jitter ladder float for float (0, 1e-9, 1e-8, ..., 10000.0);
+ * a failure at 10000.0 is GPK_NOT_PD (numpy.linalg.LinAlgError, mc_part.py:40-41). */
+
+/* mc_part.joint_pmin(m, V, Nf) (mc_part.py:7-68) on caller operands: m (nb x np row-major; the reference's Mb is np = 1),
+ * V (nb x nb, only its lower triangle is read), F drawn from `seed`.  pmin (nb) = count of each point as the column
+ * minimum (numpy.argmin: the first index wins a tie) over the nf np columns, divided by nf np and clamped below at
+ * 1e-70.  n_jitter (may be NULL): 1 when the factorisation needed jitter (the reference logs it), else 0.  Uses its own
+ * scratch; no fit is needed.  1 <= nb <= 64, np >= 1, nf >= 1, nf np < 2^31. */
+int gpk_mc_pmin(gpk_handle* h, const double* m, int np, const double* V, int nb, int nf, unsigned long long seed,
+                double* pmin, int* n_jitter);
+/* The draws F (nb x nf row-major) that `seed` gives gpk_mc_pmin and gpk_esmc_update; F[k][f] depends on (seed, k, f)
+ * only.  nb >= 1, nf >= 1. */
+int gpk_mc_draws(gpk_handle* h, unsigned long long seed, int nb, int nf, double* F);
+/* InformationGainMC.update after the representer points are sampled (information_gain_mc.py:103-121): Mb, Vb =
+ * predict(zb, full_cov=True) (clipped like the reference), F from `seed`, pmin = joint_pmin(Mb as (nb, 1), Vb, nf),
+ * logP = log(pmin), H = -sum_i exp(logP_i) (logP_i + lmb_i), the scaled zb and U = K^-1 K(X, zb) as gpk_es_update builds
+ * them; everything the candidates need stays on the device.  zb (nb x d raw inputs), lmb (nb: GPK_BAD_ARG "lmb should
+ * not be infinite." when one is not finite), sn2 the model's noise, W (np) the innovation quantiles.  logP and pmin (nb)
+ * may be NULL.  2 <= nb <= 64, np >= 1, nf >= 1, nf np < 2^31.  GPK_NOT_PD as for gpk_mc_pmin.  After it, gpk_es_compute
+ * and the other consumers of gpk_es_update are GPK_BAD_ARG until the next gpk_es_update, and the reverse holds for the
+ * gpk_esmc_* consumers; gpk_es_moments, gpk_es_dims and gpk_es_get_u serve either update. */
+int gpk_esmc_update(gpk_handle* h, const double* zb, int nb, const double* lmb, double sn2, const double* W, int np,
+                    int nf, unsigned long long seed, double* logP, double* pmin);
+/* InformationGainMC.compute (information_gain_mc.py:67-79, 123-156) over m candidates Xs (m x d raw inputs), one value
+ * each: with v the predictive variance (noise included), iv = 1 / (v - sn2), sigma the clipped covariance to zb (as
+ * gpk_es_compute), nc_a = sigma_a iv: Mb_new[a][p] = Mb_a + nc_a sqrt(v + 1e-10) W_p, Vb_new[a][b] = Vb[a][b] -
+ * nc_a sigma_b, new = joint_pmin(Mb_new, Vb_new, nf) on the update's F, and
+ *   value = sum_i new_i (log new_i + lmb_i) + H   (larger is more information; NaN or +inf -> -DBL_MAX).
+ * There is no bounds test (the reference has none).  GPK_BAD_ARG before gpk_esmc_update, after the model changed since,
+ * or after a gpk_es_update; GPK_NOT_PD when a candidate's factorisation fails at every rung (on the _dev variant that
+ * candidate's value is NaN and the status is not read back). */
+int gpk_esmc_compute(gpk_handle* h, const double* Xs, long m, double* out);
+/* the same on device pointers (d_Xs: m x d, d_out: m doubles), asynchronous on the handle's stream */
+int gpk_esmc_compute_dev(gpk_handle* h, const void* d_Xs, long m, void* d_out);
+/* MarginalizationGPMCMC.compute over InformationGainMC estimators as one call: gpk_esmc_compute of every objective[i],
+ * each handle on its own stream, then the mean over the n handles (gpk_reduce_models mode 0, also for n = 1); bit-identical
+ * to the n gpk_esmc_compute values reduced by gpk_reduce_models.  Arguments and errors as for gpk_es_multi, with
+ * gpk_esmc_update in place of gpk_es_update, and GPK_NOT_PD as for gpk_esmc_compute. */
+int gpk_esmc_multi(gpk_handle* const* objective, int n, const double* Xs, long m, double* out, double* best_val,
+                   long* best_idx);
+int gpk_esmc_multi_dev(gpk_handle* const* objective, int n, const void* d_Xs, long m, void* d_out, void* d_best);
+/* gpk_maximize_de_es over the sampling-based entropy change: -(gpk_esmc_multi's value of the member over objective[0 ..
+ * n-1]); n = 1: -(gpk_esmc_compute's value), no reduction.  Arguments and outputs as for gpk_maximize_de_es; GPK_NOT_PD
+ * as for gpk_esmc_compute (checked after every generation). */
+int gpk_maximize_de_esmc(gpk_handle* const* objective, int n, unsigned long long seed, long pop, int maxiter,
+                         double mut_lo, double mut_hi, double recombination, double tol, double atol,
+                         const double* lower, const double* upper, double* best_x, double* best_energy, int* nit,
+                         long* nfev, double* population, double* energies);
+/* Diagnostics of the current gpk_esmc_update: its draws F (nb x nf row-major), and its Mb (nb) and Vb (nb x nb), as a
+ * host restatement needs them; GPK_BAD_ARG as for gpk_esmc_compute. */
+int gpk_esmc_get_draws(gpk_handle* h, double* F);
+int gpk_esmc_get_state(gpk_handle* h, double* Mb, double* Vb);
+/* factorisations that needed jitter in the handle's last host-synchronised p_min call (gpk_mc_pmin, gpk_esmc_update,
+ * gpk_esmc_compute; for gpk_esmc_multi and gpk_maximize_de_esmc: on objective[0], over all models, a DE run counted
+ * from its start) */
+int gpk_esmc_last_jitter(gpk_handle* h, long* n_jitter);
+
 /* basis functions of the environment column of Fabolas models (robo/fmin/fabolas.py:96-102) */
 typedef enum {
     GPK_BASIS_S = 0,           /* basis(s) = s          (the cost model)      */

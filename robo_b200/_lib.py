@@ -87,6 +87,18 @@ _SIGNATURES = {
     "gpk_es_moments": [_vp, _dp, C.c_long, _dp, _dp],
     "gpk_es_get_u": [_vp, _dp],
     "gpk_es_dims": [_vp, _ip, _ip],
+    "gpk_mc_pmin": [_vp, _dp, C.c_int, _dp, C.c_int, C.c_int, C.c_ulonglong, _dp, _ip],
+    "gpk_mc_draws": [_vp, C.c_ulonglong, C.c_int, C.c_int, _dp],
+    "gpk_esmc_update": [_vp, _dp, C.c_int, _dp, C.c_double, _dp, C.c_int, C.c_int, C.c_ulonglong, _dp, _dp],
+    "gpk_esmc_compute": [_vp, _dp, C.c_long, _dp],
+    "gpk_esmc_compute_dev": [_vp, _vp, C.c_long, _vp],
+    "gpk_esmc_multi": [C.POINTER(_vp), C.c_int, _dp, C.c_long, _dp, _dp, _lp],
+    "gpk_esmc_multi_dev": [C.POINTER(_vp), C.c_int, _vp, C.c_long, _vp, _vp],
+    "gpk_maximize_de_esmc": [C.POINTER(_vp), C.c_int, C.c_ulonglong, C.c_long, C.c_int, C.c_double, C.c_double,
+                             C.c_double, C.c_double, C.c_double, _dp, _dp, _dp, _dp, _ip, _lp, _dp, _dp],
+    "gpk_esmc_get_draws": [_vp, _dp],
+    "gpk_esmc_get_state": [_vp, _dp, _dp],
+    "gpk_esmc_last_jitter": [_vp, _lp],
     "gpk_predict_mean": [_vp, _dp, C.c_long, _dp],
     "gpk_predict_mean_dev": [_vp, _vp, C.c_long, _vp],
     "gpk_es_cost_multi": [C.POINTER(_vp), C.POINTER(_vp), C.c_int, _dp, C.c_long, _dp, _dp, C.c_int, C.c_int, C.c_int,
@@ -546,6 +558,67 @@ class Handle(object):
         self._check(self.lib.gpk_es_get_u(self._h, _as_dp(U)))
         return U
 
+    # -- sampling-based entropy search (gpk_esmc.cuh) --------------------------------------------------------------
+    def mc_pmin(self, m, V, nf, seed):
+        """gpk_mc_pmin: joint_pmin on caller operands, m (nb,) or (nb, np), V (nb, nb) -> (pmin (nb,), n_jitter)."""
+        m, V = f64(m), f64(V)
+        if m.ndim == 1:
+            m = m[:, None]
+        nb, np_ = m.shape
+        if V.shape != (nb, nb):
+            raise ValueError("mc_pmin: V must be %d x %d" % (nb, nb))
+        pmin, nj = np.empty(nb), C.c_int(0)
+        self._check(self.lib.gpk_mc_pmin(self._h, _as_dp(m), np_, _as_dp(V), nb, int(nf),
+                                         int(seed) & 0xFFFFFFFFFFFFFFFF, _as_dp(pmin), C.byref(nj)))
+        return pmin, nj.value
+
+    def mc_draws(self, seed, nb, nf):
+        """gpk_mc_draws: the draws F (nb, nf) a seed gives."""
+        F = np.empty((int(nb), int(nf)))
+        self._check(self.lib.gpk_mc_draws(self._h, int(seed) & 0xFFFFFFFFFFFFFFFF, int(nb), int(nf), _as_dp(F)))
+        return F
+
+    def esmc_update(self, zb, lmb, sn2, W, nf, seed):
+        """gpk_esmc_update -> dict(logP (nb,), pmin (nb,), n_jitter)."""
+        zb, lmb, W = f64(zb), f64(lmb).ravel(), f64(W).ravel()
+        nb = zb.shape[0]
+        if lmb.size != nb:
+            raise ValueError("esmc_update: lmb needs one value per representer point")
+        logP, pmin = np.empty(nb), np.empty(nb)
+        self._check(self.lib.gpk_esmc_update(self._h, _as_dp(zb), nb, _as_dp(lmb), float(sn2), _as_dp(W), W.size,
+                                             int(nf), int(seed) & 0xFFFFFFFFFFFFFFFF, _as_dp(logP), _as_dp(pmin)))
+        self._esmc_nf = int(nf)
+        return dict(logP=logP, pmin=pmin, n_jitter=self.esmc_last_jitter())
+
+    def esmc_compute(self, Xs):
+        """gpk_esmc_compute: the sampling-based entropy change of every row of Xs (m, d) -> (m,)."""
+        Xs = f64(Xs)
+        out = np.empty(Xs.shape[0])
+        self._check(self.lib.gpk_esmc_compute(self._h, _as_dp(Xs), Xs.shape[0], _as_dp(out)))
+        return out
+
+    def esmc_compute_dev(self, d_Xs_ptr, m, d_out_ptr):
+        self._check(self.lib.gpk_esmc_compute_dev(self._h, _vp(d_Xs_ptr), int(m), _vp(d_out_ptr)))
+
+    def esmc_get_draws(self):
+        """gpk_esmc_get_draws (diagnostic): the current update's F (nb, nf)."""
+        F = np.empty((self.es_dims()[1], self._esmc_nf))
+        self._check(self.lib.gpk_esmc_get_draws(self._h, _as_dp(F)))
+        return F
+
+    def esmc_get_state(self):
+        """gpk_esmc_get_state (diagnostic): the current update's (Mb (nb,), Vb (nb, nb))."""
+        nb = self.es_dims()[1]
+        Mb, Vb = np.empty(nb), np.empty((nb, nb))
+        self._check(self.lib.gpk_esmc_get_state(self._h, _as_dp(Mb), _as_dp(Vb)))
+        return Mb, Vb
+
+    def esmc_last_jitter(self):
+        """gpk_esmc_last_jitter: factorisations that needed jitter in the last synchronised p_min call."""
+        n = C.c_long(0)
+        self._check(self.lib.gpk_esmc_last_jitter(self._h, C.byref(n)))
+        return n.value
+
     def predict_mean(self, Xs):
         """gpk_predict_mean: the predictive mean alone of every row of Xs (m, d) -> (m,)."""
         Xs = f64(Xs)
@@ -715,6 +788,27 @@ def es_multi_dev(objective, d_Xs_ptr, m, d_out_ptr, d_best_ptr=0):
                                       _vp(d_best_ptr or 0)))
 
 
+def esmc_multi(objective, Xs, want_values=True):
+    """gpk_esmc_multi: the sampling-based entropy change of every row of Xs (m, d) under each handle, averaged over the
+    handles -> dict(values (m,) or None, best_val, best_idx)."""
+    h0 = objective[0]
+    ho = _handles(objective)
+    Xs = f64(Xs)
+    m = Xs.shape[0]
+    out = np.empty(m) if want_values else None
+    bv, bi = C.c_double(), C.c_long(-1)
+    h0._check(h0.lib.gpk_esmc_multi(ho, len(objective), _as_dp(Xs), m, _as_dp(out) if want_values else None,
+                                    C.byref(bv), C.byref(bi)))
+    return dict(values=out, best_val=bv.value, best_idx=bi.value)
+
+
+def esmc_multi_dev(objective, d_Xs_ptr, m, d_out_ptr, d_best_ptr=0):
+    """Device-batch variant, asynchronous on objective[0]'s stream."""
+    h0 = objective[0]
+    h0._check(h0.lib.gpk_esmc_multi_dev(_handles(objective), len(objective), _vp(d_Xs_ptr), int(m), _vp(d_out_ptr or 0),
+                                        _vp(d_best_ptr or 0)))
+
+
 def _de_result(x, be, nit, nfev, P, E, want_population):
     r = dict(x=x, energy=be.value, nit=nit.value, nfev=nfev.value)
     if want_population:
@@ -739,6 +833,26 @@ def maximize_de_es(objective, seed, pop, maxiter, mutation, recombination, tol, 
                                         float(atol), _as_dp(lo), _as_dp(up), _as_dp(x), C.byref(be), C.byref(nit),
                                         C.byref(nfev), _as_dp(P) if P is not None else None,
                                         _as_dp(E) if E is not None else None))
+    return _de_result(x, be, nit, nfev, P, E, want_population)
+
+
+def maximize_de_esmc(objective, seed, pop, maxiter, mutation, recombination, tol, atol, lower, upper,
+                     want_population=False):
+    """gpk_maximize_de_esmc: differential evolution minimising minus the sampling-based entropy change (one handle:
+    gpk_esmc_compute's value; several: gpk_esmc_multi's mean) -> as maximize_de_es."""
+    h0 = objective[0]
+    ho = _handles(objective)
+    lo, up = f64(lower).ravel(), f64(upper).ravel()
+    x = np.empty(lo.size)
+    pop = int(pop)
+    P = np.empty((pop, lo.size)) if want_population and pop > 0 else None
+    E = np.empty(pop) if want_population and pop > 0 else None
+    be, nit, nfev = C.c_double(), C.c_int(), C.c_long()
+    h0._check(h0.lib.gpk_maximize_de_esmc(ho, len(objective), int(seed) & 0xFFFFFFFFFFFFFFFF, pop, int(maxiter),
+                                          float(mutation[0]), float(mutation[1]), float(recombination), float(tol),
+                                          float(atol), _as_dp(lo), _as_dp(up), _as_dp(x), C.byref(be), C.byref(nit),
+                                          C.byref(nfev), _as_dp(P) if P is not None else None,
+                                          _as_dp(E) if E is not None else None))
     return _de_result(x, be, nit, nfev, P, E, want_population)
 
 

@@ -40,8 +40,10 @@ def sample_representers_device(estimators):
     """The representer points of every estimator (InformationGain or InformationGainPerUnitCost) drawn on the device by
     the stretch move (gpk_sample_representers), one call for all estimators that share the sampler's arguments.  Each
     estimator draws its seed from its own rng (one draw per update); eta is its sampling acquisition's incumbent value
-    (0 for LCB).  Raises TypeError when an estimator cannot sample on the device, and the reference's ValueErrors:
-    ei.py's on a negative EI value, and InformationGainPerUnitCost's when -inf remains after 5 runs."""
+    (0 for LCB); the stretch move runs the estimator's REPRESENTER_STEPS steps for at most REPRESENTER_RUNS runs (50 and 5
+    for InformationGain, 200 and 1 for InformationGainMC), which join the grouping key.  Raises TypeError when an
+    estimator cannot sample on the device, and the reference's ValueErrors: ei.py's on a negative EI value, and
+    InformationGainPerUnitCost's when -inf remains after 5 runs."""
     from robo_b200 import _lib
     calls = {}
     for e in estimators:
@@ -53,12 +55,14 @@ def sample_representers_device(estimators):
         handle, lower, upper, fabolas = e._representer_spec()
         eta = 0.0 if kind == "lcb" else float(e.model.get_incumbent()[1])
         seed = int(e.rng.randint(0, 2 ** 63, dtype=np.int64))
-        key = (kind, float(sa.par), int(e.Nb), lower.tobytes(), upper.tobytes(),
+        steps, runs = int(e.REPRESENTER_STEPS), int(e.REPRESENTER_RUNS)
+        key = (kind, float(sa.par), int(e.Nb), steps, runs, lower.tobytes(), upper.tobytes(),
                None if fabolas is None else tuple((k, np.asarray(v).tobytes()) for k, v in sorted(fabolas.items())))
-        calls.setdefault(key, (kind, float(sa.par), int(e.Nb), lower, upper, fabolas, []))[-1].append(
+        calls.setdefault(key, (kind, float(sa.par), int(e.Nb), steps, runs, lower, upper, fabolas, []))[-1].append(
             (e, handle, seed, eta))
-    for kind, par, nb, lower, upper, fabolas, members in calls.values():
-        r = _lib.sample_representers([m[1] for m in members], [m[2] for m in members], nb, 50, 5, _lib.ACQ_KIND[kind],
+    for kind, par, nb, steps, runs, lower, upper, fabolas, members in calls.values():
+        r = _lib.sample_representers([m[1] for m in members], [m[2] for m in members], nb, steps, runs,
+                                     _lib.ACQ_KIND[kind],
                                      [m[3] for m in members], par, lower, upper, fabolas=fabolas)
         if kind == "ei" and r["n_negative"] > 0:
             raise ValueError("Expected Improvement is smaller than 0!")      # ei.py:86-88
@@ -67,6 +71,9 @@ def sample_representers_device(estimators):
 
 
 class InformationGain(BaseAcquisitionFunction):
+
+    # the stretch move of the representer points (information_gain.py:68-81): at most 5 runs of 50 steps
+    REPRESENTER_STEPS, REPRESENTER_RUNS = 50, 5
 
     def __init__(self, model, lower, upper, Nb=50, Np=400, sampling_acquisition=None,
                  sampling_acquisition_kw={"par": 0.0}, rng=None, representer_sampler="host", **kwargs):

@@ -24,6 +24,8 @@ class MarginalizationGPMCMC(BaseAcquisitionFunction):
         for i in range(len(self.model.models)):
             estimator = deepcopy(self.acquisition_func)
             estimator.model = self.model.models[i]
+            if hasattr(estimator, "stream"):         # InformationGainMC: its own draws per sub-model
+                estimator.stream = i
             if self.cost_model is not None and len(self.cost_model.models) > 0:
                 estimator.cost_model = self.cost_model.models[i]
             self.estimators.append(estimator)
@@ -63,6 +65,10 @@ class MarginalizationGPMCMC(BaseAcquisitionFunction):
             # information gain per unit cost over the (objective, cost) sub-model pairs as ONE call (gpk_es_cost_multi)
             ho, hc, lo, up, bo, bc, oh = es
             return _lib.es_cost_multi(ho, hc, np.asarray(X_test, dtype=np.float64), lo, up, bo, bc, oh)["values"]
+        handles = self._esmc_spec() if not derivative else None
+        if handles is not None:
+            # the sampling-based information gain of every estimator and the mean over them as ONE call (gpk_esmc_multi)
+            return _lib.esmc_multi(handles, np.asarray(X_test, dtype=np.float64))["values"]
         handles = self._es_spec() if not derivative else None
         if handles is not None:
             # the information gain of every estimator and the mean over them as ONE call (gpk_es_multi)
@@ -89,6 +95,9 @@ class MarginalizationGPMCMC(BaseAcquisitionFunction):
             ho, hc, lo, up, bo, bc, oh = es
             r = _lib.es_cost_multi(ho, hc, np.asarray(X_test, dtype=np.float64), lo, up, bo, bc, oh, want_values=False)
             return int(r["best_idx"])
+        handles = self._esmc_spec()
+        if handles is not None:
+            return int(_lib.esmc_multi(handles, np.asarray(X_test, dtype=np.float64), want_values=False)["best_idx"])
         handles = self._es_spec()
         if handles is not None:
             return int(_lib.es_multi(handles, np.asarray(X_test, dtype=np.float64), want_values=False)["best_idx"])
@@ -113,14 +122,25 @@ class MarginalizationGPMCMC(BaseAcquisitionFunction):
         return device_spec(self.estimators)
 
     def _es_spec(self):
-        """The objective handles of the fused call (gpk_es_multi) when every estimator is an InformationGain, not per
-        unit cost, on a device GaussianProcess sub-model; raises the estimators' own ValueErrors (before update(), an
-        infinite lmb)."""
+        """The objective handles of the fused call (gpk_es_multi) when every estimator is an InformationGain, neither
+        per unit cost nor sampling-based, on a device GaussianProcess sub-model; raises the estimators' own ValueErrors
+        (before update(), an infinite lmb)."""
         from robo_b200.acquisition_functions.information_gain import InformationGain
+        from robo_b200.acquisition_functions.information_gain_mc import InformationGainMC
         from robo_b200.acquisition_functions.information_gain_per_unit_cost import InformationGainPerUnitCost
         from robo_b200.maximizers.device_spec import raw_inputs as _raw_inputs
         if len(self.estimators) == 0 or not all(isinstance(e, InformationGain) and
-                                                not isinstance(e, InformationGainPerUnitCost) and _raw_inputs(e.model)
+                                                not isinstance(e, (InformationGainPerUnitCost, InformationGainMC))
+                                                and _raw_inputs(e.model) for e in self.estimators):
+            return None
+        return [e._ready_handle() for e in self.estimators]
+
+    def _esmc_spec(self):
+        """The objective handles of the fused call (gpk_esmc_multi) when every estimator is an InformationGainMC on a
+        device GaussianProcess sub-model; raises the estimators' own ValueErrors."""
+        from robo_b200.acquisition_functions.information_gain_mc import InformationGainMC
+        from robo_b200.maximizers.device_spec import raw_inputs as _raw_inputs
+        if len(self.estimators) == 0 or not all(isinstance(e, InformationGainMC) and _raw_inputs(e.model)
                                                 for e in self.estimators):
             return None
         return [e._ready_handle() for e in self.estimators]

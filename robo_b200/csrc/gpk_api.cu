@@ -28,6 +28,7 @@
 #include "gpk_de.cuh"
 #include "gpk_lbfgs.cuh"
 #include "gpk_es.cuh"
+#include "gpk_esmc.cuh"
 #include "gpk_rs.cuh"
 #include "gpk_hyper.cuh"
 
@@ -164,6 +165,12 @@ struct gpk_handle {
     int es_nb = 0, es_np = 0;
     double es_sn2 = 0.0, es_H = 0.0;
     long es_linv_serial = -1;       // linv_serial U was built for (-1: no update yet)
+    int es_kind = 0;                // which update is current: ES_KIND_EP (gpk_es_update) or ES_KIND_MC (gpk_esmc_update)
+    // sampling-based entropy search (gpk_esmc_update / gpk_esmc_compute): Mb, Vb, W, lmb, scaled zb and the draws F;
+    // the scratch of gpk_mc_pmin / gpk_mc_draws; the two status words of the last pass (gpk_esmc.cuh)
+    DevBuf mc_state, mc_buf, mc_stat;
+    int es_nf = 0;
+    long mc_last_jitter = 0;
     // multi-GPU (gpk_comm_*): NCCL communicator bound at run time, one 16-byte pair per rank
     void* comm = nullptr;
     int rank = 0, world = 1;
@@ -1027,6 +1034,17 @@ struct EsLayout {
     }
 };
 
+// layout of h->mc_state (doubles): Mb (nb), Vb (nb x nb), W (np), lmb (nb), scaled zb (nb x d), F (nb x nf)
+struct McLayout {
+    size_t Mb, Vb, W, lmb, zb, F, total;
+    McLayout(int nb, int np_, int d, int nf) {
+        Mb = 0; Vb = Mb + nb; W = Vb + (size_t)nb * nb; lmb = W + np_; zb = lmb + nb; F = zb + (size_t)nb * d;
+        total = F + (size_t)nb * nf;
+    }
+};
+
+enum { ES_KIND_NONE = 0, ES_KIND_EP = 1, ES_KIND_MC = 2 };
+
 // Posterior mean alone of m candidates resident on the device (d_mu: m doubles), asynchronous on the handle's stream.
 // The int8 path's covariance builder with its digit stores compiled out writes each 128-column tile's share of K* alpha,
 // and gpk_mu_parts_finish_kernel sums the shares in tile order: no K* in HBM, no L^-1 slices, no contraction.  Every
@@ -1073,8 +1091,8 @@ int es_reserve(gpk_handle* h) {
 // reads.  Asynchronous on the handle's stream; needs es_reserve and a current gpk_es_update.
 int es_moments_pass(gpk_handle* h, const double* X, long rows) {
     const int nb = h->es_nb, d = h->d;
-    EsLayout L(nb, h->es_np, d);
-    const double* st = ptr<double>(h->es_state);
+    const double* zs = h->es_kind == ES_KIND_MC ? ptr<double>(h->mc_state) + McLayout(nb, h->es_np, d, h->es_nf).zb
+                                                : ptr<double>(h->es_state) + EsLayout(nb, h->es_np, d).zb;
     double* var = ptr<double>(h->es_work);
     double* sig = var + ES_CH;
     const double* lo = h->has_bounds ? ptr<double>(h->lower) : nullptr;
@@ -1084,7 +1102,7 @@ int es_moments_pass(gpk_handle* h, const double* X, long rows) {
     if ((rc = score_dev(h, X, rows, GPK_ACQ_NONE, 0.0, 0.0, nullptr, nullptr, var, nullptr, nullptr))) return rc;
     gpk_es_sigma_kernel<<<(unsigned)rows, GPK_ES_THREADS, 0, h->stream>>>(h->spec, X, rows, d, lo, up,
                                                                           ptr<double>(h->Xrow), h->n,
-                                                                          ptr<double>(h->es_U), st + L.zb, nb,
+                                                                          ptr<double>(h->es_U), zs, nb,
                                                                           out_scale, sig);
     CKL();
     return GPK_OK;
@@ -1113,13 +1131,104 @@ int es_dh_dev(gpk_handle* h, const double* Xm, const double* Xb, long m, double*
     return GPK_OK;
 }
 
-// the checks gpk_es_compute makes before it runs: a current gpk_es_update on an unchanged model
-int es_ready(gpk_handle* h, gpk_handle* report, const char* who) {
+// the checks gpk_es_compute makes before it runs: a current gpk_es_update on an unchanged model.  kind: the update the
+// caller needs (ES_KIND_EP: gpk_es_update, ES_KIND_MC: gpk_esmc_update, ES_KIND_NONE: either).
+int es_ready(gpk_handle* h, gpk_handle* report, const char* who, int kind = ES_KIND_EP) {
     gpk_handle* r = report ? report : h;
-    if (h->es_linv_serial < 0) { set_err(r, "%s: call gpk_es_update first", who); return GPK_BAD_ARG; }
+    const char* upd = kind == ES_KIND_MC ? "gpk_esmc_update" : "gpk_es_update";
+    if (h->es_linv_serial < 0) { set_err(r, "%s: call %s first", who, upd); return GPK_BAD_ARG; }
     if (!h->linv_ready || h->es_linv_serial != h->linv_serial) {
-        set_err(r, "%s: the model changed since gpk_es_update", who);
+        set_err(r, "%s: the model changed since %s", who, upd);
         return GPK_BAD_ARG;
+    }
+    if (kind != ES_KIND_NONE && h->es_kind != kind) {
+        set_err(r, "%s: the current update is %s, not %s", who,
+                h->es_kind == ES_KIND_MC ? "gpk_esmc_update" : "gpk_es_update", upd);
+        return GPK_BAD_ARG;
+    }
+    return GPK_OK;
+}
+
+// The zb half of an entropy-search update, shared by gpk_es_update and gpk_esmc_update: the raw representer points zb
+// (nb x d, host) scaled like the model's inputs into zs (device), and U = L^-T (L^-1 K(X, zb)) in fp64 from the handle's
+// L^-1 into h->es_U.  Asynchronous on the handle's stream.
+int es_build_u(gpk_handle* h, const double* zb, int nb, double* zs) {
+    const int d = h->d, n = h->n, NP = h->NP;
+    const size_t D = (size_t)nb;
+    cudaStream_t s = h->stream;
+    int rc;
+    if ((rc = ensure(h, h->tmp1, D * d * 8))) return rc;
+    CK(cudaMemcpyAsync(h->tmp1.p, zb, D * d * 8, cudaMemcpyHostToDevice, s));
+    const double* lo = h->has_bounds ? ptr<double>(h->lower) : nullptr;
+    const double* up = h->has_bounds ? ptr<double>(h->upper) : nullptr;
+    gpk_es_scale_kernel<<<(unsigned)((D * d + 255) / 256), 256, 0, s>>>(ptr<double>(h->tmp1), nb, d, lo, up, zs);
+    CKL();
+    if (!h->linv_ready && (rc = build_linv(h))) return rc;
+    if ((rc = ensure(h, h->es_U, (size_t)NP * D * 8 * 2))) return rc;
+    double* U = ptr<double>(h->es_U);
+    double* tmp = U + (size_t)NP * D;
+    CK(cudaMemsetAsync(tmp, 0, (size_t)NP * D * 8, s));
+    gpk_es_kxz_kernel<<<(unsigned)(((long)n * nb + 255) / 256), 256, 0, s>>>(h->spec, ptr<double>(h->Xrow), n, d, zs, nb,
+                                                                              tmp);
+    CKL();
+    gpk_es_trmm_kernel<<<(unsigned)(((long)NP * nb + 255) / 256), 256, 0, s>>>(ptr<double>(h->P), NP, tmp, nb, 0, U);
+    CKL();
+    gpk_es_trmm_kernel<<<(unsigned)(((long)NP * nb + 255) / 256), 256, 0, s>>>(ptr<double>(h->P), NP, U, nb, 1, tmp);
+    CKL();
+    CK(cudaMemcpyAsync(U, tmp, (size_t)NP * D * 8, cudaMemcpyDeviceToDevice, s));
+    return GPK_OK;
+}
+
+// gpk_mc_pmin_kernel's ~100 KB of shared memory, with the carveout that lets two CTAs share an SM
+int mc_kernel_attrs(gpk_handle* h) {
+    CK(cudaFuncSetAttribute(gpk_mc_pmin_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GPK_MC_SMEM));
+    CK(cudaFuncSetAttribute(gpk_mc_pmin_kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
+                            cudaSharedmemCarveoutMaxShared));
+    return GPK_OK;
+}
+
+// the 2 status words of gpk_mc_pmin_kernel on h (device), zeroed on h's stream
+int mc_stat_reset(gpk_handle* h) {
+    int rc;
+    if ((rc = ensure(h, h->mc_stat, 2 * sizeof(int)))) return rc;
+    CK(cudaMemsetAsync(h->mc_stat.p, 0, 2 * sizeof(int), h->stream));
+    return GPK_OK;
+}
+
+// Waits for h's stream and reads the status words at d_stat: GPK_NOT_PD (numpy.linalg.LinAlgError, mc_part.py:40-41)
+// when a factorisation failed at every rung of the jitter ladder; the jittered count goes to h->mc_last_jitter.
+int mc_stat_check(gpk_handle* h, const int* d_stat, const char* who) {
+    int st[2] = {0, 0};
+    CK(cudaMemcpyAsync(st, d_stat, sizeof(st), cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    h->mc_last_jitter = st[GPK_MC_STAT_JITTER];
+    if (st[GPK_MC_STAT_NOT_PD] > 0) {
+        set_err(h, "%s: Cholesky decomposition failed. (%d factorisation(s) not positive definite at noise 10000)", who,
+                st[GPK_MC_STAT_NOT_PD]);
+        return GPK_NOT_PD;
+    }
+    return GPK_OK;
+}
+
+// The sampling-based entropy change of m candidates on the device (InformationGainMC.compute): v and sigma by
+// es_moments_pass, then gpk_mc_pmin_kernel, in passes of ES_CH.  The status words go to d_stat (2 ints, device), which
+// the caller zeroes and reads.  Asynchronous on the handle's stream; needs a current gpk_esmc_update.
+int esmc_dev(gpk_handle* h, const double* X, long m, double* d_out, int* d_stat) {
+    const int nb = h->es_nb, d = h->d;
+    McLayout L(nb, h->es_np, d, h->es_nf);
+    const double* st = ptr<double>(h->mc_state);
+    int rc;
+    if ((rc = es_reserve(h))) return rc;
+    const double* var = ptr<double>(h->es_work);
+    const double* sig = var + ES_CH;
+    if ((rc = mc_kernel_attrs(h))) return rc;
+    for (long c0 = 0; c0 < m; c0 += ES_CH) {
+        const long rows = std::min(ES_CH, m - c0);
+        if ((rc = es_moments_pass(h, X + c0 * d, rows))) return rc;
+        gpk_mc_pmin_kernel<<<(unsigned)rows, GPK_MC_THREADS, GPK_MC_SMEM, h->stream>>>(
+            nullptr, st + L.Mb, st + L.W, h->es_np, st + L.Vb, nb, st + L.F, h->es_nf, var, sig, h->es_sn2, st + L.lmb,
+            h->es_H, d_out + c0, nullptr, nullptr, d_stat);
+        CKL();
     }
     return GPK_OK;
 }
@@ -1186,7 +1295,7 @@ int gpk_destroy(gpk_handle* h) {
                       &h->out_var, &h->out_acq, &h->block_best, &h->best, &h->nneg, &h->Vt, &h->cov, &h->XsT,
                       &h->tmpjobs, &h->alpha, &h->tmp1, &h->tmp2, &h->tmp3, &h->chain_cnt, &h->dprof, &h->Xts, &h->oz_Pq, &h->oz_Kq, &h->oz_Kq2, &h->oz_eP, &h->oz_emax, &h->oz_pmu2, &h->oz_probe,
                       &h->multi_cand, &h->multi_A, &h->multi_B, &h->multi_out, &h->multi_bb, &h->gather, &h->best_global,
-                      &h->de_pop, &h->de_trial, &h->de_param, &h->de_E, &h->de_small, &h->de_sort, &h->lb_buf, &h->ep_buf, &h->es_state, &h->es_U, &h->es_work, &h->es_in, &h->fab_in, &h->rs_buf, &h->hy_buf};
+                      &h->de_pop, &h->de_trial, &h->de_param, &h->de_E, &h->de_small, &h->de_sort, &h->lb_buf, &h->ep_buf, &h->es_state, &h->es_U, &h->es_work, &h->es_in, &h->mc_state, &h->mc_buf, &h->mc_stat, &h->fab_in, &h->rs_buf, &h->hy_buf};
     for (DevBuf* b : bufs)
         if (b->p) cudaFree(b->p);
     if (h->ev_ok)
@@ -2715,7 +2824,7 @@ int gpk_es_update(gpk_handle* h, const double* zb, int nb, const double* lmb, do
     if (np_ < 1) BAD("gpk_es_update: Np = %d < 1", np_);
     for (int i = 0; i < nb; ++i)
         if (!std::isfinite(lmb[i])) BAD("lmb should not be infinite.");
-    const int d = h->d, n = h->n, NP = h->NP;
+    const int d = h->d;
     const size_t D = (size_t)nb, T = D * (D + 1) / 2;
     std::vector<double> mu(D), V(D * D), lp(D), dMu(D * D), dSig(D * T), dMuMu(D * D * D);
     if ((rc = gpk_predict_cov(h, zb, nb, mu.data(), V.data()))) return rc;          // predict(zb, full_cov=True)
@@ -2744,31 +2853,14 @@ int gpk_es_update(gpk_handle* h, const double* zb, int nb, const double* lmb, do
     CK(cudaMemcpyAsync(st + L.lo, lower, (size_t)d * 8, cudaMemcpyHostToDevice, s));
     CK(cudaMemcpyAsync(st + L.up, upper, (size_t)d * 8, cudaMemcpyHostToDevice, s));
     // scaled zb, then U = L^-T (L^-1 K(X, zb)) in fp64 from the handle's L^-1
-    if ((rc = ensure(h, h->tmp1, D * d * 8))) return rc;
-    CK(cudaMemcpyAsync(h->tmp1.p, zb, D * d * 8, cudaMemcpyHostToDevice, s));
-    const double* lo = h->has_bounds ? ptr<double>(h->lower) : nullptr;
-    const double* up = h->has_bounds ? ptr<double>(h->upper) : nullptr;
-    gpk_es_scale_kernel<<<(unsigned)((D * d + 255) / 256), 256, 0, s>>>(ptr<double>(h->tmp1), nb, d, lo, up, st + L.zb);
-    CKL();
-    if (!h->linv_ready && (rc = build_linv(h))) return rc;
-    if ((rc = ensure(h, h->es_U, (size_t)NP * D * 8 * 2))) return rc;
-    double* U = ptr<double>(h->es_U);
-    double* tmp = U + (size_t)NP * D;
-    CK(cudaMemsetAsync(tmp, 0, (size_t)NP * D * 8, s));
-    gpk_es_kxz_kernel<<<(unsigned)(((long)n * nb + 255) / 256), 256, 0, s>>>(h->spec, ptr<double>(h->Xrow), n, d, st + L.zb,
-                                                                              nb, tmp);
-    CKL();
-    gpk_es_trmm_kernel<<<(unsigned)(((long)NP * nb + 255) / 256), 256, 0, s>>>(ptr<double>(h->P), NP, tmp, nb, 0, U);
-    CKL();
-    gpk_es_trmm_kernel<<<(unsigned)(((long)NP * nb + 255) / 256), 256, 0, s>>>(ptr<double>(h->P), NP, U, nb, 1, tmp);
-    CKL();
-    CK(cudaMemcpyAsync(U, tmp, (size_t)NP * D * 8, cudaMemcpyDeviceToDevice, s));
+    if ((rc = es_build_u(h, zb, nb, st + L.zb))) return rc;
     CK(cudaStreamSynchronize(s));
     h->es_nb = nb;
     h->es_np = np_;
     h->es_sn2 = sn2;
     h->es_H = H;
     h->es_linv_serial = h->linv_serial;
+    h->es_kind = ES_KIND_EP;
     if (logP) std::copy(lp.begin(), lp.end(), logP);
     if (dlogPdMu) std::copy(dMu.begin(), dMu.end(), dlogPdMu);
     if (dlogPdSigma) std::copy(dSig.begin(), dSig.end(), dlogPdSigma);
@@ -2804,7 +2896,7 @@ int gpk_es_moments(gpk_handle* h, const double* Xs, long m, double* var, double*
     int rc = require(h, true, true, true);
     if (rc) return rc;
     if (!Xs || !var || !sigma || m <= 0) BAD("gpk_es_moments: need candidates, var and sigma");
-    if ((rc = es_ready(h, nullptr, "gpk_es_moments"))) return rc;
+    if ((rc = es_ready(h, nullptr, "gpk_es_moments", ES_KIND_NONE))) return rc;
     CK(cudaSetDevice(h->device));
     const int nb = h->es_nb, d = h->d;
     if ((rc = es_reserve(h))) return rc;
@@ -2827,7 +2919,7 @@ int gpk_es_dims(gpk_handle* h, int* n, int* nb) {
     int rc = require(h, true, true, true);
     if (rc) return rc;
     if (!n || !nb) BAD("gpk_es_dims: null output");
-    if ((rc = es_ready(h, nullptr, "gpk_es_dims"))) return rc;
+    if ((rc = es_ready(h, nullptr, "gpk_es_dims", ES_KIND_NONE))) return rc;
     *n = h->n;
     *nb = h->es_nb;
     return GPK_OK;
@@ -2837,10 +2929,180 @@ int gpk_es_get_u(gpk_handle* h, double* U) {
     int rc = require(h, true, true, true);
     if (rc) return rc;
     if (!U) BAD("gpk_es_get_u: null output");
-    if ((rc = es_ready(h, nullptr, "gpk_es_get_u"))) return rc;
+    if ((rc = es_ready(h, nullptr, "gpk_es_get_u", ES_KIND_NONE))) return rc;
     CK(cudaSetDevice(h->device));
     CK(cudaMemcpyAsync(U, h->es_U.p, (size_t)h->n * h->es_nb * 8, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
+    return GPK_OK;
+}
+
+// ---- sampling-based entropy search (gpk_esmc.cuh) ----------------------------------------------------------------
+int gpk_mc_draws(gpk_handle* h, unsigned long long seed, int nb, int nf, double* F) {
+    if (!h) return GPK_BAD_ARG;
+    if (!F || nb < 1 || nf < 1 || (long)nb * nf > (1L << 28)) BAD("gpk_mc_draws: need F, nb >= 1, nf >= 1");
+    CK(cudaSetDevice(h->device));
+    const size_t bytes = (size_t)nb * nf * 8;
+    int rc;
+    if ((rc = ensure(h, h->mc_buf, bytes))) return rc;
+    const long work = (long)nb * ((nf + 1) / 2);
+    gpk_mc_draws_kernel<<<(unsigned)((work + 255) / 256), 256, 0, h->stream>>>(seed, nb, nf, ptr<double>(h->mc_buf));
+    CKL();
+    CK(cudaMemcpyAsync(F, h->mc_buf.p, bytes, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    return GPK_OK;
+}
+
+// the shape checks of joint_pmin's operands: 1 <= nb <= 64, np >= 1, nf >= 1, nf * np columns counted in an int
+static int mc_check_shape(gpk_handle* h, int nb, int np_, int nf, int nb_min, const char* who) {
+    if (nb < nb_min || nb > GPK_MC_MAX_NB) BAD("%s: Nb = %d outside %d .. %d", who, nb, nb_min, GPK_MC_MAX_NB);
+    if (np_ < 1 || nf < 1) BAD("%s: need Np >= 1 and Nf >= 1 (Np = %d, Nf = %d)", who, np_, nf);
+    if ((long)nf * np_ > 0x7FFFFFFFL) BAD("%s: Nf Np = %ld columns exceed the int counts", who, (long)nf * np_);
+    return GPK_OK;
+}
+
+int gpk_mc_pmin(gpk_handle* h, const double* m, int np_, const double* V, int nb, int nf, unsigned long long seed,
+                double* pmin, int* n_jitter) {
+    if (!h) return GPK_BAD_ARG;
+    int rc;
+    if (!m || !V || !pmin) BAD("gpk_mc_pmin: need m, V and pmin");
+    if ((rc = mc_check_shape(h, nb, np_, nf, 1, "gpk_mc_pmin"))) return rc;
+    CK(cudaSetDevice(h->device));
+    // scratch in doubles: m (nb x np), V (nb x nb), F (nb x nf), pmin (nb), then the status words
+    const size_t om = 0, oV = om + (size_t)nb * np_, oF = oV + (size_t)nb * nb, oP = oF + (size_t)nb * nf, oS = oP + nb;
+    if ((rc = ensure(h, h->mc_buf, oS * 8 + 2 * sizeof(int)))) return rc;
+    double* b = ptr<double>(h->mc_buf);
+    int* dst = (int*)(b + oS);
+    cudaStream_t st = h->stream;
+    CK(cudaMemcpyAsync(b + om, m, (size_t)nb * np_ * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(b + oV, V, (size_t)nb * nb * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaMemsetAsync(dst, 0, 2 * sizeof(int), st));
+    const long work = (long)nb * ((nf + 1) / 2);
+    gpk_mc_draws_kernel<<<(unsigned)((work + 255) / 256), 256, 0, st>>>(seed, nb, nf, b + oF);
+    CKL();
+    if ((rc = mc_kernel_attrs(h))) return rc;
+    gpk_mc_pmin_kernel<<<1, GPK_MC_THREADS, GPK_MC_SMEM, st>>>(b + om, nullptr, nullptr, np_, b + oV, nb, b + oF, nf,
+                                                                 nullptr, nullptr, 0.0, nullptr, 0.0, nullptr, b + oP,
+                                                                 nullptr, dst);
+    CKL();
+    CK(cudaMemcpyAsync(pmin, b + oP, (size_t)nb * 8, cudaMemcpyDeviceToHost, st));
+    if ((rc = mc_stat_check(h, dst, "gpk_mc_pmin"))) return rc;
+    if (n_jitter) *n_jitter = (int)h->mc_last_jitter;
+    return GPK_OK;
+}
+
+int gpk_esmc_update(gpk_handle* h, const double* zb, int nb, const double* lmb, double sn2, const double* W, int np_,
+                    int nf, unsigned long long seed, double* logP, double* pmin) {
+    int rc = require(h, true, true, true);
+    if (rc) return rc;
+    if (!zb || !lmb || !W) BAD("gpk_esmc_update: need zb, lmb and W");
+    if ((rc = mc_check_shape(h, nb, np_, nf, 2, "gpk_esmc_update"))) return rc;
+    for (int i = 0; i < nb; ++i)
+        if (!std::isfinite(lmb[i])) BAD("lmb should not be infinite.");
+    const int d = h->d;
+    const size_t D = (size_t)nb;
+    h->es_linv_serial = -1;                     // no update is current until this one completes
+    std::vector<double> mu(D), V(D * D), pm(D);
+    if ((rc = gpk_predict_cov(h, zb, nb, mu.data(), V.data()))) return rc;          // predict(zb, full_cov=True)
+    McLayout L(nb, np_, d, nf);
+    if ((rc = ensure(h, h->mc_state, L.total * 8))) return rc;
+    double* st = ptr<double>(h->mc_state);
+    cudaStream_t s = h->stream;
+    CK(cudaMemcpyAsync(st + L.Mb, mu.data(), D * 8, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(st + L.Vb, V.data(), D * D * 8, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(st + L.W, W, (size_t)np_ * 8, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(st + L.lmb, lmb, D * 8, cudaMemcpyHostToDevice, s));
+    const long work = (long)nb * ((nf + 1) / 2);
+    gpk_mc_draws_kernel<<<(unsigned)((work + 255) / 256), 256, 0, s>>>(seed, nb, nf, st + L.F);
+    CKL();
+    // pmin = joint_pmin(Mb, Vb, Nf) with Mb as (Nb, 1): one column of innovations
+    if ((rc = ensure(h, h->mc_buf, D * 8))) return rc;
+    if ((rc = mc_stat_reset(h))) return rc;
+    if ((rc = mc_kernel_attrs(h))) return rc;
+    gpk_mc_pmin_kernel<<<1, GPK_MC_THREADS, GPK_MC_SMEM, s>>>(st + L.Mb, nullptr, nullptr, 1, st + L.Vb, nb, st + L.F, nf,
+                                                                nullptr, nullptr, 0.0, nullptr, 0.0, nullptr,
+                                                                ptr<double>(h->mc_buf), nullptr, ptr<int>(h->mc_stat));
+    CKL();
+    CK(cudaMemcpyAsync(pm.data(), h->mc_buf.p, D * 8, cudaMemcpyDeviceToHost, s));
+    if ((rc = mc_stat_check(h, ptr<int>(h->mc_stat), "gpk_esmc_update"))) return rc;
+    // logP = log(pmin); H of the loss (information_gain.py:82), summed in index order
+    std::vector<double> lp(D);
+    double H = 0.0;
+    for (size_t i = 0; i < D; ++i) {
+        lp[i] = std::log(pm[i]);
+        H += std::exp(lp[i]) * (lp[i] + lmb[i]);
+    }
+    H = -H;
+    if ((rc = es_build_u(h, zb, nb, st + L.zb))) return rc;
+    CK(cudaStreamSynchronize(s));
+    h->es_nb = nb;
+    h->es_np = np_;
+    h->es_nf = nf;
+    h->es_sn2 = sn2;
+    h->es_H = H;
+    h->es_linv_serial = h->linv_serial;
+    h->es_kind = ES_KIND_MC;
+    if (logP) std::copy(lp.begin(), lp.end(), logP);
+    if (pmin) std::copy(pm.begin(), pm.end(), pmin);
+    return GPK_OK;
+}
+
+int gpk_esmc_compute_dev(gpk_handle* h, const void* d_Xs, long m, void* d_out) {
+    int rc = require(h, true, true, true);
+    if (rc) return rc;
+    if (!d_Xs || !d_out || m <= 0) BAD("gpk_esmc_compute_dev: need candidates and out");
+    if ((rc = es_ready(h, nullptr, "gpk_esmc_compute", ES_KIND_MC))) return rc;
+    CK(cudaSetDevice(h->device));
+    if ((rc = mc_stat_reset(h))) return rc;
+    return esmc_dev(h, (const double*)d_Xs, m, (double*)d_out, ptr<int>(h->mc_stat));
+}
+
+int gpk_esmc_compute(gpk_handle* h, const double* Xs, long m, double* out) {
+    int rc = require(h, true, true, true);
+    if (rc) return rc;
+    if (!Xs || !out || m <= 0) BAD("gpk_esmc_compute: need candidates and out");
+    CK(cudaSetDevice(h->device));
+    if ((rc = es_ready(h, nullptr, "gpk_esmc_compute", ES_KIND_MC))) return rc;
+    if ((rc = ensure(h, h->es_in, (size_t)m * (h->d + 1) * 8))) return rc;
+    double* dX = ptr<double>(h->es_in);
+    double* dout = dX + (size_t)m * h->d;
+    CK(cudaMemcpyAsync(dX, Xs, (size_t)m * h->d * 8, cudaMemcpyHostToDevice, h->stream));
+    if ((rc = gpk_esmc_compute_dev(h, dX, m, dout))) return rc;
+    CK(cudaMemcpyAsync(out, dout, (size_t)m * 8, cudaMemcpyDeviceToHost, h->stream));
+    return mc_stat_check(h, ptr<int>(h->mc_stat), "gpk_esmc_compute");
+}
+
+int gpk_esmc_get_draws(gpk_handle* h, double* F) {
+    int rc = require(h, true, true, true);
+    if (rc) return rc;
+    if (!F) BAD("gpk_esmc_get_draws: null output");
+    if ((rc = es_ready(h, nullptr, "gpk_esmc_get_draws", ES_KIND_MC))) return rc;
+    CK(cudaSetDevice(h->device));
+    const McLayout L(h->es_nb, h->es_np, h->d, h->es_nf);
+    CK(cudaMemcpyAsync(F, ptr<double>(h->mc_state) + L.F, (size_t)h->es_nb * h->es_nf * 8, cudaMemcpyDeviceToHost,
+                       h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    return GPK_OK;
+}
+
+int gpk_esmc_get_state(gpk_handle* h, double* Mb, double* Vb) {
+    int rc = require(h, true, true, true);
+    if (rc) return rc;
+    if (!Mb || !Vb) BAD("gpk_esmc_get_state: null output");
+    if ((rc = es_ready(h, nullptr, "gpk_esmc_get_state", ES_KIND_MC))) return rc;
+    CK(cudaSetDevice(h->device));
+    const int nb = h->es_nb;
+    const McLayout L(nb, h->es_np, h->d, h->es_nf);
+    const double* st = ptr<double>(h->mc_state);
+    CK(cudaMemcpyAsync(Mb, st + L.Mb, (size_t)nb * 8, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaMemcpyAsync(Vb, st + L.Vb, (size_t)nb * nb * 8, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    return GPK_OK;
+}
+
+int gpk_esmc_last_jitter(gpk_handle* h, long* n_jitter) {
+    if (!h) return GPK_BAD_ARG;
+    if (!n_jitter) BAD("gpk_esmc_last_jitter: null output");
+    *n_jitter = h->mc_last_jitter;
     return GPK_OK;
 }
 

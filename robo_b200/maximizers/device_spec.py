@@ -16,16 +16,23 @@ def raw_inputs(model):
 def device_spec(acq, who):
     """What scores the acquisition ``acq`` on the device:
         ("es_cost", device_spec's tuple)   InformationGainPerUnitCost, alone or marginalised (gpk_es_cost_multi)
+        ("esmc", handles)                  InformationGainMC, alone or marginalised (gpk_esmc_compute / gpk_esmc_multi)
         ("es", handles)                    InformationGain, alone or marginalised (gpk_es_compute / gpk_es_multi)
         ("acq", (kind, etas, par, handles)) EI / LogEI / PI / LCB (gpk_acq_multi)
     TypeError, naming the maximizer ``who``, when the acquisition does not run on device models."""
     from robo_b200.acquisition_functions.information_gain import InformationGain
+    from robo_b200.acquisition_functions.information_gain_mc import InformationGainMC
     from robo_b200.acquisition_functions.information_gain_per_unit_cost import (InformationGainPerUnitCost,
                                                                                 device_spec as es_cost_spec)
     estimators = acq.estimators if hasattr(acq, "_fused_spec") else [acq]
     # InformationGainPerUnitCost is an InformationGain: it is recognised first
     if estimators and all(isinstance(e, InformationGainPerUnitCost) for e in estimators):
         return "es_cost", es_cost_spec(estimators)
+    # so is InformationGainMC: recognised before InformationGain, whose EP path it must not take
+    if estimators and all(isinstance(e, InformationGainMC) for e in estimators):
+        if not all(raw_inputs(e.model) for e in estimators):
+            raise TypeError("%s needs InformationGainMC on robo_b200 GaussianProcess models" % who)
+        return "esmc", [e._ready_handle() for e in estimators]
     if estimators and all(isinstance(e, InformationGain) for e in estimators):
         if not all(raw_inputs(e.model) for e in estimators):
             raise TypeError("%s needs InformationGain on robo_b200 GaussianProcess models" % who)
@@ -53,9 +60,21 @@ def acq_spec(acq, who):
     return kind, [eta], float(acq.par), [model.gp.handle]
 
 
-def _run(which, spec, es_cost, es, acq):
+def is_sampling_based(acq):
+    """The acquisition is InformationGainMC, alone or marginalised: its surface is piecewise constant in x."""
+    from robo_b200.acquisition_functions.information_gain_mc import InformationGainMC
+    estimators = acq.estimators if hasattr(acq, "_fused_spec") else [acq]
+    return len(estimators) > 0 and all(isinstance(e, InformationGainMC) for e in estimators)
+
+
+def _run(which, spec, es_cost, es, acq, esmc=None):
     """Calls the maximizer of ``which`` over ``spec`` (what ``device_spec`` returned): es_cost(ho, hc, **configuration),
-    es(handles) or acq(handles, kind code, etas, par).  ValueError as ei.py:86-88 when EI came out negative."""
+    es(handles), esmc(handles) or acq(handles, kind code, etas, par).  ValueError as ei.py:86-88 when EI came out
+    negative; TypeError when the maximizer has no ``esmc``."""
+    if which == "esmc":
+        if esmc is None:
+            raise TypeError("the sampling-based information gain has no device path for this maximizer")
+        return esmc(spec)
     if which == "es_cost":
         ho, hc, lo, up, bo, bc, oh = spec
         return es_cost(ho, hc, cfg_lower=lo, cfg_upper=up, basis_objective=bo, basis_cost=bc, overhead=oh)
@@ -75,7 +94,8 @@ def maximize_de(which, spec, seed, pop, maxiter, mutation, recombination, tol, a
     return _run(which, spec,
                 lambda ho, hc, **cfg: _lib.maximize_de_es_cost(ho, hc, *args, **cfg),
                 lambda hs: _lib.maximize_de_es(hs, *args),
-                lambda hs, kind, etas, par: _lib.maximize_de(hs, *args, kind=kind, eta=etas, par=par))
+                lambda hs, kind, etas, par: _lib.maximize_de(hs, *args, kind=kind, eta=etas, par=par),
+                lambda hs: _lib.maximize_de_esmc(hs, *args))
 
 
 def maximize_lbfgs(which, spec, x0, lower, upper):

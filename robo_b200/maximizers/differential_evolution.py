@@ -13,14 +13,16 @@ cannot be reproduced by anyone; here the seed is drawn from ``rng`` at construct
 DeviceRandomSampling.
 
 The acquisition may be EI / LogEI / PI / LCB (gpk_maximize_de), InformationGain (gpk_maximize_de_es: the entropy
-change, marginalised by gpk_es_multi over a GP-MCMC ensemble) or InformationGainPerUnitCost, Fabolas's acquisition
+change, marginalised by gpk_es_multi over a GP-MCMC ensemble), InformationGainMC (gpk_maximize_de_esmc: the
+sampling-based entropy change on the update's common draws) or InformationGainPerUnitCost, Fabolas's acquisition
 (gpk_maximize_de_es_cost over the extended box), each alone or under MarginalizationGPMCMC.
 
 With ``polish=True`` (scipy's default, which the reference uses) L-BFGS-B refines the device winner on the host
 through the reference's single-point objective, and scipy's acceptance rule applies: lower energy, success, inside
 the bounds.  With ``polish="device"`` the same refinement runs as one start of the device's multi-start L-BFGS
 (gpk_maximize_lbfgs*, the engine of SciPyOptimizer) over the same scoring path as the evolution, under the same
-acceptance rule.
+acceptance rule.  InformationGainMC refuses ``polish="device"`` with ValueError: its surface is piecewise constant
+in x, so forward differences have nothing to follow; ``polish=True`` runs the reference's host polish over it.
 """
 import sys
 
@@ -59,6 +61,9 @@ class DifferentialEvolution(BaseMaximizer):
 
     def maximize(self):
         which, spec = self._device_spec()
+        if which == "esmc" and self.polish == "device":
+            raise ValueError("DifferentialEvolution: polish='device' does not apply to InformationGainMC, whose "
+                             "surface is piecewise constant in x; use polish=True or polish=False")
         lower, upper = np.asarray(self.lower, dtype=np.float64), np.asarray(self.upper, dtype=np.float64)
         seed = (self.seed + 0x9E3779B97F4A7C15 * self.calls) & 0xFFFFFFFFFFFFFFFF
         self.calls += 1

@@ -11,7 +11,9 @@ forward differences, not L-BFGS-B's Cauchy point and subspace minimisation (incl
 
 Starts follow the reference's recipe, drawn from ``self.rng`` instead of numpy's global stream: int(0.5 n) uniform in
 the box, then int(0.5 n) normal around the incumbent with scale 0.5.  An acquisition that does not run on device
-models takes the reference's host loop unchanged, so the class is a drop-in for the reference's.
+models takes the reference's host loop unchanged, so the class is a drop-in for the reference's.  So does
+InformationGainMC, alone or marginalised: its Monte-Carlo surface is piecewise constant in x, so forward-difference
+L-BFGS has nothing to follow on the device either (as in the reference), and each start scores one row per call.
 """
 import sys
 from functools import partial
@@ -21,7 +23,7 @@ from scipy import optimize
 
 from robo_b200.initial_design import init_random_uniform
 from robo_b200.maximizers.base_maximizer import BaseMaximizer
-from robo_b200.maximizers.device_spec import device_spec, maximize_lbfgs
+from robo_b200.maximizers.device_spec import device_spec, is_sampling_based, maximize_lbfgs
 
 
 class SciPyOptimizer(BaseMaximizer):
@@ -55,6 +57,8 @@ class SciPyOptimizer(BaseMaximizer):
         starts = self._starts()
         if len(starts) == 0:
             raise ValueError("SciPyOptimizer needs n_restarts >= 2 (int(0.5 n_restarts) starts of each kind)")
+        if is_sampling_based(self.objective_func):
+            return self._maximize_host(starts)
         try:
             which, spec = device_spec(self.objective_func, "SciPyOptimizer")
         except TypeError:
