@@ -84,9 +84,6 @@ const char* gpk_version(void);
  *               broadcast load per pair and term from an axis-major operand under 0
  *   "chunk"     candidates per scoring pass (multiple of 128); 0 = automatic [default]: the K* buffer is kept near
  *               512 MB (16384 candidates at N = 4096, 65536 at N <= 1024)
- *   "graph"     1 = the split-chain schedule of a factorisation (~600 launches / event records / stream waits at
- *               N = 4096) is captured once per layout into a CUDA graph and replayed per fit [default]; 0 = enqueue
- *               every call directly
  *   "ozaki"     1 = variance contraction on the int8 tensor pipe (wgmma s8, register accumulators) through an
  *               error-free split of L^-1 and K* into 7 balanced base-256 digits each, 28 digit-pair products
  *               (gpk_ozaki.cuh); used while max |L^-1| < 64 and N <= 16384, otherwise the fp64 kernel runs [default;
@@ -104,12 +101,7 @@ const char* gpk_version(void);
  *   "depth2"    1 = trailing updates of two consecutive panels in one K = 256 contraction (odd steps; even steps update
  *               only the next-but-one block column); 0 = one K = 128 update per step (bit-identical factor);
  *               2 = automatic [default]: on for N >= 6144, where the trailing updates gate the fit
- *   "chainsplit" 1 = split Cholesky chain: diag(k+1) waits only for block row k+1 of step k (one launch on
- *               four 32-row tiles), the rows below run on a second high-priority stream, trailing update with
- *               look-ahead 2;
- *               0 = plain look-ahead schedule [default] (bit-identical factor)
  *   "diagprof"  1 = the diagonal-block kernel records clock64() stamps per phase (gpk_get_diag_profile)
- *   "pdl"       1 = programmatic dependent launch for the kernels of the Cholesky chain [default]
  *   "overlap"   1 = build K* of chunk i+1 on the side stream while chunk i contracts [default]
  *   "meanonly"  1 = gpk_predict_mean (and the cost models of gpk_es_cost_multi) run the mean-only builder pass [default];
  *               0 = they take the mean of the full scoring pass, variance contraction included (tools/fabolas_acq_bench.py

@@ -200,11 +200,10 @@ class Handle(object):
             self.set_option("loader", int(os.environ["GPK_LOADER"]))
         if os.environ.get("GPK_CHUNK"):
             self.set_option("chunk", int(os.environ["GPK_CHUNK"]))
-        # schedule and contraction switches: GPK_CHAINSPLIT=0|1, GPK_OZAKI=0|1 (fp64 | int8 variance contraction),
-        # GPK_GRAPH, GPK_DEPTH2, GPK_OZPERSIST, GPK_OZCLUSTER, GPK_OZGRID (see gpk_set_option in include/gpk.h)
-        for env, key in (("GPK_CHAINSPLIT", "chainsplit"), ("GPK_OZAKI", "ozaki"), ("GPK_GRAPH", "graph"),
-                         ("GPK_DEPTH2", "depth2"), ("GPK_OZPERSIST", "ozpersist"), ("GPK_OZCLUSTER", "ozcluster"),
-                         ("GPK_OZGRID", "ozgrid")):
+        # schedule and contraction switches: GPK_OZAKI=0|1 (fp64 | int8 variance contraction), GPK_DEPTH2,
+        # GPK_OZPERSIST, GPK_OZCLUSTER, GPK_OZGRID (see gpk_set_option in include/gpk.h)
+        for env, key in (("GPK_OZAKI", "ozaki"), ("GPK_DEPTH2", "depth2"), ("GPK_OZPERSIST", "ozpersist"),
+                         ("GPK_OZCLUSTER", "ozcluster"), ("GPK_OZGRID", "ozgrid")):
             if os.environ.get(env):
                 self.set_option(key, int(os.environ[env]))
 

@@ -23,7 +23,6 @@
 #include "gpk_gemm.cuh"
 #include "gpk_kernels.cuh"
 #include "gpk_diag16.cuh"
-#include "gpk_chain.cuh"
 #include "gpk_ozaki.cuh"
 #include "gpk_de.cuh"
 #include "gpk_lbfgs.cuh"
@@ -51,8 +50,6 @@ struct gpk_handle {
     cudaStream_t own_stream = nullptr;
     cudaStream_t side_stream = nullptr;     // trailing updates of the look-ahead Cholesky
     std::vector<cudaEvent_t> ev_panel, ev_rest;
-    cudaStream_t panel_stream = nullptr;    // split chain: panel solve / next-panel update of the rows below block row k+1
-    std::vector<cudaEvent_t> ev_cs;         // split chain: 5 events per step (diag, X, trsm', pu', rest_a)
     // variance contraction on the int8 tensor pipe (gpk_ozaki.cuh); 0 = fp64 DMMA kernels
     int ozaki = 1;
     DevBuf oz_Pq, oz_Kq, oz_Kq2, oz_eP, oz_emax, oz_pmu2;
@@ -74,12 +71,6 @@ struct gpk_handle {
     CUtensorMap mapOzP, mapOzK, mapOzK2;
     double oz_launches = 0;
     int n_sm = 0;
-    int use_graph = 1;              // split chain: one CUDA graph per layout, replayed per fit
-    cudaGraphExec_t fit_graph = nullptr;
-    double fit_graph_launches = 0;
-    int chainsplit = 0;             // 1: diag(k+1) waits only for block row k+1 of step k (gpk_chain_step_kernel on 4 CTAs)
-    int pdl = 1;                    // programmatic dependent launch on the Cholesky chain
-    DevBuf chain_cnt;
     char err[1024] = {0};
     int loader = LOADER_TMA_WS;
     long chunk = 16384;
@@ -435,7 +426,7 @@ int launch_gemm(gpk_handle* h, const CUtensorMap& mA, const CUtensorMap& mB, con
                 cudaStream_t stream = nullptr, bool pdl = false) {
     if (njobs <= 0) return GPK_OK;
     if (stream == nullptr) stream = h->stream;
-    if (pdl && h->pdl && h->loader != LOADER_CPASYNC && MI == 2) {
+    if (pdl && h->loader != LOADER_CPASYNC && MI == 2) {
         CK(launch_pdl(gpk_gemm_nt_kernel<EPI, LOADER_TMA, MI>, dim3(njobs), dim3(GEMM_THREADS),
                       (size_t)gemm_smem_bytes(LOADER_TMA, MI), stream, mA, mB, a));
         h->launches_total += 1;
@@ -471,7 +462,6 @@ int set_kernel_attrs(gpk_handle* h) {
     }
     CK(cudaFuncSetAttribute(gpk_cov_tma_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cov_tma_smem_bytes(GPK_MAX_TERMS, 8)));
     CK(cudaFuncSetAttribute(gpk_cov_tma_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cov_tma_smem_bytes(GPK_MAX_TERMS, 4)));
-    CK(cudaFuncSetAttribute(gpk_chain_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, CH_SMEM));
     CK(cudaFuncSetAttribute(gpk_potrf_diag_dmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DIAG_SMEM));
     return GPK_OK;
 }
@@ -1242,10 +1232,6 @@ extern "C" {
 
 int gpk_comm_destroy(gpk_handle* h);
 
-static void drop_fit_graph(gpk_handle* h) {
-    if (h->fit_graph) { cudaGraphExecDestroy(h->fit_graph); h->fit_graph = nullptr; }
-}
-
 const char* gpk_version(void) { return "gpk 0.2 (sm_90a, fp64 DMMA + TMA)"; }
 
 const char* gpk_last_error(gpk_handle* h) { return h ? h->err : "null handle"; }
@@ -1265,7 +1251,6 @@ int gpk_create(gpk_handle** out, int device) {
         if (cudaStreamCreateWithPriority(&h->own_stream, cudaStreamNonBlocking, hi) != cudaSuccess) { delete h; return GPK_CUDA_ERROR; }
         if (cudaStreamCreateWithPriority(&h->side_stream, cudaStreamNonBlocking, lo) != cudaSuccess) { delete h; return GPK_CUDA_ERROR; }
         if (cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking) != cudaSuccess) { delete h; return GPK_CUDA_ERROR; }
-        if (cudaStreamCreateWithPriority(&h->panel_stream, cudaStreamNonBlocking, hi) != cudaSuccess) { delete h; return GPK_CUDA_ERROR; }
     }
     h->stream = h->own_stream;
     for (int i = 0; i < 16; ++i)
@@ -1287,13 +1272,12 @@ int gpk_destroy(gpk_handle* h) {
     if (!h) return GPK_OK;
     cudaSetDevice(h->device);
     cudaStreamSynchronize(h->stream);
-    drop_fit_graph(h);
     gpk_comm_destroy(h);
     if (h->ev_multi) cudaEventDestroy(h->ev_multi);
     DevBuf* bufs[] = {&h->Xrow, &h->Xt, &h->y, &h->Kbuf, &h->P, &h->Q, &h->W, &h->lower, &h->upper, &h->logdet_part,
                       &h->scal, &h->status, &h->jobs, &h->cand, &h->Kstar, &h->Kstar2, &h->cand2, &h->part_mu, &h->part_ssq, &h->out_mu,
                       &h->out_var, &h->out_acq, &h->block_best, &h->best, &h->nneg, &h->Vt, &h->cov, &h->XsT,
-                      &h->tmpjobs, &h->alpha, &h->tmp1, &h->tmp2, &h->tmp3, &h->chain_cnt, &h->dprof, &h->Xts, &h->oz_Pq, &h->oz_Kq, &h->oz_Kq2, &h->oz_eP, &h->oz_emax, &h->oz_pmu2, &h->oz_probe,
+                      &h->tmpjobs, &h->alpha, &h->tmp1, &h->tmp2, &h->tmp3, &h->dprof, &h->Xts, &h->oz_Pq, &h->oz_Kq, &h->oz_Kq2, &h->oz_eP, &h->oz_emax, &h->oz_pmu2, &h->oz_probe,
                       &h->multi_cand, &h->multi_A, &h->multi_B, &h->multi_out, &h->multi_bb, &h->gather, &h->best_global,
                       &h->de_pop, &h->de_trial, &h->de_param, &h->de_E, &h->de_small, &h->de_sort, &h->lb_buf, &h->ep_buf, &h->es_state, &h->es_U, &h->es_work, &h->es_in, &h->mc_state, &h->mc_buf, &h->mc_stat, &h->fab_in, &h->rs_buf, &h->hy_buf};
     for (DevBuf* b : bufs)
@@ -1303,8 +1287,6 @@ int gpk_destroy(gpk_handle* h) {
     if (h->ev_order) cudaEventDestroy(h->ev_order);
     for (int i = 0; i < 2; ++i)
         if (h->stage[i]) cudaFreeHost(h->stage[i]);
-    for (cudaEvent_t e : h->ev_cs) cudaEventDestroy(e);
-    if (h->panel_stream) cudaStreamDestroy(h->panel_stream);
     for (cudaEvent_t e : h->ev_panel) cudaEventDestroy(e);
     for (cudaEvent_t e : h->ev_rest) cudaEventDestroy(e);
     for (cudaEvent_t e : h->ev_cov) cudaEventDestroy(e);
@@ -1323,12 +1305,6 @@ int gpk_destroy(gpk_handle* h) {
 
 int gpk_set_option(gpk_handle* h, const char* key, long value) {
     if (!h || !key) return GPK_BAD_ARG;
-    drop_fit_graph(h);                       // every switch may change what a factorisation launches
-    if (!strcmp(key, "graph")) {
-        if (value != 0 && value != 1) BAD("graph must be 0 or 1");
-        h->use_graph = (int)value;
-        return GPK_OK;
-    }
     if (!strcmp(key, "loader")) {
         if (value < LOADER_CPASYNC || value > LOADER_TMA_WS) BAD("loader must be 0 (cp.async), 1 (TMA) or 2 (TMA, warp-specialised)");
         if (value != LOADER_CPASYNC && get_encode_fn() == nullptr) BAD("TMA descriptors unavailable on this driver");
@@ -1361,16 +1337,6 @@ int gpk_set_option(gpk_handle* h, const char* key, long value) {
     if (!strcmp(key, "depth2")) {
         if (value < 0 || value > 2) BAD("depth2 must be 0, 1 or 2 (automatic)");
         h->depth2 = (int)value;
-        return GPK_OK;
-    }
-    if (!strcmp(key, "chainsplit")) {
-        if (value != 0 && value != 1) BAD("chainsplit must be 0 or 1");
-        h->chainsplit = (int)value;
-        return GPK_OK;
-    }
-    if (!strcmp(key, "pdl")) {
-        if (value != 0 && value != 1) BAD("pdl must be 0 or 1");
-        h->pdl = (int)value;
         return GPK_OK;
     }
     if (!strcmp(key, "meanonly")) {
@@ -1438,7 +1404,6 @@ int gpk_set_data(gpk_handle* h, const double* X, const double* y, int n, int d) 
     if ((rc = ensure(h, h->logdet_part, (size_t)(NP / BM) * 8))) return rc;
     const bool relayout = (h->layout_NP != NP) || g1 || g2 || g3 || g4;
     h->n = n; h->d = d; h->NP = (int)NP; h->nb = (int)(NP / BM);
-    if (relayout || h->jobs_nb != (int)(NP / BM)) drop_fit_graph(h);       // the graph holds buffer / job-table addresses
     if (relayout) {
         CK(cudaMemsetAsync(h->Kbuf.p, 0, (size_t)(NP + BM) * NP * 8, h->stream));
         CK(cudaMemsetAsync(h->P.p, 0, (size_t)NP * NP * 8, h->stream));
@@ -1559,158 +1524,13 @@ int gpk_fit_begin(gpk_handle* h, double diag_add, double mean) {
         h->ev_rest.push_back(e2);
     }
     std::vector<char> rest_recorded(nb, 0);
-    // ---- split chain (option "chainsplit" = 1): only block row k+1 of step k stays between diag(k) and diag(k+1) ---
-    // Step k of the plain look-ahead schedule (below) puts diag(k) -> panel solve (all rows) -> update of block column
-    // k+1 (all rows) on the critical chain.  diag(k+1) only needs A[k+1,k+1] -= L[k+1,k] L[k+1,k]^T with
-    // L[k+1,k] = A[k+1,k] inv(L_kk)^T: one launch of gpk_chain_step_kernel on the four 32-row tiles of block row k+1
-    // ("X(k)").  The rows below go to a second high-priority stream and overlap diag(k+1); the trailing update is cut
-    // in two (block column k+2 first) so that the chain waits for one column, not for the whole update (look-ahead 2).
-    // Every tile still receives its panels in increasing order: the factor is bit-identical to the plain schedule.
-    //   C (h->stream)     diag(k) . X(k) . diag(k+1) ...
-    //   P (panel_stream)  solve'(k) [rows > k+1] . update'(k) [block column k+1, rows > k+1]
-    //   R (side_stream)   rest_a(k) [block column k+2] . rest_b(k) [block columns >= k+3]
-    const bool split = h->chainsplit && h->loader != LOADER_CPASYNC && nb >= 3;
-    if (split) {
-        if ((rc = ensure(h, h->chain_cnt, (size_t)nb * 4))) return rc;
-        while ((int)h->ev_cs.size() < 5 * nb + 3) {
-            cudaEvent_t e;
-            CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-            h->ev_cs.push_back(e);
-        }
-        auto evD = [&](int k) { return h->ev_cs[5 * k]; };
-        auto evX = [&](int k) { return h->ev_cs[5 * k + 1]; };
-        auto evT = [&](int k) { return h->ev_cs[5 * k + 2]; };
-        auto evPU = [&](int k) { return h->ev_cs[5 * k + 3]; };
-        auto evRA = [&](int k) { return h->ev_cs[5 * k + 4]; };
-        cudaStream_t C = h->stream, Pst = h->panel_stream, R = h->side_stream;
-        cudaEvent_t evFork = h->ev_cs[5 * nb], evJoinP = h->ev_cs[5 * nb + 1], evJoinR = h->ev_cs[5 * nb + 2];
-        // the whole schedule of one factorisation (about 6 launches, 5 event records and 7 stream waits per step);
-        // depends on the buffers and job tables only, so it is captured ONCE into a CUDA graph and replayed per fit
-        auto enqueue = [&]() -> int {
-        std::vector<char> haveX(nb, 0), havePU(nb, 0), haveRA(nb, 0);
-        CK(cudaMemsetAsync(h->chain_cnt.p, 0, (size_t)nb * 4, C));
-        CK(cudaEventRecord(evFork, C));                            // K is built: the other streams may start
-        CK(cudaStreamWaitEvent(Pst, evFork, 0));
-        CK(cudaStreamWaitEvent(R, evFork, 0));
-        gpk_diag_prezero_kernel<<<nb, 256, 0, C>>>(K, (long)NP, ptr<double>(h->P), (long)NP);
-        CKL();
-        for (int k = 0; k < nb; ++k) {
-            long long* dprof = h->diag_prof ? ptr<long long>(h->dprof) : nullptr;
-            // ---- C: diag(k)
-            gpk_potrf_diag_dmma_kernel<<<1, 256, DIAG_SMEM, C>>>(K, NP, k, ptr<double>(h->P), ptr<double>(h->Q), NP,
-                                                                 ptr<int>(h->status), ptr<double>(h->logdet_part), dprof);
-            CKL();
-            CK(cudaEventRecord(evD(k), C));
-            const int nsolve = h->trsm32_r[k].cnt, nupd = h->pu32_r[k].cnt;
-            const bool hasX = (k + 1 < nb);                              // block row k+1 exists: 4 solve + 4 update tiles
-            // ---- C: X(k)
-            if (hasX) {
-                if (k >= 1 && havePU[k - 1]) CK(cudaStreamWaitEvent(C, evPU(k - 1), 0));     // A[k+1,k] carries panel k-1
-                if (k >= 1 && haveRA[k - 1]) CK(cudaStreamWaitEvent(C, evRA(k - 1), 0));     // A[k+1,k+1] carries panel k-1
-                ChainArgs c;
-                c.K = K; c.ld = NP; c.P = ptr<double>(h->P); c.ldp = NP;
-                c.solve_jobs = ptr<GemmJob>(h->jobs) + h->trsm32_r[k].off;
-                c.update_jobs = ptr<GemmJob>(h->jobs) + h->pu32_r[k].off;
-                c.counter = ptr<int>(h->chain_cnt) + k;
-                c.status = ptr<int>(h->status);
-                gpk_chain_step_kernel<<<4, GEMM_THREADS, CH_SMEM, C>>>(c);
-                CKL();
-                CK(cudaEventRecord(evX(k), C));
-                haveX[k] = 1;
-            }
-            // ---- P: the rest of the panel (rows below block row k+1, and the right-hand-side row)
-            const int skip = hasX ? 4 : 0;
-            GemmArgs a;
-            memset(&a, 0, sizeof(a));
-            a.A = K; a.lda = NP; a.B = ptr<double>(h->P); a.ldb = NP; a.C = K; a.ldc = NP;
-            a.alpha = 1.0; a.beta = 0; a.job_mode = JOBS_TABLE; a.status = ptr<int>(h->status);
-            a.jobs = ptr<GemmJob>(h->jobs) + h->trsm32_r[k].off + skip;
-            CK(cudaStreamWaitEvent(Pst, evD(k), 0));
-            if (nsolve - skip > 0) {
-                if ((rc = launch_gemm<EPI_STORE, 2>(h, h->mapK32, h->mapP, a, nsolve - skip, Pst))) return rc;
-            }
-            CK(cudaEventRecord(evT(k), Pst));
-            if (hasX && nupd - 4 > 0) {
-                GemmArgs u;
-                memset(&u, 0, sizeof(u));
-                u.A = K; u.lda = NP; u.B = K; u.ldb = NP; u.C = K; u.ldc = NP;
-                u.alpha = -1.0; u.beta = 1; u.job_mode = JOBS_TABLE; u.status = ptr<int>(h->status);
-                u.jobs = ptr<GemmJob>(h->jobs) + h->pu32_r[k].off + 4;
-                CK(cudaStreamWaitEvent(Pst, evX(k), 0));                                       // L[k+1,k] is the B operand
-                if (k >= 1 && haveRA[k - 1]) CK(cudaStreamWaitEvent(Pst, evRA(k - 1), 0));    // column k+1 carries panel k-1
-                if ((rc = launch_gemm<EPI_STORE, 2>(h, h->mapK32, h->mapK, u, nupd - 4, Pst))) return rc;
-                CK(cudaEventRecord(evPU(k), Pst));
-                havePU[k] = 1;
-            }
-            // ---- R: trailing update beyond block column k+1: column k+2 first (what step k+1 waits for), then the rest
-            const int off = h->syrk_r[k].off, cnt = h->syrk_r[k].cnt, npu = nb - k;       // first npu jobs: block column k+1
-            if (cnt > npu) {
-                const int na = nb - k - 1;                                                // block column k+2: rows k+2 .. nb
-                GemmArgs s2;
-                memset(&s2, 0, sizeof(s2));
-                s2.A = K; s2.lda = NP; s2.B = K; s2.ldb = NP; s2.C = K; s2.ldc = NP;
-                s2.alpha = -1.0; s2.beta = 1; s2.job_mode = JOBS_TABLE; s2.status = ptr<int>(h->status);
-                CK(cudaStreamWaitEvent(R, evT(k), 0));
-                if (hasX) CK(cudaStreamWaitEvent(R, evX(k), 0));
-                s2.jobs = ptr<GemmJob>(h->jobs) + off + npu;
-                if ((rc = launch_gemm<EPI_STORE>(h, h->mapK, h->mapK, s2, std::min(na, cnt - npu), R))) return rc;
-                CK(cudaEventRecord(evRA(k), R));
-                haveRA[k] = 1;
-                if (cnt - npu - na > 0) {
-                    s2.jobs = ptr<GemmJob>(h->jobs) + off + npu + na;
-                    if ((rc = launch_gemm<EPI_STORE>(h, h->mapK, h->mapK, s2, cnt - npu - na, R))) return rc;
-                }
-            }
-        }
-        // join: everything the factor consists of is complete once P and R have drained
-        CK(cudaEventRecord(evJoinP, Pst));
-        CK(cudaStreamWaitEvent(C, evJoinP, 0));
-        CK(cudaEventRecord(evJoinR, R));
-        CK(cudaStreamWaitEvent(C, evJoinR, 0));
-        gpk_diag_qfill_kernel<<<nb, 256, 0, C>>>(ptr<double>(h->P), ptr<double>(h->Q), (long)NP, ptr<int>(h->status));
-        CKL();
-        return GPK_OK;
-        };
-        const bool want_graph = h->use_graph && !h->diag_prof;
-        if (want_graph && h->fit_graph == nullptr) {
-            // capture (thread-local mode: other threads' CUDA calls are unaffected); P and R join the capture through
-            // evFork and are joined back before the end.  A failed capture falls back to direct enqueueing.
-            const double launches_before = h->launches_total;
-            cudaGraph_t graph = nullptr;
-            if (cudaStreamBeginCapture(C, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
-                const int erc = enqueue();
-                const cudaError_t ce = cudaStreamEndCapture(C, &graph);
-                if (erc == GPK_OK && ce == cudaSuccess && graph != nullptr &&
-                    cudaGraphInstantiate(&h->fit_graph, graph, 0) == cudaSuccess) {
-                    h->fit_graph_launches = h->launches_total - launches_before;
-                } else {
-                    h->fit_graph = nullptr;
-                    h->use_graph = 0;                               // do not try again on this handle
-                }
-                if (graph) cudaGraphDestroy(graph);
-                cudaGetLastError();
-                h->launches_total = launches_before;
-            } else {
-                cudaGetLastError();
-                h->use_graph = 0;
-            }
-        }
-        if (want_graph && h->fit_graph != nullptr) {
-            CK(cudaGraphLaunch(h->fit_graph, C));
-            h->launches_total += h->fit_graph_launches;
-        } else if ((rc = enqueue())) {
-            return rc;
-        }
-    }
-    // ---- plain look-ahead schedule [default]: diag(k), then the panel solve and the update of block column k+1 in
-    // 32-row tiles on the critical stream; the rest of the trailing update on the side stream
-    if (!split) {
-        gpk_diag_prezero_kernel<<<nb, 256, 0, h->stream>>>(K, (long)NP, ptr<double>(h->P), (long)NP);
-        CKL();
-    }
-    for (int k = 0; k < nb && !split; ++k) {
+    // ---- look-ahead schedule: diag(k), then the panel solve and the update of block column k+1 in 32-row tiles on the
+    // critical stream; the rest of the trailing update on the side stream
+    gpk_diag_prezero_kernel<<<nb, 256, 0, h->stream>>>(K, (long)NP, ptr<double>(h->P), (long)NP);
+    CKL();
+    for (int k = 0; k < nb; ++k) {
         long long* dprof = h->diag_prof ? ptr<long long>(h->dprof) : nullptr;
-        if (h->pdl && k > 0)
+        if (k > 0)
             CK(launch_pdl(gpk_potrf_diag_dmma_kernel, dim3(1), dim3(256), (size_t)DIAG_SMEM, h->stream, K, (long)NP, k,
                           ptr<double>(h->P), ptr<double>(h->Q), (long)NP, ptr<int>(h->status), ptr<double>(h->logdet_part), dprof));
         else
@@ -1769,10 +1589,8 @@ int gpk_fit_begin(gpk_handle* h, double diag_add, double mean) {
             }
         }
     }
-    if (!split) {
-        gpk_diag_qfill_kernel<<<nb, 256, 0, h->stream>>>(ptr<double>(h->P), ptr<double>(h->Q), (long)NP, ptr<int>(h->status));
-        CKL();
-    }
+    gpk_diag_qfill_kernel<<<nb, 256, 0, h->stream>>>(ptr<double>(h->P), ptr<double>(h->Q), (long)NP, ptr<int>(h->status));
+    CKL();
     CK(cudaEventRecord(h->ev[2], h->stream));
     gpk_fit_reduce_kernel<<<1, 256, 0, h->stream>>>(K + NP * NP, h->n, ptr<double>(h->logdet_part), nb,
                                                     ptr<double>(h->scal));

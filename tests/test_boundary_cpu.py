@@ -127,14 +127,3 @@ def test_bench_reference_arm_contract_and_loud_failure_without_gpu():
                              capture_output=True, text=True, timeout=600, cwd=root)
         assert out.returncode != 0 and "CUDA" in (out.stderr + out.stdout)
 
-
-def test_split_chain_schedule_is_race_free_and_order_preserving():
-    """tools/chain_schedule_check.py transcribes the launches / event records / stream waits of the split-chain
-    Cholesky schedule (gpk_fit_begin) into a happens-before graph: every conflicting pair of launches must be ordered
-    and every tile must receive its panels in increasing order (the GPU suite checks bit-identity of the factor)."""
-    import importlib.util
-    spec = importlib.util.spec_from_file_location("chain_schedule_check", os.path.join(ROOT, "tools", "chain_schedule_check.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    for nb in (3, 4, 7, 12, 32):
-        assert mod.check(nb) == 0

@@ -120,41 +120,17 @@ def test_cholesky_forward_solve_logdet(N, D, loader):
     assert np.abs(np.triu(Linv, 1)).max() == 0.0
 
 
-def test_cholesky_lookahead_and_split_chain_agree():
-    """the plain look-ahead schedule and the split chain with look-ahead 2 yield the same factor to rounding"""
-    from robo_b200 import _lib
-    X, y, _, theta, noise = O.synthetic_problem(600, 5, 1, seed_train=11)
-    ref = None
-    for split in (0, 1):
-        h = _lib.Handle(0)
-        h.set_option("chainsplit", split)
-        h.set_data(X, y)
-        f = product_kernel("matern52", theta, 5).flatten()
-        h.set_kernel(f["family"], f["log_amp"], f["axis"], f["group"], f["log_metric"])
-        logdet, ll = h.fit(1e-3 + G.TINY, float(np.mean(y)))
-        L, Li = h.get_factor(600), h.get_linv(600)
-        if ref is None:
-            ref = (logdet, ll, L, Li)
-        else:
-            assert abs(ll - ref[1]) <= 1e-12 * abs(ref[1]) and abs(logdet - ref[0]) <= 1e-12 * abs(ref[0])
-            np.testing.assert_allclose(L, ref[2], rtol=0, atol=1e-12 * np.abs(ref[2]).max())
-            np.testing.assert_allclose(Li, ref[3], rtol=0, atol=1e-11 * np.abs(ref[3]).max())
-        h.close()
-
-
 @pytest.mark.parametrize("N", [384, 1500, 4096])
-def test_split_chain_schedule_is_bit_identical(N):
-    """the split chain (diag(k+1) waits only for block row k+1; trailing update with look-ahead 2) and the depth-2
-    trailing update (two panels per K = 256 contraction) apply the panels to every tile in the same order as the plain
-    look-ahead schedule: identical bits in the factor, z and log-det"""
+def test_depth2_trailing_update_is_bit_identical(N):
+    """the depth-2 trailing update (two panels per K = 256 contraction) applies the panels to every tile in the same
+    order as one K = 128 update per step: identical bits in the factor, z and log-det, whether it is forced on (1) or
+    chosen from N (2, the default)"""
     from robo_b200 import _lib
     D = 6
     X, y, _, theta, noise = O.synthetic_problem(N, D, 1, seed_train=5)
     got = []
-    for split, graph, depth2 in ((1, 1, 1), (0, 1, 1), (1, 0, 1), (0, 1, 0)):
+    for depth2 in (1, 0, 2):
         h = _lib.Handle(0)
-        h.set_option("chainsplit", split)
-        h.set_option("graph", graph)                        # CUDA-graph replay of the schedule vs direct enqueueing
         h.set_option("depth2", depth2)                      # K = 256 trailing updates vs one K = 128 update per step
         h.set_data(X, y)
         f = product_kernel("matern52", theta, D).flatten()
@@ -588,7 +564,8 @@ def test_bad_arguments_raise_value_errors():
     h.fit(1e-3, 0.0)
     with pytest.raises(ValueError):
         h.set_option("chunk", 100)
-    for key in ("nonsense", "diag", "smalltile", "fusechain", "lookahead", "cov", "persist", "ozfused", "ozpdl", "covctas"):
+    for key in ("nonsense", "diag", "smalltile", "fusechain", "lookahead", "cov", "persist", "ozfused", "ozpdl", "covctas",
+                "chainsplit", "graph", "pdl"):
         with pytest.raises(ValueError):
             h.set_option(key, 1)
 

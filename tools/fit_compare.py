@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Fit time of the Cholesky schedules (split chain vs plain look-ahead) at the BASELINE sizes, next to cuSOLVER's
-dense potrf on the same GPU (torch.linalg.cholesky -> cusolverDnDpotrf / cusolverDnXpotrf; SURVEY.md section 7 step 4
-asked for that baseline).  Prints one JSON line per size.  python tools/fit_compare.py"""
+"""Fit time of the look-ahead Cholesky schedule (automatic depth-2 trailing updates, and depth2 = 0) at the BASELINE
+sizes, next to cuSOLVER's dense potrf on the same GPU (torch.linalg.cholesky -> cusolverDnDpotrf / cusolverDnXpotrf;
+SURVEY.md section 7 step 4 asked for that baseline).  Prints one JSON line per size.  python tools/fit_compare.py"""
 import json
 import os
 import sys
@@ -15,14 +15,12 @@ from robo_b200 import _lib                                   # noqa: E402
 from robo_b200 import kernels as K                           # noqa: E402
 
 
-def ours(N, D, split, reps=6, graph=1, depth2=1):
+def ours(N, D, reps=6, depth2=2):
     rng = np.random.RandomState(1234)
     X = rng.rand(N, D)
     y = np.sinc(X * 10 - 5).sum(axis=1) + 0.01 * rng.randn(N)
     theta = np.concatenate(([0.0], np.full(D, np.log(D / 4.0))))
     h = _lib.Handle(0)
-    h.set_option("chainsplit", split)
-    h.set_option("graph", graph)
     h.set_option("depth2", depth2)
     h.set_data(X, y)
     f = K.Product(K.ConstantKernel(theta[0], ndim=D), K.Matern52Kernel(np.exp(theta[1:]), ndim=D)).flatten()
@@ -58,18 +56,13 @@ def cusolver(N, reps=6):
 
 
 for N, D in ((1024, 8), (2048, 3), (4096, 16), (8192, 32)):
-    a = ours(N, D, 1)
-    a0 = ours(N, D, 1, graph=0)
-    b = ours(N, D, 0)
-    b0 = ours(N, D, 0, depth2=0)
+    b = ours(N, D)
+    b0 = ours(N, D, depth2=0)
     c = cusolver(N)
     flop = N ** 3 / 3.0
     print(json.dumps({"N": N, "D": D,
-                      "split_chain": {"fit_ms": a[0], "kbuild_ms": a[1], "potrf_incl_forward_solve_logdet_ms": a[2], "linv_ms": a[3],
-                                      "potrf_tflops": flop / (a[2] * 1e-3) / 1e12},
-                      "split_chain_direct_enqueue": {"fit_ms": a0[0], "potrf_incl_forward_solve_logdet_ms": a0[2]},
                       "plain_lookahead": {"fit_ms": b[0], "kbuild_ms": b[1], "potrf_incl_forward_solve_logdet_ms": b[2],
-                                          "potrf_tflops": flop / (b[2] * 1e-3) / 1e12},
+                                          "linv_ms": b[3], "potrf_tflops": flop / (b[2] * 1e-3) / 1e12},
                       "plain_lookahead_depth1": {"fit_ms": b0[0], "potrf_incl_forward_solve_logdet_ms": b0[2]},
                       "cusolver_torch_linalg_cholesky": {"potrf_ms": c[0], "forward_solve_ms": c[1],
                                                          "potrf_tflops": flop / (c[0] * 1e-3) / 1e12}}))

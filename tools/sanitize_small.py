@@ -33,11 +33,11 @@ for loader in (2, 1, 0):
     X2, y2 = np.vstack([X, rng.rand(10, D)]), np.concatenate([y, rng.rand(10)])
     print(" append", h.fit_append(X2, y2, 1e-3 + 1.25e-12, float(y2.mean())), h.predict(Xs[:64])[0][:2])
     h.close()
-# round-2 kernels: int8 contraction (digit builder, several chunks), split chain replayed from a CUDA graph, depth-2
-# trailing updates, fused multi-model scoring, raw posterior covariance
+# round-2 kernels: int8 contraction (digit builder, several chunks), depth-2 trailing updates, fused multi-model
+# scoring, raw posterior covariance
 Xb = rng.rand(2304, D)
 hs = []
-for opts in ({"ozaki": 1}, {"ozaki": 0, "chainsplit": 1, "graph": 1, "depth2": 1},
+for opts in ({"ozaki": 1}, {"ozaki": 0, "depth2": 1},
              # int8 contraction variants: one tile per CTA / persistent walk
              {"ozaki": 1, "ozpersist": 0}, {"ozaki": 1, "ozpersist": 1}):
     h = _lib.Handle(0)
