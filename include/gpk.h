@@ -494,6 +494,113 @@ int gpk_maximize_lbfgs_es_cost(gpk_handle* const* objective, gpk_handle* const* 
                                double overhead, int maxcor, int maxiter, long maxfun, double ftol, double pgtol,
                                double* x_out, double* energy, int* nit, long* nfev, int* status);
 
+/* CMAES.maximize (robo/maximizers/cmaes.py:50-81) on the device: cma.fmin(obj_func, x0, sigma0, restarts, bounds,
+ * maxfevals) minimising the energy e = -acq(x) of the reference's obj_func (cmaes.py:66-68), without the `cma` package.
+ * The standard (mu/mu_w, lambda)-CMA-ES of Hansen's tutorial ("The CMA Evolution Strategy: A Tutorial", 2016, Table 1
+ * defaults, positive weights only): every generation samples lambda members from N(m, sigma^2 C), scores them in one
+ * batched pass, ranks them, updates m, sigma, the paths p_sigma / p_c and C, and eigendecomposes C (parallel cyclic
+ * Jacobi) when purecma's lazy rule asks for it; all of it stays on the device and only a 24-byte status record crosses
+ * PCIe per generation.  robo_b200/csrc/gpk_cmaes.cuh states every step, the Philox counter layout and every rounding.
+ * Bounds go through cma's BoundTransform, BoxConstraintsLinQuadTransformation, restated per coordinate with
+ *   a_l = min((u - l) / 2, (1 + |l|) / 20),  a_u = min((u - l) / 2, (1 + |u|) / 20):
+ * shift periodically into [l - a_l, u + a_u] (period 2 (u - l + a_l + a_u)) when farther out than a_l + (u - l) / 2
+ * beyond l - a_l (a_u likewise at the top), mirror at u + a_u and l - a_l, then T(x) = l + (x - (l - a_l))^2 / (4 a_l)
+ * on [l - a_l, l + a_l), the identity up to u - a_u and u - (x - (u + a_u))^2 / (4 a_u) above.  The distribution lives
+ * in genotype space, scoring sees the phenotype T(x), and the result is the best phenotype seen (an earlier generation,
+ * then the lower index, win ties).  The start mean is the genotype of x0: l - a_l + 2 sqrt(a_l (x0 - l)) near l, the
+ * identity inside, u + a_u - 2 sqrt(a_u (u - x0)) near u.
+ * Stop tests after every generation, the first that holds: maxfevals (evaluations over all runs >= n_func_evals, so the
+ * overshoot is below lambda), tolfun 1e-11 (the range of this generation's energies and of the best energies of the
+ * last 10 + ceil(30 d / lambda) generations, once that many exist; NaN ignored), tolx 1e-11 (sigma max_j max(|p_c,j|,
+ * sqrt(C_jj))), conditioncov 1e14 (the ratio of the largest to the smallest eigenvalue of C), numerical (sigma, m, C or
+ * an eigenvalue not finite, or sigma or an eigenvalue <= 0).  IPOP restarts (cma.fmin's incpopsize = 2): run r has
+ * lambda_0 2^r members and its own constants, and starts again from the genotype of x0 and sigma0; the budget is
+ * shared, and a run that stops on maxfevals ends the restarts.
+ * `cma` itself is not restated bit for bit, only in law: the Philox stream replaces numpy's, and these parts of recent
+ * `cma` versions are not restated: active CMA (negative recombination weights, on by default there), the resampling of
+ * members whose energy is NaN (here a NaN energy ranks last), and the noeffectaxis / noeffectcoord / tolstagnation /
+ * tolupsigma stops.
+ * consts: (restarts + 1) rows of GPK_CMA_NCONST doubles, one per run, laid out as GPK_CMA_C_* (the constants of
+ * robo_b200._lib.cmaes_constants, computed on the host so that no log runs on the device); weights w_0 .. w_mu-1 at
+ * GPK_CMA_C_W.  d (the handles' input dimension) 2 .. GPK_CMA_MAX_D; lower < upper and x0 inside [lower, upper] (d each,
+ * x0 finite); sigma0 > 0; n_func_evals >= 1; 0 <= restarts; every run's lambda 2 .. GPK_CMA_MAX_LAMBDA, mu = lambda / 2
+ * (rounded down), history length <= GPK_CMA_HIST and flat index < lambda; otherwise GPK_BAD_ARG.
+ * Out (gpk_cmaes_result; best_x required, every other pointer may be NULL): best_x (d) and best_energy (NaN when no
+ * finite energy was seen), nfev_total; per run (restarts + 1 each; runs not started give 0, 0, GPK_CMA_RUNNING) nit
+ * generations, nfev evaluations and stop (gpk_cmaes_stop); the last run's final m (genotype, d), sigma, p_sigma (d),
+ * p_c (d) and C (d x d). */
+#define GPK_CMA_MAX_D 64
+#define GPK_CMA_MAX_LAMBDA 2048          /* covers restarts doublings: lambda_0 2^restarts <= this */
+#define GPK_CMA_HIST 160                 /* longest tolfun history: 10 + ceil(30 d / lambda) <= 130 for 2 <= d <= 64 */
+#define GPK_CMA_C_LAMBDA 0
+#define GPK_CMA_C_MU 1
+#define GPK_CMA_C_MUEFF 2
+#define GPK_CMA_C_CS 3                   /* c_sigma */
+#define GPK_CMA_C_DS 4                   /* d_sigma */
+#define GPK_CMA_C_CC 5
+#define GPK_CMA_C_C1 6
+#define GPK_CMA_C_CMU 7
+#define GPK_CMA_C_CHI 8                  /* E||N(0, I)|| = sqrt(d) (1 - 1 / (4 d) + 1 / (21 d^2)) */
+#define GPK_CMA_C_HIST 9                 /* tolfun history length 10 + ceil(30 d / lambda) */
+#define GPK_CMA_C_EIG 10                 /* lambda / ((c1 + cmu) d 10): evaluations between eigendecompositions */
+#define GPK_CMA_C_FLAT 11                /* ceil(0.7 lambda) - 1: the rank of the flat-fitness test */
+#define GPK_CMA_C_OMCS 12                /* 1 - c_sigma */
+#define GPK_CMA_C_CPS 13                 /* sqrt(c_sigma (2 - c_sigma) mueff) */
+#define GPK_CMA_C_OMCC 14                /* 1 - c_c */
+#define GPK_CMA_C_CCC 15                 /* sqrt(c_c (2 - c_c) mueff) */
+#define GPK_CMA_C_CCD 16                 /* c_c (2 - c_c) */
+#define GPK_CMA_C_A0 17                  /* 1 - c1 - cmu */
+#define GPK_CMA_C_HTH 18                 /* (1.4 + 2 / (d + 1)) chi: the h_sigma threshold */
+#define GPK_CMA_C_CSDS 19                /* c_sigma / d_sigma */
+#define GPK_CMA_C_W 20
+#define GPK_CMA_NCONST (GPK_CMA_C_W + GPK_CMA_MAX_LAMBDA / 2)
+typedef enum {
+    GPK_CMA_RUNNING = 0,       /* not stopped (a run that was never started reports this too) */
+    GPK_CMA_MAXFEVALS = 1,
+    GPK_CMA_TOLFUN = 2,
+    GPK_CMA_TOLX = 3,
+    GPK_CMA_CONDITIONCOV = 4,
+    GPK_CMA_NUMERICAL = 5
+} gpk_cmaes_stop;
+typedef struct {
+    double* best_x;
+    double* best_energy;
+    long* nfev_total;
+    int* nit;
+    long* nfev;
+    int* stop;
+    double* m;
+    double* sigma;
+    double* ps;
+    double* pc;
+    double* C;
+} gpk_cmaes_result;
+/* EI / LogEI / PI / LCB over the mean of the n_models handles (one handle: gpk_acq's value; eta[n_models] and par as
+ * for gpk_acq_multi); n_negative: EI values < 0 over all evaluations (ei.py:86-88 raises on them). */
+int gpk_maximize_cmaes(gpk_handle* const* models, int n_models, int acq_kind, const double* eta, double par,
+                       unsigned long long seed, const double* x0, double sigma0, const double* lower,
+                       const double* upper, long n_func_evals, int restarts, const double* consts,
+                       gpk_cmaes_result* out, long* n_negative);
+/* -(gpk_es_multi's value over objective[0 .. n-1]); n = 1: -(gpk_es_compute's value).  One GPU. */
+int gpk_maximize_cmaes_es(gpk_handle* const* objective, int n, unsigned long long seed, const double* x0, double sigma0,
+                          const double* lower, const double* upper, long n_func_evals, int restarts,
+                          const double* consts, gpk_cmaes_result* out);
+/* -(gpk_esmc_multi's value); GPK_NOT_PD as for gpk_esmc_compute (checked after every generation).  One GPU. */
+int gpk_maximize_cmaes_esmc(gpk_handle* const* objective, int n, unsigned long long seed, const double* x0,
+                            double sigma0, const double* lower, const double* upper, long n_func_evals, int restarts,
+                            const double* consts, gpk_cmaes_result* out);
+/* -(gpk_es_cost_multi's value over the (objective[i], cost[i]) pairs) in the extended box lower / upper (d each);
+ * cfg_lower / cfg_upper (n_bounds = d - 1), the basis codes and the overhead as for gpk_es_cost_multi.  One GPU. */
+int gpk_maximize_cmaes_es_cost(gpk_handle* const* objective, gpk_handle* const* cost, int n, unsigned long long seed,
+                               const double* x0, double sigma0, const double* lower, const double* upper,
+                               long n_func_evals, int restarts, const double* consts, const double* cfg_lower,
+                               const double* cfg_upper, int n_bounds, int basis_objective, int basis_cost,
+                               double overhead, gpk_cmaes_result* out);
+/* The standard normals gpk_maximize_cmaes* draw in generations g0 .. g1 - 1 of run `run` with `lambda` members in
+ * dimension d: out ((g1 - g0) x lambda x d, row-major); z depends on (seed, run, g, member, coordinate) only.
+ * 0 <= run < 256, 0 <= g0 < g1, 1 <= lambda <= GPK_CMA_MAX_LAMBDA, 1 <= d <= GPK_CMA_MAX_D. */
+int gpk_cmaes_draws(gpk_handle* h, unsigned long long seed, int run, int g0, int g1, int lambda, int d, double* out);
+
 /* The representer points of n entropy-search estimators in one call: the emcee 2.x stretch move (a = 2) of
  * robo_b200/util/ensemble_sampler.py, replacing the host loops of information_gain.py:68-81 and
  * information_gain_per_unit_cost.py:152-172.  Estimator i walks nb walkers of dimension dw on models[i], seeded by

@@ -27,6 +27,12 @@ BASIS_S, BASIS_ONE_MINUS_S_SQ = range(2)      # gpk_basis: the environment colum
 PRIOR_NONE, PRIOR_DEFAULT, PRIOR_ENV = range(3)   # gpk_prior_kind: the hyper-priors gpk_sample_hypers restates
 HYPER_MAX_N = 232                              # GPK_HYPER_MAX_N: most training points of gpk_sample_hypers
 HYPER_MAX_DIM = 96                             # GPK_HYPER_MAX_DIM: most entries of theta (log noise included)
+CMA_MAX_D, CMA_MAX_LAMBDA, CMA_HIST = 64, 2048, 160   # GPK_CMA_MAX_D / GPK_CMA_MAX_LAMBDA / GPK_CMA_HIST
+CMA_C_W = 20                                   # GPK_CMA_C_W: where a run's weights start in its constant row
+CMA_NCONST = CMA_C_W + CMA_MAX_LAMBDA // 2     # GPK_CMA_NCONST: doubles per run in the constant table
+# gpk_cmaes_stop: why a CMA-ES run stopped (RUNNING: not stopped, or never started)
+CMA_RUNNING, CMA_MAXFEVALS, CMA_TOLFUN, CMA_TOLX, CMA_CONDITIONCOV, CMA_NUMERICAL = range(6)
+CMA_STOP_NAMES = ("running", "maxfevals", "tolfun", "tolx", "conditioncov", "numerical")
 
 _dp = C.POINTER(C.c_double)
 _ip = C.POINTER(C.c_int)
@@ -121,6 +127,15 @@ _SIGNATURES = {
     "gpk_maximize_lbfgs_es_cost": [C.POINTER(_vp), C.POINTER(_vp), C.c_int, C.c_long, _dp, _dp, _dp, _dp, _dp, C.c_int,
                                    C.c_int, C.c_int, C.c_double, C.c_int, C.c_int, C.c_long, C.c_double, C.c_double,
                                    _dp, _dp, _ip, _lp, _ip],
+    "gpk_maximize_cmaes": [C.POINTER(_vp), C.c_int, C.c_int, _dp, C.c_double, C.c_ulonglong, _dp, C.c_double, _dp, _dp,
+                           C.c_long, C.c_int, _dp, _vp, _lp],
+    "gpk_maximize_cmaes_es": [C.POINTER(_vp), C.c_int, C.c_ulonglong, _dp, C.c_double, _dp, _dp, C.c_long, C.c_int, _dp,
+                              _vp],
+    "gpk_maximize_cmaes_esmc": [C.POINTER(_vp), C.c_int, C.c_ulonglong, _dp, C.c_double, _dp, _dp, C.c_long, C.c_int,
+                                _dp, _vp],
+    "gpk_maximize_cmaes_es_cost": [C.POINTER(_vp), C.POINTER(_vp), C.c_int, C.c_ulonglong, _dp, C.c_double, _dp, _dp,
+                                   C.c_long, C.c_int, _dp, _dp, _dp, C.c_int, C.c_int, C.c_int, C.c_double, _vp],
+    "gpk_cmaes_draws": [_vp, C.c_ulonglong, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _dp],
     "gpk_sample_representers": [C.POINTER(_vp), C.c_int, C.POINTER(C.c_ulonglong), C.c_int, C.c_int, C.c_int, C.c_int,
                                 _dp, C.c_double, _dp, _dp, C.c_int, C.c_int, _dp, _dp, C.c_int, C.c_double, _dp, _dp,
                                 _ip, _lp, _lp],
@@ -951,6 +966,137 @@ def maximize_lbfgs_es_cost(objective, cost, x0, lower, upper, cfg_lower, cfg_upp
                                                 int(basis_cost), float(overhead), *_lb_opts(options),
                                                 *_lb_out_ptrs(outs)))
     return _lb_result(outs)
+
+
+def cmaes_run_constants(d, lam):
+    """The constants of one CMA-ES run of population lam in dimension d (Hansen's tutorial, Table 1, positive weights
+    only; purecma's lazy eigendecomposition gap; cma's tolfun history length) as a dict.  gpk_maximize_cmaes* and
+    tests/cmaes_model.py both take them from here, so no log runs on the device."""
+    import math
+    d, lam = int(d), int(lam)
+    mu = lam // 2
+    w = math.log((lam + 1) / 2.0) - np.log(np.arange(1, mu + 1, dtype=np.float64))
+    w = w / np.sum(w)
+    mueff = 1.0 / np.sum(w * w)
+    cs = (mueff + 2.0) / (d + mueff + 5.0)
+    ds = 1.0 + 2.0 * max(0.0, math.sqrt((mueff - 1.0) / (d + 1.0)) - 1.0) + cs
+    cc = (4.0 + mueff / d) / (d + 4.0 + 2.0 * mueff / d)
+    c1 = 2.0 / ((d + 1.3) ** 2 + mueff)
+    cmu = min(1.0 - c1, 2.0 * (mueff - 2.0 + 1.0 / mueff) / ((d + 2.0) ** 2 + mueff))
+    chi = math.sqrt(d) * (1.0 - 1.0 / (4.0 * d) + 1.0 / (21.0 * d * d))
+    return dict(lam=lam, mu=mu, w=w, mueff=float(mueff), cs=cs, ds=ds, cc=cc, c1=c1, cmu=cmu, chi=chi,
+                hist=10 + int(math.ceil(30.0 * d / lam)), eig_gap=lam / (c1 + cmu) / d / 10.0,
+                flat=int(math.ceil(0.7 * lam)) - 1, omcs=1.0 - cs, cps=math.sqrt(cs * (2.0 - cs) * mueff),
+                omcc=1.0 - cc, ccc=math.sqrt(cc * (2.0 - cc) * mueff), ccd=cc * (2.0 - cc), a0=1.0 - c1 - cmu,
+                hth=(1.4 + 2.0 / (d + 1.0)) * chi, csds=cs / ds)
+
+
+def cmaes_lambda(d, run=0):
+    """The population of IPOP run ``run``: (4 + floor(3 ln d)) 2^run."""
+    import math
+    return (4 + int(3.0 * math.log(d))) << int(run)
+
+
+def cmaes_constants(d, restarts):
+    """The constant table of gpk_maximize_cmaes*: (restarts + 1, CMA_NCONST), one GPK_CMA_C_* row per run.  A run whose
+    lambda exceeds CMA_MAX_LAMBDA keeps its lambda but no weights; the library refuses it."""
+    keys = ("lam", "mu", "mueff", "cs", "ds", "cc", "c1", "cmu", "chi", "hist", "eig_gap", "flat", "omcs", "cps", "omcc",
+            "ccc", "ccd", "a0", "hth", "csds")
+    tab = np.zeros((int(restarts) + 1, CMA_NCONST))
+    for r in range(int(restarts) + 1):
+        c = cmaes_run_constants(d, cmaes_lambda(d, r))
+        tab[r, :CMA_C_W] = [c[k] for k in keys]
+        if c["mu"] <= CMA_MAX_LAMBDA // 2:
+            tab[r, CMA_C_W:CMA_C_W + c["mu"]] = c["w"]
+    return tab
+
+
+class _CmaesResult(C.Structure):
+    _fields_ = [(name, _vp) for name in ("best_x", "best_energy", "nfev_total", "nit", "nfev", "stop", "m", "sigma",
+                                         "ps", "pc", "C")]
+
+
+def _cmaes_io(x0, lower, upper, restarts):
+    lo, up, x0 = f64(lower).ravel(), f64(upper).ravel(), f64(x0).ravel()
+    if not lo.size == up.size == x0.size:
+        raise ValueError("maximize_cmaes: x0, lower and upper need d entries each")
+    d, runs = lo.size, int(restarts) + 1
+    if runs < 1:
+        raise ValueError("maximize_cmaes: need restarts >= 0")
+    outs = dict(best_x=np.empty(d), best_energy=np.empty(1), nfev_total=np.zeros(1, dtype=np.int_),
+                nit=np.zeros(runs, dtype=np.intc), nfev=np.zeros(runs, dtype=np.int_), stop=np.zeros(runs, dtype=np.intc),
+                m=np.empty(d), sigma=np.empty(1), ps=np.empty(d), pc=np.empty(d), C=np.empty((d, d)))
+    res = _CmaesResult(*[outs[k].ctypes.data for k, _ in _CmaesResult._fields_])
+    return x0, lo, up, f64(cmaes_constants(d, restarts)), outs, res
+
+
+def _cmaes_result(outs):
+    return dict(x=outs["best_x"], energy=float(outs["best_energy"][0]), nfev_total=int(outs["nfev_total"][0]),
+                nit=outs["nit"].astype(np.int64), nfev=outs["nfev"].astype(np.int64),
+                stop=outs["stop"].astype(np.int64), m=outs["m"], sigma=float(outs["sigma"][0]), ps=outs["ps"],
+                pc=outs["pc"], C=outs["C"])
+
+
+def maximize_cmaes(handles, kind, eta, par, seed, x0, lower, upper, n_func_evals=1000, restarts=0, sigma0=0.6):
+    """gpk_maximize_cmaes over ``handles`` (all fitted, same device): CMA-ES from x0 (d,) minimising -acq (kind ACQ_EI
+    ... ACQ_LCB, acq the mean over the handles) -> dict(x (d,), energy, nfev_total, nit / nfev / stop per run, the last
+    run's final m, sigma, ps, pc and C, n_negative)."""
+    h0 = handles[0]
+    x0, lo, up, tab, outs, res = _cmaes_io(x0, lower, upper, restarts)
+    nn = C.c_long()
+    h0._check(h0.lib.gpk_maximize_cmaes(_handles(handles), len(handles), int(kind), _as_dp(_etas(eta, len(handles))),
+                                        float(par), int(seed) & 0xFFFFFFFFFFFFFFFF, _as_dp(x0), float(sigma0),
+                                        _as_dp(lo), _as_dp(up), int(n_func_evals), int(restarts), _as_dp(tab),
+                                        C.byref(res), C.byref(nn)))
+    r = _cmaes_result(outs)
+    r["n_negative"] = nn.value
+    return r
+
+
+def maximize_cmaes_es(objective, seed, x0, lower, upper, n_func_evals=1000, restarts=0, sigma0=0.6):
+    """gpk_maximize_cmaes_es: the same minimising minus the entropy change (one handle: gpk_es_compute's value;
+    several: gpk_es_multi's mean) -> as maximize_cmaes without n_negative."""
+    h0 = objective[0]
+    x0, lo, up, tab, outs, res = _cmaes_io(x0, lower, upper, restarts)
+    h0._check(h0.lib.gpk_maximize_cmaes_es(_handles(objective), len(objective), int(seed) & 0xFFFFFFFFFFFFFFFF,
+                                           _as_dp(x0), float(sigma0), _as_dp(lo), _as_dp(up), int(n_func_evals),
+                                           int(restarts), _as_dp(tab), C.byref(res)))
+    return _cmaes_result(outs)
+
+
+def maximize_cmaes_esmc(objective, seed, x0, lower, upper, n_func_evals=1000, restarts=0, sigma0=0.6):
+    """gpk_maximize_cmaes_esmc: the same minimising minus the sampling-based entropy change -> as maximize_cmaes_es."""
+    h0 = objective[0]
+    x0, lo, up, tab, outs, res = _cmaes_io(x0, lower, upper, restarts)
+    h0._check(h0.lib.gpk_maximize_cmaes_esmc(_handles(objective), len(objective), int(seed) & 0xFFFFFFFFFFFFFFFF,
+                                             _as_dp(x0), float(sigma0), _as_dp(lo), _as_dp(up), int(n_func_evals),
+                                             int(restarts), _as_dp(tab), C.byref(res)))
+    return _cmaes_result(outs)
+
+
+def maximize_cmaes_es_cost(objective, cost, seed, x0, lower, upper, cfg_lower, cfg_upper, basis_objective, basis_cost,
+                           overhead, n_func_evals=1000, restarts=0, sigma0=0.6):
+    """gpk_maximize_cmaes_es_cost: the same over the extended box lower / upper (d) minimising minus the information
+    gain per unit cost of gpk_es_cost_multi (configuration bounds cfg_lower / cfg_upper, d - 1) -> as
+    maximize_cmaes_es."""
+    ho, hc, clo, cup = _es_cost_args(objective, cost, cfg_lower, cfg_upper)
+    h0 = objective[0]
+    x0, lo, up, tab, outs, res = _cmaes_io(x0, lower, upper, restarts)
+    if lo.size != clo.size + 1:
+        raise ValueError("maximize_cmaes_es_cost: the box needs d entries, the configuration bounds d - 1")
+    h0._check(h0.lib.gpk_maximize_cmaes_es_cost(ho, hc, len(objective), int(seed) & 0xFFFFFFFFFFFFFFFF, _as_dp(x0),
+                                                float(sigma0), _as_dp(lo), _as_dp(up), int(n_func_evals),
+                                                int(restarts), _as_dp(tab), _as_dp(clo), _as_dp(cup), clo.size,
+                                                int(basis_objective), int(basis_cost), float(overhead), C.byref(res)))
+    return _cmaes_result(outs)
+
+
+def cmaes_draws(handle, seed, run, g0, g1, lam, d):
+    """gpk_cmaes_draws: the normals of generations g0 .. g1 - 1 of run ``run`` -> ((g1 - g0), lam, d)."""
+    out = np.empty((int(g1) - int(g0), int(lam), int(d)))
+    handle._check(handle.lib.gpk_cmaes_draws(handle._h, int(seed) & 0xFFFFFFFFFFFFFFFF, int(run), int(g0), int(g1),
+                                             int(lam), int(d), _as_dp(out)))
+    return out
 
 
 def sample_representers(models, seeds, nb, steps, max_runs, kind, eta, par, lower, upper, fabolas=None):

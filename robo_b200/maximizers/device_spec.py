@@ -1,5 +1,6 @@
 """What scores an acquisition on the device, shared by the device maximizers (DifferentialEvolution, SciPyOptimizer),
-and the differential-evolution and multi-start L-BFGS calls over it (gpk_maximize_de*, gpk_maximize_lbfgs*)."""
+and the differential-evolution, multi-start L-BFGS and CMA-ES calls over it (gpk_maximize_de*, gpk_maximize_lbfgs*,
+gpk_maximize_cmaes*)."""
 import numpy as np
 
 from robo_b200 import _lib
@@ -105,6 +106,18 @@ def maximize_lbfgs(which, spec, x0, lower, upper):
                 lambda ho, hc, **cfg: _lib.maximize_lbfgs_es_cost(ho, hc, x0, lower, upper, **cfg),
                 lambda hs: _lib.maximize_lbfgs_es(hs, x0, lower, upper),
                 lambda hs, kind, etas, par: _lib.maximize_lbfgs(hs, kind, etas, par, x0, lower, upper))
+
+
+def maximize_cmaes(which, spec, seed, x0, lower, upper, n_func_evals, restarts):
+    """CMA-ES on the device from x0 over what ``device_spec`` returned, sigma0 = 0.6 as the reference passes it ->
+    _lib's result dict (x, energy, nfev_total, nit / nfev / stop per run, the last run's state)."""
+    args = (seed, x0, lower, upper, n_func_evals, restarts)
+    return _run(which, spec,
+                lambda ho, hc, **cfg: _lib.maximize_cmaes_es_cost(ho, hc, seed, x0, lower, upper, n_func_evals=n_func_evals,
+                                                                  restarts=restarts, **cfg),
+                lambda hs: _lib.maximize_cmaes_es(hs, *args),
+                lambda hs, kind, etas, par: _lib.maximize_cmaes(hs, kind, etas, par, *args),
+                lambda hs: _lib.maximize_cmaes_esmc(hs, *args))
 
 
 def lbfgs_success(status):

@@ -113,6 +113,10 @@ r = _lib.maximize_lbfgs([h], _lib.ACQ_LOG_EI, [float(y[:100].min())], 0.0, x0, n
                         maxiter=8)
 print("lbfgs", r["nfev"], r["status"],
       _lib.maximize_lbfgs([h], _lib.OBJ_MEAN_STD, None, 0.0, x0, np.zeros(D), np.ones(D), maxiter=8)["status"])
+# CMA-ES: the init, sample and update kernels (the Jacobi sweeps included) over two runs, and the draws kernel
+r = _lib.maximize_cmaes([h], _lib.ACQ_LOG_EI, [float(y[:100].min())], 0.0, 5, rng.rand(D), np.zeros(D), np.ones(D),
+                        n_func_evals=300, restarts=1)
+print("cmaes", r["nit"], r["stop"], _lib.cmaes_draws(h, 5, 1, 0, 2, 6, D).shape)
 h.close()
 h = _lib.moments_handle()
 print(h.acq_moments(rng.randn(100), rng.rand(100) + 0.1, _lib.ACQ_LOG_EI, 0.0, 0.0)[0][:3])
