@@ -601,6 +601,73 @@ int gpk_maximize_cmaes_es_cost(gpk_handle* const* objective, gpk_handle* const* 
  * 0 <= run < 256, 0 <= g0 < g1, 1 <= lambda <= GPK_CMA_MAX_LAMBDA, 1 <= d <= GPK_CMA_MAX_D. */
 int gpk_cmaes_draws(gpk_handle* h, unsigned long long seed, int run, int g0, int g1, int lambda, int d, double* out);
 
+/* Direct.maximize (robo/maximizers/direct.py:56-85) on the device: DIRECT.solve(obj_func, l, u, maxT = n_iters,
+ * maxf = n_func_evals) minimising the energy e = -acq(x) of the reference's _direct_acquisition_fkt_wrapper
+ * (direct.py:50-54), without the `DIRECT` package.  Jones' original DIRECT (algmethod = 0, eps = 1e-4) as Gablonsky's
+ * DIRECT 2.0.4 runs it: every iteration chooses its potentially optimal rectangles and writes the points it samples
+ * (c +- delta e_i over each chosen rectangle's longest sides, mapped to the box as (c + l / (u - l)) (u - l)) into one
+ * row buffer in one CTA, scores them in one batched pass, and divides, inserts and updates the incumbent in one CTA;
+ * only a 24-byte status record crosses PCIe per iteration.  robo_b200/csrc/gpk_direct.cuh states every step.
+ * The level of a rectangle is Gablonsky's n k + j (k: its fewest trisections, j: its sides trisected k + 1 times), of
+ * size 0.5 sqrt(n - j + j / 9) / 3^k; one energy-sorted list per level.  Selection: the head of each level on the
+ * lower-right hull passing Jones' test f - K d <= minf - 1e-4 |minf|, then every rectangle within 1e-13 of a chosen
+ * head at its level.  The rules follow scipy.optimize.direct (scipy's C translation of the same code), the one
+ * executable form of it available: a head whose lower slope bound exceeds its upper one is kept without Jones' test.
+ * Stop tests after every iteration, the first that holds: a rectangle at level >= GPK_DIRECT_MAXDEEP - 1 was chosen
+ * (MAXDEEP_HIT; the chosen ones before it are divided), more than GPK_DIRECT_MAXDIV rectangles were chosen
+ * (MAXDIV_HIT; nothing sampled), (minf + 1e100) 100 / 1e100 <= 0.01 (the package's fglobal = -1e100, fglper = 0.01),
+ * nfev >= n_func_evals (so the last iteration overshoots); and the run ends without sampling when iteration n_iters
+ * would begin (iterations 2 .. n_iters - 1 sample, the first one being the root's division; nit = max(n_iters, 2)
+ * then, as scipy counts).  The result x is the package's
+ * c (u - l) + (l / (u - l)) (u - l) of the best centre, which can differ from the scored row in the last bit.
+ * Non-finite energies: NaN is stored as +inf; +inf and -inf are kept (-inf ends the run on the fglobal test).
+ * Not restated: the package's stdout report and log file, its hidden-constraint flag (the reference's wrapper
+ * always returns 0), DIRECT-L (algmethod = 1) and its other options.
+ * d (the handles' input dimension) 1 .. GPK_DIRECT_MAX_D; lower < upper (d each, finite); n_func_evals >= 1;
+ * n_iters >= 1; (2 d + 1) max(n_func_evals, 2 d + 1) <= GPK_DIRECT_MAX_RECTS (the store: every iteration starts
+ * below the budget or at the 2 d + 1 initial points and adds at most 2 d rows per stored rectangle); otherwise
+ * GPK_BAD_ARG.  Device memory: that many rectangles of d centre doubles and d ints, and as many rows of d doubles.
+ * Out (gpk_direct_result; best_x required, every other pointer may be NULL): best_x (d), best_energy, nit, nfev, stop
+ * (gpk_direct_stop), rows: the rows sampled by iterations 2 .. nit (nit - 1 of them; nit - 2 when the run stops on
+ * n_iters; n_iters - 1 entries reserved by the caller). */
+#define GPK_DIRECT_MAX_D 64
+#define GPK_DIRECT_MAXDEEP 600
+#define GPK_DIRECT_MAXDIV 5000
+#define GPK_DIRECT_MAX_RECTS (1L << 22)
+typedef enum {
+    GPK_DIRECT_RUNNING = 0,
+    GPK_DIRECT_MAXF = 1,
+    GPK_DIRECT_MAXT = 2,
+    GPK_DIRECT_FGLOBAL_HIT = 3,
+    GPK_DIRECT_MAXDEEP_HIT = 4,
+    GPK_DIRECT_MAXDIV_HIT = 5
+} gpk_direct_stop;
+typedef struct {
+    double* best_x;
+    double* best_energy;
+    int* nit;
+    long* nfev;
+    int* stop;
+    long* rows;
+} gpk_direct_result;
+/* EI / LogEI / PI / LCB over the mean of the n_models handles (eta[n_models] and par as for gpk_acq_multi);
+ * n_negative: EI values < 0 over all evaluations (ei.py:86-88 raises on them). */
+int gpk_maximize_direct(gpk_handle* const* models, int n_models, int acq_kind, const double* eta, double par,
+                        const double* lower, const double* upper, long n_func_evals, int n_iters,
+                        gpk_direct_result* out, long* n_negative);
+/* -(gpk_es_multi's value over objective[0 .. n-1]); n = 1: -(gpk_es_compute's value).  One GPU. */
+int gpk_maximize_direct_es(gpk_handle* const* objective, int n, const double* lower, const double* upper,
+                           long n_func_evals, int n_iters, gpk_direct_result* out);
+/* -(gpk_esmc_multi's value); GPK_NOT_PD as for gpk_esmc_compute (checked after every pass).  One GPU. */
+int gpk_maximize_direct_esmc(gpk_handle* const* objective, int n, const double* lower, const double* upper,
+                             long n_func_evals, int n_iters, gpk_direct_result* out);
+/* -(gpk_es_cost_multi's value over the (objective[i], cost[i]) pairs) in the extended box lower / upper (d each);
+ * cfg_lower / cfg_upper (n_bounds = d - 1), the basis codes and the overhead as for gpk_es_cost_multi.  One GPU. */
+int gpk_maximize_direct_es_cost(gpk_handle* const* objective, gpk_handle* const* cost, int n, const double* lower,
+                                const double* upper, long n_func_evals, int n_iters, const double* cfg_lower,
+                                const double* cfg_upper, int n_bounds, int basis_objective, int basis_cost,
+                                double overhead, gpk_direct_result* out);
+
 /* The representer points of n entropy-search estimators in one call: the emcee 2.x stretch move (a = 2) of
  * robo_b200/util/ensemble_sampler.py, replacing the host loops of information_gain.py:68-81 and
  * information_gain_per_unit_cost.py:152-172.  Estimator i walks nb walkers of dimension dw on models[i], seeded by

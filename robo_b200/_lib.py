@@ -33,6 +33,11 @@ CMA_NCONST = CMA_C_W + CMA_MAX_LAMBDA // 2     # GPK_CMA_NCONST: doubles per run
 # gpk_cmaes_stop: why a CMA-ES run stopped (RUNNING: not stopped, or never started)
 CMA_RUNNING, CMA_MAXFEVALS, CMA_TOLFUN, CMA_TOLX, CMA_CONDITIONCOV, CMA_NUMERICAL = range(6)
 CMA_STOP_NAMES = ("running", "maxfevals", "tolfun", "tolx", "conditioncov", "numerical")
+DIRECT_MAX_D, DIRECT_MAXDEEP, DIRECT_MAXDIV = 64, 600, 5000   # GPK_DIRECT_MAX_D / _MAXDEEP / _MAXDIV
+DIRECT_MAX_RECTS = 1 << 22                     # GPK_DIRECT_MAX_RECTS: most rectangles of one run's store
+# gpk_direct_stop: why a DIRECT run stopped
+DIRECT_RUNNING, DIRECT_MAXF, DIRECT_MAXT, DIRECT_FGLOBAL, DIRECT_MAXDEEP_HIT, DIRECT_MAXDIV_HIT = range(6)
+DIRECT_STOP_NAMES = ("running", "maxf", "maxT", "fglobal", "maxdeep", "maxdiv")
 
 _dp = C.POINTER(C.c_double)
 _ip = C.POINTER(C.c_int)
@@ -135,6 +140,11 @@ _SIGNATURES = {
                                 _dp, _vp],
     "gpk_maximize_cmaes_es_cost": [C.POINTER(_vp), C.POINTER(_vp), C.c_int, C.c_ulonglong, _dp, C.c_double, _dp, _dp,
                                    C.c_long, C.c_int, _dp, _dp, _dp, C.c_int, C.c_int, C.c_int, C.c_double, _vp],
+    "gpk_maximize_direct": [C.POINTER(_vp), C.c_int, C.c_int, _dp, C.c_double, _dp, _dp, C.c_long, C.c_int, _vp, _lp],
+    "gpk_maximize_direct_es": [C.POINTER(_vp), C.c_int, _dp, _dp, C.c_long, C.c_int, _vp],
+    "gpk_maximize_direct_esmc": [C.POINTER(_vp), C.c_int, _dp, _dp, C.c_long, C.c_int, _vp],
+    "gpk_maximize_direct_es_cost": [C.POINTER(_vp), C.POINTER(_vp), C.c_int, _dp, _dp, C.c_long, C.c_int, _dp, _dp,
+                                    C.c_int, C.c_int, C.c_int, C.c_double, _vp],
     "gpk_cmaes_draws": [_vp, C.c_ulonglong, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _dp],
     "gpk_sample_representers": [C.POINTER(_vp), C.c_int, C.POINTER(C.c_ulonglong), C.c_int, C.c_int, C.c_int, C.c_int,
                                 _dp, C.c_double, _dp, _dp, C.c_int, C.c_int, _dp, _dp, C.c_int, C.c_double, _dp, _dp,
@@ -1097,6 +1107,77 @@ def cmaes_draws(handle, seed, run, g0, g1, lam, d):
     handle._check(handle.lib.gpk_cmaes_draws(handle._h, int(seed) & 0xFFFFFFFFFFFFFFFF, int(run), int(g0), int(g1),
                                              int(lam), int(d), _as_dp(out)))
     return out
+
+
+class _DirectResult(C.Structure):
+    _fields_ = [(name, _vp) for name in ("best_x", "best_energy", "nit", "nfev", "stop", "rows")]
+
+
+def _direct_io(lower, upper, n_iters):
+    lo, up = f64(lower).ravel(), f64(upper).ravel()
+    if lo.size != up.size:
+        raise ValueError("maximize_direct: lower and upper need d entries each")
+    outs = dict(best_x=np.empty(lo.size), best_energy=np.empty(1), nit=np.zeros(1, dtype=np.intc),
+                nfev=np.zeros(1, dtype=np.int_), stop=np.zeros(1, dtype=np.intc),
+                rows=np.zeros(max(int(n_iters) - 1, 1), dtype=np.int_))
+    res = _DirectResult(*[outs[k].ctypes.data for k, _ in _DirectResult._fields_])
+    return lo, up, outs, res
+
+
+def _direct_result(outs):
+    nit, stop = int(outs["nit"][0]), int(outs["stop"][0])
+    sampled = max(nit - 1 - (stop == DIRECT_MAXT), 0)            # iterations 2 .. nit, the last one not under maxT
+    return dict(x=outs["best_x"], energy=float(outs["best_energy"][0]), nit=nit, nfev=int(outs["nfev"][0]),
+                stop=stop, rows=outs["rows"][:sampled].astype(np.int64))
+
+
+def maximize_direct(handles, kind, eta, par, lower, upper, n_func_evals=400, n_iters=200):
+    """gpk_maximize_direct over ``handles`` (all fitted, same device): DIRECT in the box lower / upper (d,) minimising
+    -acq (kind ACQ_EI ... ACQ_LCB, acq the mean over the handles) -> dict(x (d,), energy, nit, nfev, stop, rows (the
+    rows of iterations 2 .. nit), n_negative)."""
+    h0 = handles[0]
+    lo, up, outs, res = _direct_io(lower, upper, n_iters)
+    nn = C.c_long()
+    h0._check(h0.lib.gpk_maximize_direct(_handles(handles), len(handles), int(kind), _as_dp(_etas(eta, len(handles))),
+                                         float(par), _as_dp(lo), _as_dp(up), int(n_func_evals), int(n_iters),
+                                         C.byref(res), C.byref(nn)))
+    r = _direct_result(outs)
+    r["n_negative"] = nn.value
+    return r
+
+
+def maximize_direct_es(objective, lower, upper, n_func_evals=400, n_iters=200):
+    """gpk_maximize_direct_es: the same minimising minus the entropy change -> as maximize_direct without n_negative."""
+    h0 = objective[0]
+    lo, up, outs, res = _direct_io(lower, upper, n_iters)
+    h0._check(h0.lib.gpk_maximize_direct_es(_handles(objective), len(objective), _as_dp(lo), _as_dp(up),
+                                            int(n_func_evals), int(n_iters), C.byref(res)))
+    return _direct_result(outs)
+
+
+def maximize_direct_esmc(objective, lower, upper, n_func_evals=400, n_iters=200):
+    """gpk_maximize_direct_esmc: the same minimising minus the sampling-based entropy change."""
+    h0 = objective[0]
+    lo, up, outs, res = _direct_io(lower, upper, n_iters)
+    h0._check(h0.lib.gpk_maximize_direct_esmc(_handles(objective), len(objective), _as_dp(lo), _as_dp(up),
+                                              int(n_func_evals), int(n_iters), C.byref(res)))
+    return _direct_result(outs)
+
+
+def maximize_direct_es_cost(objective, cost, lower, upper, cfg_lower, cfg_upper, basis_objective, basis_cost,
+                            overhead, n_func_evals=400, n_iters=200):
+    """gpk_maximize_direct_es_cost: the same over the extended box lower / upper (d) minimising minus the information
+    gain per unit cost of gpk_es_cost_multi (configuration bounds cfg_lower / cfg_upper, d - 1)."""
+    ho, hc, clo, cup = _es_cost_args(objective, cost, cfg_lower, cfg_upper)
+    h0 = objective[0]
+    lo, up, outs, res = _direct_io(lower, upper, n_iters)
+    if lo.size != clo.size + 1:
+        raise ValueError("maximize_direct_es_cost: the box needs d entries, the configuration bounds d - 1")
+    h0._check(h0.lib.gpk_maximize_direct_es_cost(ho, hc, len(objective), _as_dp(lo), _as_dp(up), int(n_func_evals),
+                                                 int(n_iters), _as_dp(clo), _as_dp(cup), clo.size,
+                                                 int(basis_objective), int(basis_cost), float(overhead),
+                                                 C.byref(res)))
+    return _direct_result(outs)
 
 
 def sample_representers(models, seeds, nb, steps, max_runs, kind, eta, par, lower, upper, fabolas=None):

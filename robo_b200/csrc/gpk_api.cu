@@ -27,6 +27,7 @@
 #include "gpk_de.cuh"
 #include "gpk_lbfgs.cuh"
 #include "gpk_cmaes.cuh"
+#include "gpk_direct.cuh"
 #include "gpk_es.cuh"
 #include "gpk_esmc.cuh"
 #include "gpk_rs.cuh"
@@ -144,6 +145,9 @@ struct gpk_handle {
     // CMA-ES (gpk_maximize_cmaes*): state, status record, constant table, bounds and x0, the Z / Y / G / P rows of a
     // generation; owned by the first handle of the call (gpk_cmaes_draws uses it as scratch)
     DevBuf cma_buf;
+    // DIRECT (gpk_maximize_direct*): state, status record, box, rectangle store, row buffer, selection; owned by the
+    // first handle of the call
+    DevBuf dir_buf;
     DevBuf ep_buf;                  // scratch of gpk_ep_joint_min (operands, raw and renormalised outputs, status)
     // entropy search (gpk_es_update / gpk_es_compute): EP state, W, bounds, scaled zb, U = K^-1 K(X, zb), per-chunk v, sigma
     DevBuf es_state, es_U, es_work, es_in;
@@ -1283,7 +1287,7 @@ int gpk_destroy(gpk_handle* h) {
                       &h->out_var, &h->out_acq, &h->block_best, &h->best, &h->nneg, &h->Vt, &h->cov, &h->XsT,
                       &h->tmpjobs, &h->alpha, &h->tmp1, &h->tmp2, &h->tmp3, &h->dprof, &h->Xts, &h->oz_Pq, &h->oz_Kq, &h->oz_Kq2, &h->oz_eP, &h->oz_emax, &h->oz_pmu2, &h->oz_probe,
                       &h->multi_cand, &h->multi_A, &h->multi_B, &h->multi_out, &h->multi_bb, &h->gather, &h->best_global,
-                      &h->de_pop, &h->de_trial, &h->de_param, &h->de_E, &h->de_small, &h->de_sort, &h->lb_buf, &h->cma_buf, &h->ep_buf, &h->es_state, &h->es_U, &h->es_work, &h->es_in, &h->mc_state, &h->mc_buf, &h->mc_stat, &h->fab_in, &h->rs_buf, &h->hy_buf};
+                      &h->de_pop, &h->de_trial, &h->de_param, &h->de_E, &h->de_small, &h->de_sort, &h->lb_buf, &h->cma_buf, &h->dir_buf, &h->ep_buf, &h->es_state, &h->es_U, &h->es_work, &h->es_in, &h->mc_state, &h->mc_buf, &h->mc_stat, &h->fab_in, &h->rs_buf, &h->hy_buf};
     for (DevBuf* b : bufs)
         if (b->p) cudaFree(b->p);
     if (h->ev_ok)

@@ -1,6 +1,7 @@
-"""What scores an acquisition on the device, shared by the device maximizers (DifferentialEvolution, SciPyOptimizer),
-and the differential-evolution, multi-start L-BFGS and CMA-ES calls over it (gpk_maximize_de*, gpk_maximize_lbfgs*,
-gpk_maximize_cmaes*)."""
+"""What scores an acquisition on the device, shared by the device maximizers (DifferentialEvolution, SciPyOptimizer,
+CMAES, Direct, GridSearch), and the differential-evolution, multi-start L-BFGS, CMA-ES and DIRECT calls over it
+(gpk_maximize_de*, gpk_maximize_lbfgs*, gpk_maximize_cmaes*, gpk_maximize_direct*) and the one-shot scoring of a
+batch (gpk_acq_multi, gpk_es_multi, gpk_esmc_multi, gpk_es_cost_multi)."""
 import numpy as np
 
 from robo_b200 import _lib
@@ -118,6 +119,29 @@ def maximize_cmaes(which, spec, seed, x0, lower, upper, n_func_evals, restarts):
                 lambda hs: _lib.maximize_cmaes_es(hs, *args),
                 lambda hs, kind, etas, par: _lib.maximize_cmaes(hs, kind, etas, par, *args),
                 lambda hs: _lib.maximize_cmaes_esmc(hs, *args))
+
+
+def maximize_direct(which, spec, lower, upper, n_func_evals, n_iters):
+    """DIRECT on the device in the box lower / upper over what ``device_spec`` returned -> _lib's result dict (x,
+    energy, nit, nfev, stop, rows)."""
+    args = (lower, upper, n_func_evals, n_iters)
+    return _run(which, spec,
+                lambda ho, hc, **cfg: _lib.maximize_direct_es_cost(ho, hc, lower, upper, n_func_evals=n_func_evals,
+                                                                   n_iters=n_iters, **cfg),
+                lambda hs: _lib.maximize_direct_es(hs, *args),
+                lambda hs, kind, etas, par: _lib.maximize_direct(hs, kind, etas, par, *args),
+                lambda hs: _lib.maximize_direct_esmc(hs, *args))
+
+
+def score_batch(which, spec, X):
+    """The one-shot value of every row of X (m, d) over what ``device_spec`` returned, with numpy's first arg-max ->
+    dict(values (m,), best_idx)."""
+    return _run(which, spec,
+                lambda ho, hc, **cfg: _lib.es_cost_multi(ho, hc, X, cfg["cfg_lower"], cfg["cfg_upper"],
+                                                         cfg["basis_objective"], cfg["basis_cost"], cfg["overhead"]),
+                lambda hs: _lib.es_multi(hs, X),
+                lambda hs, kind, etas, par: _lib.acq_multi(hs, X, 0, kind=kind, eta=etas, par=par, want_argmax=True),
+                lambda hs: _lib.esmc_multi(hs, X))
 
 
 def lbfgs_success(status):

@@ -117,6 +117,9 @@ print("lbfgs", r["nfev"], r["status"],
 r = _lib.maximize_cmaes([h], _lib.ACQ_LOG_EI, [float(y[:100].min())], 0.0, 5, rng.rand(D), np.zeros(D), np.ones(D),
                         n_func_evals=300, restarts=1)
 print("cmaes", r["nit"], r["stop"], _lib.cmaes_draws(h, 5, 1, 0, 2, 6, D).shape)
+# DIRECT: the init, select, divide and result kernels over a run that ends on its budget
+r = _lib.maximize_direct([h], _lib.ACQ_LOG_EI, [float(y[:100].min())], 0.0, np.zeros(D), np.ones(D), n_func_evals=200)
+print("direct", r["nit"], r["nfev"], _lib.DIRECT_STOP_NAMES[r["stop"]])
 h.close()
 h = _lib.moments_handle()
 print(h.acq_moments(rng.randn(100), rng.rand(100) + 0.1, _lib.ACQ_LOG_EI, 0.0, 0.0)[0][:3])
