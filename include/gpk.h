@@ -719,6 +719,49 @@ int gpk_hyper_lnpost(gpk_handle* h, const double* theta, int count, int dim, dou
 int gpk_sample_hypers(gpk_handle* h, const double* p0, int nwalkers, int dim, int steps, unsigned long long seed,
                       double* pos, double* lnpost, long* n_accepted);
 
+/* ---- Bayesian linear regression on the device (robo_b200/csrc/gpk_blr.cuh) ----------------------------------------
+ * robo/models/bayesian_linear_regression.py with its default prior (robo/priors/bayesian_linear_regression_prior.py).
+ * A handle becomes a BLR handle with gpk_blr_set_data and stays one: the Gaussian-process entry points (gpk_set_data,
+ * gpk_set_kernel, gpk_set_input_bounds, gpk_set_output_transform, gpk_fit*, the hyper sampler, gpk_predict_grad,
+ * gpk_predict_cov / gpk_posterior_cov / gpk_predict_mean*, gpk_kernel_matrix, gpk_nll_grad, the introspection calls,
+ * ES / ESMC / ES_COST and gpk_sample_representers) return GPK_BAD_ARG with a message naming the model kind.  The
+ * scoring entry points (gpk_acq, gpk_acq_dev, gpk_predict, gpk_maximize_random and every entry point over several
+ * models with an EI / LogEI / PI / LCB or posterior objective: gpk_acq_multi, gpk_maximize_de, gpk_maximize_lbfgs,
+ * gpk_maximize_cmaes, gpk_maximize_direct) score a fitted BLR handle through its predictive pass. */
+#define GPK_BLR_MAX_F 64       /* most features: linear D <= 63, quadratic D <= 31, none D <= 64 */
+typedef enum {
+    GPK_BLR_LINEAR = 0,        /* phi(x) = [x, 1]       linear_basis_func    (bayesian_linear_regression.py:11-12) */
+    GPK_BLR_QUADRATIC = 1,     /* phi(x) = [x^2, x, 1]  quadratic_basis_func (:15-17)                           */
+    GPK_BLR_NONE = 2           /* phi(x) = x            basis_func=None (:154-157)                              */
+} gpk_blr_basis;
+/* gpk_blr_set_data: X (n x d) and y (n) as train() receives them (:152-160); Phi (n x F) is built on the device, and
+ *   Phi^T Phi and Phi^T y are formed once, each entry a fixed-order reduction.  Drops the weight posteriors.  prior_par
+ *   = lognormal sigma, lognormal mean (scipy's loc), horseshoe scale (BayesianLinearRegressionPrior: 0.1, -10, 0.1).
+ *   GPK_BAD_ARG: an unknown basis, F > GPK_BLR_MAX_F, a handle that holds a Gaussian-process model.
+ * gpk_blr_lnpost: marginal_log_likelihood (:76-113) of count thetas = (log alpha, log beta) (count x 2), one CTA each,
+ *   NaN -> -inf: the values gpk_blr_sample sees, bit for bit.  The quirks are kept: the 2-norm of the residual, not its
+ *   square (:108); log det A taken as +inf / -inf where numpy's det overflows / underflows (:110); the prior
+ *   lognorm.logpdf(theta_0, sigma, loc) + Horseshoe(scale).lnprob(1 / theta_1) (prior :45-49).  A pivot that is not > 0
+ *   gives -inf where the reference's inv raises LinAlgError.
+ * gpk_blr_sample: one EnsembleSampler.run_mcmc(p0, steps) (:162-188 through emcee 2.x, a = 2) of nwalkers x 2 walkers:
+ *   one launch for the initial log-posteriors, one per half-step, keyed by `seed` (Philox4x32-10, gpk_blr.cuh).  Out:
+ *   pos (nwalkers x 2), lnpost (nwalkers), n_accepted (nwalkers, may be NULL), back in one transfer at the end.
+ *   GPK_BAD_ARG: no data, an odd number of walkers or fewer than 4, steps < 0.
+ * gpk_blr_fit: the k weight posteriors (:197-210) of hypers (k x 2, (alpha, beta) rows, not logs), resident for the
+ *   predictive pass: m_i and L_i^-1 of A_i = beta_i Phi^T Phi + alpha_i I.  GPK_NOT_PD when a pivot of some A_i is not
+ *   > 0 (the reference's inv raises LinAlgError or returns a useless inverse).
+ * gpk_blr_get_models: the fit's m (k x F) and S = A^-1 (k x F x F) for `models`; dims: n, F, k.
+ * The predictive pass (predict, :213-254): mu_i = phi^T m_i, var_i = 1 / beta_i + ||L_i^-1 phi||^2, their sums over i
+ * in order divided by k, var clipped to DBL_EPSILON, then the acquisition closed form of gpk_acq_moments (hyper-samples
+ * averaged before the closed form, the reference's BLR semantics). */
+int gpk_blr_set_data(gpk_handle* h, const double* X, const double* y, int n, int d, int basis, const double* prior_par);
+int gpk_blr_lnpost(gpk_handle* h, const double* thetas, int count, double* out);
+int gpk_blr_sample(gpk_handle* h, unsigned long long seed, int nwalkers, const double* p0, int steps, double* pos,
+                   double* lnpost, long* n_accepted);
+int gpk_blr_fit(gpk_handle* h, const double* hypers, int k);
+int gpk_blr_get_models(gpk_handle* h, double* m, double* S);
+int gpk_blr_dims(gpk_handle* h, int* n, int* F, int* k);
+
 /* kernel.get_value(X1, X2) (test/test_models/test_gaussian_process.py:44-46) with the
  * handle's current kernel; no input scaling.  out is (n1, n2) row-major. */
 int gpk_kernel_matrix(gpk_handle* h, const double* X1, long n1, const double* X2, long n2,

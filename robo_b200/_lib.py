@@ -27,6 +27,8 @@ BASIS_S, BASIS_ONE_MINUS_S_SQ = range(2)      # gpk_basis: the environment colum
 PRIOR_NONE, PRIOR_DEFAULT, PRIOR_ENV = range(3)   # gpk_prior_kind: the hyper-priors gpk_sample_hypers restates
 HYPER_MAX_N = 232                              # GPK_HYPER_MAX_N: most training points of gpk_sample_hypers
 HYPER_MAX_DIM = 96                             # GPK_HYPER_MAX_DIM: most entries of theta (log noise included)
+BLR_LINEAR, BLR_QUADRATIC, BLR_NONE = range(3)  # gpk_blr_basis: the features of a BayesianLinearRegression handle
+BLR_MAX_F = 64                                 # GPK_BLR_MAX_F: most features of a BayesianLinearRegression handle
 CMA_MAX_D, CMA_MAX_LAMBDA, CMA_HIST = 64, 2048, 160   # GPK_CMA_MAX_D / GPK_CMA_MAX_LAMBDA / GPK_CMA_HIST
 CMA_C_W = 20                                   # GPK_CMA_C_W: where a run's weights start in its constant row
 CMA_NCONST = CMA_C_W + CMA_MAX_LAMBDA // 2     # GPK_CMA_NCONST: doubles per run in the constant table
@@ -152,6 +154,12 @@ _SIGNATURES = {
     "gpk_set_hyper_model": [_vp, C.c_int, _ip, _ip, C.c_int, C.c_double, C.c_double, C.c_int, _dp, C.c_int, C.c_int],
     "gpk_hyper_lnpost": [_vp, _dp, C.c_int, C.c_int, _dp, _dp],
     "gpk_sample_hypers": [_vp, _dp, C.c_int, C.c_int, C.c_int, C.c_ulonglong, _dp, _dp, _lp],
+    "gpk_blr_set_data": [_vp, _dp, _dp, C.c_int, C.c_int, C.c_int, _dp],
+    "gpk_blr_lnpost": [_vp, _dp, C.c_int, _dp],
+    "gpk_blr_sample": [_vp, C.c_ulonglong, C.c_int, _dp, C.c_int, _dp, _dp, _lp],
+    "gpk_blr_fit": [_vp, _dp, C.c_int],
+    "gpk_blr_get_models": [_vp, _dp, _dp],
+    "gpk_blr_dims": [_vp, _ip, _ip, _ip],
     "gpk_get_timings": [_vp, _dp],
     "gpk_get_diag_profile": [_vp, C.POINTER(C.c_longlong)],
 }
@@ -1259,6 +1267,63 @@ def sample_hypers(handle, p0, steps, seed):
     handle._check(handle.lib.gpk_sample_hypers(handle._h, _as_dp(P), nw, dim, int(steps), int(seed) & 0xFFFFFFFFFFFFFFFF,
                                                _as_dp(pos), _as_dp(lnp), acc.ctypes.data_as(_lp)))
     return dict(pos=pos, lnpost=lnp, n_accepted=acc)
+
+
+def blr_features(n_dims, basis):
+    """F, the number of features of a BayesianLinearRegression handle on n_dims inputs."""
+    return {BLR_LINEAR: n_dims + 1, BLR_QUADRATIC: 2 * n_dims + 1, BLR_NONE: n_dims}[basis]
+
+
+def blr_set_data(handle, X, y, basis, prior_par):
+    """gpk_blr_set_data: the training set and its features (basis: BLR_*) on the handle, which becomes a
+    BayesianLinearRegression handle; prior_par = (lognormal sigma, lognormal mean, horseshoe scale)."""
+    X, y, par = f64(X), f64(y).ravel(), f64(prior_par).ravel()
+    n, d = X.shape
+    if par.size != 3:
+        raise ValueError("blr_set_data: the prior needs 3 constants")
+    handle._check(handle.lib.gpk_blr_set_data(handle._h, _as_dp(X), _as_dp(y), n, d, int(basis), _as_dp(par)))
+
+
+def blr_lnpost(handle, thetas):
+    """gpk_blr_lnpost: the log-posterior (marginal log-likelihood plus prior, NaN -> -inf) of every row of thetas
+    (count, 2) = (log alpha, log beta), as gpk_blr_sample computes it."""
+    T = f64(np.atleast_2d(thetas))
+    if T.ndim != 2 or T.shape[1] != 2:
+        raise ValueError("blr_lnpost: thetas must have shape (count, 2)")
+    out = np.empty(T.shape[0])
+    handle._check(handle.lib.gpk_blr_lnpost(handle._h, _as_dp(T), T.shape[0], _as_dp(out)))
+    return out
+
+
+def blr_sample(handle, seed, p0, steps):
+    """gpk_blr_sample: one stretch-move run of the walkers p0 (nwalkers, 2) for `steps` steps ->
+    dict(pos (nwalkers, 2), lnpost (nwalkers,), n_accepted (nwalkers,))."""
+    P = f64(np.atleast_2d(p0))
+    if P.ndim != 2 or P.shape[1] != 2:
+        raise ValueError("blr_sample: p0 must have shape (nwalkers, 2)")
+    nw = P.shape[0]
+    pos, lnp = np.empty((nw, 2)), np.empty(nw)
+    acc = np.zeros(nw, dtype=np.int64)
+    handle._check(handle.lib.gpk_blr_sample(handle._h, int(seed) & 0xFFFFFFFFFFFFFFFF, nw, _as_dp(P), int(steps),
+                                            _as_dp(pos), _as_dp(lnp), acc.ctypes.data_as(_lp)))
+    return dict(pos=pos, lnpost=lnp, n_accepted=acc)
+
+
+def blr_fit(handle, hypers):
+    """gpk_blr_fit: the weight posteriors of the (alpha, beta) rows of hypers, resident on the handle."""
+    H = f64(np.atleast_2d(hypers))
+    if H.ndim != 2 or H.shape[1] != 2:
+        raise ValueError("blr_fit: hypers must have shape (k, 2)")
+    handle._check(handle.lib.gpk_blr_fit(handle._h, _as_dp(H), H.shape[0]))
+
+
+def blr_models(handle):
+    """gpk_blr_get_models: [(m (F,), S (F, F))] of the last gpk_blr_fit."""
+    n, F, k = C.c_int(), C.c_int(), C.c_int()
+    handle._check(handle.lib.gpk_blr_dims(handle._h, C.byref(n), C.byref(F), C.byref(k)))
+    M, S = np.empty((k.value, F.value)), np.empty((k.value, F.value, F.value))
+    handle._check(handle.lib.gpk_blr_get_models(handle._h, _as_dp(M), _as_dp(S)))
+    return [(M[i].copy(), S[i].copy()) for i in range(k.value)]
 
 
 _moments_handle = {}

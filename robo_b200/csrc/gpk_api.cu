@@ -32,6 +32,7 @@
 #include "gpk_esmc.cuh"
 #include "gpk_rs.cuh"
 #include "gpk_hyper.cuh"
+#include "gpk_blr.cuh"
 
 namespace {
 
@@ -161,6 +162,14 @@ struct gpk_handle {
     bool has_hyper = false;
     HyperModel hyper;
     DevBuf hy_buf;
+    // Bayesian linear regression (gpk_blr.cuh): set once by gpk_blr_set_data, after which the handle serves the BLR
+    // entry points and the scoring ones only.  blr_data: Phi (n x F), y, G = Phi^T Phi, b = Phi^T y; blr_post: the fit's
+    // M (k x F), L^-1 and S (k x F x F each), 1 / beta (k), failure flags; blr_work: thetas / walkers and their values;
+    // blr_bb: the predictive pass's block arg-max pairs
+    bool blr = false, blr_fitted = false;
+    int blr_basis = 0, blr_F = 0, blr_k = 0;
+    BlrPrior blr_prior;
+    DevBuf blr_data, blr_post, blr_work, blr_bb;
     int es_nb = 0, es_np = 0;
     double es_sn2 = 0.0, es_H = 0.0;
     long es_linv_serial = -1;       // linv_serial U was built for (-1: no update yet)
@@ -734,12 +743,26 @@ __global__ void gpk_resid_kernel(const double* __restrict__ y, double mean, int 
     if (i < NP) out[i] = (i < n) ? y[i] - mean : 0.0;
 }
 
+// the message of every Gaussian-process entry point called with a BLR handle
+#define BLR_REFUSAL "the handle holds a Bayesian linear regression model (gpk_blr_set_data); this entry point serves " \
+                    "Gaussian-process handles only"
+
 int require(gpk_handle* h, bool data, bool spec, bool fitted) {
     if (!h) return GPK_BAD_ARG;
+    if (h->blr) { set_err(h, BLR_REFUSAL); return GPK_BAD_ARG; }
     if (data && !h->has_data) { set_err(h, "gpk_set_data has not been called"); return GPK_BAD_ARG; }
     if (spec && !h->has_spec) { set_err(h, "gpk_set_kernel has not been called"); return GPK_BAD_ARG; }
     if (fitted && !h->fitted) { set_err(h, "model is not fitted (gpk_fit)"); return GPK_NOT_FITTED; }
     return GPK_OK;
+}
+
+// the preconditions of the entry points that score either model kind: a fitted GP, or a BLR handle after gpk_blr_fit
+int require_model(gpk_handle* h) {
+    if (h && h->blr) {
+        if (!h->blr_fitted) { set_err(h, "model is not fitted (gpk_blr_fit)"); return GPK_NOT_FITTED; }
+        return GPK_OK;
+    }
+    return require(h, true, true, true);
 }
 
 // L^-1 by recursive block inversion (P lower, Q = P^T upper), after a successful fit.
@@ -863,9 +886,16 @@ struct Feeder {
 // index_offset: position of dX[0] in the caller's batch (offset into the output arrays and into the arg-max index);
 // global_base: added to the arg-max index only (first index of this rank's shard in a sharded batch); reset: start a
 // new running arg-max / negative-EI count (false when a host batch is fed in several pieces)
+int blr_score(gpk_handle* h, const double* dX, long m, int kind, double eta, double par, double* d_out, double* d_mu,
+              double* d_var, BestPair* d_best, unsigned long long* d_nneg, long index_offset, bool reset, long global_base,
+              Feeder* feeder);
+
 int score_dev(gpk_handle* h, const double* dX, long m, int kind, double eta, double par, double* d_out,
               double* d_mu, double* d_var, BestPair* d_best, unsigned long long* d_nneg,
               long index_offset = 0, bool reset = true, long global_base = 0, Feeder* feeder = nullptr) {
+    if (h->blr)
+        return blr_score(h, dX, m, kind, eta, par, d_out, d_mu, d_var, d_best, d_nneg, index_offset, reset, global_base,
+                         feeder);
     int rc = build_linv(h);
     if (rc) return rc;
     const long NP = h->NP;
@@ -1134,6 +1164,7 @@ int es_dh_dev(gpk_handle* h, const double* Xm, const double* Xb, long m, double*
 int es_ready(gpk_handle* h, gpk_handle* report, const char* who, int kind = ES_KIND_EP) {
     gpk_handle* r = report ? report : h;
     const char* upd = kind == ES_KIND_MC ? "gpk_esmc_update" : "gpk_es_update";
+    if (h->blr) { set_err(r, "%s: " BLR_REFUSAL, who); return GPK_BAD_ARG; }
     if (h->es_linv_serial < 0) { set_err(r, "%s: call %s first", who, upd); return GPK_BAD_ARG; }
     if (!h->linv_ready || h->es_linv_serial != h->linv_serial) {
         set_err(r, "%s: the model changed since %s", who, upd);
@@ -1231,6 +1262,80 @@ int esmc_dev(gpk_handle* h, const double* X, long m, double* d_out, int* d_stat)
     return GPK_OK;
 }
 
+// the layout of h->blr_data (doubles): Phi (n x F), y (n), G (F x F), b (F)
+inline double* blr_phi(gpk_handle* h) { return ptr<double>(h->blr_data); }
+inline double* blr_y(gpk_handle* h) { return blr_phi(h) + (size_t)h->n * h->blr_F; }
+inline double* blr_G(gpk_handle* h) { return blr_y(h) + h->n; }
+inline double* blr_b(gpk_handle* h) { return blr_G(h) + (size_t)h->blr_F * h->blr_F; }
+
+// the layout of h->blr_post (doubles) for k posteriors: M (k x F), L^-1 (k x F x F), S (k x F x F), 1 / beta (k), then
+// k int failure flags
+struct BlrPost {
+    size_t M, Li, S, ib, fail, total;
+    BlrPost(int k, int F) {
+        const size_t FF = (size_t)F * F;
+        M = 0; Li = M + (size_t)k * F; S = Li + k * FF; ib = S + k * FF; fail = ib + k;
+        total = fail * 8 + (size_t)k * 4;
+    }
+};
+
+int blr_ready(gpk_handle* h, const char* who) {
+    if (!h) return GPK_BAD_ARG;
+    if (!h->blr) BAD("%s: gpk_blr_set_data has not been called", who);
+    CK(cudaSetDevice(h->device));
+    const int sm_eval = (int)(gpk_blr_smem_doubles(h->blr_F) * 8);
+    CK(cudaFuncSetAttribute(gpk_blr_eval_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, sm_eval));
+    CK(cudaFuncSetAttribute(gpk_blr_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, sm_eval));
+    CK(cudaFuncSetAttribute(gpk_blr_fit_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                            sm_eval + h->blr_F * h->blr_F * 8));
+    CK(cudaFuncSetAttribute(gpk_blr_score_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                            h->blr_F * GPK_BLR_SCORE_THREADS * 8));
+    return GPK_OK;
+}
+
+// score_dev for a BLR handle: the predictive pass of gpk_blr_score_kernel over the m rows dX, with score_dev's outputs,
+// offsets and running arg-max
+int blr_score(gpk_handle* h, const double* dX, long m, int kind, double eta, double par, double* d_out, double* d_mu,
+              double* d_var, BestPair* d_best, unsigned long long* d_nneg, long index_offset, bool reset, long global_base,
+              Feeder* feeder) {
+    int rc;
+    if ((rc = blr_ready(h, "scoring"))) return rc;
+    const int nblk = (int)((m + GPK_BLR_SCORE_THREADS - 1) / GPK_BLR_SCORE_THREADS);
+    if ((rc = ensure(h, h->blr_bb, (size_t)std::max(nblk, 1) * sizeof(BestPair)))) return rc;
+    if ((rc = ensure(h, h->best, sizeof(BestPair)))) return rc;
+    if ((rc = ensure(h, h->nneg, 8))) return rc;
+    if (d_best == nullptr) d_best = ptr<BestPair>(h->best);
+    if (d_nneg == nullptr) d_nneg = ptr<unsigned long long>(h->nneg);
+    if (reset) {
+        CK(cudaMemsetAsync(d_best, 0xFF, sizeof(BestPair), h->stream));
+        CK(cudaMemsetAsync(d_nneg, 0, 8, h->stream));
+    }
+    if (feeder && (rc = feeder->ready(0, m, h->stream))) return rc;
+    const int F = h->blr_F, k = h->blr_k;
+    const BlrPost L(k, F);
+    double* post = ptr<double>(h->blr_post);
+    BlrScoreArgs a;
+    memset(&a, 0, sizeof(a));
+    a.X = dX; a.m = m; a.D = h->d; a.F = F; a.basis = h->blr_basis; a.k = k;
+    a.M = post + L.M; a.Li = post + L.Li; a.ib = post + L.ib;
+    a.base = global_base + index_offset;
+    a.acq_kind = kind; a.eta = eta; a.par = par;
+    a.out_mu = d_mu ? d_mu + index_offset : nullptr;
+    a.out_var = d_var ? d_var + index_offset : nullptr;
+    a.out_acq = d_out ? d_out + index_offset : nullptr;
+    a.block_best = ptr<BestPair>(h->blr_bb);
+    a.n_negative = d_nneg;
+    if (m > 0) {
+        gpk_blr_score_kernel<<<nblk, GPK_BLR_SCORE_THREADS, (size_t)F * GPK_BLR_SCORE_THREADS * 8, h->stream>>>(a);
+        CKL();
+        if (kind != GPK_ACQ_NONE) {
+            gpk_argmax_final_kernel<<<1, 256, 0, h->stream>>>(ptr<BestPair>(h->blr_bb), nblk, d_best);
+            CKL();
+        }
+    }
+    return GPK_OK;
+}
+
 }  // namespace
 
 // =============================================================================================
@@ -1287,7 +1392,8 @@ int gpk_destroy(gpk_handle* h) {
                       &h->out_var, &h->out_acq, &h->block_best, &h->best, &h->nneg, &h->Vt, &h->cov, &h->XsT,
                       &h->tmpjobs, &h->alpha, &h->tmp1, &h->tmp2, &h->tmp3, &h->dprof, &h->Xts, &h->oz_Pq, &h->oz_Kq, &h->oz_Kq2, &h->oz_eP, &h->oz_emax, &h->oz_pmu2, &h->oz_probe,
                       &h->multi_cand, &h->multi_A, &h->multi_B, &h->multi_out, &h->multi_bb, &h->gather, &h->best_global,
-                      &h->de_pop, &h->de_trial, &h->de_param, &h->de_E, &h->de_small, &h->de_sort, &h->lb_buf, &h->cma_buf, &h->dir_buf, &h->ep_buf, &h->es_state, &h->es_U, &h->es_work, &h->es_in, &h->mc_state, &h->mc_buf, &h->mc_stat, &h->fab_in, &h->rs_buf, &h->hy_buf};
+                      &h->de_pop, &h->de_trial, &h->de_param, &h->de_E, &h->de_small, &h->de_sort, &h->lb_buf, &h->cma_buf, &h->dir_buf, &h->ep_buf, &h->es_state, &h->es_U, &h->es_work, &h->es_in, &h->mc_state, &h->mc_buf, &h->mc_stat, &h->fab_in, &h->rs_buf, &h->hy_buf,
+                      &h->blr_data, &h->blr_post, &h->blr_work, &h->blr_bb};
     for (DevBuf* b : bufs)
         if (b->p) cudaFree(b->p);
     if (h->ev_ok)
@@ -1396,6 +1502,7 @@ int gpk_synchronize(gpk_handle* h) {
 
 int gpk_set_data(gpk_handle* h, const double* X, const double* y, int n, int d) {
     if (!h) return GPK_BAD_ARG;
+    if (h->blr) BAD("gpk_set_data: " BLR_REFUSAL);
     if (!X || !y || n <= 0 || d <= 0) BAD("gpk_set_data: need X, y, n > 0, d > 0");
     if (d > GPK_MAX_TERMS) BAD("gpk_set_data: d = %d exceeds GPK_MAX_TERMS = %d", d, GPK_MAX_TERMS);
     CK(cudaSetDevice(h->device));
@@ -1441,6 +1548,7 @@ int gpk_set_data(gpk_handle* h, const double* X, const double* y, int n, int d) 
 
 int gpk_set_input_bounds(gpk_handle* h, const double* lower, const double* upper, int d) {
     if (!h) return GPK_BAD_ARG;
+    if (h->blr) BAD("gpk_set_input_bounds: " BLR_REFUSAL);
     CK(cudaSetDevice(h->device));
     if (!lower || !upper) { h->has_bounds = false; return GPK_OK; }
     if (d <= 0 || d > GPK_MAX_TERMS) BAD("gpk_set_input_bounds: bad d");
@@ -1456,6 +1564,7 @@ int gpk_set_input_bounds(gpk_handle* h, const double* lower, const double* upper
 
 int gpk_set_output_transform(gpk_handle* h, int enabled, double y_mean, double y_std) {
     if (!h) return GPK_BAD_ARG;
+    if (h->blr) BAD("gpk_set_output_transform: " BLR_REFUSAL);
     h->norm_out = enabled ? 1 : 0;
     h->y_mean = y_mean;
     h->y_std = y_std;
@@ -1465,6 +1574,7 @@ int gpk_set_output_transform(gpk_handle* h, int enabled, double y_mean, double y
 int gpk_set_kernel(gpk_handle* h, int family, double log_amp, int n_terms, const int* axis, const int* group,
                    const double* log_metric) {
     if (!h) return GPK_BAD_ARG;
+    if (h->blr) BAD("gpk_set_kernel: " BLR_REFUSAL);
     if (family < GPK_MATERN52 || family > GPK_MATERN32) BAD("gpk_set_kernel: unknown family %d", family);
     if (n_terms <= 0 || n_terms > GPK_MAX_TERMS || !axis || !group || !log_metric)
         BAD("gpk_set_kernel: need 1..%d terms", GPK_MAX_TERMS);
@@ -1653,6 +1763,7 @@ int gpk_fit(gpk_handle* h, double diag_add, double mean, double* logdet, double*
 int gpk_fit_append(gpk_handle* h, const double* X, const double* y, int n, int d, double diag_add, double mean,
                    double* logdet, double* loglik) {
     if (!h) return GPK_BAD_ARG;
+    if (h->blr) BAD("gpk_fit_append: " BLR_REFUSAL);
     if (!X || !y || n <= 0 || d <= 0) BAD("gpk_fit_append: need X, y, n > 0, d > 0");
     const long NP = h->NP;
     const int nb = h->nb, b = nb - 1, N1 = b * BM;
@@ -1779,7 +1890,7 @@ int gpk_fit_append(gpk_handle* h, const double* X, const double* y, int n, int d
 
 int gpk_acq_dev(gpk_handle* h, const void* d_Xs, long m, int kind, double eta, double par, void* d_out, void* d_mu,
                 void* d_var, void* d_best) {
-    int rc = require(h, true, true, true);
+    int rc = require_model(h);
     if (rc) return rc;
     if (!d_Xs || m <= 0) BAD("gpk_acq_dev: need candidates");
     if (kind < GPK_ACQ_NONE || kind > GPK_ACQ_LCB) BAD("gpk_acq_dev: unknown acquisition %d", kind);
@@ -1850,7 +1961,7 @@ struct HostFeeder : Feeder {
 
 int gpk_acq(gpk_handle* h, const double* Xs, long m, int kind, double eta, double par, double* out, double* mu,
             double* var, double* best_val, long* best_idx, long* n_negative) {
-    int rc = require(h, true, true, true);
+    int rc = require_model(h);
     if (rc) return rc;
     if (!Xs || m <= 0) BAD("gpk_acq: need candidates");
     if (kind < GPK_ACQ_NONE || kind > GPK_ACQ_LCB) BAD("gpk_acq: unknown acquisition %d", kind);
@@ -1936,7 +2047,7 @@ int gpk_generate_candidates(gpk_handle* h, unsigned long long seed, long first, 
 int gpk_maximize_random(gpk_handle* h, unsigned long long seed, long first, long count, long n_uniform,
                         const double* lower, const double* upper, const double* incumbent, double scale, int kind,
                         double eta, double par, double* best_x, double* best_val, long* best_idx) {
-    int rc = require(h, true, true, true);
+    int rc = require_model(h);
     if (rc) return rc;
     if (!lower || !upper || !incumbent || count <= 0 || first < 0) BAD("gpk_maximize_random: bad arguments");
     if (kind < GPK_ACQ_EI || kind > GPK_ACQ_LCB) BAD("gpk_maximize_random: unknown acquisition %d", kind);
@@ -2219,6 +2330,7 @@ int gpk_set_hyper_model(gpk_handle* h, int n_params, const int* amp_slot, const 
                         double mean, double tiny, int prior_kind, const double* prior_par, int n_ls, int n_lr) {
     if (!h) return GPK_BAD_ARG;
     const char* who = "gpk_set_hyper_model";
+    if (h->blr) BAD("%s: " BLR_REFUSAL, who);
     h->has_hyper = false;
     if (!h->has_spec) BAD("%s: gpk_set_kernel has not been called", who);
     if (n_params < 1 || n_params + 1 > GPK_HYPER_MAX_DIM || !amp_slot || !term_param)
@@ -2341,6 +2453,146 @@ int gpk_sample_hypers(gpk_handle* h, const double* p0, int nwalkers, int dim, in
     memcpy(pos, out.data(), nP * 8);
     memcpy(lnpost, out.data() + nP, (size_t)nwalkers * 8);
     if (n_accepted) memcpy(n_accepted, out.data() + nP + nwalkers, (size_t)nwalkers * 8);
+    return GPK_OK;
+}
+
+// ---------------------------------------------------------------------------------------
+// Bayesian linear regression (gpk_blr.cuh; robo/models/bayesian_linear_regression.py)
+// ---------------------------------------------------------------------------------------
+int gpk_blr_set_data(gpk_handle* h, const double* X, const double* y, int n, int d, int basis, const double* prior_par) {
+    if (!h) return GPK_BAD_ARG;
+    const char* who = "gpk_blr_set_data";
+    if (!h->blr && (h->has_data || h->has_spec))
+        BAD("%s: the handle holds a Gaussian-process model; use a new handle for Bayesian linear regression", who);
+    if (!X || !y || !prior_par || n <= 0 || d <= 0) BAD("%s: need X, y, prior_par, n > 0, d > 0", who);
+    if (basis < GPK_BLR_LINEAR || basis > GPK_BLR_NONE) BAD("%s: unknown basis %d", who, basis);
+    const long F = basis == GPK_BLR_LINEAR ? (long)d + 1 : basis == GPK_BLR_QUADRATIC ? 2L * d + 1 : d;
+    if (F > GPK_BLR_MAX_F)
+        BAD("%s: %ld features (d = %d) exceed GPK_BLR_MAX_F = %d", who, F, d, GPK_BLR_MAX_F);
+    CK(cudaSetDevice(h->device));
+    int rc;
+    h->blr = true;
+    h->blr_fitted = false;
+    h->n = n; h->d = d; h->blr_F = (int)F; h->blr_basis = basis;
+    h->blr_prior.ln_sigma = prior_par[0]; h->blr_prior.ln_loc = prior_par[1]; h->blr_prior.hs_scale = prior_par[2];
+    if ((rc = ensure(h, h->blr_data, ((size_t)n * F + n + F * F + F) * 8))) return rc;
+    if ((rc = ensure(h, h->cand, (size_t)n * d * 8))) return rc;
+    CK(cudaMemcpyAsync(h->cand.p, X, (size_t)n * d * 8, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(blr_y(h), y, (size_t)n * 8, cudaMemcpyHostToDevice, h->stream));
+    gpk_blr_phi_kernel<<<(n + 255) / 256, 256, 0, h->stream>>>(ptr<double>(h->cand), n, d, (int)F, basis, blr_phi(h));
+    CKL();
+    gpk_blr_gram_kernel<<<(unsigned)(F * F + F), 256, 0, h->stream>>>(blr_phi(h), blr_y(h), n, (int)F, blr_G(h), blr_b(h));
+    CKL();
+    CK(cudaStreamSynchronize(h->stream));     // host buffers are caller-owned: done with them
+    h->has_data = true;
+    return GPK_OK;
+}
+
+int gpk_blr_lnpost(gpk_handle* h, const double* thetas, int count, double* out) {
+    const char* who = "gpk_blr_lnpost";
+    int rc = blr_ready(h, who);
+    if (rc) return rc;
+    if (count < 1 || !thetas || !out) BAD("%s: need count >= 1, thetas and out", who);
+    if ((rc = ensure(h, h->blr_work, (size_t)count * 3 * 8))) return rc;
+    double* dT = ptr<double>(h->blr_work);
+    double* dv = dT + 2 * (size_t)count;
+    CK(cudaMemcpyAsync(dT, thetas, (size_t)count * 2 * 8, cudaMemcpyHostToDevice, h->stream));
+    gpk_blr_eval_kernel<<<count, GPK_BLR_THREADS, gpk_blr_smem_doubles(h->blr_F) * 8, h->stream>>>(
+        blr_phi(h), blr_y(h), blr_G(h), blr_b(h), h->n, h->blr_F, h->blr_prior, dT, dv);
+    CKL();
+    CK(cudaMemcpyAsync(out, dv, (size_t)count * 8, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    return GPK_OK;
+}
+
+int gpk_blr_sample(gpk_handle* h, unsigned long long seed, int nwalkers, const double* p0, int steps, double* pos,
+                   double* lnpost, long* n_accepted) {
+    static_assert(sizeof(long) == sizeof(long long) && sizeof(long long) == sizeof(double),
+                  "the accept counts travel in the walkers' transfer");
+    const char* who = "gpk_blr_sample";
+    int rc = blr_ready(h, who);
+    if (rc) return rc;
+    if (!p0 || !pos || !lnpost) BAD("%s: need p0, pos and lnpost", who);
+    if (nwalkers % 2 != 0 || nwalkers < 4)
+        BAD("%s: need an even number of walkers >= 4 (twice the dimension 2; nwalkers = %d)", who, nwalkers);
+    if (steps < 0) BAD("%s: need steps >= 0", who);
+    // P (nwalkers x 2), L (nwalkers), accept counts (nwalkers): contiguous, so that one copy brings the run back
+    const size_t nP = 2 * (size_t)nwalkers, total = nP + 2 * (size_t)nwalkers;
+    if ((rc = ensure(h, h->blr_work, total * 8))) return rc;
+    double* P = ptr<double>(h->blr_work);
+    double* L = P + nP;
+    long long* acc = (long long*)(L + nwalkers);
+    const size_t smem = gpk_blr_smem_doubles(h->blr_F) * 8;
+    CK(cudaMemcpyAsync(P, p0, nP * 8, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemsetAsync(acc, 0, (size_t)nwalkers * 8, h->stream));
+    gpk_blr_eval_kernel<<<nwalkers, GPK_BLR_THREADS, smem, h->stream>>>(blr_phi(h), blr_y(h), blr_G(h), blr_b(h), h->n,
+                                                                       h->blr_F, h->blr_prior, P, L);
+    CKL();
+    for (int s = 0; s < steps; ++s)
+        for (int half = 0; half < 2; ++half) {
+            gpk_blr_step_kernel<<<nwalkers / 2, GPK_BLR_THREADS, smem, h->stream>>>(
+                blr_phi(h), blr_y(h), blr_G(h), blr_b(h), h->n, h->blr_F, h->blr_prior, nwalkers, s, half, seed, P, L, acc);
+            CKL();
+        }
+    std::vector<double> out(total);
+    CK(cudaMemcpyAsync(out.data(), P, total * 8, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    memcpy(pos, out.data(), nP * 8);
+    memcpy(lnpost, out.data() + nP, (size_t)nwalkers * 8);
+    if (n_accepted) memcpy(n_accepted, out.data() + nP + nwalkers, (size_t)nwalkers * 8);
+    return GPK_OK;
+}
+
+int gpk_blr_fit(gpk_handle* h, const double* hypers, int k) {
+    const char* who = "gpk_blr_fit";
+    int rc = blr_ready(h, who);
+    if (rc) return rc;
+    if (!hypers || k < 1) BAD("%s: need hypers and k >= 1", who);
+    h->blr_fitted = false;
+    const int F = h->blr_F;
+    const BlrPost L(k, F);
+    if ((rc = ensure(h, h->blr_post, L.total))) return rc;
+    if ((rc = ensure(h, h->blr_work, (size_t)k * 2 * 8))) return rc;
+    double* post = ptr<double>(h->blr_post);
+    double* dH = ptr<double>(h->blr_work);
+    CK(cudaMemcpyAsync(dH, hypers, (size_t)k * 2 * 8, cudaMemcpyHostToDevice, h->stream));
+    gpk_blr_fit_kernel<<<k, GPK_BLR_THREADS, (gpk_blr_smem_doubles(F) + (size_t)F * F) * 8, h->stream>>>(
+        blr_G(h), blr_b(h), F, dH, post + L.M, post + L.Li, post + L.S, post + L.ib, (int*)(post + L.fail));
+    CKL();
+    std::vector<int> fail(k);
+    CK(cudaMemcpyAsync(fail.data(), post + L.fail, (size_t)k * 4, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    for (int i = 0; i < k; ++i)
+        if (fail[i]) {
+            set_err(h, "%s: A = beta Phi^T Phi + alpha I of hypers %d (alpha = %g, beta = %g) is not positive definite",
+                    who, i, hypers[2 * i], hypers[2 * i + 1]);
+            return GPK_NOT_PD;
+        }
+    h->blr_k = k;
+    h->blr_fitted = true;
+    return GPK_OK;
+}
+
+int gpk_blr_get_models(gpk_handle* h, double* m, double* S) {
+    const char* who = "gpk_blr_get_models";
+    int rc = blr_ready(h, who);
+    if (rc) return rc;
+    if (!h->blr_fitted) { set_err(h, "%s: model is not fitted (gpk_blr_fit)", who); return GPK_NOT_FITTED; }
+    const BlrPost L(h->blr_k, h->blr_F);
+    const double* post = ptr<double>(h->blr_post);
+    if (m) CK(cudaMemcpyAsync(m, post + L.M, (size_t)h->blr_k * h->blr_F * 8, cudaMemcpyDeviceToHost, h->stream));
+    if (S)
+        CK(cudaMemcpyAsync(S, post + L.S, (size_t)h->blr_k * h->blr_F * h->blr_F * 8, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    return GPK_OK;
+}
+
+int gpk_blr_dims(gpk_handle* h, int* n, int* F, int* k) {
+    int rc = blr_ready(h, "gpk_blr_dims");
+    if (rc) return rc;
+    if (n) *n = h->n;
+    if (F) *F = h->blr_F;
+    if (k) *k = h->blr_fitted ? h->blr_k : 0;
     return GPK_OK;
 }
 

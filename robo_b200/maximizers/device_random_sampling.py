@@ -14,6 +14,7 @@ import numpy as np
 from robo_b200 import _lib
 from robo_b200.distributed import allgather_best, pack_pair, shard_bounds
 from robo_b200.maximizers.base_maximizer import BaseMaximizer
+from robo_b200.models.bayesian_linear_regression import BayesianLinearRegression
 
 
 class DeviceRandomSampling(BaseMaximizer):
@@ -31,8 +32,11 @@ class DeviceRandomSampling(BaseMaximizer):
         es = self._es_cost_spec(acq)
         if es is not None:
             return self._maximize_es_cost(acq, es)
-        if not hasattr(model, "gp") or not hasattr(model.gp, "handle"):
-            raise TypeError("DeviceRandomSampling needs a robo_b200 GaussianProcess model")
+        blr = isinstance(model, BayesianLinearRegression)
+        if not blr and (not hasattr(model, "gp") or not hasattr(model.gp, "handle")):
+            raise TypeError("DeviceRandomSampling needs a robo_b200 GaussianProcess or BayesianLinearRegression model")
+        if blr and self.world > 1:
+            raise ValueError("DeviceRandomSampling of a BayesianLinearRegression runs on one GPU")
         kind = _lib.ACQ_KIND[acq.kind]
         inc_x, inc_y = model.get_incumbent()
         eta = 0.0 if acq.kind == "lcb" else float(inc_y)
@@ -41,9 +45,12 @@ class DeviceRandomSampling(BaseMaximizer):
         # random_sampling.py:38-47: int(0.7 n) uniform points followed by int(0.3 n) Gaussian ones (n = 5 gives 3 + 1)
         n_uniform = int(self.n_samples * .7)
         n_total = n_uniform + int(self.n_samples * .3)
-        model.gp._restore()
-        model.gp._push_cfg()
-        handle = model.gp.handle
+        if blr:
+            handle = model._ready_handle()
+        else:
+            model.gp._restore()
+            model.gp._push_cfg()
+            handle = model.gp.handle
         if self.world > 1 and handle.comm_info()["world"] == self.world:
             # candidates, scoring, exchange and merge behind one C-ABI call (gpk_maximize_random_sharded)
             x, val, idx = handle.maximize_random_sharded(seed, n_total, n_uniform, self.lower, self.upper, inc_x, 0.1,

@@ -148,3 +148,31 @@ class EnvPrior(object):
         p0[:, pos:end] = samples
         p0[:, -1] = self.horseshoe.sample_from_prior(n_samples)[:, 0]
         return p0
+
+
+class BayesianLinearRegressionPrior(object):
+    """bayesian_linear_regression_prior.py:8-60, with its quirks: lnprob adds LognormalPrior(sigma=0.1, mean=-10) of
+    theta[0] (scipy's loc = -10) and HorseshoePrior(0.1) of 1 / theta[-1], one over log beta rather than the noise
+    (:45-49); sample_from_prior draws a lognormal SAMPLE (about 4.5e-5) as log alpha and log beta = log(1 / exp(sigma))
+    with the horseshoe's one randn() shared by all walkers (:51-60).  gpk_blr_lnpost restates lnprob on the device."""
+
+    def __init__(self, rng=None):
+        self.rng = np.random.RandomState(np.random.randint(0, 10000)) if rng is None else rng
+        self.ln_prior_alpha = LognormalPrior(sigma=0.1, mean=-10, rng=self.rng)
+        self.horseshoe = HorseshoePrior(scale=0.1, rng=self.rng)
+
+    def lnprob(self, theta):
+        lp = 0
+        lp += self.ln_prior_alpha.lnprob(theta[0])
+        lp += self.horseshoe.lnprob(1 / theta[-1])
+        return lp
+
+    def sample_from_prior(self, n_samples):
+        p0 = np.zeros([n_samples, 2])
+        p0[:, 0] = self.ln_prior_alpha.sample_from_prior(n_samples)[:, 0]
+        sigmas = self.horseshoe.sample_from_prior(n_samples)[:, 0]
+        p0[:, -1] = np.log(1 / np.exp(sigmas))
+        return p0
+
+    def gradient(self, theta):
+        pass

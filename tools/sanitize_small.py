@@ -121,6 +121,18 @@ print("cmaes", r["nit"], r["stop"], _lib.cmaes_draws(h, 5, 1, 0, 2, 6, D).shape)
 r = _lib.maximize_direct([h], _lib.ACQ_LOG_EI, [float(y[:100].min())], 0.0, np.zeros(D), np.ones(D), n_func_evals=200)
 print("direct", r["nit"], r["nfev"], _lib.DIRECT_STOP_NAMES[r["stop"]])
 h.close()
+# Bayesian linear regression: features, Gram reduction, log-posterior, sampler half-steps, fit and the predictive pass
+# (quadratic basis, F = 7), scored directly and through DIRECT
+h = _lib.Handle(0)
+_lib.blr_set_data(h, X[:60], y[:60], _lib.BLR_QUADRATIC, (0.1, -10.0, 0.1))
+p0 = np.column_stack([-9.0 + 0.1 * rng.randn(6), 2.0 + rng.rand(6)])
+r = _lib.blr_sample(h, 3, p0, 4)
+print("blr lnpost", _lib.blr_lnpost(h, p0)[:2], "run", r["n_accepted"])
+_lib.blr_fit(h, np.exp(r["pos"]))
+print("blr predict", h.predict(Xs[:300])[1][:2], "acq", h.acq(Xs[:300], _lib.ACQ_EI, float(y.min()), 0.0)["best_idx"])
+r = _lib.maximize_direct([h], _lib.ACQ_EI, [float(y.min())], 0.0, np.zeros(D), np.ones(D), n_func_evals=100)
+print("blr direct", r["nit"], r["nfev"])
+h.close()
 h = _lib.moments_handle()
 print(h.acq_moments(rng.randn(100), rng.rand(100) + 0.1, _lib.ACQ_LOG_EI, 0.0, 0.0)[0][:3])
 print(h.reduce_models(rng.rand(4, 50), rng.rand(4, 50))[1][:3])
