@@ -762,6 +762,46 @@ int gpk_blr_fit(gpk_handle* h, const double* hypers, int k);
 int gpk_blr_get_models(gpk_handle* h, double* m, double* S);
 int gpk_blr_dims(gpk_handle* h, int* n, int* F, int* k);
 
+/* ---- Random forest on the device (robo_b200/csrc/gpk_rf.cuh) --------------------------------------------------------
+ * robo/models/random_forest.py, with the pyrfr forest it wraps restated (pyrfr's source is not available): bagged CART
+ * regression trees on the residual sum of squares, every feature tried at every node, min_samples_to_split 2,
+ * min_samples_in_leaf 1, no depth or node limit, a node with max y - min y <= 1e-8 is a leaf.  gpk_rf.cuh states every
+ * step and its order; tests/rf_model.py restates them and the device equals it bit for bit.  A handle becomes an RF
+ * handle with gpk_rf_set_data and stays one: the Gaussian-process entry points and the BLR ones return GPK_BAD_ARG with a
+ * message naming the model kind, and the RF entry points refuse Gaussian-process and BLR handles.  The scoring entry
+ * points (gpk_acq, gpk_acq_dev, gpk_predict, gpk_maximize_random and every entry point over several models with an EI /
+ * LogEI / PI / LCB or posterior objective: gpk_acq_multi, gpk_maximize_de, gpk_maximize_lbfgs, gpk_maximize_cmaes,
+ * gpk_maximize_direct) score a fitted RF handle through its predictive pass. */
+#define GPK_RF_MAX_N 16384     /* most training points of a forest */
+#define GPK_RF_MAX_D 64        /* most input dimensions of a forest */
+#define GPK_RF_MAX_T 512       /* most trees of a forest */
+/* gpk_rf_set_data: X (n x d) and y (n) as train() receives them (random_forest.py:59-83, which adds them row by row to
+ *   a pyrfr data container); each feature's rows are ordered by (x_f, row index) once here.  Drops the trees.
+ *   GPK_BAD_ARG: n > GPK_RF_MAX_N, d > GPK_RF_MAX_D, a non-finite entry, a handle holding another model kind.
+ * gpk_rf_fit: rf.fit(data, engine) (:83) with the options of :52-57: T trees (num_trees), n_per_tree draws each
+ *   (num_data_points_per_tree; 0: n, :75-76), with replacement when bootstrap (do_bootstrapping) and without otherwise
+ *   (n_per_tree <= n), total_variance (compute_law_of_total_variance).  The draws are Philox4x32-10 keyed by seed,
+ *   with counter (draw, tree, `counter`, tag): a caller advances `counter` once per fit as pyrfr's engine advances.
+ *   Every tree grows on the device; there is no host round trip per node.  GPK_BAD_ARG: T outside 1..GPK_RF_MAX_T,
+ *   n_per_tree > n without bootstrap.
+ * gpk_rf_dims: n, d, T (0 before a fit) and the node slots per tree (2 n).
+ * gpk_rf_get_trees: the trees in breadth-first order, T x slots each (any pointer may be NULL): n_nodes (T), feat (-1:
+ *   leaf), thr, left (right = left + 1; -1 at a leaf), and the leaves' W (samples with multiplicity), mean and var (0 at
+ *   a split node).  Slots past n_nodes are undefined.
+ * gpk_rf_set_trees: the same arrays back onto an RF handle that holds the training set (a pickled or copied model);
+ *   GPK_BAD_ARG for a node that is neither a leaf nor a split whose children follow it.
+ * The predictive pass (predict_mean_var, :103-109 loops it over the rows): the (m_t, v_t) of the leaf x falls into in
+ * every tree; mean = sum m_t / T, var = sum (m_t - mean)^2 / T (+ sum v_t / T with total_variance), sums in ascending t;
+ * no clip.  The acquisition closed form of gpk_acq_moments follows, except that EI is 0 where var is 0 (ei.py:72-74). */
+int gpk_rf_set_data(gpk_handle* h, const double* X, const double* y, int n, int d);
+int gpk_rf_fit(gpk_handle* h, unsigned long long seed, unsigned counter, int T, int n_per_tree, int bootstrap,
+               int total_variance);
+int gpk_rf_dims(gpk_handle* h, int* n, int* d, int* T, int* slots);
+int gpk_rf_get_trees(gpk_handle* h, int* n_nodes, int* feat, double* thr, int* left, double* W, double* mean,
+                     double* var);
+int gpk_rf_set_trees(gpk_handle* h, int T, int total_variance, const int* n_nodes, const int* feat, const double* thr,
+                     const int* left, const double* W, const double* mean, const double* var);
+
 /* kernel.get_value(X1, X2) (test/test_models/test_gaussian_process.py:44-46) with the
  * handle's current kernel; no input scaling.  out is (n1, n2) row-major. */
 int gpk_kernel_matrix(gpk_handle* h, const double* X1, long n1, const double* X2, long n2,

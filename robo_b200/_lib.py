@@ -29,6 +29,7 @@ HYPER_MAX_N = 232                              # GPK_HYPER_MAX_N: most training 
 HYPER_MAX_DIM = 96                             # GPK_HYPER_MAX_DIM: most entries of theta (log noise included)
 BLR_LINEAR, BLR_QUADRATIC, BLR_NONE = range(3)  # gpk_blr_basis: the features of a BayesianLinearRegression handle
 BLR_MAX_F = 64                                 # GPK_BLR_MAX_F: most features of a BayesianLinearRegression handle
+RF_MAX_N, RF_MAX_D, RF_MAX_T = 16384, 64, 512  # GPK_RF_MAX_N / GPK_RF_MAX_D / GPK_RF_MAX_T: the largest forest
 CMA_MAX_D, CMA_MAX_LAMBDA, CMA_HIST = 64, 2048, 160   # GPK_CMA_MAX_D / GPK_CMA_MAX_LAMBDA / GPK_CMA_HIST
 CMA_C_W = 20                                   # GPK_CMA_C_W: where a run's weights start in its constant row
 CMA_NCONST = CMA_C_W + CMA_MAX_LAMBDA // 2     # GPK_CMA_NCONST: doubles per run in the constant table
@@ -160,6 +161,11 @@ _SIGNATURES = {
     "gpk_blr_fit": [_vp, _dp, C.c_int],
     "gpk_blr_get_models": [_vp, _dp, _dp],
     "gpk_blr_dims": [_vp, _ip, _ip, _ip],
+    "gpk_rf_set_data": [_vp, _dp, _dp, C.c_int, C.c_int],
+    "gpk_rf_fit": [_vp, C.c_ulonglong, C.c_uint, C.c_int, C.c_int, C.c_int, C.c_int],
+    "gpk_rf_dims": [_vp, _ip, _ip, _ip, _ip],
+    "gpk_rf_get_trees": [_vp, _ip, _ip, _dp, _ip, _dp, _dp, _dp],
+    "gpk_rf_set_trees": [_vp, C.c_int, C.c_int, _ip, _ip, _dp, _ip, _dp, _dp, _dp],
     "gpk_get_timings": [_vp, _dp],
     "gpk_get_diag_profile": [_vp, C.POINTER(C.c_longlong)],
 }
@@ -1324,6 +1330,54 @@ def blr_models(handle):
     M, S = np.empty((k.value, F.value)), np.empty((k.value, F.value, F.value))
     handle._check(handle.lib.gpk_blr_get_models(handle._h, _as_dp(M), _as_dp(S)))
     return [(M[i].copy(), S[i].copy()) for i in range(k.value)]
+
+
+RF_FIELDS = ("feat", "thr", "left", "W", "mean", "var")     # gpk_rf_get_trees' node arrays, in its argument order
+
+
+def rf_set_data(handle, X, y):
+    """gpk_rf_set_data: the training set on the handle, which becomes a random-forest handle."""
+    X, y = f64(X), f64(y).ravel()
+    if X.ndim != 2 or X.shape[0] != y.size:
+        raise ValueError("rf_set_data: X must be (n, d) and y (n,)")
+    n, d = X.shape
+    handle._check(handle.lib.gpk_rf_set_data(handle._h, _as_dp(X), _as_dp(y), n, d))
+
+
+def rf_fit(handle, seed, counter, num_trees, n_per_tree, bootstrap, total_variance):
+    """gpk_rf_fit: grow the forest on the device (draws keyed by seed and the fit counter)."""
+    handle._check(handle.lib.gpk_rf_fit(handle._h, int(seed) & 0xFFFFFFFFFFFFFFFF, int(counter) & 0xFFFFFFFF,
+                                        int(num_trees), int(n_per_tree), int(bool(bootstrap)),
+                                        int(bool(total_variance))))
+
+
+def rf_trees(handle):
+    """gpk_rf_get_trees: dict(n_nodes (T,), feat, thr, left, W, mean, var (T, 2 n) each, breadth-first node order;
+    right child = left + 1, feat -1 at a leaf; slots past n_nodes are zero)."""
+    n, d, T, S = C.c_int(), C.c_int(), C.c_int(), C.c_int()
+    handle._check(handle.lib.gpk_rf_dims(handle._h, C.byref(n), C.byref(d), C.byref(T), C.byref(S)))
+    T, S = T.value, S.value
+    if T == 0:
+        raise RuntimeError("rf_trees: model is not fitted (gpk_rf_fit)")
+    nn = np.empty(T, dtype=np.int32)
+    out = {k: np.empty((T, S), dtype=np.int32 if k in ("feat", "left") else np.float64) for k in RF_FIELDS}
+    ptrs = [out[k].ctypes.data_as(_ip if out[k].dtype == np.int32 else _dp) for k in RF_FIELDS]
+    handle._check(handle.lib.gpk_rf_get_trees(handle._h, nn.ctypes.data_as(_ip), *ptrs))
+    pad = np.arange(S)[None, :] >= nn[:, None]
+    for k in RF_FIELDS:
+        out[k][pad] = 0
+    out["n_nodes"] = nn
+    return out
+
+
+def rf_set_trees(handle, trees, total_variance):
+    """gpk_rf_set_trees: the arrays of rf_trees back onto a handle that holds the same training set."""
+    nn = np.ascontiguousarray(trees["n_nodes"], dtype=np.int32)
+    arr = {k: np.ascontiguousarray(trees[k], dtype=np.int32 if k in ("feat", "left") else np.float64)
+           for k in RF_FIELDS}
+    ptrs = [arr[k].ctypes.data_as(_ip if arr[k].dtype == np.int32 else _dp) for k in RF_FIELDS]
+    handle._check(handle.lib.gpk_rf_set_trees(handle._h, nn.size, int(bool(total_variance)), nn.ctypes.data_as(_ip),
+                                              *ptrs))
 
 
 _moments_handle = {}

@@ -33,6 +33,7 @@
 #include "gpk_rs.cuh"
 #include "gpk_hyper.cuh"
 #include "gpk_blr.cuh"
+#include "gpk_rf.cuh"
 
 namespace {
 
@@ -170,6 +171,12 @@ struct gpk_handle {
     int blr_basis = 0, blr_F = 0, blr_k = 0;
     BlrPrior blr_prior;
     DevBuf blr_data, blr_post, blr_work, blr_bb;
+    // random forest (gpk_rf.cuh): set once by gpk_rf_set_data, after which the handle serves the RF entry points and the
+    // scoring ones only.  rf_data: X (n x d), y (n), the per-feature row order (d x n ints); rf_work: the growth's
+    // per-tree multiplicities, lists and segments; rf_nodes: the trees (RfNodes); rf_bb: the block arg-max pairs
+    bool rf = false, rf_fitted = false;
+    int rf_T = 0, rf_total = 0;
+    DevBuf rf_data, rf_work, rf_nodes, rf_bb;
     int es_nb = 0, es_np = 0;
     double es_sn2 = 0.0, es_H = 0.0;
     long es_linv_serial = -1;       // linv_serial U was built for (-1: no update yet)
@@ -746,10 +753,18 @@ __global__ void gpk_resid_kernel(const double* __restrict__ y, double mean, int 
 // the message of every Gaussian-process entry point called with a BLR handle
 #define BLR_REFUSAL "the handle holds a Bayesian linear regression model (gpk_blr_set_data); this entry point serves " \
                     "Gaussian-process handles only"
+// ... and with a random-forest handle
+#define RF_REFUSAL "the handle holds a random forest (gpk_rf_set_data); this entry point serves Gaussian-process " \
+                   "handles only"
+
+// the refusal of a Gaussian-process entry point for the handle's model kind, or nullptr for a Gaussian-process handle
+const char* gp_refusal(const gpk_handle* h) {
+    return h->blr ? BLR_REFUSAL : h->rf ? RF_REFUSAL : nullptr;
+}
 
 int require(gpk_handle* h, bool data, bool spec, bool fitted) {
     if (!h) return GPK_BAD_ARG;
-    if (h->blr) { set_err(h, BLR_REFUSAL); return GPK_BAD_ARG; }
+    if (gp_refusal(h)) { set_err(h, "%s", gp_refusal(h)); return GPK_BAD_ARG; }
     if (data && !h->has_data) { set_err(h, "gpk_set_data has not been called"); return GPK_BAD_ARG; }
     if (spec && !h->has_spec) { set_err(h, "gpk_set_kernel has not been called"); return GPK_BAD_ARG; }
     if (fitted && !h->fitted) { set_err(h, "model is not fitted (gpk_fit)"); return GPK_NOT_FITTED; }
@@ -760,6 +775,10 @@ int require(gpk_handle* h, bool data, bool spec, bool fitted) {
 int require_model(gpk_handle* h) {
     if (h && h->blr) {
         if (!h->blr_fitted) { set_err(h, "model is not fitted (gpk_blr_fit)"); return GPK_NOT_FITTED; }
+        return GPK_OK;
+    }
+    if (h && h->rf) {
+        if (!h->rf_fitted) { set_err(h, "model is not fitted (gpk_rf_fit)"); return GPK_NOT_FITTED; }
         return GPK_OK;
     }
     return require(h, true, true, true);
@@ -889,6 +908,9 @@ struct Feeder {
 int blr_score(gpk_handle* h, const double* dX, long m, int kind, double eta, double par, double* d_out, double* d_mu,
               double* d_var, BestPair* d_best, unsigned long long* d_nneg, long index_offset, bool reset, long global_base,
               Feeder* feeder);
+int rf_score(gpk_handle* h, const double* dX, long m, int kind, double eta, double par, double* d_out, double* d_mu,
+             double* d_var, BestPair* d_best, unsigned long long* d_nneg, long index_offset, bool reset, long global_base,
+             Feeder* feeder);
 
 int score_dev(gpk_handle* h, const double* dX, long m, int kind, double eta, double par, double* d_out,
               double* d_mu, double* d_var, BestPair* d_best, unsigned long long* d_nneg,
@@ -896,6 +918,9 @@ int score_dev(gpk_handle* h, const double* dX, long m, int kind, double eta, dou
     if (h->blr)
         return blr_score(h, dX, m, kind, eta, par, d_out, d_mu, d_var, d_best, d_nneg, index_offset, reset, global_base,
                          feeder);
+    if (h->rf)
+        return rf_score(h, dX, m, kind, eta, par, d_out, d_mu, d_var, d_best, d_nneg, index_offset, reset, global_base,
+                        feeder);
     int rc = build_linv(h);
     if (rc) return rc;
     const long NP = h->NP;
@@ -1164,7 +1189,7 @@ int es_dh_dev(gpk_handle* h, const double* Xm, const double* Xb, long m, double*
 int es_ready(gpk_handle* h, gpk_handle* report, const char* who, int kind = ES_KIND_EP) {
     gpk_handle* r = report ? report : h;
     const char* upd = kind == ES_KIND_MC ? "gpk_esmc_update" : "gpk_es_update";
-    if (h->blr) { set_err(r, "%s: " BLR_REFUSAL, who); return GPK_BAD_ARG; }
+    if (gp_refusal(h)) { set_err(r, "%s: %s", who, gp_refusal(h)); return GPK_BAD_ARG; }
     if (h->es_linv_serial < 0) { set_err(r, "%s: call %s first", who, upd); return GPK_BAD_ARG; }
     if (!h->linv_ready || h->es_linv_serial != h->linv_serial) {
         set_err(r, "%s: the model changed since %s", who, upd);
@@ -1281,6 +1306,8 @@ struct BlrPost {
 
 int blr_ready(gpk_handle* h, const char* who) {
     if (!h) return GPK_BAD_ARG;
+    if (h->rf) BAD("%s: the handle holds a random forest (gpk_rf_set_data); use a new handle for Bayesian linear "
+                   "regression", who);
     if (!h->blr) BAD("%s: gpk_blr_set_data has not been called", who);
     CK(cudaSetDevice(h->device));
     const int sm_eval = (int)(gpk_blr_smem_doubles(h->blr_F) * 8);
@@ -1330,6 +1357,79 @@ int blr_score(gpk_handle* h, const double* dX, long m, int kind, double eta, dou
         CKL();
         if (kind != GPK_ACQ_NONE) {
             gpk_argmax_final_kernel<<<1, 256, 0, h->stream>>>(ptr<BestPair>(h->blr_bb), nblk, d_best);
+            CKL();
+        }
+    }
+    return GPK_OK;
+}
+
+// the layout of h->rf_data: X (n x d doubles), y (n doubles), the per-feature row order (d x n ints)
+inline double* rf_X(gpk_handle* h) { return ptr<double>(h->rf_data); }
+inline double* rf_y(gpk_handle* h) { return rf_X(h) + (size_t)h->n * h->d; }
+inline int* rf_order(gpk_handle* h) { return (int*)(rf_y(h) + h->n); }
+
+// the layout of h->rf_nodes (bytes) for T trees of S = 2 n node slots: feat, left (T x S ints), n_nodes (T ints, padded
+// to 8 bytes), thr, W, mean, var (T x S doubles each)
+struct RfNodes {
+    size_t feat, left, nn, thr, W, mean, var, total;
+    RfNodes(int T, long S) {
+        const size_t TS = (size_t)T * S;
+        feat = 0; left = feat + TS * 4; nn = left + TS * 4;
+        thr = nn + ((size_t)T * 4 + 7) / 8 * 8;
+        W = thr + TS * 8; mean = W + TS * 8; var = mean + TS * 8; total = var + TS * 8;
+    }
+};
+
+int rf_ready(gpk_handle* h, const char* who) {
+    if (!h) return GPK_BAD_ARG;
+    if (h->blr) BAD("%s: the handle holds a Bayesian linear regression model (gpk_blr_set_data); use a new handle for a "
+                    "random forest", who);
+    if (!h->rf) BAD("%s: gpk_rf_set_data has not been called", who);
+    CK(cudaSetDevice(h->device));
+    return GPK_OK;
+}
+
+// score_dev for a random-forest handle: gpk_rf_score_kernel over the m rows dX, with score_dev's outputs, offsets and
+// running arg-max
+int rf_score(gpk_handle* h, const double* dX, long m, int kind, double eta, double par, double* d_out, double* d_mu,
+             double* d_var, BestPair* d_best, unsigned long long* d_nneg, long index_offset, bool reset, long global_base,
+             Feeder* feeder) {
+    int rc;
+    if ((rc = rf_ready(h, "scoring"))) return rc;
+    const long nblk = (m + GPK_RF_SCORE_WARPS - 1) / GPK_RF_SCORE_WARPS;
+    if ((rc = ensure(h, h->rf_bb, (size_t)std::max(nblk, 1L) * sizeof(BestPair)))) return rc;
+    if ((rc = ensure(h, h->best, sizeof(BestPair)))) return rc;
+    if ((rc = ensure(h, h->nneg, 8))) return rc;
+    if (d_best == nullptr) d_best = ptr<BestPair>(h->best);
+    if (d_nneg == nullptr) d_nneg = ptr<unsigned long long>(h->nneg);
+    if (reset) {
+        CK(cudaMemsetAsync(d_best, 0xFF, sizeof(BestPair), h->stream));
+        CK(cudaMemsetAsync(d_nneg, 0, 8, h->stream));
+    }
+    if (feeder && (rc = feeder->ready(0, m, h->stream))) return rc;
+    const long S = 2L * h->n;
+    const RfNodes L(h->rf_T, S);
+    char* nodes = ptr<char>(h->rf_nodes);
+    RfScoreArgs a;
+    memset(&a, 0, sizeof(a));
+    a.X = dX; a.m = m; a.D = h->d; a.T = h->rf_T; a.S = S;
+    a.feat = (const int*)(nodes + L.feat); a.left = (const int*)(nodes + L.left);
+    a.thr = (const double*)(nodes + L.thr); a.mean = (const double*)(nodes + L.mean);
+    a.var = (const double*)(nodes + L.var);
+    a.total_var = h->rf_total;
+    a.base = global_base + index_offset;
+    a.acq_kind = kind; a.eta = eta; a.par = par;
+    a.out_mu = d_mu ? d_mu + index_offset : nullptr;
+    a.out_var = d_var ? d_var + index_offset : nullptr;
+    a.out_acq = d_out ? d_out + index_offset : nullptr;
+    a.block_best = ptr<BestPair>(h->rf_bb);
+    a.n_negative = d_nneg;
+    if (m > 0) {
+        gpk_rf_score_kernel<<<(unsigned)nblk, GPK_RF_SCORE_WARPS * 32, gpk_rf_score_smem_doubles(h->rf_T) * 8,
+                              h->stream>>>(a);
+        CKL();
+        if (kind != GPK_ACQ_NONE) {
+            gpk_argmax_final_kernel<<<1, 256, 0, h->stream>>>(ptr<BestPair>(h->rf_bb), (int)nblk, d_best);
             CKL();
         }
     }
@@ -1393,7 +1493,8 @@ int gpk_destroy(gpk_handle* h) {
                       &h->tmpjobs, &h->alpha, &h->tmp1, &h->tmp2, &h->tmp3, &h->dprof, &h->Xts, &h->oz_Pq, &h->oz_Kq, &h->oz_Kq2, &h->oz_eP, &h->oz_emax, &h->oz_pmu2, &h->oz_probe,
                       &h->multi_cand, &h->multi_A, &h->multi_B, &h->multi_out, &h->multi_bb, &h->gather, &h->best_global,
                       &h->de_pop, &h->de_trial, &h->de_param, &h->de_E, &h->de_small, &h->de_sort, &h->lb_buf, &h->cma_buf, &h->dir_buf, &h->ep_buf, &h->es_state, &h->es_U, &h->es_work, &h->es_in, &h->mc_state, &h->mc_buf, &h->mc_stat, &h->fab_in, &h->rs_buf, &h->hy_buf,
-                      &h->blr_data, &h->blr_post, &h->blr_work, &h->blr_bb};
+                      &h->blr_data, &h->blr_post, &h->blr_work, &h->blr_bb,
+                      &h->rf_data, &h->rf_work, &h->rf_nodes, &h->rf_bb};
     for (DevBuf* b : bufs)
         if (b->p) cudaFree(b->p);
     if (h->ev_ok)
@@ -1502,7 +1603,7 @@ int gpk_synchronize(gpk_handle* h) {
 
 int gpk_set_data(gpk_handle* h, const double* X, const double* y, int n, int d) {
     if (!h) return GPK_BAD_ARG;
-    if (h->blr) BAD("gpk_set_data: " BLR_REFUSAL);
+    if (gp_refusal(h)) BAD("gpk_set_data: %s", gp_refusal(h));
     if (!X || !y || n <= 0 || d <= 0) BAD("gpk_set_data: need X, y, n > 0, d > 0");
     if (d > GPK_MAX_TERMS) BAD("gpk_set_data: d = %d exceeds GPK_MAX_TERMS = %d", d, GPK_MAX_TERMS);
     CK(cudaSetDevice(h->device));
@@ -1548,7 +1649,7 @@ int gpk_set_data(gpk_handle* h, const double* X, const double* y, int n, int d) 
 
 int gpk_set_input_bounds(gpk_handle* h, const double* lower, const double* upper, int d) {
     if (!h) return GPK_BAD_ARG;
-    if (h->blr) BAD("gpk_set_input_bounds: " BLR_REFUSAL);
+    if (gp_refusal(h)) BAD("gpk_set_input_bounds: %s", gp_refusal(h));
     CK(cudaSetDevice(h->device));
     if (!lower || !upper) { h->has_bounds = false; return GPK_OK; }
     if (d <= 0 || d > GPK_MAX_TERMS) BAD("gpk_set_input_bounds: bad d");
@@ -1564,7 +1665,7 @@ int gpk_set_input_bounds(gpk_handle* h, const double* lower, const double* upper
 
 int gpk_set_output_transform(gpk_handle* h, int enabled, double y_mean, double y_std) {
     if (!h) return GPK_BAD_ARG;
-    if (h->blr) BAD("gpk_set_output_transform: " BLR_REFUSAL);
+    if (gp_refusal(h)) BAD("gpk_set_output_transform: %s", gp_refusal(h));
     h->norm_out = enabled ? 1 : 0;
     h->y_mean = y_mean;
     h->y_std = y_std;
@@ -1574,7 +1675,7 @@ int gpk_set_output_transform(gpk_handle* h, int enabled, double y_mean, double y
 int gpk_set_kernel(gpk_handle* h, int family, double log_amp, int n_terms, const int* axis, const int* group,
                    const double* log_metric) {
     if (!h) return GPK_BAD_ARG;
-    if (h->blr) BAD("gpk_set_kernel: " BLR_REFUSAL);
+    if (gp_refusal(h)) BAD("gpk_set_kernel: %s", gp_refusal(h));
     if (family < GPK_MATERN52 || family > GPK_MATERN32) BAD("gpk_set_kernel: unknown family %d", family);
     if (n_terms <= 0 || n_terms > GPK_MAX_TERMS || !axis || !group || !log_metric)
         BAD("gpk_set_kernel: need 1..%d terms", GPK_MAX_TERMS);
@@ -1763,7 +1864,7 @@ int gpk_fit(gpk_handle* h, double diag_add, double mean, double* logdet, double*
 int gpk_fit_append(gpk_handle* h, const double* X, const double* y, int n, int d, double diag_add, double mean,
                    double* logdet, double* loglik) {
     if (!h) return GPK_BAD_ARG;
-    if (h->blr) BAD("gpk_fit_append: " BLR_REFUSAL);
+    if (gp_refusal(h)) BAD("gpk_fit_append: %s", gp_refusal(h));
     if (!X || !y || n <= 0 || d <= 0) BAD("gpk_fit_append: need X, y, n > 0, d > 0");
     const long NP = h->NP;
     const int nb = h->nb, b = nb - 1, N1 = b * BM;
@@ -2330,7 +2431,7 @@ int gpk_set_hyper_model(gpk_handle* h, int n_params, const int* amp_slot, const 
                         double mean, double tiny, int prior_kind, const double* prior_par, int n_ls, int n_lr) {
     if (!h) return GPK_BAD_ARG;
     const char* who = "gpk_set_hyper_model";
-    if (h->blr) BAD("%s: " BLR_REFUSAL, who);
+    if (gp_refusal(h)) BAD("%s: %s", who, gp_refusal(h));
     h->has_hyper = false;
     if (!h->has_spec) BAD("%s: gpk_set_kernel has not been called", who);
     if (n_params < 1 || n_params + 1 > GPK_HYPER_MAX_DIM || !amp_slot || !term_param)
@@ -2462,6 +2563,8 @@ int gpk_sample_hypers(gpk_handle* h, const double* p0, int nwalkers, int dim, in
 int gpk_blr_set_data(gpk_handle* h, const double* X, const double* y, int n, int d, int basis, const double* prior_par) {
     if (!h) return GPK_BAD_ARG;
     const char* who = "gpk_blr_set_data";
+    if (h->rf) BAD("%s: the handle holds a random forest (gpk_rf_set_data); use a new handle for Bayesian linear "
+                   "regression", who);
     if (!h->blr && (h->has_data || h->has_spec))
         BAD("%s: the handle holds a Gaussian-process model; use a new handle for Bayesian linear regression", who);
     if (!X || !y || !prior_par || n <= 0 || d <= 0) BAD("%s: need X, y, prior_par, n > 0, d > 0", who);
@@ -2593,6 +2696,154 @@ int gpk_blr_dims(gpk_handle* h, int* n, int* F, int* k) {
     if (n) *n = h->n;
     if (F) *F = h->blr_F;
     if (k) *k = h->blr_fitted ? h->blr_k : 0;
+    return GPK_OK;
+}
+
+// ---------------------------------------------------------------------------------------
+// Random forest (gpk_rf.cuh; robo/models/random_forest.py)
+// ---------------------------------------------------------------------------------------
+int gpk_rf_set_data(gpk_handle* h, const double* X, const double* y, int n, int d) {
+    if (!h) return GPK_BAD_ARG;
+    const char* who = "gpk_rf_set_data";
+    if (h->blr) BAD("%s: the handle holds a Bayesian linear regression model (gpk_blr_set_data); use a new handle for a "
+                    "random forest", who);
+    if (!h->rf && (h->has_data || h->has_spec))
+        BAD("%s: the handle holds a Gaussian-process model; use a new handle for a random forest", who);
+    if (!X || !y || n <= 0 || d <= 0) BAD("%s: need X, y, n > 0, d > 0", who);
+    if (n > GPK_RF_MAX_N) BAD("%s: n = %d training points exceed GPK_RF_MAX_N = %d", who, n, GPK_RF_MAX_N);
+    if (d > GPK_RF_MAX_D) BAD("%s: d = %d exceeds GPK_RF_MAX_D = %d", who, d, GPK_RF_MAX_D);
+    for (long i = 0; i < (long)n * d; ++i)
+        if (!std::isfinite(X[i])) BAD("%s: X must be finite", who);
+    for (int i = 0; i < n; ++i)
+        if (!std::isfinite(y[i])) BAD("%s: y must be finite", who);
+    CK(cudaSetDevice(h->device));
+    // each feature's rows ordered by (x_f, row index), once per training set
+    std::vector<int> order((size_t)d * n);
+    for (int f = 0; f < d; ++f) {
+        int* o = order.data() + (size_t)f * n;
+        for (int i = 0; i < n; ++i) o[i] = i;
+        std::sort(o, o + n, [&](int a, int b) {
+            const double xa = X[(size_t)a * d + f], xb = X[(size_t)b * d + f];
+            return xa < xb || (xa == xb && a < b);
+        });
+    }
+    int rc;
+    h->rf = true;
+    h->rf_fitted = false;
+    h->n = n; h->d = d;
+    if ((rc = ensure(h, h->rf_data, ((size_t)n * d + n) * 8 + (size_t)d * n * 4))) return rc;
+    CK(cudaMemcpyAsync(rf_X(h), X, (size_t)n * d * 8, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(rf_y(h), y, (size_t)n * 8, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(rf_order(h), order.data(), (size_t)d * n * 4, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaStreamSynchronize(h->stream));     // host buffers are caller-owned: done with them
+    return GPK_OK;
+}
+
+int gpk_rf_fit(gpk_handle* h, unsigned long long seed, unsigned counter, int T, int n_per_tree, int bootstrap,
+               int total_variance) {
+    const char* who = "gpk_rf_fit";
+    int rc = rf_ready(h, who);
+    if (rc) return rc;
+    const int n = h->n, d = h->d;
+    if (T < 1 || T > GPK_RF_MAX_T) BAD("%s: need 1 <= num_trees <= GPK_RF_MAX_T = %d (num_trees = %d)", who, GPK_RF_MAX_T, T);
+    if (n_per_tree < 0) BAD("%s: need n_points_per_tree >= 0", who);
+    const int nt = n_per_tree > 0 ? n_per_tree : n;
+    if (!bootstrap && nt > n)
+        BAD("%s: without bootstrapping a tree cannot take %d of %d points (n_points_per_tree <= n)", who, nt, n);
+    h->rf_fitted = false;
+    const long S = 2L * n;
+    const RfNodes L(T, S);
+    if ((rc = ensure(h, h->rf_nodes, L.total))) return rc;
+    // growth scratch per CTA: multiplicities (n), two list buffers (2 (d + 1) n) and the segments (3 x 2 n), ints;
+    // trees are grown in batches that keep it near 512 MB
+    const size_t per_tree = (size_t)n * (1 + 2 * (size_t)(d + 1) + 6) * 4;
+    const int batch = (int)std::max<size_t>(1, std::min<size_t>((size_t)T, ((size_t)512 << 20) / per_tree));
+    if ((rc = ensure(h, h->rf_work, per_tree * batch))) return rc;
+    char* nodes = ptr<char>(h->rf_nodes);
+    int* work = ptr<int>(h->rf_work);
+    RfGrowArgs a;
+    memset(&a, 0, sizeof(a));
+    a.X = rf_X(h); a.y = rf_y(h); a.order = rf_order(h);
+    a.n = n; a.d = d; a.nt = nt; a.bootstrap = bootstrap ? 1 : 0;
+    a.seed = seed; a.counter = counter;
+    a.cnt = work;
+    a.lists = work + (size_t)batch * n;
+    a.seg = a.lists + (size_t)batch * 2 * (d + 1) * n;
+    a.feat = (int*)(nodes + L.feat); a.left = (int*)(nodes + L.left); a.n_nodes = (int*)(nodes + L.nn);
+    a.thr = (double*)(nodes + L.thr); a.W = (double*)(nodes + L.W); a.mean = (double*)(nodes + L.mean);
+    a.var = (double*)(nodes + L.var);
+    for (int t0 = 0; t0 < T; t0 += batch) {
+        a.t0 = t0;
+        gpk_rf_grow_kernel<<<std::min(batch, T - t0), GPK_RF_GROW_THREADS, 0, h->stream>>>(a);
+        CKL();
+    }
+    CK(cudaStreamSynchronize(h->stream));
+    h->rf_T = T;
+    h->rf_total = total_variance ? 1 : 0;
+    h->rf_fitted = true;
+    return GPK_OK;
+}
+
+int gpk_rf_dims(gpk_handle* h, int* n, int* d, int* T, int* slots) {
+    int rc = rf_ready(h, "gpk_rf_dims");
+    if (rc) return rc;
+    if (n) *n = h->n;
+    if (d) *d = h->d;
+    if (T) *T = h->rf_fitted ? h->rf_T : 0;
+    if (slots) *slots = 2 * h->n;
+    return GPK_OK;
+}
+
+int gpk_rf_get_trees(gpk_handle* h, int* n_nodes, int* feat, double* thr, int* left, double* W, double* mean,
+                     double* var) {
+    const char* who = "gpk_rf_get_trees";
+    int rc = rf_ready(h, who);
+    if (rc) return rc;
+    if (!h->rf_fitted) { set_err(h, "%s: model is not fitted (gpk_rf_fit)", who); return GPK_NOT_FITTED; }
+    const long S = 2L * h->n;
+    const size_t TS = (size_t)h->rf_T * S;
+    const RfNodes L(h->rf_T, S);
+    const char* nodes = ptr<char>(h->rf_nodes);
+    const struct { void* dst; size_t off, bytes; } parts[] = {
+        {n_nodes, L.nn, (size_t)h->rf_T * 4}, {feat, L.feat, TS * 4}, {thr, L.thr, TS * 8}, {left, L.left, TS * 4},
+        {W, L.W, TS * 8}, {mean, L.mean, TS * 8}, {var, L.var, TS * 8}};
+    for (const auto& p : parts)
+        if (p.dst) CK(cudaMemcpyAsync(p.dst, nodes + p.off, p.bytes, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    return GPK_OK;
+}
+
+int gpk_rf_set_trees(gpk_handle* h, int T, int total_variance, const int* n_nodes, const int* feat, const double* thr,
+                     const int* left, const double* W, const double* mean, const double* var) {
+    const char* who = "gpk_rf_set_trees";
+    int rc = rf_ready(h, who);
+    if (rc) return rc;
+    if (T < 1 || T > GPK_RF_MAX_T) BAD("%s: need 1 <= T <= GPK_RF_MAX_T = %d", who, GPK_RF_MAX_T);
+    if (!n_nodes || !feat || !thr || !left || !W || !mean || !var) BAD("%s: need every node array", who);
+    const long S = 2L * h->n;
+    // every walk must end in a leaf: a split node's children come after it and exist
+    for (int t = 0; t < T; ++t) {
+        const int nn = n_nodes[t];
+        if (nn < 1 || nn >= S) BAD("%s: tree %d has %d nodes (1 .. %ld allowed)", who, t, nn, S - 1);
+        for (int v = 0; v < nn; ++v) {
+            const int f = feat[(size_t)t * S + v], c = left[(size_t)t * S + v];
+            if (f >= h->d || (f >= 0 && (c <= v || c + 1 >= nn)))
+                BAD("%s: node %d of tree %d is not a valid split or leaf", who, v, t);
+        }
+    }
+    h->rf_fitted = false;
+    const size_t TS = (size_t)T * S;
+    const RfNodes L(T, S);
+    if ((rc = ensure(h, h->rf_nodes, L.total))) return rc;
+    char* nodes = ptr<char>(h->rf_nodes);
+    const struct { const void* src; size_t off, bytes; } parts[] = {
+        {n_nodes, L.nn, (size_t)T * 4}, {feat, L.feat, TS * 4}, {thr, L.thr, TS * 8}, {left, L.left, TS * 4},
+        {W, L.W, TS * 8}, {mean, L.mean, TS * 8}, {var, L.var, TS * 8}};
+    for (const auto& p : parts) CK(cudaMemcpyAsync(nodes + p.off, p.src, p.bytes, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    h->rf_T = T;
+    h->rf_total = total_variance ? 1 : 0;
+    h->rf_fitted = true;
     return GPK_OK;
 }
 

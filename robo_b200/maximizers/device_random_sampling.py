@@ -8,6 +8,10 @@ candidate i comes from Philox4x32-10 keyed by (seed, i), which makes the result 
 chunking and of the number of GPUs: with ``world > 1`` every rank scores a contiguous index range and
 one 16-byte all_gather settles the arg-max (robo_b200/distributed.py).  Nothing but the winning point
 crosses PCIe.
+
+Over a RandomForest, whose predictive std can be exactly 0, EI keeps the reference's batch rule (ei.py:72-74: a zero
+std anywhere makes the whole batch [[0]], so RandomSampling's arg-max is row 0): when any candidate has a zero
+variance, the first candidate is returned.
 """
 import numpy as np
 
@@ -15,6 +19,7 @@ from robo_b200 import _lib
 from robo_b200.distributed import allgather_best, pack_pair, shard_bounds
 from robo_b200.maximizers.base_maximizer import BaseMaximizer
 from robo_b200.models.bayesian_linear_regression import BayesianLinearRegression
+from robo_b200.models.random_forest import RandomForest
 
 
 class DeviceRandomSampling(BaseMaximizer):
@@ -33,10 +38,14 @@ class DeviceRandomSampling(BaseMaximizer):
         if es is not None:
             return self._maximize_es_cost(acq, es)
         blr = isinstance(model, BayesianLinearRegression)
-        if not blr and (not hasattr(model, "gp") or not hasattr(model.gp, "handle")):
-            raise TypeError("DeviceRandomSampling needs a robo_b200 GaussianProcess or BayesianLinearRegression model")
+        rf = isinstance(model, RandomForest)
+        if not (blr or rf) and (not hasattr(model, "gp") or not hasattr(model.gp, "handle")):
+            raise TypeError("DeviceRandomSampling needs a robo_b200 GaussianProcess, BayesianLinearRegression or "
+                            "RandomForest model")
         if blr and self.world > 1:
             raise ValueError("DeviceRandomSampling of a BayesianLinearRegression runs on one GPU")
+        if rf and self.world > 1:
+            raise ValueError("DeviceRandomSampling of a RandomForest runs on one GPU")
         kind = _lib.ACQ_KIND[acq.kind]
         inc_x, inc_y = model.get_incumbent()
         eta = 0.0 if acq.kind == "lcb" else float(inc_y)
@@ -45,7 +54,7 @@ class DeviceRandomSampling(BaseMaximizer):
         # random_sampling.py:38-47: int(0.7 n) uniform points followed by int(0.3 n) Gaussian ones (n = 5 gives 3 + 1)
         n_uniform = int(self.n_samples * .7)
         n_total = n_uniform + int(self.n_samples * .3)
-        if blr:
+        if blr or rf:
             handle = model._ready_handle()
         else:
             model.gp._restore()
@@ -67,6 +76,10 @@ class DeviceRandomSampling(BaseMaximizer):
                 dev = "cuda:%d" % torch.cuda.current_device() if torch.cuda.is_available() else "cpu"
                 val, idx = allgather_best(pack_pair(val, idx, dev), self.group)
                 x = handle.generate_candidates(seed, idx, 1, n_uniform, self.lower, self.upper, inc_x, 0.1)[0]
+        if rf and acq.kind == "ei":
+            X = handle.generate_candidates(seed, 0, n_total, n_uniform, self.lower, self.upper, inc_x, 0.1)
+            if (np.sqrt(model.predict(X)[1]) == 0).any():
+                x, val, idx = X[0], 0.0, 0
         self.last = dict(seed=seed, best_idx=idx, best_val=val)
         return x
 

@@ -7,6 +7,7 @@ import numpy as np
 from robo_b200 import _lib
 from robo_b200.models.bayesian_linear_regression import BayesianLinearRegression
 from robo_b200.models.gaussian_process import GaussianProcess
+from robo_b200.models.random_forest import RandomForest
 
 KINDS = ("ei", "log_ei", "pi", "lcb")
 
@@ -45,7 +46,7 @@ def device_spec(acq, who):
 
 def acq_spec(acq, who):
     """(kind, eta per model, par, handles) of the acquisition, or TypeError when it does not run on device GPs whose
-    inputs go to the handle untransformed or on a BayesianLinearRegression (eta: its min observed y)."""
+    inputs go to the handle untransformed or on a BayesianLinearRegression or RandomForest (eta: its min observed y)."""
     if hasattr(acq, "_fused_spec"):                          # MarginalizationGPMCMC
         fused = acq._fused_spec()
         if fused is None or not all(raw_inputs(m) for m in acq.model.models):
@@ -54,7 +55,7 @@ def acq_spec(acq, who):
         return kind, etas, par, handles
     model = getattr(acq, "model", None)
     kind = getattr(acq, "kind", None)
-    if isinstance(model, BayesianLinearRegression) and kind in KINDS and getattr(acq, "cost_model", None) is None:
+    if isinstance(model, (BayesianLinearRegression, RandomForest)) and kind in KINDS and getattr(acq, "cost_model", None) is None:
         eta = 0.0 if kind == "lcb" else float(model.get_incumbent()[1])
         return kind, [eta], float(acq.par), [model._ready_handle()]
     if kind not in KINDS or getattr(acq, "cost_model", None) is not None or not raw_inputs(model) \

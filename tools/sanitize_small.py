@@ -133,6 +133,19 @@ print("blr predict", h.predict(Xs[:300])[1][:2], "acq", h.acq(Xs[:300], _lib.ACQ
 r = _lib.maximize_direct([h], _lib.ACQ_EI, [float(y.min())], 0.0, np.zeros(D), np.ones(D), n_func_evals=100)
 print("blr direct", r["nit"], r["nfev"])
 h.close()
+# random forest: draws, growth (bootstrap and Fisher-Yates), the node read-back and upload, the predictive pass, scored
+# directly and through DIRECT
+h = _lib.Handle(0)
+_lib.rf_set_data(h, X[:60], y[:60])
+_lib.rf_fit(h, 3, 0, 33, 0, True, True)
+t = _lib.rf_trees(h)
+_lib.rf_fit(h, 3, 1, 5, 40, False, False)
+_lib.rf_set_trees(h, t, True)
+print("rf nodes", t["n_nodes"][:3], "predict", h.predict(Xs[:300])[1][:2],
+      "acq", h.acq(Xs[:300], _lib.ACQ_EI, float(y.min()), 0.0)["best_idx"])
+r = _lib.maximize_direct([h], _lib.ACQ_EI, [float(y.min())], 0.0, np.zeros(D), np.ones(D), n_func_evals=100)
+print("rf direct", r["nit"], r["nfev"])
+h.close()
 h = _lib.moments_handle()
 print(h.acq_moments(rng.randn(100), rng.rand(100) + 0.1, _lib.ACQ_LOG_EI, 0.0, 0.0)[0][:3])
 print(h.reduce_models(rng.rand(4, 50), rng.rand(4, 50))[1][:3])
