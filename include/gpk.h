@@ -86,7 +86,8 @@ const char* gpk_version(void);
  *               512 MB (16384 candidates at N = 4096, 65536 at N <= 1024)
  *   "ozaki"     1 = variance contraction on the int8 tensor pipe (wgmma s8, register accumulators) through an
  *               error-free split of L^-1 and K* into 7 balanced base-256 digits each, 28 digit-pair products
- *               (gpk_ozaki.cuh); used while max |L^-1| < 64 and N <= 16384, otherwise the fp64 kernel runs [default;
+ *               (gpk_ozaki.cuh); used while max |L^-1| < 64, N <= 16384 and the kernel has no environment factor
+ *               (gpk_set_env_factor), otherwise the fp64 kernel runs [default;
  *               batches of >= 2048 candidates]; 0 = always fp64 DMMA.  The posterior mean never goes through the digits
  *               (fp64 K* alpha); the covariance builder writes the digits and the mean partials itself, no fp64 K*
  *               in HBM
@@ -134,6 +135,18 @@ int gpk_set_output_transform(gpk_handle* h, int enabled, double y_mean, double y
  * (gaussian_process.py:110,151). */
 int gpk_set_kernel(gpk_handle* h, int family, double log_amp, int n_terms,
                    const int* axis, const int* group, const double* log_metric);
+
+/* Environment factor of Fabolas (robo/fmin/fabolas.py:104-117, BayesianLinearRegressionKernel): multiplies the
+ * handle's kernel by
+ *     k_env(z, z') = exp(log_a) + exp(log_b) * z * z'
+ * on input column `axis` (the coordinate the radial terms see: after the input-bounds scaling; for a FabolasGP the
+ * basis-transformed dataset size).  This is a restatement from the Fabolas paper (arXiv:1605.07079: a Bayesian linear
+ * regression in the features (1, z) with the prior covariance diag(exp(log_a), exp(log_b))) and the reference's call
+ * sites; the george fork that defines the kernel is not public, so it has not been checked against that source.
+ * axis = -1 removes the factor; gpk_set_kernel also removes it.  GPK_BAD_ARG for a non-finite parameter or an axis < -1;
+ * an axis outside the data's width is refused by gpk_fit / gpk_kernel_matrix / the hyper sampler.  Scoring with the
+ * factor always takes the fp64 contraction (the int8 split assumes 0 < k <= amp). */
+int gpk_set_env_factor(gpk_handle* h, int axis, double log_a, double log_b);
 
 /* ---- fit: K build + Cholesky + forward solve + log-det ------------------------------- */
 /* Replaces george GP.compute + GP.log_likelihood (gaussian_process.py:119,155,159):
@@ -698,7 +711,9 @@ int gpk_sample_representers(gpk_handle* const* models, int n, const unsigned lon
  *
  * gpk_set_hyper_model: how theta maps to the handle's kernel structure (family, axes, groups of the last gpk_set_kernel;
  *   its parameter values are not used).  n_params = len(kernel) (theta has n_params + 1 entries, the log noise last);
- *   amp_slot[p] = 1 when parameter p is an amplitude slot (log_amp = 0.0 + those entries in order), 0 for a metric slot;
+ *   amp_slot[p] = 1 when parameter p is an amplitude slot (log_amp = 0.0 + those entries in order), 0 for a metric slot,
+ *   2 for log_a and 3 for log_b of the environment factor (one each, exactly when gpk_set_env_factor set a factor; its
+ *   axis is the handle's);
  *   term_param[t] (n_terms entries) = the metric slot that sets term t (kernels.py flatten()["slots"]).  The diagonal is
  *   fl(sqrt(fl(yerr^2 + tiny)))^2 with yerr = sqrt(exp(theta[-1])), the constant mean `mean`.  prior_kind: gpk_prior_kind;
  *   prior_par (7 entries, NULL for GPK_PRIOR_NONE) = lognormal sigma, lognormal mean (scipy's loc), tophat lower, tophat
@@ -840,7 +855,8 @@ int gpk_maximize_random_sharded(gpk_handle* h, unsigned long long seed, long n_t
 
 /* ---- marginal-likelihood gradient (gaussian_process.py:168-191, corrected noise term) -- */
 /* grad[n_terms + 2] = d(-loglik)/d[log_amp, log_metric_t..., log sigma^2]; requires a
- * preceding successful gpk_fit with the same parameters.  noise_var = sigma^2. */
+ * preceding successful gpk_fit with the same parameters.  noise_var = sigma^2.  With the environment factor
+ * (gpk_set_env_factor) grad has n_terms + 4 entries: [log_amp, log_metric_t..., log_a, log_b, log sigma^2]. */
 int gpk_nll_grad(gpk_handle* h, double noise_var, double* grad);
 
 /* fp64 issue-rate peaks of this GPU in TFLOP/s, measured with register-resident operands: the DMMA

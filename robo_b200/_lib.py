@@ -57,6 +57,7 @@ _SIGNATURES = {
     "gpk_set_input_bounds": [_vp, _dp, _dp, C.c_int],
     "gpk_set_output_transform": [_vp, C.c_int, C.c_double, C.c_double],
     "gpk_set_kernel": [_vp, C.c_int, C.c_double, C.c_int, _ip, _ip, _dp],
+    "gpk_set_env_factor": [_vp, C.c_int, C.c_double, C.c_double],
     "gpk_fit": [_vp, C.c_double, C.c_double, _dp, _dp],
     "gpk_fit_begin": [_vp, C.c_double, C.c_double],
     "gpk_fit_end": [_vp, _dp, _dp],
@@ -305,6 +306,10 @@ class Handle(object):
         self._check(self.lib.gpk_set_kernel(self._h, int(family), float(log_amp), axis.size,
                                             axis.ctypes.data_as(_ip), group.ctypes.data_as(_ip), _as_dp(lm)))
 
+    def set_env_factor(self, axis, log_a=0.0, log_b=0.0):
+        """gpk_set_env_factor: multiply the kernel by exp(log_a) + exp(log_b) z z' on column axis (-1: remove)."""
+        self._check(self.lib.gpk_set_env_factor(self._h, int(axis), float(log_a), float(log_b)))
+
     def fit(self, diag_add, mean):
         logdet, ll = C.c_double(), C.c_double()
         self._check(self.lib.gpk_fit(self._h, float(diag_add), float(mean), C.byref(logdet), C.byref(ll)))
@@ -454,9 +459,10 @@ class Handle(object):
                                              float(par), _as_dp(out), C.byref(nn)))
         return out, nn.value
 
-    def nll_grad(self, noise_var, n_terms):
-        """d(-loglik)/d[log_amp, log_metric_t..., log sigma^2] of the current fit."""
-        g = np.empty(n_terms + 2)
+    def nll_grad(self, noise_var, n_terms, env=False):
+        """d(-loglik)/d[log_amp, log_metric_t..., (log_a, log_b with the environment factor,) log sigma^2] of the
+        current fit."""
+        g = np.empty(n_terms + (4 if env else 2))
         self._check(self.lib.gpk_nll_grad(self._h, float(noise_var), _as_dp(g)))
         return g
 
@@ -1234,10 +1240,12 @@ def sample_representers(models, seeds, nb, steps, max_runs, kind, eta, par, lowe
 
 def set_hyper_model(handle, slots, n_terms, mean, tiny, prior_kind=PRIOR_NONE, prior_par=None, n_ls=0, n_lr=0):
     """gpk_set_hyper_model: theta -> the handle's kernel (set_kernel first; its structure is used, not its values).
-    slots: kernels.py flatten()["slots"] (one ("amp", None) or ("metric", [terms]) per kernel parameter); n_terms: the
-    kernel's metric terms; mean / tiny: the constant mean and the jitter added to yerr^2; prior_par: the 7 constants of
-    include/gpk.h (None without a prior)."""
-    amp = np.array([1 if kind == "amp" else 0 for kind, _ in slots], dtype=np.int32)
+    slots: kernels.py flatten()["slots"] (one ("amp", None), ("metric", [terms]), ("lin_a", None) or ("lin_b", None)
+    per kernel parameter; the last two need the environment factor set on the handle); n_terms: the kernel's metric
+    terms; mean / tiny: the constant mean and the jitter added to yerr^2; prior_par: the 7 constants of include/gpk.h
+    (None without a prior)."""
+    kinds = {"metric": 0, "amp": 1, "lin_a": 2, "lin_b": 3}
+    amp = np.array([kinds[kind] for kind, _ in slots], dtype=np.int32)
     term = np.full(int(n_terms), -1, dtype=np.int32)
     for p, (kind, terms) in enumerate(slots):
         if kind == "metric":

@@ -328,8 +328,11 @@ inline size_t cov_operand_rows(const gpk_handle* h, int d) { return (size_t)std:
 // out[c][j] = k(cand_c, point_j) for m candidates (row-major raw inputs, bounds lo / up applied on the fly) against
 // the n points of `operand` (built by build_cov_operand, ld = ldx columns); out has ldo columns and at least
 // round_up(m, tile) rows.  small: the 128 x 16 tile variant that fits next to a resident variance-GEMM CTA.
+// pts (row-major raw inputs, dc columns, bounds plo / pup) are the operand's n points before build_cov_operand: the
+// environment factor reads its coordinate there, since the term-major operand carries the radial terms only.
 int launch_cov_tiles(gpk_handle* h, cudaStream_t st, const double* operand, long ldx, int n, const double* cand, int dc,
-                     long m, long m_padded, const double* lo, const double* up, double* out, long ldo, int tri, bool small) {
+                     long m, long m_padded, const double* lo, const double* up, double* out, long ldo, int tri, bool small,
+                     const double* pts, const double* plo, const double* pup) {
     const unsigned gx = (unsigned)(ldx / 128);
     if (cov_tma(h)) {
         CUtensorMap map;
@@ -347,6 +350,11 @@ int launch_cov_tiles(gpk_handle* h, cudaStream_t st, const double* operand, long
         gpk_cov_kernel<16><<<dim3(gx, (unsigned)(m_padded / 32)), 256, 0, st>>>(h->spec, operand, ldx, n, cand, dc, m, lo, up, out, ldo, tri);
     }
     CKL();
+    if (h->spec.env_axis >= 0 && m > 0) {
+        gpk_env_scale_kernel<<<dim3(gx, (unsigned)std::min<long>((m + 1) / 2, 1024)), 256, 0, st>>>(
+            h->spec, cand, dc, m, lo, up, pts, dc, n, plo, pup, out, ldo, tri);
+        CKL();
+    }
     return GPK_OK;
 }
 inline const double* train_operand(const gpk_handle* h) { return cov_tma(h) ? ptr<double>(h->Xts) : ptr<double>(h->Xt); }
@@ -851,9 +859,10 @@ int make_oz_map(gpk_handle* h, CUtensorMap* map, void* base, long rows_total, lo
 
 // Slices of L^-1 for the int8 contraction, once per factorisation.  Returns true in *usable when the factor is
 // conditioned well enough for S = 8 slices (row exponents <= OZ_MAX_EXP) and the sizes fit the int32 accumulators.
+// A kernel with the environment factor is never eligible: the digit split of K* assumes 0 < k <= amp.
 int prepare_ozaki(gpk_handle* h, bool* usable) {
     *usable = false;
-    if (!h->ozaki || h->loader == LOADER_CPASYNC || h->NP > 16384) return GPK_OK;
+    if (!h->ozaki || h->loader == LOADER_CPASYNC || h->NP > 16384 || h->spec.env_axis >= 0) return GPK_OK;
     const long NP = h->NP;
     if (h->oz_linv_serial != h->linv_serial) {
         int rc;
@@ -982,7 +991,8 @@ int score_dev(gpk_handle* h, const double* dX, long m, int kind, double eta, dou
         const double* up = h->has_bounds ? ptr<double>(h->upper) : nullptr;
         if (!use_oz)
             return launch_cov_tiles(h, st, train_operand(h), NP, h->n, dX + base * h->d, h->d, mc, mcp, lo, up,
-                                    second ? ptr<double>(h->Kstar2) : ptr<double>(h->Kstar), NP, 0, small);
+                                    second ? ptr<double>(h->Kstar2) : ptr<double>(h->Kstar), NP, 0, small,
+                                    ptr<double>(h->Xrow), nullptr, nullptr);
         // K* never reaches HBM in fp64: digits + this tile's share of the mean straight out of the builder
         CUtensorMap map;
         int mrc = make_cov_map(h, &map, (void*)train_operand(h), h->spec.n_terms, NP);
@@ -992,10 +1002,12 @@ int score_dev(gpk_handle* h, const double* dX, long m, int kind, double eta, dou
         const int gx = (int)(NP / 128);
         if (small)
             gpk_cov_oz_kernel<4><<<(unsigned)(gx * (mcp / 16)), 256, cov_oz_smem_bytes(h->spec.n_terms, 4), st>>>(
-                map, h->spec, h->n, dX + base * h->d, h->d, mc, lo, up, ptr<double>(h->alpha), oz_eK, qdst, NP, cap * NP, pmu, cap, gx);
+                map, h->spec, h->n, dX + base * h->d, h->d, mc, lo, up, ptr<double>(h->alpha), oz_eK, qdst, NP, cap * NP, pmu, cap, gx,
+                nullptr);
         else
             gpk_cov_oz_kernel<8><<<(unsigned)(gx * (mcp / 32)), 256, cov_oz_smem_bytes(h->spec.n_terms, 8), st>>>(
-                map, h->spec, h->n, dX + base * h->d, h->d, mc, lo, up, ptr<double>(h->alpha), oz_eK, qdst, NP, cap * NP, pmu, cap, gx);
+                map, h->spec, h->n, dX + base * h->d, h->d, mc, lo, up, ptr<double>(h->alpha), oz_eK, qdst, NP, cap * NP, pmu, cap, gx,
+                nullptr);
         CKL();
         return GPK_OK;
     };
@@ -1052,6 +1064,12 @@ int score_dev(gpk_handle* h, const double* dX, long m, int kind, double eta, dou
         f.part_mu = ptr<double>(h->part_mu); f.part_ssq = ptr<double>(h->part_ssq);
         f.ldpart = cap; f.nparts = h->nb; f.m = mc; f.base = global_base + index_offset + base;
         f.kss = h->spec.amp; f.mean = h->mean;
+        if (h->spec.env_axis >= 0) {
+            f.env_axis = h->spec.env_axis; f.env_c0 = h->spec.env_c0; f.env_c1 = h->spec.env_c1;
+            f.env_cand = dX + base * h->d; f.env_dc = h->d;
+            f.env_lo = h->has_bounds ? ptr<double>(h->lower) : nullptr;
+            f.env_up = h->has_bounds ? ptr<double>(h->upper) : nullptr;
+        }
         f.norm_out = h->norm_out; f.y_mean = h->y_mean; f.y_std = h->y_std;
         f.acq_kind = kind; f.eta = eta; f.par = par;
         f.out_mu = d_mu ? d_mu + index_offset + base : nullptr;
@@ -1123,7 +1141,7 @@ int predict_mean_dev(gpk_handle* h, const double* dX, long m, double* d_mu) {
         const long mcp = round_up(mc, BM);
         gpk_cov_oz_kernel<8, false><<<(unsigned)(gx * (mcp / 32)), 256, cov_oz_smem_bytes(h->spec.n_terms, 8), h->stream>>>(
             map, h->spec, h->n, dX + base * h->d, h->d, mc, lo, up, ptr<double>(h->alpha), 0, nullptr, NP, 0,
-            ptr<double>(h->part_mu), cap, gx);
+            ptr<double>(h->part_mu), cap, gx, ptr<double>(h->Xrow));
         CKL();
         gpk_mu_parts_finish_kernel<<<(unsigned)((mc + 255) / 256), 256, 0, h->stream>>>(
             ptr<double>(h->part_mu), cap, h->nb, mc, h->mean, h->norm_out, h->y_mean, h->y_std, d_mu + base);
@@ -1457,6 +1475,7 @@ int gpk_create(gpk_handle** out, int device) {
     gpk_handle* h = new gpk_handle();
     h->device = device;
     memset(&h->spec, 0, sizeof(h->spec));
+    h->spec.env_axis = -1;
     if (cudaSetDevice(device) != cudaSuccess) { delete h; return GPK_CUDA_ERROR; }
     {
         int lo = 0, hi = 0;
@@ -1545,7 +1564,9 @@ int gpk_set_option(gpk_handle* h, const char* key, long value) {
         return GPK_OK;
     }
     if (!strcmp(key, "ozaki")) {
-        if (value != 0 && value != 1) BAD("ozaki must be 0 (fp64 DMMA) or 1 (int8 tensor pipe, error-free split)");
+        if (value != 0 && value != 1)
+            BAD("ozaki must be 0 (fp64 DMMA) or 1 (int8 tensor pipe, error-free split; kernels with the environment "
+                "factor always take fp64)");
         h->ozaki = (int)value;
         return GPK_OK;
     }
@@ -1693,10 +1714,25 @@ int gpk_set_kernel(gpk_handle* h, int family, double log_amp, int n_terms, const
         s.last[t] = (t == n_terms - 1) || (group[t + 1] != group[t]);
     }
     if (group[0] != 0) BAD("gpk_set_kernel: groups must start at 0");
+    s.env_axis = -1;
     h->spec = s;
     h->log_amp = log_amp;
     h->log_metric.assign(log_metric, log_metric + n_terms);
     h->has_spec = true;
+    h->fitted = false;
+    h->linv_ready = false;
+    h->alpha_ready = false;
+    return GPK_OK;
+}
+
+int gpk_set_env_factor(gpk_handle* h, int axis, double log_a, double log_b) {
+    if (!h) return GPK_BAD_ARG;
+    if (gp_refusal(h)) BAD("gpk_set_env_factor: %s", gp_refusal(h));
+    if (axis < -1 || axis >= GPK_MAX_TERMS) BAD("gpk_set_env_factor: axis %d out of range", axis);
+    if (!std::isfinite(log_a) || !std::isfinite(log_b)) BAD("gpk_set_env_factor: log_a and log_b must be finite");
+    h->spec.env_axis = axis;
+    h->spec.env_c0 = axis >= 0 ? exp(log_a) : 0.0;
+    h->spec.env_c1 = axis >= 0 ? exp(log_b) : 0.0;
     h->fitted = false;
     h->linv_ready = false;
     h->alpha_ready = false;
@@ -1709,6 +1745,7 @@ int gpk_fit_begin(gpk_handle* h, double diag_add, double mean) {
     CK(cudaSetDevice(h->device));
     for (int t = 0; t < h->spec.n_terms; ++t)
         if (h->spec.axis[t] >= h->d) BAD("gpk_fit: kernel axis %d >= d = %d", h->spec.axis[t], h->d);
+    if (h->spec.env_axis >= h->d) BAD("gpk_fit: environment axis %d >= d = %d", h->spec.env_axis, h->d);
     const long NP = h->NP;
     const int nb = h->nb;
     if (!h->maps_ok && (rc = rebuild_maps(h))) return rc;        // staging mode changed after gpk_set_data
@@ -1727,7 +1764,7 @@ int gpk_fit_begin(gpk_handle* h, double diag_add, double mean) {
                 return rc;
         }
         if ((rc = launch_cov_tiles(h, h->stream, train_operand(h), NP, h->n, ptr<double>(h->Xrow), h->d, (long)h->n, NP,
-                                   nullptr, nullptr, K, NP, 1, false)))
+                                   nullptr, nullptr, K, NP, 1, false, ptr<double>(h->Xrow), nullptr, nullptr)))
             return rc;
         gpk_kfix_kernel<<<(unsigned)((NP + 255) / 256), 256, 0, h->stream>>>(K, NP, h->n, (int)NP, diag_add,
                                                                             ptr<double>(h->y), mean);
@@ -1902,7 +1939,8 @@ int gpk_fit_append(gpk_handle* h, const double* X, const double* y, int n, int d
                 return rc;
         }
         if ((rc = launch_cov_tiles(h, h->stream, train_operand(h), NP, n, ptr<double>(h->Xrow) + (long)N1 * d, d,
-                                   (long)(n - N1), BM, nullptr, nullptr, K + (long)N1 * NP, NP, 0, false)))
+                                   (long)(n - N1), BM, nullptr, nullptr, K + (long)N1 * NP, NP, 0, false,
+                                   ptr<double>(h->Xrow), nullptr, nullptr)))
             return rc;
         gpk_kfix_rows_kernel<<<1, 128, 0, h->stream>>>(K, NP, n, (int)NP, diag_add, N1);
         CKL();
@@ -2217,12 +2255,12 @@ static int predict_cov_impl(gpk_handle* h, const double* Xs, long m, double* mu,
     const double* up = h->has_bounds ? ptr<double>(h->upper) : nullptr;
     // K* (mp x NP)
     if ((rc = launch_cov_tiles(h, h->stream, train_operand(h), NP, h->n, ptr<double>(h->cand), h->d, m, mp, lo, up,
-                               ptr<double>(h->Kstar), NP, 0, false)))
+                               ptr<double>(h->Kstar), NP, 0, false, ptr<double>(h->Xrow), nullptr, nullptr)))
         return rc;
     // K** (mp x mp): candidates against the (scaled, transposed) candidates
     if ((rc = build_cov_operand(h, h->stream, ptr<double>(h->cand), m, h->d, lo, up, ptr<double>(h->XsT), mp))) return rc;
     if ((rc = launch_cov_tiles(h, h->stream, ptr<double>(h->XsT), mp, (int)m, ptr<double>(h->cand), h->d, m, mp, lo, up,
-                               ptr<double>(h->cov), mp, 0, false)))
+                               ptr<double>(h->cov), mp, 0, false, ptr<double>(h->cand), lo, up)))
         return rc;
     // V^T = (L^-1 K*^T)^T  ->  Vt[cand][i]
     std::vector<GemmJob> jobs;
@@ -2317,7 +2355,7 @@ int gpk_predict_grad(gpk_handle* h, const double* Xs, long m, int kind, double e
     if ((rc = ensure_score_scratch(h, mp))) return rc;       // score_dev may have sized the K* map for a smaller chunk
     // K* again into the first buffer (score_dev may have used either), then Vt = (L^-1 K*^T)^T, Wt = (L^-T V)^T
     if ((rc = launch_cov_tiles(h, h->stream, train_operand(h), NP, h->n, ptr<double>(h->cand), d, m, mp, lo, up,
-                               ptr<double>(h->Kstar), NP, 0, false)))
+                               ptr<double>(h->Kstar), NP, 0, false, ptr<double>(h->Xrow), nullptr, nullptr)))
         return rc;
     std::vector<GemmJob> jobs;
     for (int ib = nb - 1; ib >= 0; --ib)
@@ -2446,17 +2484,29 @@ int gpk_set_hyper_model(gpk_handle* h, int n_params, const int* amp_slot, const 
     m.n_terms = n_terms;
     m.n_params = n_params;
     std::vector<int> used(n_params, 0);
-    for (int p = 0; p < n_params; ++p) m.amp[p] = amp_slot[p] ? 1 : 0;
+    m.env_axis = m.env_pa = m.env_pb = -1;
+    for (int p = 0; p < n_params; ++p) {
+        if (amp_slot[p] < 0 || amp_slot[p] > 3) BAD("%s: slot kind %d of parameter %d is not 0..3", who, amp_slot[p], p);
+        m.amp[p] = amp_slot[p] == 1 ? 1 : 0;
+        int* env_p = amp_slot[p] == 2 ? &m.env_pa : amp_slot[p] == 3 ? &m.env_pb : nullptr;
+        if (env_p) {
+            if (*env_p >= 0) BAD("%s: more than one log_%c slot", who, amp_slot[p] == 2 ? 'a' : 'b');
+            *env_p = p;
+        }
+    }
+    if ((m.env_pa >= 0) != (m.env_pb >= 0) || (m.env_pa >= 0) != (h->spec.env_axis >= 0))
+        BAD("%s: the log_a / log_b slots must match the kernel's environment factor", who);
+    m.env_axis = h->spec.env_axis;
     for (int t = 0; t < n_terms; ++t) {
         const int p = term_param[t];
-        if (p < 0 || p >= n_params || m.amp[p]) BAD("%s: term %d is not set by a metric slot", who, t);
+        if (p < 0 || p >= n_params || amp_slot[p] != 0) BAD("%s: term %d is not set by a metric slot", who, t);
         m.axis[t] = h->spec.axis[t];
         m.last[t] = h->spec.last[t];
         m.term_param[t] = p;
         used[p] = 1;
     }
     for (int p = 0; p < n_params; ++p)
-        if (!m.amp[p] && !used[p]) BAD("%s: metric slot %d sets no term", who, p);
+        if (amp_slot[p] == 0 && !used[p]) BAD("%s: metric slot %d sets no term", who, p);
     m.mean = mean;
     m.tiny = tiny;
     m.prior = prior_kind;
@@ -2477,6 +2527,8 @@ int hyper_ready(gpk_handle* h, int dim, const char* who) {
     int rc = require(h, true, true, false);
     if (rc) return rc;
     if (!h->has_hyper) BAD("%s: gpk_set_hyper_model has not been called", who);
+    if (h->hyper.env_axis != h->spec.env_axis) BAD("%s: the kernel structure changed since gpk_set_hyper_model", who);
+    if (h->spec.env_axis >= h->d) BAD("%s: environment axis %d >= d = %d", who, h->spec.env_axis, h->d);
     const HyperModel& m = h->hyper;
     if (m.n_terms != h->spec.n_terms || m.family != h->spec.family)
         BAD("%s: the kernel structure changed since gpk_set_hyper_model", who);
@@ -2853,6 +2905,7 @@ int gpk_kernel_matrix(gpk_handle* h, const double* X1, long n1, const double* X2
     if (!X1 || !X2 || !out || n1 <= 0 || n2 <= 0 || d <= 0 || d > GPK_MAX_TERMS) BAD("gpk_kernel_matrix: bad arguments");
     for (int t = 0; t < h->spec.n_terms; ++t)
         if (h->spec.axis[t] >= d) BAD("gpk_kernel_matrix: kernel axis %d >= d = %d", h->spec.axis[t], d);
+    if (h->spec.env_axis >= d) BAD("gpk_kernel_matrix: environment axis %d >= d = %d", h->spec.env_axis, d);
     CK(cudaSetDevice(h->device));
     const long n1p = round_up(n1, 32), n2p = round_up(n2, 128);
     if ((rc = ensure(h, h->tmp1, (size_t)n1 * d * 8))) return rc;
@@ -2865,7 +2918,7 @@ int gpk_kernel_matrix(gpk_handle* h, const double* X1, long n1, const double* X2
     CK(cudaMemcpyAsync(X2row, X2, (size_t)n2 * d * 8, cudaMemcpyHostToDevice, h->stream));
     if ((rc = build_cov_operand(h, h->stream, X2row, n2, d, nullptr, nullptr, X2t, n2p))) return rc;
     if ((rc = launch_cov_tiles(h, h->stream, X2t, n2p, (int)n2, ptr<double>(h->tmp1), d, n1, n1p, nullptr, nullptr,
-                               ptr<double>(h->tmp3), n2p, 0, false)))
+                               ptr<double>(h->tmp3), n2p, 0, false, X2row, nullptr, nullptr)))
         return rc;
     CK(cudaMemcpy2DAsync(out, (size_t)n2 * 8, h->tmp3.p, (size_t)n2p * 8, (size_t)n2 * 8, (size_t)n1,
                          cudaMemcpyDeviceToHost, h->stream));
@@ -2880,7 +2933,7 @@ int gpk_nll_grad(gpk_handle* h, double noise_var, double* grad) {
     CK(cudaSetDevice(h->device));
     if ((rc = build_linv(h))) return rc;
     const long NP = h->NP;
-    const int nv = h->spec.n_terms + 2;
+    const int nv = h->spec.n_terms + (h->spec.env_axis >= 0 ? 4 : 2);
     // alpha = L^-T z
     if ((rc = ensure(h, h->alpha, (size_t)NP * 8))) return rc;
     gpk_rowdot_kernel<<<(unsigned)((NP + 7) / 8), 256, 0, h->stream>>>(ptr<double>(h->Q), NP, NP, (int)NP, 1,

@@ -361,7 +361,8 @@ __global__ void gpk_ep_apply_kernel(int D, double* __restrict__ dMu, double* __r
 
 #define GPK_ES_THREADS 256
 
-// k(a, b) of the handle's kernel on scaled inputs: amp * prod_g f(sum_{t in g} (a - b)^2 / metric_t)
+// k(a, b) of the handle's kernel on scaled inputs: amp * prod_g f(sum_{t in g} (a - b)^2 / metric_t), times the
+// environment factor when the kernel has one
 __device__ __forceinline__ double gpk_es_kval(const KSpec& s, const double* a, const double* b) {
     double prod = 1.0, r2 = 0.0;
     for (int t = 0; t < s.n_terms; ++t) {
@@ -372,7 +373,8 @@ __device__ __forceinline__ double gpk_es_kval(const KSpec& s, const double* a, c
             r2 = 0.0;
         }
     }
-    return s.amp * prod;
+    const double k = s.amp * prod;
+    return s.env_axis >= 0 ? k * gpk_env(s.env_c0, s.env_c1, a[s.env_axis], b[s.env_axis]) : k;
 }
 
 // raw representer points -> scaled (x - lower) / (upper - lower) when the handle scales its inputs

@@ -8,7 +8,8 @@
 //   - kernel: log_amp = 0.0 + the amplitude-slot entries in slot order, amp = exp(log_amp); every term t takes
 //     inv_metric_t = 1 / exp(theta[term_param[t]]) (an isotropic metric slot lists all the terms of its group);
 //     K_ij = amp prod_g gpk_radial(family, sum_{t in g} (x_i - x_j)^2 inv_metric_t) on the handle's inputs, family /
-//     axes / groups of the handle's KSpec
+//     axes / groups of the handle's KSpec; with the environment factor (gpk_set_env_factor) K_ij is multiplied by
+//     gpk_env(exp(theta[env_pa]), exp(theta[env_pb]), z_i, z_j), z = input column env_axis
 //   - diagonal: diag_add = fl(sqrt(fl(yerr^2 + tiny)))^2, yerr = sqrt(exp(theta[-1]))  (_LikelihoodPool.loglik)
 //   - packed fp64 lower triangle in shared memory (n <= GPK_HYPER_MAX_N), right-looking Cholesky one column at a time
 //     with the residual r = y - mean carried as an extra row, so r ends as z = L^-1 r; a pivot that is not > 0 (NaN
@@ -49,6 +50,7 @@ struct HyperModel {
     int last[GPK_MAX_TERMS];
     int term_param[GPK_MAX_TERMS];            // the metric slot (parameter index) of term t
     unsigned char amp[GPK_HYPER_MAX_DIM];     // 1: parameter p is an amplitude slot
+    int env_axis, env_pa, env_pb;             // environment factor: its column and the parameters log_a, log_b (-1: none)
     double mean, tiny;
     int prior, n_ls, n_lr;
     double ln_sigma, ln_loc, th_lo, th_hi, hs_scale, nrm_sigma, nrm_mean;
@@ -57,7 +59,7 @@ struct HyperModel {
 // doubles of dynamic shared memory gpk_hy_eval needs for n training points
 __host__ __device__ inline long gpk_hy_smem_doubles(int n)
 {
-    return (long)n * (n + 1) / 2 + n + (n + 1) + 2 * GPK_HY_THREADS + 4 + GPK_MAX_TERMS;
+    return (long)n * (n + 1) / 2 + n + (n + 1) + 2 * GPK_HY_THREADS + 6 + GPK_MAX_TERMS;
 }
 
 // scipy.stats.lognorm.logpdf(x, s, loc=loc): -inf for x <= loc, NaN stays NaN
@@ -133,8 +135,8 @@ __device__ void gpk_hy_eval(const HyperModel& m, const double* __restrict__ Xt, 
     double* r = A + (long)n * (n + 1) / 2;           // y - mean, then z = L^-1 (y - mean)
     double* col = r + n;                             // column k of L (rows k + 1 .. n; row n = the residual row)
     double* red = col + n + 1;                       // 2 NT partial sums
-    double* par = red + 2 * NT;                      // amp, diag_add, lp, ll
-    double* im = par + 4;                            // inv_metric of every term
+    double* par = red + 2 * NT;                      // amp, diag_add, lp, ll, env c0, env c1
+    double* im = par + 6;                            // inv_metric of every term
 
     bool out = false;
     for (int j = 0; j < D; ++j) out = out || th[j] < -20.0 || th[j] > 20.0;
@@ -147,6 +149,7 @@ __device__ void gpk_hy_eval(const HyperModel& m, const double* __restrict__ Xt, 
         const double yerr = sqrt(exp(th[D - 1]));
         const double s = sqrt(__dadd_rn(__dmul_rn(yerr, yerr), m.tiny));
         par[1] = __dmul_rn(s, s);
+        if (m.env_axis >= 0) { par[4] = exp(th[m.env_pa]); par[5] = exp(th[m.env_pb]); }
     }
     for (int t = tid; t < m.n_terms; t += NT) im[t] = 1.0 / exp(th[m.term_param[t]]);
     __syncthreads();
@@ -163,7 +166,11 @@ __device__ void gpk_hy_eval(const HyperModel& m, const double* __restrict__ Xt, 
                     r2 = fma(d * d, im[t], r2);
                     if (m.last[t]) { pr *= gpk_radial(m.family, r2); r2 = 0.0; }
                 }
-                const double v = amp * pr;
+                double v = amp * pr;
+                if (m.env_axis >= 0) {
+                    const double* za = Xt + (long)m.env_axis * ldx;
+                    v *= gpk_env(par[4], par[5], za[i], za[j]);
+                }
                 row[j] = (j == i) ? v + dg : v;
             }
             if (lane == 0) r[i] = y[i] - m.mean;

@@ -20,7 +20,24 @@ struct KSpec {
     double inv_metric[GPK_MAX_TERMS];
     double scale[GPK_MAX_TERMS];    // sqrt(c_f / metric_t): coordinates pre-scaled so that q = sum (s - s')^2 is the
                                     // radial argument directly (c_f = 5 Matern-5/2, 3 Matern-3/2, 1/2 ExpSquared)
+    // environment factor (gpk_set_env_factor): k *= env_c0 + env_c1 * z * z', z = x[env_axis] after the input-bounds
+    // scaling; env_axis = -1: none
+    int env_axis;
+    double env_c0, env_c1;
 };
+
+// The environment factor of Fabolas, restated from arXiv:1605.07079 (not checked against the george fork that defines
+// BayesianLinearRegressionKernel): c0 + c1 z z', with c0 = exp(log_a), c1 = exp(log_b).  Its derivatives are
+// d/dlog_a = c0, d/dlog_b = c1 z z', d/dz = c1 z' (gpk_env_dz).  Test restatement: tests/env_kernel_model.py (env_value).
+__device__ __forceinline__ double gpk_env(double c0, double c1, double z, double z2) { return fma(c1 * z, z2, c0); }
+__device__ __forceinline__ double gpk_env_dz(double c1, double z2) { return c1 * z2; }
+
+// x[axis] of one row of raw inputs, scaled (x - lower) / (upper - lower) when bounds are given
+__device__ __forceinline__ double gpk_env_coord(const double* row, int axis, const double* lower, const double* upper) {
+    double v = row[axis];
+    if (lower != nullptr) v = (v - lower[axis]) / (upper[axis] - lower[axis]);
+    return v;
+}
 
 // f as a function of q = c_f * r2 (pre-scaled coordinates, gpk_cov_tma_kernel)
 __device__ __forceinline__ double gpk_radial_q(int family, double q) {

@@ -162,6 +162,27 @@ gpk_cov_tma_kernel(const __grid_constant__ CUtensorMap mapX, const KSpec ks, int
     }
 }
 
+// Environment factor over a tile the builders above wrote: out[c][j] *= c0 + c1 z_c z_j, z = column env_axis of the
+// candidates (row-major raw inputs cand, bounds lo / up) and of the points (row-major raw inputs pts, bounds plo / pup).
+// Runs only when the kernel has the factor, so the builders, their registers and their bits stay those of the kernel
+// without it.  tri != 0: only the tiles the triangular K build wrote (column tile start <= the row's 32-row block end).
+__global__ void __launch_bounds__(256)
+gpk_env_scale_kernel(const KSpec ks, const double* __restrict__ cand, int dc, long m,
+                     const double* __restrict__ lo, const double* __restrict__ up,
+                     const double* __restrict__ pts, int dp, int n,
+                     const double* __restrict__ plo, const double* __restrict__ pup,
+                     double* __restrict__ out, long ldo, int tri)
+{
+    const int j = blockIdx.x * 128 + (threadIdx.x & 127);
+    if (j >= n) return;
+    const double zj = gpk_env_coord(pts + (long)j * dp, ks.env_axis, plo, pup);
+    for (long c = (long)blockIdx.y * 2 + (threadIdx.x >> 7); c < m; c += (long)gridDim.y * 2) {
+        if (tri && (long)(j & ~127) > (c | 31)) continue;
+        const double zc = gpk_env_coord(cand + c * dc, ks.env_axis, lo, up);
+        out[c * ldo + j] *= gpk_env(ks.env_c0, ks.env_c1, zc, zj);
+    }
+}
+
 inline size_t cov_tma_smem_bytes(int n_terms, int cc) { return (size_t)n_terms * 1024 + (size_t)4 * cc * n_terms * 8 + 8 + 128; }
 
 // Xs[t][j] = scaled x_j[axis_t] * scale_t  (term-major operand of gpk_cov_tma_kernel), zero padded to ldx columns
@@ -224,6 +245,9 @@ struct FinishArgs {
     long m;                 // valid candidates in this chunk
     long base;              // global index of the chunk's first candidate
     double kss;             // k(x*, x*) = amplitude (stationary kernels)
+    // environment factor: k(x*, x*) = kss * (c0 + c1 z*^2), z* from the chunk's candidates (env_cand NULL: none)
+    int env_axis; double env_c0, env_c1;
+    const double* env_cand; int env_dc; const double* env_lo; const double* env_up;
     double mean;            // GP constant mean
     int norm_out; double y_mean, y_std;
     int acq_kind; double eta, par;
@@ -243,7 +267,12 @@ __global__ void __launch_bounds__(256) gpk_finish_kernel(const FinishArgs f)
             ssq += f.part_ssq[(long)p * f.ldpart + c];
             mu += f.part_mu[(long)p * f.ldpart + c];
         }
-        double var = f.kss - ssq;
+        double kss = f.kss;
+        if (f.env_cand != nullptr) {
+            const double z = gpk_env_coord(f.env_cand + c * f.env_dc, f.env_axis, f.env_lo, f.env_up);
+            kss *= gpk_env(f.env_c0, f.env_c1, z, z);
+        }
+        double var = kss - ssq;
         mu += f.mean;
         if (f.norm_out) { mu = mu * f.y_std + f.y_mean; var = var * (f.y_std * f.y_std); }
         if (var < GPK_EPS) var = GPK_EPS;                  // np.clip(var, eps, inf); NaN stays NaN
@@ -354,6 +383,8 @@ __global__ void gpk_cov_finish_kernel(double* __restrict__ cov, long ld, long m,
 // partial sums: [sum w k, sum_t ..., trace A]; a second kernel adds the CTAs in fixed order.
 //   dk/d log_amp      = k
 //   dk/d log_metric_t = -k * (dlog f / d r2)(r2_g) * (x_t - x'_t)^2 / metric_t      (t in group g)
+// With the environment factor k = amp R (c0 + c1 z z'), nv = n_terms + 4: [sum w k, sum_t ..., log_a, log_b, trace A],
+//   dk/d log_a = amp R c0,   dk/d log_b = amp R c1 z z'
 // ---------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
 gpk_grad_trace_kernel(const KSpec ks, const double* __restrict__ Xt, long ldx, int n,
@@ -362,9 +393,11 @@ gpk_grad_trace_kernel(const KSpec ks, const double* __restrict__ Xt, long ldx, i
                       double* __restrict__ part)
 {
     __shared__ double sc[32][GPK_MAX_TERMS + 1];
+    __shared__ double szc[32];
     __shared__ double red[8];
     const int tid = threadIdx.x;
-    const int nt = ks.n_terms, nv = nt + 2;
+    const bool env = ks.env_axis >= 0;
+    const int nt = ks.n_terms, nv = nt + (env ? 4 : 2);
     const long bid = (long)blockIdx.y * gridDim.x + blockIdx.x;
     const int j = blockIdx.x * 128 + (tid & 127);
     const long c0 = (long)blockIdx.y * 32;
@@ -377,13 +410,15 @@ gpk_grad_trace_kernel(const KSpec ks, const double* __restrict__ Xt, long ldx, i
         long ci = c0 + c;
         sc[c][t] = (ci < n) ? Xrow[ci * dc + ks.axis[t]] : 0.0;
     }
+    if (env && tid < 32) szc[tid] = (c0 + tid < n) ? Xrow[(c0 + tid) * dc + ks.env_axis] : 0.0;
     __syncthreads();
 
     const int cg = (tid >> 7) * 16;
     const bool jv = j < n;
     double gl[GPK_MAX_TERMS];                                // per-term partial sums (local memory)
     for (int t = 0; t < nt; ++t) gl[t] = 0.0;
-    double gamp = 0.0, gtr = 0.0;
+    double gamp = 0.0, gtr = 0.0, genva = 0.0, genvb = 0.0;
+    const double zj = (env && jv) ? Xt[(long)ks.env_axis * ldx + j] : 0.0;
 
     double r2[16], wk[16];
 #pragma unroll
@@ -410,6 +445,12 @@ gpk_grad_trace_kernel(const KSpec ks, const double* __restrict__ Xt, long ldx, i
             if (i == j) { gtr += a; w = a; } else w = 2.0 * a;
         }
         wk[c] = w * ks.amp * wk[c];
+        if (env) {
+            const double zc = szc[cg + c];
+            genva = fma(wk[c], ks.env_c0, genva);
+            genvb = fma(wk[c], ks.env_c1 * zc * zj, genvb);
+            wk[c] *= gpk_env(ks.env_c0, ks.env_c1, zc, zj);
+        }
         gamp += wk[c];
     }
     int t0 = 0;
@@ -444,7 +485,7 @@ gpk_grad_trace_kernel(const KSpec ks, const double* __restrict__ Xt, long ldx, i
     }
     // block reduction of the nv values (fixed order: lanes, then warps)
     for (int v = 0; v < nv; ++v) {
-        double x = (v == 0) ? gamp : (v == nv - 1 ? gtr : gl[v - 1]);
+        double x = (v == 0) ? gamp : (v == nv - 1 ? gtr : (v <= nt ? gl[v - 1] : (v == nt + 1 ? genva : genvb)));
 #pragma unroll
         for (int off = 16; off > 0; off >>= 1) x += __shfl_xor_sync(0xffffffffu, x, off);
         if ((tid & 31) == 0) red[tid >> 5] = x;
@@ -569,6 +610,8 @@ __global__ void gpk_candidates_kernel(unsigned long long seed, long first, long 
 //   d k / d x*_t    =  k * (dlog f / d r2)(r2_g) * 2 (x*_t - x_jt) / metric_t    per kernel term t (axis a = axis[t])
 // One CTA per candidate, threads stride over the training points, block reduction per term, chain
 // rule of the input scaling (1 / (upper - lower)) and of the output transform applied at the end.
+// With the environment factor k = amp R (c0 + c1 z* z_j): the terms above use that k, the environment axis gains
+//   d k / d z* = amp R c1 z_j,   and  d var / d z* gains d k(x*, x*) / d z* = 2 amp c1 z*.
 // ---------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
 gpk_predict_grad_kernel(const KSpec ks, const double* __restrict__ Xt, long ldx, int n,
@@ -581,6 +624,9 @@ gpk_predict_grad_kernel(const KSpec ks, const double* __restrict__ Xt, long ldx,
     __shared__ double red[16];
     const int tid = threadIdx.x, nt = ks.n_terms;
     const long c = blockIdx.x;
+    const bool env = ks.env_axis >= 0;
+    const double zs = env ? gpk_env_coord(cand + c * dc, ks.env_axis, lower, upper) : 0.0;
+    double gem = 0.0, gev = 0.0;                                        // environment-axis sums
     for (int t = tid; t < nt; t += 256) {
         const int a = ks.axis[t];
         double v = cand[c * dc + a];
@@ -597,6 +643,13 @@ gpk_predict_grad_kernel(const KSpec ks, const double* __restrict__ Xt, long ldx,
             const double d = xs[t] - Xt[(long)ks.axis[t] * ldx + j];
             r2 = fma(d * d, ks.inv_metric[t], r2);
             if (ks.last[t]) { k *= gpk_radial(ks.family, r2); r2 = 0.0; }
+        }
+        if (env) {
+            const double zj = Xt[(long)ks.env_axis * ldx + j];
+            const double dkz = k * gpk_env_dz(ks.env_c1, zj);
+            gem = fma(alpha[j], dkz, gem);
+            gev = fma(-2.0 * Wt[c * ldw + j], dkz, gev);
+            k *= gpk_env(ks.env_c0, ks.env_c1, zs, zj);
         }
         const double ka = k * alpha[j], kw = -2.0 * k * Wt[c * ldw + j];
         int t0 = 0;
@@ -638,6 +691,27 @@ gpk_predict_grad_kernel(const KSpec ks, const double* __restrict__ Xt, long ldx,
             dvar[c * dc + a] += sv * scale;
         }
         __syncthreads();
+    }
+    if (env) {
+#pragma unroll
+        for (int pass = 0; pass < 2; ++pass) {
+            double x = pass == 0 ? gem : gev;
+#pragma unroll
+            for (int off = 16; off > 0; off >>= 1) x += __shfl_xor_sync(0xffffffffu, x, off);
+            if ((tid & 31) == 0) red[pass * 8 + (tid >> 5)] = x;
+        }
+        __syncthreads();
+        if (tid == 0) {
+            double sm = 0.0, sv = 0.0;
+            for (int w = 0; w < 8; ++w) { sm += red[w]; sv += red[8 + w]; }
+            sv += 2.0 * ks.amp * ks.env_c1 * zs;                       // d k(x*, x*) / d z*
+            const int a = ks.env_axis;
+            double scale = 1.0;
+            if (lower != nullptr) scale = 1.0 / (upper[a] - lower[a]);
+            if (norm_out) { sm *= y_std; sv *= y_std * y_std; }
+            dmu[c * dc + a] += sm * scale;
+            dvar[c * dc + a] += sv * scale;
+        }
     }
 }
 

@@ -358,6 +358,8 @@ gpk_oz_vargemm_kernel(const __grid_constant__ CUtensorMap mapP, const __grid_con
 // + split kernel (8 B read, 8 B written) + mean dot (8 B read) by 8 B written per element.
 // DIGITS = false compiles the digit stores out (Kq unused): the mean-only prediction (gpk_predict_mean) writes nothing
 // but part_mu, with the same arithmetic and reduction order, so its mean is bit-identical to the int8 scoring pass's.
+// Only that instance applies the environment factor (k *= c0 + c1 z_c z_j, z_j from the row-major training inputs Xenv):
+// the digit split assumes 0 < k <= amp, so scoring with the factor takes the fp64 contraction.
 // ---------------------------------------------------------------------------------------
 template <int CC, bool DIGITS = true>
 __global__ void __launch_bounds__(256, CC == 8 ? 2 : 4)
@@ -365,7 +367,7 @@ gpk_cov_oz_kernel(const __grid_constant__ CUtensorMap mapX, const KSpec ks, int 
                   const double* __restrict__ cand, int dc, long m,
                   const double* __restrict__ lower, const double* __restrict__ upper,
                   const double* __restrict__ alpha, int eK, int8_t* __restrict__ Kq, long ldq, long slice_stride,
-                  double* __restrict__ part_mu, long ldpart, int gx)
+                  double* __restrict__ part_mu, long ldpart, int gx, const double* __restrict__ Xenv)
 {
     // one CTA per (train tile bx of 128 columns, candidate group of 4 CC rows): a 1-D grid of gx x (candidate groups)
     constexpr int TC = 4 * CC;
@@ -441,8 +443,13 @@ gpk_cov_oz_kernel(const __grid_constant__ CUtensorMap mapX, const KSpec ks, int 
     for (int c = 0; c < CC; ++c) {
         const long ci = c0 + cgp * CC + c;
         const bool cv = ci < m;
-        const double k0 = (cv && v0) ? ks.amp * pr[c][0] : 0.0;
-        const double k1 = (cv && v1) ? ks.amp * pr[c][1] : 0.0;
+        double k0 = (cv && v0) ? ks.amp * pr[c][0] : 0.0;
+        double k1 = (cv && v1) ? ks.amp * pr[c][1] : 0.0;
+        if (!DIGITS && ks.env_axis >= 0 && cv) {
+            const double zc = gpk_env_coord(cand + ci * dc, ks.env_axis, lower, upper);
+            if (v0) k0 *= gpk_env(ks.env_c0, ks.env_c1, zc, Xenv[(long)j0 * dc + ks.env_axis]);
+            if (v1) k1 *= gpk_env(ks.env_c0, ks.env_c1, zc, Xenv[(long)(j0 + 1) * dc + ks.env_axis]);
+        }
         if (DIGITS) {
             // digits: two adjacent int8 per slice
             const unsigned long long y0 = oz_digits(k0 * sc), y1 = oz_digits(k1 * sc);

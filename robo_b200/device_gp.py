@@ -117,7 +117,8 @@ class DeviceGP(object):
         yerr_tot = np.sqrt(np.float64(self._yerr) ** 2 + np.exp(self.white_noise))
         diag_add = float(yerr_tot ** 2)
         sig = (int(f["family"]), float(f["log_amp"]), tuple(int(a) for a in f["axis"]),
-               tuple(int(g) for g in f["group"]), tuple(float(v) for v in np.asarray(f["log_metric"]).ravel()), diag_add)
+               tuple(int(g) for g in f["group"]), tuple(float(v) for v in np.asarray(f["log_metric"]).ravel()), diag_add,
+               f["env"])
         self.computed = False
         # Rows appended to an already factorised training set with the same kernel and noise (BaseModel.update /
         # train(do_optimize=False) inside the solver loop): only the last block row of the factor changes.
@@ -141,6 +142,8 @@ class DeviceGP(object):
             self._data_dirty = False
         self._push_cfg()
         h.set_kernel(f["family"], f["log_amp"], f["axis"], f["group"], f["log_metric"])
+        if f["env"] is not None:
+            h.set_env_factor(*f["env"])
         self.log_determinant, self._ll = h.fit(diag_add, self.mean)
         self._fit_x = self._x.copy()
         self._fit_sig = sig
@@ -166,7 +169,7 @@ class DeviceGP(object):
         diag_add = float(yerr_tot ** 2)
         self._pending_sig = (int(f["family"]), float(f["log_amp"]), tuple(int(a) for a in f["axis"]),
                              tuple(int(g) for g in f["group"]),
-                             tuple(float(v) for v in np.asarray(f["log_metric"]).ravel()), diag_add)
+                             tuple(float(v) for v in np.asarray(f["log_metric"]).ravel()), diag_add, f["env"])
         self.computed = False
         self._fit_x = None
         if self._data_dirty:
@@ -174,6 +177,8 @@ class DeviceGP(object):
             self._data_dirty = False
         self._push_cfg()
         h.set_kernel(f["family"], f["log_amp"], f["axis"], f["group"], f["log_metric"])
+        if f["env"] is not None:
+            h.set_env_factor(*f["env"])
         h.fit_begin(diag_add, self.mean)
 
     def compute_end(self):
@@ -211,10 +216,18 @@ class DeviceGP(object):
         if not self.computed:
             raise RuntimeError("You need to compute the model first")
         f = self.kernel.flatten()
-        g = self.handle.nll_grad(noise_var, len(f["axis"]))
+        nt = len(f["axis"])
+        g = self.handle.nll_grad(noise_var, nt) if f["env"] is None else self.handle.nll_grad(noise_var, nt, env=True)
         out = np.empty(len(f["slots"]) + 1)
         for p, (kind, terms) in enumerate(f["slots"]):
-            out[p] = g[0] if kind == "amp" else sum(g[1 + t] for t in terms)
+            if kind == "amp":
+                out[p] = g[0]
+            elif kind == "lin_a":
+                out[p] = g[1 + nt]
+            elif kind == "lin_b":
+                out[p] = g[2 + nt]
+            else:
+                out[p] = sum(g[1 + t] for t in terms)
         out[-1] = g[-1]
         return out
 

@@ -12,7 +12,8 @@ test/test_models/test_gaussian_process.py:44-46).  These classes keep that surfa
 
 Every value is computed on the GPU (gpk_kernel_matrix); nothing here evaluates a kernel on
 the CPU.  Supported algebra: products of ConstantKernel and radial kernels of ONE family
-(Matern-5/2, Matern-3/2 or ExpSquared).  Sums are not representable on the device path and
+(Matern-5/2, Matern-3/2 or ExpSquared), times at most one BayesianLinearRegressionKernel
+(include/gpk.h: gpk_set_env_factor).  Sums are not representable on the device path and
 raise NotImplementedError when flattened.
 """
 import numpy as np
@@ -20,7 +21,7 @@ import numpy as np
 from . import _lib
 
 __all__ = ["Kernel", "ConstantKernel", "Matern52Kernel", "Matern32Kernel", "ExpSquaredKernel",
-           "Product", "Sum"]
+           "BayesianLinearRegressionKernel", "Product", "Sum"]
 
 
 class Kernel(object):
@@ -81,10 +82,11 @@ class Kernel(object):
         raise NotImplementedError
 
     def flatten(self):
-        """-> dict(family, log_amp, axis, group, log_metric, slots) for gpk_set_kernel.
-        slots[i] = ('amp', None) or ('metric', [term indices]) for parameter i, used to map
-        gradients back onto the george parameter vector."""
-        acc = dict(family=None, log_amp=0.0, axis=[], group=[], log_metric=[], slots=[], ngroups=0)
+        """-> dict(family, log_amp, axis, group, log_metric, slots, env) for gpk_set_kernel.
+        slots[i] = ('amp', None), ('metric', [term indices]), ('lin_a', None) or ('lin_b', None) for
+        parameter i, used to map gradients back onto the george parameter vector.  env = None, or
+        (axis, log_a, log_b) of the environment factor (gpk_set_env_factor)."""
+        acc = dict(family=None, log_amp=0.0, axis=[], group=[], log_metric=[], slots=[], ngroups=0, env=None)
         self._collect(acc)
         if acc["family"] is None:
             raise NotImplementedError("the device path needs at least one radial kernel factor")
@@ -105,6 +107,8 @@ class Kernel(object):
         f = self.flatten()
         h = _lib.moments_handle(device)
         h.set_kernel(f["family"], f["log_amp"], f["axis"], f["group"], f["log_metric"])
+        if f["env"] is not None:
+            h.set_env_factor(*f["env"])
         return h.kernel_matrix(x1, x2)
 
 
@@ -184,6 +188,43 @@ class Matern32Kernel(_Radial):
 
 class ExpSquaredKernel(_Radial):
     family = _lib.EXPSQUARED
+
+
+class BayesianLinearRegressionKernel(Kernel):
+    """The environment kernel of Fabolas (robo/fmin/fabolas.py:104-117) on one input column z:
+
+        k(z, z') = exp(log_a) + exp(log_b) * z * z'
+
+    a Bayesian linear regression in the features (1, z) with prior covariance diag(exp(log_a), exp(log_b)).
+    Restated from the Fabolas paper (Klein et al., arXiv:1605.07079) and the reference's call sites: the george fork
+    that defines this kernel is not public, so the definition has not been checked against it.  FabolasGP passes the
+    basis-transformed dataset size as z.  Parameter vector (log_a, log_b)."""
+
+    def __init__(self, log_a, log_b, ndim=1, axes=None):
+        super(BayesianLinearRegressionKernel, self).__init__(ndim, axes)
+        if len(self.axes) != 1:
+            raise ValueError("BayesianLinearRegressionKernel takes exactly one axis")
+        self.log_a, self.log_b = float(log_a), float(log_b)
+
+    def get_parameter_vector(self, include_frozen=False):
+        return np.array([self.log_a, self.log_b])
+
+    def set_parameter_vector(self, vector, include_frozen=False):
+        vector = np.atleast_1d(np.asarray(vector, dtype=np.float64))
+        if len(vector) != 2:
+            raise ValueError("dimension mismatch")
+        self.log_a, self.log_b = float(vector[0]), float(vector[1])
+
+    def get_parameter_names(self, include_frozen=False):
+        return ("log_a", "log_b")
+
+    def _collect(self, acc):
+        if acc["env"] is not None:
+            raise NotImplementedError("products of two BayesianLinearRegressionKernel factors are not supported on "
+                                      "the device")
+        acc["env"] = (int(self.axes[0]), self.log_a, self.log_b)
+        acc["slots"].append(("lin_a", None))
+        acc["slots"].append(("lin_b", None))
 
 
 class _Operator(Kernel):

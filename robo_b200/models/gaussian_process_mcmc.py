@@ -54,6 +54,8 @@ class _LikelihoodPool(object):
                     self.kernel.set_parameter_vector(theta[:-1])
                     f = self.kernel.flatten()
                     h.set_kernel(f["family"], f["log_amp"], f["axis"], f["group"], f["log_metric"])
+                    if f["env"] is not None:
+                        h.set_env_factor(*f["env"])
                     yerr = np.sqrt(np.exp(theta[-1]))
                     diag_add = float(np.sqrt(np.float64(yerr) ** 2 + TINY) ** 2)
                     h.fit_begin(diag_add, self.mean)
@@ -220,6 +222,8 @@ class GaussianProcessMCMC(BaseModel):
         h = self._hyper_handle
         h.set_data(self.X, self.y)
         h.set_kernel(f["family"], f["log_amp"], f["axis"], f["group"], f["log_metric"])
+        if f["env"] is not None:
+            h.set_env_factor(*f["env"])
         _lib.set_hyper_model(h, f["slots"], len(f["axis"]), float(self.mean), TINY, prior_kind, prior_par, n_ls, n_lr)
 
         def run(p0, steps):
