@@ -65,11 +65,15 @@ typedef enum {
 #define GPK_HYPER_MAX_N 232
 #define GPK_HYPER_MAX_DIM 96
 
+/* tasks of the multi-task factor (gpk_set_task_factor): n_tasks (n_tasks + 1) / 2 <= 36 Cholesky entries */
+#define GPK_MAX_TASKS 8
+
 /* hyper-priors the device restates (robo/priors/default_priors.py, robo/priors/env_priors.py) */
 typedef enum {
     GPK_PRIOR_NONE = 0,
     GPK_PRIOR_DEFAULT = 1,     /* DefaultPrior */
-    GPK_PRIOR_ENV = 2          /* EnvPrior     */
+    GPK_PRIOR_ENV = 2,         /* EnvPrior     */
+    GPK_PRIOR_MTBO = 3         /* MTBOPrior    */
 } gpk_prior_kind;
 
 /* ---- lifetime ---------------------------------------------------------------------- */
@@ -87,7 +91,7 @@ const char* gpk_version(void);
  *   "ozaki"     1 = variance contraction on the int8 tensor pipe (wgmma s8, register accumulators) through an
  *               error-free split of L^-1 and K* into 7 balanced base-256 digits each, 28 digit-pair products
  *               (gpk_ozaki.cuh); used while max |L^-1| < 64, N <= 16384 and the kernel has no environment factor
- *               (gpk_set_env_factor), otherwise the fp64 kernel runs [default;
+ *               (gpk_set_env_factor) or task factor (gpk_set_task_factor), otherwise the fp64 kernel runs [default;
  *               batches of >= 2048 candidates]; 0 = always fp64 DMMA.  The posterior mean never goes through the digits
  *               (fp64 K* alpha); the covariance builder writes the digits and the mean partials itself, no fp64 K*
  *               in HBM
@@ -147,6 +151,21 @@ int gpk_set_kernel(gpk_handle* h, int family, double log_amp, int n_terms,
  * an axis outside the data's width is refused by gpk_fit / gpk_kernel_matrix / the hyper sampler.  Scoring with the
  * factor always takes the fp64 contraction (the int8 split assumes 0 < k <= amp). */
 int gpk_set_env_factor(gpk_handle* h, int axis, double log_a, double log_b);
+
+/* Task factor of multi-task Bayesian optimisation (robo/fmin/mtbo.py:101, :134, george's TaskKernel(ndim, axis,
+ * n_tasks)): multiplies the handle's kernel by
+ *     K_t[t, t'],   K_t = L L^T,   L lower triangular n_tasks x n_tasks,   L_pq = exp(theta[p (p + 1) / 2 + q])
+ * on input column `axis`, theta holding the n_tasks (n_tasks + 1) / 2 entries of L packed row by row (L00, L10, L11,
+ * L20, ...).  K_t[a, b] = sum_{q <= min(a, b)} L_aq L_bq in ascending q.  This is a restatement from the paper (Swersky,
+ * Snoek, Adams, NIPS 2013: a free-form positive-definite task covariance) and the reference's call sites; the george
+ * fork that defines the kernel is not public, so it has not been checked against that source.  A coordinate is a task
+ * only when it is an integer in [0, n_tasks): a candidate with any other value gets a NaN factor, and training inputs
+ * with one are refused by gpk_fit.  axis = -1 removes the factor; gpk_set_kernel also removes it.  GPK_BAD_ARG for a
+ * non-finite theta, n_tasks outside 1..GPK_MAX_TASKS, an axis < -1 or an environment factor already set (and
+ * gpk_set_env_factor refuses a task factor); gpk_fit / gpk_kernel_matrix / the hyper sampler refuse an axis outside the
+ * data's width, and gpk_fit refuses input bounds (the task column must reach the kernel unscaled).  Scoring with the
+ * factor always takes the fp64 contraction (K_t entries may exceed 1). */
+int gpk_set_task_factor(gpk_handle* h, int axis, int n_tasks, const double* theta);
 
 /* ---- fit: K build + Cholesky + forward solve + log-det ------------------------------- */
 /* Replaces george GP.compute + GP.log_likelihood (gaussian_process.py:119,155,159):
@@ -394,10 +413,12 @@ int gpk_esmc_get_state(gpk_handle* h, double* Mb, double* Vb);
  * from its start) */
 int gpk_esmc_last_jitter(gpk_handle* h, long* n_jitter);
 
-/* basis functions of the environment column of Fabolas models (robo/fmin/fabolas.py:96-102) */
+/* maps of the last input column of Fabolas models (robo/fmin/fabolas.py:96-102) and MTBO models
+ * (robo/models/mtbo_gp.py:12-15) */
 typedef enum {
-    GPK_BASIS_S = 0,           /* basis(s) = s          (the cost model)      */
-    GPK_BASIS_ONE_MINUS_S_SQ = 1   /* basis(s) = (1 - s)^2  (the objective model) */
+    GPK_BASIS_S = 0,           /* basis(s) = s          (the Fabolas cost model)      */
+    GPK_BASIS_ONE_MINUS_S_SQ = 1,  /* basis(s) = (1 - s)^2  (the Fabolas objective model) */
+    GPK_BASIS_TASK = 2         /* basis(s) = rint(s)    (MTBO: the task index, half to even as np.rint) */
 } gpk_basis;
 
 /* InformationGainPerUnitCost.compute (robo/acquisition_functions/information_gain_per_unit_cost.py:67-106) over n
@@ -713,11 +734,15 @@ int gpk_sample_representers(gpk_handle* const* models, int n, const unsigned lon
  *   its parameter values are not used).  n_params = len(kernel) (theta has n_params + 1 entries, the log noise last);
  *   amp_slot[p] = 1 when parameter p is an amplitude slot (log_amp = 0.0 + those entries in order), 0 for a metric slot,
  *   2 for log_a and 3 for log_b of the environment factor (one each, exactly when gpk_set_env_factor set a factor; its
- *   axis is the handle's);
+ *   axis is the handle's), 4 for an entry of the task factor's Cholesky factor (exactly n_tasks (n_tasks + 1) / 2 of
+ *   them, in packed order, when gpk_set_task_factor set a factor; its axis and n_tasks are the handle's);
  *   term_param[t] (n_terms entries) = the metric slot that sets term t (kernels.py flatten()["slots"]).  The diagonal is
  *   fl(sqrt(fl(yerr^2 + tiny)))^2 with yerr = sqrt(exp(theta[-1])), the constant mean `mean`.  prior_kind: gpk_prior_kind;
  *   prior_par (7 entries, NULL for GPK_PRIOR_NONE) = lognormal sigma, lognormal mean (scipy's loc), tophat lower, tophat
  *   upper, horseshoe scale, normal sigma, normal mean (the last two for GPK_PRIOR_ENV); n_ls, n_lr: EnvPrior's slices.
+ *   GPK_PRIOR_MTBO (MTBOPrior, env_priors.py:188-206): lognorm(theta_0) + Tophat(theta[1:n_ls+1]) + a second tophat
+ *   over theta[n_ls+1:n_ls+1+n_lr] (n_lr = n_kt, the task Cholesky entries) with prior_par[5], prior_par[6] its lower
+ *   and upper bound + Horseshoe(theta[-1]).
  * gpk_hyper_lnpost: the log-likelihood ll (-inf for any |theta_j| > 20, a pivot that is not > 0 or a non-finite result)
  *   and the log-prior lp (0 without a prior) of count thetas (count x dim); the sampler's log-posterior is lp + ll where
  *   ll is finite (ll alone without a prior), -inf otherwise, NaN -> -inf.  The same device routine and block shape as
@@ -856,7 +881,9 @@ int gpk_maximize_random_sharded(gpk_handle* h, unsigned long long seed, long n_t
 /* ---- marginal-likelihood gradient (gaussian_process.py:168-191, corrected noise term) -- */
 /* grad[n_terms + 2] = d(-loglik)/d[log_amp, log_metric_t..., log sigma^2]; requires a
  * preceding successful gpk_fit with the same parameters.  noise_var = sigma^2.  With the environment factor
- * (gpk_set_env_factor) grad has n_terms + 4 entries: [log_amp, log_metric_t..., log_a, log_b, log sigma^2]. */
+ * (gpk_set_env_factor) grad has n_terms + 4 entries: [log_amp, log_metric_t..., log_a, log_b, log sigma^2]; with the
+ * task factor (gpk_set_task_factor) n_terms + 2 + n_kt: [log_amp, log_metric_t..., theta_task (packed)..., log sigma^2],
+ * dK_t[a, b] / dtheta_pq = L_pq (delta_ap L_bq + delta_bp L_aq). */
 int gpk_nll_grad(gpk_handle* h, double noise_var, double* grad);
 
 /* fp64 issue-rate peaks of this GPU in TFLOP/s, measured with register-resident operands: the DMMA

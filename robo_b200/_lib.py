@@ -23,8 +23,9 @@ OBJ_MEAN, OBJ_MEAN_STD = 5, 6                  # GPK_OBJ_MEAN / GPK_OBJ_MEAN_STD
 LB_MAX_D = 64                                  # GPK_LB_MAX_D: largest input dimension of gpk_maximize_lbfgs*
 # gpk_lb_status: why a start of gpk_maximize_lbfgs* stopped (FTOL and PGTOL are scipy's success)
 LB_FTOL, LB_PGTOL, LB_MAXITER, LB_MAXFUN, LB_ABNORMAL, LB_INVALID = range(6)
-BASIS_S, BASIS_ONE_MINUS_S_SQ = range(2)      # gpk_basis: the environment column's basis of a Fabolas model
-PRIOR_NONE, PRIOR_DEFAULT, PRIOR_ENV = range(3)   # gpk_prior_kind: the hyper-priors gpk_sample_hypers restates
+BASIS_S, BASIS_ONE_MINUS_S_SQ, BASIS_TASK = range(3)   # gpk_basis: the last column's map of a Fabolas / MTBO model
+PRIOR_NONE, PRIOR_DEFAULT, PRIOR_ENV, PRIOR_MTBO = range(4)   # gpk_prior_kind: the hyper-priors gpk_sample_hypers restates
+MAX_TASKS = 8                                 # GPK_MAX_TASKS
 HYPER_MAX_N = 232                              # GPK_HYPER_MAX_N: most training points of gpk_sample_hypers
 HYPER_MAX_DIM = 96                             # GPK_HYPER_MAX_DIM: most entries of theta (log noise included)
 BLR_LINEAR, BLR_QUADRATIC, BLR_NONE = range(3)  # gpk_blr_basis: the features of a BayesianLinearRegression handle
@@ -58,6 +59,7 @@ _SIGNATURES = {
     "gpk_set_output_transform": [_vp, C.c_int, C.c_double, C.c_double],
     "gpk_set_kernel": [_vp, C.c_int, C.c_double, C.c_int, _ip, _ip, _dp],
     "gpk_set_env_factor": [_vp, C.c_int, C.c_double, C.c_double],
+    "gpk_set_task_factor": [_vp, C.c_int, C.c_int, _dp],
     "gpk_fit": [_vp, C.c_double, C.c_double, _dp, _dp],
     "gpk_fit_begin": [_vp, C.c_double, C.c_double],
     "gpk_fit_end": [_vp, _dp, _dp],
@@ -310,6 +312,16 @@ class Handle(object):
         """gpk_set_env_factor: multiply the kernel by exp(log_a) + exp(log_b) z z' on column axis (-1: remove)."""
         self._check(self.lib.gpk_set_env_factor(self._h, int(axis), float(log_a), float(log_b)))
 
+    def set_task_factor(self, axis, n_tasks=1, theta=None):
+        """gpk_set_task_factor: multiply the kernel by K_t[t, t'] = (L L^T)[t, t'] on column axis, L_pq =
+        exp(theta[p (p + 1) / 2 + q]) (-1: remove)."""
+        th = None
+        if int(axis) >= 0:
+            th = np.ascontiguousarray(np.asarray(theta, dtype=np.float64).ravel())
+            if th.size != int(n_tasks) * (int(n_tasks) + 1) // 2:
+                raise ValueError("set_task_factor: need n_tasks (n_tasks + 1) / 2 entries")
+        self._check(self.lib.gpk_set_task_factor(self._h, int(axis), int(n_tasks), _as_dp(th) if th is not None else None))
+
     def fit(self, diag_add, mean):
         logdet, ll = C.c_double(), C.c_double()
         self._check(self.lib.gpk_fit(self._h, float(diag_add), float(mean), C.byref(logdet), C.byref(ll)))
@@ -459,10 +471,10 @@ class Handle(object):
                                              float(par), _as_dp(out), C.byref(nn)))
         return out, nn.value
 
-    def nll_grad(self, noise_var, n_terms, env=False):
-        """d(-loglik)/d[log_amp, log_metric_t..., (log_a, log_b with the environment factor,) log sigma^2] of the
-        current fit."""
-        g = np.empty(n_terms + (4 if env else 2))
+    def nll_grad(self, noise_var, n_terms, env=False, n_kt=0):
+        """d(-loglik)/d[log_amp, log_metric_t..., (log_a, log_b with the environment factor, or the n_kt task entries
+        with the task factor,) log sigma^2] of the current fit."""
+        g = np.empty(n_terms + (4 if env else 2) + int(n_kt))
         self._check(self.lib.gpk_nll_grad(self._h, float(noise_var), _as_dp(g)))
         return g
 
@@ -1240,11 +1252,12 @@ def sample_representers(models, seeds, nb, steps, max_runs, kind, eta, par, lowe
 
 def set_hyper_model(handle, slots, n_terms, mean, tiny, prior_kind=PRIOR_NONE, prior_par=None, n_ls=0, n_lr=0):
     """gpk_set_hyper_model: theta -> the handle's kernel (set_kernel first; its structure is used, not its values).
-    slots: kernels.py flatten()["slots"] (one ("amp", None), ("metric", [terms]), ("lin_a", None) or ("lin_b", None)
-    per kernel parameter; the last two need the environment factor set on the handle); n_terms: the kernel's metric
+    slots: kernels.py flatten()["slots"] (one ("amp", None), ("metric", [terms]), ("lin_a", None), ("lin_b", None) or
+    ("task", k) per kernel parameter; lin_a / lin_b need the environment factor set on the handle, the task slots (in
+    packed order) its task factor); n_terms: the kernel's metric
     terms; mean / tiny: the constant mean and the jitter added to yerr^2; prior_par: the 7 constants of include/gpk.h
     (None without a prior)."""
-    kinds = {"metric": 0, "amp": 1, "lin_a": 2, "lin_b": 3}
+    kinds = {"metric": 0, "amp": 1, "lin_a": 2, "lin_b": 3, "task": 4}
     amp = np.array([kinds[kind] for kind, _ in slots], dtype=np.int32)
     term = np.full(int(n_terms), -1, dtype=np.int32)
     for p, (kind, terms) in enumerate(slots):

@@ -2,9 +2,10 @@
 (Swersky et al., NIPS 2013, with the optimisation overhead added to the cost) with its numerical work on the GPU.
 
 The entropy change dh of the objective model divided by the predicted cost, exp(log_cost) + overhead, where log_cost is
-the cost model's predictive MEAN (:91).  Both models are FabolasGP models, which map their inputs on the host
-(configuration columns scaled to [0, 1], the environment column through a basis function); here the whole value is one
-device call (gpk_es_cost_multi): the raw batch is transformed on the device bit for bit as FabolasGP.normalize does, the
+the cost model's predictive MEAN (:91).  Both models are FabolasGP models or both MTBOGP models, which map their inputs
+on the host (configuration columns scaled to [0, 1], the last column through a basis function, or np.rint for MTBO's task
+index); here the whole value is one device call (gpk_es_cost_multi): the raw batch is transformed on the device bit for
+bit as the models' normalize does, the
 objective's entropy change runs on the transformed batch with its bounds test on the raw one (DBL_EPSILON outside the
 raw extended [lower, upper], as the reference's dh_fun tests), the cost model runs a mean-only prediction.
 
@@ -48,10 +49,19 @@ def basis_code(basis_func):
     raise TypeError("InformationGainPerUnitCost runs on the device only for the basis functions s and (1 - s) ** 2")
 
 
+def model_basis(model):
+    """gpk_basis code of the last column's map of a FabolasGP (its basis function) or an MTBOGP (BASIS_TASK)."""
+    from robo_b200.models.mtbo_gp import MTBOGP
+    if isinstance(model, MTBOGP):
+        return _lib.BASIS_TASK
+    return basis_code(model.basis_function)
+
+
 def _fabolas_device(model, role):
     from robo_b200.models.fabolas_gp import FabolasGP
-    if not isinstance(model, FabolasGP) or not hasattr(getattr(model, "gp", None), "handle"):
-        raise TypeError("InformationGainPerUnitCost runs on robo_b200 FabolasGP models (%s model)" % role)
+    from robo_b200.models.mtbo_gp import MTBOGP
+    if not isinstance(model, (FabolasGP, MTBOGP)) or not hasattr(getattr(model, "gp", None), "handle"):
+        raise TypeError("InformationGainPerUnitCost runs on robo_b200 FabolasGP or MTBOGP models (%s model)" % role)
     model.gp._restore()
     model.gp._push_cfg()
     return model.gp.handle
@@ -79,7 +89,7 @@ def device_spec(pairs):
             elif not (_same_bits(mlo, lo) and _same_bits(mup, up)):
                 raise TypeError("InformationGainPerUnitCost on the device needs one set of configuration bounds for the "
                                 "objective and the cost models")
-        codes.add((basis_code(e.model.basis_function), basis_code(e.cost_model.basis_function)))
+        codes.add((model_basis(e.model), model_basis(e.cost_model)))
         overheads.add(float(e.overhead))
     if len(codes) != 1 or len(overheads) != 1:
         raise TypeError("InformationGainPerUnitCost on the device needs one basis per model family and one overhead")
@@ -120,7 +130,7 @@ class InformationGainPerUnitCost(InformationGain):
         lower, upper = self._config_bounds()
         fabolas = dict(cfg_lower=np.asarray(self.model.lower, dtype=np.float64).ravel(),
                        cfg_upper=np.asarray(self.model.upper, dtype=np.float64).ravel(),
-                       basis=basis_code(self.model.basis_function), env_value=float(self.upper[is_env == 1][0]))
+                       basis=model_basis(self.model), env_value=float(self.upper[is_env == 1][0]))
         return handle, np.asarray(lower, dtype=np.float64), np.asarray(upper, dtype=np.float64), fabolas
 
     def _set_representers(self, zb, lmb):
@@ -135,7 +145,8 @@ class InformationGainPerUnitCost(InformationGain):
         proj *= self.upper[self.is_env == 1].shape[0]
         self.zb = np.concatenate((self.zb, proj), axis=1)
 
-    # InformationGain.update's device hooks: FabolasGP handle; zb transformed on the host as the model maps its inputs
+    # InformationGain.update's device hooks: FabolasGP / MTBOGP handle; zb transformed on the host as the model maps its
+    # inputs
     def _device_handle(self, model):
         return _fabolas_device(model, "objective")
 

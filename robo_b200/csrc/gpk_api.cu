@@ -11,6 +11,7 @@
 //   Kstar [chunk][NP]    K(X*, X) of the current candidate chunk
 //   part_mu/part_ssq [nb][chunk]  per-row-block partial sums of the variance contraction
 #include <algorithm>
+#include <climits>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
@@ -89,6 +90,9 @@ struct gpk_handle {
     double log_amp = 0.0;
     std::vector<double> log_metric;
     bool has_bounds = false;
+    std::vector<double> task_theta; // gpk_set_task_factor's packed log-entries (the gradient's contraction)
+    std::vector<int> col_tasks;     // per input column: 1 + the largest value when every value is an integer >= 0 (the
+                                    // fewest tasks that make the column valid task indices), INT_MAX otherwise
     int norm_out = 0;
     double y_mean = 0.0, y_std = 1.0, mean = 0.0, diag_add = 0.0;
 
@@ -350,8 +354,8 @@ int launch_cov_tiles(gpk_handle* h, cudaStream_t st, const double* operand, long
         gpk_cov_kernel<16><<<dim3(gx, (unsigned)(m_padded / 32)), 256, 0, st>>>(h->spec, operand, ldx, n, cand, dc, m, lo, up, out, ldo, tri);
     }
     CKL();
-    if (h->spec.env_axis >= 0 && m > 0) {
-        gpk_env_scale_kernel<<<dim3(gx, (unsigned)std::min<long>((m + 1) / 2, 1024)), 256, 0, st>>>(
+    if ((h->spec.env_axis >= 0 || h->spec.task_axis >= 0) && m > 0) {
+        gpk_factor_scale_kernel<<<dim3(gx, (unsigned)std::min<long>((m + 1) / 2, 1024)), 256, 0, st>>>(
             h->spec, cand, dc, m, lo, up, pts, dc, n, plo, pup, out, ldo, tri);
         CKL();
     }
@@ -859,10 +863,12 @@ int make_oz_map(gpk_handle* h, CUtensorMap* map, void* base, long rows_total, lo
 
 // Slices of L^-1 for the int8 contraction, once per factorisation.  Returns true in *usable when the factor is
 // conditioned well enough for S = 8 slices (row exponents <= OZ_MAX_EXP) and the sizes fit the int32 accumulators.
-// A kernel with the environment factor is never eligible: the digit split of K* assumes 0 < k <= amp.
+// A kernel with the environment or task factor is never eligible: the digit split of K* assumes 0 < k <= amp.
 int prepare_ozaki(gpk_handle* h, bool* usable) {
     *usable = false;
-    if (!h->ozaki || h->loader == LOADER_CPASYNC || h->NP > 16384 || h->spec.env_axis >= 0) return GPK_OK;
+    if (!h->ozaki || h->loader == LOADER_CPASYNC || h->NP > 16384 || h->spec.env_axis >= 0 ||
+        h->spec.task_axis >= 0)
+        return GPK_OK;
     const long NP = h->NP;
     if (h->oz_linv_serial != h->linv_serial) {
         int rc;
@@ -1069,6 +1075,11 @@ int score_dev(gpk_handle* h, const double* dX, long m, int kind, double eta, dou
             f.env_cand = dX + base * h->d; f.env_dc = h->d;
             f.env_lo = h->has_bounds ? ptr<double>(h->lower) : nullptr;
             f.env_up = h->has_bounds ? ptr<double>(h->upper) : nullptr;
+        } else if (h->spec.task_axis >= 0) {
+            f.env_axis = h->spec.task_axis;
+            f.env_cand = dX + base * h->d; f.env_dc = h->d;
+            f.task_n = h->spec.n_tasks;
+            for (int t = 0; t < f.task_n; ++t) f.task_diag[t] = h->spec.task_K[t * f.task_n + t];
         }
         f.norm_out = h->norm_out; f.y_mean = h->y_mean; f.y_std = h->y_std;
         f.acq_kind = kind; f.eta = eta; f.par = par;
@@ -1476,6 +1487,7 @@ int gpk_create(gpk_handle** out, int device) {
     h->device = device;
     memset(&h->spec, 0, sizeof(h->spec));
     h->spec.env_axis = -1;
+    h->spec.task_axis = -1;
     if (cudaSetDevice(device) != cudaSuccess) { delete h; return GPK_CUDA_ERROR; }
     {
         int lo = 0, hi = 0;
@@ -1622,6 +1634,33 @@ int gpk_synchronize(gpk_handle* h) {
     return GPK_OK;
 }
 
+namespace {
+// col_tasks (gpk_handle) of n rows of row-major inputs X (d columns)
+std::vector<int> scan_task_columns(const double* X, int n, int d) {
+    std::vector<int> cols(d, 0);
+    for (int i = 0; i < n; ++i)
+        for (int j = 0; j < d; ++j) {
+            const double v = X[(long)i * d + j];
+            int& c = cols[j];
+            if (c == INT_MAX) continue;
+            c = (v >= 0.0 && v < 1e9 && v == floor(v)) ? std::max(c, (int)v + 1) : INT_MAX;
+        }
+    return cols;
+}
+
+// the task factor's conditions on a training set with column summary cols: axis inside the data, no input bounds,
+// valid task indices
+int task_data_check(gpk_handle* h, const std::vector<int>& cols, const char* who) {
+    const KSpec& s = h->spec;
+    if (s.task_axis < 0) return GPK_OK;
+    if (s.task_axis >= h->d) BAD("%s: task axis %d >= d = %d", who, s.task_axis, h->d);
+    if (h->has_bounds) BAD("%s: the task factor needs unscaled inputs (no input bounds)", who);
+    if ((int)cols.size() != h->d || cols[s.task_axis] > s.n_tasks)
+        BAD("%s: training column %d holds a value that is not a task index in [0, %d)", who, s.task_axis, s.n_tasks);
+    return GPK_OK;
+}
+}  // namespace
+
 int gpk_set_data(gpk_handle* h, const double* X, const double* y, int n, int d) {
     if (!h) return GPK_BAD_ARG;
     if (gp_refusal(h)) BAD("gpk_set_data: %s", gp_refusal(h));
@@ -1659,6 +1698,7 @@ int gpk_set_data(gpk_handle* h, const double* X, const double* y, int n, int d) 
         CKL();
     }
     CK(cudaStreamSynchronize(h->stream));     // host buffers are caller-owned: done with them
+    h->col_tasks = scan_task_columns(X, n, d);
     if ((rc = build_job_tables(h))) return rc;
     if (!h->maps_ok && (rc = rebuild_maps(h))) return rc;
     h->has_data = true;
@@ -1715,6 +1755,7 @@ int gpk_set_kernel(gpk_handle* h, int family, double log_amp, int n_terms, const
     }
     if (group[0] != 0) BAD("gpk_set_kernel: groups must start at 0");
     s.env_axis = -1;
+    s.task_axis = -1;
     h->spec = s;
     h->log_amp = log_amp;
     h->log_metric.assign(log_metric, log_metric + n_terms);
@@ -1730,6 +1771,7 @@ int gpk_set_env_factor(gpk_handle* h, int axis, double log_a, double log_b) {
     if (gp_refusal(h)) BAD("gpk_set_env_factor: %s", gp_refusal(h));
     if (axis < -1 || axis >= GPK_MAX_TERMS) BAD("gpk_set_env_factor: axis %d out of range", axis);
     if (!std::isfinite(log_a) || !std::isfinite(log_b)) BAD("gpk_set_env_factor: log_a and log_b must be finite");
+    if (axis >= 0 && h->spec.task_axis >= 0) BAD("gpk_set_env_factor: the kernel has a task factor");
     h->spec.env_axis = axis;
     h->spec.env_c0 = axis >= 0 ? exp(log_a) : 0.0;
     h->spec.env_c1 = axis >= 0 ? exp(log_b) : 0.0;
@@ -1739,6 +1781,29 @@ int gpk_set_env_factor(gpk_handle* h, int axis, double log_a, double log_b) {
     return GPK_OK;
 }
 
+int gpk_set_task_factor(gpk_handle* h, int axis, int n_tasks, const double* theta) {
+    if (!h) return GPK_BAD_ARG;
+    if (gp_refusal(h)) BAD("gpk_set_task_factor: %s", gp_refusal(h));
+    if (axis < -1 || axis >= GPK_MAX_TERMS) BAD("gpk_set_task_factor: axis %d out of range", axis);
+    if (axis >= 0) {
+        if (n_tasks < 1 || n_tasks > GPK_MAX_TASKS)
+            BAD("gpk_set_task_factor: n_tasks = %d outside 1..%d (GPK_MAX_TASKS)", n_tasks, GPK_MAX_TASKS);
+        if (!theta) BAD("gpk_set_task_factor: need theta");
+        for (int k = 0; k < n_tasks * (n_tasks + 1) / 2; ++k)
+            if (!std::isfinite(theta[k])) BAD("gpk_set_task_factor: theta[%d] is not finite", k);
+        if (h->spec.env_axis >= 0) BAD("gpk_set_task_factor: the kernel has an environment factor");
+        gpk_task_matrix(n_tasks, theta, h->spec.task_K);
+        h->task_theta.assign(theta, theta + n_tasks * (n_tasks + 1) / 2);
+    }
+    h->spec.task_axis = axis;
+    h->spec.n_tasks = axis >= 0 ? n_tasks : 0;
+    h->fitted = false;
+    h->linv_ready = false;
+    h->alpha_ready = false;
+    return GPK_OK;
+}
+
+
 int gpk_fit_begin(gpk_handle* h, double diag_add, double mean) {
     int rc = require(h, true, true, false);
     if (rc) return rc;
@@ -1746,6 +1811,7 @@ int gpk_fit_begin(gpk_handle* h, double diag_add, double mean) {
     for (int t = 0; t < h->spec.n_terms; ++t)
         if (h->spec.axis[t] >= h->d) BAD("gpk_fit: kernel axis %d >= d = %d", h->spec.axis[t], h->d);
     if (h->spec.env_axis >= h->d) BAD("gpk_fit: environment axis %d >= d = %d", h->spec.env_axis, h->d);
+    if ((rc = task_data_check(h, h->col_tasks, "gpk_fit"))) return rc;
     const long NP = h->NP;
     const int nb = h->nb;
     if (!h->maps_ok && (rc = rebuild_maps(h))) return rc;        // staging mode changed after gpk_set_data
@@ -1914,6 +1980,9 @@ int gpk_fit_append(gpk_handle* h, const double* X, const double* y, int n, int d
     CK(cudaSetDevice(h->device));
     int rc;
     if (!h->maps_ok && (rc = rebuild_maps(h))) return rc;
+    // checked before anything is uploaded; committed once the device holds the new rows
+    std::vector<int> cols = scan_task_columns(X, n, d);
+    if ((rc = task_data_check(h, cols, "gpk_fit_append"))) return rc;
     double* K = ptr<double>(h->Kbuf);
     double* P = ptr<double>(h->P);
     double* Q = ptr<double>(h->Q);
@@ -2013,10 +2082,12 @@ int gpk_fit_append(gpk_handle* h, const double* X, const double* y, int n, int d
         h->linv_ready = false;
         h->alpha_ready = false;
         h->n = n;
+        h->col_tasks = std::move(cols);
         set_err(h, "matrix is not positive definite: pivot %d <= 0", st - 1);
         return GPK_NOT_PD;
     }
     h->n = n;
+    h->col_tasks = std::move(cols);
     h->mean = mean;
     h->alpha_ready = false;
     h->linv_serial += 1;                 // L^-1 changed in place: slices / alpha derived from it are stale
@@ -2391,9 +2462,12 @@ int gpk_predict_grad(gpk_handle* h, const double* Xs, long m, int kind, double e
     CKL();
     double* d_dmu = ptr<double>(h->tmp1);
     double* d_dvar = d_dmu + m * d;
-    gpk_predict_grad_kernel<<<(unsigned)m, 256, 0, h->stream>>>(h->spec, ptr<double>(h->Xt), NP, h->n, ptr<double>(h->cand), d,
-                                                              lo, up, ptr<double>(h->alpha), ptr<double>(h->cov), NP,
-                                                              h->norm_out, h->y_std, d_dmu, d_dvar);
+    {
+        auto kern = h->spec.task_axis >= 0 ? gpk_predict_grad_kernel<true> : gpk_predict_grad_kernel<false>;
+        kern<<<(unsigned)m, 256, 0, h->stream>>>(h->spec, ptr<double>(h->Xt), NP, h->n, ptr<double>(h->cand), d, lo, up,
+                                                 ptr<double>(h->alpha), ptr<double>(h->cov), NP, h->norm_out, h->y_std,
+                                                 d_dmu, d_dvar);
+    }
     CKL();
     CK(cudaMemcpyAsync(mu, h->out_mu.p, (size_t)m * 8, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaMemcpyAsync(var, h->out_var.p, (size_t)m * 8, cudaMemcpyDeviceToHost, h->stream));
@@ -2475,9 +2549,10 @@ int gpk_set_hyper_model(gpk_handle* h, int n_params, const int* amp_slot, const 
     if (n_params < 1 || n_params + 1 > GPK_HYPER_MAX_DIM || !amp_slot || !term_param)
         BAD("%s: need 1 <= n_params <= %d and the slot table", who, GPK_HYPER_MAX_DIM - 1);
     if (n_terms != h->spec.n_terms) BAD("%s: %d terms in the slot table, the kernel has %d", who, n_terms, h->spec.n_terms);
-    if (prior_kind < GPK_PRIOR_NONE || prior_kind > GPK_PRIOR_ENV) BAD("%s: unknown prior kind %d", who, prior_kind);
+    if (prior_kind < GPK_PRIOR_NONE || prior_kind > GPK_PRIOR_MTBO) BAD("%s: unknown prior kind %d", who, prior_kind);
     if (prior_kind != GPK_PRIOR_NONE && !prior_par) BAD("%s: the prior needs its constants", who);
-    if (prior_kind == GPK_PRIOR_ENV && (n_ls < 0 || n_lr < 0)) BAD("%s: need n_ls >= 0 and n_lr >= 0", who);
+    if ((prior_kind == GPK_PRIOR_ENV || prior_kind == GPK_PRIOR_MTBO) && (n_ls < 0 || n_lr < 0))
+        BAD("%s: need n_ls >= 0 and n_lr >= 0", who);
     HyperModel m;
     memset(&m, 0, sizeof(m));
     m.family = h->spec.family;
@@ -2485,8 +2560,13 @@ int gpk_set_hyper_model(gpk_handle* h, int n_params, const int* amp_slot, const 
     m.n_params = n_params;
     std::vector<int> used(n_params, 0);
     m.env_axis = m.env_pa = m.env_pb = -1;
+    m.task_axis = -1;
     for (int p = 0; p < n_params; ++p) {
-        if (amp_slot[p] < 0 || amp_slot[p] > 3) BAD("%s: slot kind %d of parameter %d is not 0..3", who, amp_slot[p], p);
+        if (amp_slot[p] < 0 || amp_slot[p] > 4) BAD("%s: slot kind %d of parameter %d is not 0..4", who, amp_slot[p], p);
+        if (amp_slot[p] == 4) {
+            if (m.n_kt == GPK_MAX_TASKS * (GPK_MAX_TASKS + 1) / 2) BAD("%s: too many task slots", who);
+            m.task_p[m.n_kt++] = (unsigned char)p;
+        }
         m.amp[p] = amp_slot[p] == 1 ? 1 : 0;
         int* env_p = amp_slot[p] == 2 ? &m.env_pa : amp_slot[p] == 3 ? &m.env_pb : nullptr;
         if (env_p) {
@@ -2497,6 +2577,11 @@ int gpk_set_hyper_model(gpk_handle* h, int n_params, const int* amp_slot, const 
     if ((m.env_pa >= 0) != (m.env_pb >= 0) || (m.env_pa >= 0) != (h->spec.env_axis >= 0))
         BAD("%s: the log_a / log_b slots must match the kernel's environment factor", who);
     m.env_axis = h->spec.env_axis;
+    if (m.n_kt != (h->spec.task_axis >= 0 ? h->spec.n_tasks * (h->spec.n_tasks + 1) / 2 : 0))
+        BAD("%s: %d task slots, the kernel's task factor has %d entries", who, m.n_kt,
+            h->spec.task_axis >= 0 ? h->spec.n_tasks * (h->spec.n_tasks + 1) / 2 : 0);
+    m.task_axis = h->spec.task_axis;
+    m.n_tasks = h->spec.n_tasks;
     for (int t = 0; t < n_terms; ++t) {
         const int p = term_param[t];
         if (p < 0 || p >= n_params || amp_slot[p] != 0) BAD("%s: term %d is not set by a metric slot", who, t);
@@ -2529,6 +2614,9 @@ int hyper_ready(gpk_handle* h, int dim, const char* who) {
     if (!h->has_hyper) BAD("%s: gpk_set_hyper_model has not been called", who);
     if (h->hyper.env_axis != h->spec.env_axis) BAD("%s: the kernel structure changed since gpk_set_hyper_model", who);
     if (h->spec.env_axis >= h->d) BAD("%s: environment axis %d >= d = %d", who, h->spec.env_axis, h->d);
+    if (h->hyper.task_axis != h->spec.task_axis || h->hyper.n_tasks != h->spec.n_tasks)
+        BAD("%s: the kernel structure changed since gpk_set_hyper_model", who);
+    if ((rc = task_data_check(h, h->col_tasks, who))) return rc;
     const HyperModel& m = h->hyper;
     if (m.n_terms != h->spec.n_terms || m.family != h->spec.family)
         BAD("%s: the kernel structure changed since gpk_set_hyper_model", who);
@@ -2906,6 +2994,7 @@ int gpk_kernel_matrix(gpk_handle* h, const double* X1, long n1, const double* X2
     for (int t = 0; t < h->spec.n_terms; ++t)
         if (h->spec.axis[t] >= d) BAD("gpk_kernel_matrix: kernel axis %d >= d = %d", h->spec.axis[t], d);
     if (h->spec.env_axis >= d) BAD("gpk_kernel_matrix: environment axis %d >= d = %d", h->spec.env_axis, d);
+    if (h->spec.task_axis >= d) BAD("gpk_kernel_matrix: task axis %d >= d = %d", h->spec.task_axis, d);
     CK(cudaSetDevice(h->device));
     const long n1p = round_up(n1, 32), n2p = round_up(n2, 128);
     if ((rc = ensure(h, h->tmp1, (size_t)n1 * d * 8))) return rc;
@@ -2933,6 +3022,7 @@ int gpk_nll_grad(gpk_handle* h, double noise_var, double* grad) {
     CK(cudaSetDevice(h->device));
     if ((rc = build_linv(h))) return rc;
     const long NP = h->NP;
+    const int nT = h->spec.task_axis >= 0 ? h->spec.n_tasks : 0;
     const int nv = h->spec.n_terms + (h->spec.env_axis >= 0 ? 4 : 2);
     // alpha = L^-T z
     if ((rc = ensure(h, h->alpha, (size_t)NP * 8))) return rc;
@@ -2954,15 +3044,46 @@ int gpk_nll_grad(gpk_handle* h, double noise_var, double* grad) {
     }
     dim3 tg((unsigned)(NP / 128), (unsigned)(NP / 32));
     const long nblocks = (long)tg.x * tg.y;
-    if ((rc = ensure(h, h->tmp1, (size_t)nblocks * nv * 8))) return rc;
-    if ((rc = ensure(h, h->tmp2, (size_t)nv * 8))) return rc;
-    gpk_grad_trace_kernel<<<tg, 256, 0, h->stream>>>(h->spec, ptr<double>(h->Xt), NP, h->n, ptr<double>(h->Xrow), h->d,
-                                                     ptr<double>(h->W), NP, ptr<double>(h->alpha), ptr<double>(h->tmp1));
+    if ((rc = ensure(h, h->tmp1, (size_t)nblocks * (nv + nT * nT) * 8))) return rc;
+    if ((rc = ensure(h, h->tmp2, (size_t)(nv + nT * nT) * 8))) return rc;
+    {
+        auto kern = h->spec.task_axis >= 0 ? gpk_grad_trace_kernel<true> : gpk_grad_trace_kernel<false>;
+        kern<<<tg, 256, 0, h->stream>>>(h->spec, ptr<double>(h->Xt), NP, h->n, ptr<double>(h->Xrow), h->d,
+                                        ptr<double>(h->W), NP, ptr<double>(h->alpha), ptr<double>(h->tmp1));
+    }
     CKL();
     gpk_grad_final_kernel<<<nv, 256, 0, h->stream>>>(ptr<double>(h->tmp1), nblocks, nv, noise_var, ptr<double>(h->tmp2));
     CKL();
-    CK(cudaMemcpyAsync(grad, h->tmp2.p, (size_t)nv * 8, cudaMemcpyDeviceToHost, h->stream));
+    if (nT == 0) {
+        CK(cudaMemcpyAsync(grad, h->tmp2.p, (size_t)nv * 8, cudaMemcpyDeviceToHost, h->stream));
+        CK(cudaStreamSynchronize(h->stream));
+        return GPK_OK;
+    }
+    // task factor: the T x T sums G_ab (gpk_grad_task_kernel, times -1/2) contracted with
+    // dK_t[a][b] / dtheta_pq = L_pq (delta_ap L_bq + delta_bp L_aq), L_pq = exp(theta[p (p + 1) / 2 + q])
+    double* tpart = ptr<double>(h->tmp1) + (size_t)nblocks * nv;
+    gpk_grad_task_kernel<<<tg, 256, 0, h->stream>>>(h->spec, ptr<double>(h->Xt), NP, h->n, ptr<double>(h->W), NP,
+                                                    ptr<double>(h->alpha), tpart);
+    CKL();
+    gpk_grad_final_kernel<<<nT * nT, 256, 0, h->stream>>>(tpart, nblocks, nT * nT, 1.0, ptr<double>(h->tmp2) + nv);
+    CKL();
+    std::vector<double> g(nv + nT * nT);
+    CK(cudaMemcpyAsync(g.data(), h->tmp2.p, g.size() * 8, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
+    const int nt = h->spec.n_terms, nkt = nT * (nT + 1) / 2;
+    const double* G = g.data() + nv;
+    std::vector<double> L(nT * nT, 0.0);
+    for (int p = 0; p < nT; ++p)
+        for (int q = 0; q <= p; ++q) L[p * nT + q] = std::exp(h->task_theta[p * (p + 1) / 2 + q]);
+    for (int v = 0; v <= nt; ++v) grad[v] = g[v];
+    for (int p = 0; p < nT; ++p)
+        for (int q = 0; q <= p; ++q) {
+            double acc = 0.0;
+            for (int b = q; b < nT; ++b) acc += G[p * nT + b] * L[b * nT + q];   // a = p, q <= b
+            for (int a = q; a < nT; ++a) acc += G[a * nT + p] * L[a * nT + q];   // b = p, q <= a
+            grad[nt + 1 + p * (p + 1) / 2 + q] = L[p * nT + q] * acc;
+        }
+    grad[nt + 1 + nkt] = g[nv - 1];
     return GPK_OK;
 }
 

@@ -362,7 +362,7 @@ __global__ void gpk_ep_apply_kernel(int D, double* __restrict__ dMu, double* __r
 #define GPK_ES_THREADS 256
 
 // k(a, b) of the handle's kernel on scaled inputs: amp * prod_g f(sum_{t in g} (a - b)^2 / metric_t), times the
-// environment factor when the kernel has one
+// environment or task factor when the kernel has one
 __device__ __forceinline__ double gpk_es_kval(const KSpec& s, const double* a, const double* b) {
     double prod = 1.0, r2 = 0.0;
     for (int t = 0; t < s.n_terms; ++t) {
@@ -374,7 +374,8 @@ __device__ __forceinline__ double gpk_es_kval(const KSpec& s, const double* a, c
         }
     }
     const double k = s.amp * prod;
-    return s.env_axis >= 0 ? k * gpk_env(s.env_c0, s.env_c1, a[s.env_axis], b[s.env_axis]) : k;
+    if (s.env_axis >= 0) return k * gpk_env(s.env_c0, s.env_c1, a[s.env_axis], b[s.env_axis]);
+    return s.task_axis >= 0 ? k * gpk_task(s, a[s.task_axis], b[s.task_axis]) : k;
 }
 
 // raw representer points -> scaled (x - lower) / (upper - lower) when the handle scales its inputs
@@ -566,9 +567,10 @@ __global__ void __launch_bounds__(GPK_ES_THREADS) gpk_es_dh_kernel(const double*
 // ---------------------------------------------------------------------------------------
 // Information gain per unit cost (robo/acquisition_functions/information_gain_per_unit_cost.py) over Fabolas models
 // ---------------------------------------------------------------------------------------
-// FabolasGP.normalize on the device (robo/models/fabolas_gp.py:122-126): out[c][j] = (x_j - lo_j) / (up_j - lo_j) for
-// the d - 1 configuration columns, basis(x_{d-1}) for the last (environment) column.  numpy's (1 - s) ** 2 on an array
-// is one multiply t * t, and its true division is IEEE: the result is bit-identical to the host transform.
+// FabolasGP.normalize / MTBOGP's normalize on the device (robo/models/fabolas_gp.py:122-126, mtbo_gp.py:12-15):
+// out[c][j] = (x_j - lo_j) / (up_j - lo_j) for the d - 1 configuration columns, basis(x_{d-1}) for the last (environment
+// or task) column.  numpy's (1 - s) ** 2 on an array is one multiply t * t, its true division is IEEE, and CUDA's rint
+// rounds half to even as np.rint does: the result is bit-identical to the host transform.
 __global__ void gpk_fabolas_transform_kernel(const double* __restrict__ X, long m, int d, const double* __restrict__ lo,
                                              const double* __restrict__ up, int basis, double* __restrict__ out) {
     const long e = (long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -581,6 +583,8 @@ __global__ void gpk_fabolas_transform_kernel(const double* __restrict__ X, long 
     } else if (basis == GPK_BASIS_ONE_MINUS_S_SQ) {
         const double t = 1.0 - x;
         v = t * t;
+    } else if (basis == GPK_BASIS_TASK) {
+        v = rint(x);
     } else {
         v = x;
     }

@@ -9,7 +9,9 @@
 //     inv_metric_t = 1 / exp(theta[term_param[t]]) (an isotropic metric slot lists all the terms of its group);
 //     K_ij = amp prod_g gpk_radial(family, sum_{t in g} (x_i - x_j)^2 inv_metric_t) on the handle's inputs, family /
 //     axes / groups of the handle's KSpec; with the environment factor (gpk_set_env_factor) K_ij is multiplied by
-//     gpk_env(exp(theta[env_pa]), exp(theta[env_pb]), z_i, z_j), z = input column env_axis
+//     gpk_env(exp(theta[env_pa]), exp(theta[env_pb]), z_i, z_j), z = input column env_axis; with the task factor
+//     (gpk_set_task_factor) by K_t[t_i][t_j] of gpk_task_matrix over the task slots theta[task_p[k]] in packed order,
+//     t = input column task_axis (valid task indices: gpk_fit's check), K_t built by thread 0 into the reduction scratch
 //   - diagonal: diag_add = fl(sqrt(fl(yerr^2 + tiny)))^2, yerr = sqrt(exp(theta[-1]))  (_LikelihoodPool.loglik)
 //   - packed fp64 lower triangle in shared memory (n <= GPK_HYPER_MAX_N), right-looking Cholesky one column at a time
 //     with the residual r = y - mean carried as an extra row, so r ends as z = L^-1 r; a pivot that is not > 0 (NaN
@@ -19,7 +21,9 @@
 //   - prior (thread 0), the reference classes' lnprob restated with their quirks: none; DefaultPrior = lognorm.logpdf
 //     (theta_0, sigma, loc) + Tophat(theta[1:-1]) + Horseshoe(theta[-1]) (+inf at theta == 0); EnvPrior = lognorm(theta_0)
 //     + Tophat(theta[1:n_ls+1]) + sum of NormalPrior.lnprob (the pdf, not its log) over theta[n_ls+1:n_ls+n_lr+1]
-//     + Horseshoe(theta[-1]); Python's slice bounds, the additions in the order of the lnprob methods
+//     + Horseshoe(theta[-1]); MTBOPrior = lognorm(theta_0) + Tophat(theta[1:n_ls+1]) + Tophat(nrm_sigma, nrm_mean as
+//     its bounds)(theta[n_ls+1:n_ls+n_lr+1]) + Horseshoe(theta[-1]); Python's slice bounds, the additions in the order
+//     of the lnprob methods
 //   - log-posterior = fl(lp + ll) where ll is finite (ll alone without a prior), -inf otherwise; NaN -> -inf
 //     (loglikelihood_batch, EnsembleSampler._lnprob_many)
 //
@@ -51,6 +55,8 @@ struct HyperModel {
     int term_param[GPK_MAX_TERMS];            // the metric slot (parameter index) of term t
     unsigned char amp[GPK_HYPER_MAX_DIM];     // 1: parameter p is an amplitude slot
     int env_axis, env_pa, env_pb;             // environment factor: its column and the parameters log_a, log_b (-1: none)
+    int task_axis, n_tasks, n_kt;             // task factor: its column (-1: none), tasks, Cholesky entries
+    unsigned char task_p[GPK_MAX_TASKS * (GPK_MAX_TASKS + 1) / 2];   // the parameter of packed entry k
     double mean, tiny;
     int prior, n_ls, n_lr;
     double ln_sigma, ln_loc, th_lo, th_hi, hs_scale, nrm_sigma, nrm_mean;
@@ -111,6 +117,11 @@ __device__ double gpk_hy_prior(const HyperModel& m, const double* th, int D)
         const int a = min(m.n_ls + 1, D), b = min(m.n_ls + m.n_lr + 1, D);
         for (int j = a; j < b; ++j) lp = __dadd_rn(lp, gpk_hy_normal_pdf(th[j], m.nrm_sigma, m.nrm_mean));
         lp = __dadd_rn(lp, gpk_hy_horseshoe(th[D - 1], m.hs_scale));
+    } else if (m.prior == GPK_PRIOR_MTBO) {
+        lp = __dadd_rn(lp, gpk_hy_lognorm(th[0], m.ln_sigma, m.ln_loc));
+        lp = __dadd_rn(lp, gpk_hy_tophat(th, D, 1, m.n_ls + 1, m.th_lo, m.th_hi));
+        lp = __dadd_rn(lp, gpk_hy_tophat(th, D, m.n_ls + 1, m.n_ls + 1 + m.n_lr, m.nrm_sigma, m.nrm_mean));
+        lp = __dadd_rn(lp, gpk_hy_horseshoe(th[D - 1], m.hs_scale));
     }
     return lp;
 }
@@ -135,6 +146,7 @@ __device__ void gpk_hy_eval(const HyperModel& m, const double* __restrict__ Xt, 
     double* r = A + (long)n * (n + 1) / 2;           // y - mean, then z = L^-1 (y - mean)
     double* col = r + n;                             // column k of L (rows k + 1 .. n; row n = the residual row)
     double* red = col + n + 1;                       // 2 NT partial sums
+    double* kt = red;                                // task factor's K_t during the K build (red is free until the sums)
     double* par = red + 2 * NT;                      // amp, diag_add, lp, ll, env c0, env c1
     double* im = par + 6;                            // inv_metric of every term
 
@@ -150,6 +162,11 @@ __device__ void gpk_hy_eval(const HyperModel& m, const double* __restrict__ Xt, 
         const double s = sqrt(__dadd_rn(__dmul_rn(yerr, yerr), m.tiny));
         par[1] = __dmul_rn(s, s);
         if (m.env_axis >= 0) { par[4] = exp(th[m.env_pa]); par[5] = exp(th[m.env_pb]); }
+        if (m.task_axis >= 0) {
+            double* tt = kt + GPK_MAX_TASKS * GPK_MAX_TASKS;    // the packed entries, gathered
+            for (int k = 0; k < m.n_kt; ++k) tt[k] = th[m.task_p[k]];
+            gpk_task_matrix(m.n_tasks, tt, kt);
+        }
     }
     for (int t = tid; t < m.n_terms; t += NT) im[t] = 1.0 / exp(th[m.term_param[t]]);
     __syncthreads();
@@ -170,6 +187,9 @@ __device__ void gpk_hy_eval(const HyperModel& m, const double* __restrict__ Xt, 
                 if (m.env_axis >= 0) {
                     const double* za = Xt + (long)m.env_axis * ldx;
                     v *= gpk_env(par[4], par[5], za[i], za[j]);
+                } else if (m.task_axis >= 0) {
+                    const double* ta = Xt + (long)m.task_axis * ldx;
+                    v *= kt[(int)ta[i] * m.n_tasks + (int)ta[j]];
                 }
                 row[j] = (j == i) ? v + dg : v;
             }

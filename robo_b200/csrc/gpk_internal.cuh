@@ -24,6 +24,10 @@ struct KSpec {
     // scaling; env_axis = -1: none
     int env_axis;
     double env_c0, env_c1;
+    // task factor (gpk_set_task_factor): k *= task_K[t * n_tasks + t'], t = x[task_axis] (never scaled); task_axis = -1:
+    // none.  At most one of env_axis / task_axis is set.
+    int task_axis, n_tasks;
+    double task_K[GPK_MAX_TASKS * GPK_MAX_TASKS];
 };
 
 // The environment factor of Fabolas, restated from arXiv:1605.07079 (not checked against the george fork that defines
@@ -37,6 +41,44 @@ __device__ __forceinline__ double gpk_env_coord(const double* row, int axis, con
     double v = row[axis];
     if (lower != nullptr) v = (v - lower[axis]) / (upper[axis] - lower[axis]);
     return v;
+}
+
+// The task factor of MTBO, restated from Swersky, Snoek, Adams (NIPS 2013) and the reference's call sites (not checked
+// against the george fork that defines TaskKernel): K_t = L L^T, L lower triangular, L_pq = exp(theta[p (p + 1) / 2 + q])
+// packed row by row; K_t[a][b] = sum_{q <= min(a, b)} L_aq L_bq, multiplied and added in ascending q with no fused
+// multiply-add.  Host and device share this definition; the test restatement is tests/task_kernel_model.py
+// (task_value).  Kt: n x n row-major.
+__host__ __device__ inline void gpk_task_matrix(int n, const double* theta, double* Kt) {
+    for (int a = 0; a < n; ++a)
+        for (int b = 0; b <= a; ++b) {
+            double s = 0.0;
+            for (int q = 0; q <= b; ++q) {
+#ifdef __CUDA_ARCH__
+                s = __dadd_rn(s, __dmul_rn(exp(theta[a * (a + 1) / 2 + q]), exp(theta[b * (b + 1) / 2 + q])));
+#else
+                s = s + exp(theta[a * (a + 1) / 2 + q]) * exp(theta[b * (b + 1) / 2 + q]);   // x86-64: no contraction
+#endif
+            }
+            Kt[a * n + b] = s;
+            Kt[b * n + a] = s;
+        }
+}
+
+// the task a coordinate names: an integer in [0, n), otherwise -1 (NaN included)
+__host__ __device__ __forceinline__ int gpk_task_index(double t, int n) {
+    return (t >= 0.0 && t < (double)n && t == floor(t)) ? (int)t : -1;
+}
+
+// K_t[t][t'] of the kernel's task factor, NaN when either coordinate is not a task
+__device__ __forceinline__ double gpk_task(const KSpec& s, double t, double t2) {
+    const int a = gpk_task_index(t, s.n_tasks), b = gpk_task_index(t2, s.n_tasks);
+    return (a < 0 || b < 0) ? __longlong_as_double(0x7ff8000000000000LL) : s.task_K[a * s.n_tasks + b];
+}
+
+// the kernel's single-column factor (environment or task): its column (-1: none) and its value at coordinates z, z'
+__device__ __forceinline__ int gpk_factor_axis(const KSpec& s) { return s.env_axis >= 0 ? s.env_axis : s.task_axis; }
+__device__ __forceinline__ double gpk_factor(const KSpec& s, double z, double z2) {
+    return s.env_axis >= 0 ? gpk_env(s.env_c0, s.env_c1, z, z2) : gpk_task(s, z, z2);
 }
 
 // f as a function of q = c_f * r2 (pre-scaled coordinates, gpk_cov_tma_kernel)

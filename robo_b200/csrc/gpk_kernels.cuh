@@ -162,12 +162,13 @@ gpk_cov_tma_kernel(const __grid_constant__ CUtensorMap mapX, const KSpec ks, int
     }
 }
 
-// Environment factor over a tile the builders above wrote: out[c][j] *= c0 + c1 z_c z_j, z = column env_axis of the
-// candidates (row-major raw inputs cand, bounds lo / up) and of the points (row-major raw inputs pts, bounds plo / pup).
-// Runs only when the kernel has the factor, so the builders, their registers and their bits stay those of the kernel
-// without it.  tri != 0: only the tiles the triangular K build wrote (column tile start <= the row's 32-row block end).
+// Single-column factor over a tile the builders above wrote: out[c][j] *= gpk_factor(z_c, z_j) (the environment factor
+// c0 + c1 z_c z_j or the task factor K_t[z_c][z_j]), z = column gpk_factor_axis of the candidates (row-major raw inputs
+// cand, bounds lo / up) and of the points (row-major raw inputs pts, bounds plo / pup).  Runs only when the kernel has a
+// factor, so the builders, their registers and their bits stay those of the kernel without it.  tri != 0: only the
+// tiles the triangular K build wrote (column tile start <= the row's 32-row block end).
 __global__ void __launch_bounds__(256)
-gpk_env_scale_kernel(const KSpec ks, const double* __restrict__ cand, int dc, long m,
+gpk_factor_scale_kernel(const KSpec ks, const double* __restrict__ cand, int dc, long m,
                      const double* __restrict__ lo, const double* __restrict__ up,
                      const double* __restrict__ pts, int dp, int n,
                      const double* __restrict__ plo, const double* __restrict__ pup,
@@ -175,11 +176,12 @@ gpk_env_scale_kernel(const KSpec ks, const double* __restrict__ cand, int dc, lo
 {
     const int j = blockIdx.x * 128 + (threadIdx.x & 127);
     if (j >= n) return;
-    const double zj = gpk_env_coord(pts + (long)j * dp, ks.env_axis, plo, pup);
+    const int ax = gpk_factor_axis(ks);
+    const double zj = gpk_env_coord(pts + (long)j * dp, ax, plo, pup);
     for (long c = (long)blockIdx.y * 2 + (threadIdx.x >> 7); c < m; c += (long)gridDim.y * 2) {
         if (tri && (long)(j & ~127) > (c | 31)) continue;
-        const double zc = gpk_env_coord(cand + c * dc, ks.env_axis, lo, up);
-        out[c * ldo + j] *= gpk_env(ks.env_c0, ks.env_c1, zc, zj);
+        const double zc = gpk_env_coord(cand + c * dc, ax, lo, up);
+        out[c * ldo + j] *= gpk_factor(ks, zc, zj);
     }
 }
 
@@ -248,6 +250,9 @@ struct FinishArgs {
     // environment factor: k(x*, x*) = kss * (c0 + c1 z*^2), z* from the chunk's candidates (env_cand NULL: none)
     int env_axis; double env_c0, env_c1;
     const double* env_cand; int env_dc; const double* env_lo; const double* env_up;
+    // task factor instead (task_n > 0): k(x*, x*) = kss * task_diag[t*], t* = column env_axis of env_cand, NaN when t*
+    // is not a task
+    int task_n; double task_diag[GPK_MAX_TASKS];
     double mean;            // GP constant mean
     int norm_out; double y_mean, y_std;
     int acq_kind; double eta, par;
@@ -270,7 +275,12 @@ __global__ void __launch_bounds__(256) gpk_finish_kernel(const FinishArgs f)
         double kss = f.kss;
         if (f.env_cand != nullptr) {
             const double z = gpk_env_coord(f.env_cand + c * f.env_dc, f.env_axis, f.env_lo, f.env_up);
-            kss *= gpk_env(f.env_c0, f.env_c1, z, z);
+            if (f.task_n > 0) {
+                const int t = gpk_task_index(z, f.task_n);
+                kss *= t >= 0 ? f.task_diag[t] : __longlong_as_double(0x7ff8000000000000LL);
+            } else {
+                kss *= gpk_env(f.env_c0, f.env_c1, z, z);
+            }
         }
         double var = kss - ssq;
         mu += f.mean;
@@ -385,7 +395,11 @@ __global__ void gpk_cov_finish_kernel(double* __restrict__ cov, long ld, long m,
 //   dk/d log_metric_t = -k * (dlog f / d r2)(r2_g) * (x_t - x'_t)^2 / metric_t      (t in group g)
 // With the environment factor k = amp R (c0 + c1 z z'), nv = n_terms + 4: [sum w k, sum_t ..., log_a, log_b, trace A],
 //   dk/d log_a = amp R c0,   dk/d log_b = amp R c1 z z'
+// With the task factor k = amp R K_t[t_i][t_j] (training tasks are valid indices) the sums above use that k, nv stays
+// n_terms + 2; the task entries come from gpk_grad_task_kernel.  TASK = false compiles the task code out: a kernel
+// without the task factor runs the code it ran before the factor existed.
 // ---------------------------------------------------------------------------------------
+template <bool TASK>
 __global__ void __launch_bounds__(256)
 gpk_grad_trace_kernel(const KSpec ks, const double* __restrict__ Xt, long ldx, int n,
                       const double* __restrict__ Xrow, int dc,
@@ -396,8 +410,9 @@ gpk_grad_trace_kernel(const KSpec ks, const double* __restrict__ Xt, long ldx, i
     __shared__ double szc[32];
     __shared__ double red[8];
     const int tid = threadIdx.x;
-    const bool env = ks.env_axis >= 0;
+    const bool env = !TASK && ks.env_axis >= 0;
     const int nt = ks.n_terms, nv = nt + (env ? 4 : 2);
+    const int fax = TASK ? ks.task_axis : ks.env_axis;
     const long bid = (long)blockIdx.y * gridDim.x + blockIdx.x;
     const int j = blockIdx.x * 128 + (tid & 127);
     const long c0 = (long)blockIdx.y * 32;
@@ -410,7 +425,7 @@ gpk_grad_trace_kernel(const KSpec ks, const double* __restrict__ Xt, long ldx, i
         long ci = c0 + c;
         sc[c][t] = (ci < n) ? Xrow[ci * dc + ks.axis[t]] : 0.0;
     }
-    if (env && tid < 32) szc[tid] = (c0 + tid < n) ? Xrow[(c0 + tid) * dc + ks.env_axis] : 0.0;
+    if ((env || TASK) && tid < 32) szc[tid] = (c0 + tid < n) ? Xrow[(c0 + tid) * dc + fax] : 0.0;
     __syncthreads();
 
     const int cg = (tid >> 7) * 16;
@@ -418,7 +433,7 @@ gpk_grad_trace_kernel(const KSpec ks, const double* __restrict__ Xt, long ldx, i
     double gl[GPK_MAX_TERMS];                                // per-term partial sums (local memory)
     for (int t = 0; t < nt; ++t) gl[t] = 0.0;
     double gamp = 0.0, gtr = 0.0, genva = 0.0, genvb = 0.0;
-    const double zj = (env && jv) ? Xt[(long)ks.env_axis * ldx + j] : 0.0;
+    const double zj = ((env || TASK) && jv) ? Xt[(long)fax * ldx + j] : 0.0;
 
     double r2[16], wk[16];
 #pragma unroll
@@ -450,6 +465,8 @@ gpk_grad_trace_kernel(const KSpec ks, const double* __restrict__ Xt, long ldx, i
             genva = fma(wk[c], ks.env_c0, genva);
             genvb = fma(wk[c], ks.env_c1 * zc * zj, genvb);
             wk[c] *= gpk_env(ks.env_c0, ks.env_c1, zc, zj);
+        } else if (TASK) {
+            wk[c] *= ks.task_K[(int)szc[cg + c] * ks.n_tasks + (int)zj];
         }
         gamp += wk[c];
     }
@@ -486,6 +503,58 @@ gpk_grad_trace_kernel(const KSpec ks, const double* __restrict__ Xt, long ldx, i
     // block reduction of the nv values (fixed order: lanes, then warps)
     for (int v = 0; v < nv; ++v) {
         double x = (v == 0) ? gamp : (v == nv - 1 ? gtr : (v <= nt ? gl[v - 1] : (v == nt + 1 ? genva : genvb)));
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) x += __shfl_xor_sync(0xffffffffu, x, off);
+        if ((tid & 31) == 0) red[tid >> 5] = x;
+        __syncthreads();
+        if (tid == 0) {
+            double sum = 0.0;
+            for (int w = 0; w < 8; ++w) sum += red[w];
+            part[bid * nv + v] = sum;
+        }
+        __syncthreads();
+    }
+}
+
+// Task entries of the marginal-likelihood gradient: the same tiling and weights w_ij as gpk_grad_trace_kernel, per CTA
+// the T x T partial sums G_ab = sum_{i >= j, t_i = a, t_j = b} w_ij amp R_ij (row-major, T = n_tasks), R the radial
+// product.  gpk_grad_final_kernel adds the CTAs (with noise_var = 1: no noise entry) and gpk_nll_grad contracts G with
+// dK_t[a][b] / dtheta_pq on the host.  A kernel of its own, so the trace kernel's registers stay those of the kernel
+// without a task factor.
+__global__ void __launch_bounds__(256)
+gpk_grad_task_kernel(const KSpec ks, const double* __restrict__ Xt, long ldx, int n,
+                     const double* __restrict__ Kinv, long ldk, const double* __restrict__ alpha,
+                     double* __restrict__ part)
+{
+    __shared__ double red[8];
+    const int tid = threadIdx.x, nT = ks.n_tasks, nv = nT * nT;
+    const long bid = (long)blockIdx.y * gridDim.x + blockIdx.x;
+    const int j = blockIdx.x * 128 + (tid & 127);
+    const long c0 = (long)blockIdx.y * 32;
+    if ((long)blockIdx.x * 128 > c0 + 31) {
+        for (int v = tid; v < nv; v += 256) part[bid * nv + v] = 0.0;
+        return;
+    }
+    const bool jv = j < n;
+    const double* tx = Xt + (long)ks.task_axis * ldx;
+    const int tj = jv ? (int)tx[j] : 0;
+    double g[GPK_MAX_TASKS];                                 // G_{a, t_j}: this thread's column task is t_j
+    for (int a = 0; a < nT; ++a) g[a] = 0.0;
+    for (int c = 0; c < 16; ++c) {
+        const long i = c0 + (tid >> 7) * 16 + c;
+        if (!(jv && i < n && j <= i)) continue;
+        double r = 1.0, r2 = 0.0;
+        for (int t = 0; t < ks.n_terms; ++t) {
+            const double* xa = Xt + (long)ks.axis[t] * ldx;
+            const double d = xa[i] - xa[j];
+            r2 = fma(d * d, ks.inv_metric[t], r2);
+            if (ks.last[t]) { r *= gpk_radial(ks.family, r2); r2 = 0.0; }
+        }
+        const double a = alpha[i] * alpha[j] - Kinv[i * ldk + j];
+        g[(int)tx[i]] += (i == j ? a : 2.0 * a) * ks.amp * r;
+    }
+    for (int v = 0; v < nv; ++v) {                           // fixed order: lanes, then warps
+        double x = (v % nT == tj) ? g[v / nT] : 0.0;
 #pragma unroll
         for (int off = 16; off > 0; off >>= 1) x += __shfl_xor_sync(0xffffffffu, x, off);
         if ((tid & 31) == 0) red[tid >> 5] = x;
@@ -612,7 +681,10 @@ __global__ void gpk_candidates_kernel(unsigned long long seed, long first, long 
 // rule of the input scaling (1 / (upper - lower)) and of the output transform applied at the end.
 // With the environment factor k = amp R (c0 + c1 z* z_j): the terms above use that k, the environment axis gains
 //   d k / d z* = amp R c1 z_j,   and  d var / d z* gains d k(x*, x*) / d z* = 2 amp c1 z*.
+// With the task factor k = amp R K_t[t*][t_j]: the terms above use that k; the task axis and k(x*, x*) = amp K_t[t*][t*]
+// have zero derivative (the task index is piecewise constant).  TASK = false compiles the task code out.
 // ---------------------------------------------------------------------------------------
+template <bool TASK>
 __global__ void __launch_bounds__(256)
 gpk_predict_grad_kernel(const KSpec ks, const double* __restrict__ Xt, long ldx, int n,
                         const double* __restrict__ cand, int dc,
@@ -624,7 +696,7 @@ gpk_predict_grad_kernel(const KSpec ks, const double* __restrict__ Xt, long ldx,
     __shared__ double red[16];
     const int tid = threadIdx.x, nt = ks.n_terms;
     const long c = blockIdx.x;
-    const bool env = ks.env_axis >= 0;
+    const bool env = !TASK && ks.env_axis >= 0;
     const double zs = env ? gpk_env_coord(cand + c * dc, ks.env_axis, lower, upper) : 0.0;
     double gem = 0.0, gev = 0.0;                                        // environment-axis sums
     for (int t = tid; t < nt; t += 256) {
@@ -650,6 +722,8 @@ gpk_predict_grad_kernel(const KSpec ks, const double* __restrict__ Xt, long ldx,
             gem = fma(alpha[j], dkz, gem);
             gev = fma(-2.0 * Wt[c * ldw + j], dkz, gev);
             k *= gpk_env(ks.env_c0, ks.env_c1, zs, zj);
+        } else if (TASK) {                                              // unscaled: the task factor refuses bounds
+            k *= gpk_task(ks, cand[c * dc + ks.task_axis], Xt[(long)ks.task_axis * ldx + j]);
         }
         const double ka = k * alpha[j], kw = -2.0 * k * Wt[c * ldw + j];
         int t0 = 0;

@@ -118,7 +118,7 @@ class DeviceGP(object):
         diag_add = float(yerr_tot ** 2)
         sig = (int(f["family"]), float(f["log_amp"]), tuple(int(a) for a in f["axis"]),
                tuple(int(g) for g in f["group"]), tuple(float(v) for v in np.asarray(f["log_metric"]).ravel()), diag_add,
-               f["env"])
+               f["env"], f["task"])
         self.computed = False
         # Rows appended to an already factorised training set with the same kernel and noise (BaseModel.update /
         # train(do_optimize=False) inside the solver loop): only the last block row of the factor changes.
@@ -144,6 +144,8 @@ class DeviceGP(object):
         h.set_kernel(f["family"], f["log_amp"], f["axis"], f["group"], f["log_metric"])
         if f["env"] is not None:
             h.set_env_factor(*f["env"])
+        if f["task"] is not None:
+            h.set_task_factor(*f["task"])
         self.log_determinant, self._ll = h.fit(diag_add, self.mean)
         self._fit_x = self._x.copy()
         self._fit_sig = sig
@@ -169,7 +171,8 @@ class DeviceGP(object):
         diag_add = float(yerr_tot ** 2)
         self._pending_sig = (int(f["family"]), float(f["log_amp"]), tuple(int(a) for a in f["axis"]),
                              tuple(int(g) for g in f["group"]),
-                             tuple(float(v) for v in np.asarray(f["log_metric"]).ravel()), diag_add, f["env"])
+                             tuple(float(v) for v in np.asarray(f["log_metric"]).ravel()), diag_add, f["env"],
+                             f["task"])
         self.computed = False
         self._fit_x = None
         if self._data_dirty:
@@ -179,6 +182,8 @@ class DeviceGP(object):
         h.set_kernel(f["family"], f["log_amp"], f["axis"], f["group"], f["log_metric"])
         if f["env"] is not None:
             h.set_env_factor(*f["env"])
+        if f["task"] is not None:
+            h.set_task_factor(*f["task"])
         h.fit_begin(diag_add, self.mean)
 
     def compute_end(self):
@@ -217,7 +222,12 @@ class DeviceGP(object):
             raise RuntimeError("You need to compute the model first")
         f = self.kernel.flatten()
         nt = len(f["axis"])
-        g = self.handle.nll_grad(noise_var, nt) if f["env"] is None else self.handle.nll_grad(noise_var, nt, env=True)
+        if f["env"] is not None:
+            g = self.handle.nll_grad(noise_var, nt, env=True)
+        elif f["task"] is not None:
+            g = self.handle.nll_grad(noise_var, nt, n_kt=len(f["task"][2]))
+        else:
+            g = self.handle.nll_grad(noise_var, nt)
         out = np.empty(len(f["slots"]) + 1)
         for p, (kind, terms) in enumerate(f["slots"]):
             if kind == "amp":
@@ -226,6 +236,8 @@ class DeviceGP(object):
                 out[p] = g[1 + nt]
             elif kind == "lin_b":
                 out[p] = g[2 + nt]
+            elif kind == "task":
+                out[p] = g[1 + nt + terms]
             else:
                 out[p] = sum(g[1 + t] for t in terms)
         out[-1] = g[-1]

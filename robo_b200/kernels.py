@@ -13,7 +13,7 @@ test/test_models/test_gaussian_process.py:44-46).  These classes keep that surfa
 Every value is computed on the GPU (gpk_kernel_matrix); nothing here evaluates a kernel on
 the CPU.  Supported algebra: products of ConstantKernel and radial kernels of ONE family
 (Matern-5/2, Matern-3/2 or ExpSquared), times at most one BayesianLinearRegressionKernel
-(include/gpk.h: gpk_set_env_factor).  Sums are not representable on the device path and
+(include/gpk.h: gpk_set_env_factor) or one TaskKernel (gpk_set_task_factor).  Sums are not representable on the device path and
 raise NotImplementedError when flattened.
 """
 import numpy as np
@@ -21,7 +21,7 @@ import numpy as np
 from . import _lib
 
 __all__ = ["Kernel", "ConstantKernel", "Matern52Kernel", "Matern32Kernel", "ExpSquaredKernel",
-           "BayesianLinearRegressionKernel", "Product", "Sum"]
+           "BayesianLinearRegressionKernel", "TaskKernel", "Product", "Sum"]
 
 
 class Kernel(object):
@@ -51,6 +51,11 @@ class Kernel(object):
     @property
     def vector(self):
         return self.get_parameter_vector()
+
+    @vector.setter
+    def vector(self, v):
+        # george 0.2's kernel.vector assignment, which robo/models/mtbo_gp.py:94 uses to set the parameters
+        self.set_parameter_vector(v)
 
     @property
     def pars(self):
@@ -82,12 +87,16 @@ class Kernel(object):
         raise NotImplementedError
 
     def flatten(self):
-        """-> dict(family, log_amp, axis, group, log_metric, slots, env) for gpk_set_kernel.
-        slots[i] = ('amp', None), ('metric', [term indices]), ('lin_a', None) or ('lin_b', None) for
+        """-> dict(family, log_amp, axis, group, log_metric, slots, env, task) for gpk_set_kernel.
+        slots[i] = ('amp', None), ('metric', [term indices]), ('lin_a', None), ('lin_b', None) or ('task', k) for
         parameter i, used to map gradients back onto the george parameter vector.  env = None, or
-        (axis, log_a, log_b) of the environment factor (gpk_set_env_factor)."""
-        acc = dict(family=None, log_amp=0.0, axis=[], group=[], log_metric=[], slots=[], ngroups=0, env=None)
+        (axis, log_a, log_b) of the environment factor (gpk_set_env_factor); task = None, or (axis, n_tasks,
+        theta tuple) of the task factor (gpk_set_task_factor), whose k-th packed entry is slot ('task', k)."""
+        acc = dict(family=None, log_amp=0.0, axis=[], group=[], log_metric=[], slots=[], ngroups=0, env=None, task=None)
         self._collect(acc)
+        if acc["env"] is not None and acc["task"] is not None:
+            raise NotImplementedError("a kernel with both a BayesianLinearRegressionKernel and a TaskKernel factor is "
+                                      "not supported on the device")
         if acc["family"] is None:
             raise NotImplementedError("the device path needs at least one radial kernel factor")
         return acc
@@ -109,6 +118,8 @@ class Kernel(object):
         h.set_kernel(f["family"], f["log_amp"], f["axis"], f["group"], f["log_metric"])
         if f["env"] is not None:
             h.set_env_factor(*f["env"])
+        if f["task"] is not None:
+            h.set_task_factor(*f["task"])
         return h.kernel_matrix(x1, x2)
 
 
@@ -225,6 +236,47 @@ class BayesianLinearRegressionKernel(Kernel):
         acc["env"] = (int(self.axes[0]), self.log_a, self.log_b)
         acc["slots"].append(("lin_a", None))
         acc["slots"].append(("lin_b", None))
+
+
+class TaskKernel(Kernel):
+    """The task kernel of multi-task Bayesian optimisation (robo/fmin/mtbo.py:101, :134: george's
+    TaskKernel(ndim, axis, num_tasks)) on input column ``axis``, whose values are task indices:
+
+        k(t, t') = K_t[t, t'],   K_t = L L^T,   L_pq = exp(theta[p (p + 1) / 2 + q])   (q <= p)
+
+    a free-form positive-definite task covariance (Swersky, Snoek, Adams, NIPS 2013) through its Cholesky factor, packed
+    row by row (L00, L10, L11, L20, ...).  Restated from the paper and the reference's call sites: the george fork that
+    defines this kernel is not public, so the definition has not been checked against it.  A coordinate that is not an
+    integer in [0, num_tasks) has a NaN factor.  The parameter vector (num_tasks (num_tasks + 1) / 2 log-entries)
+    starts at zeros, L all ones."""
+
+    def __init__(self, ndim, axis, num_tasks):
+        super(TaskKernel, self).__init__(ndim, axes=axis)
+        if len(self.axes) != 1:
+            raise ValueError("TaskKernel takes exactly one axis")
+        self.num_tasks = int(num_tasks)
+        if not 1 <= self.num_tasks <= _lib.MAX_TASKS:
+            raise ValueError("TaskKernel supports 1 to %d tasks on the device" % _lib.MAX_TASKS)
+        self.theta = np.zeros(self.num_tasks * (self.num_tasks + 1) // 2)
+
+    def get_parameter_vector(self, include_frozen=False):
+        return self.theta.copy()
+
+    def set_parameter_vector(self, vector, include_frozen=False):
+        vector = np.atleast_1d(np.asarray(vector, dtype=np.float64)).ravel()
+        if len(vector) != len(self.theta):
+            raise ValueError("dimension mismatch")
+        self.theta = vector.copy()
+
+    def get_parameter_names(self, include_frozen=False):
+        return tuple("L_%d_%d" % (p, q) for p in range(self.num_tasks) for q in range(p + 1))
+
+    def _collect(self, acc):
+        if acc["task"] is not None:
+            raise NotImplementedError("products of two TaskKernel factors are not supported on the device")
+        acc["task"] = (int(self.axes[0]), self.num_tasks, tuple(float(v) for v in self.theta))
+        for k in range(len(self.theta)):
+            acc["slots"].append(("task", k))
 
 
 class _Operator(Kernel):

@@ -56,6 +56,8 @@ class _LikelihoodPool(object):
                     h.set_kernel(f["family"], f["log_amp"], f["axis"], f["group"], f["log_metric"])
                     if f["env"] is not None:
                         h.set_env_factor(*f["env"])
+                    if f["task"] is not None:
+                        h.set_task_factor(*f["task"])
                     yerr = np.sqrt(np.exp(theta[-1]))
                     diag_add = float(np.sqrt(np.float64(yerr) ** 2 + TINY) ** 2)
                     h.fit_begin(diag_add, self.mean)
@@ -79,8 +81,8 @@ class _LikelihoodPool(object):
 
 
 def _hyper_prior(prior):
-    """(gpk_prior_kind, the 7 constants, n_ls, n_lr) of a prior the device restates: None, DefaultPrior or EnvPrior
-    (the reference's classes or robo_b200.priors'); TypeError for any other."""
+    """(gpk_prior_kind, the 7 constants, n_ls, n_lr) of a prior the device restates: None, DefaultPrior, EnvPrior or
+    MTBOPrior (the reference's classes or robo_b200.priors'); TypeError for any other."""
     if prior is None:
         return _lib.PRIOR_NONE, None, 0, 0
     cls = type(prior)
@@ -93,7 +95,11 @@ def _hyper_prior(prior):
             return _lib.PRIOR_DEFAULT, par, 0, 0
         par[5:] = [prior.bayes_lin_prior.sigma, prior.bayes_lin_prior.mean]
         return _lib.PRIOR_ENV, par, int(prior.n_ls), int(prior.n_lr)
-    raise TypeError("hyper_sampler='device' restates None, DefaultPrior and EnvPrior only, not %s.%s"
+    if ours and cls.__name__ == "MTBOPrior":
+        par = [prior.ln_prior.sigma, prior.ln_prior.mean, prior.tophat.min, prior.tophat.max, prior.horseshoe.scale,
+               prior.tophat_task.min, prior.tophat_task.max]
+        return _lib.PRIOR_MTBO, par, int(prior.n_ls), int(prior.n_kt)
+    raise TypeError("hyper_sampler='device' restates None, DefaultPrior, EnvPrior and MTBOPrior only, not %s.%s"
                     % (mod, cls.__name__))
 
 
@@ -224,6 +230,8 @@ class GaussianProcessMCMC(BaseModel):
         h.set_kernel(f["family"], f["log_amp"], f["axis"], f["group"], f["log_metric"])
         if f["env"] is not None:
             h.set_env_factor(*f["env"])
+        if f["task"] is not None:
+            h.set_task_factor(*f["task"])
         _lib.set_hyper_model(h, f["slots"], len(f["axis"]), float(self.mean), TINY, prior_kind, prior_par, n_ls, n_lr)
 
         def run(p0, steps):

@@ -150,6 +150,38 @@ class EnvPrior(object):
         return p0
 
 
+class MTBOPrior(object):
+    """env_priors.py:158-228 (the MTBO prior): lognormal(sigma 1, loc 0) on the amplitude, tophat(-10, 2) on the n_ls
+    length scales, tophat(-1, 0) on the n_kt Cholesky entries of the task kernel as one vector test, horseshoe(0.1) on
+    the noise.  sample_from_prior draws the task slice through numpy's (1, n, n_kt) broadcast, as the reference does."""
+
+    def __init__(self, n_dims, n_ls, n_kt, rng=None):
+        self.rng = np.random.RandomState(np.random.randint(0, 10000)) if rng is None else rng
+        self.n_dims, self.n_ls, self.n_kt = n_dims, n_ls, n_kt
+        self.tophat = TophatPrior(-10, 2, rng=self.rng)
+        self.ln_prior = LognormalPrior(mean=0.0, sigma=1.0, rng=self.rng)
+        self.horseshoe = HorseshoePrior(scale=0.1, rng=self.rng)
+        self.tophat_task = TophatPrior(-1, 0, rng=self.rng)
+
+    def lnprob(self, theta):
+        lp = 0
+        lp += self.ln_prior.lnprob(theta[0])
+        lp += self.tophat.lnprob(theta[1:self.n_ls + 1])
+        lp += self.tophat_task.lnprob(theta[self.n_ls + 1:self.n_ls + 1 + self.n_kt])
+        lp += self.horseshoe.lnprob(theta[-1])
+        return lp
+
+    def sample_from_prior(self, n_samples):
+        p0 = np.zeros([n_samples, self.n_dims])
+        p0[:, 0] = self.ln_prior.sample_from_prior(n_samples)[:, 0]
+        ls_sample = np.array([self.tophat.sample_from_prior(n_samples)[:, 0] for _ in range(0, self.n_ls)]).T
+        p0[:, 1:(self.n_ls + 1)] = ls_sample
+        pos, end = self.n_ls + 1, self.n_ls + self.n_kt + 1
+        p0[:, pos:end] = np.array([self.tophat_task.sample_from_prior(n_samples) for _ in range(0, end - pos)]).T
+        p0[:, -1] = self.horseshoe.sample_from_prior(n_samples)[:, 0]
+        return p0
+
+
 class BayesianLinearRegressionPrior(object):
     """bayesian_linear_regression_prior.py:8-60, with its quirks: lnprob adds LognormalPrior(sigma=0.1, mean=-10) of
     theta[0] (scipy's loc = -10) and HorseshoePrior(0.1) of 1 / theta[-1], one over log beta rather than the noise
