@@ -40,6 +40,21 @@ class FabolasGP(GaussianProcess):
 
     device_inputs = normalize
 
+    def input_gradient(self, X_test, G):
+        """The chain rule through normalize: 1 / (upper - lower) on the configuration columns, the basis function's
+        derivative on s (-2 (1 - s) for (1 - s)^2, 1 for s).  NotImplementedError for any other basis function, whose
+        derivative is not known here."""
+        from robo_b200 import _lib
+        from robo_b200.acquisition_functions.information_gain_per_unit_cost import basis_code
+        try:
+            code = basis_code(self.basis_function)
+        except TypeError:
+            raise NotImplementedError("input gradients of a FabolasGP need the basis function s or (1 - s) ** 2")
+        lo, hi = normalization._column_range(X_test[:, :-1], self.lower, self.upper)
+        s = X_test[:, -1]
+        ds = np.ones_like(s) if code == _lib.BASIS_S else -2.0 * (1.0 - s)
+        return np.concatenate((G[:, :-1] / (hi - lo), G[:, -1:] * ds[:, None]), axis=1)
+
     def train(self, X, y, do_optimize=True):
         self.original_X = X
         return super(FabolasGP, self).train(self.normalize(X), y, do_optimize)

@@ -195,6 +195,11 @@ class GaussianProcess(BaseModel):
         itself); subclasses that transform inputs on the host (FabolasGP) return the transformed array."""
         return X_test
 
+    def input_gradient(self, X_test, G):
+        """A gradient G (M, D) with respect to device_inputs(X_test), taken back to the raw inputs X_test by the
+        chain rule; the identity here, where the handle applies (and differentiates) the input scaling itself."""
+        return G
+
     def score(self, X_test, kind, eta=None, par=0.0, want_values=True):
         """Fused predict -> acquisition -> arg-max used by robo_b200.acquisition_functions.
         ``kind``: one of 'ei', 'log_ei', 'pi', 'lcb'."""
@@ -214,8 +219,8 @@ class GaussianProcess(BaseModel):
         if not self.is_trained:
             raise Exception('Model has to be trained first!')
         assert len(X_test.shape) == 2
-        r = self.gp.predict_grad(X_test)
-        return r["dmu"], r["dvar"]
+        r = self.gp.predict_grad(self.device_inputs(X_test))
+        return self.input_gradient(X_test, r["dmu"]), self.input_gradient(X_test, r["dvar"])
 
     def score_with_gradient(self, X_test, kind, eta=None, par=0.0):
         """(f (M,), df (M, D)) for 'ei', 'pi', 'lcb' — value and input gradient of the acquisition."""
@@ -224,8 +229,8 @@ class GaussianProcess(BaseModel):
             raise Exception('Model has to be trained first!')
         if eta is None:
             eta = 0.0 if kind == "lcb" else self.get_incumbent()[1]
-        r = self.gp.predict_grad(X_test, _lib.ACQ_KIND[kind], float(eta), float(par))
-        return r["f"], r["df"]
+        r = self.gp.predict_grad(self.device_inputs(X_test), _lib.ACQ_KIND[kind], float(eta), float(par))
+        return r["f"], self.input_gradient(X_test, r["df"])
 
     def sample_functions(self, X_test, n_funcs=1):
         """Posterior function samples at X_test (gaussian_process.py:298-332): mean and

@@ -39,6 +39,12 @@ class MTBOGP(GaussianProcess):
 
     device_inputs = normalize
 
+    def input_gradient(self, X_test, G):
+        """The chain rule through normalize: 1 / (upper - lower) on the configuration columns, 0 on the task column
+        (np.rint is piecewise constant)."""
+        lo, hi = normalization._column_range(X_test[:, :-1], self.lower, self.upper)
+        return np.concatenate((G[:, :-1] / (hi - lo), np.zeros_like(G[:, -1:])), axis=1)
+
     def train(self, X, y, do_optimize=True):
         self.original_X = X
         return super(MTBOGP, self).train(self.normalize(X), y, do_optimize)

@@ -38,7 +38,8 @@ def have_longdouble():
 
 
 def kernel_ld(k, A, B):
-    """k(A, B) of a george_oracle kernel tree in longdouble; A (n1, D), B (n2, D) float64 inputs."""
+    """k(A, B) of a george_oracle kernel tree in longdouble; A (n1, D), B (n2, D) float64 inputs.  The factor kernels of
+    tests/env_kernel_model.py (EnvKernel) and tests/task_kernel_model.py (TaskKernel) are understood too."""
     if isinstance(k, G.Product):
         return kernel_ld(k.k1, A, B) * kernel_ld(k.k2, A, B)
     if isinstance(k, G.Sum):
@@ -51,6 +52,19 @@ def kernel_ld(k, A, B):
             d = A[:, a].astype(LD)[:, None] - B[:, a].astype(LD)[None, :]
             r2 += d * d / LD(md)
         return k._f(r2)
+    from tests import env_kernel_model as EM
+    from tests import task_kernel_model as TM
+    if isinstance(k, EM.EnvKernel):                 # c0 + c1 z z'
+        a = int(k.axes[0])
+        return np.exp(LD(k.log_a)) + np.exp(LD(k.log_b)) * (A[:, a].astype(LD)[:, None] * B[:, a].astype(LD)[None, :])
+    if isinstance(k, TM.TaskKernel):                # K_t[t, t'], K_t = L L^T in longdouble, NaN off the tasks
+        from tests import fit_reference as FR
+        a = int(k.axes[0])
+        Kt, _ = FR.task_factor_ld(k.theta, k.n_tasks)
+        ia, ib = TM.task_index(A[:, a], k.n_tasks), TM.task_index(B[:, a], k.n_tasks)
+        out = Kt[np.ix_(np.maximum(ia, 0), np.maximum(ib, 0))]
+        out[(ia < 0)[:, None] | (ib < 0)[None, :]] = np.nan
+        return out
     raise TypeError("kernel_ld: unsupported kernel %r" % type(k))
 
 
@@ -138,6 +152,27 @@ def fma(a, b, c):
     """fl(a b + c), the product and sum taken in longdouble (64-bit significand) and rounded once to fp64; differs
     from a true fma only by a rare double rounding."""
     return (np.asarray(a, dtype=LD) * np.asarray(b, dtype=LD) + np.asarray(c, dtype=LD)).astype(np.float64)
+
+
+def fma_exact(a, b, c):
+    """fl(a b + c) correctly rounded (a true fma), elementwise.  The longdouble result of fma() is rounded a second time
+    to fp64; that double rounding can only go wrong where the longdouble value is exactly halfway between two fp64
+    numbers (rounding to 64 bits is monotone and every fp64 midpoint is a 64-bit number).  Those entries are recomputed
+    exactly with fractions.Fraction, so the result is the true fma's bits everywhere."""
+    from fractions import Fraction
+    a, b, c = np.broadcast_arrays(np.asarray(a, dtype=np.float64), np.asarray(b, dtype=np.float64),
+                                  np.asarray(c, dtype=np.float64))
+    v = np.asarray(a, dtype=LD) * np.asarray(b, dtype=LD) + np.asarray(c, dtype=LD)
+    out = v.astype(np.float64)
+    rest = np.abs((v - out.astype(LD)).astype(np.float64))
+    sp = np.spacing(np.abs(out))
+    tie = np.isfinite(out) & (rest > 0) & ((rest == sp / 2) | (rest == sp / 4))
+    out = np.array(out)
+    for idx in zip(*np.nonzero(tie)):
+        exact = Fraction(float(a[idx])) * Fraction(float(b[idx])) + Fraction(float(c[idx]))
+        lo = float(exact)                    # Fraction -> float rounds to nearest, ties to even
+        out[idx] = lo
+    return out
 
 
 def device_u(L64, Kxz):

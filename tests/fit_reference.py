@@ -48,7 +48,7 @@ EPS = float(np.finfo(np.float64).eps)
 BM = 128
 SLICES = 6
 
-C_FACTOR, C_PANEL, C_SOLVE, C_LOGDET, C_INV, C_GRAD, C_COV = 2.0, 2.0, 2.0, 2.0, 2.0, 2.0, 2.0
+C_FACTOR, C_PANEL, C_SOLVE, C_LOGDET, C_INV, C_GRAD, C_COV, C_PGRAD, C_HY = 2.0, 2.0, 2.0, 2.0, 2.0, 2.0, 2.0, 2.0, 2.0
 
 
 def have_longdouble():
@@ -238,34 +238,91 @@ def _radial(family, r2):
     return (1 + s) * np.exp(-s), -(LD(3) / 2) / (1 + s)   # Matern-3/2
 
 
-def kernel_terms_ld(flat, X):
-    """k(X, X) and dk/dtheta for theta = [log_amp, log_metric_t ...] of a flattened kernel (robo_b200.kernels
-    flatten()), in longdouble: dk/dlog_amp = k, dk/dlog_metric_t = -k dlog f(r2_g)/dr2 (x_t - x'_t)^2 / metric_t."""
-    X = np.asarray(X, dtype=np.float64)
+def _radial_ld(flat, A, B):
+    """amp prod_g f_g(r2_g) between the rows of A and B in longdouble, with the per-term (d log f / d r2_g) and the scaled
+    squared distances D2_t = (a_t - b_t)^2 / metric_t."""
     axis, group, lm = list(flat["axis"]), list(flat["group"]), list(flat["log_metric"])
-    fam = int(flat["family"])
-    amp = np.exp(LD(flat["log_amp"]))
-    nt = len(axis)
+    k = np.full((len(A), len(B)), np.exp(LD(flat["log_amp"])), dtype=LD)
     D2 = []
-    for t in range(nt):
-        d = X[:, axis[t]].astype(LD)[:, None] - X[:, axis[t]].astype(LD)[None, :]
+    for t in range(len(axis)):
+        d = A[:, axis[t]].astype(LD)[:, None] - B[:, axis[t]].astype(LD)[None, :]
         D2.append(d * d / np.exp(LD(lm[t])))
-    k = np.full(D2[0].shape, amp, dtype=LD)
     dlog = {}
     for g in sorted(set(group)):
-        ts = [t for t in range(nt) if group[t] == g]
-        r2 = sum(D2[t] for t in ts)
-        f, dl = _radial(fam, r2)
+        ts = [t for t in range(len(axis)) if group[t] == g]
+        f, dl = _radial(int(flat["family"]), sum(D2[t] for t in ts))
         k = k * f
         for t in ts:
             dlog[t] = dl
-    grads = [k] + [-k * dlog[t] * D2[t] for t in range(nt)]
-    return k, grads
+    return k, dlog, D2
+
+
+def task_factor_ld(theta, n_tasks):
+    """(K_t, [dK_t / dtheta_k in packed order]) in longdouble: K_t = L L^T, L_pq = exp(theta_k), k = p (p + 1) / 2 + q,
+    dK_t / dtheta_pq = L_pq (e_p L_q^T + L_q e_p^T)."""
+    L = np.zeros((n_tasks, n_tasks), dtype=LD)
+    for p in range(n_tasks):
+        for q in range(p + 1):
+            L[p, q] = np.exp(LD(theta[p * (p + 1) // 2 + q]))
+    dK = []
+    for p in range(n_tasks):
+        for q in range(p + 1):
+            D = np.zeros((n_tasks, n_tasks), dtype=LD)
+            D[p, :] += L[p, q] * L[:, q]
+            D[:, p] += L[p, q] * L[:, q]
+            dK.append(D)
+    return L @ L.T, dK
+
+
+def factor_ld(flat, A, B):
+    """The single-column factor of a flattened kernel between the rows of A and B in longdouble, and its parameter
+    derivatives [d/dlog_a, d/dlog_b] or [dK_t[t, t'] / dtheta_k ...]; (None, []) without a factor.  Task coordinates
+    that are not tasks give NaN (as the device)."""
+    env, task = flat.get("env"), flat.get("task")
+    if env is not None:
+        ax, la, lb = env
+        c0, c1 = np.exp(LD(la)), np.exp(LD(lb))
+        zz = A[:, ax].astype(LD)[:, None] * B[:, ax].astype(LD)[None, :]
+        return c0 + c1 * zz, [np.full(zz.shape, c0, dtype=LD), c1 * zz]
+    if task is not None:
+        ax, nT, theta = task
+        Kt, dKt = task_factor_ld(theta, nT)
+        ia, ib = _task_index(A[:, ax], nT), _task_index(B[:, ax], nT)
+        bad = (ia < 0)[:, None] | (ib < 0)[None, :]
+        sel = np.ix_(np.maximum(ia, 0), np.maximum(ib, 0))
+        F = Kt[sel]
+        F[bad] = np.nan
+        return F, [D[sel] for D in dKt]
+    return None, []
+
+
+def _task_index(t, n):
+    t = np.asarray(t, dtype=np.float64)
+    ok = (t >= 0) & (t < n) & (t == np.floor(t))
+    return np.where(ok, np.where(ok, t, 0), -1).astype(int)
+
+
+def kernel_terms_ld(flat, X):
+    """k(X, X) and dk/dtheta in the device's order, in longdouble: theta = [log_amp, log_metric_t ...] then, with the
+    environment factor, [log_a, log_b], with the task factor the n_kt packed entries of L.  Radial part R (amp
+    included): dR/dlog_amp = R, dR/dlog_metric_t = -R dlog f(r2_g)/dr2 (x_t - x'_t)^2 / metric_t; each is multiplied by
+    the factor F, and the factor's own derivatives are R dF/dtheta (env: R c0, R c1 z z'; task: R dK_t[t, t']/dtheta)."""
+    X = np.asarray(X, dtype=np.float64)
+    k, dlog, D2 = _radial_ld(flat, X, X)
+    grads = [k] + [-k * dlog[t] * D2[t] for t in range(len(D2))]
+    F, dF = factor_ld(flat, X, X)
+    if F is None:
+        return k, grads
+    return k * F, [g * F for g in grads] + [k * d for d in dF]
 
 
 def grad_reference(flat, X, Xinv, z, noise_var, gemm=None):
-    """(g_ref (nt + 2,) float64, bound (nt + 2,)) from the device's X^ = L^-1 and z^."""
+    """(g_ref, bound) in the device's layout (n_terms + 2 entries, + 2 with the environment factor, + n_kt with the task
+    factor, the noise entry last) from the device's X^ = L^-1 and z^.  The task entries are contracted on the host
+    from the per-pair sums G_ab = sum_{t_i = a, t_j = b} A_ij R_ij; their bound gains that contraction's rounding,
+    (2 n_tasks) u sum_ab |G_ab| |dK_t[a, b]|."""
     gemm = gemm or _gemm_numpy
+    X = np.asarray(X, dtype=np.float64)
     N = X.shape[0]
     a = exact_matmul(Xinv.T, z[:, None], gemm)[:, 0]
     Kinv = exact_matmul(Xinv.T, Xinv, gemm)
@@ -282,23 +339,165 @@ def grad_reference(flat, X, Xinv, z, noise_var, gemm=None):
         adK = np.abs(dK.astype(np.float64))
         bnd.append(C_GRAD * ((N + 64 + nblk / 256) * U * np.sum(adK * mag0) + np.sum(adK * dmag)) / 2)
     g, bnd = np.array(g), np.array(bnd)
+    if flat.get("task") is not None:
+        ax, nT, theta = flat["task"]
+        R, _, _ = _radial_ld(flat, X, X)
+        ti = _task_index(X[:, ax], nT)
+        onehot = (ti[:, None] == np.arange(nT)[None, :]).astype(LD)
+        Gab = np.abs((onehot.T @ (A * R) @ onehot).astype(np.float64))
+        _, dKt = task_factor_ld(theta, nT)
+        nterm = len(flat["axis"]) + 1
+        for k, D in enumerate(dKt):
+            bnd[nterm + k] += C_GRAD * 2 * nT * U * np.sum(Gab * np.abs(D.astype(np.float64))) / 2
     g[-1] *= noise_var
     bnd[-1] *= noise_var
     return g, bnd
 
 
+# ---- predictive gradients ----------------------------------------------------------------------------------------------
+def kernel_ld(flat, A, B):
+    """k(A, B) of a flattened kernel, factor included, in longdouble (A, B float64 rows as the device reads them)."""
+    k, _, _ = _radial_ld(flat, np.asarray(A, dtype=np.float64), np.asarray(B, dtype=np.float64))
+    F, _ = factor_ld(flat, np.asarray(A, dtype=np.float64), np.asarray(B, dtype=np.float64))
+    return k if F is None else k * F
+
+
+def predict_grad_reference(flat, X, Xinv, z, Xs, lower=None, upper=None, y_std=None, gemm=None):
+    """(dmu, dvar, bound_mu, bound_var), each (m, d), of gpk_predict_grad restated in longdouble from the device's
+    X^ = L^-1 and z^ (cov_reference's way): alpha = X^T z^, w = X^T (X^ k*), and for candidate x*, scaled
+    xn = (x* - lower) / (upper - lower) in fp64 as the device scales it,
+        dmu_a  = y_std / (upper_a - lower_a) sum_j alpha_j dk_j/dxn_a
+        dvar_a = y_std^2 / (upper_a - lower_a) (dk**/dxn_a - 2 sum_j w_j dk_j/dxn_a)
+    with k_j = R_j F_j: dk_j/dxn_a = F_j dR_j/dxn_a on the radial axes, R_j c1 z_j on the environment axis (and
+    dk**/dz* = 2 amp c1 z*), exactly 0 on the task axis.  Bound per entry (the same scaling):
+        C_PGRAD [(N + n_terms + 16) u sum_j |dk_j| (|alpha_j| + 2 |w_j|) + sum_j |dk_j| (|dalpha_j| + 2 |dw_j|)
+                 + 8 u |dk**|]
+    with dalpha = gamma_N |X^T| |z^| (alpha = Q z^) and dw = (2 gamma_N + (n_terms + 16) u) |X^T| (|X^| |k*|) (the two
+    products and the device's own K* entries), the error alpha^ and w^ carry, as grad_reference carries it."""
+    gemm = gemm or _gemm_numpy
+    X = np.asarray(X, dtype=np.float64)
+    Xs = np.asarray(Xs, dtype=np.float64)
+    N, d = X.shape
+    m = Xs.shape[0]
+    Xn = Xs if lower is None else (Xs - lower) / (upper - lower)
+    span = np.ones(d) if lower is None else (np.asarray(upper, dtype=np.float64) - lower)
+    ys = 1.0 if y_std is None else float(y_std)
+    nt = len(flat["axis"])
+    alpha = exact_matmul(Xinv.T, z[:, None], gemm)[:, 0]
+    R, dlog, D2 = _radial_ld(flat, Xn, X)
+    F, _ = factor_ld(flat, Xn, X)
+    Ks = R if F is None else R * F
+    ah, al = split2(exact_matmul(Xinv, Ks.T.astype(np.float64), gemm))
+    w = exact_matmul(Xinv.T, ah, gemm) + gemm(Xinv.T, al).astype(LD)        # (N, m)
+    absX = np.abs(Xinv)
+    dal = gamma(N) * (absX.T @ np.abs(z))
+    dw = (2 * gamma(N) + (nt + 16) * U) * gemm(absX.T, gemm(absX, np.abs(Ks.T.astype(np.float64))))
+    Fm = np.ones_like(R) if F is None else F
+    dk = [np.zeros((m, N), dtype=LD) for _ in range(d)]
+    axis, lm = list(flat["axis"]), list(flat["log_metric"])
+    for t in range(nt):
+        diff = Xn[:, axis[t]].astype(LD)[:, None] - X[:, axis[t]].astype(LD)[None, :]
+        dk[axis[t]] = dk[axis[t]] + Fm * R * dlog[t] * 2 * diff / np.exp(LD(lm[t]))
+    dkss = np.zeros((m, d), dtype=LD)
+    env = flat.get("env")
+    if env is not None:
+        ax, la, lb = env
+        c1 = np.exp(LD(lb))
+        dk[ax] = R * c1 * X[:, ax].astype(LD)[None, :]
+        dkss[:, ax] = 2 * np.exp(LD(flat["log_amp"])) * c1 * Xn[:, ax].astype(LD)
+    dmu, dvar = np.zeros((m, d)), np.zeros((m, d))
+    bmu, bvar = np.zeros((m, d)), np.zeros((m, d))
+    for a in range(d):
+        s = LD(ys) / LD(span[a])
+        dmu[:, a] = ((dk[a] @ alpha.astype(LD)) * s).astype(np.float64)
+        dvar[:, a] = ((dkss[:, a] - 2 * np.sum(dk[a] * w.T, axis=1)) * s * LD(ys)).astype(np.float64)
+        adk = np.abs(dk[a].astype(np.float64))
+        aw, aal = np.abs(w.T.astype(np.float64)), np.abs(alpha.astype(np.float64))
+        cm = (N + nt + 16) * U * (adk @ aal) + adk @ dal
+        cv = (N + nt + 16) * U * 2 * np.sum(adk * aw, axis=1) + 2 * np.sum(adk * dw.T, axis=1) \
+            + 8 * U * np.abs(dkss[:, a].astype(np.float64))
+        bmu[:, a] = C_PGRAD * cm * ys / span[a]
+        bvar[:, a] = C_PGRAD * cv * ys * ys / span[a]
+    return dmu, dvar, bmu, bvar
+
+
+# ---- the hyper sampler's log-likelihood (gpk_hy_eval) ------------------------------------------------------------------
+def cholesky_ld(K):
+    """Lower Cholesky factor of a longdouble matrix in longdouble (None when a pivot is not positive)."""
+    K = np.array(K, dtype=LD)
+    n = K.shape[0]
+    L = np.zeros_like(K)
+    for j in range(n):
+        s = K[j:, j] - L[j:, :j] @ L[j, :j]
+        if not s[0] > 0:
+            return None
+        L[j, j] = np.sqrt(s[0])
+        L[j + 1:, j] = s[1:] / L[j, j]
+    return L
+
+
+def forward_ld(L, r):
+    z = np.zeros(L.shape[0], dtype=LD)
+    for i in range(L.shape[0]):
+        z[i] = (r[i] - L[i, :i] @ z[:i]) / L[i, i]
+    return z
+
+
+def hy_loglik_reference(flat, X, y, mean, diag_add, n_tasks=0):
+    """dict(ll, bound, first_order) of the log-likelihood gpk_hy_eval computes for one theta, or None when the reference's
+    own K is not positive definite.  gpk_hyper_lnpost returns only ll, so the device's L^ cannot be read back: the bound
+    is first order, stated from the reference's K, L and alpha = K^-1 (y - mean) in longdouble.  With ll(K) =
+    -r^T K^-1 r / 2 - log det K / 2 - n log(2 pi) / 2, a perturbation dK moves it by (alpha^T dK alpha - tr(K^-1 dK)) / 2
+    to first order, so
+        |ll_dev - ll_ref| <= C_HY ( [sum_ij |K^-1|_ij E_ij + sum_ij |alpha_i| E_ij |alpha_j|] / 2
+                                    + (n + 8) u (sum_i |log L_ii| + z^T z) )
+        E = (gamma_{n+1} + 2 gamma_n) |L| |L^T| + E_build
+    where gamma_{n+1} |L| |L^T| is the backward error of the column-by-column Cholesky (Higham, Thm 10.3), 2 gamma_n
+    |L| |L^T| that of the forward solve taken onto K ((L + dL)(L + dL)^T), and E_build = (n_terms + 2 n_tasks + 24) u
+    |K| the per-entry error of the inline build (the radial evaluation, amp, the factor's fma or the K_t table the
+    kernel forms from theta, and the diagonal fl(sqrt(yerr^2 + tiny))^2); the last term is the rounding of the sums
+    of z^2 and log L_ii.  first_order = ||K^-1||_2 ||E||_F, which must be small (the test asserts <= 0.1) for the
+    neglected second-order terms not to matter."""
+    X = np.asarray(X, dtype=np.float64)
+    n = X.shape[0]
+    K = kernel_ld(flat, X, X)
+    K[np.diag_indices(n)] += LD(diag_add)
+    L = cholesky_ld(K)
+    if L is None:
+        return None
+    r = np.asarray(y, dtype=np.float64).astype(LD) - LD(mean)
+    z = forward_ld(L, r)
+    Linv = np.linalg.inv(L.astype(np.float64))
+    Kinv = exact_matmul(Linv.T, Linv)
+    alpha = (Kinv @ r).astype(np.float64)
+    logL = np.log(np.diag(L))
+    ll = -np.sum(z * z) / 2 - np.sum(logL) - LD(n) * np.log(2 * LD(np.pi)) / 2
+    aL = np.abs(L.astype(np.float64))
+    E = (gamma(n + 1) + 2 * gamma(n)) * (aL @ aL.T) \
+        + (len(flat["axis"]) + 2 * n_tasks + 24) * U * np.abs(K.astype(np.float64))
+    aK = np.abs(Kinv.astype(np.float64))
+    bound = C_HY * ((np.sum(aK * E) + np.abs(alpha) @ E @ np.abs(alpha)) / 2
+                    + (n + 8) * U * float(np.sum(np.abs(logL)) + np.sum(z * z)))
+    first = float(np.linalg.norm(aK, 2) * np.linalg.norm(E))
+    return dict(ll=ll, bound=float(bound), first_order=first)
+
+
 # ---- posterior covariance --------------------------------------------------------------------------------------------
 def cov_reference(Xinv, Ks, Kss, z, mean, ys2=1.0, y_mean=0.0, y_std=1.0, gemm=None):
     """dict(cov (unclipped, fp64), cov_bound, mu, mu_bound) from the device's X^, z^ and the kernel blocks
-    K* (m, N) and K** (m, m)."""
+    K* (m, N) and K** (m, m); K** as a vector (m,) gives the variances (m,) instead of the covariance."""
     gemm = gemm or _gemm_numpy
     N = Xinv.shape[0]
     V = exact_matmul(Xinv, Ks.T, gemm)                    # (N, m)
-    Vh, Vl = split2(V)
-    VtV = exact_matmul(Vh.T, Vh, gemm) + (gemm(Vh.T, Vl) + gemm(Vl.T, Vh)).astype(LD)
-    cov = ((Kss.astype(LD) - VtV) * LD(ys2)).astype(np.float64)
     W = gemm(np.abs(Xinv), np.abs(Ks.T))
-    cb = C_COV * (N + 16) * U * (np.abs(Kss) + gemm(W.T, W)) * ys2
+    if np.ndim(Kss) == 1:                                 # K** given as its diagonal: the variances alone
+        cov = ((Kss.astype(LD) - np.sum(V * V, axis=0)) * LD(ys2)).astype(np.float64)
+        cb = C_COV * (N + 16) * U * (np.abs(Kss) + np.sum(W * W, axis=0)) * ys2
+    else:
+        Vh, Vl = split2(V)
+        VtV = exact_matmul(Vh.T, Vh, gemm) + (gemm(Vh.T, Vl) + gemm(Vl.T, Vh)).astype(LD)
+        cov = ((Kss.astype(LD) - VtV) * LD(ys2)).astype(np.float64)
+        cb = C_COV * (N + 16) * U * (np.abs(Kss) + gemm(W.T, W)) * ys2
     ah, al = split2(exact_matmul(Xinv.T, z[:, None], gemm))         # a = X^T z
     mu_n = exact_matmul(Ks, ah, gemm)[:, 0] + gemm(Ks, al)[:, 0].astype(LD) + LD(mean)
     mu = (mu_n * LD(y_std) + LD(y_mean)).astype(np.float64)

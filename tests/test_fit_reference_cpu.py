@@ -262,3 +262,301 @@ def test_append_emulation_passes(emulated):
     assert R.factor_check(L2, e["K"], X2)[0] <= 1
     lc = R.linv_checks(L2, X2)
     assert lc["diag"][0] <= 1 and lc["node"][0] <= 1
+
+
+# ---- the single-column factors: environment (Fabolas) and task (MTBO) ---------------------------------------------------
+ENV_FLAT = dict(family=0, log_amp=0.2, axis=[0, 1], group=[0, 1], log_metric=[-1.0, -0.5], env=(2, 0.1, -0.3),
+                task=None)
+TASK_THETA = (-0.2, 0.3, -0.6, 0.1, -0.4, -1.0)
+
+
+def task_flat(n_tasks=3, theta=TASK_THETA):
+    return dict(family=0, log_amp=0.2, axis=[0, 1], group=[0, 1], log_metric=[-1.0, -0.5], env=None,
+                task=(2, n_tasks, tuple(theta[:n_tasks * (n_tasks + 1) // 2])))
+
+
+def factor_data(kind, N, seed=0, n_tasks=3):
+    rng = np.random.RandomState(seed)
+    X = rng.rand(N, 3)
+    if kind == "env":
+        X[:, 2] = (1 - rng.rand(N)) ** 2
+    else:
+        X[:, 2] = rng.randint(0, n_tasks, N)
+    y = np.sin(3 * X[:, 0]) + 0.3 * X[:, 2] + 0.1 * rng.randn(N)
+    return X, y - np.mean(y)
+
+
+def _mp_kernel(mpmath, flat, x1, x2, theta):
+    """k(x1, x2) in mpmath, theta = [log_amp, log_metric..., factor parameters] (Matern-5/2 per group)."""
+    nt = len(flat["axis"])
+    k = mpmath.exp(theta[0])
+    for g in sorted(set(flat["group"])):
+        r2 = mpmath.mpf(0)
+        for t in range(nt):
+            if flat["group"][t] == g:
+                ax = flat["axis"][t]
+                r2 += (mpmath.mpf(float(x1[ax])) - mpmath.mpf(float(x2[ax]))) ** 2 / mpmath.exp(theta[1 + t])
+        s = mpmath.sqrt(5 * r2)
+        k *= (1 + s + s * s / 3) * mpmath.exp(-s)
+    fp = theta[1 + nt:]
+    if flat["env"] is not None:
+        ax = flat["env"][0]
+        return k * (mpmath.exp(fp[0]) + mpmath.exp(fp[1]) * mpmath.mpf(float(x1[ax])) * mpmath.mpf(float(x2[ax])))
+    ax, nT, _ = flat["task"]
+    a, b = int(x1[ax]), int(x2[ax])
+    Lm = [[mpmath.exp(fp[p * (p + 1) // 2 + q]) if q <= p else 0 for q in range(nT)] for p in range(nT)]
+    return k * mpmath.fsum(Lm[a][q] * Lm[b][q] for q in range(nT))
+
+
+@pytest.mark.parametrize("kind", ["env", "task"])
+def test_factor_terms_against_mpmath(kind):
+    """K and every dK/dtheta of kernel_terms_ld, the factor entries included, against mpmath derivatives of the kernel
+    written out independently (300-bit, numerical differentiation at that precision)"""
+    mpmath = pytest.importorskip("mpmath")
+    mpmath.mp.prec = 300
+    flat = ENV_FLAT if kind == "env" else task_flat()
+    X, _ = factor_data(kind, 4, seed=3)
+    K, grads = R.kernel_terms_ld(flat, X)
+    fp = list(flat["env"][1:]) if kind == "env" else list(flat["task"][2])
+    theta0 = [mpmath.mpf(flat["log_amp"])] + [mpmath.mpf(v) for v in flat["log_metric"]] + [mpmath.mpf(v) for v in fp]
+    assert len(grads) == len(theta0)
+    for i in range(4):
+        for j in range(4):
+            ref = _mp_kernel(mpmath, flat, X[i], X[j], theta0)
+            assert abs(mpmath.mpf(float(K[i, j])) - ref) <= 4e-16 * abs(ref) + 1e-300
+            for p in range(len(theta0)):
+                def f(v, p=p):
+                    th = list(theta0)
+                    th[p] = v
+                    return _mp_kernel(mpmath, flat, X[i], X[j], th)
+                d = mpmath.diff(f, theta0[p])
+                got = grads[p][i, j]
+                # to longdouble precision (the reference's own rounding): 1e-17 of the largest term
+                assert abs(mpmath.mpf(float(got)) + mpmath.mpf(float(got - np.longdouble(float(got)))) - d) \
+                    <= 1e-17 * max(abs(ref), 1e-300), (kind, i, j, p)
+
+
+def test_fma_exact_where_double_rounding_bites():
+    """the longdouble fma of es_reference rounds twice; fma_exact must return the correctly rounded bits on the cases
+    where that goes wrong, and agree with it everywhere else"""
+    from fractions import Fraction
+    from tests import es_reference as ER
+    t = 2.0 ** -53
+    a = np.array([t * (1 + 2.0 ** -17), t * (1 + 2.0 ** -17), 1 + 2.0 ** -30, 3.0])
+    b = np.array([1.0, -1.0, 1 + 2.0 ** -30, 1.0 / 3.0])
+    c = np.array([1.0, -1.0, -1.0, -1.0])
+    got = ER.fma_exact(a, b, c)
+    for i in range(len(a)):
+        exact = float(Fraction(a[i]) * Fraction(b[i]) + Fraction(c[i]))
+        assert got[i] == exact, (i, got[i], exact)
+    # the first two: 1 + 2^-53 + 2^-70 is just above a midpoint, rounded to it in longdouble, then to even (1.0)
+    assert ER.fma(a[:2], b[:2], c[:2])[0] == 1.0 and got[0] == 1.0 + 2.0 ** -52 and got[1] == -(1.0 + 2.0 ** -52)
+    rng = np.random.RandomState(0)
+    a, b, c = rng.rand(3, 20000)
+    got = ER.fma_exact(a, b, c)
+    ref = np.array([float(Fraction(x) * Fraction(y) + Fraction(w)) for x, y, w in zip(a[:2000], b[:2000], c[:2000])])
+    assert np.array_equal(got[:2000], ref)
+
+
+def factor_problem(kind, N=300, seed=11, n_tasks=3):
+    flat = ENV_FLAT if kind == "env" else task_flat(n_tasks)
+    X, r = factor_data(kind, N, seed, n_tasks)
+    K = R.kernel_terms_ld(flat, X)[0].astype(np.float64)
+    K[np.diag_indices_from(K)] += 1e-2
+    L = np.linalg.cholesky(K)
+    Xin = spla.solve_triangular(L, np.eye(N), lower=True)
+    z = spla.solve_triangular(L, r, lower=True)
+    return dict(flat=flat, X=X, r=r, K=K, L=L, Xin=Xin, z=z)
+
+
+def factor_grad(e, dK_override=None, task_defect=None):
+    """gpk_nll_grad emulated in fp64: A = alpha alpha^T - K^-1 from X^, the radial and environment entries as
+    -1/2 sum A dK, the task entries contracted on the host from the per-pair sums G_ab (held for a >= b only).
+    dK_override: {entry: dK}.  task_defect: 'diag_once' (the a = b = p term of G counted once), ('drop', a, b)."""
+    flat, X = e["flat"], e["X"]
+    a = e["Xin"].T @ e["z"]
+    A = np.outer(a, a) - e["Xin"].T @ e["Xin"]
+    _, grads = R.kernel_terms_ld(flat, X)
+    nr = len(flat["axis"]) + 1
+    g = []
+    for p, dK in enumerate(grads):
+        if task_defect is not None and p >= nr:
+            break
+        dK = (dK_override or {}).get(p, dK)
+        g.append(-0.5 * np.sum(A * np.asarray(dK, dtype=np.float64)))
+    if task_defect is not None:
+        ax, nT, theta = flat["task"]
+        Rm = R._radial_ld(flat, X, X)[0].astype(np.float64)
+        t = X[:, ax].astype(int)
+        G = np.zeros((nT, nT))
+        for p in range(nT):
+            for q in range(p + 1):
+                G[p, q] = np.sum((A * Rm)[np.ix_(t == p, t == q)])
+        if isinstance(task_defect, tuple):
+            G[task_defect[1], task_defect[2]] = 0.0
+        Lt = np.array([[np.exp(theta[p * (p + 1) // 2 + q]) if q <= p else 0.0 for q in range(nT)] for p in range(nT)])
+        for p in range(nT):
+            for q in range(p + 1):
+                # dK_ab/dtheta_pq = L_pq (d_ap L_bq + d_bp L_aq): the row sum over b and the column sum over a
+                row = sum((G[p, b] if p >= b else G[b, p]) * Lt[b, q] for b in range(nT))
+                col = sum((G[a_, p] if a_ >= p else G[p, a_]) * Lt[a_, q] for a_ in range(nT))
+                if task_defect == "diag_once":
+                    col -= G[p, p] * Lt[p, q]
+                g.append(-0.5 * Lt[p, q] * (row + col))
+    g.append(-0.5 * np.trace(A) * 1e-2)
+    return np.array(g)
+
+
+def old_fd_ok(g, g0):
+    """the older central-difference check: rel = 1e-5, abs = 1e-6 per entry"""
+    return bool(np.all(np.abs(g - g0) <= 1e-5 * np.abs(g0) + 1e-6))
+
+
+@pytest.mark.parametrize("kind", ["env", "task"])
+def test_factor_checks_pass_on_the_emulation(kind):
+    e = factor_problem(kind)
+    g = factor_grad(e, task_defect="none" if kind == "task" else None)
+    g_ref, bnd = R.grad_reference(e["flat"], e["X"], e["Xin"], e["z"], 1e-2)
+    assert g.shape == g_ref.shape == (len(e["flat"]["axis"]) + (4 if kind == "env" else 2 + 6),)
+    assert np.all(np.abs(g - g_ref) <= bnd), np.abs(g - g_ref) / bnd
+    assert R.factor_check(e["L"], e["K"], e["Xin"])[0] <= 1
+    Xs = np.random.RandomState(5).rand(40, 3)
+    lo, up = np.array([0.0, 0.0, 0.0]), np.array([1.0, 1.0, 1.0])
+    Xs[:, 2] = np.random.RandomState(6).randint(0, 3, 40) if kind == "task" else Xs[:, 2]
+    dmu, dvar, bm, bv = R.predict_grad_reference(e["flat"], e["X"], e["Xin"], e["z"], Xs)
+    em, ev = emulate_predict_grad(e, Xs)
+    assert np.all(np.abs(em - dmu) <= bm) and np.all(np.abs(ev - dvar) <= bv)
+    if kind == "task":
+        assert np.all(dmu[:, 2] == 0) and np.all(dvar[:, 2] == 0)
+
+
+def emulate_predict_grad(e, Xs, lower=None, upper=None, drop_env_chain=False):
+    """gpk_predict_grad in fp64 (no output transform), from central differences-free closed forms"""
+    flat, X = e["flat"], e["X"]
+    Xn = Xs if lower is None else (Xs - lower) / (upper - lower)
+    span = np.ones(3) if lower is None else upper - lower
+    Ks = R.kernel_ld(flat, Xn, X).astype(np.float64)
+    alpha = e["Xin"].T @ e["z"]
+    W = (e["Xin"].T @ (e["Xin"] @ Ks.T)).T
+    Rm = R._radial_ld(flat, Xn, X)[0].astype(np.float64)
+    F = Ks / Rm
+    dmu, dvar = np.zeros(Xs.shape), np.zeros(Xs.shape)
+    for t, ax in enumerate(flat["axis"]):
+        s = np.sqrt(5 * (Xn[:, ax][:, None] - X[:, ax][None, :]) ** 2 / np.exp(flat["log_metric"][t]))
+        dl = -(5.0 / 6) * (1 + s) / (1 + s + s * s / 3)
+        dk = Ks * dl * 2 * (Xn[:, ax][:, None] - X[:, ax][None, :]) / np.exp(flat["log_metric"][t])
+        dmu[:, ax] = dk @ alpha / span[ax]
+        dvar[:, ax] = -2 * np.sum(dk * W, axis=1) / span[ax]
+    if flat["env"] is not None:
+        ax, la, lb = flat["env"]
+        dk = Rm * np.exp(lb) * X[:, ax][None, :]
+        sc = 1.0 if drop_env_chain else span[ax]
+        dmu[:, ax] = dk @ alpha / sc
+        dvar[:, ax] = (2 * np.exp(flat["log_amp"]) * np.exp(lb) * Xn[:, ax] - 2 * np.sum(dk * W, axis=1)) / sc
+    return dmu, dvar
+
+
+def factor_defect_rows():
+    """[(defect, old check passes?, new error / bound)] on N = 300, D = 2 + the factor column, diag 1e-2"""
+    rows = []
+    e = factor_problem("env")
+    flat, X = e["flat"], e["X"]
+    g_ref, bnd = R.grad_reference(flat, X, e["Xin"], e["z"], 1e-2)
+    g0 = factor_grad(e)
+    nr = len(flat["axis"]) + 1
+    # genvb accumulated with z_c z_c instead of z_c z_j
+    Rm = R._radial_ld(flat, X, X)[0]
+    z = X[:, 2].astype(np.longdouble)
+    g = factor_grad(e, {nr + 1: Rm * np.exp(np.longdouble(flat["env"][2])) * (z * z)[:, None]})
+    rows.append(("genvb with z_c z_c instead of z_c z_j", old_fd_ok(g, g0), R.ratio(np.abs(g - g_ref), bnd)))
+    # the factor scale skips the last, ragged 128-column tile (N = 300: columns 256..299) of the fit's K
+    N = X.shape[0]
+    Rk = R._radial_ld(flat, X, X)[0].astype(np.float64)
+    Kd = e["K"].copy()
+    Kd[:, 256:] = Rk[:, 256:] + 1e-2 * np.eye(N)[:, 256:]
+    Kd = np.tril(Kd) + np.tril(Kd, -1).T
+    try:
+        Ld = np.linalg.cholesky(Kd)
+        Xd = spla.solve_triangular(Ld, np.eye(N), lower=True)
+        ll = lambda L, r: -0.5 * np.sum(spla.solve_triangular(L, r, lower=True) ** 2) - np.sum(np.log(np.diag(L)))
+        old = abs(ll(Ld, e["r"]) - ll(e["L"], e["r"])) <= 1e-9 * abs(ll(e["L"], e["r"]))
+        rows.append(("factor scale skips the last ragged column tile", old, R.factor_check(Ld, e["K"], Xd)[0]))
+    except np.linalg.LinAlgError:
+        rows.append(("factor scale skips the last ragged column tile", False, np.inf))
+    # k** with the raw z* instead of the scaled one (environment axis bounds [0, 2])
+    lo, up = np.zeros(3), np.array([1.0, 1.0, 2.0])
+    Xs = np.random.RandomState(4).rand(50, 3) * up
+    Xn = (Xs - lo) / (up - lo)
+    Ks = R.kernel_ld(flat, Xn, X).astype(np.float64)
+    Kss = R.kernel_ld(flat, Xn, Xn).astype(np.float64)
+    ref = R.cov_reference(e["Xin"], Ks, Kss, e["z"], 0.0)
+    V = e["Xin"] @ Ks.T
+    amp, c0, c1 = np.exp(flat["log_amp"]), np.exp(flat["env"][1]), np.exp(flat["env"][2])
+    var_ok = np.diag(Kss) - np.sum(V * V, axis=0)
+    var_bad = amp * (c0 + c1 * Xs[:, 2] ** 2) - np.sum(V * V, axis=0)
+    vref = np.clip(np.diag(ref["cov"]), R.EPS, np.inf)
+    old = bool(np.max(np.abs(var_bad - vref) / np.maximum(vref, 1e-6)) < 1e-8)
+    assert R.ratio(np.abs(var_ok - np.diag(ref["cov"])), np.diag(ref["cov_bound"])) <= 1
+    rows.append(("k** from the raw z* instead of the scaled one", old,
+                 R.ratio(np.abs(var_bad - np.diag(ref["cov"])), np.diag(ref["cov_bound"]))))
+    # the 1 / (upper - lower) chain factor missing on the environment axis of predict_grad
+    dmu, dvar, bm, bv = R.predict_grad_reference(flat, X, e["Xin"], e["z"], Xs, lo, up)
+    em, ev = emulate_predict_grad(e, Xs, lo, up)
+    assert np.all(np.abs(em - dmu) <= bm) and np.all(np.abs(ev - dvar) <= bv)
+    dm, dv = emulate_predict_grad(e, Xs, lo, up, drop_env_chain=True)
+    old = bool(np.allclose(dm, em, rtol=1e-5, atol=1e-6) and np.allclose(dv, ev, rtol=1e-5, atol=1e-6))
+    rows.append(("predict_grad without 1 / (upper - lower) on the env axis", old,
+                 max(R.ratio(np.abs(dm - dmu), bm), R.ratio(np.abs(dv - dvar), bv))))
+    # the task factor
+    e = factor_problem("task")
+    flat, X = e["flat"], e["X"]
+    g_ref, bnd = R.grad_reference(flat, X, e["Xin"], e["z"], 1e-2)
+    g0 = factor_grad(e, task_defect="none")
+    assert np.all(np.abs(g0 - g_ref) <= bnd)
+    g = factor_grad(e, task_defect="diag_once")
+    rows.append(("task contraction: the a = b = p term of G counted once", old_fd_ok(g, g0),
+                 R.ratio(np.abs(g - g_ref), bnd)))
+    g = factor_grad(e, task_defect=("drop", 2, 0))
+    rows.append(("task contraction: the pair G_20 dropped", old_fd_ok(g, g0), R.ratio(np.abs(g - g_ref), bnd)))
+    # gpk_hy_eval reading K_t[t_i][t_i] for both indices
+    yv = e["r"][:120]
+    Xh = X[:120]
+    ref = R.hy_loglik_reference(flat, Xh, yv, 0.0, 1e-2, n_tasks=3)
+    assert ref["first_order"] <= 0.1
+    Rh = R._radial_ld(flat, Xh, Xh)[0].astype(np.float64)
+    Kt = R.task_factor_ld(flat["task"][2], 3)[0].astype(np.float64)
+    t = Xh[:, 2].astype(int)
+    Kb = Rh * Kt[t, t][:, None] + 1e-2 * np.eye(120)
+    Kb = np.tril(Kb) + np.tril(Kb, -1).T
+    try:
+        Lb = np.linalg.cholesky(Kb)
+        zb = spla.solve_triangular(Lb, yv, lower=True)
+        llb = -0.5 * zb @ zb - np.sum(np.log(np.diag(Lb))) - 60 * np.log(2 * np.pi)
+        old = abs(llb - float(ref["ll"])) <= 1e-9 * abs(float(ref["ll"])) + 1e-9
+        rows.append(("hy_eval: K_t[t_i][t_i] for both indices", old, abs(llb - float(ref["ll"])) / ref["bound"]))
+    except np.linalg.LinAlgError:
+        rows.append(("hy_eval: K_t[t_i][t_i] for both indices", False, np.inf))
+    return rows
+
+
+def test_factor_defect_table():
+    """every injected factor defect fails the new bounds (ratio > 1); the table printed is DESIGN.md section 2's"""
+    rows = factor_defect_rows()
+    for name, old_ok, r in rows:
+        print("%-58s old check passes: %-5s new error / bound: %.3g" % (name, old_ok, r))
+        assert r > 1, name
+    assert len(rows) == 7
+
+
+def test_hy_loglik_reference_on_fp64():
+    """the bound holds for an fp64 Cholesky of the same K (the device's algorithm class) at every factor"""
+    for kind in ("env", "task"):
+        flat = ENV_FLAT if kind == "env" else task_flat()
+        X, y = factor_data(kind, 60, seed=2)
+        ref = R.hy_loglik_reference(flat, X, y, 0.1, 1e-3, n_tasks=3 if kind == "task" else 0)
+        K = R.kernel_ld(flat, X, X).astype(np.float64) + 1e-3 * np.eye(60)
+        L = np.linalg.cholesky(K)
+        zz = spla.solve_triangular(L, y - 0.1, lower=True)
+        ll = -0.5 * zz @ zz - np.sum(np.log(np.diag(L))) - 30 * np.log(2 * np.pi)
+        assert ref["first_order"] <= 0.1
+        assert abs(ll - float(ref["ll"])) <= ref["bound"], (kind, abs(ll - float(ref["ll"])), ref["bound"])
