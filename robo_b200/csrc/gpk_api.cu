@@ -333,7 +333,7 @@ inline size_t cov_operand_rows(const gpk_handle* h, int d) { return (size_t)std:
 // the n points of `operand` (built by build_cov_operand, ld = ldx columns); out has ldo columns and at least
 // round_up(m, tile) rows.  small: the 128 x 16 tile variant that fits next to a resident variance-GEMM CTA.
 // pts (row-major raw inputs, dc columns, bounds plo / pup) are the operand's n points before build_cov_operand: the
-// environment factor reads its coordinate there, since the term-major operand carries the radial terms only.
+// kernel's factor reads its coordinate there, since the term-major operand carries the radial terms only.
 int launch_cov_tiles(gpk_handle* h, cudaStream_t st, const double* operand, long ldx, int n, const double* cand, int dc,
                      long m, long m_padded, const double* lo, const double* up, double* out, long ldo, int tri, bool small,
                      const double* pts, const double* plo, const double* pup) {
@@ -354,7 +354,7 @@ int launch_cov_tiles(gpk_handle* h, cudaStream_t st, const double* operand, long
         gpk_cov_kernel<16><<<dim3(gx, (unsigned)(m_padded / 32)), 256, 0, st>>>(h->spec, operand, ldx, n, cand, dc, m, lo, up, out, ldo, tri);
     }
     CKL();
-    if ((h->spec.env_axis >= 0 || h->spec.task_axis >= 0) && m > 0) {
+    if (h->spec.factor.kind != GPK_FACTOR_NONE && m > 0) {
         gpk_factor_scale_kernel<<<dim3(gx, (unsigned)std::min<long>((m + 1) / 2, 1024)), 256, 0, st>>>(
             h->spec, cand, dc, m, lo, up, pts, dc, n, plo, pup, out, ldo, tri);
         CKL();
@@ -863,11 +863,10 @@ int make_oz_map(gpk_handle* h, CUtensorMap* map, void* base, long rows_total, lo
 
 // Slices of L^-1 for the int8 contraction, once per factorisation.  Returns true in *usable when the factor is
 // conditioned well enough for S = 8 slices (row exponents <= OZ_MAX_EXP) and the sizes fit the int32 accumulators.
-// A kernel with the environment or task factor is never eligible: the digit split of K* assumes 0 < k <= amp.
+// A kernel with a factor is never eligible: the digit split of K* assumes 0 < k <= amp.
 int prepare_ozaki(gpk_handle* h, bool* usable) {
     *usable = false;
-    if (!h->ozaki || h->loader == LOADER_CPASYNC || h->NP > 16384 || h->spec.env_axis >= 0 ||
-        h->spec.task_axis >= 0)
+    if (!h->ozaki || h->loader == LOADER_CPASYNC || h->NP > 16384 || h->spec.factor.kind != GPK_FACTOR_NONE)
         return GPK_OK;
     const long NP = h->NP;
     if (h->oz_linv_serial != h->linv_serial) {
@@ -1070,17 +1069,10 @@ int score_dev(gpk_handle* h, const double* dX, long m, int kind, double eta, dou
         f.part_mu = ptr<double>(h->part_mu); f.part_ssq = ptr<double>(h->part_ssq);
         f.ldpart = cap; f.nparts = h->nb; f.m = mc; f.base = global_base + index_offset + base;
         f.kss = h->spec.amp; f.mean = h->mean;
-        if (h->spec.env_axis >= 0) {
-            f.env_axis = h->spec.env_axis; f.env_c0 = h->spec.env_c0; f.env_c1 = h->spec.env_c1;
-            f.env_cand = dX + base * h->d; f.env_dc = h->d;
-            f.env_lo = h->has_bounds ? ptr<double>(h->lower) : nullptr;
-            f.env_up = h->has_bounds ? ptr<double>(h->upper) : nullptr;
-        } else if (h->spec.task_axis >= 0) {
-            f.env_axis = h->spec.task_axis;
-            f.env_cand = dX + base * h->d; f.env_dc = h->d;
-            f.task_n = h->spec.n_tasks;
-            for (int t = 0; t < f.task_n; ++t) f.task_diag[t] = h->spec.task_K[t * f.task_n + t];
-        }
+        f.factor = h->spec.factor;
+        f.cand = dX + base * h->d; f.cand_dc = h->d;
+        f.lo = h->has_bounds ? ptr<double>(h->lower) : nullptr;
+        f.up = h->has_bounds ? ptr<double>(h->upper) : nullptr;
         f.norm_out = h->norm_out; f.y_mean = h->y_mean; f.y_std = h->y_std;
         f.acq_kind = kind; f.eta = eta; f.par = par;
         f.out_mu = d_mu ? d_mu + index_offset + base : nullptr;
@@ -1486,8 +1478,6 @@ int gpk_create(gpk_handle** out, int device) {
     gpk_handle* h = new gpk_handle();
     h->device = device;
     memset(&h->spec, 0, sizeof(h->spec));
-    h->spec.env_axis = -1;
-    h->spec.task_axis = -1;
     if (cudaSetDevice(device) != cudaSuccess) { delete h; return GPK_CUDA_ERROR; }
     {
         int lo = 0, hi = 0;
@@ -1648,15 +1638,27 @@ std::vector<int> scan_task_columns(const double* X, int n, int d) {
     return cols;
 }
 
-// the task factor's conditions on a training set with column summary cols: axis inside the data, no input bounds,
-// valid task indices
-int task_data_check(gpk_handle* h, const std::vector<int>& cols, const char* who) {
-    const KSpec& s = h->spec;
-    if (s.task_axis < 0) return GPK_OK;
-    if (s.task_axis >= h->d) BAD("%s: task axis %d >= d = %d", who, s.task_axis, h->d);
+// The kernel's factor against inputs of d columns: its axis inside them.  With cols, the column summary of a training
+// set (scan_task_columns), the task factor also needs unscaled inputs (no input bounds) and valid task indices.
+int factor_data_check(gpk_handle* h, int d, const std::vector<int>* cols, const char* who) {
+    const KFactor& f = h->spec.factor;
+    if (f.kind == GPK_FACTOR_NONE) return GPK_OK;
+    if (f.axis >= d)
+        BAD("%s: %s axis %d >= d = %d", who, f.kind == GPK_FACTOR_ENV ? "environment" : "task", f.axis, d);
+    if (f.kind != GPK_FACTOR_TASK || !cols) return GPK_OK;
     if (h->has_bounds) BAD("%s: the task factor needs unscaled inputs (no input bounds)", who);
-    if ((int)cols.size() != h->d || cols[s.task_axis] > s.n_tasks)
-        BAD("%s: training column %d holds a value that is not a task index in [0, %d)", who, s.task_axis, s.n_tasks);
+    if ((int)cols->size() != d || (*cols)[f.axis] > f.n_tasks)
+        BAD("%s: training column %d holds a value that is not a task index in [0, %d)", who, f.axis, f.n_tasks);
+    return GPK_OK;
+}
+
+// gpk_set_env_factor / gpk_set_task_factor after their checks: f (kind NONE: clear) replaces the kernel's factor,
+// except that clearing one kind leaves a factor of the other kind in place
+int set_factor(gpk_handle* h, int kind, const KFactor& f) {
+    if (f.kind != GPK_FACTOR_NONE || h->spec.factor.kind == kind) h->spec.factor = f;
+    h->fitted = false;
+    h->linv_ready = false;
+    h->alpha_ready = false;
     return GPK_OK;
 }
 }  // namespace
@@ -1754,8 +1756,6 @@ int gpk_set_kernel(gpk_handle* h, int family, double log_amp, int n_terms, const
         s.last[t] = (t == n_terms - 1) || (group[t + 1] != group[t]);
     }
     if (group[0] != 0) BAD("gpk_set_kernel: groups must start at 0");
-    s.env_axis = -1;
-    s.task_axis = -1;
     h->spec = s;
     h->log_amp = log_amp;
     h->log_metric.assign(log_metric, log_metric + n_terms);
@@ -1771,36 +1771,33 @@ int gpk_set_env_factor(gpk_handle* h, int axis, double log_a, double log_b) {
     if (gp_refusal(h)) BAD("gpk_set_env_factor: %s", gp_refusal(h));
     if (axis < -1 || axis >= GPK_MAX_TERMS) BAD("gpk_set_env_factor: axis %d out of range", axis);
     if (!std::isfinite(log_a) || !std::isfinite(log_b)) BAD("gpk_set_env_factor: log_a and log_b must be finite");
-    if (axis >= 0 && h->spec.task_axis >= 0) BAD("gpk_set_env_factor: the kernel has a task factor");
-    h->spec.env_axis = axis;
-    h->spec.env_c0 = axis >= 0 ? exp(log_a) : 0.0;
-    h->spec.env_c1 = axis >= 0 ? exp(log_b) : 0.0;
-    h->fitted = false;
-    h->linv_ready = false;
-    h->alpha_ready = false;
-    return GPK_OK;
+    if (axis >= 0 && h->spec.factor.kind == GPK_FACTOR_TASK) BAD("gpk_set_env_factor: the kernel has a task factor");
+    KFactor f{};
+    if (axis >= 0) {
+        const double p[2] = {log_a, log_b};
+        f = KFactor{GPK_FACTOR_ENV, axis};
+        gpk_factor_build(f, p);
+    }
+    return set_factor(h, GPK_FACTOR_ENV, f);
 }
 
 int gpk_set_task_factor(gpk_handle* h, int axis, int n_tasks, const double* theta) {
     if (!h) return GPK_BAD_ARG;
     if (gp_refusal(h)) BAD("gpk_set_task_factor: %s", gp_refusal(h));
     if (axis < -1 || axis >= GPK_MAX_TERMS) BAD("gpk_set_task_factor: axis %d out of range", axis);
+    KFactor f{};
     if (axis >= 0) {
         if (n_tasks < 1 || n_tasks > GPK_MAX_TASKS)
             BAD("gpk_set_task_factor: n_tasks = %d outside 1..%d (GPK_MAX_TASKS)", n_tasks, GPK_MAX_TASKS);
         if (!theta) BAD("gpk_set_task_factor: need theta");
         for (int k = 0; k < n_tasks * (n_tasks + 1) / 2; ++k)
             if (!std::isfinite(theta[k])) BAD("gpk_set_task_factor: theta[%d] is not finite", k);
-        if (h->spec.env_axis >= 0) BAD("gpk_set_task_factor: the kernel has an environment factor");
-        gpk_task_matrix(n_tasks, theta, h->spec.task_K);
+        if (h->spec.factor.kind == GPK_FACTOR_ENV) BAD("gpk_set_task_factor: the kernel has an environment factor");
+        f = KFactor{GPK_FACTOR_TASK, axis, n_tasks};
+        gpk_factor_build(f, theta);
         h->task_theta.assign(theta, theta + n_tasks * (n_tasks + 1) / 2);
     }
-    h->spec.task_axis = axis;
-    h->spec.n_tasks = axis >= 0 ? n_tasks : 0;
-    h->fitted = false;
-    h->linv_ready = false;
-    h->alpha_ready = false;
-    return GPK_OK;
+    return set_factor(h, GPK_FACTOR_TASK, f);
 }
 
 
@@ -1810,8 +1807,7 @@ int gpk_fit_begin(gpk_handle* h, double diag_add, double mean) {
     CK(cudaSetDevice(h->device));
     for (int t = 0; t < h->spec.n_terms; ++t)
         if (h->spec.axis[t] >= h->d) BAD("gpk_fit: kernel axis %d >= d = %d", h->spec.axis[t], h->d);
-    if (h->spec.env_axis >= h->d) BAD("gpk_fit: environment axis %d >= d = %d", h->spec.env_axis, h->d);
-    if ((rc = task_data_check(h, h->col_tasks, "gpk_fit"))) return rc;
+    if ((rc = factor_data_check(h, h->d, &h->col_tasks, "gpk_fit"))) return rc;
     const long NP = h->NP;
     const int nb = h->nb;
     if (!h->maps_ok && (rc = rebuild_maps(h))) return rc;        // staging mode changed after gpk_set_data
@@ -1982,7 +1978,7 @@ int gpk_fit_append(gpk_handle* h, const double* X, const double* y, int n, int d
     if (!h->maps_ok && (rc = rebuild_maps(h))) return rc;
     // checked before anything is uploaded; committed once the device holds the new rows
     std::vector<int> cols = scan_task_columns(X, n, d);
-    if ((rc = task_data_check(h, cols, "gpk_fit_append"))) return rc;
+    if ((rc = factor_data_check(h, d, &cols, "gpk_fit_append"))) return rc;
     double* K = ptr<double>(h->Kbuf);
     double* P = ptr<double>(h->P);
     double* Q = ptr<double>(h->Q);
@@ -2463,7 +2459,8 @@ int gpk_predict_grad(gpk_handle* h, const double* Xs, long m, int kind, double e
     double* d_dmu = ptr<double>(h->tmp1);
     double* d_dvar = d_dmu + m * d;
     {
-        auto kern = h->spec.task_axis >= 0 ? gpk_predict_grad_kernel<true> : gpk_predict_grad_kernel<false>;
+        auto kern = h->spec.factor.kind == GPK_FACTOR_TASK ? gpk_predict_grad_kernel<GPK_FACTOR_TASK>
+                                                           : gpk_predict_grad_kernel<GPK_FACTOR_ENV>;
         kern<<<(unsigned)m, 256, 0, h->stream>>>(h->spec, ptr<double>(h->Xt), NP, h->n, ptr<double>(h->cand), d, lo, up,
                                                  ptr<double>(h->alpha), ptr<double>(h->cov), NP, h->norm_out, h->y_std,
                                                  d_dmu, d_dvar);
@@ -2559,29 +2556,29 @@ int gpk_set_hyper_model(gpk_handle* h, int n_params, const int* amp_slot, const 
     m.n_terms = n_terms;
     m.n_params = n_params;
     std::vector<int> used(n_params, 0);
-    m.env_axis = m.env_pa = m.env_pb = -1;
-    m.task_axis = -1;
+    int pa = -1, pb = -1;                     // the log_a and log_b slots; the task slots go straight into m.fp
     for (int p = 0; p < n_params; ++p) {
         if (amp_slot[p] < 0 || amp_slot[p] > 4) BAD("%s: slot kind %d of parameter %d is not 0..4", who, amp_slot[p], p);
         if (amp_slot[p] == 4) {
-            if (m.n_kt == GPK_MAX_TASKS * (GPK_MAX_TASKS + 1) / 2) BAD("%s: too many task slots", who);
-            m.task_p[m.n_kt++] = (unsigned char)p;
+            if (m.n_fp == GPK_MAX_TASKS * (GPK_MAX_TASKS + 1) / 2) BAD("%s: too many task slots", who);
+            m.fp[m.n_fp++] = (unsigned char)p;
         }
         m.amp[p] = amp_slot[p] == 1 ? 1 : 0;
-        int* env_p = amp_slot[p] == 2 ? &m.env_pa : amp_slot[p] == 3 ? &m.env_pb : nullptr;
+        int* env_p = amp_slot[p] == 2 ? &pa : amp_slot[p] == 3 ? &pb : nullptr;
         if (env_p) {
             if (*env_p >= 0) BAD("%s: more than one log_%c slot", who, amp_slot[p] == 2 ? 'a' : 'b');
             *env_p = p;
         }
     }
-    if ((m.env_pa >= 0) != (m.env_pb >= 0) || (m.env_pa >= 0) != (h->spec.env_axis >= 0))
+    const KFactor& f = h->spec.factor;
+    if ((pa >= 0) != (pb >= 0) || (pa >= 0) != (f.kind == GPK_FACTOR_ENV))
         BAD("%s: the log_a / log_b slots must match the kernel's environment factor", who);
-    m.env_axis = h->spec.env_axis;
-    if (m.n_kt != (h->spec.task_axis >= 0 ? h->spec.n_tasks * (h->spec.n_tasks + 1) / 2 : 0))
-        BAD("%s: %d task slots, the kernel's task factor has %d entries", who, m.n_kt,
-            h->spec.task_axis >= 0 ? h->spec.n_tasks * (h->spec.n_tasks + 1) / 2 : 0);
-    m.task_axis = h->spec.task_axis;
-    m.n_tasks = h->spec.n_tasks;
+    const int n_kt = f.kind == GPK_FACTOR_TASK ? f.n_tasks * (f.n_tasks + 1) / 2 : 0;
+    if (m.n_fp != n_kt) BAD("%s: %d task slots, the kernel's task factor has %d entries", who, m.n_fp, n_kt);
+    if (pa >= 0) { m.fp[0] = (unsigned char)pa; m.fp[1] = (unsigned char)pb; m.n_fp = 2; }
+    m.f_kind = f.kind;
+    m.f_axis = f.axis;
+    m.f_n_tasks = f.n_tasks;
     for (int t = 0; t < n_terms; ++t) {
         const int p = term_param[t];
         if (p < 0 || p >= n_params || amp_slot[p] != 0) BAD("%s: term %d is not set by a metric slot", who, t);
@@ -2612,12 +2609,11 @@ int hyper_ready(gpk_handle* h, int dim, const char* who) {
     int rc = require(h, true, true, false);
     if (rc) return rc;
     if (!h->has_hyper) BAD("%s: gpk_set_hyper_model has not been called", who);
-    if (h->hyper.env_axis != h->spec.env_axis) BAD("%s: the kernel structure changed since gpk_set_hyper_model", who);
-    if (h->spec.env_axis >= h->d) BAD("%s: environment axis %d >= d = %d", who, h->spec.env_axis, h->d);
-    if (h->hyper.task_axis != h->spec.task_axis || h->hyper.n_tasks != h->spec.n_tasks)
-        BAD("%s: the kernel structure changed since gpk_set_hyper_model", who);
-    if ((rc = task_data_check(h, h->col_tasks, who))) return rc;
     const HyperModel& m = h->hyper;
+    const KFactor& f = h->spec.factor;
+    if (m.f_kind != f.kind || m.f_axis != f.axis || m.f_n_tasks != f.n_tasks)
+        BAD("%s: the kernel structure changed since gpk_set_hyper_model", who);
+    if ((rc = factor_data_check(h, h->d, &h->col_tasks, who))) return rc;
     if (m.n_terms != h->spec.n_terms || m.family != h->spec.family)
         BAD("%s: the kernel structure changed since gpk_set_hyper_model", who);
     for (int t = 0; t < m.n_terms; ++t) {
@@ -2993,8 +2989,7 @@ int gpk_kernel_matrix(gpk_handle* h, const double* X1, long n1, const double* X2
     if (!X1 || !X2 || !out || n1 <= 0 || n2 <= 0 || d <= 0 || d > GPK_MAX_TERMS) BAD("gpk_kernel_matrix: bad arguments");
     for (int t = 0; t < h->spec.n_terms; ++t)
         if (h->spec.axis[t] >= d) BAD("gpk_kernel_matrix: kernel axis %d >= d = %d", h->spec.axis[t], d);
-    if (h->spec.env_axis >= d) BAD("gpk_kernel_matrix: environment axis %d >= d = %d", h->spec.env_axis, d);
-    if (h->spec.task_axis >= d) BAD("gpk_kernel_matrix: task axis %d >= d = %d", h->spec.task_axis, d);
+    if ((rc = factor_data_check(h, d, nullptr, "gpk_kernel_matrix"))) return rc;
     CK(cudaSetDevice(h->device));
     const long n1p = round_up(n1, 32), n2p = round_up(n2, 128);
     if ((rc = ensure(h, h->tmp1, (size_t)n1 * d * 8))) return rc;
@@ -3022,8 +3017,10 @@ int gpk_nll_grad(gpk_handle* h, double noise_var, double* grad) {
     CK(cudaSetDevice(h->device));
     if ((rc = build_linv(h))) return rc;
     const long NP = h->NP;
-    const int nT = h->spec.task_axis >= 0 ? h->spec.n_tasks : 0;
-    const int nv = h->spec.n_terms + (h->spec.env_axis >= 0 ? 4 : 2);
+    // [amp, metric..., factor parameters..., noise]: environment entries from the trace kernel, task entries below
+    const int fk = h->spec.factor.kind;
+    const int nT = fk == GPK_FACTOR_TASK ? h->spec.factor.n_tasks : 0;
+    const int nv = h->spec.n_terms + (fk == GPK_FACTOR_ENV ? 4 : 2);
     // alpha = L^-T z
     if ((rc = ensure(h, h->alpha, (size_t)NP * 8))) return rc;
     gpk_rowdot_kernel<<<(unsigned)((NP + 7) / 8), 256, 0, h->stream>>>(ptr<double>(h->Q), NP, NP, (int)NP, 1,
@@ -3047,7 +3044,8 @@ int gpk_nll_grad(gpk_handle* h, double noise_var, double* grad) {
     if ((rc = ensure(h, h->tmp1, (size_t)nblocks * (nv + nT * nT) * 8))) return rc;
     if ((rc = ensure(h, h->tmp2, (size_t)(nv + nT * nT) * 8))) return rc;
     {
-        auto kern = h->spec.task_axis >= 0 ? gpk_grad_trace_kernel<true> : gpk_grad_trace_kernel<false>;
+        auto kern = fk == GPK_FACTOR_ENV ? gpk_grad_trace_kernel<GPK_FACTOR_ENV>
+                  : fk == GPK_FACTOR_TASK ? gpk_grad_trace_kernel<GPK_FACTOR_TASK> : gpk_grad_trace_kernel<GPK_FACTOR_NONE>;
         kern<<<tg, 256, 0, h->stream>>>(h->spec, ptr<double>(h->Xt), NP, h->n, ptr<double>(h->Xrow), h->d,
                                         ptr<double>(h->W), NP, ptr<double>(h->alpha), ptr<double>(h->tmp1));
     }

@@ -362,7 +362,7 @@ __global__ void gpk_ep_apply_kernel(int D, double* __restrict__ dMu, double* __r
 #define GPK_ES_THREADS 256
 
 // k(a, b) of the handle's kernel on scaled inputs: amp * prod_g f(sum_{t in g} (a - b)^2 / metric_t), times the
-// environment or task factor when the kernel has one
+// kernel's factor when it has one
 __device__ __forceinline__ double gpk_es_kval(const KSpec& s, const double* a, const double* b) {
     double prod = 1.0, r2 = 0.0;
     for (int t = 0; t < s.n_terms; ++t) {
@@ -374,8 +374,7 @@ __device__ __forceinline__ double gpk_es_kval(const KSpec& s, const double* a, c
         }
     }
     const double k = s.amp * prod;
-    if (s.env_axis >= 0) return k * gpk_env(s.env_c0, s.env_c1, a[s.env_axis], b[s.env_axis]);
-    return s.task_axis >= 0 ? k * gpk_task(s, a[s.task_axis], b[s.task_axis]) : k;
+    return s.factor.kind != GPK_FACTOR_NONE ? k * gpk_factor_value(s.factor, a[s.factor.axis], b[s.factor.axis]) : k;
 }
 
 // raw representer points -> scaled (x - lower) / (upper - lower) when the handle scales its inputs

@@ -8,10 +8,9 @@
 //   - kernel: log_amp = 0.0 + the amplitude-slot entries in slot order, amp = exp(log_amp); every term t takes
 //     inv_metric_t = 1 / exp(theta[term_param[t]]) (an isotropic metric slot lists all the terms of its group);
 //     K_ij = amp prod_g gpk_radial(family, sum_{t in g} (x_i - x_j)^2 inv_metric_t) on the handle's inputs, family /
-//     axes / groups of the handle's KSpec; with the environment factor (gpk_set_env_factor) K_ij is multiplied by
-//     gpk_env(exp(theta[env_pa]), exp(theta[env_pb]), z_i, z_j), z = input column env_axis; with the task factor
-//     (gpk_set_task_factor) by K_t[t_i][t_j] of gpk_task_matrix over the task slots theta[task_p[k]] in packed order,
-//     t = input column task_axis (valid task indices: gpk_fit's check), K_t built by thread 0 into the reduction scratch
+//     axes / groups of the handle's KSpec; with a factor K_ij is multiplied by gpk_factor_value(z_i, z_j), z = the
+//     factor's input column, the factor built by thread 0 (gpk_factor_build) into the reduction scratch from the
+//     parameters theta[fp[k]] that feed it: log_a, log_b (slot kinds 2, 3) or the packed task entries (slot kind 4)
 //   - diagonal: diag_add = fl(sqrt(fl(yerr^2 + tiny)))^2, yerr = sqrt(exp(theta[-1]))  (_LikelihoodPool.loglik)
 //   - packed fp64 lower triangle in shared memory (n <= GPK_HYPER_MAX_N), right-looking Cholesky one column at a time
 //     with the residual r = y - mean carried as an extra row, so r ends as z = L^-1 r; a pivot that is not > 0 (NaN
@@ -54,9 +53,9 @@ struct HyperModel {
     int last[GPK_MAX_TERMS];
     int term_param[GPK_MAX_TERMS];            // the metric slot (parameter index) of term t
     unsigned char amp[GPK_HYPER_MAX_DIM];     // 1: parameter p is an amplitude slot
-    int env_axis, env_pa, env_pb;             // environment factor: its column and the parameters log_a, log_b (-1: none)
-    int task_axis, n_tasks, n_kt;             // task factor: its column (-1: none), tasks, Cholesky entries
-    unsigned char task_p[GPK_MAX_TASKS * (GPK_MAX_TASKS + 1) / 2];   // the parameter of packed entry k
+    int f_kind, f_axis, f_n_tasks;            // the kernel's factor: KFactor's kind, axis, n_tasks
+    int n_fp;                                 // the parameters that feed it, in gpk_factor_build's order
+    unsigned char fp[GPK_MAX_TASKS * (GPK_MAX_TASKS + 1) / 2];
     double mean, tiny;
     int prior, n_ls, n_lr;
     double ln_sigma, ln_loc, th_lo, th_hi, hs_scale, nrm_sigma, nrm_mean;
@@ -65,7 +64,7 @@ struct HyperModel {
 // doubles of dynamic shared memory gpk_hy_eval needs for n training points
 __host__ __device__ inline long gpk_hy_smem_doubles(int n)
 {
-    return (long)n * (n + 1) / 2 + n + (n + 1) + 2 * GPK_HY_THREADS + 6 + GPK_MAX_TERMS;
+    return (long)n * (n + 1) / 2 + n + (n + 1) + 2 * GPK_HY_THREADS + 4 + GPK_MAX_TERMS;
 }
 
 // scipy.stats.lognorm.logpdf(x, s, loc=loc): -inf for x <= loc, NaN stays NaN
@@ -146,9 +145,9 @@ __device__ void gpk_hy_eval(const HyperModel& m, const double* __restrict__ Xt, 
     double* r = A + (long)n * (n + 1) / 2;           // y - mean, then z = L^-1 (y - mean)
     double* col = r + n;                             // column k of L (rows k + 1 .. n; row n = the residual row)
     double* red = col + n + 1;                       // 2 NT partial sums
-    double* kt = red;                                // task factor's K_t during the K build (red is free until the sums)
-    double* par = red + 2 * NT;                      // amp, diag_add, lp, ll, env c0, env c1
-    double* im = par + 6;                            // inv_metric of every term
+    KFactor* kf = reinterpret_cast<KFactor*>(red);   // the factor during the K build (red is free until the sums)
+    double* par = red + 2 * NT;                      // amp, diag_add, lp, ll
+    double* im = par + 4;                            // inv_metric of every term
 
     bool out = false;
     for (int j = 0; j < D; ++j) out = out || th[j] < -20.0 || th[j] > 20.0;
@@ -161,11 +160,11 @@ __device__ void gpk_hy_eval(const HyperModel& m, const double* __restrict__ Xt, 
         const double yerr = sqrt(exp(th[D - 1]));
         const double s = sqrt(__dadd_rn(__dmul_rn(yerr, yerr), m.tiny));
         par[1] = __dmul_rn(s, s);
-        if (m.env_axis >= 0) { par[4] = exp(th[m.env_pa]); par[5] = exp(th[m.env_pb]); }
-        if (m.task_axis >= 0) {
-            double* tt = kt + GPK_MAX_TASKS * GPK_MAX_TASKS;    // the packed entries, gathered
-            for (int k = 0; k < m.n_kt; ++k) tt[k] = th[m.task_p[k]];
-            gpk_task_matrix(m.n_tasks, tt, kt);
+        if (m.f_kind != GPK_FACTOR_NONE) {
+            double* fpv = red + sizeof(KFactor) / sizeof(double);   // the factor's parameters, gathered
+            for (int k = 0; k < m.n_fp; ++k) fpv[k] = th[m.fp[k]];
+            kf->kind = m.f_kind; kf->axis = m.f_axis; kf->n_tasks = m.f_n_tasks;
+            gpk_factor_build(*kf, fpv);
         }
     }
     for (int t = tid; t < m.n_terms; t += NT) im[t] = 1.0 / exp(th[m.term_param[t]]);
@@ -184,12 +183,9 @@ __device__ void gpk_hy_eval(const HyperModel& m, const double* __restrict__ Xt, 
                     if (m.last[t]) { pr *= gpk_radial(m.family, r2); r2 = 0.0; }
                 }
                 double v = amp * pr;
-                if (m.env_axis >= 0) {
-                    const double* za = Xt + (long)m.env_axis * ldx;
-                    v *= gpk_env(par[4], par[5], za[i], za[j]);
-                } else if (m.task_axis >= 0) {
-                    const double* ta = Xt + (long)m.task_axis * ldx;
-                    v *= kt[(int)ta[i] * m.n_tasks + (int)ta[j]];
+                if (m.f_kind != GPK_FACTOR_NONE) {
+                    const double* za = Xt + (long)m.f_axis * ldx;
+                    v *= gpk_factor_value(*kf, za[i], za[j]);
                 }
                 row[j] = (j == i) ? v + dg : v;
             }

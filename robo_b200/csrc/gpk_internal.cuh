@@ -9,8 +9,21 @@
 #define GPK_TILE 128          // block size of every blocked algorithm (rows per tile)
 #define GPK_EPS 2.220446049250313e-16
 
+// The kernel's single-column factor: k *= gpk_factor_value(f, z, z'), z = column `axis` of each input row.  The kind
+// decides everything else: the environment factor (gpk_set_env_factor) c0 + c1 z z' on the input-bounds-scaled
+// coordinate, the task factor (gpk_set_task_factor) K[t * n_tasks + t'] on the raw coordinate (never scaled; gpk_fit
+// refuses input bounds with it).  A kernel has at most one factor, so one descriptor carries either.
+enum { GPK_FACTOR_NONE = 0, GPK_FACTOR_ENV = 1, GPK_FACTOR_TASK = 2 };
+struct KFactor {
+    int kind;                       // GPK_FACTOR_*; NONE: every other field is zero
+    int axis;                       // the input column z is read from
+    int n_tasks;                    // task: K is n_tasks x n_tasks, row-major
+    double c0, c1;                  // environment: c0 = exp(log_a), c1 = exp(log_b)
+    double K[GPK_MAX_TASKS * GPK_MAX_TASKS];
+};
+
 // Kernel specification passed by value to the covariance-building kernels.
-// k(x,x') = amp * prod_g f( sum_{t in g} (x[axis_t]-x'[axis_t])^2 * inv_metric_t )
+// k(x,x') = amp * prod_g f( sum_{t in g} (x[axis_t]-x'[axis_t])^2 * inv_metric_t ) [* the factor]
 struct KSpec {
     int family;
     int n_terms;
@@ -20,14 +33,7 @@ struct KSpec {
     double inv_metric[GPK_MAX_TERMS];
     double scale[GPK_MAX_TERMS];    // sqrt(c_f / metric_t): coordinates pre-scaled so that q = sum (s - s')^2 is the
                                     // radial argument directly (c_f = 5 Matern-5/2, 3 Matern-3/2, 1/2 ExpSquared)
-    // environment factor (gpk_set_env_factor): k *= env_c0 + env_c1 * z * z', z = x[env_axis] after the input-bounds
-    // scaling; env_axis = -1: none
-    int env_axis;
-    double env_c0, env_c1;
-    // task factor (gpk_set_task_factor): k *= task_K[t * n_tasks + t'], t = x[task_axis] (never scaled); task_axis = -1:
-    // none.  At most one of env_axis / task_axis is set.
-    int task_axis, n_tasks;
-    double task_K[GPK_MAX_TASKS * GPK_MAX_TASKS];
+    KFactor factor;                 // last, so the kernels that never read it see the same parameter layout
 };
 
 // The environment factor of Fabolas, restated from arXiv:1605.07079 (not checked against the george fork that defines
@@ -35,13 +41,6 @@ struct KSpec {
 // d/dlog_a = c0, d/dlog_b = c1 z z', d/dz = c1 z' (gpk_env_dz).  Test restatement: tests/env_kernel_model.py (env_value).
 __device__ __forceinline__ double gpk_env(double c0, double c1, double z, double z2) { return fma(c1 * z, z2, c0); }
 __device__ __forceinline__ double gpk_env_dz(double c1, double z2) { return c1 * z2; }
-
-// x[axis] of one row of raw inputs, scaled (x - lower) / (upper - lower) when bounds are given
-__device__ __forceinline__ double gpk_env_coord(const double* row, int axis, const double* lower, const double* upper) {
-    double v = row[axis];
-    if (lower != nullptr) v = (v - lower[axis]) / (upper[axis] - lower[axis]);
-    return v;
-}
 
 // The task factor of MTBO, restated from Swersky, Snoek, Adams (NIPS 2013) and the reference's call sites (not checked
 // against the george fork that defines TaskKernel): K_t = L L^T, L lower triangular, L_pq = exp(theta[p (p + 1) / 2 + q])
@@ -69,16 +68,31 @@ __host__ __device__ __forceinline__ int gpk_task_index(double t, int n) {
     return (t >= 0.0 && t < (double)n && t == floor(t)) ? (int)t : -1;
 }
 
-// K_t[t][t'] of the kernel's task factor, NaN when either coordinate is not a task
-__device__ __forceinline__ double gpk_task(const KSpec& s, double t, double t2) {
-    const int a = gpk_task_index(t, s.n_tasks), b = gpk_task_index(t2, s.n_tasks);
-    return (a < 0 || b < 0) ? __longlong_as_double(0x7ff8000000000000LL) : s.task_K[a * s.n_tasks + b];
+// The factor's coordinate in one row of raw inputs: row[axis], scaled (x - lower) / (upper - lower) when bounds are
+// given and the factor is the environment factor.  FK here and in gpk_factor_value: the kind when the caller's
+// instance fixes it at compile time (the gradient kernels), so the other kind's code is compiled out; -1: f.kind.
+template <int FK = -1>
+__device__ __forceinline__ double gpk_factor_coord(const KFactor& f, const double* row, const double* lower,
+                                                   const double* upper) {
+    double v = row[f.axis];
+    if ((FK < 0 ? f.kind : FK) == GPK_FACTOR_ENV && lower != nullptr)
+        v = (v - lower[f.axis]) / (upper[f.axis] - lower[f.axis]);
+    return v;
 }
 
-// the kernel's single-column factor (environment or task): its column (-1: none) and its value at coordinates z, z'
-__device__ __forceinline__ int gpk_factor_axis(const KSpec& s) { return s.env_axis >= 0 ? s.env_axis : s.task_axis; }
-__device__ __forceinline__ double gpk_factor(const KSpec& s, double z, double z2) {
-    return s.env_axis >= 0 ? gpk_env(s.env_c0, s.env_c1, z, z2) : gpk_task(s, z, z2);
+// The factor's value at coordinates z, z' (kind != NONE): gpk_env, or K_t[z][z'] (NaN when either is not a task)
+template <int FK = -1>
+__device__ __forceinline__ double gpk_factor_value(const KFactor& f, double z, double z2) {
+    if ((FK < 0 ? f.kind : FK) == GPK_FACTOR_ENV) return gpk_env(f.c0, f.c1, z, z2);
+    const int a = gpk_task_index(z, f.n_tasks), b = gpk_task_index(z2, f.n_tasks);
+    return (a < 0 || b < 0) ? __longlong_as_double(0x7ff8000000000000LL) : f.K[a * f.n_tasks + b];
+}
+
+// The factor's values from its log-parameters p (kind, axis and n_tasks already set): environment (log_a, log_b),
+// task the n_tasks (n_tasks + 1) / 2 packed entries of gpk_task_matrix.  Host or device exp, whichever side calls it.
+__host__ __device__ inline void gpk_factor_build(KFactor& f, const double* p) {
+    if (f.kind == GPK_FACTOR_ENV) { f.c0 = exp(p[0]); f.c1 = exp(p[1]); }
+    else if (f.kind == GPK_FACTOR_TASK) gpk_task_matrix(f.n_tasks, p, f.K);
 }
 
 // f as a function of q = c_f * r2 (pre-scaled coordinates, gpk_cov_tma_kernel)

@@ -162,11 +162,11 @@ gpk_cov_tma_kernel(const __grid_constant__ CUtensorMap mapX, const KSpec ks, int
     }
 }
 
-// Single-column factor over a tile the builders above wrote: out[c][j] *= gpk_factor(z_c, z_j) (the environment factor
-// c0 + c1 z_c z_j or the task factor K_t[z_c][z_j]), z = column gpk_factor_axis of the candidates (row-major raw inputs
-// cand, bounds lo / up) and of the points (row-major raw inputs pts, bounds plo / pup).  Runs only when the kernel has a
-// factor, so the builders, their registers and their bits stay those of the kernel without it.  tri != 0: only the
-// tiles the triangular K build wrote (column tile start <= the row's 32-row block end).
+// Single-column factor over a tile the builders above wrote: out[c][j] *= gpk_factor_value(z_c, z_j), z the factor's
+// coordinate of the candidates (row-major raw inputs cand, bounds lo / up) and of the points (row-major raw inputs
+// pts, bounds plo / pup).  Runs only when the kernel has a factor, so the builders, their registers and their bits
+// stay those of the kernel without it.  tri != 0: only the tiles the triangular K build wrote (column tile start <= the
+// row's 32-row block end).
 __global__ void __launch_bounds__(256)
 gpk_factor_scale_kernel(const KSpec ks, const double* __restrict__ cand, int dc, long m,
                      const double* __restrict__ lo, const double* __restrict__ up,
@@ -176,12 +176,11 @@ gpk_factor_scale_kernel(const KSpec ks, const double* __restrict__ cand, int dc,
 {
     const int j = blockIdx.x * 128 + (threadIdx.x & 127);
     if (j >= n) return;
-    const int ax = gpk_factor_axis(ks);
-    const double zj = gpk_env_coord(pts + (long)j * dp, ax, plo, pup);
+    const double zj = gpk_factor_coord(ks.factor, pts + (long)j * dp, plo, pup);
     for (long c = (long)blockIdx.y * 2 + (threadIdx.x >> 7); c < m; c += (long)gridDim.y * 2) {
         if (tri && (long)(j & ~127) > (c | 31)) continue;
-        const double zc = gpk_env_coord(cand + c * dc, ax, lo, up);
-        out[c * ldo + j] *= gpk_factor(ks, zc, zj);
+        const double zc = gpk_factor_coord(ks.factor, cand + c * dc, lo, up);
+        out[c * ldo + j] *= gpk_factor_value(ks.factor, zc, zj);
     }
 }
 
@@ -247,12 +246,10 @@ struct FinishArgs {
     long m;                 // valid candidates in this chunk
     long base;              // global index of the chunk's first candidate
     double kss;             // k(x*, x*) = amplitude (stationary kernels)
-    // environment factor: k(x*, x*) = kss * (c0 + c1 z*^2), z* from the chunk's candidates (env_cand NULL: none)
-    int env_axis; double env_c0, env_c1;
-    const double* env_cand; int env_dc; const double* env_lo; const double* env_up;
-    // task factor instead (task_n > 0): k(x*, x*) = kss * task_diag[t*], t* = column env_axis of env_cand, NaN when t*
-    // is not a task
-    int task_n; double task_diag[GPK_MAX_TASKS];
+    // the kernel's factor: k(x*, x*) = kss * gpk_factor_value(z*, z*), z* from the chunk's candidates (row-major raw
+    // inputs, cand_dc columns, bounds lo / up)
+    KFactor factor;
+    const double* cand; int cand_dc; const double* lo; const double* up;
     double mean;            // GP constant mean
     int norm_out; double y_mean, y_std;
     int acq_kind; double eta, par;
@@ -273,14 +270,9 @@ __global__ void __launch_bounds__(256) gpk_finish_kernel(const FinishArgs f)
             mu += f.part_mu[(long)p * f.ldpart + c];
         }
         double kss = f.kss;
-        if (f.env_cand != nullptr) {
-            const double z = gpk_env_coord(f.env_cand + c * f.env_dc, f.env_axis, f.env_lo, f.env_up);
-            if (f.task_n > 0) {
-                const int t = gpk_task_index(z, f.task_n);
-                kss *= t >= 0 ? f.task_diag[t] : __longlong_as_double(0x7ff8000000000000LL);
-            } else {
-                kss *= gpk_env(f.env_c0, f.env_c1, z, z);
-            }
+        if (f.factor.kind != GPK_FACTOR_NONE) {
+            const double z = gpk_factor_coord(f.factor, f.cand + c * f.cand_dc, f.lo, f.up);
+            kss *= gpk_factor_value(f.factor, z, z);
         }
         double var = kss - ssq;
         mu += f.mean;
@@ -396,10 +388,10 @@ __global__ void gpk_cov_finish_kernel(double* __restrict__ cov, long ld, long m,
 // With the environment factor k = amp R (c0 + c1 z z'), nv = n_terms + 4: [sum w k, sum_t ..., log_a, log_b, trace A],
 //   dk/d log_a = amp R c0,   dk/d log_b = amp R c1 z z'
 // With the task factor k = amp R K_t[t_i][t_j] (training tasks are valid indices) the sums above use that k, nv stays
-// n_terms + 2; the task entries come from gpk_grad_task_kernel.  TASK = false compiles the task code out: a kernel
-// without the task factor runs the code it ran before the factor existed.
+// n_terms + 2; the task entries come from gpk_grad_task_kernel.  FK = the kernel's factor kind (GPK_FACTOR_*): each
+// instance compiles the other factors' code out.
 // ---------------------------------------------------------------------------------------
-template <bool TASK>
+template <int FK>
 __global__ void __launch_bounds__(256)
 gpk_grad_trace_kernel(const KSpec ks, const double* __restrict__ Xt, long ldx, int n,
                       const double* __restrict__ Xrow, int dc,
@@ -410,9 +402,8 @@ gpk_grad_trace_kernel(const KSpec ks, const double* __restrict__ Xt, long ldx, i
     __shared__ double szc[32];
     __shared__ double red[8];
     const int tid = threadIdx.x;
-    const bool env = !TASK && ks.env_axis >= 0;
-    const int nt = ks.n_terms, nv = nt + (env ? 4 : 2);
-    const int fax = TASK ? ks.task_axis : ks.env_axis;
+    const int nt = ks.n_terms, nv = nt + (FK == GPK_FACTOR_ENV ? 4 : 2);
+    const int fax = ks.factor.axis;
     const long bid = (long)blockIdx.y * gridDim.x + blockIdx.x;
     const int j = blockIdx.x * 128 + (tid & 127);
     const long c0 = (long)blockIdx.y * 32;
@@ -425,7 +416,7 @@ gpk_grad_trace_kernel(const KSpec ks, const double* __restrict__ Xt, long ldx, i
         long ci = c0 + c;
         sc[c][t] = (ci < n) ? Xrow[ci * dc + ks.axis[t]] : 0.0;
     }
-    if ((env || TASK) && tid < 32) szc[tid] = (c0 + tid < n) ? Xrow[(c0 + tid) * dc + fax] : 0.0;
+    if (FK != GPK_FACTOR_NONE && tid < 32) szc[tid] = (c0 + tid < n) ? Xrow[(c0 + tid) * dc + fax] : 0.0;
     __syncthreads();
 
     const int cg = (tid >> 7) * 16;
@@ -433,7 +424,7 @@ gpk_grad_trace_kernel(const KSpec ks, const double* __restrict__ Xt, long ldx, i
     double gl[GPK_MAX_TERMS];                                // per-term partial sums (local memory)
     for (int t = 0; t < nt; ++t) gl[t] = 0.0;
     double gamp = 0.0, gtr = 0.0, genva = 0.0, genvb = 0.0;
-    const double zj = ((env || TASK) && jv) ? Xt[(long)fax * ldx + j] : 0.0;
+    const double zj = (FK != GPK_FACTOR_NONE && jv) ? Xt[(long)fax * ldx + j] : 0.0;
 
     double r2[16], wk[16];
 #pragma unroll
@@ -460,13 +451,13 @@ gpk_grad_trace_kernel(const KSpec ks, const double* __restrict__ Xt, long ldx, i
             if (i == j) { gtr += a; w = a; } else w = 2.0 * a;
         }
         wk[c] = w * ks.amp * wk[c];
-        if (env) {
+        if constexpr (FK == GPK_FACTOR_ENV) {
             const double zc = szc[cg + c];
-            genva = fma(wk[c], ks.env_c0, genva);
-            genvb = fma(wk[c], ks.env_c1 * zc * zj, genvb);
-            wk[c] *= gpk_env(ks.env_c0, ks.env_c1, zc, zj);
-        } else if (TASK) {
-            wk[c] *= ks.task_K[(int)szc[cg + c] * ks.n_tasks + (int)zj];
+            genva = fma(wk[c], ks.factor.c0, genva);
+            genvb = fma(wk[c], ks.factor.c1 * zc * zj, genvb);
+            wk[c] *= gpk_env(ks.factor.c0, ks.factor.c1, zc, zj);
+        } else if constexpr (FK == GPK_FACTOR_TASK) {
+            wk[c] *= ks.factor.K[(int)szc[cg + c] * ks.factor.n_tasks + (int)zj];
         }
         gamp += wk[c];
     }
@@ -527,7 +518,7 @@ gpk_grad_task_kernel(const KSpec ks, const double* __restrict__ Xt, long ldx, in
                      double* __restrict__ part)
 {
     __shared__ double red[8];
-    const int tid = threadIdx.x, nT = ks.n_tasks, nv = nT * nT;
+    const int tid = threadIdx.x, nT = ks.factor.n_tasks, nv = nT * nT;
     const long bid = (long)blockIdx.y * gridDim.x + blockIdx.x;
     const int j = blockIdx.x * 128 + (tid & 127);
     const long c0 = (long)blockIdx.y * 32;
@@ -536,7 +527,7 @@ gpk_grad_task_kernel(const KSpec ks, const double* __restrict__ Xt, long ldx, in
         return;
     }
     const bool jv = j < n;
-    const double* tx = Xt + (long)ks.task_axis * ldx;
+    const double* tx = Xt + (long)ks.factor.axis * ldx;
     const int tj = jv ? (int)tx[j] : 0;
     double g[GPK_MAX_TASKS];                                 // G_{a, t_j}: this thread's column task is t_j
     for (int a = 0; a < nT; ++a) g[a] = 0.0;
@@ -682,9 +673,11 @@ __global__ void gpk_candidates_kernel(unsigned long long seed, long first, long 
 // With the environment factor k = amp R (c0 + c1 z* z_j): the terms above use that k, the environment axis gains
 //   d k / d z* = amp R c1 z_j,   and  d var / d z* gains d k(x*, x*) / d z* = 2 amp c1 z*.
 // With the task factor k = amp R K_t[t*][t_j]: the terms above use that k; the task axis and k(x*, x*) = amp K_t[t*][t*]
-// have zero derivative (the task index is piecewise constant).  TASK = false compiles the task code out.
+// have zero derivative (the task index is piecewise constant).  FK = GPK_FACTOR_TASK or GPK_FACTOR_ENV: each instance
+// compiles the other factor's code out.  A kernel without a factor runs the ENV instance, which tests the kind at run
+// time: an instance of its own compiles to 8 / 8 bytes of spills where this one has none (sm_90a, CUDA 12.9).
 // ---------------------------------------------------------------------------------------
-template <bool TASK>
+template <int FK>
 __global__ void __launch_bounds__(256)
 gpk_predict_grad_kernel(const KSpec ks, const double* __restrict__ Xt, long ldx, int n,
                         const double* __restrict__ cand, int dc,
@@ -696,8 +689,8 @@ gpk_predict_grad_kernel(const KSpec ks, const double* __restrict__ Xt, long ldx,
     __shared__ double red[16];
     const int tid = threadIdx.x, nt = ks.n_terms;
     const long c = blockIdx.x;
-    const bool env = !TASK && ks.env_axis >= 0;
-    const double zs = env ? gpk_env_coord(cand + c * dc, ks.env_axis, lower, upper) : 0.0;
+    const bool fac = FK == GPK_FACTOR_TASK || ks.factor.kind == GPK_FACTOR_ENV;
+    const double zs = fac ? gpk_factor_coord<FK>(ks.factor, cand + c * dc, lower, upper) : 0.0;
     double gem = 0.0, gev = 0.0;                                        // environment-axis sums
     for (int t = tid; t < nt; t += 256) {
         const int a = ks.axis[t];
@@ -716,14 +709,14 @@ gpk_predict_grad_kernel(const KSpec ks, const double* __restrict__ Xt, long ldx,
             r2 = fma(d * d, ks.inv_metric[t], r2);
             if (ks.last[t]) { k *= gpk_radial(ks.family, r2); r2 = 0.0; }
         }
-        if (env) {
-            const double zj = Xt[(long)ks.env_axis * ldx + j];
-            const double dkz = k * gpk_env_dz(ks.env_c1, zj);
-            gem = fma(alpha[j], dkz, gem);
-            gev = fma(-2.0 * Wt[c * ldw + j], dkz, gev);
-            k *= gpk_env(ks.env_c0, ks.env_c1, zs, zj);
-        } else if (TASK) {                                              // unscaled: the task factor refuses bounds
-            k *= gpk_task(ks, cand[c * dc + ks.task_axis], Xt[(long)ks.task_axis * ldx + j]);
+        if (fac) {
+            const double zj = Xt[(long)ks.factor.axis * ldx + j];
+            if constexpr (FK == GPK_FACTOR_ENV) {
+                const double dkz = k * gpk_env_dz(ks.factor.c1, zj);
+                gem = fma(alpha[j], dkz, gem);
+                gev = fma(-2.0 * Wt[c * ldw + j], dkz, gev);
+            }
+            k *= gpk_factor_value<FK>(ks.factor, zs, zj);
         }
         const double ka = k * alpha[j], kw = -2.0 * k * Wt[c * ldw + j];
         int t0 = 0;
@@ -766,7 +759,7 @@ gpk_predict_grad_kernel(const KSpec ks, const double* __restrict__ Xt, long ldx,
         }
         __syncthreads();
     }
-    if (env) {
+    if (FK == GPK_FACTOR_ENV && fac) {
 #pragma unroll
         for (int pass = 0; pass < 2; ++pass) {
             double x = pass == 0 ? gem : gev;
@@ -778,8 +771,8 @@ gpk_predict_grad_kernel(const KSpec ks, const double* __restrict__ Xt, long ldx,
         if (tid == 0) {
             double sm = 0.0, sv = 0.0;
             for (int w = 0; w < 8; ++w) { sm += red[w]; sv += red[8 + w]; }
-            sv += 2.0 * ks.amp * ks.env_c1 * zs;                       // d k(x*, x*) / d z*
-            const int a = ks.env_axis;
+            sv += 2.0 * ks.amp * ks.factor.c1 * zs;                    // d k(x*, x*) / d z*
+            const int a = ks.factor.axis;
             double scale = 1.0;
             if (lower != nullptr) scale = 1.0 / (upper[a] - lower[a]);
             if (norm_out) { sm *= y_std; sv *= y_std * y_std; }

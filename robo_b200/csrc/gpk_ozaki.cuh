@@ -358,8 +358,7 @@ gpk_oz_vargemm_kernel(const __grid_constant__ CUtensorMap mapP, const __grid_con
 // + split kernel (8 B read, 8 B written) + mean dot (8 B read) by 8 B written per element.
 // DIGITS = false compiles the digit stores out (Kq unused): the mean-only prediction (gpk_predict_mean) writes nothing
 // but part_mu, with the same arithmetic and reduction order, so its mean is bit-identical to the int8 scoring pass's.
-// Only that instance applies the single-column factor (environment or task, gpk_factor; z_j from the row-major training
-// inputs Xenv): the digit split assumes 0 < k <= amp, so scoring with a factor takes the fp64 contraction.
+// Only that instance applies the kernel's factor (gpk_factor_value; z_j from the row-major training inputs Xenv): the digit split assumes 0 < k <= amp, so scoring with a factor takes the fp64 contraction.
 // ---------------------------------------------------------------------------------------
 template <int CC, bool DIGITS = true>
 __global__ void __launch_bounds__(256, CC == 8 ? 2 : 4)
@@ -445,11 +444,10 @@ gpk_cov_oz_kernel(const __grid_constant__ CUtensorMap mapX, const KSpec ks, int 
         const bool cv = ci < m;
         double k0 = (cv && v0) ? ks.amp * pr[c][0] : 0.0;
         double k1 = (cv && v1) ? ks.amp * pr[c][1] : 0.0;
-        if (!DIGITS && gpk_factor_axis(ks) >= 0 && cv) {
-            const int ax = gpk_factor_axis(ks);
-            const double zc = gpk_env_coord(cand + ci * dc, ax, lower, upper);
-            if (v0) k0 *= gpk_factor(ks, zc, Xenv[(long)j0 * dc + ax]);
-            if (v1) k1 *= gpk_factor(ks, zc, Xenv[(long)(j0 + 1) * dc + ax]);
+        if (!DIGITS && ks.factor.kind != GPK_FACTOR_NONE && cv) {
+            const double zc = gpk_factor_coord(ks.factor, cand + ci * dc, lower, upper);
+            if (v0) k0 *= gpk_factor_value(ks.factor, zc, Xenv[(long)j0 * dc + ks.factor.axis]);
+            if (v1) k1 *= gpk_factor_value(ks.factor, zc, Xenv[(long)(j0 + 1) * dc + ks.factor.axis]);
         }
         if (DIGITS) {
             // digits: two adjacent int8 per slice

@@ -15,8 +15,16 @@ george adds yerr^2 + exp(white_noise) to the diagonal, white_noise = log(1.25e-1
 import numpy as np
 
 from . import _lib
+from .kernels import load_kernel
 
 TINY = 1.25e-12
+
+
+def _fit_signature(f, diag_add):
+    """What a factorisation depends on besides the data: the flattened kernel f and the diagonal term."""
+    return (int(f["family"]), float(f["log_amp"]), tuple(int(a) for a in f["axis"]),
+            tuple(int(g) for g in f["group"]), tuple(float(v) for v in np.asarray(f["log_metric"]).ravel()), diag_add,
+            f["env"], f["task"])
 
 
 class DeviceGP(object):
@@ -116,9 +124,7 @@ class DeviceGP(object):
         self._yerr = float(yerr)
         yerr_tot = np.sqrt(np.float64(self._yerr) ** 2 + np.exp(self.white_noise))
         diag_add = float(yerr_tot ** 2)
-        sig = (int(f["family"]), float(f["log_amp"]), tuple(int(a) for a in f["axis"]),
-               tuple(int(g) for g in f["group"]), tuple(float(v) for v in np.asarray(f["log_metric"]).ravel()), diag_add,
-               f["env"], f["task"])
+        sig = _fit_signature(f, diag_add)
         self.computed = False
         # Rows appended to an already factorised training set with the same kernel and noise (BaseModel.update /
         # train(do_optimize=False) inside the solver loop): only the last block row of the factor changes.
@@ -141,11 +147,7 @@ class DeviceGP(object):
             h.set_data(self._x, self._y)
             self._data_dirty = False
         self._push_cfg()
-        h.set_kernel(f["family"], f["log_amp"], f["axis"], f["group"], f["log_metric"])
-        if f["env"] is not None:
-            h.set_env_factor(*f["env"])
-        if f["task"] is not None:
-            h.set_task_factor(*f["task"])
+        load_kernel(h, f)
         self.log_determinant, self._ll = h.fit(diag_add, self.mean)
         self._fit_x = self._x.copy()
         self._fit_sig = sig
@@ -169,21 +171,14 @@ class DeviceGP(object):
         self._yerr = float(yerr)
         yerr_tot = np.sqrt(np.float64(self._yerr) ** 2 + np.exp(self.white_noise))
         diag_add = float(yerr_tot ** 2)
-        self._pending_sig = (int(f["family"]), float(f["log_amp"]), tuple(int(a) for a in f["axis"]),
-                             tuple(int(g) for g in f["group"]),
-                             tuple(float(v) for v in np.asarray(f["log_metric"]).ravel()), diag_add, f["env"],
-                             f["task"])
+        self._pending_sig = _fit_signature(f, diag_add)
         self.computed = False
         self._fit_x = None
         if self._data_dirty:
             h.set_data(self._x, self._y)
             self._data_dirty = False
         self._push_cfg()
-        h.set_kernel(f["family"], f["log_amp"], f["axis"], f["group"], f["log_metric"])
-        if f["env"] is not None:
-            h.set_env_factor(*f["env"])
-        if f["task"] is not None:
-            h.set_task_factor(*f["task"])
+        load_kernel(h, f)
         h.fit_begin(diag_add, self.mean)
 
     def compute_end(self):
@@ -222,12 +217,8 @@ class DeviceGP(object):
             raise RuntimeError("You need to compute the model first")
         f = self.kernel.flatten()
         nt = len(f["axis"])
-        if f["env"] is not None:
-            g = self.handle.nll_grad(noise_var, nt, env=True)
-        elif f["task"] is not None:
-            g = self.handle.nll_grad(noise_var, nt, n_kt=len(f["task"][2]))
-        else:
-            g = self.handle.nll_grad(noise_var, nt)
+        g = self.handle.nll_grad(noise_var, nt, env=f["env"] is not None,
+                                 n_kt=0 if f["task"] is None else len(f["task"][2]))
         out = np.empty(len(f["slots"]) + 1)
         for p, (kind, terms) in enumerate(f["slots"]):
             if kind == "amp":

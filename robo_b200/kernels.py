@@ -113,14 +113,18 @@ class Kernel(object):
     def get_value(self, x1, x2=None, device=0):
         x1 = self._parse(x1)
         x2 = x1 if x2 is None else self._parse(x2)
-        f = self.flatten()
         h = _lib.moments_handle(device)
-        h.set_kernel(f["family"], f["log_amp"], f["axis"], f["group"], f["log_metric"])
-        if f["env"] is not None:
-            h.set_env_factor(*f["env"])
-        if f["task"] is not None:
-            h.set_task_factor(*f["task"])
+        load_kernel(h, self.flatten())
         return h.kernel_matrix(x1, x2)
+
+
+def load_kernel(h, f):
+    """Loads a flattened kernel (Kernel.flatten) onto a handle: gpk_set_kernel, then its environment or task factor."""
+    h.set_kernel(f["family"], f["log_amp"], f["axis"], f["group"], f["log_metric"])
+    if f["env"] is not None:
+        h.set_env_factor(*f["env"])
+    if f["task"] is not None:
+        h.set_task_factor(*f["task"])
 
 
 class ConstantKernel(Kernel):

@@ -21,6 +21,7 @@ import numpy as np
 
 from robo_b200 import _lib, priors
 from robo_b200.device_gp import DeviceGP, TINY
+from robo_b200.kernels import load_kernel
 from robo_b200.models.base_model import BaseModel
 from robo_b200.models.gaussian_process import GaussianProcess
 from robo_b200.util import normalization
@@ -52,12 +53,7 @@ class _LikelihoodPool(object):
                 h = self.handles[i]
                 try:                                                # :194-197: any failure of one theta is -inf for it
                     self.kernel.set_parameter_vector(theta[:-1])
-                    f = self.kernel.flatten()
-                    h.set_kernel(f["family"], f["log_amp"], f["axis"], f["group"], f["log_metric"])
-                    if f["env"] is not None:
-                        h.set_env_factor(*f["env"])
-                    if f["task"] is not None:
-                        h.set_task_factor(*f["task"])
+                    load_kernel(h, self.kernel.flatten())
                     yerr = np.sqrt(np.exp(theta[-1]))
                     diag_add = float(np.sqrt(np.float64(yerr) ** 2 + TINY) ** 2)
                     h.fit_begin(diag_add, self.mean)
@@ -227,11 +223,7 @@ class GaussianProcessMCMC(BaseModel):
             self._hyper_handle = _lib.Handle(self.device)
         h = self._hyper_handle
         h.set_data(self.X, self.y)
-        h.set_kernel(f["family"], f["log_amp"], f["axis"], f["group"], f["log_metric"])
-        if f["env"] is not None:
-            h.set_env_factor(*f["env"])
-        if f["task"] is not None:
-            h.set_task_factor(*f["task"])
+        load_kernel(h, f)
         _lib.set_hyper_model(h, f["slots"], len(f["axis"]), float(self.mean), TINY, prior_kind, prior_par, n_ls, n_lr)
 
         def run(p0, steps):
