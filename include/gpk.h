@@ -842,6 +842,43 @@ int gpk_rf_get_trees(gpk_handle* h, int* n_nodes, int* feat, double* thr, int* l
 int gpk_rf_set_trees(gpk_handle* h, int T, int total_variance, const int* n_nodes, const int* feat, const double* thr,
                      const int* left, const double* W, const double* mean, const double* var);
 
+/* ---- Bayesian neural network on the device (robo_b200/csrc/gpk_bnn.cuh) -------------------------------------------
+ * robo/models/wrapper_bohamiann.py, with the pybnn network and sampler it wraps restated (pybnn's source is not
+ * available): a D -> 50 -> 50 -> 1 tanh network with a homoscedastic log-variance, sampled by adaptive SGHMC.
+ * gpk_bnn.cuh states every step and its order; tests/bnn_model.py restates them and the device chain equals it bit for
+ * bit on the device's normals.  A handle becomes a BNN handle with gpk_bnn_set_data and stays one: the Gaussian-process,
+ * BLR and RF entry points return GPK_BAD_ARG with a message naming the model kind, and the BNN entry points refuse the
+ * other kinds.  The scoring entry points (as for an RF handle) score a trained BNN handle through its predictive pass. */
+#define GPK_BNN_MAX_D 64         /* most input dimensions */
+#define GPK_BNN_MAX_N 4096       /* most training points: the chain keeps an epoch's order (12 bytes a row) in shared
+                                    memory beside theta, its gradient and the batch's activations */
+#define GPK_BNN_MAX_BATCH 32     /* largest batch */
+/* gpk_bnn_set_data: X (n x d) and y (n) as train() receives them.  Each column of X and y is scaled to zero mean and unit
+ *   population std on the host (pybnn's normalize_input / normalize_output); the scaled copy and the statistics stay on
+ *   the handle.  Drops the samples.  GPK_BAD_ARG: n < 2, a constant column or a constant y (pybnn would divide by zero),
+ *   n > GPK_BNN_MAX_N, d > GPK_BNN_MAX_D, a non-finite entry, a handle holding another model kind.
+ * gpk_bnn_train: one fresh chain of num_steps adaptive-SGHMC steps in one launch (step size lr, friction mdecay, eps;
+ *   adaptation while the step count t <= burn_in; batches of `batch` rows), keeping theta after step s when s > burn_in
+ *   and (s - burn_in) % keep_every == 0.  The draws are Philox4x32-10 keyed by seed with `counter` in their counter: a
+ *   caller advances it once per train.  GPK_BAD_ARG: lr, mdecay or eps not finite and > 0 (eps >= 0), batch outside
+ *   1..GPK_BNN_MAX_BATCH, keep_every < 1, burn_in < 0, num_steps outside 1..2^31 - 1, no network kept.
+ * gpk_bnn_dims: n, d, the parameters per network P = 50 d + 2652 and the kept networks S (0 before a train).
+ * gpk_bnn_get_samples: the S x P kept networks, in gpk_bnn.cuh's parameter order.
+ * gpk_bnn_set_samples: S networks back onto a BNN handle that holds the training set (a pickled or copied model).
+ * gpk_bnn_get_state: the chain's final theta, momentum p and adaptation state tau, g, vhat (P each; any may be NULL).
+ * gpk_bnn_draws: Z (ns x P): the normals of steps step0 .. step0 + ns - 1 of a chain (seed, counter); step -1 holds the
+ *   initial weights' normals.  For tests that restate the chain on the device's normals.
+ * The predictive pass: m = mean_k f_k and v = mean_k (f_k - m)^2 + mean_k exp(lv_k) over the kept networks in order, then
+ * m y_std + y_mean and v y_std^2; no clip.  The acquisition closed form of gpk_acq_moments follows. */
+int gpk_bnn_set_data(gpk_handle* h, const double* X, const double* y, int n, int d);
+int gpk_bnn_train(gpk_handle* h, unsigned long long seed, unsigned counter, double lr, double mdecay, double eps,
+                  long burn_in, long num_steps, long keep_every, int batch);
+int gpk_bnn_dims(gpk_handle* h, int* n, int* d, int* P, int* S);
+int gpk_bnn_get_samples(gpk_handle* h, double* samples);
+int gpk_bnn_set_samples(gpk_handle* h, int S, const double* samples);
+int gpk_bnn_get_state(gpk_handle* h, double* theta, double* p, double* tau, double* g, double* vhat);
+int gpk_bnn_draws(gpk_handle* h, unsigned long long seed, unsigned counter, int step0, int ns, double* Z);
+
 /* kernel.get_value(X1, X2) (test/test_models/test_gaussian_process.py:44-46) with the
  * handle's current kernel; no input scaling.  out is (n1, n2) row-major. */
 int gpk_kernel_matrix(gpk_handle* h, const double* X1, long n1, const double* X2, long n2,

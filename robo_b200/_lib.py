@@ -31,6 +31,7 @@ HYPER_MAX_DIM = 96                             # GPK_HYPER_MAX_DIM: most entries
 BLR_LINEAR, BLR_QUADRATIC, BLR_NONE = range(3)  # gpk_blr_basis: the features of a BayesianLinearRegression handle
 BLR_MAX_F = 64                                 # GPK_BLR_MAX_F: most features of a BayesianLinearRegression handle
 RF_MAX_N, RF_MAX_D, RF_MAX_T = 16384, 64, 512  # GPK_RF_MAX_N / GPK_RF_MAX_D / GPK_RF_MAX_T: the largest forest
+BNN_MAX_N, BNN_MAX_D, BNN_MAX_BATCH = 4096, 64, 32   # GPK_BNN_MAX_N / GPK_BNN_MAX_D / GPK_BNN_MAX_BATCH
 CMA_MAX_D, CMA_MAX_LAMBDA, CMA_HIST = 64, 2048, 160   # GPK_CMA_MAX_D / GPK_CMA_MAX_LAMBDA / GPK_CMA_HIST
 CMA_C_W = 20                                   # GPK_CMA_C_W: where a run's weights start in its constant row
 CMA_NCONST = CMA_C_W + CMA_MAX_LAMBDA // 2     # GPK_CMA_NCONST: doubles per run in the constant table
@@ -169,6 +170,14 @@ _SIGNATURES = {
     "gpk_rf_dims": [_vp, _ip, _ip, _ip, _ip],
     "gpk_rf_get_trees": [_vp, _ip, _ip, _dp, _ip, _dp, _dp, _dp],
     "gpk_rf_set_trees": [_vp, C.c_int, C.c_int, _ip, _ip, _dp, _ip, _dp, _dp, _dp],
+    "gpk_bnn_set_data": [_vp, _dp, _dp, C.c_int, C.c_int],
+    "gpk_bnn_train": [_vp, C.c_ulonglong, C.c_uint, C.c_double, C.c_double, C.c_double, C.c_long, C.c_long, C.c_long,
+                      C.c_int],
+    "gpk_bnn_dims": [_vp, _ip, _ip, _ip, _ip],
+    "gpk_bnn_get_samples": [_vp, _dp],
+    "gpk_bnn_set_samples": [_vp, C.c_int, _dp],
+    "gpk_bnn_get_state": [_vp, _dp, _dp, _dp, _dp, _dp],
+    "gpk_bnn_draws": [_vp, C.c_ulonglong, C.c_uint, C.c_int, C.c_int, _dp],
     "gpk_get_timings": [_vp, _dp],
     "gpk_get_diag_profile": [_vp, C.POINTER(C.c_longlong)],
 }
@@ -1399,6 +1408,69 @@ def rf_set_trees(handle, trees, total_variance):
     ptrs = [arr[k].ctypes.data_as(_ip if arr[k].dtype == np.int32 else _dp) for k in RF_FIELDS]
     handle._check(handle.lib.gpk_rf_set_trees(handle._h, nn.size, int(bool(total_variance)), nn.ctypes.data_as(_ip),
                                               *ptrs))
+
+
+def bnn_params(n_dims):
+    """P, the parameters of one network of a BNN handle on n_dims inputs."""
+    return 50 * int(n_dims) + 2652
+
+
+def bnn_set_data(handle, X, y):
+    """gpk_bnn_set_data: the training set on the handle (normalised there), which becomes a BNN handle."""
+    X, y = f64(X), f64(y).ravel()
+    if X.ndim != 2 or X.shape[0] != y.size:
+        raise ValueError("bnn_set_data: X must be (n, d) and y (n,)")
+    n, d = X.shape
+    handle._check(handle.lib.gpk_bnn_set_data(handle._h, _as_dp(X), _as_dp(y), n, d))
+
+
+def bnn_train(handle, seed, counter, lr, mdecay, eps, burn_in, num_steps, keep_every, batch):
+    """gpk_bnn_train: one adaptive-SGHMC chain in one launch (draws keyed by seed and the train counter)."""
+    handle._check(handle.lib.gpk_bnn_train(handle._h, int(seed) & 0xFFFFFFFFFFFFFFFF, int(counter) & 0xFFFFFFFF,
+                                           float(lr), float(mdecay), float(eps), int(burn_in), int(num_steps),
+                                           int(keep_every), int(batch)))
+
+
+def bnn_dims(handle):
+    """gpk_bnn_dims -> (n, d, P, S)."""
+    n, d, P, S = C.c_int(), C.c_int(), C.c_int(), C.c_int()
+    handle._check(handle.lib.gpk_bnn_dims(handle._h, C.byref(n), C.byref(d), C.byref(P), C.byref(S)))
+    return n.value, d.value, P.value, S.value
+
+
+def bnn_samples(handle):
+    """gpk_bnn_get_samples: the (S, P) kept networks."""
+    _, _, P, S = bnn_dims(handle)
+    if S == 0:
+        raise RuntimeError("bnn_samples: model is not trained (gpk_bnn_train)")
+    out = np.empty((S, P))
+    handle._check(handle.lib.gpk_bnn_get_samples(handle._h, _as_dp(out)))
+    return out
+
+
+def bnn_set_samples(handle, samples):
+    """gpk_bnn_set_samples: the (S, P) networks of bnn_samples back onto a handle that holds the same training set."""
+    Z = f64(samples)
+    if Z.ndim != 2 or Z.shape[1] != bnn_dims(handle)[2]:
+        raise ValueError("bnn_set_samples: samples must be (S, P)")
+    handle._check(handle.lib.gpk_bnn_set_samples(handle._h, Z.shape[0], _as_dp(Z)))
+
+
+def bnn_state(handle):
+    """gpk_bnn_get_state -> dict(theta, p, tau, g, vhat) of the last chain (P each)."""
+    P = bnn_dims(handle)[2]
+    out = {k: np.empty(P) for k in ("theta", "p", "tau", "g", "vhat")}
+    handle._check(handle.lib.gpk_bnn_get_state(handle._h, *[_as_dp(out[k]) for k in ("theta", "p", "tau", "g", "vhat")]))
+    return out
+
+
+def bnn_draws(handle, seed, counter, step0, ns):
+    """gpk_bnn_draws: the (ns, P) normals of chain steps step0 .. step0 + ns - 1 (step -1: the initial weights)."""
+    P = bnn_dims(handle)[2]
+    Z = np.empty((int(ns), P))
+    handle._check(handle.lib.gpk_bnn_draws(handle._h, int(seed) & 0xFFFFFFFFFFFFFFFF, int(counter) & 0xFFFFFFFF,
+                                           int(step0), int(ns), _as_dp(Z)))
+    return Z
 
 
 _moments_handle = {}

@@ -35,6 +35,7 @@
 #include "gpk_hyper.cuh"
 #include "gpk_blr.cuh"
 #include "gpk_rf.cuh"
+#include "gpk_bnn.cuh"
 
 namespace {
 
@@ -181,6 +182,14 @@ struct gpk_handle {
     bool rf = false, rf_fitted = false;
     int rf_T = 0, rf_total = 0;
     DevBuf rf_data, rf_work, rf_nodes, rf_bb;
+    // Bayesian neural network (gpk_bnn.cuh): set once by gpk_bnn_set_data, after which the handle serves the BNN entry
+    // points and the scoring ones only.  bnn_data: the scaled X (n x d), y (n), the input mean and std (d each);
+    // bnn_samples: the kept networks (S x P); bnn_state: the chain's final theta, p, tau, g, vhat (P each); bnn_bb: the
+    // block arg-max pairs
+    bool bnn = false;
+    int bnn_P = 0, bnn_S = 0;
+    double bnn_ymean = 0.0, bnn_ystd = 1.0;
+    DevBuf bnn_data, bnn_samples, bnn_state, bnn_bb;
     int es_nb = 0, es_np = 0;
     double es_sn2 = 0.0, es_H = 0.0;
     long es_linv_serial = -1;       // linv_serial U was built for (-1: no update yet)
@@ -768,10 +777,13 @@ __global__ void gpk_resid_kernel(const double* __restrict__ y, double mean, int 
 // ... and with a random-forest handle
 #define RF_REFUSAL "the handle holds a random forest (gpk_rf_set_data); this entry point serves Gaussian-process " \
                    "handles only"
+// ... and with a Bayesian-neural-network handle
+#define BNN_REFUSAL "the handle holds a Bayesian neural network (gpk_bnn_set_data); this entry point serves " \
+                    "Gaussian-process handles only"
 
 // the refusal of a Gaussian-process entry point for the handle's model kind, or nullptr for a Gaussian-process handle
 const char* gp_refusal(const gpk_handle* h) {
-    return h->blr ? BLR_REFUSAL : h->rf ? RF_REFUSAL : nullptr;
+    return h->blr ? BLR_REFUSAL : h->rf ? RF_REFUSAL : h->bnn ? BNN_REFUSAL : nullptr;
 }
 
 int require(gpk_handle* h, bool data, bool spec, bool fitted) {
@@ -791,6 +803,10 @@ int require_model(gpk_handle* h) {
     }
     if (h && h->rf) {
         if (!h->rf_fitted) { set_err(h, "model is not fitted (gpk_rf_fit)"); return GPK_NOT_FITTED; }
+        return GPK_OK;
+    }
+    if (h && h->bnn) {
+        if (h->bnn_S < 1) { set_err(h, "model is not trained (gpk_bnn_train)"); return GPK_NOT_FITTED; }
         return GPK_OK;
     }
     return require(h, true, true, true);
@@ -925,6 +941,9 @@ int blr_score(gpk_handle* h, const double* dX, long m, int kind, double eta, dou
 int rf_score(gpk_handle* h, const double* dX, long m, int kind, double eta, double par, double* d_out, double* d_mu,
              double* d_var, BestPair* d_best, unsigned long long* d_nneg, long index_offset, bool reset, long global_base,
              Feeder* feeder);
+int bnn_score(gpk_handle* h, const double* dX, long m, int kind, double eta, double par, double* d_out, double* d_mu,
+              double* d_var, BestPair* d_best, unsigned long long* d_nneg, long index_offset, bool reset, long global_base,
+              Feeder* feeder);
 
 int score_dev(gpk_handle* h, const double* dX, long m, int kind, double eta, double par, double* d_out,
               double* d_mu, double* d_var, BestPair* d_best, unsigned long long* d_nneg,
@@ -935,6 +954,9 @@ int score_dev(gpk_handle* h, const double* dX, long m, int kind, double eta, dou
     if (h->rf)
         return rf_score(h, dX, m, kind, eta, par, d_out, d_mu, d_var, d_best, d_nneg, index_offset, reset, global_base,
                         feeder);
+    if (h->bnn)
+        return bnn_score(h, dX, m, kind, eta, par, d_out, d_mu, d_var, d_best, d_nneg, index_offset, reset, global_base,
+                         feeder);
     int rc = build_linv(h);
     if (rc) return rc;
     const long NP = h->NP;
@@ -1329,6 +1351,8 @@ int blr_ready(gpk_handle* h, const char* who) {
     if (!h) return GPK_BAD_ARG;
     if (h->rf) BAD("%s: the handle holds a random forest (gpk_rf_set_data); use a new handle for Bayesian linear "
                    "regression", who);
+    if (h->bnn) BAD("%s: the handle holds a Bayesian neural network (gpk_bnn_set_data); use a new handle for Bayesian "
+                    "linear regression", who);
     if (!h->blr) BAD("%s: gpk_blr_set_data has not been called", who);
     CK(cudaSetDevice(h->device));
     const int sm_eval = (int)(gpk_blr_smem_doubles(h->blr_F) * 8);
@@ -1405,6 +1429,8 @@ int rf_ready(gpk_handle* h, const char* who) {
     if (!h) return GPK_BAD_ARG;
     if (h->blr) BAD("%s: the handle holds a Bayesian linear regression model (gpk_blr_set_data); use a new handle for a "
                     "random forest", who);
+    if (h->bnn) BAD("%s: the handle holds a Bayesian neural network (gpk_bnn_set_data); use a new handle for a random "
+                    "forest", who);
     if (!h->rf) BAD("%s: gpk_rf_set_data has not been called", who);
     CK(cudaSetDevice(h->device));
     return GPK_OK;
@@ -1451,6 +1477,68 @@ int rf_score(gpk_handle* h, const double* dX, long m, int kind, double eta, doub
         CKL();
         if (kind != GPK_ACQ_NONE) {
             gpk_argmax_final_kernel<<<1, 256, 0, h->stream>>>(ptr<BestPair>(h->rf_bb), (int)nblk, d_best);
+            CKL();
+        }
+    }
+    return GPK_OK;
+}
+
+// the layout of h->bnn_data: the scaled X (n x d), the scaled y (n), the input mean and std (d each)
+inline double* bnn_X(gpk_handle* h) { return ptr<double>(h->bnn_data); }
+inline double* bnn_y(gpk_handle* h) { return bnn_X(h) + (size_t)h->n * h->d; }
+inline double* bnn_xm(gpk_handle* h) { return bnn_y(h) + h->n; }
+inline double* bnn_xs(gpk_handle* h) { return bnn_xm(h) + h->d; }
+
+int bnn_ready(gpk_handle* h, const char* who) {
+    if (!h) return GPK_BAD_ARG;
+    if (h->blr) BAD("%s: the handle holds a Bayesian linear regression model (gpk_blr_set_data); use a new handle for a "
+                    "Bayesian neural network", who);
+    if (h->rf) BAD("%s: the handle holds a random forest (gpk_rf_set_data); use a new handle for a Bayesian neural "
+                   "network", who);
+    if (!h->bnn) BAD("%s: gpk_bnn_set_data has not been called", who);
+    CK(cudaSetDevice(h->device));
+    return GPK_OK;
+}
+
+// score_dev for a BNN handle: gpk_bnn_score_kernel over the m rows dX, with score_dev's outputs, offsets and running
+// arg-max
+int bnn_score(gpk_handle* h, const double* dX, long m, int kind, double eta, double par, double* d_out, double* d_mu,
+              double* d_var, BestPair* d_best, unsigned long long* d_nneg, long index_offset, bool reset, long global_base,
+              Feeder* feeder) {
+    int rc;
+    if ((rc = bnn_ready(h, "scoring"))) return rc;
+    constexpr long TILE = GPK_BNN_SCORE_THREADS * GPK_BNN_SCORE_C;
+    const long nblk = (m + TILE - 1) / TILE;
+    if ((rc = ensure(h, h->bnn_bb, (size_t)std::max(nblk, 1L) * sizeof(BestPair)))) return rc;
+    if ((rc = ensure(h, h->best, sizeof(BestPair)))) return rc;
+    if ((rc = ensure(h, h->nneg, 8))) return rc;
+    if (d_best == nullptr) d_best = ptr<BestPair>(h->best);
+    if (d_nneg == nullptr) d_nneg = ptr<unsigned long long>(h->nneg);
+    if (reset) {
+        CK(cudaMemsetAsync(d_best, 0xFF, sizeof(BestPair), h->stream));
+        CK(cudaMemsetAsync(d_nneg, 0, 8, h->stream));
+    }
+    if (feeder && (rc = feeder->ready(0, m, h->stream))) return rc;
+    BnnScoreArgs a;
+    memset(&a, 0, sizeof(a));
+    a.X = dX; a.m = m; a.D = h->d; a.P = h->bnn_P; a.S = h->bnn_S;
+    a.samples = ptr<double>(h->bnn_samples);
+    a.xm = bnn_xm(h); a.xs = bnn_xs(h);
+    a.y_mean = h->bnn_ymean; a.y_std = h->bnn_ystd;
+    a.base = global_base + index_offset;
+    a.acq_kind = kind; a.eta = eta; a.par = par;
+    a.out_mu = d_mu ? d_mu + index_offset : nullptr;
+    a.out_var = d_var ? d_var + index_offset : nullptr;
+    a.out_acq = d_out ? d_out + index_offset : nullptr;
+    a.block_best = ptr<BestPair>(h->bnn_bb);
+    a.n_negative = d_nneg;
+    if (m > 0) {
+        const size_t smem = (size_t)gpk_bnn_score_smem(h->d);
+        CK(cudaFuncSetAttribute(gpk_bnn_score_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        gpk_bnn_score_kernel<<<(unsigned)nblk, GPK_BNN_SCORE_THREADS, smem, h->stream>>>(a);
+        CKL();
+        if (kind != GPK_ACQ_NONE) {
+            gpk_argmax_final_kernel<<<1, 256, 0, h->stream>>>(ptr<BestPair>(h->bnn_bb), (int)nblk, d_best);
             CKL();
         }
     }
@@ -1515,7 +1603,8 @@ int gpk_destroy(gpk_handle* h) {
                       &h->multi_cand, &h->multi_A, &h->multi_B, &h->multi_out, &h->multi_bb, &h->gather, &h->best_global,
                       &h->de_pop, &h->de_trial, &h->de_param, &h->de_E, &h->de_small, &h->de_sort, &h->lb_buf, &h->cma_buf, &h->dir_buf, &h->ep_buf, &h->es_state, &h->es_U, &h->es_work, &h->es_in, &h->mc_state, &h->mc_buf, &h->mc_stat, &h->fab_in, &h->rs_buf, &h->hy_buf,
                       &h->blr_data, &h->blr_post, &h->blr_work, &h->blr_bb,
-                      &h->rf_data, &h->rf_work, &h->rf_nodes, &h->rf_bb};
+                      &h->rf_data, &h->rf_work, &h->rf_nodes, &h->rf_bb,
+                      &h->bnn_data, &h->bnn_samples, &h->bnn_state, &h->bnn_bb};
     for (DevBuf* b : bufs)
         if (b->p) cudaFree(b->p);
     if (h->ev_ok)
@@ -2701,6 +2790,8 @@ int gpk_blr_set_data(gpk_handle* h, const double* X, const double* y, int n, int
     const char* who = "gpk_blr_set_data";
     if (h->rf) BAD("%s: the handle holds a random forest (gpk_rf_set_data); use a new handle for Bayesian linear "
                    "regression", who);
+    if (h->bnn) BAD("%s: the handle holds a Bayesian neural network (gpk_bnn_set_data); use a new handle for Bayesian "
+                    "linear regression", who);
     if (!h->blr && (h->has_data || h->has_spec))
         BAD("%s: the handle holds a Gaussian-process model; use a new handle for Bayesian linear regression", who);
     if (!X || !y || !prior_par || n <= 0 || d <= 0) BAD("%s: need X, y, prior_par, n > 0, d > 0", who);
@@ -2843,6 +2934,8 @@ int gpk_rf_set_data(gpk_handle* h, const double* X, const double* y, int n, int 
     const char* who = "gpk_rf_set_data";
     if (h->blr) BAD("%s: the handle holds a Bayesian linear regression model (gpk_blr_set_data); use a new handle for a "
                     "random forest", who);
+    if (h->bnn) BAD("%s: the handle holds a Bayesian neural network (gpk_bnn_set_data); use a new handle for a random "
+                    "forest", who);
     if (!h->rf && (h->has_data || h->has_spec))
         BAD("%s: the handle holds a Gaussian-process model; use a new handle for a random forest", who);
     if (!X || !y || n <= 0 || d <= 0) BAD("%s: need X, y, n > 0, d > 0", who);
@@ -2980,6 +3073,166 @@ int gpk_rf_set_trees(gpk_handle* h, int T, int total_variance, const int* n_node
     h->rf_T = T;
     h->rf_total = total_variance ? 1 : 0;
     h->rf_fitted = true;
+    return GPK_OK;
+}
+
+// ---------------------------------------------------------------------------------------
+// Bayesian neural network (gpk_bnn.cuh; robo/models/wrapper_bohamiann.py)
+// ---------------------------------------------------------------------------------------
+int gpk_bnn_set_data(gpk_handle* h, const double* X, const double* y, int n, int d) {
+    if (!h) return GPK_BAD_ARG;
+    const char* who = "gpk_bnn_set_data";
+    if (h->blr) BAD("%s: the handle holds a Bayesian linear regression model (gpk_blr_set_data); use a new handle for a "
+                    "Bayesian neural network", who);
+    if (h->rf) BAD("%s: the handle holds a random forest (gpk_rf_set_data); use a new handle for a Bayesian neural "
+                   "network", who);
+    if (!h->bnn && (h->has_data || h->has_spec))
+        BAD("%s: the handle holds a Gaussian-process model; use a new handle for a Bayesian neural network", who);
+    if (!X || !y || n <= 0 || d <= 0) BAD("%s: need X, y, n > 0, d > 0", who);
+    if (n < 2) BAD("%s: need n >= 2 training points to normalise the data (n = %d)", who, n);
+    if (n > GPK_BNN_MAX_N) BAD("%s: n = %d training points exceed GPK_BNN_MAX_N = %d", who, n, GPK_BNN_MAX_N);
+    if (d > GPK_BNN_MAX_D) BAD("%s: d = %d exceeds GPK_BNN_MAX_D = %d", who, d, GPK_BNN_MAX_D);
+    for (long i = 0; i < (long)n * d; ++i)
+        if (!std::isfinite(X[i])) BAD("%s: X must be finite", who);
+    for (int i = 0; i < n; ++i)
+        if (!std::isfinite(y[i])) BAD("%s: y must be finite", who);
+    // column statistics: sums in ascending row order, population std
+    const size_t nd = (size_t)n * d;
+    std::vector<double> buf(nd + n + 2 * (size_t)d);
+    double* xs = buf.data();
+    double* ys = xs + nd;
+    double* xm = ys + n;
+    double* xsd = xm + d;
+    auto stats = [n](const double* v, long stride, double* mean, double* sd) {
+        double s = 0.0;
+        for (int i = 0; i < n; ++i) s += v[(long)i * stride];
+        const double m = s / (double)n;
+        double q = 0.0;
+        for (int i = 0; i < n; ++i) {
+            const double e = v[(long)i * stride] - m;
+            q += e * e;
+        }
+        *mean = m;
+        *sd = std::sqrt(q / (double)n);
+    };
+    for (int c = 0; c < d; ++c) {
+        stats(X + c, d, xm + c, xsd + c);
+        if (!(xsd[c] > 0.0)) BAD("%s: input column %d is constant; it cannot be normalised", who, c);
+        for (int i = 0; i < n; ++i) xs[(size_t)i * d + c] = (X[(size_t)i * d + c] - xm[c]) / xsd[c];
+    }
+    double ym, ysd;
+    stats(y, 1, &ym, &ysd);
+    if (!(ysd > 0.0)) BAD("%s: y is constant; it cannot be normalised", who);
+    for (int i = 0; i < n; ++i) ys[i] = (y[i] - ym) / ysd;
+    CK(cudaSetDevice(h->device));
+    int rc;
+    h->bnn = true;
+    h->bnn_S = 0;
+    h->n = n; h->d = d;
+    h->bnn_P = gpk_bnn_params(d);
+    h->bnn_ymean = ym; h->bnn_ystd = ysd;
+    if ((rc = ensure(h, h->bnn_data, buf.size() * 8))) return rc;
+    CK(cudaMemcpyAsync(bnn_X(h), buf.data(), buf.size() * 8, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaStreamSynchronize(h->stream));     // the staging vector dies here
+    return GPK_OK;
+}
+
+int gpk_bnn_train(gpk_handle* h, unsigned long long seed, unsigned counter, double lr, double mdecay, double eps,
+                  long burn_in, long num_steps, long keep_every, int batch) {
+    const char* who = "gpk_bnn_train";
+    int rc = bnn_ready(h, who);
+    if (rc) return rc;
+    if (!(std::isfinite(lr) && lr > 0.0) || !(std::isfinite(mdecay) && mdecay > 0.0) || !(std::isfinite(eps) && eps >= 0.0))
+        BAD("%s: need finite lr > 0, mdecay > 0 and eps >= 0", who);
+    if (batch < 1 || batch > GPK_BNN_MAX_BATCH) BAD("%s: need 1 <= batch <= GPK_BNN_MAX_BATCH = %d", who, GPK_BNN_MAX_BATCH);
+    if (keep_every < 1 || burn_in < 0) BAD("%s: need keep_every >= 1 and burn_in >= 0", who);
+    if (num_steps < 1 || num_steps > INT_MAX) BAD("%s: need 1 <= num_steps <= 2^31 - 1", who);
+    const long S = num_steps - 1 > burn_in ? (num_steps - 1 - burn_in) / keep_every : 0;
+    if (S < 1) BAD("%s: the chain keeps no network (num_steps = %ld, burn_in = %ld, keep_every = %ld)", who, num_steps,
+                   burn_in, keep_every);
+    const int P = h->bnn_P;
+    h->bnn_S = 0;
+    if ((rc = ensure(h, h->bnn_samples, (size_t)S * P * 8))) return rc;
+    if ((rc = ensure(h, h->bnn_state, (size_t)5 * P * 8))) return rc;
+    const size_t smem = (size_t)gpk_bnn_chain_smem(h->n, h->d, batch);
+    CK(cudaFuncSetAttribute(gpk_bnn_chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    BnnChainArgs a;
+    memset(&a, 0, sizeof(a));
+    a.X = bnn_X(h); a.y = bnn_y(h);
+    a.n = h->n; a.d = h->d; a.P = P; a.B = batch;
+    a.seed = seed; a.counter = counter;
+    a.lr = lr; a.mdecay = mdecay; a.eps = eps;
+    a.burn_in = burn_in; a.num_steps = num_steps; a.keep_every = keep_every;
+    a.samples = ptr<double>(h->bnn_samples);
+    a.state = ptr<double>(h->bnn_state);
+    gpk_bnn_chain_kernel<<<1, GPK_BNN_THREADS, smem, h->stream>>>(a);
+    CKL();
+    CK(cudaStreamSynchronize(h->stream));
+    h->bnn_S = (int)S;
+    return GPK_OK;
+}
+
+int gpk_bnn_dims(gpk_handle* h, int* n, int* d, int* P, int* S) {
+    int rc = bnn_ready(h, "gpk_bnn_dims");
+    if (rc) return rc;
+    if (n) *n = h->n;
+    if (d) *d = h->d;
+    if (P) *P = h->bnn_P;
+    if (S) *S = h->bnn_S;
+    return GPK_OK;
+}
+
+int gpk_bnn_get_samples(gpk_handle* h, double* samples) {
+    const char* who = "gpk_bnn_get_samples";
+    int rc = bnn_ready(h, who);
+    if (rc) return rc;
+    if (h->bnn_S < 1) { set_err(h, "%s: model is not trained (gpk_bnn_train)", who); return GPK_NOT_FITTED; }
+    if (!samples) BAD("%s: need the output array", who);
+    CK(cudaMemcpyAsync(samples, h->bnn_samples.p, (size_t)h->bnn_S * h->bnn_P * 8, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    return GPK_OK;
+}
+
+int gpk_bnn_set_samples(gpk_handle* h, int S, const double* samples) {
+    const char* who = "gpk_bnn_set_samples";
+    int rc = bnn_ready(h, who);
+    if (rc) return rc;
+    if (S < 1 || !samples) BAD("%s: need S >= 1 networks", who);
+    h->bnn_S = 0;
+    if ((rc = ensure(h, h->bnn_samples, (size_t)S * h->bnn_P * 8))) return rc;
+    CK(cudaMemcpyAsync(h->bnn_samples.p, samples, (size_t)S * h->bnn_P * 8, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    h->bnn_S = S;
+    return GPK_OK;
+}
+
+int gpk_bnn_get_state(gpk_handle* h, double* theta, double* p, double* tau, double* g, double* vhat) {
+    const char* who = "gpk_bnn_get_state";
+    int rc = bnn_ready(h, who);
+    if (rc) return rc;
+    if (h->bnn_S < 1 || !h->bnn_state.p) { set_err(h, "%s: no chain has run (gpk_bnn_train)", who); return GPK_NOT_FITTED; }
+    double* out[5] = {theta, p, tau, g, vhat};
+    const size_t P = h->bnn_P;
+    for (int i = 0; i < 5; ++i)
+        if (out[i]) CK(cudaMemcpyAsync(out[i], ptr<double>(h->bnn_state) + i * P, P * 8, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    return GPK_OK;
+}
+
+int gpk_bnn_draws(gpk_handle* h, unsigned long long seed, unsigned counter, int step0, int ns, double* Z) {
+    const char* who = "gpk_bnn_draws";
+    int rc = bnn_ready(h, who);
+    if (rc) return rc;
+    if (ns < 1 || !Z) BAD("%s: need ns >= 1 and an output array", who);
+    const int P = h->bnn_P;
+    const size_t bytes = (size_t)ns * P * 8;
+    if ((rc = ensure(h, h->tmp1, bytes))) return rc;
+    const long threads = (long)ns * (P / 2);
+    gpk_bnn_draws_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, h->stream>>>(seed, counter, step0, ns, P,
+                                                                                  ptr<double>(h->tmp1));
+    CKL();
+    CK(cudaMemcpyAsync(Z, h->tmp1.p, bytes, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
     return GPK_OK;
 }
 

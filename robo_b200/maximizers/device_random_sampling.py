@@ -20,6 +20,7 @@ from robo_b200.distributed import allgather_best, pack_pair, shard_bounds
 from robo_b200.maximizers.base_maximizer import BaseMaximizer
 from robo_b200.models.bayesian_linear_regression import BayesianLinearRegression
 from robo_b200.models.random_forest import RandomForest
+from robo_b200.models.wrapper_bohamiann import WrapperBohamiann
 
 
 class DeviceRandomSampling(BaseMaximizer):
@@ -39,13 +40,16 @@ class DeviceRandomSampling(BaseMaximizer):
             return self._maximize_es_cost(acq, es)
         blr = isinstance(model, BayesianLinearRegression)
         rf = isinstance(model, RandomForest)
-        if not (blr or rf) and (not hasattr(model, "gp") or not hasattr(model.gp, "handle")):
-            raise TypeError("DeviceRandomSampling needs a robo_b200 GaussianProcess, BayesianLinearRegression or "
-                            "RandomForest model")
+        bnn = isinstance(model, WrapperBohamiann)
+        if not (blr or rf or bnn) and (not hasattr(model, "gp") or not hasattr(model.gp, "handle")):
+            raise TypeError("DeviceRandomSampling needs a robo_b200 GaussianProcess, BayesianLinearRegression, "
+                            "RandomForest or WrapperBohamiann model")
         if blr and self.world > 1:
             raise ValueError("DeviceRandomSampling of a BayesianLinearRegression runs on one GPU")
         if rf and self.world > 1:
             raise ValueError("DeviceRandomSampling of a RandomForest runs on one GPU")
+        if bnn and self.world > 1:
+            raise ValueError("DeviceRandomSampling of a WrapperBohamiann runs on one GPU")
         kind = _lib.ACQ_KIND[acq.kind]
         inc_x, inc_y = model.get_incumbent()
         eta = 0.0 if acq.kind == "lcb" else float(inc_y)
@@ -54,7 +58,7 @@ class DeviceRandomSampling(BaseMaximizer):
         # random_sampling.py:38-47: int(0.7 n) uniform points followed by int(0.3 n) Gaussian ones (n = 5 gives 3 + 1)
         n_uniform = int(self.n_samples * .7)
         n_total = n_uniform + int(self.n_samples * .3)
-        if blr or rf:
+        if blr or rf or bnn:
             handle = model._ready_handle()
         else:
             model.gp._restore()

@@ -8,6 +8,7 @@ from robo_b200 import _lib
 from robo_b200.models.bayesian_linear_regression import BayesianLinearRegression
 from robo_b200.models.gaussian_process import GaussianProcess
 from robo_b200.models.random_forest import RandomForest
+from robo_b200.models.wrapper_bohamiann import WrapperBohamiann
 
 KINDS = ("ei", "log_ei", "pi", "lcb")
 
@@ -46,7 +47,8 @@ def device_spec(acq, who):
 
 def acq_spec(acq, who):
     """(kind, eta per model, par, handles) of the acquisition, or TypeError when it does not run on device GPs whose
-    inputs go to the handle untransformed or on a BayesianLinearRegression or RandomForest (eta: its min observed y)."""
+    inputs go to the handle untransformed or on a BayesianLinearRegression, RandomForest or WrapperBohamiann (eta: its
+    min observed y)."""
     if hasattr(acq, "_fused_spec"):                          # MarginalizationGPMCMC
         fused = acq._fused_spec()
         if fused is None or not all(raw_inputs(m) for m in acq.model.models):
@@ -55,7 +57,7 @@ def acq_spec(acq, who):
         return kind, etas, par, handles
     model = getattr(acq, "model", None)
     kind = getattr(acq, "kind", None)
-    if isinstance(model, (BayesianLinearRegression, RandomForest)) and kind in KINDS and getattr(acq, "cost_model", None) is None:
+    if isinstance(model, (BayesianLinearRegression, RandomForest, WrapperBohamiann)) and kind in KINDS and getattr(acq, "cost_model", None) is None:
         eta = 0.0 if kind == "lcb" else float(model.get_incumbent()[1])
         return kind, [eta], float(acq.par), [model._ready_handle()]
     if kind not in KINDS or getattr(acq, "cost_model", None) is not None or not raw_inputs(model) \

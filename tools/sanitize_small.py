@@ -146,6 +146,18 @@ print("rf nodes", t["n_nodes"][:3], "predict", h.predict(Xs[:300])[1][:2],
 r = _lib.maximize_direct([h], _lib.ACQ_EI, [float(y.min())], 0.0, np.zeros(D), np.ones(D), n_func_evals=100)
 print("rf direct", r["nit"], r["nfev"])
 h.close()
+# Bayesian neural network: the chain (burn-in, cut-over, keeps), its draws, the sample read-back and upload, the
+# predictive pass over a ragged tile, scored directly and through DIRECT
+h = _lib.Handle(0)
+_lib.bnn_set_data(h, X[:23], y[:23])
+_lib.bnn_train(h, 5, 0, 1e-2, 0.05, 1e-10, 4, 30, 5, 20)
+Zb = _lib.bnn_draws(h, 5, 0, -1, 3)
+_lib.bnn_set_samples(h, _lib.bnn_samples(h))
+print("bnn samples", _lib.bnn_dims(h), "draws", Zb[0, :2], "predict", h.predict(Xs[:300])[1][:2],
+      "acq", h.acq(Xs[:300], _lib.ACQ_EI, float(y.min()), 0.0)["best_idx"])
+r = _lib.maximize_direct([h], _lib.ACQ_EI, [float(y.min())], 0.0, np.zeros(D), np.ones(D), n_func_evals=100)
+print("bnn direct", r["nit"], r["nfev"])
+h.close()
 h = _lib.moments_handle()
 print(h.acq_moments(rng.randn(100), rng.rand(100) + 0.1, _lib.ACQ_LOG_EI, 0.0, 0.0)[0][:3])
 print(h.reduce_models(rng.rand(4, 50), rng.rand(4, 50))[1][:3])
