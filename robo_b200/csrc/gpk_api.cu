@@ -48,6 +48,9 @@ struct DevBuf {
     size_t cap = 0;
 };
 
+// the model a handle holds: a Gaussian process unless a gpk_*_set_data made it a surrogate, which it stays for life
+enum ModelKind { MODEL_GP, MODEL_BLR, MODEL_RF, MODEL_BNN };
+
 }  // namespace
 
 struct gpk_handle {
@@ -168,28 +171,27 @@ struct gpk_handle {
     bool has_hyper = false;
     HyperModel hyper;
     DevBuf hy_buf;
-    // Bayesian linear regression (gpk_blr.cuh): set once by gpk_blr_set_data, after which the handle serves the BLR
-    // entry points and the scoring ones only.  blr_data: Phi (n x F), y, G = Phi^T Phi, b = Phi^T y; blr_post: the fit's
-    // M (k x F), L^-1 and S (k x F x F each), 1 / beta (k), failure flags; blr_work: thetas / walkers and their values;
-    // blr_bb: the predictive pass's block arg-max pairs
-    bool blr = false, blr_fitted = false;
+    // a surrogate handle serves its own entry points and the scoring ones only; its scoring pass uses block_best, best
+    // and nneg as the GP's does
+    ModelKind model = MODEL_GP;
+    // Bayesian linear regression (gpk_blr.cuh, gpk_blr_set_data).  blr_data: Phi (n x F), y, G = Phi^T Phi,
+    // b = Phi^T y; blr_post: the fit's M (k x F), L^-1 and S (k x F x F each), 1 / beta (k), failure flags; blr_work:
+    // thetas / walkers and their values
+    bool blr_fitted = false;
     int blr_basis = 0, blr_F = 0, blr_k = 0;
     BlrPrior blr_prior;
-    DevBuf blr_data, blr_post, blr_work, blr_bb;
-    // random forest (gpk_rf.cuh): set once by gpk_rf_set_data, after which the handle serves the RF entry points and the
-    // scoring ones only.  rf_data: X (n x d), y (n), the per-feature row order (d x n ints); rf_work: the growth's
-    // per-tree multiplicities, lists and segments; rf_nodes: the trees (RfNodes); rf_bb: the block arg-max pairs
-    bool rf = false, rf_fitted = false;
+    DevBuf blr_data, blr_post, blr_work;
+    // random forest (gpk_rf.cuh, gpk_rf_set_data).  rf_data: X (n x d), y (n), the per-feature row order (d x n ints);
+    // rf_work: the growth's per-tree multiplicities, lists and segments; rf_nodes: the trees (RfNodes)
+    bool rf_fitted = false;
     int rf_T = 0, rf_total = 0;
-    DevBuf rf_data, rf_work, rf_nodes, rf_bb;
-    // Bayesian neural network (gpk_bnn.cuh): set once by gpk_bnn_set_data, after which the handle serves the BNN entry
-    // points and the scoring ones only.  bnn_data: the scaled X (n x d), y (n), the input mean and std (d each);
-    // bnn_samples: the kept networks (S x P); bnn_state: the chain's final theta, p, tau, g, vhat (P each); bnn_bb: the
-    // block arg-max pairs
-    bool bnn = false;
+    DevBuf rf_data, rf_work, rf_nodes;
+    // Bayesian neural network (gpk_bnn.cuh, gpk_bnn_set_data).  bnn_data: the scaled X (n x d), y (n), the input mean
+    // and std (d each); bnn_samples: the kept networks (S x P); bnn_state: the chain's final theta, p, tau, g, vhat
+    // (P each)
     int bnn_P = 0, bnn_S = 0;
     double bnn_ymean = 0.0, bnn_ystd = 1.0;
-    DevBuf bnn_data, bnn_samples, bnn_state, bnn_bb;
+    DevBuf bnn_data, bnn_samples, bnn_state;
     int es_nb = 0, es_np = 0;
     double es_sn2 = 0.0, es_H = 0.0;
     long es_linv_serial = -1;       // linv_serial U was built for (-1: no update yet)
@@ -771,19 +773,49 @@ __global__ void gpk_resid_kernel(const double* __restrict__ y, double mean, int 
     if (i < NP) out[i] = (i < n) ? y[i] - mean : 0.0;
 }
 
-// the message of every Gaussian-process entry point called with a BLR handle
-#define BLR_REFUSAL "the handle holds a Bayesian linear regression model (gpk_blr_set_data); this entry point serves " \
-                    "Gaussian-process handles only"
-// ... and with a random-forest handle
-#define RF_REFUSAL "the handle holds a random forest (gpk_rf_set_data); this entry point serves Gaussian-process " \
-                   "handles only"
-// ... and with a Bayesian-neural-network handle
-#define BNN_REFUSAL "the handle holds a Bayesian neural network (gpk_bnn_set_data); this entry point serves " \
-                    "Gaussian-process handles only"
+// What the refusals between model kinds say about each kind, indexed by ModelKind
+struct ModelInfo {
+    const char* holds;          // "the handle holds <holds>"
+    const char* set_data;       // the entry point that gives a handle this kind
+    const char* use_for;        // "use a new handle for <use_for>"
+    const char* not_fitted;     // the scoring entry points' refusal before the model is trained
+    const char* gp_refusal;     // the Gaussian-process entry points' refusal
+};
+#define SURROGATE(what, set_data, use_for, not_fitted)                                                               \
+    {what " (" set_data ")", set_data, use_for, not_fitted,                                                         \
+     "the handle holds " what " (" set_data "); this entry point serves Gaussian-process handles only"}
+const ModelInfo MODELS[] = {
+    {"a Gaussian-process model", nullptr, nullptr, nullptr, nullptr},
+    SURROGATE("a Bayesian linear regression model", "gpk_blr_set_data", "Bayesian linear regression",
+              "model is not fitted (gpk_blr_fit)"),
+    SURROGATE("a random forest", "gpk_rf_set_data", "a random forest", "model is not fitted (gpk_rf_fit)"),
+    SURROGATE("a Bayesian neural network", "gpk_bnn_set_data", "a Bayesian neural network",
+              "model is not trained (gpk_bnn_train)"),
+};
+#undef SURROGATE
 
 // the refusal of a Gaussian-process entry point for the handle's model kind, or nullptr for a Gaussian-process handle
-const char* gp_refusal(const gpk_handle* h) {
-    return h->blr ? BLR_REFUSAL : h->rf ? RF_REFUSAL : h->bnn ? BNN_REFUSAL : nullptr;
+const char* gp_refusal(const gpk_handle* h) { return MODELS[h->model].gp_refusal; }
+
+// the refusal of the `kind` entry point `who` on a handle that holds another model
+int refuse_model(gpk_handle* h, ModelKind kind, const char* who) {
+    BAD("%s: the handle holds %s; use a new handle for %s", who, MODELS[h->model].holds, MODELS[kind].use_for);
+}
+
+// gpk_*_set_data's check before the handle takes the surrogate `kind`: it holds no other surrogate, and no GP data or
+// kernel
+int claim_model(gpk_handle* h, ModelKind kind, const char* who) {
+    if (h->model == MODEL_GP ? h->has_data || h->has_spec : h->model != kind) return refuse_model(h, kind, who);
+    return GPK_OK;
+}
+
+// the check of every other `kind` entry point: the handle holds that surrogate; then its device is made current
+int model_ready(gpk_handle* h, ModelKind kind, const char* who) {
+    if (!h) return GPK_BAD_ARG;
+    if (h->model != MODEL_GP && h->model != kind) return refuse_model(h, kind, who);
+    if (h->model != kind) BAD("%s: %s has not been called", who, MODELS[kind].set_data);
+    CK(cudaSetDevice(h->device));
+    return GPK_OK;
 }
 
 int require(gpk_handle* h, bool data, bool spec, bool fitted) {
@@ -795,21 +827,12 @@ int require(gpk_handle* h, bool data, bool spec, bool fitted) {
     return GPK_OK;
 }
 
-// the preconditions of the entry points that score either model kind: a fitted GP, or a BLR handle after gpk_blr_fit
+// the preconditions of the entry points that score any model kind: a fitted GP, or a trained surrogate
 int require_model(gpk_handle* h) {
-    if (h && h->blr) {
-        if (!h->blr_fitted) { set_err(h, "model is not fitted (gpk_blr_fit)"); return GPK_NOT_FITTED; }
-        return GPK_OK;
-    }
-    if (h && h->rf) {
-        if (!h->rf_fitted) { set_err(h, "model is not fitted (gpk_rf_fit)"); return GPK_NOT_FITTED; }
-        return GPK_OK;
-    }
-    if (h && h->bnn) {
-        if (h->bnn_S < 1) { set_err(h, "model is not trained (gpk_bnn_train)"); return GPK_NOT_FITTED; }
-        return GPK_OK;
-    }
-    return require(h, true, true, true);
+    if (!h || h->model == MODEL_GP) return require(h, true, true, true);
+    const bool trained = h->model == MODEL_BLR ? h->blr_fitted : h->model == MODEL_RF ? h->rf_fitted : h->bnn_S >= 1;
+    if (!trained) { set_err(h, "%s", MODELS[h->model].not_fitted); return GPK_NOT_FITTED; }
+    return GPK_OK;
 }
 
 // L^-1 by recursive block inversion (P lower, Q = P^T upper), after a successful fit.
@@ -931,32 +954,34 @@ struct Feeder {
     virtual ~Feeder() {}
 };
 
+int surrogate_score(gpk_handle* h, const double* dX, long m, int kind, double eta, double par, double* d_out,
+                    double* d_mu, double* d_var, BestPair* d_best, unsigned long long* d_nneg, long index_offset,
+                    bool reset, long global_base, Feeder* feeder);
+
+// the outputs of a scoring launch whose first candidate is row `offset` of the caller's batch (score_dev's arguments)
+ScoreOut score_out(gpk_handle* h, int kind, double eta, double par, double* d_out, double* d_mu, double* d_var,
+                   unsigned long long* d_nneg, long offset, long global_base) {
+    ScoreOut o;
+    o.base = global_base + offset;
+    o.acq_kind = kind; o.eta = eta; o.par = par;
+    o.out_mu = d_mu ? d_mu + offset : nullptr;
+    o.out_var = d_var ? d_var + offset : nullptr;
+    o.out_acq = d_out ? d_out + offset : nullptr;
+    o.block_best = ptr<BestPair>(h->block_best);
+    o.n_negative = d_nneg;
+    return o;
+}
+
 // Score m candidates resident on the device.  All output pointers are device pointers or NULL.
 // index_offset: position of dX[0] in the caller's batch (offset into the output arrays and into the arg-max index);
 // global_base: added to the arg-max index only (first index of this rank's shard in a sharded batch); reset: start a
 // new running arg-max / negative-EI count (false when a host batch is fed in several pieces)
-int blr_score(gpk_handle* h, const double* dX, long m, int kind, double eta, double par, double* d_out, double* d_mu,
-              double* d_var, BestPair* d_best, unsigned long long* d_nneg, long index_offset, bool reset, long global_base,
-              Feeder* feeder);
-int rf_score(gpk_handle* h, const double* dX, long m, int kind, double eta, double par, double* d_out, double* d_mu,
-             double* d_var, BestPair* d_best, unsigned long long* d_nneg, long index_offset, bool reset, long global_base,
-             Feeder* feeder);
-int bnn_score(gpk_handle* h, const double* dX, long m, int kind, double eta, double par, double* d_out, double* d_mu,
-              double* d_var, BestPair* d_best, unsigned long long* d_nneg, long index_offset, bool reset, long global_base,
-              Feeder* feeder);
-
 int score_dev(gpk_handle* h, const double* dX, long m, int kind, double eta, double par, double* d_out,
               double* d_mu, double* d_var, BestPair* d_best, unsigned long long* d_nneg,
               long index_offset = 0, bool reset = true, long global_base = 0, Feeder* feeder = nullptr) {
-    if (h->blr)
-        return blr_score(h, dX, m, kind, eta, par, d_out, d_mu, d_var, d_best, d_nneg, index_offset, reset, global_base,
-                         feeder);
-    if (h->rf)
-        return rf_score(h, dX, m, kind, eta, par, d_out, d_mu, d_var, d_best, d_nneg, index_offset, reset, global_base,
-                        feeder);
-    if (h->bnn)
-        return bnn_score(h, dX, m, kind, eta, par, d_out, d_mu, d_var, d_best, d_nneg, index_offset, reset, global_base,
-                         feeder);
+    if (h->model != MODEL_GP)
+        return surrogate_score(h, dX, m, kind, eta, par, d_out, d_mu, d_var, d_best, d_nneg, index_offset, reset,
+                               global_base, feeder);
     int rc = build_linv(h);
     if (rc) return rc;
     const long NP = h->NP;
@@ -1089,19 +1114,14 @@ int score_dev(gpk_handle* h, const double* dX, long m, int kind, double eta, dou
         FinishArgs f;
         memset(&f, 0, sizeof(f));
         f.part_mu = ptr<double>(h->part_mu); f.part_ssq = ptr<double>(h->part_ssq);
-        f.ldpart = cap; f.nparts = h->nb; f.m = mc; f.base = global_base + index_offset + base;
+        f.ldpart = cap; f.nparts = h->nb; f.m = mc;
         f.kss = h->spec.amp; f.mean = h->mean;
         f.factor = h->spec.factor;
         f.cand = dX + base * h->d; f.cand_dc = h->d;
         f.lo = h->has_bounds ? ptr<double>(h->lower) : nullptr;
         f.up = h->has_bounds ? ptr<double>(h->upper) : nullptr;
         f.norm_out = h->norm_out; f.y_mean = h->y_mean; f.y_std = h->y_std;
-        f.acq_kind = kind; f.eta = eta; f.par = par;
-        f.out_mu = d_mu ? d_mu + index_offset + base : nullptr;
-        f.out_var = d_var ? d_var + index_offset + base : nullptr;
-        f.out_acq = d_out ? d_out + index_offset + base : nullptr;
-        f.block_best = ptr<BestPair>(h->block_best);
-        f.n_negative = d_nneg;
+        f.o = score_out(h, kind, eta, par, d_out, d_mu, d_var, d_nneg, index_offset + base, global_base);
         if (use_oz && second) f.part_mu = ptr<double>(h->oz_pmu2);
         const int fb = (int)((mc + 255) / 256);
         gpk_finish_kernel<<<fb, 256, 0, h->stream>>>(f);
@@ -1348,13 +1368,8 @@ struct BlrPost {
 };
 
 int blr_ready(gpk_handle* h, const char* who) {
-    if (!h) return GPK_BAD_ARG;
-    if (h->rf) BAD("%s: the handle holds a random forest (gpk_rf_set_data); use a new handle for Bayesian linear "
-                   "regression", who);
-    if (h->bnn) BAD("%s: the handle holds a Bayesian neural network (gpk_bnn_set_data); use a new handle for Bayesian "
-                    "linear regression", who);
-    if (!h->blr) BAD("%s: gpk_blr_set_data has not been called", who);
-    CK(cudaSetDevice(h->device));
+    int rc = model_ready(h, MODEL_BLR, who);
+    if (rc) return rc;
     const int sm_eval = (int)(gpk_blr_smem_doubles(h->blr_F) * 8);
     CK(cudaFuncSetAttribute(gpk_blr_eval_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, sm_eval));
     CK(cudaFuncSetAttribute(gpk_blr_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, sm_eval));
@@ -1362,49 +1377,6 @@ int blr_ready(gpk_handle* h, const char* who) {
                             sm_eval + h->blr_F * h->blr_F * 8));
     CK(cudaFuncSetAttribute(gpk_blr_score_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                             h->blr_F * GPK_BLR_SCORE_THREADS * 8));
-    return GPK_OK;
-}
-
-// score_dev for a BLR handle: the predictive pass of gpk_blr_score_kernel over the m rows dX, with score_dev's outputs,
-// offsets and running arg-max
-int blr_score(gpk_handle* h, const double* dX, long m, int kind, double eta, double par, double* d_out, double* d_mu,
-              double* d_var, BestPair* d_best, unsigned long long* d_nneg, long index_offset, bool reset, long global_base,
-              Feeder* feeder) {
-    int rc;
-    if ((rc = blr_ready(h, "scoring"))) return rc;
-    const int nblk = (int)((m + GPK_BLR_SCORE_THREADS - 1) / GPK_BLR_SCORE_THREADS);
-    if ((rc = ensure(h, h->blr_bb, (size_t)std::max(nblk, 1) * sizeof(BestPair)))) return rc;
-    if ((rc = ensure(h, h->best, sizeof(BestPair)))) return rc;
-    if ((rc = ensure(h, h->nneg, 8))) return rc;
-    if (d_best == nullptr) d_best = ptr<BestPair>(h->best);
-    if (d_nneg == nullptr) d_nneg = ptr<unsigned long long>(h->nneg);
-    if (reset) {
-        CK(cudaMemsetAsync(d_best, 0xFF, sizeof(BestPair), h->stream));
-        CK(cudaMemsetAsync(d_nneg, 0, 8, h->stream));
-    }
-    if (feeder && (rc = feeder->ready(0, m, h->stream))) return rc;
-    const int F = h->blr_F, k = h->blr_k;
-    const BlrPost L(k, F);
-    double* post = ptr<double>(h->blr_post);
-    BlrScoreArgs a;
-    memset(&a, 0, sizeof(a));
-    a.X = dX; a.m = m; a.D = h->d; a.F = F; a.basis = h->blr_basis; a.k = k;
-    a.M = post + L.M; a.Li = post + L.Li; a.ib = post + L.ib;
-    a.base = global_base + index_offset;
-    a.acq_kind = kind; a.eta = eta; a.par = par;
-    a.out_mu = d_mu ? d_mu + index_offset : nullptr;
-    a.out_var = d_var ? d_var + index_offset : nullptr;
-    a.out_acq = d_out ? d_out + index_offset : nullptr;
-    a.block_best = ptr<BestPair>(h->blr_bb);
-    a.n_negative = d_nneg;
-    if (m > 0) {
-        gpk_blr_score_kernel<<<nblk, GPK_BLR_SCORE_THREADS, (size_t)F * GPK_BLR_SCORE_THREADS * 8, h->stream>>>(a);
-        CKL();
-        if (kind != GPK_ACQ_NONE) {
-            gpk_argmax_final_kernel<<<1, 256, 0, h->stream>>>(ptr<BestPair>(h->blr_bb), nblk, d_best);
-            CKL();
-        }
-    }
     return GPK_OK;
 }
 
@@ -1425,91 +1397,25 @@ struct RfNodes {
     }
 };
 
-int rf_ready(gpk_handle* h, const char* who) {
-    if (!h) return GPK_BAD_ARG;
-    if (h->blr) BAD("%s: the handle holds a Bayesian linear regression model (gpk_blr_set_data); use a new handle for a "
-                    "random forest", who);
-    if (h->bnn) BAD("%s: the handle holds a Bayesian neural network (gpk_bnn_set_data); use a new handle for a random "
-                    "forest", who);
-    if (!h->rf) BAD("%s: gpk_rf_set_data has not been called", who);
-    CK(cudaSetDevice(h->device));
-    return GPK_OK;
-}
-
-// score_dev for a random-forest handle: gpk_rf_score_kernel over the m rows dX, with score_dev's outputs, offsets and
-// running arg-max
-int rf_score(gpk_handle* h, const double* dX, long m, int kind, double eta, double par, double* d_out, double* d_mu,
-             double* d_var, BestPair* d_best, unsigned long long* d_nneg, long index_offset, bool reset, long global_base,
-             Feeder* feeder) {
-    int rc;
-    if ((rc = rf_ready(h, "scoring"))) return rc;
-    const long nblk = (m + GPK_RF_SCORE_WARPS - 1) / GPK_RF_SCORE_WARPS;
-    if ((rc = ensure(h, h->rf_bb, (size_t)std::max(nblk, 1L) * sizeof(BestPair)))) return rc;
-    if ((rc = ensure(h, h->best, sizeof(BestPair)))) return rc;
-    if ((rc = ensure(h, h->nneg, 8))) return rc;
-    if (d_best == nullptr) d_best = ptr<BestPair>(h->best);
-    if (d_nneg == nullptr) d_nneg = ptr<unsigned long long>(h->nneg);
-    if (reset) {
-        CK(cudaMemsetAsync(d_best, 0xFF, sizeof(BestPair), h->stream));
-        CK(cudaMemsetAsync(d_nneg, 0, 8, h->stream));
-    }
-    if (feeder && (rc = feeder->ready(0, m, h->stream))) return rc;
-    const long S = 2L * h->n;
-    const RfNodes L(h->rf_T, S);
-    char* nodes = ptr<char>(h->rf_nodes);
-    RfScoreArgs a;
-    memset(&a, 0, sizeof(a));
-    a.X = dX; a.m = m; a.D = h->d; a.T = h->rf_T; a.S = S;
-    a.feat = (const int*)(nodes + L.feat); a.left = (const int*)(nodes + L.left);
-    a.thr = (const double*)(nodes + L.thr); a.mean = (const double*)(nodes + L.mean);
-    a.var = (const double*)(nodes + L.var);
-    a.total_var = h->rf_total;
-    a.base = global_base + index_offset;
-    a.acq_kind = kind; a.eta = eta; a.par = par;
-    a.out_mu = d_mu ? d_mu + index_offset : nullptr;
-    a.out_var = d_var ? d_var + index_offset : nullptr;
-    a.out_acq = d_out ? d_out + index_offset : nullptr;
-    a.block_best = ptr<BestPair>(h->rf_bb);
-    a.n_negative = d_nneg;
-    if (m > 0) {
-        gpk_rf_score_kernel<<<(unsigned)nblk, GPK_RF_SCORE_WARPS * 32, gpk_rf_score_smem_doubles(h->rf_T) * 8,
-                              h->stream>>>(a);
-        CKL();
-        if (kind != GPK_ACQ_NONE) {
-            gpk_argmax_final_kernel<<<1, 256, 0, h->stream>>>(ptr<BestPair>(h->rf_bb), (int)nblk, d_best);
-            CKL();
-        }
-    }
-    return GPK_OK;
-}
-
 // the layout of h->bnn_data: the scaled X (n x d), the scaled y (n), the input mean and std (d each)
 inline double* bnn_X(gpk_handle* h) { return ptr<double>(h->bnn_data); }
 inline double* bnn_y(gpk_handle* h) { return bnn_X(h) + (size_t)h->n * h->d; }
 inline double* bnn_xm(gpk_handle* h) { return bnn_y(h) + h->n; }
 inline double* bnn_xs(gpk_handle* h) { return bnn_xm(h) + h->d; }
 
-int bnn_ready(gpk_handle* h, const char* who) {
-    if (!h) return GPK_BAD_ARG;
-    if (h->blr) BAD("%s: the handle holds a Bayesian linear regression model (gpk_blr_set_data); use a new handle for a "
-                    "Bayesian neural network", who);
-    if (h->rf) BAD("%s: the handle holds a random forest (gpk_rf_set_data); use a new handle for a Bayesian neural "
-                   "network", who);
-    if (!h->bnn) BAD("%s: gpk_bnn_set_data has not been called", who);
-    CK(cudaSetDevice(h->device));
-    return GPK_OK;
-}
-
-// score_dev for a BNN handle: gpk_bnn_score_kernel over the m rows dX, with score_dev's outputs, offsets and running
-// arg-max
-int bnn_score(gpk_handle* h, const double* dX, long m, int kind, double eta, double par, double* d_out, double* d_mu,
-              double* d_var, BestPair* d_best, unsigned long long* d_nneg, long index_offset, bool reset, long global_base,
-              Feeder* feeder) {
-    int rc;
-    if ((rc = bnn_ready(h, "scoring"))) return rc;
-    constexpr long TILE = GPK_BNN_SCORE_THREADS * GPK_BNN_SCORE_C;
-    const long nblk = (m + TILE - 1) / TILE;
-    if ((rc = ensure(h, h->bnn_bb, (size_t)std::max(nblk, 1L) * sizeof(BestPair)))) return rc;
+// score_dev for a surrogate handle: its scoring kernel over the m rows dX in one launch, with score_dev's outputs,
+// offsets and running arg-max
+int surrogate_score(gpk_handle* h, const double* dX, long m, int kind, double eta, double par, double* d_out,
+                    double* d_mu, double* d_var, BestPair* d_best, unsigned long long* d_nneg, long index_offset,
+                    bool reset, long global_base, Feeder* feeder) {
+    int rc = h->model == MODEL_BLR ? blr_ready(h, "scoring") : model_ready(h, h->model, "scoring");
+    if (rc) return rc;
+    // candidates per CTA
+    const long tile = h->model == MODEL_BLR ? GPK_BLR_SCORE_THREADS
+                    : h->model == MODEL_RF  ? GPK_RF_SCORE_WARPS
+                                            : GPK_BNN_SCORE_THREADS * GPK_BNN_SCORE_C;
+    const long nblk = (m + tile - 1) / tile;
+    if ((rc = ensure(h, h->block_best, (size_t)std::max(nblk, 1L) * sizeof(BestPair)))) return rc;
     if ((rc = ensure(h, h->best, sizeof(BestPair)))) return rc;
     if ((rc = ensure(h, h->nneg, 8))) return rc;
     if (d_best == nullptr) d_best = ptr<BestPair>(h->best);
@@ -1519,28 +1425,54 @@ int bnn_score(gpk_handle* h, const double* dX, long m, int kind, double eta, dou
         CK(cudaMemsetAsync(d_nneg, 0, 8, h->stream));
     }
     if (feeder && (rc = feeder->ready(0, m, h->stream))) return rc;
-    BnnScoreArgs a;
-    memset(&a, 0, sizeof(a));
-    a.X = dX; a.m = m; a.D = h->d; a.P = h->bnn_P; a.S = h->bnn_S;
-    a.samples = ptr<double>(h->bnn_samples);
-    a.xm = bnn_xm(h); a.xs = bnn_xs(h);
-    a.y_mean = h->bnn_ymean; a.y_std = h->bnn_ystd;
-    a.base = global_base + index_offset;
-    a.acq_kind = kind; a.eta = eta; a.par = par;
-    a.out_mu = d_mu ? d_mu + index_offset : nullptr;
-    a.out_var = d_var ? d_var + index_offset : nullptr;
-    a.out_acq = d_out ? d_out + index_offset : nullptr;
-    a.block_best = ptr<BestPair>(h->bnn_bb);
-    a.n_negative = d_nneg;
-    if (m > 0) {
+    if (m == 0) return GPK_OK;
+    const ScoreOut o = score_out(h, kind, eta, par, d_out, d_mu, d_var, d_nneg, index_offset, global_base);
+    switch (h->model) {
+    case MODEL_BLR: {
+        const int F = h->blr_F, k = h->blr_k;
+        const BlrPost L(k, F);
+        const double* post = ptr<double>(h->blr_post);
+        BlrScoreArgs a;
+        memset(&a, 0, sizeof(a));
+        a.X = dX; a.m = m; a.D = h->d; a.F = F; a.basis = h->blr_basis; a.k = k;
+        a.M = post + L.M; a.Li = post + L.Li; a.ib = post + L.ib;
+        a.o = o;
+        gpk_blr_score_kernel<<<(unsigned)nblk, GPK_BLR_SCORE_THREADS, (size_t)F * GPK_BLR_SCORE_THREADS * 8, h->stream>>>(a);
+        break;
+    }
+    case MODEL_RF: {
+        const long S = 2L * h->n;
+        const RfNodes L(h->rf_T, S);
+        const char* nodes = ptr<char>(h->rf_nodes);
+        RfScoreArgs a;
+        memset(&a, 0, sizeof(a));
+        a.X = dX; a.m = m; a.D = h->d; a.T = h->rf_T; a.S = S;
+        a.feat = (const int*)(nodes + L.feat); a.left = (const int*)(nodes + L.left);
+        a.thr = (const double*)(nodes + L.thr); a.mean = (const double*)(nodes + L.mean);
+        a.var = (const double*)(nodes + L.var);
+        a.total_var = h->rf_total;
+        a.o = o;
+        gpk_rf_score_kernel<<<(unsigned)nblk, GPK_RF_SCORE_WARPS * 32, gpk_rf_score_smem_doubles(h->rf_T) * 8,
+                              h->stream>>>(a);
+        break;
+    }
+    default: {                                          // MODEL_BNN
+        BnnScoreArgs a;
+        memset(&a, 0, sizeof(a));
+        a.X = dX; a.m = m; a.D = h->d; a.P = h->bnn_P; a.S = h->bnn_S;
+        a.samples = ptr<double>(h->bnn_samples);
+        a.xm = bnn_xm(h); a.xs = bnn_xs(h);
+        a.y_mean = h->bnn_ymean; a.y_std = h->bnn_ystd;
+        a.o = o;
         const size_t smem = (size_t)gpk_bnn_score_smem(h->d);
         CK(cudaFuncSetAttribute(gpk_bnn_score_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         gpk_bnn_score_kernel<<<(unsigned)nblk, GPK_BNN_SCORE_THREADS, smem, h->stream>>>(a);
+    }
+    }
+    CKL();
+    if (kind != GPK_ACQ_NONE) {
+        gpk_argmax_final_kernel<<<1, 256, 0, h->stream>>>(ptr<BestPair>(h->block_best), (int)nblk, d_best);
         CKL();
-        if (kind != GPK_ACQ_NONE) {
-            gpk_argmax_final_kernel<<<1, 256, 0, h->stream>>>(ptr<BestPair>(h->bnn_bb), (int)nblk, d_best);
-            CKL();
-        }
     }
     return GPK_OK;
 }
@@ -1602,9 +1534,8 @@ int gpk_destroy(gpk_handle* h) {
                       &h->tmpjobs, &h->alpha, &h->tmp1, &h->tmp2, &h->tmp3, &h->dprof, &h->Xts, &h->oz_Pq, &h->oz_Kq, &h->oz_Kq2, &h->oz_eP, &h->oz_emax, &h->oz_pmu2, &h->oz_probe,
                       &h->multi_cand, &h->multi_A, &h->multi_B, &h->multi_out, &h->multi_bb, &h->gather, &h->best_global,
                       &h->de_pop, &h->de_trial, &h->de_param, &h->de_E, &h->de_small, &h->de_sort, &h->lb_buf, &h->cma_buf, &h->dir_buf, &h->ep_buf, &h->es_state, &h->es_U, &h->es_work, &h->es_in, &h->mc_state, &h->mc_buf, &h->mc_stat, &h->fab_in, &h->rs_buf, &h->hy_buf,
-                      &h->blr_data, &h->blr_post, &h->blr_work, &h->blr_bb,
-                      &h->rf_data, &h->rf_work, &h->rf_nodes, &h->rf_bb,
-                      &h->bnn_data, &h->bnn_samples, &h->bnn_state, &h->bnn_bb};
+                      &h->blr_data, &h->blr_post, &h->blr_work, &h->rf_data, &h->rf_work, &h->rf_nodes,
+                      &h->bnn_data, &h->bnn_samples, &h->bnn_state};
     for (DevBuf* b : bufs)
         if (b->p) cudaFree(b->p);
     if (h->ev_ok)
@@ -2788,20 +2719,15 @@ int gpk_sample_hypers(gpk_handle* h, const double* p0, int nwalkers, int dim, in
 int gpk_blr_set_data(gpk_handle* h, const double* X, const double* y, int n, int d, int basis, const double* prior_par) {
     if (!h) return GPK_BAD_ARG;
     const char* who = "gpk_blr_set_data";
-    if (h->rf) BAD("%s: the handle holds a random forest (gpk_rf_set_data); use a new handle for Bayesian linear "
-                   "regression", who);
-    if (h->bnn) BAD("%s: the handle holds a Bayesian neural network (gpk_bnn_set_data); use a new handle for Bayesian "
-                    "linear regression", who);
-    if (!h->blr && (h->has_data || h->has_spec))
-        BAD("%s: the handle holds a Gaussian-process model; use a new handle for Bayesian linear regression", who);
+    int rc = claim_model(h, MODEL_BLR, who);
+    if (rc) return rc;
     if (!X || !y || !prior_par || n <= 0 || d <= 0) BAD("%s: need X, y, prior_par, n > 0, d > 0", who);
     if (basis < GPK_BLR_LINEAR || basis > GPK_BLR_NONE) BAD("%s: unknown basis %d", who, basis);
     const long F = basis == GPK_BLR_LINEAR ? (long)d + 1 : basis == GPK_BLR_QUADRATIC ? 2L * d + 1 : d;
     if (F > GPK_BLR_MAX_F)
         BAD("%s: %ld features (d = %d) exceed GPK_BLR_MAX_F = %d", who, F, d, GPK_BLR_MAX_F);
     CK(cudaSetDevice(h->device));
-    int rc;
-    h->blr = true;
+    h->model = MODEL_BLR;
     h->blr_fitted = false;
     h->n = n; h->d = d; h->blr_F = (int)F; h->blr_basis = basis;
     h->blr_prior.ln_sigma = prior_par[0]; h->blr_prior.ln_loc = prior_par[1]; h->blr_prior.hs_scale = prior_par[2];
@@ -2907,7 +2833,7 @@ int gpk_blr_get_models(gpk_handle* h, double* m, double* S) {
     const char* who = "gpk_blr_get_models";
     int rc = blr_ready(h, who);
     if (rc) return rc;
-    if (!h->blr_fitted) { set_err(h, "%s: model is not fitted (gpk_blr_fit)", who); return GPK_NOT_FITTED; }
+    if (!h->blr_fitted) { set_err(h, "%s: %s", who, MODELS[MODEL_BLR].not_fitted); return GPK_NOT_FITTED; }
     const BlrPost L(h->blr_k, h->blr_F);
     const double* post = ptr<double>(h->blr_post);
     if (m) CK(cudaMemcpyAsync(m, post + L.M, (size_t)h->blr_k * h->blr_F * 8, cudaMemcpyDeviceToHost, h->stream));
@@ -2932,12 +2858,8 @@ int gpk_blr_dims(gpk_handle* h, int* n, int* F, int* k) {
 int gpk_rf_set_data(gpk_handle* h, const double* X, const double* y, int n, int d) {
     if (!h) return GPK_BAD_ARG;
     const char* who = "gpk_rf_set_data";
-    if (h->blr) BAD("%s: the handle holds a Bayesian linear regression model (gpk_blr_set_data); use a new handle for a "
-                    "random forest", who);
-    if (h->bnn) BAD("%s: the handle holds a Bayesian neural network (gpk_bnn_set_data); use a new handle for a random "
-                    "forest", who);
-    if (!h->rf && (h->has_data || h->has_spec))
-        BAD("%s: the handle holds a Gaussian-process model; use a new handle for a random forest", who);
+    int rc = claim_model(h, MODEL_RF, who);
+    if (rc) return rc;
     if (!X || !y || n <= 0 || d <= 0) BAD("%s: need X, y, n > 0, d > 0", who);
     if (n > GPK_RF_MAX_N) BAD("%s: n = %d training points exceed GPK_RF_MAX_N = %d", who, n, GPK_RF_MAX_N);
     if (d > GPK_RF_MAX_D) BAD("%s: d = %d exceeds GPK_RF_MAX_D = %d", who, d, GPK_RF_MAX_D);
@@ -2956,8 +2878,7 @@ int gpk_rf_set_data(gpk_handle* h, const double* X, const double* y, int n, int 
             return xa < xb || (xa == xb && a < b);
         });
     }
-    int rc;
-    h->rf = true;
+    h->model = MODEL_RF;
     h->rf_fitted = false;
     h->n = n; h->d = d;
     if ((rc = ensure(h, h->rf_data, ((size_t)n * d + n) * 8 + (size_t)d * n * 4))) return rc;
@@ -2971,7 +2892,7 @@ int gpk_rf_set_data(gpk_handle* h, const double* X, const double* y, int n, int 
 int gpk_rf_fit(gpk_handle* h, unsigned long long seed, unsigned counter, int T, int n_per_tree, int bootstrap,
                int total_variance) {
     const char* who = "gpk_rf_fit";
-    int rc = rf_ready(h, who);
+    int rc = model_ready(h, MODEL_RF, who);
     if (rc) return rc;
     const int n = h->n, d = h->d;
     if (T < 1 || T > GPK_RF_MAX_T) BAD("%s: need 1 <= num_trees <= GPK_RF_MAX_T = %d (num_trees = %d)", who, GPK_RF_MAX_T, T);
@@ -3014,7 +2935,7 @@ int gpk_rf_fit(gpk_handle* h, unsigned long long seed, unsigned counter, int T, 
 }
 
 int gpk_rf_dims(gpk_handle* h, int* n, int* d, int* T, int* slots) {
-    int rc = rf_ready(h, "gpk_rf_dims");
+    int rc = model_ready(h, MODEL_RF, "gpk_rf_dims");
     if (rc) return rc;
     if (n) *n = h->n;
     if (d) *d = h->d;
@@ -3026,9 +2947,9 @@ int gpk_rf_dims(gpk_handle* h, int* n, int* d, int* T, int* slots) {
 int gpk_rf_get_trees(gpk_handle* h, int* n_nodes, int* feat, double* thr, int* left, double* W, double* mean,
                      double* var) {
     const char* who = "gpk_rf_get_trees";
-    int rc = rf_ready(h, who);
+    int rc = model_ready(h, MODEL_RF, who);
     if (rc) return rc;
-    if (!h->rf_fitted) { set_err(h, "%s: model is not fitted (gpk_rf_fit)", who); return GPK_NOT_FITTED; }
+    if (!h->rf_fitted) { set_err(h, "%s: %s", who, MODELS[MODEL_RF].not_fitted); return GPK_NOT_FITTED; }
     const long S = 2L * h->n;
     const size_t TS = (size_t)h->rf_T * S;
     const RfNodes L(h->rf_T, S);
@@ -3045,7 +2966,7 @@ int gpk_rf_get_trees(gpk_handle* h, int* n_nodes, int* feat, double* thr, int* l
 int gpk_rf_set_trees(gpk_handle* h, int T, int total_variance, const int* n_nodes, const int* feat, const double* thr,
                      const int* left, const double* W, const double* mean, const double* var) {
     const char* who = "gpk_rf_set_trees";
-    int rc = rf_ready(h, who);
+    int rc = model_ready(h, MODEL_RF, who);
     if (rc) return rc;
     if (T < 1 || T > GPK_RF_MAX_T) BAD("%s: need 1 <= T <= GPK_RF_MAX_T = %d", who, GPK_RF_MAX_T);
     if (!n_nodes || !feat || !thr || !left || !W || !mean || !var) BAD("%s: need every node array", who);
@@ -3082,12 +3003,8 @@ int gpk_rf_set_trees(gpk_handle* h, int T, int total_variance, const int* n_node
 int gpk_bnn_set_data(gpk_handle* h, const double* X, const double* y, int n, int d) {
     if (!h) return GPK_BAD_ARG;
     const char* who = "gpk_bnn_set_data";
-    if (h->blr) BAD("%s: the handle holds a Bayesian linear regression model (gpk_blr_set_data); use a new handle for a "
-                    "Bayesian neural network", who);
-    if (h->rf) BAD("%s: the handle holds a random forest (gpk_rf_set_data); use a new handle for a Bayesian neural "
-                   "network", who);
-    if (!h->bnn && (h->has_data || h->has_spec))
-        BAD("%s: the handle holds a Gaussian-process model; use a new handle for a Bayesian neural network", who);
+    int rc = claim_model(h, MODEL_BNN, who);
+    if (rc) return rc;
     if (!X || !y || n <= 0 || d <= 0) BAD("%s: need X, y, n > 0, d > 0", who);
     if (n < 2) BAD("%s: need n >= 2 training points to normalise the data (n = %d)", who, n);
     if (n > GPK_BNN_MAX_N) BAD("%s: n = %d training points exceed GPK_BNN_MAX_N = %d", who, n, GPK_BNN_MAX_N);
@@ -3125,8 +3042,7 @@ int gpk_bnn_set_data(gpk_handle* h, const double* X, const double* y, int n, int
     if (!(ysd > 0.0)) BAD("%s: y is constant; it cannot be normalised", who);
     for (int i = 0; i < n; ++i) ys[i] = (y[i] - ym) / ysd;
     CK(cudaSetDevice(h->device));
-    int rc;
-    h->bnn = true;
+    h->model = MODEL_BNN;
     h->bnn_S = 0;
     h->n = n; h->d = d;
     h->bnn_P = gpk_bnn_params(d);
@@ -3140,7 +3056,7 @@ int gpk_bnn_set_data(gpk_handle* h, const double* X, const double* y, int n, int
 int gpk_bnn_train(gpk_handle* h, unsigned long long seed, unsigned counter, double lr, double mdecay, double eps,
                   long burn_in, long num_steps, long keep_every, int batch) {
     const char* who = "gpk_bnn_train";
-    int rc = bnn_ready(h, who);
+    int rc = model_ready(h, MODEL_BNN, who);
     if (rc) return rc;
     if (!(std::isfinite(lr) && lr > 0.0) || !(std::isfinite(mdecay) && mdecay > 0.0) || !(std::isfinite(eps) && eps >= 0.0))
         BAD("%s: need finite lr > 0, mdecay > 0 and eps >= 0", who);
@@ -3173,7 +3089,7 @@ int gpk_bnn_train(gpk_handle* h, unsigned long long seed, unsigned counter, doub
 }
 
 int gpk_bnn_dims(gpk_handle* h, int* n, int* d, int* P, int* S) {
-    int rc = bnn_ready(h, "gpk_bnn_dims");
+    int rc = model_ready(h, MODEL_BNN, "gpk_bnn_dims");
     if (rc) return rc;
     if (n) *n = h->n;
     if (d) *d = h->d;
@@ -3184,9 +3100,9 @@ int gpk_bnn_dims(gpk_handle* h, int* n, int* d, int* P, int* S) {
 
 int gpk_bnn_get_samples(gpk_handle* h, double* samples) {
     const char* who = "gpk_bnn_get_samples";
-    int rc = bnn_ready(h, who);
+    int rc = model_ready(h, MODEL_BNN, who);
     if (rc) return rc;
-    if (h->bnn_S < 1) { set_err(h, "%s: model is not trained (gpk_bnn_train)", who); return GPK_NOT_FITTED; }
+    if (h->bnn_S < 1) { set_err(h, "%s: %s", who, MODELS[MODEL_BNN].not_fitted); return GPK_NOT_FITTED; }
     if (!samples) BAD("%s: need the output array", who);
     CK(cudaMemcpyAsync(samples, h->bnn_samples.p, (size_t)h->bnn_S * h->bnn_P * 8, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
@@ -3195,7 +3111,7 @@ int gpk_bnn_get_samples(gpk_handle* h, double* samples) {
 
 int gpk_bnn_set_samples(gpk_handle* h, int S, const double* samples) {
     const char* who = "gpk_bnn_set_samples";
-    int rc = bnn_ready(h, who);
+    int rc = model_ready(h, MODEL_BNN, who);
     if (rc) return rc;
     if (S < 1 || !samples) BAD("%s: need S >= 1 networks", who);
     h->bnn_S = 0;
@@ -3208,7 +3124,7 @@ int gpk_bnn_set_samples(gpk_handle* h, int S, const double* samples) {
 
 int gpk_bnn_get_state(gpk_handle* h, double* theta, double* p, double* tau, double* g, double* vhat) {
     const char* who = "gpk_bnn_get_state";
-    int rc = bnn_ready(h, who);
+    int rc = model_ready(h, MODEL_BNN, who);
     if (rc) return rc;
     if (h->bnn_S < 1 || !h->bnn_state.p) { set_err(h, "%s: no chain has run (gpk_bnn_train)", who); return GPK_NOT_FITTED; }
     double* out[5] = {theta, p, tau, g, vhat};
@@ -3221,7 +3137,7 @@ int gpk_bnn_get_state(gpk_handle* h, double* theta, double* p, double* tau, doub
 
 int gpk_bnn_draws(gpk_handle* h, unsigned long long seed, unsigned counter, int step0, int ns, double* Z) {
     const char* who = "gpk_bnn_draws";
-    int rc = bnn_ready(h, who);
+    int rc = model_ready(h, MODEL_BNN, who);
     if (rc) return rc;
     if (ns < 1 || !Z) BAD("%s: need ns >= 1 and an output array", who);
     const int P = h->bnn_P;

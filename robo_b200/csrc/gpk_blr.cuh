@@ -281,11 +281,7 @@ __global__ void __launch_bounds__(GPK_BLR_THREADS) gpk_blr_fit_kernel(const doub
 struct BlrScoreArgs {
     const double* X; long m; int D, F, basis, k;
     const double* M; const double* Li; const double* ib;
-    long base;                  // global index of X[0] (arg-max)
-    int acq_kind; double eta, par;
-    double* out_mu; double* out_var; double* out_acq;
-    BestPair* block_best;
-    unsigned long long* n_negative;
+    ScoreOut o;
 };
 
 // the marginalised predictive moments of every candidate, the acquisition and the block arg-max (gpk_finish_kernel's)
@@ -318,30 +314,9 @@ __global__ void __launch_bounds__(GPK_BLR_SCORE_THREADS) gpk_blr_score_kernel(co
         const double mu = smu / (double)a.k;
         double var = svar / (double)a.k;
         if (var < GPK_EPS) var = GPK_EPS;                  // np.clip(v, eps, inf); NaN stays NaN
-        if (a.out_mu) a.out_mu[c] = mu;
-        if (a.out_var) a.out_var[c] = var;
-        if (a.acq_kind != GPK_ACQ_NONE) {
-            val = gpk_acq_value(a.acq_kind, mu, var, a.eta, a.par);
-            if (a.out_acq) a.out_acq[c] = val;
-            if (a.acq_kind == GPK_ACQ_EI && val < 0.0 && a.n_negative) atomicAdd(a.n_negative, 1ULL);
-            idx = a.base + c;
-        }
+        gpk_score_emit(a.o, c, mu, var, val, idx);
     }
-    if (a.acq_kind == GPK_ACQ_NONE) return;
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) {
-        double ov = __shfl_xor_sync(0xffffffffu, val, off);
-        long long oi = __shfl_xor_sync(0xffffffffu, idx, off);
-        if (gpk_better(ov, oi, val, idx)) { val = ov; idx = oi; }
-    }
-    __shared__ double sv[NT / 32];
-    __shared__ long long si[NT / 32];
-    if ((threadIdx.x & 31) == 0) { sv[threadIdx.x >> 5] = val; si[threadIdx.x >> 5] = idx; }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        for (int w = 1; w < NT / 32; ++w)
-            if (gpk_better(sv[w], si[w], val, idx)) { val = sv[w]; idx = si[w]; }
-        a.block_best[blockIdx.x].val = val;
-        a.block_best[blockIdx.x].idx = idx;
-    }
+    if (a.o.acq_kind == GPK_ACQ_NONE) return;
+    gpk_block_best<NT / 32>(val, idx);
+    if (threadIdx.x == 0) a.o.block_best[blockIdx.x] = {val, idx};
 }

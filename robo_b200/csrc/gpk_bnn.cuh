@@ -310,11 +310,7 @@ struct BnnScoreArgs {
     const double* samples;                 // S x P (16-byte aligned rows: P is even)
     const double* xm; const double* xs;    // input mean and std (D each)
     double y_mean, y_std;
-    long base;                             // global index of X[0] (arg-max)
-    int acq_kind; double eta, par;
-    double* out_mu; double* out_var; double* out_acq;
-    BestPair* block_best;
-    unsigned long long* n_negative;
+    ScoreOut o;
 };
 
 // dynamic shared memory of gpk_bnn_score_kernel: the two-stage ring of networks, the scaled candidate tile, 2 mbarriers
@@ -441,30 +437,12 @@ __global__ void __launch_bounds__(GPK_BNN_SCORE_THREADS) gpk_bnn_score_kernel(co
         if (ci >= a.m) continue;
         const double mu = fma(mean[c], a.y_std, a.y_mean);
         const double var = (m2[c] / Sd + vev) * ys2;
-        if (a.out_mu) a.out_mu[ci] = mu;
-        if (a.out_var) a.out_var[ci] = var;
-        if (a.acq_kind != GPK_ACQ_NONE) {
-            const double v = gpk_acq_value(a.acq_kind, mu, var, a.eta, a.par);
-            if (a.out_acq) a.out_acq[ci] = v;
-            if (a.acq_kind == GPK_ACQ_EI && v < 0.0 && a.n_negative) atomicAdd(a.n_negative, 1ULL);
-            if (gpk_better(v, a.base + ci, val, idx)) { val = v; idx = a.base + ci; }
-        }
+        double v = 0.0;
+        long long vi = -1;
+        gpk_score_emit(a.o, ci, mu, var, v, vi);
+        if (gpk_better(v, vi, val, idx)) { val = v; idx = vi; }
     }
-    if (a.acq_kind == GPK_ACQ_NONE) return;
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) {
-        double ov = __shfl_xor_sync(0xffffffffu, val, off);
-        long long oi = __shfl_xor_sync(0xffffffffu, idx, off);
-        if (gpk_better(ov, oi, val, idx)) { val = ov; idx = oi; }
-    }
-    __shared__ double sv[NT / 32];
-    __shared__ long long si[NT / 32];
-    if ((tid & 31) == 0) { sv[tid >> 5] = val; si[tid >> 5] = idx; }
-    __syncthreads();
-    if (tid == 0) {
-        for (int w = 1; w < NT / 32; ++w)
-            if (gpk_better(sv[w], si[w], val, idx)) { val = sv[w]; idx = si[w]; }
-        a.block_best[blockIdx.x].val = val;
-        a.block_best[blockIdx.x].idx = idx;
-    }
+    if (a.o.acq_kind == GPK_ACQ_NONE) return;
+    gpk_block_best<NT / 32>(val, idx);
+    if (tid == 0) a.o.block_best[blockIdx.x] = {val, idx};
 }

@@ -221,3 +221,49 @@ __device__ __forceinline__ bool gpk_better(double va, long long ia, double vb, l
 }
 
 struct BestPair { double val; long long idx; };
+
+// warp arg-max: every lane ends with the warp's best pair
+__device__ __forceinline__ void gpk_warp_best(double& val, long long& idx) {
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+        double ov = __shfl_xor_sync(0xffffffffu, val, off);
+        long long oi = __shfl_xor_sync(0xffffffffu, idx, off);
+        if (gpk_better(ov, oi, val, idx)) { val = ov; idx = oi; }
+    }
+}
+
+// block arg-max over NW warps: thread 0 ends with the block's best pair.  Every thread of the block must call it.
+template <int NW>
+__device__ __forceinline__ void gpk_block_best(double& val, long long& idx) {
+    gpk_warp_best(val, idx);
+    __shared__ double sv[NW];
+    __shared__ long long si[NW];
+    if ((threadIdx.x & 31) == 0) { sv[threadIdx.x >> 5] = val; si[threadIdx.x >> 5] = idx; }
+    __syncthreads();
+    if (threadIdx.x == 0)
+        for (int w = 1; w < NW; ++w)
+            if (gpk_better(sv[w], si[w], val, idx)) { val = sv[w]; idx = si[w]; }
+}
+
+// What a scoring kernel writes, shared by the GP epilogue and every surrogate's scoring kernel
+struct ScoreOut {
+    long base;                  // global index of the launch's candidate 0 (arg-max)
+    int acq_kind; double eta, par;
+    double* out_mu; double* out_var; double* out_acq;    // launch-local device arrays, may be NULL
+    BestPair* block_best;       // one per block
+    unsigned long long* n_negative;
+};
+
+// Candidate c's outputs: mu and var and, with an acquisition, its value, the negative-EI count and the pair (val, idx)
+// the arg-max starts from.  zero_std_ei: EI is 0 at zero variance instead of gpk_acq_value's (the random forest's rule).
+__device__ __forceinline__ void gpk_score_emit(const ScoreOut& o, long c, double mu, double var, double& val,
+                                               long long& idx, bool zero_std_ei = false) {
+    if (o.out_mu) o.out_mu[c] = mu;
+    if (o.out_var) o.out_var[c] = var;
+    if (o.acq_kind != GPK_ACQ_NONE) {
+        val = (zero_std_ei && o.acq_kind == GPK_ACQ_EI && var == 0.0) ? 0.0 : gpk_acq_value(o.acq_kind, mu, var, o.eta, o.par);
+        if (o.out_acq) o.out_acq[c] = val;
+        if (o.acq_kind == GPK_ACQ_EI && val < 0.0 && o.n_negative) atomicAdd(o.n_negative, 1ULL);
+        idx = o.base + c;
+    }
+}

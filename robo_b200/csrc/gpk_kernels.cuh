@@ -244,7 +244,6 @@ __global__ void gpk_kfix_kernel(double* __restrict__ K, long ld, int n, int NP, 
 struct FinishArgs {
     const double* part_mu; const double* part_ssq; long ldpart; int nparts;
     long m;                 // valid candidates in this chunk
-    long base;              // global index of the chunk's first candidate
     double kss;             // k(x*, x*) = amplitude (stationary kernels)
     // the kernel's factor: k(x*, x*) = kss * gpk_factor_value(z*, z*), z* from the chunk's candidates (row-major raw
     // inputs, cand_dc columns, bounds lo / up)
@@ -252,10 +251,7 @@ struct FinishArgs {
     const double* cand; int cand_dc; const double* lo; const double* up;
     double mean;            // GP constant mean
     int norm_out; double y_mean, y_std;
-    int acq_kind; double eta, par;
-    double* out_mu; double* out_var; double* out_acq;    // chunk-local device arrays, may be NULL
-    BestPair* block_best;   // one per block
-    unsigned long long* n_negative;
+    ScoreOut o;             // chunk-local: base is the global index of the chunk's first candidate
 };
 
 __global__ void __launch_bounds__(256) gpk_finish_kernel(const FinishArgs f)
@@ -278,33 +274,11 @@ __global__ void __launch_bounds__(256) gpk_finish_kernel(const FinishArgs f)
         mu += f.mean;
         if (f.norm_out) { mu = mu * f.y_std + f.y_mean; var = var * (f.y_std * f.y_std); }
         if (var < GPK_EPS) var = GPK_EPS;                  // np.clip(var, eps, inf); NaN stays NaN
-        if (f.out_mu) f.out_mu[c] = mu;
-        if (f.out_var) f.out_var[c] = var;
-        if (f.acq_kind != GPK_ACQ_NONE) {
-            val = gpk_acq_value(f.acq_kind, mu, var, f.eta, f.par);
-            if (f.out_acq) f.out_acq[c] = val;
-            if (f.acq_kind == GPK_ACQ_EI && val < 0.0 && f.n_negative) atomicAdd(f.n_negative, 1ULL);
-            idx = f.base + c;
-        }
+        gpk_score_emit(f.o, c, mu, var, val, idx);
     }
-    if (f.acq_kind == GPK_ACQ_NONE || f.block_best == nullptr) return;
-    // block arg-max
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) {
-        double ov = __shfl_xor_sync(0xffffffffu, val, off);
-        long long oi = __shfl_xor_sync(0xffffffffu, idx, off);
-        if (gpk_better(ov, oi, val, idx)) { val = ov; idx = oi; }
-    }
-    __shared__ double sv[8];
-    __shared__ long long si[8];
-    if ((threadIdx.x & 31) == 0) { sv[threadIdx.x >> 5] = val; si[threadIdx.x >> 5] = idx; }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        for (int w = 1; w < 8; ++w)
-            if (gpk_better(sv[w], si[w], val, idx)) { val = sv[w]; idx = si[w]; }
-        f.block_best[blockIdx.x].val = val;
-        f.block_best[blockIdx.x].idx = idx;
-    }
+    if (f.o.acq_kind == GPK_ACQ_NONE) return;
+    gpk_block_best<8>(val, idx);
+    if (threadIdx.x == 0) f.o.block_best[blockIdx.x] = {val, idx};
 }
 
 // Mean-only epilogue (gpk_predict_mean): gpk_finish_kernel's mean, with the same fixed-order sum of the per-tile
@@ -331,21 +305,8 @@ __global__ void __launch_bounds__(256) gpk_argmax_final_kernel(const BestPair* _
     long long idx = -1;
     for (int b = threadIdx.x; b < nblocks; b += 256)
         if (gpk_better(bb[b].val, bb[b].idx, val, idx)) { val = bb[b].val; idx = bb[b].idx; }
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) {
-        double ov = __shfl_xor_sync(0xffffffffu, val, off);
-        long long oi = __shfl_xor_sync(0xffffffffu, idx, off);
-        if (gpk_better(ov, oi, val, idx)) { val = ov; idx = oi; }
-    }
-    __shared__ double sv[8];
-    __shared__ long long si[8];
-    if ((threadIdx.x & 31) == 0) { sv[threadIdx.x >> 5] = val; si[threadIdx.x >> 5] = idx; }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        for (int w = 1; w < 8; ++w)
-            if (gpk_better(sv[w], si[w], val, idx)) { val = sv[w]; idx = si[w]; }
-        if (gpk_better(val, idx, best->val, best->idx)) { best->val = val; best->idx = idx; }
-    }
+    gpk_block_best<8>(val, idx);
+    if (threadIdx.x == 0 && gpk_better(val, idx, best->val, best->idx)) { best->val = val; best->idx = idx; }
 }
 
 // Acquisition closed form on supplied moments (gpk_acq_moments).

@@ -268,11 +268,7 @@ struct RfScoreArgs {
     const double* X; long m; int D, T; long S;           // S: node slots per tree
     const int* feat; const int* left; const double* thr; const double* mean; const double* var;
     int total_var;
-    long base;                  // global index of X[0] (arg-max)
-    int acq_kind; double eta, par;
-    double* out_mu; double* out_var; double* out_acq;
-    BestPair* block_best;
-    unsigned long long* n_negative;
+    ScoreOut o;
 };
 
 // doubles of dynamic shared memory of gpk_rf_score_kernel for T trees
@@ -311,28 +307,11 @@ __global__ void __launch_bounds__(GPK_RF_SCORE_WARPS * 32) gpk_rf_score_kernel(c
             }
             double vr = __ddiv_rn(sq, Td);
             if (a.total_var) vr = __dadd_rn(vr, __ddiv_rn(sv, Td));
-            if (a.out_mu) a.out_mu[c] = mu;
-            if (a.out_var) a.out_var[c] = vr;
-            if (a.acq_kind != GPK_ACQ_NONE) {
-                // a zero std gives EI 0 (ei.py:72-74), not s (z Phi(z) + phi(z)) = 0 * inf
-                val = (a.acq_kind == GPK_ACQ_EI && vr == 0.0) ? 0.0 : gpk_acq_value(a.acq_kind, mu, vr, a.eta, a.par);
-                if (a.out_acq) a.out_acq[c] = val;
-                if (a.acq_kind == GPK_ACQ_EI && val < 0.0 && a.n_negative) atomicAdd(a.n_negative, 1ULL);
-                idx = a.base + c;
-            }
+            // a zero std gives EI 0 (ei.py:72-74), not s (z Phi(z) + phi(z)) = 0 * inf
+            gpk_score_emit(a.o, c, mu, vr, val, idx, true);
         }
     }
-    if (a.acq_kind == GPK_ACQ_NONE) return;
-    __shared__ double sv[GPK_RF_SCORE_WARPS];
-    __shared__ long long si[GPK_RF_SCORE_WARPS];
-    if (lane == 0) { sv[warp] = val; si[warp] = idx; }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        val = sv[0];
-        idx = si[0];
-        for (int w = 1; w < GPK_RF_SCORE_WARPS; ++w)
-            if (gpk_better(sv[w], si[w], val, idx)) { val = sv[w]; idx = si[w]; }
-        a.block_best[blockIdx.x].val = val;
-        a.block_best[blockIdx.x].idx = idx;
-    }
+    if (a.o.acq_kind == GPK_ACQ_NONE) return;
+    gpk_block_best<GPK_RF_SCORE_WARPS>(val, idx);
+    if (threadIdx.x == 0) a.o.block_best[blockIdx.x] = {val, idx};
 }

@@ -18,9 +18,8 @@ import numpy as np
 from robo_b200 import _lib
 from robo_b200.distributed import allgather_best, pack_pair, shard_bounds
 from robo_b200.maximizers.base_maximizer import BaseMaximizer
-from robo_b200.models.bayesian_linear_regression import BayesianLinearRegression
+from robo_b200.maximizers.device_spec import DEVICE_SURROGATES
 from robo_b200.models.random_forest import RandomForest
-from robo_b200.models.wrapper_bohamiann import WrapperBohamiann
 
 
 class DeviceRandomSampling(BaseMaximizer):
@@ -38,18 +37,12 @@ class DeviceRandomSampling(BaseMaximizer):
         es = self._es_cost_spec(acq)
         if es is not None:
             return self._maximize_es_cost(acq, es)
-        blr = isinstance(model, BayesianLinearRegression)
-        rf = isinstance(model, RandomForest)
-        bnn = isinstance(model, WrapperBohamiann)
-        if not (blr or rf or bnn) and (not hasattr(model, "gp") or not hasattr(model.gp, "handle")):
+        surrogate = isinstance(model, DEVICE_SURROGATES)
+        if not surrogate and (not hasattr(model, "gp") or not hasattr(model.gp, "handle")):
             raise TypeError("DeviceRandomSampling needs a robo_b200 GaussianProcess, BayesianLinearRegression, "
                             "RandomForest or WrapperBohamiann model")
-        if blr and self.world > 1:
-            raise ValueError("DeviceRandomSampling of a BayesianLinearRegression runs on one GPU")
-        if rf and self.world > 1:
-            raise ValueError("DeviceRandomSampling of a RandomForest runs on one GPU")
-        if bnn and self.world > 1:
-            raise ValueError("DeviceRandomSampling of a WrapperBohamiann runs on one GPU")
+        if surrogate and self.world > 1:
+            raise ValueError("DeviceRandomSampling of a %s runs on one GPU" % type(model).__name__)
         kind = _lib.ACQ_KIND[acq.kind]
         inc_x, inc_y = model.get_incumbent()
         eta = 0.0 if acq.kind == "lcb" else float(inc_y)
@@ -58,7 +51,7 @@ class DeviceRandomSampling(BaseMaximizer):
         # random_sampling.py:38-47: int(0.7 n) uniform points followed by int(0.3 n) Gaussian ones (n = 5 gives 3 + 1)
         n_uniform = int(self.n_samples * .7)
         n_total = n_uniform + int(self.n_samples * .3)
-        if blr or rf or bnn:
+        if surrogate:
             handle = model._ready_handle()
         else:
             model.gp._restore()
@@ -80,7 +73,7 @@ class DeviceRandomSampling(BaseMaximizer):
                 dev = "cuda:%d" % torch.cuda.current_device() if torch.cuda.is_available() else "cpu"
                 val, idx = allgather_best(pack_pair(val, idx, dev), self.group)
                 x = handle.generate_candidates(seed, idx, 1, n_uniform, self.lower, self.upper, inc_x, 0.1)[0]
-        if rf and acq.kind == "ei":
+        if isinstance(model, RandomForest) and acq.kind == "ei":
             X = handle.generate_candidates(seed, 0, n_total, n_uniform, self.lower, self.upper, inc_x, 0.1)
             if (np.sqrt(model.predict(X)[1]) == 0).any():
                 x, val, idx = X[0], 0.0, 0

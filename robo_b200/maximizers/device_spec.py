@@ -11,6 +11,8 @@ from robo_b200.models.random_forest import RandomForest
 from robo_b200.models.wrapper_bohamiann import WrapperBohamiann
 
 KINDS = ("ei", "log_ei", "pi", "lcb")
+# the models other than GaussianProcess that score on the device: each holds one handle of its own (_ready_handle)
+DEVICE_SURROGATES = (BayesianLinearRegression, RandomForest, WrapperBohamiann)
 
 
 def raw_inputs(model):
@@ -57,7 +59,7 @@ def acq_spec(acq, who):
         return kind, etas, par, handles
     model = getattr(acq, "model", None)
     kind = getattr(acq, "kind", None)
-    if isinstance(model, (BayesianLinearRegression, RandomForest, WrapperBohamiann)) and kind in KINDS and getattr(acq, "cost_model", None) is None:
+    if isinstance(model, DEVICE_SURROGATES) and kind in KINDS and getattr(acq, "cost_model", None) is None:
         eta = 0.0 if kind == "lcb" else float(model.get_incumbent()[1])
         return kind, [eta], float(acq.par), [model._ready_handle()]
     if kind not in KINDS or getattr(acq, "cost_model", None) is not None or not raw_inputs(model) \
