@@ -82,10 +82,6 @@ int gpk_destroy(gpk_handle* h);
 const char* gpk_last_error(gpk_handle* h);
 const char* gpk_version(void);
 /* key in
- *   "loader"    operand staging of the GEMM tile engine: 2 = TMA with a dedicated producer warp and
- *               full/empty mbarriers [default], 1 = TMA issued by a consumer thread, 0 = cp.async (cross-check).
- *               The covariance builder follows it: TMA-staged, pre-scaled term-major operands under 1 and 2; one
- *               broadcast load per pair and term from an axis-major operand under 0
  *   "chunk"     candidates per scoring pass (multiple of 128); 0 = automatic [default]: the K* buffer is kept near
  *               512 MB (16384 candidates at N = 4096, 65536 at N <= 1024)
  *   "ozaki"     1 = variance contraction on the int8 tensor pipe (wgmma s8, register accumulators) through an
@@ -202,7 +198,7 @@ int gpk_predict(gpk_handle* h, const double* Xs, long m, double* mu, double* var
  * digit stores compiled out and sums the per-tile shares of K* alpha in the same fixed order, alpha = L^-T z built once
  * per fit: mu is bit-identical to gpk_predict's wherever gpk_predict takes the int8 path (option "ozaki", m >= 2048),
  * and within rounding of its fp64 path elsewhere; no variance work.  Xs (m, d) raw inputs, m >= 1; mu (m).
- * GPK_BAD_ARG under option "loader" = 0 (the builder needs TMA), GPK_NOT_FITTED before gpk_fit. */
+ * GPK_NOT_FITTED before gpk_fit. */
 int gpk_predict_mean(gpk_handle* h, const double* Xs, long m, double* mu);
 /* the same on device pointers (d_Xs: m x d, d_mu: m doubles), asynchronous on the handle's stream */
 int gpk_predict_mean_dev(gpk_handle* h, const void* d_Xs, long m, void* d_mu);
@@ -435,7 +431,7 @@ typedef enum {
  * lower / upper (n_bounds = d - 1 entries each): the configuration bounds of the models' transform.  out (m) and best_val / best_idx
  * (numpy.argmax of out) may be NULL.  GPK_BAD_ARG: n < 1, m < 1, a basis code out of range, lower >= upper, handles on
  * different devices or with different input dimensions, a handle listed twice (objective and cost lists together), an
- * objective handle without a current gpk_es_update (or changed since), a cost handle under option "loader" = 0. */
+ * objective handle without a current gpk_es_update (or changed since). */
 int gpk_es_cost_multi(gpk_handle* const* objective, gpk_handle* const* cost, int n, const double* Xs, long m,
                       const double* lower, const double* upper, int n_bounds, int basis_objective, int basis_cost,
                       double overhead,

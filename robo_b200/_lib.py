@@ -246,9 +246,7 @@ class Handle(object):
             raise RuntimeError("gpk_create failed on device %d (status %d): no usable CUDA device; "
                                "robo_b200 has no CPU fallback" % (self.device, rc))
         self._h = h
-        # test/diagnostic overrides: GPK_LOADER=0|1 (cp.async | TMA staging), GPK_CHUNK=<multiple of 128>
-        if os.environ.get("GPK_LOADER"):
-            self.set_option("loader", int(os.environ["GPK_LOADER"]))
+        # test/diagnostic override: GPK_CHUNK=<multiple of 128>
         if os.environ.get("GPK_CHUNK"):
             self.set_option("chunk", int(os.environ["GPK_CHUNK"]))
         # schedule and contraction switches: GPK_OZAKI=0|1 (fp64 | int8 variance contraction), GPK_DEPTH2,

@@ -81,7 +81,6 @@ struct gpk_handle {
     double oz_launches = 0;
     int n_sm = 0;
     char err[1024] = {0};
-    int loader = LOADER_TMA_WS;
     long chunk = 16384;
     bool chunk_user = false;        // false: candidates per scoring pass chosen from N (chunk_rows)
     int diag_prof = 0;            // 1: the blocked diagonal kernel records clock64() stamps per phase (diagnostics)
@@ -319,22 +318,12 @@ int make_cov_map(gpk_handle* h, CUtensorMap* map, void* base, int n_terms, long 
     return GPK_OK;
 }
 
-// The covariance builder follows the tile engine's loader: gpk_cov_tma_kernel with TMA, gpk_cov_kernel under cp.async
-// (loader 0, also what gpk_create falls back to when the driver has no cuTensorMapEncodeTiled)
-inline bool cov_tma(const gpk_handle* h) { return h->loader != LOADER_CPASYNC; }
-
 // "Transposed" operand of the covariance builder for n points X (row-major, n x d) into dst with ld columns:
-// term-major + pre-scaled for the TMA kernel (dst needs n_terms x ld doubles), axis-major for gpk_cov_kernel
-// (d x ld doubles).  lo / up: input bounds to apply first (NULL: none).
+// term-major and pre-scaled (dst needs n_terms x ld doubles).  lo / up: input bounds to apply first (NULL: none).
 int build_cov_operand(gpk_handle* h, cudaStream_t st, const double* X, long n, int d, const double* lo, const double* up,
                       double* dst, long ld) {
-    if (cov_tma(h)) {
-        const long total = (long)h->spec.n_terms * ld;
-        gpk_termmajor_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(h->spec, X, n, d, lo, up, dst, ld);
-    } else {
-        const long total = (long)d * ld;
-        gpk_transpose_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(X, n, d, lo, up, dst, ld);
-    }
+    const long total = (long)h->spec.n_terms * ld;
+    gpk_termmajor_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(h->spec, X, n, d, lo, up, dst, ld);
     CKL();
     return GPK_OK;
 }
@@ -349,21 +338,15 @@ int launch_cov_tiles(gpk_handle* h, cudaStream_t st, const double* operand, long
                      long m, long m_padded, const double* lo, const double* up, double* out, long ldo, int tri, bool small,
                      const double* pts, const double* plo, const double* pup) {
     const unsigned gx = (unsigned)(ldx / 128);
-    if (cov_tma(h)) {
-        CUtensorMap map;
-        int rc = make_cov_map(h, &map, (void*)operand, h->spec.n_terms, ldx);
-        if (rc) return rc;
-        if (small)
-            gpk_cov_tma_kernel<4><<<dim3(gx, (unsigned)(m_padded / 16)), 256, cov_tma_smem_bytes(h->spec.n_terms, 4), st>>>(
-                map, h->spec, n, cand, dc, m, lo, up, out, ldo, tri);
-        else
-            gpk_cov_tma_kernel<8><<<dim3(gx, (unsigned)(m_padded / 32)), 256, cov_tma_smem_bytes(h->spec.n_terms, 8), st>>>(
-                map, h->spec, n, cand, dc, m, lo, up, out, ldo, tri);
-    } else if (small) {
-        gpk_cov_kernel<8><<<dim3(gx, (unsigned)(m_padded / 16)), 256, 0, st>>>(h->spec, operand, ldx, n, cand, dc, m, lo, up, out, ldo, tri);
-    } else {
-        gpk_cov_kernel<16><<<dim3(gx, (unsigned)(m_padded / 32)), 256, 0, st>>>(h->spec, operand, ldx, n, cand, dc, m, lo, up, out, ldo, tri);
-    }
+    CUtensorMap map;
+    int rc = make_cov_map(h, &map, (void*)operand, h->spec.n_terms, ldx);
+    if (rc) return rc;
+    if (small)
+        gpk_cov_tma_kernel<4><<<dim3(gx, (unsigned)(m_padded / 16)), 256, cov_tma_smem_bytes(h->spec.n_terms, 4), st>>>(
+            map, h->spec, n, cand, dc, m, lo, up, out, ldo, tri);
+    else
+        gpk_cov_tma_kernel<8><<<dim3(gx, (unsigned)(m_padded / 32)), 256, cov_tma_smem_bytes(h->spec.n_terms, 8), st>>>(
+            map, h->spec, n, cand, dc, m, lo, up, out, ldo, tri);
     CKL();
     if (h->spec.factor.kind != GPK_FACTOR_NONE && m > 0) {
         gpk_factor_scale_kernel<<<dim3(gx, (unsigned)std::min<long>((m + 1) / 2, 1024)), 256, 0, st>>>(
@@ -372,7 +355,6 @@ int launch_cov_tiles(gpk_handle* h, cudaStream_t st, const double* operand, long
     }
     return GPK_OK;
 }
-inline const double* train_operand(const gpk_handle* h) { return cov_tma(h) ? ptr<double>(h->Xts) : ptr<double>(h->Xt); }
 
 // ---- GEMM launch ---------------------------------------------------------------------------
 // Launch with the programmatic-stream-serialization attribute (PDL): the kernel's launch latency and prologue
@@ -468,36 +450,27 @@ int launch_oz_contraction(gpk_handle* h, const CUtensorMap& mapP, const CUtensor
     return GPK_OK;
 }
 
+// MI = 8: 128-row tiles on gpk_gemm_ws_kernel; MI = 2: the 32-row chain tiles (store only), through PDL
 template <int EPI, int MI = 8>
 int launch_gemm(gpk_handle* h, const CUtensorMap& mA, const CUtensorMap& mB, const GemmArgs& a, int njobs,
-                cudaStream_t stream = nullptr, bool pdl = false) {
+                cudaStream_t stream = nullptr) {
+    static_assert(MI == 8 || (MI == 2 && EPI == EPI_STORE), "128-row tiles, or 32-row chain tiles that store");
     if (njobs <= 0) return GPK_OK;
     if (stream == nullptr) stream = h->stream;
-    if (pdl && h->loader != LOADER_CPASYNC && MI == 2) {
-        CK(launch_pdl(gpk_gemm_nt_kernel<EPI, LOADER_TMA, MI>, dim3(njobs), dim3(GEMM_THREADS),
-                      (size_t)gemm_smem_bytes(LOADER_TMA, MI), stream, mA, mB, a));
+    if constexpr (MI == 2) {
+        CK(launch_pdl(gpk_gemm_nt_kernel, dim3(njobs), dim3(GEMM_THREADS), (size_t)GEMM_SMEM_CHAIN, stream, mA, mB, a));
         h->launches_total += 1;
         return GPK_OK;
     }
-    if (h->loader == LOADER_TMA_WS && MI == 8)
-        gpk_gemm_ws_kernel<EPI><<<njobs, WS_THREADS, GEMM_SMEM_TMA, stream>>>(mA, mB, a);
-    else if (h->loader != LOADER_CPASYNC)
-        gpk_gemm_nt_kernel<EPI, LOADER_TMA, MI><<<njobs, GEMM_THREADS, gemm_smem_bytes(LOADER_TMA, MI), stream>>>(mA, mB, a);
-    else
-        gpk_gemm_nt_kernel<EPI, LOADER_CPASYNC, MI><<<njobs, GEMM_THREADS, gemm_smem_bytes(LOADER_CPASYNC, MI), stream>>>(mA, mB, a);
+    gpk_gemm_ws_kernel<EPI><<<njobs, WS_THREADS, GEMM_SMEM_TMA, stream>>>(mA, mB, a);
     CKL();
     return GPK_OK;
 }
 
 int set_kernel_attrs(gpk_handle* h) {
-    CK(cudaFuncSetAttribute(gpk_gemm_nt_kernel<EPI_STORE, LOADER_TMA, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM_TMA));
-    CK(cudaFuncSetAttribute(gpk_gemm_nt_kernel<EPI_COLREDUCE, LOADER_TMA, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM_TMA));
-    CK(cudaFuncSetAttribute(gpk_gemm_nt_kernel<EPI_STORE, LOADER_CPASYNC, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM_PAD));
-    CK(cudaFuncSetAttribute(gpk_gemm_nt_kernel<EPI_COLREDUCE, LOADER_CPASYNC, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM_PAD));
     CK(cudaFuncSetAttribute(gpk_gemm_ws_kernel<EPI_STORE>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM_TMA));
     CK(cudaFuncSetAttribute(gpk_gemm_ws_kernel<EPI_COLREDUCE>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM_TMA));
-    CK(cudaFuncSetAttribute(gpk_gemm_nt_kernel<EPI_STORE, LOADER_TMA, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm_smem_bytes(LOADER_TMA, 2)));
-    CK(cudaFuncSetAttribute(gpk_gemm_nt_kernel<EPI_STORE, LOADER_CPASYNC, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm_smem_bytes(LOADER_CPASYNC, 2)));
+    CK(cudaFuncSetAttribute(gpk_gemm_nt_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM_CHAIN));
     CK(cudaFuncSetAttribute(gpk_oz_vargemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, OZ_SMEM));
     CK(cudaFuncSetAttribute(gpk_cov_oz_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cov_oz_smem_bytes(GPK_MAX_TERMS, 8)));
     CK(cudaFuncSetAttribute(gpk_cov_oz_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cov_oz_smem_bytes(GPK_MAX_TERMS, 4)));
@@ -651,7 +624,6 @@ int build_job_tables(gpk_handle* h) {
 }
 
 int rebuild_maps(gpk_handle* h) {
-    if (h->loader == LOADER_CPASYNC) { h->maps_ok = true; return GPK_OK; }
     const long NP = h->NP;
     int rc;
     if ((rc = make_map(h, &h->mapK, h->Kbuf.p, NP + BM, NP, NP))) return rc;
@@ -673,13 +645,13 @@ int ensure_score_scratch(gpk_handle* h, long rows) {
     int rc;
     if ((rc = ensure(h, h->Kstar, (size_t)rows * NP * 8, &grew))) return rc;
     if (grew || h->mapKs_rows != rows) {
-        if (h->loader != LOADER_CPASYNC && (rc = make_map(h, &h->mapKs, h->Kstar.p, rows, NP, NP))) return rc;
+        if ((rc = make_map(h, &h->mapKs, h->Kstar.p, rows, NP, NP))) return rc;
         h->mapKs_rows = rows;
     }
     if (h->overlap) {
         if ((rc = ensure(h, h->Kstar2, (size_t)rows * NP * 8, &grew))) return rc;
         if (grew || h->mapKs2_rows != rows) {
-            if (h->loader != LOADER_CPASYNC && (rc = make_map(h, &h->mapKs2, h->Kstar2.p, rows, NP, NP))) return rc;
+            if ((rc = make_map(h, &h->mapKs2, h->Kstar2.p, rows, NP, NP))) return rc;
             h->mapKs2_rows = rows;
         }
     }
@@ -905,7 +877,7 @@ int make_oz_map(gpk_handle* h, CUtensorMap* map, void* base, long rows_total, lo
 // A kernel with a factor is never eligible: the digit split of K* assumes 0 < k <= amp.
 int prepare_ozaki(gpk_handle* h, bool* usable) {
     *usable = false;
-    if (!h->ozaki || h->loader == LOADER_CPASYNC || h->NP > 16384 || h->spec.factor.kind != GPK_FACTOR_NONE)
+    if (!h->ozaki || h->NP > 16384 || h->spec.factor.kind != GPK_FACTOR_NONE)
         return GPK_OK;
     const long NP = h->NP;
     if (h->oz_linv_serial != h->linv_serial) {
@@ -1042,12 +1014,12 @@ int score_dev(gpk_handle* h, const double* dX, long m, int kind, double eta, dou
         const double* lo = h->has_bounds ? ptr<double>(h->lower) : nullptr;
         const double* up = h->has_bounds ? ptr<double>(h->upper) : nullptr;
         if (!use_oz)
-            return launch_cov_tiles(h, st, train_operand(h), NP, h->n, dX + base * h->d, h->d, mc, mcp, lo, up,
+            return launch_cov_tiles(h, st, ptr<double>(h->Xts), NP, h->n, dX + base * h->d, h->d, mc, mcp, lo, up,
                                     second ? ptr<double>(h->Kstar2) : ptr<double>(h->Kstar), NP, 0, small,
                                     ptr<double>(h->Xrow), nullptr, nullptr);
         // K* never reaches HBM in fp64: digits + this tile's share of the mean straight out of the builder
         CUtensorMap map;
-        int mrc = make_cov_map(h, &map, (void*)train_operand(h), h->spec.n_terms, NP);
+        int mrc = make_cov_map(h, &map, h->Xts.p, h->spec.n_terms, NP);
         if (mrc) return mrc;
         int8_t* qdst = second ? ptr<int8_t>(h->oz_Kq2) : ptr<int8_t>(h->oz_Kq);
         double* pmu = second ? ptr<double>(h->oz_pmu2) : ptr<double>(h->part_mu);
@@ -1169,7 +1141,6 @@ enum { ES_KIND_NONE = 0, ES_KIND_EP = 1, ES_KIND_MC = 2 };
 int predict_mean_dev(gpk_handle* h, const double* dX, long m, double* d_mu) {
     if (!h->mean_only)                      // option "meanonly" = 0: the mean of the full scoring pass (comparisons)
         return score_dev(h, dX, m, GPK_ACQ_NONE, 0.0, 0.0, nullptr, d_mu, nullptr, nullptr, nullptr);
-    if (!cov_tma(h)) BAD("gpk_predict_mean: needs the TMA covariance builder (option loader 1 or 2)");
     int rc;
     if ((rc = build_linv(h))) return rc;
     if ((rc = ensure_alpha(h))) return rc;
@@ -1177,7 +1148,7 @@ int predict_mean_dev(gpk_handle* h, const double* dX, long m, double* d_mu) {
     const long cap = std::min<long>(chunk_rows(h), round_up(m, BM));
     if ((rc = ensure(h, h->part_mu, (size_t)h->nb * cap * 8))) return rc;
     CUtensorMap map;
-    if ((rc = make_cov_map(h, &map, (void*)train_operand(h), h->spec.n_terms, NP))) return rc;
+    if ((rc = make_cov_map(h, &map, h->Xts.p, h->spec.n_terms, NP))) return rc;
     const double* lo = h->has_bounds ? ptr<double>(h->lower) : nullptr;
     const double* up = h->has_bounds ? ptr<double>(h->upper) : nullptr;
     const int gx = (int)(NP / 128);
@@ -1513,11 +1484,15 @@ int gpk_create(gpk_handle** out, int device) {
     if (cudaEventCreateWithFlags(&h->ev_order, cudaEventDisableTiming) != cudaSuccess) { delete h; return GPK_CUDA_ERROR; }
     int rc = set_kernel_attrs(h);
     if (rc) { fprintf(stderr, "gpk_create: %s\n", h->err); delete h; return rc; }
+    if (get_encode_fn() == nullptr) {
+        fprintf(stderr, "gpk_create: the driver has no cuTensorMapEncodeTiled (TMA descriptors)\n");
+        delete h;
+        return GPK_CUDA_ERROR;
+    }
     rc = ensure(h, h->status, 4);
     if (!rc) rc = ensure(h, h->scal, 64);
     if (rc) { delete h; return rc; }
     if (cudaMallocHost((void**)&h->pin, 64) != cudaSuccess) { delete h; return GPK_CUDA_ERROR; }
-    if (get_encode_fn() == nullptr) h->loader = LOADER_CPASYNC;
     *out = h;
     return GPK_OK;
 }
@@ -1561,15 +1536,6 @@ int gpk_destroy(gpk_handle* h) {
 
 int gpk_set_option(gpk_handle* h, const char* key, long value) {
     if (!h || !key) return GPK_BAD_ARG;
-    if (!strcmp(key, "loader")) {
-        if (value < LOADER_CPASYNC || value > LOADER_TMA_WS) BAD("loader must be 0 (cp.async), 1 (TMA) or 2 (TMA, warp-specialised)");
-        if (value != LOADER_CPASYNC && get_encode_fn() == nullptr) BAD("TMA descriptors unavailable on this driver");
-        h->loader = (int)value;
-        h->maps_ok = false;
-        h->mapKs_rows = 0;
-        h->mapVt_rows = 0;
-        return GPK_OK;
-    }
     if (!strcmp(key, "ozpersist")) {
         if (value != 0 && value != 1 && value != 3) BAD("ozpersist must be 0, 1 or 3");
         h->oz_persist = (int)value;
@@ -1840,12 +1806,11 @@ int gpk_fit_begin(gpk_handle* h, double diag_add, double mean) {
 
     CK(cudaEventRecord(h->ev[0], h->stream));
     {
-        if (cov_tma(h)) {               // the pre-scaled operand depends on the hyper-parameters: rebuilt per fit (n_terms x NP)
-            if ((rc = ensure(h, h->Xts, (size_t)GPK_MAX_TERMS * NP * 8))) return rc;
-            if ((rc = build_cov_operand(h, h->stream, ptr<double>(h->Xrow), h->n, h->d, nullptr, nullptr, ptr<double>(h->Xts), NP)))
-                return rc;
-        }
-        if ((rc = launch_cov_tiles(h, h->stream, train_operand(h), NP, h->n, ptr<double>(h->Xrow), h->d, (long)h->n, NP,
+        // the pre-scaled operand depends on the hyper-parameters: rebuilt per fit (n_terms x NP)
+        if ((rc = ensure(h, h->Xts, (size_t)GPK_MAX_TERMS * NP * 8))) return rc;
+        if ((rc = build_cov_operand(h, h->stream, ptr<double>(h->Xrow), h->n, h->d, nullptr, nullptr, ptr<double>(h->Xts), NP)))
+            return rc;
+        if ((rc = launch_cov_tiles(h, h->stream, ptr<double>(h->Xts), NP, h->n, ptr<double>(h->Xrow), h->d, (long)h->n, NP,
                                    nullptr, nullptr, K, NP, 1, false, ptr<double>(h->Xrow), nullptr, nullptr)))
             return rc;
         gpk_kfix_kernel<<<(unsigned)((NP + 255) / 256), 256, 0, h->stream>>>(K, NP, h->n, (int)NP, diag_add,
@@ -1884,7 +1849,7 @@ int gpk_fit_begin(gpk_handle* h, double diag_add, double mean) {
         a.job_mode = JOBS_TABLE;
         a.status = ptr<int>(h->status);
         a.jobs = ptr<GemmJob>(h->jobs) + h->trsm32_r[k].off;
-        if ((rc = launch_gemm<EPI_STORE, 2>(h, h->mapK32, h->mapP, a, h->trsm32_r[k].cnt, nullptr, true))) return rc;
+        if ((rc = launch_gemm<EPI_STORE, 2>(h, h->mapK32, h->mapP, a, h->trsm32_r[k].cnt))) return rc;
         GemmArgs s;
         memset(&s, 0, sizeof(s));
         s.A = K; s.lda = NP;
@@ -1902,7 +1867,7 @@ int gpk_fit_begin(gpk_handle* h, double diag_add, double mean) {
             CK(cudaEventRecord(h->ev_panel[k], h->stream));                       // panel k solved
             if (k >= 1 && rest_recorded[k - 1]) CK(cudaStreamWaitEvent(h->stream, h->ev_rest[k - 1], 0));
             s.jobs = ptr<GemmJob>(h->jobs) + h->pu32_r[k].off;
-            if ((rc = launch_gemm<EPI_STORE, 2>(h, h->mapK32, h->mapK, s, h->pu32_r[k].cnt, nullptr, true))) return rc;
+            if ((rc = launch_gemm<EPI_STORE, 2>(h, h->mapK32, h->mapK, s, h->pu32_r[k].cnt))) return rc;
             const bool d2 = h->depth2 == 1 || (h->depth2 == 2 && nb >= 48);
             if (cnt > npu && !d2) {
                 CK(cudaStreamWaitEvent(h->side_stream, h->ev_panel[k], 0));
@@ -2018,12 +1983,10 @@ int gpk_fit_append(gpk_handle* h, const double* X, const double* y, int n, int d
     }
     // block row b of K (all columns), diagonal term, padding rows
     {
-        if (cov_tma(h)) {
-            if ((rc = ensure(h, h->Xts, (size_t)GPK_MAX_TERMS * NP * 8))) return rc;
-            if ((rc = build_cov_operand(h, h->stream, ptr<double>(h->Xrow), n, d, nullptr, nullptr, ptr<double>(h->Xts), NP)))
-                return rc;
-        }
-        if ((rc = launch_cov_tiles(h, h->stream, train_operand(h), NP, n, ptr<double>(h->Xrow) + (long)N1 * d, d,
+        if ((rc = ensure(h, h->Xts, (size_t)GPK_MAX_TERMS * NP * 8))) return rc;
+        if ((rc = build_cov_operand(h, h->stream, ptr<double>(h->Xrow), n, d, nullptr, nullptr, ptr<double>(h->Xts), NP)))
+            return rc;
+        if ((rc = launch_cov_tiles(h, h->stream, ptr<double>(h->Xts), NP, n, ptr<double>(h->Xrow) + (long)N1 * d, d,
                                    (long)(n - N1), BM, nullptr, nullptr, K + (long)N1 * NP, NP, 0, false,
                                    ptr<double>(h->Xrow), nullptr, nullptr)))
             return rc;
@@ -2331,7 +2294,7 @@ static int predict_cov_impl(gpk_handle* h, const double* Xs, long m, double* mu,
     bool grew = false;
     if ((rc = ensure(h, h->Vt, (size_t)mp * NP * 8, &grew))) return rc;
     if (grew || h->mapVt_rows != mp) {
-        if (h->loader != LOADER_CPASYNC && (rc = make_map(h, &h->mapVt, h->Vt.p, mp, NP, NP))) return rc;
+        if ((rc = make_map(h, &h->mapVt, h->Vt.p, mp, NP, NP))) return rc;
         h->mapVt_rows = mp;
     }
     if ((rc = ensure(h, h->cov, (size_t)mp * mp * 8))) return rc;
@@ -2341,7 +2304,7 @@ static int predict_cov_impl(gpk_handle* h, const double* Xs, long m, double* mu,
     const double* lo = h->has_bounds ? ptr<double>(h->lower) : nullptr;
     const double* up = h->has_bounds ? ptr<double>(h->upper) : nullptr;
     // K* (mp x NP)
-    if ((rc = launch_cov_tiles(h, h->stream, train_operand(h), NP, h->n, ptr<double>(h->cand), h->d, m, mp, lo, up,
+    if ((rc = launch_cov_tiles(h, h->stream, ptr<double>(h->Xts), NP, h->n, ptr<double>(h->cand), h->d, m, mp, lo, up,
                                ptr<double>(h->Kstar), NP, 0, false, ptr<double>(h->Xrow), nullptr, nullptr)))
         return rc;
     // K** (mp x mp): candidates against the (scaled, transposed) candidates
@@ -2423,7 +2386,7 @@ int gpk_predict_grad(gpk_handle* h, const double* Xs, long m, int kind, double e
     bool grew = false;
     if ((rc = ensure(h, h->Vt, (size_t)mp * NP * 8, &grew))) return rc;
     if (grew || h->mapVt_rows != mp) {
-        if (h->loader != LOADER_CPASYNC && (rc = make_map(h, &h->mapVt, h->Vt.p, mp, NP, NP))) return rc;
+        if ((rc = make_map(h, &h->mapVt, h->Vt.p, mp, NP, NP))) return rc;
         h->mapVt_rows = mp;
     }
     if ((rc = ensure(h, h->cov, (size_t)mp * NP * 8))) return rc;            // Wt = (K^-1 K*^T)^T
@@ -2441,7 +2404,7 @@ int gpk_predict_grad(gpk_handle* h, const double* Xs, long m, int kind, double e
     const double* up = h->has_bounds ? ptr<double>(h->upper) : nullptr;
     if ((rc = ensure_score_scratch(h, mp))) return rc;       // score_dev may have sized the K* map for a smaller chunk
     // K* again into the first buffer (score_dev may have used either), then Vt = (L^-1 K*^T)^T, Wt = (L^-T V)^T
-    if ((rc = launch_cov_tiles(h, h->stream, train_operand(h), NP, h->n, ptr<double>(h->cand), d, m, mp, lo, up,
+    if ((rc = launch_cov_tiles(h, h->stream, ptr<double>(h->Xts), NP, h->n, ptr<double>(h->cand), d, m, mp, lo, up,
                                ptr<double>(h->Kstar), NP, 0, false, ptr<double>(h->Xrow), nullptr, nullptr)))
         return rc;
     std::vector<GemmJob> jobs;

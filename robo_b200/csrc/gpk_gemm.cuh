@@ -5,41 +5,32 @@
 //   Cholesky trailing update A_ij -=  L_ik * L_jk^T                          (store, beta = 1)
 //   triangular inverse       T'   =  Q * L^T ;  R = -P * T'^T               (store C and C^T)
 //   predictive variance      V    =  L^-1 * K*^T  ->  sum_i V_ic^2 , sum_i V_ic z_i   (column reduce)
-// One CTA = one 128x128 output tile described by a GemmJob; 8 warps, each a 64x32 sub-tile of
-// m8n8k4 DMMA fragments (64 fp64 accumulators per thread).  Limitation on H100: m8n8k4 is Hopper's legacy fp64 MMA
-// shape and issues at about half of the fp64 tensor-core rate (measured with gpk_measure_fp64_peaks against cuBLAS
-// DGEMM, DESIGN.md section 5); the m16n8k{4,8,16} shapes are the way to the full rate.  Operand tiles (128 rows x 16 k,
-// 16 KB each) are staged through a 4-stage shared-memory ring either by
-//   LOADER_TMA     cp.async.bulk.tensor.2d + mbarrier complete_tx, 128B-swizzled (sm_90a)
-//   LOADER_CPASYNC cp.async.cg 16B with a padded (conflict-free) row stride
-// Both give bank-conflict-free 8-byte fragment loads (see frag_offsets()).
+// One CTA = one output tile described by a GemmJob; 8 DMMA warps, each a (TM/2)x32 sub-tile of m8n8k4 fragments.
+// Limitation on H100: m8n8k4 is Hopper's legacy fp64 MMA shape and issues at about half of the fp64 tensor-core rate
+// (measured with gpk_measure_fp64_peaks against cuBLAS DGEMM, DESIGN.md section 5); the m16n8k{4,8,16} shapes are the way
+// to the full rate.  Operand tiles (rows x 16 k) are staged by cp.async.bulk.tensor.2d + mbarrier complete_tx,
+// 128B-swizzled (sm_90a), which gives bank-conflict-free 8-byte fragment loads (see rowmap()).  Two kernels:
+//   gpk_gemm_ws_kernel   128 x 128 tiles (throughput): a dedicated producer warp issues the loads into a 4-stage ring
+//   gpk_gemm_nt_kernel   32 x 128 tiles (the latency-critical panel solve / next-panel update of the Cholesky chain,
+//                        launched with programmatic dependent launch): thread 0 issues every load up front
 #pragma once
 #include "gpk_internal.cuh"
 
-enum { LOADER_CPASYNC = 0, LOADER_TMA = 1, LOADER_TMA_WS = 2 };
 enum { EPI_STORE = 0, EPI_COLREDUCE = 1 };
 enum { JOBS_TABLE = 0, JOBS_VARIANCE = 1 };
 
 constexpr int BM = 128, BN = 128, BK = 16, NSTAGE = 4, GEMM_THREADS = 256;
 constexpr int VAR_GROUP = 16;                                    // candidate blocks per L2-resident group
-constexpr int PAD_STRIDE = 20;                                   // doubles per row, cp.async mode
 constexpr int STAGE_BYTES_TMA = (BM + BN) * BK * 8;              // 32768
-constexpr int STAGE_BYTES_PAD = (BM + BN) * PAD_STRIDE * 8;      // 40960
 constexpr int CT_STRIDE = 129;                                   // doubles per row of the epilogue staging tile
 constexpr int CT_BYTES = BM * CT_STRIDE * 8;                     // 132096
 constexpr int RING_TMA = NSTAGE * STAGE_BYTES_TMA > CT_BYTES ? NSTAGE * STAGE_BYTES_TMA : ((CT_BYTES + 1023) / 1024) * 1024;
-constexpr int RING_PAD = NSTAGE * STAGE_BYTES_PAD > CT_BYTES ? NSTAGE * STAGE_BYTES_PAD : ((CT_BYTES + 1023) / 1024) * 1024;
 constexpr int GEMM_SMEM_TMA = RING_TMA + 1024 /*align*/ + 64 /*barriers*/ + 2048 /*reduce*/;
-constexpr int GEMM_SMEM_PAD = RING_PAD + 1024 + 64 + 2048;
-// Tile height is a template parameter: MI = 8 -> 128 rows (throughput tiles), MI = 2 -> 32 rows (the
-// latency-critical panel solve / next-panel update of the Cholesky chain: 4x more CTAs, 1/4 the time each).
-// The 32-row chain tiles contract over K = 128 only (8 k-steps): their ring holds all 8 steps, so every operand
-// load is in flight before the first DMMA instead of trickling through a 4-deep ring (latency, not bandwidth).
-__host__ __device__ constexpr int gemm_nstage(int mi) { return mi <= 2 ? 8 : NSTAGE; }
-constexpr int gemm_smem_bytes(int loader, int mi) {
-    return mi == 8 ? (loader == LOADER_TMA ? GEMM_SMEM_TMA : GEMM_SMEM_PAD)
-                   : gemm_nstage(mi) * ((16 * mi + BN) * (loader == LOADER_TMA ? BK : PAD_STRIDE) * 8) + 1024 + 64 + 2048;
-}
+// The 32-row chain tiles contract over K = 128 only (8 k-steps): their ring holds all 8 steps, so every operand load is
+// in flight before the first DMMA instead of trickling through a 4-deep ring (latency, not bandwidth).
+constexpr int CHAIN_TM = 32, CHAIN_NSTAGE = 8;
+constexpr int CHAIN_RING = CHAIN_NSTAGE * (CHAIN_TM + BN) * BK * 8;
+constexpr int GEMM_SMEM_CHAIN = CHAIN_RING + 1024 /*align*/ + 64 /*barriers*/;
 
 struct GemmJob {
     int a_row;      // first row of the A tile
@@ -52,7 +43,7 @@ struct GemmJob {
 };
 
 struct GemmArgs {
-    const double* A; long lda;         // used by the cp.async loader (TMA uses the tensor maps)
+    const double* A; long lda;         // not read on the device: the kernels load through mapA / mapB
     const double* B; long ldb;
     double* C; long ldc;               // may be NULL
     double* Ct; long ldct;             // transposed copy of the output tile, may be NULL
@@ -83,13 +74,6 @@ __device__ __forceinline__ void sts64(uint32_t addr, double v) {
 __device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double b) {
     asm ("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
                  : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
-}
-__device__ __forceinline__ void cp_async16(uint32_t smem, const void* gmem) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" :: "r"(smem), "l"(gmem) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N> __device__ __forceinline__ void cp_async_wait() {
-    asm volatile("cp.async.wait_group %0;" :: "n"(N) : "memory");
 }
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(bar), "r"(count) : "memory");
@@ -129,21 +113,17 @@ __device__ __forceinline__ void fence_proxy_async() {
 // Which tile row feeds fragment row g (0..7) of an 8-row block.  With the 128B TMA swizzle the
 // 16-byte chunk index is XORed with (row & 7); mapping fragment rows {0,1,2,3 | 4,5,6,7} to tile
 // rows {0,2,4,6 | 1,3,5,7} makes the 16 lanes of each half-warp (4 rows x 4 k) hit 16 distinct
-// 8-byte banks.  The padded layout (stride 20 doubles) is conflict-free with the identity map.
-template <int LOADER> __device__ __forceinline__ int rowmap(int g) {
-    return LOADER == LOADER_TMA ? (((g & 3) << 1) | (g >> 2)) : g;
-}
+// 8-byte banks.
+__device__ __forceinline__ int rowmap(int g) { return ((g & 3) << 1) | (g >> 2); }
 
 // Byte offset inside an operand stage of element (row, k).
-template <int LOADER> __device__ __forceinline__ int tile_off(int row, int k) {
-    if (LOADER == LOADER_TMA) return row * 128 + ((((k >> 1) ^ (row & 7))) << 4) + ((k & 1) << 3);
-    return (row * PAD_STRIDE + k) * 8;
+__device__ __forceinline__ int tile_off(int row, int k) {
+    return row * 128 + ((((k >> 1) ^ (row & 7))) << 4) + ((k & 1) << 3);
 }
 
 // ---------------------------------------------------------------------------------------
-// the kernel: output tile (16*MI) x 128
+// 32 x 128 chain tile (EPI_STORE, job table)
 // ---------------------------------------------------------------------------------------
-template <int EPI, int LOADER, int MI>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gpk_gemm_nt_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
                    const GemmArgs g)
@@ -152,43 +132,23 @@ gpk_gemm_nt_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
     // start while the producing kernel drains; nothing is read before the dependency is resolved.
     cudaGridDependencySynchronize();
     if (g.status != nullptr && *g.status != 0) return;
-    static_assert(MI == 8 || MI == 2, "tile height 128 or 32");
-    static_assert(EPI == EPI_STORE || MI == 8, "column-reduce epilogue uses full tiles");
-    constexpr int TM = 16 * MI;                                          // tile rows (A rows)
-    constexpr int NS = gemm_nstage(MI);                                  // ring depth
-    constexpr int HM = TM / 2;                                           // rows per warp row-group
+    constexpr int MI = CHAIN_TM / 16;                                   // 8-row fragment blocks per warp
+    constexpr int TM = CHAIN_TM;                                        // tile rows (A rows)
+    constexpr int NS = CHAIN_NSTAGE;                                    // ring depth
+    constexpr int HM = TM / 2;                                          // rows per warp row-group
 
     extern __shared__ unsigned char smem_raw[];
     // all shared-memory traffic goes through 32-bit shared-window addresses (LDS/STS, not generic LD/ST)
     const uint32_t smem = (smem_u32(smem_raw) + 1023u) & ~1023u;        // 1024B alignment for the 128B swizzle
-    constexpr int ROWB = LOADER == LOADER_TMA ? BK * 8 : PAD_STRIDE * 8; // bytes per staged row
+    constexpr int ROWB = BK * 8;                                        // bytes per staged row
     constexpr int A_BYTES = TM * ROWB;
     constexpr int STAGE_BYTES = (TM + BN) * ROWB;
-    constexpr int RING_MIN = NS * STAGE_BYTES;
-    constexpr int CT_NEED = ((TM * CT_STRIDE * 8 + 1023) / 1024) * 1024;
-    constexpr int RING = MI == 8 ? (LOADER == LOADER_TMA ? RING_TMA : RING_PAD)
-                                 : RING_MIN;                            // (32-row tiles: CT tile fits the ring)
-    static_assert(RING >= CT_NEED, "epilogue staging tile must fit the operand ring");
-    const uint32_t full_bar = smem + RING;                              // NSTAGE x 8 bytes
-    const uint32_t red = smem + RING + 64;                              // 2 x 128 doubles
+    constexpr int RING = CHAIN_RING;
+    static_assert(RING == NS * STAGE_BYTES, "ring = NS stages");
+    static_assert(RING >= ((TM * CT_STRIDE * 8 + 1023) / 1024) * 1024, "epilogue staging tile must fit the operand ring");
+    const uint32_t full_bar = smem + RING;                              // NS x 8 bytes
 
-    // ---- job ----
-    GemmJob job;
-    if (g.job_mode == JOBS_TABLE) {
-        job = g.jobs[blockIdx.x];
-    } else {
-        // Candidate blocks are taken in groups of VAR_GROUP (16 blocks = 2048 candidates = 64 MB of
-        // K* at N = 4096, which stays L2-resident while the group walks all row-blocks of L^-1);
-        // inside a group the longest contractions (largest row-block) come first.
-        const int full = g.mcb / VAR_GROUP;
-        int id = (int)blockIdx.x, grp = id / (g.nb * VAR_GROUP), gsz = VAR_GROUP;
-        if (grp >= full) { grp = full; gsz = g.mcb - full * VAR_GROUP; }
-        id -= grp * g.nb * VAR_GROUP;
-        int ib = g.nb - 1 - id / gsz;
-        int cb = grp * VAR_GROUP + id % gsz;
-        job.a_row = ib * BM; job.b_row = cb * BN; job.k0 = 0; job.k1 = (ib + 1) * BM;
-        job.c_row = ib * BM; job.c_col = cb * BN; job.aux = ib; job.pad = 0;
-    }
+    const GemmJob job = g.jobs[blockIdx.x];
     const int KT = (job.k1 - job.k0) / BK;
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -197,47 +157,32 @@ gpk_gemm_nt_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
 
     // per-thread fragment offsets (bytes) inside a stage
     constexpr int BLK = 8 * ROWB;                                        // 8 tile rows
-    const int rA = wm * HM + rowmap<LOADER>(gq);
-    const int rB = wn * 32 + rowmap<LOADER>(gq);
+    const int rA = wm * HM + rowmap(gq);
+    const int rB = wn * 32 + rowmap(gq);
     int kxA[4], kxB[4];
 #pragma unroll
     for (int ks = 0; ks < 4; ++ks) {
-        kxA[ks] = tile_off<LOADER>(rA, ks * 4 + tq);
-        kxB[ks] = A_BYTES + tile_off<LOADER>(rB, ks * 4 + tq);
+        kxA[ks] = tile_off(rA, ks * 4 + tq);
+        kxB[ks] = A_BYTES + tile_off(rB, ks * 4 + tq);
     }
 
-    if (LOADER == LOADER_TMA) {
-        if (tid == 0) {
+    if (tid == 0) {
 #pragma unroll
-            for (int s = 0; s < NS; ++s) mbar_init(full_bar + 8 * s, 1);
-            fence_barrier_init();
-            fence_proxy_async();
-        }
-        __syncthreads();
+        for (int s = 0; s < NS; ++s) mbar_init(full_bar + 8 * s, 1);
+        fence_barrier_init();
+        fence_proxy_async();
     }
+    __syncthreads();
 
     auto issue_load = [&](int kt) {
         const int s = kt % NS;
         const uint32_t st = smem + s * STAGE_BYTES;
         const int kcol = job.k0 + kt * BK;
-        if (LOADER == LOADER_TMA) {
-            if (tid == 0) {
-                fence_proxy_async();
-                mbar_arrive_expect_tx(full_bar + 8 * s, STAGE_BYTES);
-                tma_load_2d(st, &mapA, kcol, job.a_row, full_bar + 8 * s);            // box TM rows x 16
-                tma_load_2d(st + A_BYTES, &mapB, kcol, job.b_row, full_bar + 8 * s);  // box 128 rows x 16
-            }
-        } else {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                int c = tid + i * GEMM_THREADS;          // 16-byte chunks, 8 per row
-                int row = c >> 3, kc = c & 7;
-                if (row < TM)
-                    cp_async16(st + (uint32_t)((row * PAD_STRIDE + kc * 2) * 8),
-                               g.A + (long)(job.a_row + row) * g.lda + kcol + kc * 2);
-                cp_async16(st + (uint32_t)(A_BYTES + (row * PAD_STRIDE + kc * 2) * 8),
-                           g.B + (long)(job.b_row + row) * g.ldb + kcol + kc * 2);
-            }
+        if (tid == 0) {
+            fence_proxy_async();
+            mbar_arrive_expect_tx(full_bar + 8 * s, STAGE_BYTES);
+            tma_load_2d(st, &mapA, kcol, job.a_row, full_bar + 8 * s);            // box TM rows x 16
+            tma_load_2d(st + A_BYTES, &mapB, kcol, job.b_row, full_bar + 8 * s);  // box 128 rows x 16
         }
     };
 
@@ -249,21 +194,19 @@ gpk_gemm_nt_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
 
     // ---- prologue ----
 #pragma unroll
-    for (int s = 0; s < NS - 1; ++s) {
+    for (int s = 0; s < NS - 1; ++s)
         if (s < KT) issue_load(s);
-        if (LOADER == LOADER_CPASYNC) cp_async_commit();
-    }
-    if (EPI == EPI_STORE && g.beta) {
+    if (g.beta) {
         // C_new = C_old + alpha * A B^T with alpha = +-1: start the accumulators at alpha * C_old; the
         // loads overlap the pipeline fill instead of sitting in the epilogue.
 #pragma unroll
         for (int mi = 0; mi < MI; ++mi) {
-            const long r = job.c_row + wm * HM + mi * 8 + rowmap<LOADER>(gq);
+            const long r = job.c_row + wm * HM + mi * 8 + rowmap(gq);
 #pragma unroll
             for (int ni = 0; ni < 4; ++ni)
 #pragma unroll
                 for (int j = 0; j < 2; ++j) {
-                    const long c = job.c_col + wn * 32 + ni * 8 + rowmap<LOADER>(2 * tq + j);
+                    const long c = job.c_col + wn * 32 + ni * 8 + rowmap(2 * tq + j);
                     acc[mi][ni][j] = g.alpha * g.C[r * g.ldc + c];
                 }
         }
@@ -272,15 +215,10 @@ gpk_gemm_nt_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
     // ---- main loop ----
     for (int kt = 0; kt < KT; ++kt) {
         const int s = kt % NS;
-        if (LOADER == LOADER_TMA) {
-            const uint32_t parity = (uint32_t)((kt / NS) & 1);
-            while (!mbar_try_wait(full_bar + 8 * s, parity)) { }
-        } else {
-            cp_async_wait<NS - 2>();
-        }
-        __syncthreads();          // stage s visible to all; everyone is done with stage (kt-1)%NSTAGE
+        const uint32_t parity = (uint32_t)((kt / NS) & 1);
+        while (!mbar_try_wait(full_bar + 8 * s, parity)) { }
+        __syncthreads();          // stage s visible to all; everyone is done with stage (kt-1)%NS
         if (kt + NS - 1 < KT) issue_load(kt + NS - 1);
-        if (LOADER == LOADER_CPASYNC) cp_async_commit();
 
         const uint32_t st = smem + s * STAGE_BYTES;
 #pragma unroll
@@ -296,95 +234,43 @@ gpk_gemm_nt_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
                 for (int ni = 0; ni < 4; ++ni) dmma884(acc[mi][ni][0], acc[mi][ni][1], a[mi], b[ni]);
         }
     }
-    if (LOADER == LOADER_CPASYNC) cp_async_wait<0>();
 
     // ---- epilogue ----
     // acc[mi][ni][j]  <->  tile row  wm*HM + mi*8 + rowmap(gq),  tile col  wn*32 + ni*8 + rowmap(2*tq + j)
-    if (EPI == EPI_STORE) {
-        // stage the tile through shared memory (the operand ring is free now) so that the global
-        // stores of C and of its transpose are fully coalesced
-        __syncthreads();
+    // stage the tile through shared memory (the operand ring is free now) so that the global
+    // stores of C and of its transpose are fully coalesced
+    __syncthreads();
 #pragma unroll
-        for (int mi = 0; mi < MI; ++mi) {
-            const int r = wm * HM + mi * 8 + rowmap<LOADER>(gq);
-#pragma unroll
-            for (int ni = 0; ni < 4; ++ni)
-#pragma unroll
-                for (int j = 0; j < 2; ++j) {
-                    const int c = wn * 32 + ni * 8 + rowmap<LOADER>(2 * tq + j);
-                    sts64(smem + 8 * (r * CT_STRIDE + c), g.alpha * acc[mi][ni][j]);
-                }
-        }
-        __syncthreads();
-        if (g.C) {
-            for (int e = tid; e < TM * BN; e += GEMM_THREADS) {
-                const int r = e >> 7, c = e & 127;
-                g.C[(long)(job.c_row + r) * g.ldc + job.c_col + c] = lds64(smem + 8 * (r * CT_STRIDE + c));
-            }
-        }
-        if (g.Ct) {
-            for (int e = tid; e < TM * BN; e += GEMM_THREADS) {
-                const int c = e / TM, r = e - c * TM;
-                g.Ct[(long)(job.c_col + c) * g.ldct + job.c_row + r] = lds64(smem + 8 * (r * CT_STRIDE + c));
-            }
-        }
-    } else {
-        // column reductions over the tile's 128 rows: sum v^2 and sum v * z[row]
-        double zr[MI];
-#pragma unroll
-        for (int mi = 0; mi < MI; ++mi) zr[mi] = g.z[job.c_row + wm * HM + mi * 8 + rowmap<LOADER>(gq)];
-        double ssq[4][2], smu[4][2];
+    for (int mi = 0; mi < MI; ++mi) {
+        const int r = wm * HM + mi * 8 + rowmap(gq);
 #pragma unroll
         for (int ni = 0; ni < 4; ++ni)
 #pragma unroll
             for (int j = 0; j < 2; ++j) {
-                double s2 = 0.0, sm = 0.0;
-#pragma unroll
-                for (int mi = 0; mi < MI; ++mi) {
-                    double v = acc[mi][ni][j];
-                    s2 = fma(v, v, s2);
-                    sm = fma(v, zr[mi], sm);
-                }
-                // reduce over the 8 lanes sharing tq (lane bits 2..4)
-#pragma unroll
-                for (int off = 4; off < 32; off <<= 1) {
-                    s2 += __shfl_xor_sync(0xffffffffu, s2, off);
-                    sm += __shfl_xor_sync(0xffffffffu, sm, off);
-                }
-                ssq[ni][j] = s2; smu[ni][j] = sm;
+                const int c = wn * 32 + ni * 8 + rowmap(2 * tq + j);
+                sts64(smem + 8 * (r * CT_STRIDE + c), g.alpha * acc[mi][ni][j]);
             }
-        // cross-warp (wm = 0,1) reduction through 'red' [2][128], ssq first, then mu
-        if (gq == 0) {
-#pragma unroll
-            for (int ni = 0; ni < 4; ++ni)
-#pragma unroll
-                for (int j = 0; j < 2; ++j)
-                    sts64(red + 8 * (wm * 128 + wn * 32 + ni * 8 + rowmap<LOADER>(2 * tq + j)), ssq[ni][j]);
+    }
+    __syncthreads();
+    if (g.C) {
+        for (int e = tid; e < TM * BN; e += GEMM_THREADS) {
+            const int r = e >> 7, c = e & 127;
+            g.C[(long)(job.c_row + r) * g.ldc + job.c_col + c] = lds64(smem + 8 * (r * CT_STRIDE + c));
         }
-        __syncthreads();
-        if (tid < 128)
-            g.part_ssq[(long)job.aux * g.ldpart + job.c_col + tid] = lds64(red + 8 * tid) + lds64(red + 8 * (128 + tid));
-        __syncthreads();
-        if (gq == 0) {
-#pragma unroll
-            for (int ni = 0; ni < 4; ++ni)
-#pragma unroll
-                for (int j = 0; j < 2; ++j)
-                    sts64(red + 8 * (wm * 128 + wn * 32 + ni * 8 + rowmap<LOADER>(2 * tq + j)), smu[ni][j]);
+    }
+    if (g.Ct) {
+        for (int e = tid; e < TM * BN; e += GEMM_THREADS) {
+            const int c = e / TM, r = e - c * TM;
+            g.Ct[(long)(job.c_col + c) * g.ldct + job.c_row + r] = lds64(smem + 8 * (r * CT_STRIDE + c));
         }
-        __syncthreads();
-        if (tid < 128)
-            g.part_mu[(long)job.aux * g.ldpart + job.c_col + tid] = lds64(red + 8 * tid) + lds64(red + 8 * (128 + tid));
     }
 }
 
 // ---------------------------------------------------------------------------------------
-// Warp-specialised variant of the 128 x 128 tile kernel (TMA staging only): warp 8 is a dedicated
-// producer (one elected lane issues the TMA loads), warps 0-7 are DMMA consumers.  Stage hand-over
-// uses a full/empty mbarrier pair per stage instead of a block-wide __syncthreads per k-step, so
-// consumer warps never rendezvous with each other inside the main loop and may drift by up to
-// NSTAGE-1 stages.  Same fragment layout, accumulation order and epilogues as gpk_gemm_nt_kernel
-// <EPI, LOADER_TMA, 8>: results are bit-identical.
+// 128 x 128 tile, warp-specialised: warp 8 is a dedicated producer (one elected lane issues the TMA
+// loads), warps 0-7 are DMMA consumers.  Stage hand-over uses a full/empty mbarrier pair per stage
+// instead of a block-wide __syncthreads per k-step, so consumer warps never rendezvous with each
+// other inside the main loop and may drift by up to NSTAGE-1 stages.
 // ---------------------------------------------------------------------------------------
 constexpr int WS_THREADS = GEMM_THREADS + 32;
 
@@ -394,7 +280,6 @@ gpk_gemm_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
                    const GemmArgs g)
 {
     if (g.status != nullptr && *g.status != 0) return;
-    constexpr int LOADER = LOADER_TMA;
     constexpr int MI = 8, TM = 128, HM = 64;
     extern __shared__ unsigned char smem_raw[];
     const uint32_t smem = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -454,13 +339,13 @@ gpk_gemm_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
     const int gq = lane >> 2, tq = lane & 3;
     const int wm = warp >> 2, wn = warp & 3;
     constexpr int BLK = 8 * ROWB;
-    const int rA = wm * HM + rowmap<LOADER>(gq);
-    const int rB = wn * 32 + rowmap<LOADER>(gq);
+    const int rA = wm * HM + rowmap(gq);
+    const int rB = wn * 32 + rowmap(gq);
     int kxA[4], kxB[4];
 #pragma unroll
     for (int ks = 0; ks < 4; ++ks) {
-        kxA[ks] = tile_off<LOADER>(rA, ks * 4 + tq);
-        kxB[ks] = A_BYTES + tile_off<LOADER>(rB, ks * 4 + tq);
+        kxA[ks] = tile_off(rA, ks * 4 + tq);
+        kxB[ks] = A_BYTES + tile_off(rB, ks * 4 + tq);
     }
     double acc[MI][4][2];
 #pragma unroll
@@ -470,12 +355,12 @@ gpk_gemm_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
     if (EPI == EPI_STORE && g.beta) {
 #pragma unroll
         for (int mi = 0; mi < MI; ++mi) {
-            const long r = job.c_row + wm * HM + mi * 8 + rowmap<LOADER>(gq);
+            const long r = job.c_row + wm * HM + mi * 8 + rowmap(gq);
 #pragma unroll
             for (int ni = 0; ni < 4; ++ni)
 #pragma unroll
                 for (int j = 0; j < 2; ++j) {
-                    const long c = job.c_col + wn * 32 + ni * 8 + rowmap<LOADER>(2 * tq + j);
+                    const long c = job.c_col + wn * 32 + ni * 8 + rowmap(2 * tq + j);
                     acc[mi][ni][j] = g.alpha * g.C[r * g.ldc + c];
                 }
         }
@@ -505,12 +390,12 @@ gpk_gemm_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
         named_bar_sync(1, GEMM_THREADS);                 // all consumers finished the ring
 #pragma unroll
         for (int mi = 0; mi < MI; ++mi) {
-            const int r = wm * HM + mi * 8 + rowmap<LOADER>(gq);
+            const int r = wm * HM + mi * 8 + rowmap(gq);
 #pragma unroll
             for (int ni = 0; ni < 4; ++ni)
 #pragma unroll
                 for (int j = 0; j < 2; ++j) {
-                    const int c = wn * 32 + ni * 8 + rowmap<LOADER>(2 * tq + j);
+                    const int c = wn * 32 + ni * 8 + rowmap(2 * tq + j);
                     sts64(smem + 8 * (r * CT_STRIDE + c), g.alpha * acc[mi][ni][j]);
                 }
         }
@@ -530,7 +415,7 @@ gpk_gemm_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
     } else {
         double zr[MI];
 #pragma unroll
-        for (int mi = 0; mi < MI; ++mi) zr[mi] = g.z[job.c_row + wm * HM + mi * 8 + rowmap<LOADER>(gq)];
+        for (int mi = 0; mi < MI; ++mi) zr[mi] = g.z[job.c_row + wm * HM + mi * 8 + rowmap(gq)];
         double ssq[4][2], smu[4][2];
 #pragma unroll
         for (int ni = 0; ni < 4; ++ni)
@@ -555,7 +440,7 @@ gpk_gemm_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
             for (int ni = 0; ni < 4; ++ni)
 #pragma unroll
                 for (int j = 0; j < 2; ++j)
-                    sts64(red + 8 * (wm * 128 + wn * 32 + ni * 8 + rowmap<LOADER>(2 * tq + j)), ssq[ni][j]);
+                    sts64(red + 8 * (wm * 128 + wn * 32 + ni * 8 + rowmap(2 * tq + j)), ssq[ni][j]);
         }
         named_bar_sync(1, GEMM_THREADS);
         if (tid < 128)
@@ -566,7 +451,7 @@ gpk_gemm_ws_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
             for (int ni = 0; ni < 4; ++ni)
 #pragma unroll
                 for (int j = 0; j < 2; ++j)
-                    sts64(red + 8 * (wm * 128 + wn * 32 + ni * 8 + rowmap<LOADER>(2 * tq + j)), smu[ni][j]);
+                    sts64(red + 8 * (wm * 128 + wn * 32 + ni * 8 + rowmap(2 * tq + j)), smu[ni][j]);
         }
         named_bar_sync(1, GEMM_THREADS);
         if (tid < 128)

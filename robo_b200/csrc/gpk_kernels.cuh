@@ -4,76 +4,15 @@
 
 // ---------------------------------------------------------------------------------------
 // Covariance tile builder.  out[c][j] = k(cand_c, train_j)   (row-major, ld = ldo)
-//   train points: transposed, column-contiguous  Xt[axis][j]  (coalesced across threads)
-//   candidates  : row-major raw inputs, optionally scaled (x - lower) / (upper - lower)
-// CTA = 128 train points x 32 candidates, 256 threads, 16 candidates per thread.
-// Rows c >= m and columns j >= n are written as exact zeros (padding must not contribute to
-// the contractions that follow).  tri != 0: skip tiles entirely above the diagonal (K build).
-// Used for K (cand = train), K* (scoring), K** (full_cov) and kernel.get_value.
-// ---------------------------------------------------------------------------------------
-template <int CPT>
-__global__ void __launch_bounds__(256, CPT == 16 ? 1 : 2)
-gpk_cov_kernel(const KSpec ks, const double* __restrict__ Xt, long ldx, int n,
-               const double* __restrict__ cand, int dc, long m,
-               const double* __restrict__ lower, const double* __restrict__ upper,
-               double* __restrict__ out, long ldo, int tri)
-{
-    // CPT candidates per thread: 16 (tile 128 x 32, standalone launches) or 8 (tile 128 x 16, ~60
-    // registers so that a CTA fits next to a resident variance-GEMM CTA when the two overlap)
-    constexpr int TC = 2 * CPT;
-    __shared__ double sc[TC][GPK_MAX_TERMS + 1];
-    const int tid = threadIdx.x;
-    const int j = blockIdx.x * 128 + (tid & 127);
-    const long c0 = (long)blockIdx.y * TC;
-    if (tri && (long)blockIdx.x * 128 > c0 + TC - 1) return;
-
-    const int nt = ks.n_terms;
-    for (int e = tid; e < TC * nt; e += 256) {
-        int c = e / nt, t = e - c * nt;
-        long ci = c0 + c;
-        double v = 0.0;
-        if (ci < m) {
-            int a = ks.axis[t];
-            v = cand[ci * dc + a];
-            if (lower != nullptr) v = (v - lower[a]) / (upper[a] - lower[a]);
-        }
-        sc[c][t] = v;
-    }
-    __syncthreads();
-
-    const int cg = (tid >> 7) * CPT;
-    const bool jv = j < n;
-    double r2[CPT], pr[CPT];
-#pragma unroll
-    for (int c = 0; c < CPT; ++c) { r2[c] = 0.0; pr[c] = 1.0; }
-    for (int t = 0; t < nt; ++t) {
-        const double xj = jv ? Xt[(long)ks.axis[t] * ldx + j] : 0.0;
-        const double im = ks.inv_metric[t];
-#pragma unroll
-        for (int c = 0; c < CPT; ++c) {
-            double d = sc[cg + c][t] - xj;
-            r2[c] = fma(d * d, im, r2[c]);
-        }
-        if (ks.last[t]) {
-#pragma unroll
-            for (int c = 0; c < CPT; ++c) { pr[c] *= gpk_radial(ks.family, r2[c]); r2[c] = 0.0; }
-        }
-    }
-#pragma unroll
-    for (int c = 0; c < CPT; ++c) {
-        long ci = c0 + cg + c;
-        out[ci * ldo + j] = (jv && ci < m) ? ks.amp * pr[c] : 0.0;
-    }
-}
-
-// ---------------------------------------------------------------------------------------
-// Covariance tile builder, TMA-staged (default).  Same contract as gpk_cov_kernel, other operand layout:
 //   train side : TERM-major, pre-scaled   Xs[t][j] = x_j[axis_t] * sqrt(c_f / metric_t)   (gpk_termmajor_kernel),
 //                one cp.async.bulk.tensor.2d (box n_terms x 128 columns, no swizzle) per CTA into shared memory,
 //                completion on an mbarrier; threads read their two train points with one 16-byte LDS per term
-//   candidates : row-major raw inputs, scaled (bounds, then the same per-term factor) while filling shared memory
-// so the inner loop is  d = s - x ; q = fma(d, d, q)  : 2 FP64 instructions per (pair, term) instead of 3, and one
-// broadcast LDS per CC pairs instead of one per pair (the old kernel was co-limited by the LSU).
+//   candidates : row-major raw inputs, scaled (x - lower) / (upper - lower), then by the same per-term factor, while
+//                filling shared memory
+// so the inner loop is  d = s - x ; q = fma(d, d, q)  : 2 FP64 instructions per (pair, term), and one broadcast LDS per
+// CC pairs.  Rows c >= m and columns j >= n are written as exact zeros (padding must not contribute to the contractions
+// that follow).  tri != 0: skip tiles entirely above the diagonal (K build).  Used for K (cand = train), K* (scoring),
+// K** (full_cov) and kernel.get_value.
 // CTA = 128 train points x 4 CC candidates, 256 threads, thread = 2 train points x CC candidates (CC = 8: 128 x 32 tile;
 // CC = 4: 128 x 16 tile, <= 64 registers so that a CTA fits next to a resident variance-GEMM CTA).
 // ---------------------------------------------------------------------------------------

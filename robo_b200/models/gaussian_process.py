@@ -6,7 +6,7 @@ unchanged.  What differs is where the arithmetic runs:
 
   reference (CPU)                                   here (GPU, libgpk.so)
   ------------------------------------------------  ------------------------------------------
-  george kernel.get_value: K build, 1 thread        gpk_cov_kernel (fused scaling + Matern/RBF)
+  george kernel.get_value: K build, 1 thread        gpk_cov_tma_kernel (fused scaling + Matern/RBF)
   scipy.linalg.cholesky + cho_solve (LAPACK)        blocked right-looking Cholesky, DMMA tiles,
                                                     forward solve fused as an extra block row
   gp.predict: full M x M covariance, then np.diag   fused K* -> L^-1 K*^T -> (mu, var), no M x M

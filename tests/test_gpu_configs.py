@@ -27,8 +27,7 @@ def _need_gpu():
     import torch
     if not torch.cuda.is_available():
         pytest.skip("no CUDA device")
-    for k in ("GPK_LOADER", "GPK_CHUNK"):
-        os.environ.pop(k, None)
+    os.environ.pop("GPK_CHUNK", None)
 
 
 def _diag_add(noise):

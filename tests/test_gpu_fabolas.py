@@ -235,9 +235,9 @@ def test_fabolas_end_to_end_device_samplers():
     assert np.array_equal(np.array(r1["X"]), np.array(r2["X"]))
 
 
-@pytest.mark.parametrize("opts", [{"chunk": 1024}, {"loader": 0}])
+@pytest.mark.parametrize("opts", [{"chunk": 1024}])
 def test_moments_other_scoring_paths(opts):
-    """Several pipelined chunks (side-stream builder, per-chunk prior variance) and the cp.async builder."""
+    """Several pipelined chunks (side-stream builder, per-chunk prior variance)."""
     from robo_b200 import _lib
     X, y = _problem(300, seed=21)
     bounds = (np.array([-1.0, 0.0, 0.0]), np.array([2.0, 3.0, 1.0]))

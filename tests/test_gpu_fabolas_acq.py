@@ -124,14 +124,6 @@ def test_predict_mean_close_to_fp64_predict(m, ozaki):
     assert np.max(np.abs(got - mu)) <= 1e-10 * scale
 
 
-def test_predict_mean_needs_tma_loader():
-    _, cost, X = _pair()
-    h = cost.gp.handle
-    h.set_option("loader", 0)
-    with pytest.raises(ValueError):
-        h.predict_mean(cost.normalize(X[:4]))
-
-
 # ---- one pair --------------------------------------------------------------------------------------------------
 def test_single_pair_dh_bit_identical_with_zero_cost():
     obj, cost, X = _pair(zero_cost=True)

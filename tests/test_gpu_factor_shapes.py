@@ -44,12 +44,6 @@ def _need_gpu():
         pytest.skip("no CUDA device")
 
 
-@pytest.fixture(params=["tma", "cpasync", "tma_ws"])
-def loader(request, monkeypatch):
-    monkeypatch.setenv("GPK_LOADER", {"cpasync": "0", "tma": "1", "tma_ws": "2"}[request.param])
-    return request.param
-
-
 def gemm(A, B):
     import torch
     a = torch.from_numpy(np.ascontiguousarray(A, dtype=np.float64)).cuda()
@@ -217,9 +211,9 @@ def test_fit_kernel_cases(kind, case):
 
 
 @pytest.mark.parametrize("kind", KINDS)
-def test_fit_loaders(kind, loader):
+def test_fit_matern32(kind):
     X, y = data(kind, "m32", 1153)
-    fit_and_check("%s m32 N=1153 %s" % (kind, loader), flat_of(kind, "m32"), X, y)[0].close()
+    fit_and_check("%s m32 N=1153" % kind, flat_of(kind, "m32"), X, y)[0].close()
 
 
 ILL = [("env", dict(env=(-6.0, 6.0), zclust=True)), ("env", dict(env=(-2.0, 9.5), zclust=True)),
@@ -343,12 +337,6 @@ def candidates(kind, m, X, seed, bounds=None):
     return Xs
 
 
-def mean_only_builder():
-    """gpk_predict_mean needs the TMA covariance builder: not under GPK_LOADER=0 (cp.async)"""
-    import os
-    return os.environ.get("GPK_LOADER", "1") != "0"
-
-
 def scaled(Xs, bounds):
     return Xs if bounds is None else (Xs - bounds[0]) / (bounds[1] - bounds[0])
 
@@ -403,12 +391,11 @@ def test_posterior_cov(kind, m, transform):
     r, bad = ER.sigma_check(var, np.diag(ref["cov"]), np.diag(ref["cov_bound"]) + ev * ys2)
     assert not bad.any()
     report("pred_var", tag, r)
-    if mean_only_builder():
-        report("mean_only", tag, R.ratio(np.abs(h.predict_mean(Xs) - ref["mu"]), mb))
+    report("mean_only", tag, R.ratio(np.abs(h.predict_mean(Xs) - ref["mu"]), mb))
     h.close()
 
 
-@pytest.mark.parametrize("opts", [{}, {"chunk": 1024}, {"loader": 0}])
+@pytest.mark.parametrize("opts", [{}, {"chunk": 1024}])
 @pytest.mark.parametrize("kind", ["env", "env_bounds", "task"])
 def test_predict_many_candidates(kind, opts):
     """m > 2048 rows: several pipelined chunks with chunk < m, and candidate counts that stride the factor kernel's grid"""
@@ -445,8 +432,7 @@ def test_predict_many_candidates(kind, opts):
     r, bad = ER.sigma_check(var, ref["cov"], ref["cov_bound"] + ev * 1.9 ** 2)
     assert not bad.any()
     report("pred_var", tag, r)
-    if "loader" not in opts and mean_only_builder():
-        report("mean_only", tag, R.ratio(np.abs(h.predict_mean(Xs) - ref["mu"]), ref["mu_bound"] + em * 1.9))
+    report("mean_only", tag, R.ratio(np.abs(h.predict_mean(Xs) - ref["mu"]), ref["mu_bound"] + em * 1.9))
     h.close()
 
 

@@ -44,13 +44,6 @@ def _need_gpu():
         pytest.skip("no CUDA device")
 
 
-@pytest.fixture(params=["tma", "cpasync", "tma_ws"])
-def loader(request, monkeypatch):
-    """operand staging of the GEMM tile engine (read by every new Handle)"""
-    monkeypatch.setenv("GPK_LOADER", {"cpasync": "0", "tma": "1", "tma_ws": "2"}[request.param])
-    return request.param
-
-
 def gemm(A, B):
     import torch
     a = torch.from_numpy(np.ascontiguousarray(A, dtype=np.float64)).cuda()
@@ -134,7 +127,7 @@ def test_fit_shapes(N):
     h, s, mean = fit_and_check("m52 N=%d" % N, flat_of("m52"), X, y)
     if N > 1:                               # alpha through the posterior mean: mu - mean = K* X^T z
         Xs = np.random.RandomState(N).rand(64, X.shape[1])
-        mu = h.predict(Xs)[0]                # gpk_predict: every loader (gpk_predict_mean needs the TMA builder)
+        mu = h.predict(Xs)[0]
         ref = R.cov_reference(s["X"], device_K(flat_of("m52"), Xs, X), device_K(flat_of("m52"), Xs), s["z"], mean,
                               gemm=gemm)
         report("mean_alpha", "m52 N=%d" % N, R.ratio(np.abs(mu - ref["mu"]), ref["mu_bound"]))
@@ -149,9 +142,9 @@ def test_fit_kernel_cases(case, N):
 
 
 @pytest.mark.parametrize("N", [257, 1153])
-def test_fit_loaders(N, loader):
+def test_fit_matern32(N):
     X, y = raw_data("m32", N)
-    fit_and_check("m32 N=%d %s" % (N, loader), flat_of("m32"), X, y)[0].close()
+    fit_and_check("m32 N=%d" % N, flat_of("m32"), X, y)[0].close()
 
 
 @pytest.mark.parametrize("diag_add", [1e-6, 1e-9, G.TINY])

@@ -28,8 +28,8 @@ pytestmark = pytest.mark.gpu
 
 EPS = np.finfo(np.float64).eps
 CASE_PARAMS = [pytest.param(c, v, id="%s-%s" % (c, v)) for c in KC.CASES for v in KC.VARIANTS]
-# the int8 contraction is off under GPK_OZAKI=0 and needs TMA staging (GPK_LOADER=0 selects cp.async: fp64 contraction)
-OZAKI_OFF = os.environ.get("GPK_OZAKI") == "0" or os.environ.get("GPK_LOADER") == "0"
+# the int8 contraction is off under GPK_OZAKI=0
+OZAKI_OFF = os.environ.get("GPK_OZAKI") == "0"
 
 
 @pytest.fixture(scope="module", autouse=True)

@@ -1,4 +1,4 @@
-"""Small end-to-end pass over every kernel (all staging variants) for compute-sanitizer runs."""
+"""Small end-to-end pass over every kernel for compute-sanitizer runs."""
 import os, sys
 import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -10,29 +10,27 @@ rng = np.random.RandomState(0)
 N, D, M = 300, 3, 700
 X, y, Xs = rng.rand(N, D), rng.rand(N), rng.rand(M, D)
 f = K.Product(K.ConstantKernel(0.1, ndim=D), K.Matern52Kernel(np.array([0.3, 0.5, 0.8]), ndim=D)).flatten()
-for loader in (2, 1, 0):
-    h = _lib.Handle(0)
-    h.set_option("loader", loader)
-    h.set_option("chunk", 256)
-    h.set_data(X, y)
-    h.set_input_bounds(np.zeros(D), np.ones(D))
-    h.set_output_transform(True, 0.5, 2.0)
-    h.set_kernel(f["family"], f["log_amp"], f["axis"], f["group"], f["log_metric"])
-    print("loader", loader, "fit", h.fit(1e-3 + 1.25e-12, float(y.mean())))
-    r = h.acq(Xs, _lib.ACQ_EI, float(y.min()), 0.0, want_values=True, want_moments=True)
-    print(" acq best", r["best_idx"], r["best_val"], "neg", r["n_negative"])
-    for kind in (_lib.ACQ_LOG_EI, _lib.ACQ_PI, _lib.ACQ_LCB):
-        h.acq(Xs[:300], kind, float(y.min()), 0.1)
-    mu, cov = h.predict_cov(Xs[:150])
-    g = h.nll_grad(1e-3, D)
-    pg = h.predict_grad(Xs[:5], _lib.ACQ_EI, float(y.min()), 0.0)
-    bx, bv, bi = h.maximize_random(7, 0, 1000, 700, np.zeros(D), np.ones(D), X[0], 0.1, _lib.ACQ_EI, float(y.min()), 0.0)
-    km = h.kernel_matrix(Xs[:40], X[:50])
-    print(" cov", cov.shape, "grad", np.round(g, 3), "dmu", pg["dmu"].shape, "max idx", bi, km.shape)
-    # incremental refit: 300 -> 310 rows inside the last 128-row block (NP = 384)
-    X2, y2 = np.vstack([X, rng.rand(10, D)]), np.concatenate([y, rng.rand(10)])
-    print(" append", h.fit_append(X2, y2, 1e-3 + 1.25e-12, float(y2.mean())), h.predict(Xs[:64])[0][:2])
-    h.close()
+h = _lib.Handle(0)
+h.set_option("chunk", 256)
+h.set_data(X, y)
+h.set_input_bounds(np.zeros(D), np.ones(D))
+h.set_output_transform(True, 0.5, 2.0)
+h.set_kernel(f["family"], f["log_amp"], f["axis"], f["group"], f["log_metric"])
+print("fit", h.fit(1e-3 + 1.25e-12, float(y.mean())))
+r = h.acq(Xs, _lib.ACQ_EI, float(y.min()), 0.0, want_values=True, want_moments=True)
+print(" acq best", r["best_idx"], r["best_val"], "neg", r["n_negative"])
+for kind in (_lib.ACQ_LOG_EI, _lib.ACQ_PI, _lib.ACQ_LCB):
+    h.acq(Xs[:300], kind, float(y.min()), 0.1)
+mu, cov = h.predict_cov(Xs[:150])
+g = h.nll_grad(1e-3, D)
+pg = h.predict_grad(Xs[:5], _lib.ACQ_EI, float(y.min()), 0.0)
+bx, bv, bi = h.maximize_random(7, 0, 1000, 700, np.zeros(D), np.ones(D), X[0], 0.1, _lib.ACQ_EI, float(y.min()), 0.0)
+km = h.kernel_matrix(Xs[:40], X[:50])
+print(" cov", cov.shape, "grad", np.round(g, 3), "dmu", pg["dmu"].shape, "max idx", bi, km.shape)
+# incremental refit: 300 -> 310 rows inside the last 128-row block (NP = 384)
+X2, y2 = np.vstack([X, rng.rand(10, D)]), np.concatenate([y, rng.rand(10)])
+print(" append", h.fit_append(X2, y2, 1e-3 + 1.25e-12, float(y2.mean())), h.predict(Xs[:64])[0][:2])
+h.close()
 # round-2 kernels: int8 contraction (digit builder, several chunks), depth-2 trailing updates, fused multi-model
 # scoring, raw posterior covariance
 Xb = rng.rand(2304, D)
