@@ -11,6 +11,7 @@ from robo_b200 import _lib
 from robo_b200.models.bayesian_linear_regression import (BayesianLinearRegression, linear_basis_func,
                                                          quadratic_basis_func)
 from tests import blr_model as BM
+from tests import blr_reference
 
 pytestmark = pytest.mark.gpu
 
@@ -95,19 +96,31 @@ def test_reference_unit_test_data():
     np.testing.assert_allclose(m.marginal_log_likelihood(np.array([0.0, np.log(1000)])), G["unit_mll"], rtol=1e-9)
 
 
-@pytest.mark.parametrize("name,steps", [("lin", 40), ("quad", 25), ("none", 25)])
-def test_sample_bit_for_bit_and_deterministic(name, steps):
-    h = _handle(G[name + "_X"], G[name + "_y"], BASES[name])
-    p0 = np.column_stack([-9.0 + 0.2 * np.random.RandomState(1).randn(12), 2.0 + np.random.RandomState(2).rand(12)])
+@pytest.mark.parametrize("name,steps,D,N,nw", [
+    ("lin", 40, None, None, 12), ("quad", 25, None, None, 12), ("none", 25, None, None, 12),
+    ("lin", 6, 33, 257, 4), ("none", 4, 64, 4097, 202), ("quad", 5, 31, 4097, 4), ("lin", 3, 63, 129, 202),
+    ("none", 0, 34, 257, 12)], ids=["lin-40", "quad-25", "none-25", "F34-N257-nw4", "F64-N4097-nw202", "F63-N4097-nw4",
+                                  "F64-N129-nw202", "F34-N257-steps0"])
+def test_sample_bit_for_bit_and_deterministic(name, steps, D, N, nw):
+    """The golden sets (F <= 7, N <= 50), and F = 34 and 64, N = 257 and 4097, nwalkers 4 (the least) and 202, steps 0
+    (the initial log-posteriors only)."""
+    if D is None:
+        X, y = G[name + "_X"], G[name + "_y"]
+    else:
+        X, y, _ = blr_reference.case(BASES[name], D, N)
+    h = _handle(X, y, BASES[name])
+    p0 = np.column_stack([-9.0 + 0.2 * np.random.RandomState(1).randn(nw), 2.0 + np.random.RandomState(2).rand(nw)])
     seed = 0x1234ABCD5678
     r = _lib.blr_sample(h, seed, p0, steps)
     ref = BM.run(lambda T: _lib.blr_lnpost(h, T), p0, steps, seed)
     assert np.array_equal(r["pos"].view(np.int64), ref["pos"].view(np.int64))
     assert np.array_equal(r["lnpost"].view(np.int64), ref["lnpost"].view(np.int64))
     assert np.array_equal(r["n_accepted"], ref["n_accepted"])
-    assert r["n_accepted"].sum() > 0
-    r2 = _lib.blr_sample(_handle(G[name + "_X"], G[name + "_y"], BASES[name]), seed, p0, steps)
+    assert (r["n_accepted"].sum() > 0) == (steps > 0)
+    r2 = _lib.blr_sample(_handle(X, y, BASES[name]), seed, p0, steps)
     assert np.array_equal(r2["pos"].view(np.int64), r["pos"].view(np.int64))
+    if steps == 0:
+        assert np.array_equal(r["pos"], p0)
 
 
 def test_chain_agrees_in_law_with_the_reference():
