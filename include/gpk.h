@@ -875,6 +875,53 @@ int gpk_bnn_set_samples(gpk_handle* h, int S, const double* samples);
 int gpk_bnn_get_state(gpk_handle* h, double* theta, double* p, double* tau, double* g, double* vhat);
 int gpk_bnn_draws(gpk_handle* h, unsigned long long seed, unsigned counter, int step0, int ns, double* Z);
 
+/* ---- DNGO on the device (robo_b200/csrc/gpk_dngo.cuh) ------------------------------------------------------------
+ * pybnn's DNGO (robo/fmin/bayesian_optimization.py:105-109), restated (pybnn's source is not available): a D -> 50 -> 50
+ * -> 50 -> 1 tanh network trained by Adam on minibatches, then Bayesian linear regression over its last hidden layer
+ * (the 50 features Theta) with the BLR entry points' log-posterior, sampler and weight posteriors.  gpk_dngo.cuh states
+ * every step and its order; tests/dngo_model.py restates them and the device training equals it bit for bit.  A handle
+ * becomes a DNGO handle with gpk_dngo_set_data and stays one: the Gaussian-process, RF and BNN entry points,
+ * gpk_blr_set_data and gpk_blr_fit return GPK_BAD_ARG with a message naming the model kind, and the DNGO entry points
+ * refuse the other kinds.  gpk_blr_lnpost, gpk_blr_sample, gpk_blr_get_models and gpk_blr_dims serve a trained DNGO
+ * handle's regression (F = 50, basis none, on the scaled y).  The scoring entry points (as for an RF handle) score a
+ * fitted DNGO handle through its predictive pass. */
+#define GPK_DNGO_MAX_D 64        /* most input dimensions */
+#define GPK_DNGO_MAX_N 4096      /* most training points: the training kernel keeps an epoch's order (12 bytes a row) in
+                                    shared memory beside theta, its gradient and the batch's activations */
+#define GPK_DNGO_MAX_BATCH 16    /* largest batch, min(batch, n) */
+/* gpk_dngo_set_data: X (n x d) and y (n) as train() receives them.  With normalize_input / normalize_output, each column
+ *   of X / y is scaled to zero mean and unit population std on the host (gpk_bnn_set_data's code); otherwise that side
+ *   is used as given.  prior_par as gpk_blr_set_data's.  Drops the net and the fit.  GPK_BAD_ARG: n < 2 with a flag on,
+ *   a constant column or a constant y under its flag, n > GPK_DNGO_MAX_N, d > GPK_DNGO_MAX_D, a non-finite entry, a
+ *   handle holding another model kind.
+ * gpk_dngo_train: a fresh net trained for `epochs` epochs of floor(n / B) Adam steps (B = min(batch, n); the remaining
+ *   rows of each epoch are dropped) at learning rate lr, in one launch; then Theta and the regression's Theta^T Theta and
+ *   Theta^T y.  The initial weights and the epoch orders are Philox4x32-10 keyed by seed with `counter` in their counter:
+ *   a caller advances it once per train.  Drops the fit.  GPK_BAD_ARG: lr not finite and > 0, batch < 1, epochs < 1,
+ *   B > GPK_DNGO_MAX_BATCH.
+ * gpk_dngo_fit: the BLR weight posteriors of hypers (k x 2, as gpk_blr_fit), then the collapsed predictive: m_bar = mean
+ *   m_i, Q = mean S_i + (1 / k) sum (m_i - m_bar)(m_i - m_bar)^T, its Cholesky factor R and c_bar = mean 1 / beta_i.
+ *   GPK_NOT_PD as gpk_blr_fit, or when Q's factorisation fails.
+ * gpk_dngo_dims: n, d, the parameters of the net P = 50 d + 5201 and the fit's k (0 before a fit).
+ * gpk_dngo_get_net: the trained net (P, gpk_dngo.cuh's parameter order).
+ * gpk_dngo_set_net: a net back onto a DNGO handle that holds the training set (a pickled or copied model); Theta and the
+ *   regression's products are rebuilt from it, bit for bit as gpk_dngo_train built them.  Drops the fit and the Adam
+ *   state.
+ * gpk_dngo_features: Theta (m x 50) of the m rows X (m x d, scaled as candidates are), the training pass's arithmetic.
+ * gpk_dngo_get_state: Adam's final m and v (P each; either may be NULL) and its step count t of the last train.
+ * The predictive pass: at features phi, m = phi^T m_bar and v = c_bar + ||R^T phi||^2 (the mixture of the k posteriors'
+ * mean and full variance), v clipped to DBL_EPSILON, then m y_std + y_mean and v y_std^2.  The acquisition closed form of
+ * gpk_acq_moments follows. */
+int gpk_dngo_set_data(gpk_handle* h, const double* X, const double* y, int n, int d, int normalize_input,
+                      int normalize_output, const double* prior_par);
+int gpk_dngo_train(gpk_handle* h, unsigned long long seed, unsigned counter, double lr, int batch, int epochs);
+int gpk_dngo_fit(gpk_handle* h, const double* hypers, int k);
+int gpk_dngo_dims(gpk_handle* h, int* n, int* d, int* P, int* k);
+int gpk_dngo_get_net(gpk_handle* h, double* net);
+int gpk_dngo_set_net(gpk_handle* h, const double* net);
+int gpk_dngo_features(gpk_handle* h, const double* X, long m, double* out);
+int gpk_dngo_get_state(gpk_handle* h, double* m, double* v, long long* t);
+
 /* kernel.get_value(X1, X2) (test/test_models/test_gaussian_process.py:44-46) with the
  * handle's current kernel; no input scaling.  out is (n1, n2) row-major. */
 int gpk_kernel_matrix(gpk_handle* h, const double* X1, long n1, const double* X2, long n2,

@@ -32,6 +32,8 @@ BLR_LINEAR, BLR_QUADRATIC, BLR_NONE = range(3)  # gpk_blr_basis: the features of
 BLR_MAX_F = 64                                 # GPK_BLR_MAX_F: most features of a BayesianLinearRegression handle
 RF_MAX_N, RF_MAX_D, RF_MAX_T = 16384, 64, 512  # GPK_RF_MAX_N / GPK_RF_MAX_D / GPK_RF_MAX_T: the largest forest
 BNN_MAX_N, BNN_MAX_D, BNN_MAX_BATCH = 4096, 64, 32   # GPK_BNN_MAX_N / GPK_BNN_MAX_D / GPK_BNN_MAX_BATCH
+DNGO_MAX_N, DNGO_MAX_D, DNGO_MAX_BATCH = 4096, 64, 16   # GPK_DNGO_MAX_N / GPK_DNGO_MAX_D / GPK_DNGO_MAX_BATCH
+DNGO_H = 50                                    # units per hidden layer of a DNGO net: the features per row
 CMA_MAX_D, CMA_MAX_LAMBDA, CMA_HIST = 64, 2048, 160   # GPK_CMA_MAX_D / GPK_CMA_MAX_LAMBDA / GPK_CMA_HIST
 CMA_C_W = 20                                   # GPK_CMA_C_W: where a run's weights start in its constant row
 CMA_NCONST = CMA_C_W + CMA_MAX_LAMBDA // 2     # GPK_CMA_NCONST: doubles per run in the constant table
@@ -178,6 +180,14 @@ _SIGNATURES = {
     "gpk_bnn_set_samples": [_vp, C.c_int, _dp],
     "gpk_bnn_get_state": [_vp, _dp, _dp, _dp, _dp, _dp],
     "gpk_bnn_draws": [_vp, C.c_ulonglong, C.c_uint, C.c_int, C.c_int, _dp],
+    "gpk_dngo_set_data": [_vp, _dp, _dp, C.c_int, C.c_int, C.c_int, C.c_int, _dp],
+    "gpk_dngo_train": [_vp, C.c_ulonglong, C.c_uint, C.c_double, C.c_int, C.c_int],
+    "gpk_dngo_fit": [_vp, _dp, C.c_int],
+    "gpk_dngo_dims": [_vp, _ip, _ip, _ip, _ip],
+    "gpk_dngo_get_net": [_vp, _dp],
+    "gpk_dngo_set_net": [_vp, _dp],
+    "gpk_dngo_features": [_vp, _dp, C.c_long, _dp],
+    "gpk_dngo_get_state": [_vp, _dp, _dp, C.POINTER(C.c_longlong)],
     "gpk_get_timings": [_vp, _dp],
     "gpk_get_diag_profile": [_vp, C.POINTER(C.c_longlong)],
 }
@@ -1469,6 +1479,77 @@ def bnn_draws(handle, seed, counter, step0, ns):
     handle._check(handle.lib.gpk_bnn_draws(handle._h, int(seed) & 0xFFFFFFFFFFFFFFFF, int(counter) & 0xFFFFFFFF,
                                            int(step0), int(ns), _as_dp(Z)))
     return Z
+
+
+def dngo_params(n_dims):
+    """P, the parameters of the net of a DNGO handle on n_dims inputs."""
+    return 50 * int(n_dims) + 5201
+
+
+def dngo_set_data(handle, X, y, normalize_input, normalize_output, prior_par):
+    """gpk_dngo_set_data: the training set on the handle (normalised there under the flags), which becomes a DNGO
+    handle; prior_par = (lognormal sigma, lognormal mean, horseshoe scale) of its Bayesian linear regression."""
+    X, y, par = f64(X), f64(y).ravel(), f64(prior_par).ravel()
+    if X.ndim != 2 or X.shape[0] != y.size:
+        raise ValueError("dngo_set_data: X must be (n, d) and y (n,)")
+    if par.size != 3:
+        raise ValueError("dngo_set_data: the prior needs 3 constants")
+    n, d = X.shape
+    handle._check(handle.lib.gpk_dngo_set_data(handle._h, _as_dp(X), _as_dp(y), n, d, int(bool(normalize_input)),
+                                               int(bool(normalize_output)), _as_dp(par)))
+
+
+def dngo_train(handle, seed, counter, lr, batch, epochs):
+    """gpk_dngo_train: train a fresh net by Adam in one launch (draws keyed by seed and the train counter), then the
+    features and the regression's products."""
+    handle._check(handle.lib.gpk_dngo_train(handle._h, int(seed) & 0xFFFFFFFFFFFFFFFF, int(counter) & 0xFFFFFFFF,
+                                            float(lr), int(batch), int(epochs)))
+
+
+def dngo_fit(handle, hypers):
+    """gpk_dngo_fit: the weight posteriors of the (alpha, beta) rows of hypers and the collapsed predictive."""
+    H = f64(np.atleast_2d(hypers))
+    if H.ndim != 2 or H.shape[1] != 2:
+        raise ValueError("dngo_fit: hypers must have shape (k, 2)")
+    handle._check(handle.lib.gpk_dngo_fit(handle._h, _as_dp(H), H.shape[0]))
+
+
+def dngo_dims(handle):
+    """gpk_dngo_dims -> (n, d, P, k)."""
+    n, d, P, k = C.c_int(), C.c_int(), C.c_int(), C.c_int()
+    handle._check(handle.lib.gpk_dngo_dims(handle._h, C.byref(n), C.byref(d), C.byref(P), C.byref(k)))
+    return n.value, d.value, P.value, k.value
+
+
+def dngo_net(handle):
+    """gpk_dngo_get_net: the (P,) trained net."""
+    out = np.empty(dngo_dims(handle)[2])
+    handle._check(handle.lib.gpk_dngo_get_net(handle._h, _as_dp(out)))
+    return out
+
+
+def dngo_set_net(handle, net):
+    """gpk_dngo_set_net: the net of dngo_net back onto a handle that holds the same training set."""
+    w = f64(net).ravel()
+    if w.size != dngo_dims(handle)[2]:
+        raise ValueError("dngo_set_net: the net must have P entries")
+    handle._check(handle.lib.gpk_dngo_set_net(handle._h, _as_dp(w)))
+
+
+def dngo_features(handle, X):
+    """gpk_dngo_features: the (m, 50) features of the rows X (m, d)."""
+    X = f64(np.atleast_2d(X))
+    out = np.empty((X.shape[0], DNGO_H))
+    handle._check(handle.lib.gpk_dngo_features(handle._h, _as_dp(X), X.shape[0], _as_dp(out)))
+    return out
+
+
+def dngo_state(handle):
+    """gpk_dngo_get_state -> dict(m, v (P each), t) of Adam after the last train."""
+    P = dngo_dims(handle)[2]
+    m, v, t = np.empty(P), np.empty(P), C.c_longlong()
+    handle._check(handle.lib.gpk_dngo_get_state(handle._h, _as_dp(m), _as_dp(v), C.byref(t)))
+    return dict(m=m, v=v, t=t.value)
 
 
 _moments_handle = {}

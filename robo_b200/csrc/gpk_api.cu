@@ -36,6 +36,7 @@
 #include "gpk_blr.cuh"
 #include "gpk_rf.cuh"
 #include "gpk_bnn.cuh"
+#include "gpk_dngo.cuh"
 
 namespace {
 
@@ -49,7 +50,7 @@ struct DevBuf {
 };
 
 // the model a handle holds: a Gaussian process unless a gpk_*_set_data made it a surrogate, which it stays for life
-enum ModelKind { MODEL_GP, MODEL_BLR, MODEL_RF, MODEL_BNN };
+enum ModelKind { MODEL_GP, MODEL_BLR, MODEL_RF, MODEL_BNN, MODEL_DNGO };
 
 }  // namespace
 
@@ -186,11 +187,18 @@ struct gpk_handle {
     int rf_T = 0, rf_total = 0;
     DevBuf rf_data, rf_work, rf_nodes;
     // Bayesian neural network (gpk_bnn.cuh, gpk_bnn_set_data).  bnn_data: the scaled X (n x d), y (n), the input mean
-    // and std (d each); bnn_samples: the kept networks (S x P); bnn_state: the chain's final theta, p, tau, g, vhat
-    // (P each)
+    // and std (d each), with the y statistics in bnn_ymean / bnn_ystd (a DNGO handle keeps its training set there too);
+    // bnn_samples: the kept networks (S x P); bnn_state: the chain's final theta, p, tau, g, vhat (P each)
     int bnn_P = 0, bnn_S = 0;
     double bnn_ymean = 0.0, bnn_ystd = 1.0;
     DevBuf bnn_data, bnn_samples, bnn_state;
+    // DNGO (gpk_dngo.cuh, gpk_dngo_set_data): the training set in bnn_data, the trained net (P), Adam's m and v (P each,
+    // after dngo_t steps; -1: the net was set, not trained), the scoring pack and the collapse's failure flag.  The
+    // Bayesian linear regression over the features lives in the blr_* fields (F = 50, no basis).
+    bool dngo_trained = false, dngo_fitted = false;
+    int dngo_P = 0;
+    long long dngo_t = -1;
+    DevBuf dngo_net, dngo_state, dngo_pack;
     int es_nb = 0, es_np = 0;
     double es_sn2 = 0.0, es_H = 0.0;
     long es_linv_serial = -1;       // linv_serial U was built for (-1: no update yet)
@@ -763,6 +771,7 @@ const ModelInfo MODELS[] = {
     SURROGATE("a random forest", "gpk_rf_set_data", "a random forest", "model is not fitted (gpk_rf_fit)"),
     SURROGATE("a Bayesian neural network", "gpk_bnn_set_data", "a Bayesian neural network",
               "model is not trained (gpk_bnn_train)"),
+    SURROGATE("a DNGO model", "gpk_dngo_set_data", "DNGO", "model is not fitted (gpk_dngo_fit)"),
 };
 #undef SURROGATE
 
@@ -802,7 +811,8 @@ int require(gpk_handle* h, bool data, bool spec, bool fitted) {
 // the preconditions of the entry points that score any model kind: a fitted GP, or a trained surrogate
 int require_model(gpk_handle* h) {
     if (!h || h->model == MODEL_GP) return require(h, true, true, true);
-    const bool trained = h->model == MODEL_BLR ? h->blr_fitted : h->model == MODEL_RF ? h->rf_fitted : h->bnn_S >= 1;
+    const bool trained = h->model == MODEL_BLR ? h->blr_fitted : h->model == MODEL_RF ? h->rf_fitted
+                       : h->model == MODEL_BNN ? h->bnn_S >= 1 : h->dngo_fitted;
     if (!trained) { set_err(h, "%s", MODELS[h->model].not_fitted); return GPK_NOT_FITTED; }
     return GPK_OK;
 }
@@ -1338,9 +1348,15 @@ struct BlrPost {
     }
 };
 
+// the check of the BLR entry points, which also serve the Bayesian linear regression of a trained DNGO handle
 int blr_ready(gpk_handle* h, const char* who) {
-    int rc = model_ready(h, MODEL_BLR, who);
-    if (rc) return rc;
+    int rc;
+    if (h && h->model == MODEL_DNGO) {
+        if ((rc = model_ready(h, MODEL_DNGO, who))) return rc;
+        if (!h->dngo_trained) { set_err(h, "%s: model is not trained (gpk_dngo_train)", who); return GPK_NOT_FITTED; }
+    } else if ((rc = model_ready(h, MODEL_BLR, who))) {
+        return rc;
+    }
     const int sm_eval = (int)(gpk_blr_smem_doubles(h->blr_F) * 8);
     CK(cudaFuncSetAttribute(gpk_blr_eval_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, sm_eval));
     CK(cudaFuncSetAttribute(gpk_blr_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, sm_eval));
@@ -1381,11 +1397,13 @@ int surrogate_score(gpk_handle* h, const double* dX, long m, int kind, double et
                     bool reset, long global_base, Feeder* feeder) {
     int rc = h->model == MODEL_BLR ? blr_ready(h, "scoring") : model_ready(h, h->model, "scoring");
     if (rc) return rc;
-    // candidates per CTA
+    // candidates per CTA (DNGO: per tile; one resident CTA per SM walks the tiles)
     const long tile = h->model == MODEL_BLR ? GPK_BLR_SCORE_THREADS
                     : h->model == MODEL_RF  ? GPK_RF_SCORE_WARPS
-                                            : GPK_BNN_SCORE_THREADS * GPK_BNN_SCORE_C;
-    const long nblk = (m + tile - 1) / tile;
+                    : h->model == MODEL_BNN ? GPK_BNN_SCORE_THREADS * GPK_BNN_SCORE_C
+                                            : GPK_DNGO_SCORE_THREADS;
+    const long ntiles = (m + tile - 1) / tile;
+    const long nblk = h->model == MODEL_DNGO ? std::min(ntiles, (long)h->n_sm) : ntiles;
     if ((rc = ensure(h, h->block_best, (size_t)std::max(nblk, 1L) * sizeof(BestPair)))) return rc;
     if ((rc = ensure(h, h->best, sizeof(BestPair)))) return rc;
     if ((rc = ensure(h, h->nneg, 8))) return rc;
@@ -1427,7 +1445,7 @@ int surrogate_score(gpk_handle* h, const double* dX, long m, int kind, double et
                               h->stream>>>(a);
         break;
     }
-    default: {                                          // MODEL_BNN
+    case MODEL_BNN: {
         BnnScoreArgs a;
         memset(&a, 0, sizeof(a));
         a.X = dX; a.m = m; a.D = h->d; a.P = h->bnn_P; a.S = h->bnn_S;
@@ -1438,7 +1456,23 @@ int surrogate_score(gpk_handle* h, const double* dX, long m, int kind, double et
         const size_t smem = (size_t)gpk_bnn_score_smem(h->d);
         CK(cudaFuncSetAttribute(gpk_bnn_score_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         gpk_bnn_score_kernel<<<(unsigned)nblk, GPK_BNN_SCORE_THREADS, smem, h->stream>>>(a);
+        break;
     }
+    case MODEL_DNGO: {
+        DngoScoreArgs a;
+        memset(&a, 0, sizeof(a));
+        a.X = dX; a.m = m; a.D = h->d; a.ntiles = (int)ntiles;
+        a.pack = ptr<double>(h->dngo_pack);
+        a.xm = bnn_xm(h); a.xs = bnn_xs(h);
+        a.y_mean = h->bnn_ymean; a.y_std = h->bnn_ystd;
+        a.o = o;
+        const size_t smem = (size_t)gpk_dngo_score_smem(h->d);
+        CK(cudaFuncSetAttribute(gpk_dngo_score_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        gpk_dngo_score_kernel<<<(unsigned)nblk, GPK_DNGO_SCORE_THREADS, smem, h->stream>>>(a);
+        break;
+    }
+    default:
+        BAD("scoring: unknown model kind %d", (int)h->model);
     }
     CKL();
     if (kind != GPK_ACQ_NONE) {
@@ -1510,7 +1544,7 @@ int gpk_destroy(gpk_handle* h) {
                       &h->multi_cand, &h->multi_A, &h->multi_B, &h->multi_out, &h->multi_bb, &h->gather, &h->best_global,
                       &h->de_pop, &h->de_trial, &h->de_param, &h->de_E, &h->de_small, &h->de_sort, &h->lb_buf, &h->cma_buf, &h->dir_buf, &h->ep_buf, &h->es_state, &h->es_U, &h->es_work, &h->es_in, &h->mc_state, &h->mc_buf, &h->mc_stat, &h->fab_in, &h->rs_buf, &h->hy_buf,
                       &h->blr_data, &h->blr_post, &h->blr_work, &h->rf_data, &h->rf_work, &h->rf_nodes,
-                      &h->bnn_data, &h->bnn_samples, &h->bnn_state};
+                      &h->bnn_data, &h->bnn_samples, &h->bnn_state, &h->dngo_net, &h->dngo_state, &h->dngo_pack};
     for (DevBuf* b : bufs)
         if (b->p) cudaFree(b->p);
     if (h->ev_ok)
@@ -2762,10 +2796,12 @@ int gpk_blr_sample(gpk_handle* h, unsigned long long seed, int nwalkers, const d
     return GPK_OK;
 }
 
-int gpk_blr_fit(gpk_handle* h, const double* hypers, int k) {
-    const char* who = "gpk_blr_fit";
-    int rc = blr_ready(h, who);
-    if (rc) return rc;
+}  // extern "C"
+
+namespace {
+// gpk_blr_fit's work, shared with gpk_dngo_fit: the k weight posteriors of hypers on a handle past blr_ready
+int blr_fit(gpk_handle* h, const double* hypers, int k, const char* who) {
+    int rc;
     if (!hypers || k < 1) BAD("%s: need hypers and k >= 1", who);
     h->blr_fitted = false;
     const int F = h->blr_F;
@@ -2790,6 +2826,17 @@ int gpk_blr_fit(gpk_handle* h, const double* hypers, int k) {
     h->blr_k = k;
     h->blr_fitted = true;
     return GPK_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int gpk_blr_fit(gpk_handle* h, const double* hypers, int k) {
+    const char* who = "gpk_blr_fit";
+    if (h && h->model == MODEL_DNGO) BAD("%s: the handle holds %s; its fit is gpk_dngo_fit", who, MODELS[MODEL_DNGO].holds);
+    int rc = blr_ready(h, who);
+    if (rc) return rc;
+    return blr_fit(h, hypers, k, who);
 }
 
 int gpk_blr_get_models(gpk_handle* h, double* m, double* S) {
@@ -2960,25 +3007,22 @@ int gpk_rf_set_trees(gpk_handle* h, int T, int total_variance, const int* n_node
     return GPK_OK;
 }
 
-// ---------------------------------------------------------------------------------------
-// Bayesian neural network (gpk_bnn.cuh; robo/models/wrapper_bohamiann.py)
-// ---------------------------------------------------------------------------------------
-int gpk_bnn_set_data(gpk_handle* h, const double* X, const double* y, int n, int d) {
-    if (!h) return GPK_BAD_ARG;
-    const char* who = "gpk_bnn_set_data";
-    int rc = claim_model(h, MODEL_BNN, who);
-    if (rc) return rc;
-    if (!X || !y || n <= 0 || d <= 0) BAD("%s: need X, y, n > 0, d > 0", who);
-    if (n < 2) BAD("%s: need n >= 2 training points to normalise the data (n = %d)", who, n);
-    if (n > GPK_BNN_MAX_N) BAD("%s: n = %d training points exceed GPK_BNN_MAX_N = %d", who, n, GPK_BNN_MAX_N);
-    if (d > GPK_BNN_MAX_D) BAD("%s: d = %d exceeds GPK_BNN_MAX_D = %d", who, d, GPK_BNN_MAX_D);
+}  // extern "C"
+
+namespace {
+// The host scaling of gpk_bnn_set_data and gpk_dngo_set_data: X and y must be finite; then buf = the scaled X (n x d),
+// the scaled y (n), the input mean and std (d each), and *ym / *ysd the y statistics.  Each column of X (norm_x) and y
+// (norm_y) goes to zero mean and unit population std (sums in ascending row order); a constant one is GPK_BAD_ARG.  A
+// side whose flag is off is copied as given, with mean 0 and std 1.
+int scale_set(gpk_handle* h, const char* who, const double* X, const double* y, int n, int d, bool norm_x, bool norm_y,
+              std::vector<double>& buf, double* ym, double* ysd) {
     for (long i = 0; i < (long)n * d; ++i)
         if (!std::isfinite(X[i])) BAD("%s: X must be finite", who);
     for (int i = 0; i < n; ++i)
         if (!std::isfinite(y[i])) BAD("%s: y must be finite", who);
     // column statistics: sums in ascending row order, population std
     const size_t nd = (size_t)n * d;
-    std::vector<double> buf(nd + n + 2 * (size_t)d);
+    buf.assign(nd + n + 2 * (size_t)d, 0.0);
     double* xs = buf.data();
     double* ys = xs + nd;
     double* xm = ys + n;
@@ -2996,14 +3040,44 @@ int gpk_bnn_set_data(gpk_handle* h, const double* X, const double* y, int n, int
         *sd = std::sqrt(q / (double)n);
     };
     for (int c = 0; c < d; ++c) {
+        if (!norm_x) {
+            xm[c] = 0.0; xsd[c] = 1.0;
+            for (int i = 0; i < n; ++i) xs[(size_t)i * d + c] = X[(size_t)i * d + c];
+            continue;
+        }
         stats(X + c, d, xm + c, xsd + c);
         if (!(xsd[c] > 0.0)) BAD("%s: input column %d is constant; it cannot be normalised", who, c);
         for (int i = 0; i < n; ++i) xs[(size_t)i * d + c] = (X[(size_t)i * d + c] - xm[c]) / xsd[c];
     }
+    if (!norm_y) {
+        *ym = 0.0; *ysd = 1.0;
+        for (int i = 0; i < n; ++i) ys[i] = y[i];
+        return GPK_OK;
+    }
+    stats(y, 1, ym, ysd);
+    if (!(*ysd > 0.0)) BAD("%s: y is constant; it cannot be normalised", who);
+    for (int i = 0; i < n; ++i) ys[i] = (y[i] - *ym) / *ysd;
+    return GPK_OK;
+}
+}  // namespace
+
+extern "C" {
+
+// ---------------------------------------------------------------------------------------
+// Bayesian neural network (gpk_bnn.cuh; robo/models/wrapper_bohamiann.py)
+// ---------------------------------------------------------------------------------------
+int gpk_bnn_set_data(gpk_handle* h, const double* X, const double* y, int n, int d) {
+    if (!h) return GPK_BAD_ARG;
+    const char* who = "gpk_bnn_set_data";
+    int rc = claim_model(h, MODEL_BNN, who);
+    if (rc) return rc;
+    if (!X || !y || n <= 0 || d <= 0) BAD("%s: need X, y, n > 0, d > 0", who);
+    if (n < 2) BAD("%s: need n >= 2 training points to normalise the data (n = %d)", who, n);
+    if (n > GPK_BNN_MAX_N) BAD("%s: n = %d training points exceed GPK_BNN_MAX_N = %d", who, n, GPK_BNN_MAX_N);
+    if (d > GPK_BNN_MAX_D) BAD("%s: d = %d exceeds GPK_BNN_MAX_D = %d", who, d, GPK_BNN_MAX_D);
+    std::vector<double> buf;
     double ym, ysd;
-    stats(y, 1, &ym, &ysd);
-    if (!(ysd > 0.0)) BAD("%s: y is constant; it cannot be normalised", who);
-    for (int i = 0; i < n; ++i) ys[i] = (y[i] - ym) / ysd;
+    if ((rc = scale_set(h, who, X, y, n, d, true, true, buf, &ym, &ysd))) return rc;
     CK(cudaSetDevice(h->device));
     h->model = MODEL_BNN;
     h->bnn_S = 0;
@@ -3111,6 +3185,192 @@ int gpk_bnn_draws(gpk_handle* h, unsigned long long seed, unsigned counter, int 
                                                                                   ptr<double>(h->tmp1));
     CKL();
     CK(cudaMemcpyAsync(Z, h->tmp1.p, bytes, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    return GPK_OK;
+}
+
+// ---------------------------------------------------------------------------------------
+// DNGO (gpk_dngo.cuh; pybnn's DNGO, robo/fmin/bayesian_optimization.py:105-109)
+// ---------------------------------------------------------------------------------------
+}  // extern "C"
+
+namespace {
+// G = Theta^T Theta and b = Theta^T y of the Bayesian linear regression over the features in blr_phi(h); then the handle
+// holds a trained net and no fit
+int dngo_gram(gpk_handle* h) {
+    gpk_blr_gram_kernel<<<(unsigned)(GPK_DNGO_H * GPK_DNGO_H + GPK_DNGO_H), 256, 0, h->stream>>>(
+        blr_phi(h), blr_y(h), h->n, GPK_DNGO_H, blr_G(h), blr_b(h));
+    CKL();
+    CK(cudaStreamSynchronize(h->stream));
+    h->dngo_trained = true;
+    return GPK_OK;
+}
+
+int dngo_trained(gpk_handle* h, const char* who) {
+    int rc = model_ready(h, MODEL_DNGO, who);
+    if (rc) return rc;
+    if (!h->dngo_trained) { set_err(h, "%s: model is not trained (gpk_dngo_train)", who); return GPK_NOT_FITTED; }
+    return GPK_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int gpk_dngo_set_data(gpk_handle* h, const double* X, const double* y, int n, int d, int normalize_input,
+                      int normalize_output, const double* prior_par) {
+    if (!h) return GPK_BAD_ARG;
+    const char* who = "gpk_dngo_set_data";
+    int rc = claim_model(h, MODEL_DNGO, who);
+    if (rc) return rc;
+    if (!X || !y || !prior_par || n <= 0 || d <= 0) BAD("%s: need X, y, prior_par, n > 0, d > 0", who);
+    if ((normalize_input || normalize_output) && n < 2)
+        BAD("%s: need n >= 2 training points to normalise the data (n = %d)", who, n);
+    if (n > GPK_DNGO_MAX_N) BAD("%s: n = %d training points exceed GPK_DNGO_MAX_N = %d", who, n, GPK_DNGO_MAX_N);
+    if (d > GPK_DNGO_MAX_D) BAD("%s: d = %d exceeds GPK_DNGO_MAX_D = %d", who, d, GPK_DNGO_MAX_D);
+    std::vector<double> buf;
+    double ym, ysd;
+    if ((rc = scale_set(h, who, X, y, n, d, normalize_input != 0, normalize_output != 0, buf, &ym, &ysd))) return rc;
+    CK(cudaSetDevice(h->device));
+    h->model = MODEL_DNGO;
+    h->dngo_trained = h->dngo_fitted = h->blr_fitted = false;
+    h->dngo_t = -1;
+    h->n = n; h->d = d;
+    h->dngo_P = gpk_dngo_params(d);
+    h->bnn_ymean = ym; h->bnn_ystd = ysd;
+    h->blr_F = GPK_DNGO_H; h->blr_basis = GPK_BLR_NONE;
+    h->blr_prior.ln_sigma = prior_par[0]; h->blr_prior.ln_loc = prior_par[1]; h->blr_prior.hs_scale = prior_par[2];
+    if ((rc = ensure(h, h->bnn_data, buf.size() * 8))) return rc;
+    if ((rc = ensure(h, h->blr_data, ((size_t)n * GPK_DNGO_H + n + GPK_DNGO_H * GPK_DNGO_H + GPK_DNGO_H) * 8))) return rc;
+    CK(cudaMemcpyAsync(bnn_X(h), buf.data(), buf.size() * 8, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(blr_y(h), buf.data() + (size_t)n * d, (size_t)n * 8, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaStreamSynchronize(h->stream));     // the staging vector dies here
+    return GPK_OK;
+}
+
+int gpk_dngo_train(gpk_handle* h, unsigned long long seed, unsigned counter, double lr, int batch, int epochs) {
+    const char* who = "gpk_dngo_train";
+    int rc = model_ready(h, MODEL_DNGO, who);
+    if (rc) return rc;
+    if (!(std::isfinite(lr) && lr > 0.0)) BAD("%s: need a finite lr > 0", who);
+    if (batch < 1 || epochs < 1) BAD("%s: need batch >= 1 and epochs >= 1", who);
+    const int B = std::min(batch, h->n);
+    if (B > GPK_DNGO_MAX_BATCH)
+        BAD("%s: a batch of min(batch, n) = %d rows exceeds GPK_DNGO_MAX_BATCH = %d", who, B, GPK_DNGO_MAX_BATCH);
+    const int P = h->dngo_P;
+    h->dngo_trained = h->dngo_fitted = h->blr_fitted = false;
+    h->dngo_t = -1;
+    if ((rc = ensure(h, h->dngo_net, (size_t)P * 8))) return rc;
+    if ((rc = ensure(h, h->dngo_state, (size_t)2 * P * 8))) return rc;
+    const size_t smem = (size_t)gpk_dngo_train_smem(h->n, h->d, B);
+    CK(cudaFuncSetAttribute(gpk_dngo_train_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    DngoTrainArgs a;
+    memset(&a, 0, sizeof(a));
+    a.X = bnn_X(h); a.y = bnn_y(h);
+    a.n = h->n; a.d = h->d; a.P = P; a.B = B; a.epochs = epochs;
+    a.seed = seed; a.counter = counter;
+    a.lr = lr;
+    a.state = ptr<double>(h->dngo_state);
+    a.net = ptr<double>(h->dngo_net);
+    a.Theta = blr_phi(h);
+    gpk_dngo_train_kernel<<<1, GPK_DNGO_THREADS, smem, h->stream>>>(a);
+    CKL();
+    if ((rc = dngo_gram(h))) return rc;
+    h->dngo_t = (long long)epochs * (h->n / B);
+    return GPK_OK;
+}
+
+int gpk_dngo_fit(gpk_handle* h, const double* hypers, int k) {
+    const char* who = "gpk_dngo_fit";
+    int rc = dngo_trained(h, who);
+    if (!rc) rc = blr_ready(h, who);
+    if (!rc) rc = blr_fit(h, hypers, k, who);
+    if (rc) return rc;
+    h->dngo_fitted = false;
+    const DngoPack K(h->d);
+    if ((rc = ensure(h, h->dngo_pack, (size_t)K.total * 8 + 8))) return rc;
+    double* pack = ptr<double>(h->dngo_pack);
+    int* fail = (int*)(pack + K.total);
+    const BlrPost L(k, GPK_DNGO_H);
+    const double* post = ptr<double>(h->blr_post);
+    gpk_dngo_collapse_kernel<<<1, GPK_BLR_THREADS, gpk_dngo_collapse_doubles() * 8, h->stream>>>(
+        post + L.M, post + L.S, post + L.ib, k, ptr<double>(h->dngo_net), h->d, pack, fail);
+    CKL();
+    int f = 0;
+    CK(cudaMemcpyAsync(&f, fail, 4, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    if (f) {
+        set_err(h, "%s: the mixture covariance mean S_i + cov(m_i) of the %d hypers is not positive definite", who, k);
+        return GPK_NOT_PD;
+    }
+    h->dngo_fitted = true;
+    return GPK_OK;
+}
+
+int gpk_dngo_dims(gpk_handle* h, int* n, int* d, int* P, int* k) {
+    int rc = model_ready(h, MODEL_DNGO, "gpk_dngo_dims");
+    if (rc) return rc;
+    if (n) *n = h->n;
+    if (d) *d = h->d;
+    if (P) *P = h->dngo_P;
+    if (k) *k = h->dngo_fitted ? h->blr_k : 0;
+    return GPK_OK;
+}
+
+int gpk_dngo_get_net(gpk_handle* h, double* net) {
+    const char* who = "gpk_dngo_get_net";
+    int rc = dngo_trained(h, who);
+    if (rc) return rc;
+    if (!net) BAD("%s: need the output array", who);
+    CK(cudaMemcpyAsync(net, h->dngo_net.p, (size_t)h->dngo_P * 8, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    return GPK_OK;
+}
+
+int gpk_dngo_set_net(gpk_handle* h, const double* net) {
+    const char* who = "gpk_dngo_set_net";
+    int rc = model_ready(h, MODEL_DNGO, who);
+    if (rc) return rc;
+    if (!net) BAD("%s: need the net", who);
+    const int P = h->dngo_P;
+    for (int i = 0; i < P; ++i)
+        if (!std::isfinite(net[i])) BAD("%s: the net must be finite", who);
+    h->dngo_trained = h->dngo_fitted = h->blr_fitted = false;
+    h->dngo_t = -1;
+    if ((rc = ensure(h, h->dngo_net, (size_t)P * 8))) return rc;
+    CK(cudaMemcpyAsync(h->dngo_net.p, net, (size_t)P * 8, cudaMemcpyHostToDevice, h->stream));
+    gpk_dngo_features_kernel<<<(unsigned)h->n, 64, 0, h->stream>>>(bnn_X(h), h->n, h->d, nullptr, nullptr,
+                                                                   ptr<double>(h->dngo_net), blr_phi(h));
+    CKL();
+    return dngo_gram(h);
+}
+
+int gpk_dngo_features(gpk_handle* h, const double* X, long m, double* out) {
+    const char* who = "gpk_dngo_features";
+    int rc = dngo_trained(h, who);
+    if (rc) return rc;
+    if (!X || !out || m < 1 || m > INT_MAX) BAD("%s: need X, out and 1 <= m <= 2^31 - 1", who);
+    const size_t xb = (size_t)m * h->d * 8, ob = (size_t)m * GPK_DNGO_H * 8;
+    if ((rc = ensure(h, h->tmp1, xb + ob))) return rc;
+    double* dX = ptr<double>(h->tmp1);
+    double* dO = dX + (size_t)m * h->d;
+    CK(cudaMemcpyAsync(dX, X, xb, cudaMemcpyHostToDevice, h->stream));
+    gpk_dngo_features_kernel<<<(unsigned)m, 64, 0, h->stream>>>(dX, m, h->d, bnn_xm(h), bnn_xs(h),
+                                                               ptr<double>(h->dngo_net), dO);
+    CKL();
+    CK(cudaMemcpyAsync(out, dO, ob, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    return GPK_OK;
+}
+
+int gpk_dngo_get_state(gpk_handle* h, double* m, double* v, long long* t) {
+    const char* who = "gpk_dngo_get_state";
+    int rc = model_ready(h, MODEL_DNGO, who);
+    if (rc) return rc;
+    if (h->dngo_t < 0) { set_err(h, "%s: no training has run (gpk_dngo_train)", who); return GPK_NOT_FITTED; }
+    const size_t P = h->dngo_P;
+    if (m) CK(cudaMemcpyAsync(m, ptr<double>(h->dngo_state), P * 8, cudaMemcpyDeviceToHost, h->stream));
+    if (v) CK(cudaMemcpyAsync(v, ptr<double>(h->dngo_state) + P, P * 8, cudaMemcpyDeviceToHost, h->stream));
+    if (t) *t = h->dngo_t;
     CK(cudaStreamSynchronize(h->stream));
     return GPK_OK;
 }

@@ -40,7 +40,7 @@ class DeviceRandomSampling(BaseMaximizer):
         surrogate = isinstance(model, DEVICE_SURROGATES)
         if not surrogate and (not hasattr(model, "gp") or not hasattr(model.gp, "handle")):
             raise TypeError("DeviceRandomSampling needs a robo_b200 GaussianProcess, BayesianLinearRegression, "
-                            "RandomForest or WrapperBohamiann model")
+                            "RandomForest, WrapperBohamiann or DNGO model")
         if surrogate and self.world > 1:
             raise ValueError("DeviceRandomSampling of a %s runs on one GPU" % type(model).__name__)
         kind = _lib.ACQ_KIND[acq.kind]

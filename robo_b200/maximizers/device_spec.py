@@ -6,13 +6,14 @@ import numpy as np
 
 from robo_b200 import _lib
 from robo_b200.models.bayesian_linear_regression import BayesianLinearRegression
+from robo_b200.models.dngo import DNGO
 from robo_b200.models.gaussian_process import GaussianProcess
 from robo_b200.models.random_forest import RandomForest
 from robo_b200.models.wrapper_bohamiann import WrapperBohamiann
 
 KINDS = ("ei", "log_ei", "pi", "lcb")
 # the models other than GaussianProcess that score on the device: each holds one handle of its own (_ready_handle)
-DEVICE_SURROGATES = (BayesianLinearRegression, RandomForest, WrapperBohamiann)
+DEVICE_SURROGATES = (BayesianLinearRegression, RandomForest, WrapperBohamiann, DNGO)
 
 
 def raw_inputs(model):
@@ -49,7 +50,7 @@ def device_spec(acq, who):
 
 def acq_spec(acq, who):
     """(kind, eta per model, par, handles) of the acquisition, or TypeError when it does not run on device GPs whose
-    inputs go to the handle untransformed or on a BayesianLinearRegression, RandomForest or WrapperBohamiann (eta: its
+    inputs go to the handle untransformed or on a BayesianLinearRegression, RandomForest, WrapperBohamiann or DNGO (eta: its
     min observed y)."""
     if hasattr(acq, "_fused_spec"):                          # MarginalizationGPMCMC
         fused = acq._fused_spec()

@@ -156,6 +156,20 @@ print("bnn samples", _lib.bnn_dims(h), "draws", Zb[0, :2], "predict", h.predict(
 r = _lib.maximize_direct([h], _lib.ACQ_EI, [float(y.min())], 0.0, np.zeros(D), np.ones(D), n_func_evals=100)
 print("bnn direct", r["nit"], r["nfev"])
 h.close()
+# DNGO: the training (a dropped remainder), Theta and the regression's products, its sampler and fit, the collapsed
+# predictive over a ragged tile, the net read-back and upload, scored directly and through DIRECT
+h = _lib.Handle(0)
+_lib.dngo_set_data(h, X[:23], y[:23], True, True, (0.1, -10.0, 0.1))
+_lib.dngo_train(h, 5, 0, 1e-2, 10, 3)
+Pd = _lib.blr_sample(h, 3, np.c_[rng.uniform(-3, 1, 6), rng.uniform(0, 5, 6)], 4)["pos"]
+_lib.dngo_fit(h, np.exp(Pd))
+_lib.dngo_set_net(h, _lib.dngo_net(h))
+_lib.dngo_fit(h, np.exp(Pd))
+print("dngo", _lib.dngo_dims(h), "features", _lib.dngo_features(h, Xs[:3])[0, :2], "predict",
+      h.predict(Xs[:300])[1][:2], "acq", h.acq(Xs[:300], _lib.ACQ_EI, float(y.min()), 0.0)["best_idx"])
+r = _lib.maximize_direct([h], _lib.ACQ_EI, [float(y.min())], 0.0, np.zeros(D), np.ones(D), n_func_evals=100)
+print("dngo direct", r["nit"], r["nfev"])
+h.close()
 h = _lib.moments_handle()
 print(h.acq_moments(rng.randn(100), rng.rand(100) + 0.1, _lib.ACQ_LOG_EI, 0.0, 0.0)[0][:3])
 print(h.reduce_models(rng.rand(4, 50), rng.rand(4, 50))[1][:3])
