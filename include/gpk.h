@@ -755,6 +755,23 @@ int gpk_hyper_lnpost(gpk_handle* h, const double* theta, int count, int dim, dou
 int gpk_sample_hypers(gpk_handle* h, const double* p0, int nwalkers, int dim, int steps, unsigned long long seed,
                       double* pos, double* lnpost, long* n_accepted);
 
+/* ---- GaussianProcess hyper-parameter optimisation on the device (robo_b200/csrc/gpk_hyperopt.cuh) ------------------
+ * GaussianProcess.optimize (gaussian_process.py:193-219): scipy.optimize.minimize(nll, p0, method='L-BFGS-B') without a
+ * gradient, as one call.  nll is the objective of gpk_hyper_lnpost's two parts (-ll without a prior, -(ll + lp) with
+ * one, 1e25 where that is not finite or |theta_j| > 20), the gradient scipy's forward differences with the absolute step
+ * eps.  Every round scores the trial point and its dim neighbours in one launch (one CTA each) and runs L-BFGS-B's update
+ * (every variable unbounded: the two-loop direction, the More-Thuente search, L-BFGS-B's restarts and skip rule) on the
+ * device; the host reads the status once per GPK_HO_CHUNK rounds.  The arguments are scipy's options: maxcor, maxiter,
+ * maxfun, ftol, pgtol (gtol), eps, maxls.  Needs gpk_set_data, gpk_set_kernel and gpk_set_hyper_model, as
+ * gpk_sample_hypers.  Out: theta (dim) = the last accepted iterate (results.x); f, nit, nfev (evaluations, dim + 1 per
+ * scored point) and status (GPK_LB_FTOL, _PGTOL, _MAXITER, _MAXFUN or _ABNORMAL) may be NULL.
+ * GPK_BAD_ARG: no data, kernel or hyper model, a handle of another model kind, n > GPK_HYPER_MAX_N, dim != n_params + 1
+ * or > GPK_HYPER_MAX_DIM, a non-finite p0, maxcor outside [1, 32], maxls < 1, eps <= 0, maxiter or maxfun < 1. */
+#define GPK_HO_CHUNK 16
+int gpk_optimize_hypers(gpk_handle* h, const double* p0, int dim, int maxcor, int maxiter, long maxfun, double ftol,
+                        double pgtol, double eps, int maxls, double* theta, double* f, int* nit, long* nfev,
+                        int* status);
+
 /* ---- Bayesian linear regression on the device (robo_b200/csrc/gpk_blr.cuh) ----------------------------------------
  * robo/models/bayesian_linear_regression.py with its default prior (robo/priors/bayesian_linear_regression_prior.py).
  * A handle becomes a BLR handle with gpk_blr_set_data and stays one: the Gaussian-process entry points (gpk_set_data,

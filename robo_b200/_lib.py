@@ -28,6 +28,7 @@ PRIOR_NONE, PRIOR_DEFAULT, PRIOR_ENV, PRIOR_MTBO = range(4)   # gpk_prior_kind: 
 MAX_TASKS = 8                                 # GPK_MAX_TASKS
 HYPER_MAX_N = 232                              # GPK_HYPER_MAX_N: most training points of gpk_sample_hypers
 HYPER_MAX_DIM = 96                             # GPK_HYPER_MAX_DIM: most entries of theta (log noise included)
+HO_CHUNK = 16                                  # GPK_HO_CHUNK: rounds of gpk_optimize_hypers between two status reads
 BLR_LINEAR, BLR_QUADRATIC, BLR_NONE = range(3)  # gpk_blr_basis: the features of a BayesianLinearRegression handle
 BLR_MAX_F = 64                                 # GPK_BLR_MAX_F: most features of a BayesianLinearRegression handle
 RF_MAX_N, RF_MAX_D, RF_MAX_T = 16384, 64, 512  # GPK_RF_MAX_N / GPK_RF_MAX_D / GPK_RF_MAX_T: the largest forest
@@ -161,6 +162,8 @@ _SIGNATURES = {
     "gpk_set_hyper_model": [_vp, C.c_int, _ip, _ip, C.c_int, C.c_double, C.c_double, C.c_int, _dp, C.c_int, C.c_int],
     "gpk_hyper_lnpost": [_vp, _dp, C.c_int, C.c_int, _dp, _dp],
     "gpk_sample_hypers": [_vp, _dp, C.c_int, C.c_int, C.c_int, C.c_ulonglong, _dp, _dp, _lp],
+    "gpk_optimize_hypers": [_vp, _dp, C.c_int, C.c_int, C.c_int, C.c_long, C.c_double, C.c_double, C.c_double, C.c_int,
+                            _dp, _dp, _ip, _lp, _ip],
     "gpk_blr_set_data": [_vp, _dp, _dp, C.c_int, C.c_int, C.c_int, _dp],
     "gpk_blr_lnpost": [_vp, _dp, C.c_int, _dp],
     "gpk_blr_sample": [_vp, C.c_ulonglong, C.c_int, _dp, C.c_int, _dp, _dp, _lp],
@@ -1311,6 +1314,25 @@ def sample_hypers(handle, p0, steps, seed):
     handle._check(handle.lib.gpk_sample_hypers(handle._h, _as_dp(P), nw, dim, int(steps), int(seed) & 0xFFFFFFFFFFFFFFFF,
                                                _as_dp(pos), _as_dp(lnp), acc.ctypes.data_as(_lp)))
     return dict(pos=pos, lnpost=lnp, n_accepted=acc)
+
+
+def optimize_hypers(handle, p0, maxcor=10, maxiter=15000, maxfun=15000, ftol=2.220446049250313e-09, gtol=1e-5,
+                    eps=1e-8, maxls=20):
+    """gpk_optimize_hypers: scipy.optimize.minimize(nll, p0, method='L-BFGS-B') with scipy's default options, on the
+    device -> dict(theta (dim,), f, nit, nfev, status (LB_*), rounds, noop_rounds).  rounds: the points scored (dim + 1
+    evaluations each); noop_rounds: the launches after the final round that returned at once (the rest of the last
+    chunk of HO_CHUNK)."""
+    x0 = f64(np.ravel(p0)).copy()
+    dim = x0.size
+    theta = np.empty(dim)
+    f, nfev = C.c_double(), C.c_long()
+    nit, status = C.c_int(), C.c_int()
+    handle._check(handle.lib.gpk_optimize_hypers(handle._h, _as_dp(x0), dim, int(maxcor), int(maxiter), int(maxfun),
+                                                 float(ftol), float(gtol), float(eps), int(maxls), _as_dp(theta),
+                                                 C.byref(f), C.byref(nit), C.byref(nfev), C.byref(status)))
+    rounds = nfev.value // (dim + 1)
+    return dict(theta=theta, f=f.value, nit=nit.value, nfev=nfev.value, status=status.value, rounds=rounds,
+                noop_rounds=-(-rounds // HO_CHUNK) * HO_CHUNK - rounds)
 
 
 def blr_features(n_dims, basis):

@@ -33,6 +33,7 @@
 #include "gpk_esmc.cuh"
 #include "gpk_rs.cuh"
 #include "gpk_hyper.cuh"
+#include "gpk_hyperopt.cuh"
 #include "gpk_blr.cuh"
 #include "gpk_rf.cuh"
 #include "gpk_bnn.cuh"
@@ -2707,6 +2708,63 @@ int gpk_sample_hypers(gpk_handle* h, const double* p0, int nwalkers, int dim, in
     memcpy(pos, out.data(), nP * 8);
     memcpy(lnpost, out.data() + nP, (size_t)nwalkers * 8);
     if (n_accepted) memcpy(n_accepted, out.data() + nP + nwalkers, (size_t)nwalkers * 8);
+    return GPK_OK;
+}
+
+// GaussianProcess.optimize on the device (gpk_hyperopt.cuh; gaussian_process.py:193-219)
+int gpk_optimize_hypers(gpk_handle* h, const double* p0, int dim, int maxcor, int maxiter, long maxfun, double ftol,
+                        double pgtol, double eps, int maxls, double* theta, double* f, int* nit, long* nfev,
+                        int* status) {
+    if (!h) return GPK_BAD_ARG;
+    const char* who = "gpk_optimize_hypers";
+    if (!p0 || !theta) BAD("%s: need p0 and theta", who);
+    if (dim < 1 || dim > GPK_HYPER_MAX_DIM) BAD("%s: need 1 <= dim <= %d (dim = %d)", who, GPK_HYPER_MAX_DIM, dim);
+    for (int j = 0; j < dim; ++j)
+        if (!std::isfinite(p0[j])) BAD("%s: p0[%d] = %g is not finite", who, j, p0[j]);
+    if (maxcor < 1 || maxcor > GPK_LB_MAX_COR) BAD("%s: need 1 <= maxcor <= %d (maxcor = %d)", who, GPK_LB_MAX_COR, maxcor);
+    if (maxls < 1) BAD("%s: need maxls >= 1 (maxls = %d)", who, maxls);
+    if (!(eps > 0.0)) BAD("%s: need eps > 0 (eps = %g)", who, eps);
+    if (maxiter < 1 || maxfun < 1) BAD("%s: need maxiter >= 1 and maxfun >= 1 (%d, %ld)", who, maxiter, maxfun);
+    int rc = hyper_ready(h, dim, who);
+    if (rc) return rc;
+    const size_t smem = gpk_hy_smem_doubles(h->n) * 8;
+    CK(cudaFuncSetAttribute(gpk_ho_round_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    // the state record, then the work buffer
+    const size_t nst = (sizeof(HOState) + 7) / 8, nw = (size_t)gpk_ho_work_doubles(dim, maxcor);
+    if ((rc = ensure(h, h->hy_buf, (nst + nw) * 8))) return rc;
+    HOState* dst = ptr<HOState>(h->hy_buf);
+    double* work = ptr<double>(h->hy_buf) + nst;
+    const HOWork w = gpk_ho_work(work, dim, maxcor);
+    HOState s0;
+    memset(&s0, 0, sizeof(s0));
+    s0.status = GPK_LB_RUNNING;
+    s0.phase = GPK_HO_START;
+    HOParams q;
+    q.maxcor = maxcor; q.maxiter = maxiter; q.maxls = maxls; q.maxfun = maxfun;
+    q.tol = (ftol / GPK_LB_DBL_EPS) * GPK_LB_DBL_EPS;      // scipy's factr = ftol / eps, L-BFGS-B's tol = factr eps
+    q.pgtol = pgtol; q.eps = eps;
+    CK(cudaMemcpyAsync(dst, &s0, sizeof(s0), cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(w.xt, p0, (size_t)dim * 8, cudaMemcpyHostToDevice, h->stream));
+    const double* Xt = ptr<double>(h->Xt);
+    const double* y = ptr<double>(h->y);
+    int* pst = reinterpret_cast<int*>(h->pin);
+    for (;;) {
+        for (int r = 0; r < GPK_HO_CHUNK; ++r) {
+            gpk_ho_round_kernel<<<dim + 1, GPK_HY_THREADS, smem, h->stream>>>(h->hyper, Xt, h->NP, y, h->n, q, work, dst);
+            CKL();
+        }
+        CK(cudaMemcpyAsync(pst, &dst->status, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+        CK(cudaStreamSynchronize(h->stream));
+        if (*pst != GPK_LB_RUNNING) break;
+    }
+    HOState s;
+    CK(cudaMemcpyAsync(&s, dst, sizeof(s), cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaMemcpyAsync(theta, w.x, (size_t)dim * 8, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    if (f) *f = s.f;
+    if (nit) *nit = s.nit;
+    if (nfev) *nfev = (long)s.nfev;
+    if (status) *status = s.status;
     return GPK_OK;
 }
 

@@ -17,7 +17,7 @@ from robo_b200.solver import BayesianOptimization
 def bayesian_optimization(objective_function, lower, upper, num_iterations=30, X_init=None, Y_init=None,
                           maximizer="random", acquisition_func="log_ei", model_type="gp_mcmc",
                           n_init=3, rng=None, output_path=None, n_candidates=500,
-                          chain_length=200, burnin_steps=100, hyper_sampler="host"):
+                          chain_length=200, burnin_steps=100, hyper_sampler="host", hyper_optimizer="host"):
     assert upper.shape[0] == lower.shape[0], "Dimension miss match"
     assert np.all(lower < upper), "Lower bound >= upper bound"
     assert n_init <= num_iterations, "Number of initial design point has to be <= than the number of iterations"
@@ -33,8 +33,10 @@ def bayesian_optimization(objective_function, lower, upper, num_iterations=30, X
         n_hypers += 1
 
     if model_type == "gp":
+        # hyper_optimizer="device" runs each train's L-BFGS-B over the marginal likelihood on the device
+        # (gpk_optimize_hypers), "host" with scipy
         model = GaussianProcess(kernel, prior=prior, rng=rng, normalize_output=False, normalize_input=True,
-                                lower=lower, upper=upper)
+                                lower=lower, upper=upper, hyper_optimizer=hyper_optimizer)
     elif model_type == "gp_mcmc":
         # hyper_sampler="device" samples the hyper-parameters on the device (gpk_sample_hypers), "host" with
         # EnsembleSampler; the two agree in law, not bit for bit

@@ -17,7 +17,7 @@ from robo_b200.solver import BayesianOptimization
 
 def entropy_search(objective_function, lower, upper, num_iterations=30, maximizer="random", model="gp_mcmc",
                    X_init=None, Y_init=None, n_init=3, output_path=None, rng=None, representer_sampler="host",
-                   hyper_sampler="host"):
+                   hyper_sampler="host", hyper_optimizer="host"):
     assert upper.shape[0] == lower.shape[0], "Dimension miss match"
     assert np.all(lower < upper), "Lower bound >= upper bound"
     assert n_init <= num_iterations, "Number of initial design point has to be <= than the number of iterations"
@@ -36,8 +36,10 @@ def entropy_search(objective_function, lower, upper, num_iterations=30, maximize
         n_hypers += 1
 
     if model == "gp":
+        # hyper_optimizer="device" runs each train's L-BFGS-B over the marginal likelihood on the device
+        # (gpk_optimize_hypers), "host" with scipy
         gp = GaussianProcess(kernel, prior=prior, rng=rng, normalize_output=False, normalize_input=True,
-                             lower=lower, upper=upper)
+                             lower=lower, upper=upper, hyper_optimizer=hyper_optimizer)
     elif model == "gp_mcmc":
         # hyper_sampler="device" samples the hyper-parameters on the device (gpk_sample_hypers), "host" with
         # EnsembleSampler; the two agree in law, not bit for bit

@@ -29,11 +29,12 @@ def _transform(X, lower, upper, basis_func):
 class FabolasGP(GaussianProcess):
 
     def __init__(self, kernel, basis_function, prior=None, noise=1e-3, use_gradients=False, normalize_output=False,
-                 lower=None, upper=None, rng=None, device=0):
+                 lower=None, upper=None, rng=None, device=0, hyper_optimizer="host"):
         self.basis_function = basis_function
         super(FabolasGP, self).__init__(kernel=kernel, prior=prior, noise=noise, use_gradients=use_gradients,
                                         normalize_output=normalize_output, normalize_input=False,
-                                        lower=lower, upper=upper, rng=rng, device=device)
+                                        lower=lower, upper=upper, rng=rng, device=device,
+                                        hyper_optimizer=hyper_optimizer)
 
     def normalize(self, X):
         return _transform(X, self.lower, self.upper, self.basis_function)

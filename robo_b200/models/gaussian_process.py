@@ -12,8 +12,15 @@ unchanged.  What differs is where the arithmetic runs:
   gp.predict: full M x M covariance, then np.diag   fused K* -> L^-1 K*^T -> (mu, var), no M x M
   scipy.stats.norm in ei.py/log_ei.py/pi.py         acquisition closed form in the same epilogue
 
-Hyper-parameter optimisation stays where the reference has it (scipy L-BFGS-B on the host,
-gaussian_process.py:193-219); every nll() evaluation is one gpk_fit.
+Hyper-parameter optimisation (gaussian_process.py:193-219) runs where ``hyper_optimizer`` says:
+  - "host" (default): scipy L-BFGS-B on the host, as the reference; every nll() evaluation is one gpk_fit, and scipy
+    builds each gradient by forward differences, so one optimisation is hundreds of serial fits;
+  - "device": the same minimize(nll, p0, method='L-BFGS-B') as one gpk_optimize_hypers call
+    (robo_b200/csrc/gpk_hyperopt.cuh): each round scores the trial point and its forward-difference neighbours in one
+    launch (the likelihood of one theta per CTA, as gpk_sample_hypers computes it) and runs L-BFGS-B's update on the
+    device.  The likelihood is the same function as nll() computed by another routine, so the two arms agree to
+    rounding at every point and may part where L-BFGS-B's decisions are that close; it needs N <= GPK_HYPER_MAX_N
+    (larger N optimises on the host) and a kernel and prior the device restates.
 """
 import logging
 
@@ -31,8 +38,25 @@ class GaussianProcess(BaseModel):
 
     def __init__(self, kernel, prior=None, noise=1e-3, use_gradients=False,
                  normalize_output=False, normalize_input=True,
-                 lower=None, upper=None, rng=None, device=0):
-        """Arguments as in gaussian_process.py:16-67, plus ``device`` (CUDA ordinal)."""
+                 lower=None, upper=None, rng=None, device=0, hyper_optimizer="host"):
+        """Arguments as in gaussian_process.py:16-67, plus ``device`` (CUDA ordinal) and ``hyper_optimizer``: "host"
+        (default) runs scipy's L-BFGS-B over nll() on the host; "device" runs it as one gpk_optimize_hypers call (see
+        the module docstring).  "device" raises TypeError for a prior other than None / DefaultPrior / EnvPrior /
+        MTBOPrior or a kernel the device cannot represent, and ValueError with use_gradients=True (the BFGS branch
+        has no device path)."""
+        if hyper_optimizer not in ("host", "device"):
+            raise ValueError("hyper_optimizer must be 'host' or 'device', not %r" % (hyper_optimizer,))
+        if hyper_optimizer == "device":
+            from robo_b200.models.gaussian_process_mcmc import _hyper_kernel, _hyper_prior
+            if use_gradients:
+                raise ValueError("hyper_optimizer='device' restates L-BFGS-B with finite differences; "
+                                 "use_gradients=True (BFGS with grad_nll) runs on the host only")
+            _hyper_prior(prior, "hyper_optimizer")
+            _hyper_kernel(kernel, "hyper_optimizer")
+        self.hyper_optimizer = hyper_optimizer
+        self._hyper_handle = None
+        self._hyper_fallback_logged = False
+        self.hyper_result = None
         if rng is None:
             self.rng = np.random.RandomState(np.random.randint(0, 10000))
         else:
@@ -51,6 +75,11 @@ class GaussianProcess(BaseModel):
         self.lower = lower
         self.upper = upper
         self.device = device
+
+    def __getstate__(self):
+        st = self.__dict__.copy()
+        st["_hyper_handle"] = None
+        return st
 
     # ------------------------------------------------------------------ train
     @BaseModel._check_shapes_train
@@ -162,14 +191,47 @@ class GaussianProcess(BaseModel):
         if self.use_gradients:
             res = optimize.minimize(self.nll, p0, method="BFGS", jac=self.grad_nll)
             theta = res.x
+        elif self._optimize_on_device():
+            return self._optimize_device(p0)
         else:
             try:
                 results = optimize.minimize(self.nll, p0, method='L-BFGS-B')
                 theta = results.x
+                self.hyper_result = dict(f=results.fun, nit=results.nit, nfev=results.nfev)
             except ValueError:
                 logging.error("Could not find a valid hyperparameter configuration! Use initial configuration")
                 theta = p0
         return theta
+
+    def _optimize_on_device(self):
+        from robo_b200 import _lib
+        if self.hyper_optimizer != "device":
+            return False
+        if len(self.X) > _lib.HYPER_MAX_N:
+            # the device keeps one factor per SM in shared memory: larger N optimises on the host
+            if not self._hyper_fallback_logged:
+                logger.info("N = %d exceeds GPK_HYPER_MAX_N = %d: the hyper-parameters are optimised on the host",
+                            len(self.X), _lib.HYPER_MAX_N)
+                self._hyper_fallback_logged = True
+            return False
+        return True
+
+    def _optimize_device(self, p0):
+        """optimize() as one gpk_optimize_hypers call on the training set of the handle's last set_data."""
+        from robo_b200 import _lib
+        from robo_b200.device_gp import TINY
+        from robo_b200.kernels import load_kernel
+        from robo_b200.models.gaussian_process_mcmc import _hyper_kernel, _hyper_prior
+        prior_kind, prior_par, n_ls, n_lr = _hyper_prior(self.prior, "hyper_optimizer")
+        f = _hyper_kernel(self.gp.kernel, "hyper_optimizer")
+        if self._hyper_handle is None:
+            self._hyper_handle = _lib.Handle(self.device)
+        h = self._hyper_handle
+        h.set_data(self.X, self.y)
+        load_kernel(h, f)
+        _lib.set_hyper_model(h, f["slots"], len(f["axis"]), float(self.mean), TINY, prior_kind, prior_par, n_ls, n_lr)
+        self.hyper_result = _lib.optimize_hypers(h, p0)
+        return self.hyper_result["theta"]
 
     # ------------------------------------------------------------------ posterior
     def predict_variance(self, x1, X2):

@@ -76,9 +76,9 @@ class _LikelihoodPool(object):
         self.handles = []
 
 
-def _hyper_prior(prior):
+def _hyper_prior(prior, option="hyper_sampler"):
     """(gpk_prior_kind, the 7 constants, n_ls, n_lr) of a prior the device restates: None, DefaultPrior, EnvPrior or
-    MTBOPrior (the reference's classes or robo_b200.priors'); TypeError for any other."""
+    MTBOPrior (the reference's classes or robo_b200.priors'); TypeError, naming `option`, for any other."""
     if prior is None:
         return _lib.PRIOR_NONE, None, 0, 0
     cls = type(prior)
@@ -95,16 +95,16 @@ def _hyper_prior(prior):
         par = [prior.ln_prior.sigma, prior.ln_prior.mean, prior.tophat.min, prior.tophat.max, prior.horseshoe.scale,
                prior.tophat_task.min, prior.tophat_task.max]
         return _lib.PRIOR_MTBO, par, int(prior.n_ls), int(prior.n_kt)
-    raise TypeError("hyper_sampler='device' restates None, DefaultPrior, EnvPrior and MTBOPrior only, not %s.%s"
-                    % (mod, cls.__name__))
+    raise TypeError("%s='device' restates None, DefaultPrior, EnvPrior and MTBOPrior only, not %s.%s"
+                    % (option, mod, cls.__name__))
 
 
-def _hyper_kernel(kernel):
-    """kernel.flatten(), or TypeError when the device cannot represent the kernel."""
+def _hyper_kernel(kernel, option="hyper_sampler"):
+    """kernel.flatten(), or TypeError, naming `option`, when the device cannot represent the kernel."""
     try:
         return kernel.flatten()
     except Exception as e:
-        raise TypeError("hyper_sampler='device' cannot represent this kernel: %s" % e)
+        raise TypeError("%s='device' cannot represent this kernel: %s" % (option, e))
 
 
 class GaussianProcessMCMC(BaseModel):

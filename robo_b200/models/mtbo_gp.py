@@ -29,10 +29,11 @@ def normalize(X, lower, upper):
 class MTBOGP(GaussianProcess):
 
     def __init__(self, kernel, prior=None, noise=1e-3, use_gradients=False, normalize_output=False, lower=None,
-                 upper=None, rng=None, device=0):
+                 upper=None, rng=None, device=0, hyper_optimizer="host"):
         super(MTBOGP, self).__init__(kernel=kernel, prior=prior, noise=noise, use_gradients=use_gradients,
                                      normalize_output=normalize_output, normalize_input=False,
-                                     lower=lower, upper=upper, rng=rng, device=device)
+                                     lower=lower, upper=upper, rng=rng, device=device,
+                                     hyper_optimizer=hyper_optimizer)
 
     def normalize(self, X):
         return normalize(X, self.lower, self.upper)
