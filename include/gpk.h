@@ -64,6 +64,10 @@ typedef enum {
  * lower triangle, which bounds the training points; theta holds at most GPK_HYPER_MAX_DIM entries (noise included) */
 #define GPK_HYPER_MAX_N 232
 #define GPK_HYPER_MAX_DIM 96
+/* the blocked hyper-parameter entry points (gpk_*_blocked): one fp64 matrix per theta in device memory, so the training
+ * points are bounded by the chunk's byte budget ("hyper_batch_bytes", default GPK_HYPER_BATCH_BYTES) instead */
+#define GPK_HYPER_BLOCKED_MAX_N 8192
+#define GPK_HYPER_BATCH_BYTES 4294967296L
 
 /* tasks of the multi-task factor (gpk_set_task_factor): n_tasks (n_tasks + 1) / 2 <= 36 Cholesky entries */
 #define GPK_MAX_TASKS 8
@@ -104,6 +108,9 @@ const char* gpk_version(void);
  *               2 = automatic [default]: on for N >= 6144, where the trailing updates gate the fit
  *   "diagprof"  1 = the diagonal-block kernel records clock64() stamps per phase (gpk_get_diag_profile)
  *   "overlap"   1 = build K* of chunk i+1 on the side stream while chunk i contracts [default]
+ *   "hyper_batch_bytes"  >= 1: device memory one chunk of the blocked hyper-parameter entry points (gpk_*_blocked)
+ *               may take for its matrices, (ceil(n / 128) + 2) ceil(n / 128) 131072 bytes per theta and a few kB
+ *               [default GPK_HYPER_BATCH_BYTES = 4 GiB: 7 thetas per chunk at n = 8192]; the results do not depend on it
  *   "meanonly"  1 = gpk_predict_mean (and the cost models of gpk_es_cost_multi) run the mean-only builder pass [default];
  *               0 = they take the mean of the full scoring pass, variance contraction included (tools/fabolas_acq_bench.py
  *               compares the two) */
@@ -771,6 +778,28 @@ int gpk_sample_hypers(gpk_handle* h, const double* p0, int nwalkers, int dim, in
 int gpk_optimize_hypers(gpk_handle* h, const double* p0, int dim, int maxcor, int maxiter, long maxfun, double ftol,
                         double pgtol, double eps, int maxls, double* theta, double* f, int* nit, long* nfev,
                         int* status);
+
+/* ---- the same at large N (robo_b200/csrc/gpk_hyper_blocked.cuh) ---------------------------------------------------
+ * gpk_hyper_lnpost_blocked, gpk_sample_hypers_blocked, gpk_optimize_hypers_blocked: the arguments, outputs and
+ * gpk_set_hyper_model state of gpk_hyper_lnpost, gpk_sample_hypers and gpk_optimize_hypers, for 2 <= n <=
+ * GPK_HYPER_BLOCKED_MAX_N.  The kernel matrix of every theta is built from theta in device memory and factored by the
+ * fit's blocked Cholesky (128-row blocks: its diagonal-block kernel once per matrix, its fp64 tile engine with job
+ * tables that span the chunk for the panel solves and trailing updates); the chunk holds as many thetas as
+ * "hyper_batch_bytes" (gpk_set_option) allows.  ll and lp follow gpk_hyper_lnpost's rules (-inf for any |theta_j| > 20,
+ * a pivot that is not > 0 or a non-finite result; lp the same prior routine, bit for bit); ll is another fixed-order
+ * evaluation of the same quantity, so it agrees with gpk_hyper_lnpost to rounding, not bit for bit.  The bits of a
+ * theta's ll and lp depend on theta, the data and n only, never on the chunk, the batch or the other thetas.  The
+ * sampler and the optimiser are gpk_sample_hypers's and gpk_optimize_hypers's runs over these values (the same Philox
+ * counters, rounding, L-BFGS-B update and status reads).  The chunk's device memory is released before each returns,
+ * whatever the outcome.
+ * GPK_BAD_ARG: as the counterpart, with n < 2 or n > GPK_HYPER_BLOCKED_MAX_N in place of n > GPK_HYPER_MAX_N, and one
+ * theta's matrix larger than "hyper_batch_bytes".  GPK_CUDA_ERROR: the chunk's memory could not be allocated. */
+int gpk_hyper_lnpost_blocked(gpk_handle* h, const double* theta, int count, int dim, double* ll, double* lp);
+int gpk_sample_hypers_blocked(gpk_handle* h, const double* p0, int nwalkers, int dim, int steps,
+                              unsigned long long seed, double* pos, double* lnpost, long* n_accepted);
+int gpk_optimize_hypers_blocked(gpk_handle* h, const double* p0, int dim, int maxcor, int maxiter, long maxfun,
+                                double ftol, double pgtol, double eps, int maxls, double* theta, double* f, int* nit,
+                                long* nfev, int* status);
 
 /* ---- Bayesian linear regression on the device (robo_b200/csrc/gpk_blr.cuh) ----------------------------------------
  * robo/models/bayesian_linear_regression.py with its default prior (robo/priors/bayesian_linear_regression_prior.py).

@@ -7,7 +7,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libgpk.so")
 SOURCES = ["gpk_api.cu"]
-HEADERS = ["gpk_internal.cuh", "gpk_gemm.cuh", "gpk_kernels.cuh", "gpk_diag16.cuh", "gpk_multi.inl", "gpk_ozaki.cuh", "gpk_de.cuh", "gpk_lbfgs.cuh", "gpk_cmaes.cuh", "gpk_direct.cuh", "gpk_es.cuh", "gpk_esmc.cuh", "gpk_rs.cuh", "gpk_hyper.cuh", "gpk_hyperopt.cuh", "gpk_blr.cuh", "gpk_rf.cuh", "gpk_bnn.cuh", "gpk_dngo.cuh", os.path.join("..", "..", "include", "gpk.h")]
+HEADERS = ["gpk_internal.cuh", "gpk_gemm.cuh", "gpk_kernels.cuh", "gpk_diag16.cuh", "gpk_multi.inl", "gpk_ozaki.cuh", "gpk_de.cuh", "gpk_lbfgs.cuh", "gpk_cmaes.cuh", "gpk_direct.cuh", "gpk_es.cuh", "gpk_esmc.cuh", "gpk_rs.cuh", "gpk_hyper.cuh", "gpk_hyperopt.cuh", "gpk_hyper_blocked.cuh", "gpk_blr.cuh", "gpk_rf.cuh", "gpk_bnn.cuh", "gpk_dngo.cuh", os.path.join("..", "..", "include", "gpk.h")]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC", "-shared"]
 

@@ -29,6 +29,8 @@ MAX_TASKS = 8                                 # GPK_MAX_TASKS
 HYPER_MAX_N = 232                              # GPK_HYPER_MAX_N: most training points of gpk_sample_hypers
 HYPER_MAX_DIM = 96                             # GPK_HYPER_MAX_DIM: most entries of theta (log noise included)
 HO_CHUNK = 16                                  # GPK_HO_CHUNK: rounds of gpk_optimize_hypers between two status reads
+HYPER_BLOCKED_MAX_N = 8192                     # GPK_HYPER_BLOCKED_MAX_N: most training points of gpk_*_blocked
+HYPER_BATCH_BYTES = 4294967296                 # GPK_HYPER_BATCH_BYTES: default chunk budget of gpk_*_blocked
 BLR_LINEAR, BLR_QUADRATIC, BLR_NONE = range(3)  # gpk_blr_basis: the features of a BayesianLinearRegression handle
 BLR_MAX_F = 64                                 # GPK_BLR_MAX_F: most features of a BayesianLinearRegression handle
 RF_MAX_N, RF_MAX_D, RF_MAX_T = 16384, 64, 512  # GPK_RF_MAX_N / GPK_RF_MAX_D / GPK_RF_MAX_T: the largest forest
@@ -164,6 +166,10 @@ _SIGNATURES = {
     "gpk_sample_hypers": [_vp, _dp, C.c_int, C.c_int, C.c_int, C.c_ulonglong, _dp, _dp, _lp],
     "gpk_optimize_hypers": [_vp, _dp, C.c_int, C.c_int, C.c_int, C.c_long, C.c_double, C.c_double, C.c_double, C.c_int,
                             _dp, _dp, _ip, _lp, _ip],
+    "gpk_optimize_hypers_blocked": [_vp, _dp, C.c_int, C.c_int, C.c_int, C.c_long, C.c_double, C.c_double, C.c_double, C.c_int,
+                            _dp, _dp, _ip, _lp, _ip],
+    "gpk_hyper_lnpost_blocked": [_vp, _dp, C.c_int, C.c_int, _dp, _dp],
+    "gpk_sample_hypers_blocked": [_vp, _dp, C.c_int, C.c_int, C.c_int, C.c_ulonglong, _dp, _dp, _lp],
     "gpk_blr_set_data": [_vp, _dp, _dp, C.c_int, C.c_int, C.c_int, _dp],
     "gpk_blr_lnpost": [_vp, _dp, C.c_int, _dp],
     "gpk_blr_sample": [_vp, C.c_ulonglong, C.c_int, _dp, C.c_int, _dp, _dp, _lp],
@@ -1294,30 +1300,42 @@ def set_hyper_model(handle, slots, n_terms, mean, tiny, prior_kind=PRIOR_NONE, p
                                                  _as_dp(par) if par is not None else None, int(n_ls), int(n_lr)))
 
 
-def hyper_lnpost(handle, thetas):
+def hyper_lnpost(handle, thetas, _fn="gpk_hyper_lnpost"):
     """gpk_hyper_lnpost: (log-likelihood, log-prior) of every row of thetas (count, dim), as gpk_sample_hypers computes
     them."""
     T = f64(np.atleast_2d(thetas))
     count, dim = T.shape
     ll, lp = np.empty(count), np.empty(count)
-    handle._check(handle.lib.gpk_hyper_lnpost(handle._h, _as_dp(T), count, dim, _as_dp(ll), _as_dp(lp)))
+    handle._check(getattr(handle.lib, _fn)(handle._h, _as_dp(T), count, dim, _as_dp(ll), _as_dp(lp)))
     return ll, lp
 
 
-def sample_hypers(handle, p0, steps, seed):
+def hyper_lnpost_blocked(handle, thetas):
+    """gpk_hyper_lnpost_blocked: hyper_lnpost for 2 <= N <= HYPER_BLOCKED_MAX_N, as gpk_sample_hypers_blocked and
+    gpk_optimize_hypers_blocked compute it (a batched blocked Cholesky per chunk of thetas)."""
+    return hyper_lnpost(handle, thetas, _fn="gpk_hyper_lnpost_blocked")
+
+
+def sample_hypers(handle, p0, steps, seed, _fn="gpk_sample_hypers"):
     """gpk_sample_hypers: one stretch-move run of the walkers p0 (nwalkers, dim) for `steps` steps ->
     dict(pos (nwalkers, dim), lnpost (nwalkers,), n_accepted (nwalkers,))."""
     P = f64(np.atleast_2d(p0))
     nw, dim = P.shape
     pos, lnp = np.empty((nw, dim)), np.empty(nw)
     acc = np.zeros(nw, dtype=np.int64)
-    handle._check(handle.lib.gpk_sample_hypers(handle._h, _as_dp(P), nw, dim, int(steps), int(seed) & 0xFFFFFFFFFFFFFFFF,
-                                               _as_dp(pos), _as_dp(lnp), acc.ctypes.data_as(_lp)))
+    handle._check(getattr(handle.lib, _fn)(handle._h, _as_dp(P), nw, dim, int(steps), int(seed) & 0xFFFFFFFFFFFFFFFF,
+                                           _as_dp(pos), _as_dp(lnp), acc.ctypes.data_as(_lp)))
     return dict(pos=pos, lnpost=lnp, n_accepted=acc)
 
 
+def sample_hypers_blocked(handle, p0, steps, seed):
+    """gpk_sample_hypers_blocked: sample_hypers over the log-posteriors of hyper_lnpost_blocked (N up to
+    HYPER_BLOCKED_MAX_N)."""
+    return sample_hypers(handle, p0, steps, seed, _fn="gpk_sample_hypers_blocked")
+
+
 def optimize_hypers(handle, p0, maxcor=10, maxiter=15000, maxfun=15000, ftol=2.220446049250313e-09, gtol=1e-5,
-                    eps=1e-8, maxls=20):
+                    eps=1e-8, maxls=20, _fn="gpk_optimize_hypers"):
     """gpk_optimize_hypers: scipy.optimize.minimize(nll, p0, method='L-BFGS-B') with scipy's default options, on the
     device -> dict(theta (dim,), f, nit, nfev, status (LB_*), rounds, noop_rounds).  rounds: the points scored (dim + 1
     evaluations each); noop_rounds: the launches after the final round that returned at once (the rest of the last
@@ -1327,12 +1345,18 @@ def optimize_hypers(handle, p0, maxcor=10, maxiter=15000, maxfun=15000, ftol=2.2
     theta = np.empty(dim)
     f, nfev = C.c_double(), C.c_long()
     nit, status = C.c_int(), C.c_int()
-    handle._check(handle.lib.gpk_optimize_hypers(handle._h, _as_dp(x0), dim, int(maxcor), int(maxiter), int(maxfun),
-                                                 float(ftol), float(gtol), float(eps), int(maxls), _as_dp(theta),
-                                                 C.byref(f), C.byref(nit), C.byref(nfev), C.byref(status)))
+    handle._check(getattr(handle.lib, _fn)(handle._h, _as_dp(x0), dim, int(maxcor), int(maxiter), int(maxfun),
+                                           float(ftol), float(gtol), float(eps), int(maxls), _as_dp(theta),
+                                           C.byref(f), C.byref(nit), C.byref(nfev), C.byref(status)))
     rounds = nfev.value // (dim + 1)
     return dict(theta=theta, f=f.value, nit=nit.value, nfev=nfev.value, status=status.value, rounds=rounds,
                 noop_rounds=-(-rounds // HO_CHUNK) * HO_CHUNK - rounds)
+
+
+def optimize_hypers_blocked(handle, p0, **opt):
+    """gpk_optimize_hypers_blocked: optimize_hypers over the objective of hyper_lnpost_blocked (N up to
+    HYPER_BLOCKED_MAX_N); the same options and result."""
+    return optimize_hypers(handle, p0, _fn="gpk_optimize_hypers_blocked", **opt)
 
 
 def blr_features(n_dims, basis):

@@ -34,6 +34,7 @@
 #include "gpk_rs.cuh"
 #include "gpk_hyper.cuh"
 #include "gpk_hyperopt.cuh"
+#include "gpk_hyper_blocked.cuh"
 #include "gpk_blr.cuh"
 #include "gpk_rf.cuh"
 #include "gpk_bnn.cuh"
@@ -172,6 +173,11 @@ struct gpk_handle {
     bool has_hyper = false;
     HyperModel hyper;
     DevBuf hy_buf;
+    // the blocked path (gpk_hyper_blocked.cuh): one chunk's matrices, parameters and block log-sums, released at the end
+    // of every call; the chunk's byte budget ("hyper_batch_bytes")
+    DevBuf hb_buf;
+    GemmJob* hb_jobs = nullptr;     // the chunk's job tables, inside hb_buf
+    long hyper_batch_bytes = GPK_HYPER_BATCH_BYTES;
     // a surrogate handle serves its own entry points and the scoring ones only; its scoring pass uses block_best, best
     // and nneg as the GP's does
     ModelKind model = MODEL_GP;
@@ -1543,7 +1549,7 @@ int gpk_destroy(gpk_handle* h) {
                       &h->out_var, &h->out_acq, &h->block_best, &h->best, &h->nneg, &h->Vt, &h->cov, &h->XsT,
                       &h->tmpjobs, &h->alpha, &h->tmp1, &h->tmp2, &h->tmp3, &h->dprof, &h->Xts, &h->oz_Pq, &h->oz_Kq, &h->oz_Kq2, &h->oz_eP, &h->oz_emax, &h->oz_pmu2, &h->oz_probe,
                       &h->multi_cand, &h->multi_A, &h->multi_B, &h->multi_out, &h->multi_bb, &h->gather, &h->best_global,
-                      &h->de_pop, &h->de_trial, &h->de_param, &h->de_E, &h->de_small, &h->de_sort, &h->lb_buf, &h->cma_buf, &h->dir_buf, &h->ep_buf, &h->es_state, &h->es_U, &h->es_work, &h->es_in, &h->mc_state, &h->mc_buf, &h->mc_stat, &h->fab_in, &h->rs_buf, &h->hy_buf,
+                      &h->de_pop, &h->de_trial, &h->de_param, &h->de_E, &h->de_small, &h->de_sort, &h->lb_buf, &h->cma_buf, &h->dir_buf, &h->ep_buf, &h->es_state, &h->es_U, &h->es_work, &h->es_in, &h->mc_state, &h->mc_buf, &h->mc_stat, &h->fab_in, &h->rs_buf, &h->hy_buf, &h->hb_buf,
                       &h->blr_data, &h->blr_post, &h->blr_work, &h->rf_data, &h->rf_work, &h->rf_nodes,
                       &h->bnn_data, &h->bnn_samples, &h->bnn_state, &h->dngo_net, &h->dngo_state, &h->dngo_pack};
     for (DevBuf* b : bufs)
@@ -1619,6 +1625,11 @@ int gpk_set_option(gpk_handle* h, const char* key, long value) {
                 CK(cudaMemcpy((char*)h->dprof.p + 63 * 8, &one, 8, cudaMemcpyHostToDevice));
             }
         }
+        return GPK_OK;
+    }
+    if (!strcmp(key, "hyper_batch_bytes")) {
+        if (value < 1) BAD("hyper_batch_bytes must be >= 1 (default %ld)", (long)GPK_HYPER_BATCH_BYTES);
+        h->hyper_batch_bytes = value;
         return GPK_OK;
     }
     if (!strcmp(key, "chunk")) {
@@ -2622,8 +2633,9 @@ int gpk_set_hyper_model(gpk_handle* h, int n_params, const int* amp_slot, const 
 }
 
 namespace {
-// the preconditions of gpk_hyper_lnpost / gpk_sample_hypers, and the kernels' shared-memory opt-in
-int hyper_ready(gpk_handle* h, int dim, const char* who) {
+// the preconditions of the hyper-parameter entry points; blocked: the gpk_*_blocked ones (n up to
+// GPK_HYPER_BLOCKED_MAX_N)
+int hyper_check(gpk_handle* h, int dim, const char* who, bool blocked) {
     int rc = require(h, true, true, false);
     if (rc) return rc;
     if (!h->has_hyper) BAD("%s: gpk_set_hyper_model has not been called", who);
@@ -2639,9 +2651,19 @@ int hyper_ready(gpk_handle* h, int dim, const char* who) {
             BAD("%s: the kernel structure changed since gpk_set_hyper_model", who);
         if (m.axis[t] >= h->d) BAD("%s: kernel axis %d >= d = %d", who, m.axis[t], h->d);
     }
-    if (h->n > GPK_HYPER_MAX_N) BAD("%s: n = %d exceeds GPK_HYPER_MAX_N = %d", who, h->n, GPK_HYPER_MAX_N);
+    if (!blocked && h->n > GPK_HYPER_MAX_N)
+        BAD("%s: n = %d exceeds GPK_HYPER_MAX_N = %d", who, h->n, GPK_HYPER_MAX_N);
+    if (blocked && (h->n < 2 || h->n > GPK_HYPER_BLOCKED_MAX_N))
+        BAD("%s: need 2 <= n <= GPK_HYPER_BLOCKED_MAX_N = %d (n = %d)", who, GPK_HYPER_BLOCKED_MAX_N, h->n);
     if (dim != m.n_params + 1) BAD("%s: dim = %d, the slot table needs %d", who, dim, m.n_params + 1);
     CK(cudaSetDevice(h->device));
+    return GPK_OK;
+}
+
+// the preconditions of gpk_hyper_lnpost / gpk_sample_hypers, and the kernels' shared-memory opt-in
+int hyper_ready(gpk_handle* h, int dim, const char* who) {
+    int rc = hyper_check(h, dim, who, false);
+    if (rc) return rc;
     const int smem = (int)(gpk_hy_smem_doubles(h->n) * 8);
     CK(cudaFuncSetAttribute(gpk_hy_eval_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     CK(cudaFuncSetAttribute(gpk_hy_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
@@ -2670,38 +2692,40 @@ int gpk_hyper_lnpost(gpk_handle* h, const double* theta, int count, int dim, dou
     return GPK_OK;
 }
 
-int gpk_sample_hypers(gpk_handle* h, const double* p0, int nwalkers, int dim, int steps, unsigned long long seed,
-                      double* pos, double* lnpost, long* n_accepted) {
-    static_assert(sizeof(long) == sizeof(long long) && sizeof(long long) == sizeof(double),
-                  "the accept counts travel in the walkers' transfer");
-    if (!h) return GPK_BAD_ARG;
-    const char* who = "gpk_sample_hypers";
+extern "C++" {                     // the shared drivers are templates over the launches they enqueue
+namespace {
+// the argument checks gpk_sample_hypers and gpk_sample_hypers_blocked share (before their hyper-model checks)
+int hy_args(gpk_handle* h, const char* who, const double* p0, int nwalkers, int dim, int steps, const double* pos,
+            const double* lnpost) {
     if (!p0 || !pos || !lnpost) BAD("%s: need p0, pos and lnpost", who);
     if (nwalkers % 2 != 0 || nwalkers < 2 * dim || nwalkers < 2)
         BAD("%s: need an even number of walkers >= 2 dim (nwalkers = %d, dim = %d)", who, nwalkers, dim);
     if (steps < 0) BAD("%s: need steps >= 0", who);
-    int rc = hyper_ready(h, dim, who);
-    if (rc) return rc;
-    // P (nwalkers x dim), L (nwalkers), accept counts (nwalkers): contiguous, so that one copy brings the run back
+    return GPK_OK;
+}
+
+// One EnsembleSampler.run_mcmc on the device, shared by both samplers: P (nwalkers x dim), L (nwalkers) and the accept
+// counts (nwalkers) contiguous in h->hy_buf, so that one copy brings the run back, then `extra` doubles for the caller.
+// score(P, L, extra) enqueues the initial log-posteriors, half(s, half, P, L, acc, extra) one half-step; no host
+// synchronisation until the final copy.
+template <class Score, class Half>
+int hy_run(gpk_handle* h, const double* p0, int nwalkers, int dim, int steps, size_t extra, Score score, Half half,
+           double* pos, double* lnpost, long* n_accepted) {
+    static_assert(sizeof(long) == sizeof(long long) && sizeof(long long) == sizeof(double),
+                  "the accept counts travel in the walkers' transfer");
     const size_t nP = (size_t)nwalkers * dim, total = nP + 2 * (size_t)nwalkers;
-    if ((rc = ensure(h, h->hy_buf, total * 8))) return rc;
+    int rc = ensure(h, h->hy_buf, (total + extra) * 8);
+    if (rc) return rc;
     double* P = ptr<double>(h->hy_buf);
     double* L = P + nP;
     long long* acc = (long long*)(L + nwalkers);
-    const size_t smem = gpk_hy_smem_doubles(h->n) * 8;
-    const double* Xt = ptr<double>(h->Xt);
-    const double* y = ptr<double>(h->y);
+    double* ex = P + total;
     CK(cudaMemcpyAsync(P, p0, nP * 8, cudaMemcpyHostToDevice, h->stream));
     CK(cudaMemsetAsync(acc, 0, (size_t)nwalkers * 8, h->stream));
-    gpk_hy_eval_kernel<<<nwalkers, GPK_HY_THREADS, smem, h->stream>>>(h->hyper, Xt, h->NP, y, h->n, P, nullptr,
-                                                                      nullptr, L);
-    CKL();
+    if ((rc = score(P, L, ex))) return rc;
     for (int s = 0; s < steps; ++s)
-        for (int half = 0; half < 2; ++half) {
-            gpk_hy_step_kernel<<<nwalkers / 2, GPK_HY_THREADS, smem, h->stream>>>(h->hyper, Xt, h->NP, y, h->n,
-                                                                                nwalkers, s, half, seed, P, L, acc);
-            CKL();
-        }
+        for (int hf = 0; hf < 2; ++hf)
+            if ((rc = half(s, hf, P, L, acc, ex))) return rc;
     std::vector<double> out(total);
     CK(cudaMemcpyAsync(out.data(), P, total * 8, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
@@ -2711,12 +2735,9 @@ int gpk_sample_hypers(gpk_handle* h, const double* p0, int nwalkers, int dim, in
     return GPK_OK;
 }
 
-// GaussianProcess.optimize on the device (gpk_hyperopt.cuh; gaussian_process.py:193-219)
-int gpk_optimize_hypers(gpk_handle* h, const double* p0, int dim, int maxcor, int maxiter, long maxfun, double ftol,
-                        double pgtol, double eps, int maxls, double* theta, double* f, int* nit, long* nfev,
-                        int* status) {
-    if (!h) return GPK_BAD_ARG;
-    const char* who = "gpk_optimize_hypers";
+// the argument checks gpk_optimize_hypers and gpk_optimize_hypers_blocked share (before their hyper-model checks)
+int ho_args(gpk_handle* h, const char* who, const double* p0, const double* theta, int dim, int maxcor, int maxiter,
+            long maxfun, double eps, int maxls) {
     if (!p0 || !theta) BAD("%s: need p0 and theta", who);
     if (dim < 1 || dim > GPK_HYPER_MAX_DIM) BAD("%s: need 1 <= dim <= %d (dim = %d)", who, GPK_HYPER_MAX_DIM, dim);
     for (int j = 0; j < dim; ++j)
@@ -2725,13 +2746,20 @@ int gpk_optimize_hypers(gpk_handle* h, const double* p0, int dim, int maxcor, in
     if (maxls < 1) BAD("%s: need maxls >= 1 (maxls = %d)", who, maxls);
     if (!(eps > 0.0)) BAD("%s: need eps > 0 (eps = %g)", who, eps);
     if (maxiter < 1 || maxfun < 1) BAD("%s: need maxiter >= 1 and maxfun >= 1 (%d, %ld)", who, maxiter, maxfun);
-    int rc = hyper_ready(h, dim, who);
-    if (rc) return rc;
-    const size_t smem = gpk_hy_smem_doubles(h->n) * 8;
-    CK(cudaFuncSetAttribute(gpk_ho_round_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    return GPK_OK;
+}
+
+// One L-BFGS-B run on the device, shared by both optimisers: the state record, the work buffer and `extra` doubles for
+// the caller in h->hy_buf; round(dst, work, q, extra) enqueues one round; the host reads the status once per
+// GPK_HO_CHUNK rounds.
+template <class Round>
+int ho_run(gpk_handle* h, const double* p0, int dim, int maxcor, int maxiter, long maxfun, double ftol, double pgtol,
+           double eps, int maxls, size_t extra, Round round, double* theta, double* f, int* nit, long* nfev,
+           int* status) {
     // the state record, then the work buffer
     const size_t nst = (sizeof(HOState) + 7) / 8, nw = (size_t)gpk_ho_work_doubles(dim, maxcor);
-    if ((rc = ensure(h, h->hy_buf, (nst + nw) * 8))) return rc;
+    int rc = ensure(h, h->hy_buf, (nst + nw + extra) * 8);
+    if (rc) return rc;
     HOState* dst = ptr<HOState>(h->hy_buf);
     double* work = ptr<double>(h->hy_buf) + nst;
     const HOWork w = gpk_ho_work(work, dim, maxcor);
@@ -2745,14 +2773,10 @@ int gpk_optimize_hypers(gpk_handle* h, const double* p0, int dim, int maxcor, in
     q.pgtol = pgtol; q.eps = eps;
     CK(cudaMemcpyAsync(dst, &s0, sizeof(s0), cudaMemcpyHostToDevice, h->stream));
     CK(cudaMemcpyAsync(w.xt, p0, (size_t)dim * 8, cudaMemcpyHostToDevice, h->stream));
-    const double* Xt = ptr<double>(h->Xt);
-    const double* y = ptr<double>(h->y);
     int* pst = reinterpret_cast<int*>(h->pin);
     for (;;) {
-        for (int r = 0; r < GPK_HO_CHUNK; ++r) {
-            gpk_ho_round_kernel<<<dim + 1, GPK_HY_THREADS, smem, h->stream>>>(h->hyper, Xt, h->NP, y, h->n, q, work, dst);
-            CKL();
-        }
+        for (int r = 0; r < GPK_HO_CHUNK; ++r)
+            if ((rc = round(dst, work, q, work + nw))) return rc;
         CK(cudaMemcpyAsync(pst, &dst->status, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
         CK(cudaStreamSynchronize(h->stream));
         if (*pst != GPK_LB_RUNNING) break;
@@ -2766,6 +2790,288 @@ int gpk_optimize_hypers(gpk_handle* h, const double* p0, int dim, int maxcor, in
     if (nfev) *nfev = (long)s.nfev;
     if (status) *status = s.status;
     return GPK_OK;
+}
+}  // namespace
+}  // extern "C++"
+
+int gpk_sample_hypers(gpk_handle* h, const double* p0, int nwalkers, int dim, int steps, unsigned long long seed,
+                      double* pos, double* lnpost, long* n_accepted) {
+    if (!h) return GPK_BAD_ARG;
+    const char* who = "gpk_sample_hypers";
+    int rc = hy_args(h, who, p0, nwalkers, dim, steps, pos, lnpost);
+    if (rc) return rc;
+    if ((rc = hyper_ready(h, dim, who))) return rc;
+    const size_t smem = gpk_hy_smem_doubles(h->n) * 8;
+    const double* Xt = ptr<double>(h->Xt);
+    const double* y = ptr<double>(h->y);
+    auto score = [&](double* P, double* L, double*) -> int {
+        gpk_hy_eval_kernel<<<nwalkers, GPK_HY_THREADS, smem, h->stream>>>(h->hyper, Xt, h->NP, y, h->n, P, nullptr,
+                                                                          nullptr, L);
+        CKL();
+        return GPK_OK;
+    };
+    auto half = [&](int s, int hf, double* P, double* L, long long* acc, double*) -> int {
+        gpk_hy_step_kernel<<<nwalkers / 2, GPK_HY_THREADS, smem, h->stream>>>(h->hyper, Xt, h->NP, y, h->n, nwalkers,
+                                                                            s, hf, seed, P, L, acc);
+        CKL();
+        return GPK_OK;
+    };
+    return hy_run(h, p0, nwalkers, dim, steps, 0, score, half, pos, lnpost, n_accepted);
+}
+
+// GaussianProcess.optimize on the device (gpk_hyperopt.cuh; gaussian_process.py:193-219)
+int gpk_optimize_hypers(gpk_handle* h, const double* p0, int dim, int maxcor, int maxiter, long maxfun, double ftol,
+                        double pgtol, double eps, int maxls, double* theta, double* f, int* nit, long* nfev,
+                        int* status) {
+    if (!h) return GPK_BAD_ARG;
+    const char* who = "gpk_optimize_hypers";
+    int rc = ho_args(h, who, p0, theta, dim, maxcor, maxiter, maxfun, eps, maxls);
+    if (rc) return rc;
+    if ((rc = hyper_ready(h, dim, who))) return rc;
+    const size_t smem = gpk_hy_smem_doubles(h->n) * 8;
+    CK(cudaFuncSetAttribute(gpk_ho_round_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const double* Xt = ptr<double>(h->Xt);
+    const double* y = ptr<double>(h->y);
+    auto round = [&](HOState* dst, double* work, const HOParams& q, double*) -> int {
+        gpk_ho_round_kernel<<<dim + 1, GPK_HY_THREADS, smem, h->stream>>>(h->hyper, Xt, h->NP, y, h->n, q, work, dst);
+        CKL();
+        return GPK_OK;
+    };
+    return ho_run(h, p0, dim, maxcor, maxiter, maxfun, ftol, pgtol, eps, maxls, 0, round, theta, f, nit, nfev, status);
+}
+
+// ---------------------------------------------------------------------------------------
+// The same three at large N (gpk_hyper_blocked.cuh): every theta's matrix in HBM, factored by the fit's diagonal-block
+// kernel and tile engine with job tables that span the chunk
+// ---------------------------------------------------------------------------------------
+namespace {
+// HBM layout of one chunk of B thetas in h->hb_buf: B matrices (one stacked array, tensor map mapA), B P strips
+// (mapP), B HBPar, B x nb block log-sums, B status words and the chunk's skip word
+struct HBChunk {
+    int B = 0;
+    double* A = nullptr;
+    double* P = nullptr;
+    HBPar* par = nullptr;
+    double* logpart = nullptr;
+    int* st = nullptr;
+    int* skip = nullptr;
+    CUtensorMap mapA, mapP;
+    std::vector<Range> panel_r, update_r;       // per step k: the jobs of matrix 0; matrix b follows at + b cnt
+};
+
+// The chunk size under the handle's byte budget for `count` thetas, its buffer, tensor maps and job tables.  The jobs of
+// step k are matrix-major (matrix b's jobs are rows b R of the stacked array), so a chunk of B' <= B matrices launches
+// the first B' cnt of them.
+int hb_reserve(gpk_handle* h, int count, const char* who, HBChunk* c) {
+    const int n = h->n, nb = gpk_hb_nb(n);
+    const long NP = (long)nb * HB_T, R = NP + HB_T;
+    const long per = gpk_hb_theta_bytes(n);
+    const long fit = h->hyper_batch_bytes / per;
+    if (fit < 1)
+        BAD("%s: one theta needs %ld bytes at n = %d, more than hyper_batch_bytes = %ld", who, per, n,
+            h->hyper_batch_bytes);
+    c->B = (int)std::min<long>(std::min<long>(fit, count), 32768);
+    const int B = c->B;
+    const size_t nA = (size_t)B * R * NP, nPs = (size_t)B * HB_T * NP, npar = (size_t)B * ((sizeof(HBPar) + 7) / 8);
+    const size_t nlog = (size_t)B * nb, nst = ((size_t)B + 2) / 2;
+    if ((size_t)B * R > (size_t)INT_MAX) BAD("%s: the chunk's rows exceed the job table's range", who);
+    // the job tables
+    std::vector<GemmJob> jobs;
+    c->panel_r.assign(nb, Range());
+    c->update_r.assign(nb, Range());
+    for (int k = 0; k < nb; ++k) {
+        c->panel_r[k].off = (int)jobs.size();
+        for (int b = 0; b < B; ++b) {
+            const int r0 = (int)(b * R), p0 = b * HB_T;
+            for (int i = k + 1; i <= nb; ++i)
+                jobs.push_back({r0 + i * HB_T, p0, k * HB_T, (k + 1) * HB_T, r0 + i * HB_T, k * HB_T, 0, 0});
+            if (b == 0) c->panel_r[k].cnt = (int)jobs.size() - c->panel_r[k].off;
+        }
+        c->update_r[k].off = (int)jobs.size();
+        for (int b = 0; b < B; ++b) {
+            const int r0 = (int)(b * R);
+            for (int j = k + 1; j < nb; ++j)
+                for (int i = j; i <= nb; ++i)
+                    jobs.push_back({r0 + i * HB_T, r0 + j * HB_T, k * HB_T, (k + 1) * HB_T, r0 + i * HB_T, j * HB_T, 0, 0});
+            if (b == 0) c->update_r[k].cnt = (int)jobs.size() - c->update_r[k].off;
+        }
+    }
+    const size_t njob = (jobs.size() * sizeof(GemmJob) + 7) / 8;
+    int rc = ensure(h, h->hb_buf, (nA + nPs + npar + nlog + nst + njob) * 8);
+    if (rc) return rc;
+    c->A = ptr<double>(h->hb_buf);
+    c->P = c->A + nA;
+    c->par = reinterpret_cast<HBPar*>(c->P + nPs);
+    c->logpart = c->P + nPs + npar;
+    c->st = reinterpret_cast<int*>(c->logpart + nlog);
+    c->skip = c->st + B;
+    GemmJob* djobs = reinterpret_cast<GemmJob*>(c->logpart + nlog + nst);
+    if (!jobs.empty())
+        CK(cudaMemcpyAsync(djobs, jobs.data(), jobs.size() * sizeof(GemmJob), cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemsetAsync(c->skip, 0, sizeof(int), h->stream));
+    CK(cudaStreamSynchronize(h->stream));         // the host job vector goes out of scope
+    h->hb_jobs = djobs;
+    if ((rc = make_map(h, &c->mapA, c->A, (long)B * R, NP, NP))) return rc;
+    if ((rc = make_map(h, &c->mapP, c->P, (long)B * HB_T, NP, NP))) return rc;
+    return GPK_OK;
+}
+
+// the chunk buffer goes back at the end of every blocked call, whatever its outcome (it can take most of the budget)
+void hb_release(gpk_handle* h) {
+    if (h->hb_buf.p) cudaFree(h->hb_buf.p);
+    h->hb_buf.p = nullptr;
+    h->hb_buf.cap = 0;
+    h->hb_jobs = nullptr;
+}
+
+// The log-posterior parts of the count thetas T (device, count x dim) in chunks of c.B, enqueued on the handle's stream
+// without a host synchronisation; ll / lp / post / fobj (device, count each) may be NULL.  skip (device, may be NULL:
+// the chunk's own zero word): non-zero makes every launch return at once.
+int hb_score(gpk_handle* h, const HBChunk& c, const double* T, int count, const int* skip, double* ll, double* lp,
+             double* post, double* fobj) {
+    const int n = h->n, nb = gpk_hb_nb(n), D = h->hyper.n_params + 1;
+    const long NP = (long)nb * HB_T, R = NP + HB_T;
+    if (!skip) skip = c.skip;
+    auto at = [](double* p, int off) { return p ? p + off : nullptr; };
+    int rc;
+    for (int c0 = 0; c0 < count; c0 += c.B) {
+        const int B = std::min(c.B, count - c0);
+        // the P strips: zero right of the diagonal 16-blocks, where the diagonal kernel never stores
+        CK(cudaMemsetAsync(c.P, 0, (size_t)B * HB_T * NP * 8, h->stream));
+        gpk_hb_prep_kernel<<<B, 32, 0, h->stream>>>(h->hyper, T + (size_t)c0 * D, skip, c.par, c.st);
+        CKL();
+        gpk_hb_build_kernel<<<dim3(nb, nb + 1, B), 256, 0, h->stream>>>(h->hyper, ptr<double>(h->Xt), h->NP,
+                                                                        ptr<double>(h->y), n, c.par, c.A);
+        CKL();
+        for (int k = 0; k < nb; ++k) {
+            for (int b = 0; b < B; ++b) {
+                // the fit's diagonal kernel on matrix b; it stores inv(L_kk) at P + k 128 ldp + k 128, which the
+                // offset base puts at row 0, column k 128 of matrix b's strip
+                double* Pb = reinterpret_cast<double*>(reinterpret_cast<uintptr_t>(c.P + (size_t)b * HB_T * NP) -
+                                                       (uintptr_t)k * HB_T * NP * 8);
+                gpk_potrf_diag_dmma_kernel<<<1, 256, DIAG_SMEM, h->stream>>>(c.A + (size_t)b * R * NP, NP, k, Pb,
+                                                                             nullptr, NP, c.st + b,
+                                                                             c.logpart + (size_t)b * nb, nullptr);
+                CKL();
+            }
+            GemmArgs a;
+            memset(&a, 0, sizeof(a));
+            a.A = c.A; a.lda = NP;
+            a.B = c.P; a.ldb = NP;
+            a.C = c.A; a.ldc = NP;
+            a.alpha = 1.0; a.beta = 0;
+            a.job_mode = JOBS_TABLE;
+            a.status = skip;
+            a.jobs = h->hb_jobs + c.panel_r[k].off;
+            if ((rc = launch_gemm<EPI_STORE>(h, c.mapA, c.mapP, a, B * c.panel_r[k].cnt))) return rc;
+            if (c.update_r[k].cnt > 0) {
+                a.B = c.A;
+                a.alpha = -1.0; a.beta = 1;
+                a.jobs = h->hb_jobs + c.update_r[k].off;
+                if ((rc = launch_gemm<EPI_STORE>(h, c.mapA, c.mapA, a, B * c.update_r[k].cnt))) return rc;
+            }
+        }
+        gpk_hb_finish_kernel<<<B, GPK_HY_THREADS, 0, h->stream>>>(h->hyper, n, c.par, c.A, c.logpart, c.st, at(ll, c0),
+                                                                  at(lp, c0), at(post, c0), at(fobj, c0));
+        CKL();
+    }
+    return GPK_OK;
+}
+
+int hyper_lnpost_blocked(gpk_handle* h, const double* theta, int count, int dim, double* ll, double* lp) {
+    const char* who = "gpk_hyper_lnpost_blocked";
+    if (count < 1 || !theta || !ll || !lp) BAD("%s: need count >= 1, theta, ll and lp", who);
+    int rc = hyper_check(h, dim, who, true);
+    if (rc) return rc;
+    HBChunk c;
+    if ((rc = hb_reserve(h, count, who, &c))) return rc;
+    const size_t nT = (size_t)count * dim;
+    if ((rc = ensure(h, h->hy_buf, (nT + 2 * (size_t)count) * 8))) return rc;
+    double* dT = ptr<double>(h->hy_buf);
+    double* dll = dT + nT;
+    double* dlp = dll + count;
+    CK(cudaMemcpyAsync(dT, theta, nT * 8, cudaMemcpyHostToDevice, h->stream));
+    if ((rc = hb_score(h, c, dT, count, nullptr, dll, dlp, nullptr, nullptr))) return rc;
+    CK(cudaMemcpyAsync(ll, dll, (size_t)count * 8, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaMemcpyAsync(lp, dlp, (size_t)count * 8, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    return GPK_OK;
+}
+
+int sample_hypers_blocked(gpk_handle* h, const double* p0, int nwalkers, int dim, int steps, unsigned long long seed,
+                          double* pos, double* lnpost, long* n_accepted) {
+    const char* who = "gpk_sample_hypers_blocked";
+    int rc = hy_args(h, who, p0, nwalkers, dim, steps, pos, lnpost);
+    if (rc) return rc;
+    if ((rc = hyper_check(h, dim, who, true))) return rc;
+    HBChunk c;
+    if ((rc = hb_reserve(h, nwalkers, who, &c))) return rc;
+    // after the walkers: the proposals Q (nwalkers / 2 x dim) and their log-posteriors V
+    const int hb = nwalkers / 2;
+    auto score = [&](double* P, double* L, double*) {
+        return hb_score(h, c, P, nwalkers, nullptr, nullptr, nullptr, L, nullptr);
+    };
+    auto half = [&](int s, int hf, double* P, double* L, long long* acc, double* Q) -> int {
+        double* V = Q + (size_t)hb * dim;
+        gpk_hb_propose_kernel<<<hb, 32, 0, h->stream>>>(dim, nwalkers, s, hf, seed, P, Q);
+        CKL();
+        int r = hb_score(h, c, Q, hb, nullptr, nullptr, nullptr, V, nullptr);
+        if (r) return r;
+        gpk_hb_accept_kernel<<<hb, 32, 0, h->stream>>>(dim, nwalkers, s, hf, seed, Q, V, P, L, acc);
+        CKL();
+        return GPK_OK;
+    };
+    return hy_run(h, p0, nwalkers, dim, steps, (size_t)hb * dim + hb, score, half, pos, lnpost, n_accepted);
+}
+
+int optimize_hypers_blocked(gpk_handle* h, const double* p0, int dim, int maxcor, int maxiter, long maxfun, double ftol,
+                            double pgtol, double eps, int maxls, double* theta, double* f, int* nit, long* nfev,
+                            int* status) {
+    const char* who = "gpk_optimize_hypers_blocked";
+    int rc = ho_args(h, who, p0, theta, dim, maxcor, maxiter, maxfun, eps, maxls);
+    if (rc) return rc;
+    if ((rc = hyper_check(h, dim, who, true))) return rc;
+    HBChunk c;
+    if ((rc = hb_reserve(h, dim + 1, who, &c))) return rc;
+    // after the work buffer: the stencil's thetas ((dim + 1) x dim); the chunk's skip word rises with the final status
+    auto round = [&](HOState* dst, double* work, const HOParams& q, double* T) -> int {
+        gpk_hb_stencil_kernel<<<dim + 1, 32, 0, h->stream>>>(dim, q, work, dst, T);
+        CKL();
+        const HOWork w = gpk_ho_work(work, dim, q.maxcor);
+        int r = hb_score(h, c, T, dim + 1, c.skip, nullptr, nullptr, nullptr, w.fv);
+        if (r) return r;
+        gpk_hb_update_ho_kernel<<<1, 32, 0, h->stream>>>(dim, q, work, dst, c.skip);
+        CKL();
+        return GPK_OK;
+    };
+    return ho_run(h, p0, dim, maxcor, maxiter, maxfun, ftol, pgtol, eps, maxls, (size_t)(dim + 1) * dim, round, theta,
+                  f, nit, nfev, status);
+}
+}  // namespace
+
+int gpk_hyper_lnpost_blocked(gpk_handle* h, const double* theta, int count, int dim, double* ll, double* lp) {
+    if (!h) return GPK_BAD_ARG;
+    const int rc = hyper_lnpost_blocked(h, theta, count, dim, ll, lp);
+    hb_release(h);
+    return rc;
+}
+
+int gpk_sample_hypers_blocked(gpk_handle* h, const double* p0, int nwalkers, int dim, int steps, unsigned long long seed,
+                              double* pos, double* lnpost, long* n_accepted) {
+    if (!h) return GPK_BAD_ARG;
+    const int rc = sample_hypers_blocked(h, p0, nwalkers, dim, steps, seed, pos, lnpost, n_accepted);
+    hb_release(h);
+    return rc;
+}
+
+int gpk_optimize_hypers_blocked(gpk_handle* h, const double* p0, int dim, int maxcor, int maxiter, long maxfun,
+                                double ftol, double pgtol, double eps, int maxls, double* theta, double* f, int* nit,
+                                long* nfev, int* status) {
+    if (!h) return GPK_BAD_ARG;
+    const int rc = optimize_hypers_blocked(h, p0, dim, maxcor, maxiter, maxfun, ftol, pgtol, eps, maxls, theta, f, nit,
+                                           nfev, status);
+    hb_release(h);
+    return rc;
 }
 
 // ---------------------------------------------------------------------------------------

@@ -20,7 +20,10 @@ Hyper-parameter optimisation (gaussian_process.py:193-219) runs where ``hyper_op
     launch (the likelihood of one theta per CTA, as gpk_sample_hypers computes it) and runs L-BFGS-B's update on the
     device.  The likelihood is the same function as nll() computed by another routine, so the two arms agree to
     rounding at every point and may part where L-BFGS-B's decisions are that close; it needs N <= GPK_HYPER_MAX_N
-    (larger N optimises on the host) and a kernel and prior the device restates.
+    (larger N optimises on the host) and a kernel and prior the device restates;
+  - "device_blocked": the same run as one gpk_optimize_hypers_blocked call (robo_b200/csrc/gpk_hyper_blocked.cuh),
+    each round's stencil scored by one batched blocked Cholesky over the kernel matrices in device memory, at every N
+    up to GPK_HYPER_BLOCKED_MAX_N (8192) and without a fallback.
 """
 import logging
 
@@ -41,18 +44,19 @@ class GaussianProcess(BaseModel):
                  lower=None, upper=None, rng=None, device=0, hyper_optimizer="host"):
         """Arguments as in gaussian_process.py:16-67, plus ``device`` (CUDA ordinal) and ``hyper_optimizer``: "host"
         (default) runs scipy's L-BFGS-B over nll() on the host; "device" runs it as one gpk_optimize_hypers call (see
-        the module docstring).  "device" raises TypeError for a prior other than None / DefaultPrior / EnvPrior /
-        MTBOPrior or a kernel the device cannot represent, and ValueError with use_gradients=True (the BFGS branch
-        has no device path)."""
-        if hyper_optimizer not in ("host", "device"):
-            raise ValueError("hyper_optimizer must be 'host' or 'device', not %r" % (hyper_optimizer,))
-        if hyper_optimizer == "device":
-            from robo_b200.models.gaussian_process_mcmc import _hyper_kernel, _hyper_prior
+        the module docstring), "device_blocked" as one gpk_optimize_hypers_blocked call.  Both device values raise
+        TypeError for a prior other than None / DefaultPrior / EnvPrior / MTBOPrior or a kernel the device cannot
+        represent, and ValueError with use_gradients=True (the BFGS branch has no device path)."""
+        from robo_b200.models.gaussian_process_mcmc import HYPER_PATHS, _hyper_kernel, _hyper_prior
+        if hyper_optimizer not in HYPER_PATHS:
+            raise ValueError("hyper_optimizer must be 'host', 'device' or 'device_blocked', not %r"
+                             % (hyper_optimizer,))
+        if hyper_optimizer != "host":
             if use_gradients:
-                raise ValueError("hyper_optimizer='device' restates L-BFGS-B with finite differences; "
-                                 "use_gradients=True (BFGS with grad_nll) runs on the host only")
-            _hyper_prior(prior, "hyper_optimizer")
-            _hyper_kernel(kernel, "hyper_optimizer")
+                raise ValueError("hyper_optimizer=%r restates L-BFGS-B with finite differences; "
+                                 "use_gradients=True (BFGS with grad_nll) runs on the host only" % (hyper_optimizer,))
+            _hyper_prior(prior, "hyper_optimizer", hyper_optimizer)
+            _hyper_kernel(kernel, "hyper_optimizer", hyper_optimizer)
         self.hyper_optimizer = hyper_optimizer
         self._hyper_handle = None
         self._hyper_fallback_logged = False
@@ -205,9 +209,9 @@ class GaussianProcess(BaseModel):
 
     def _optimize_on_device(self):
         from robo_b200 import _lib
-        if self.hyper_optimizer != "device":
+        if self.hyper_optimizer == "host":
             return False
-        if len(self.X) > _lib.HYPER_MAX_N:
+        if self.hyper_optimizer == "device" and len(self.X) > _lib.HYPER_MAX_N:
             # the device keeps one factor per SM in shared memory: larger N optimises on the host
             if not self._hyper_fallback_logged:
                 logger.info("N = %d exceeds GPK_HYPER_MAX_N = %d: the hyper-parameters are optimised on the host",
@@ -217,20 +221,22 @@ class GaussianProcess(BaseModel):
         return True
 
     def _optimize_device(self, p0):
-        """optimize() as one gpk_optimize_hypers call on the training set of the handle's last set_data."""
+        """optimize() as one gpk_optimize_hypers (or, for "device_blocked", gpk_optimize_hypers_blocked) call on the
+        training set of the handle's last set_data."""
         from robo_b200 import _lib
         from robo_b200.device_gp import TINY
         from robo_b200.kernels import load_kernel
         from robo_b200.models.gaussian_process_mcmc import _hyper_kernel, _hyper_prior
-        prior_kind, prior_par, n_ls, n_lr = _hyper_prior(self.prior, "hyper_optimizer")
-        f = _hyper_kernel(self.gp.kernel, "hyper_optimizer")
+        prior_kind, prior_par, n_ls, n_lr = _hyper_prior(self.prior, "hyper_optimizer", self.hyper_optimizer)
+        f = _hyper_kernel(self.gp.kernel, "hyper_optimizer", self.hyper_optimizer)
         if self._hyper_handle is None:
             self._hyper_handle = _lib.Handle(self.device)
         h = self._hyper_handle
         h.set_data(self.X, self.y)
         load_kernel(h, f)
         _lib.set_hyper_model(h, f["slots"], len(f["axis"]), float(self.mean), TINY, prior_kind, prior_par, n_ls, n_lr)
-        self.hyper_result = _lib.optimize_hypers(h, p0)
+        run = _lib.optimize_hypers_blocked if self.hyper_optimizer == "device_blocked" else _lib.optimize_hypers
+        self.hyper_result = run(h, p0)
         return self.hyper_result["theta"]
 
     # ------------------------------------------------------------------ posterior

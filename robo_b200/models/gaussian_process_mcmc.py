@@ -13,6 +13,11 @@ factorisation chains overlap on the GPU (SURVEY.md section 8f rank 1).
 proposes, evaluates the log-posteriors on chip (kernel, Cholesky and prior in one CTA per walker) and accepts; the
 final positions come back in one copy.  It draws from a counter-based Philox stream seeded from ``self.rng`` once per
 run, not from numpy's stream: the two samplers agree in law, not bit for bit, which is why ``"host"`` stays the default.
+It needs N <= GPK_HYPER_MAX_N (232); larger N samples on the host.
+
+``hyper_sampler="device_blocked"`` is the same run (gpk_sample_hypers_blocked, robo_b200/csrc/gpk_hyper_blocked.cuh)
+with each half-ensemble's log-posteriors computed by one batched blocked Cholesky over the walkers' kernel matrices in
+device memory, at every N up to GPK_HYPER_BLOCKED_MAX_N (8192) and without a fallback.
 """
 import logging
 from copy import deepcopy
@@ -76,9 +81,10 @@ class _LikelihoodPool(object):
         self.handles = []
 
 
-def _hyper_prior(prior, option="hyper_sampler"):
+def _hyper_prior(prior, option="hyper_sampler", value="device"):
     """(gpk_prior_kind, the 7 constants, n_ls, n_lr) of a prior the device restates: None, DefaultPrior, EnvPrior or
-    MTBOPrior (the reference's classes or robo_b200.priors'); TypeError, naming `option`, for any other."""
+    MTBOPrior (the reference's classes or robo_b200.priors'); TypeError, naming `option` and its `value`, for any
+    other."""
     if prior is None:
         return _lib.PRIOR_NONE, None, 0, 0
     cls = type(prior)
@@ -95,16 +101,20 @@ def _hyper_prior(prior, option="hyper_sampler"):
         par = [prior.ln_prior.sigma, prior.ln_prior.mean, prior.tophat.min, prior.tophat.max, prior.horseshoe.scale,
                prior.tophat_task.min, prior.tophat_task.max]
         return _lib.PRIOR_MTBO, par, int(prior.n_ls), int(prior.n_kt)
-    raise TypeError("%s='device' restates None, DefaultPrior, EnvPrior and MTBOPrior only, not %s.%s"
-                    % (option, mod, cls.__name__))
+    raise TypeError("%s=%r restates None, DefaultPrior, EnvPrior and MTBOPrior only, not %s.%s"
+                    % (option, value, mod, cls.__name__))
 
 
-def _hyper_kernel(kernel, option="hyper_sampler"):
-    """kernel.flatten(), or TypeError, naming `option`, when the device cannot represent the kernel."""
+def _hyper_kernel(kernel, option="hyper_sampler", value="device"):
+    """kernel.flatten(), or TypeError, naming `option` and its `value`, when the device cannot represent the kernel."""
     try:
         return kernel.flatten()
     except Exception as e:
-        raise TypeError("%s='device' cannot represent this kernel: %s" % (option, e))
+        raise TypeError("%s=%r cannot represent this kernel: %s" % (option, value, e))
+
+
+# the values of hyper_sampler and hyper_optimizer
+HYPER_PATHS = ("host", "device", "device_blocked")
 
 
 class GaussianProcessMCMC(BaseModel):
@@ -115,13 +125,15 @@ class GaussianProcessMCMC(BaseModel):
         """Arguments as in gaussian_process_mcmc.py:17-70, plus ``device`` and ``hyper_sampler``: "host" (default)
         runs EnsembleSampler with numpy's stream, as before; "device" runs each run_mcmc on the device
         (gpk_sample_hypers) with its own Philox stream, so the two agree in law, not bit for bit.  A train whose N
-        exceeds GPK_HYPER_MAX_N falls back to the host sampler.  "device" raises TypeError for a prior other than
-        None / DefaultPrior / EnvPrior or a kernel the device cannot represent."""
-        if hyper_sampler not in ("host", "device"):
-            raise ValueError("hyper_sampler must be 'host' or 'device', not %r" % (hyper_sampler,))
-        if hyper_sampler == "device":
-            _hyper_prior(prior)
-            _hyper_kernel(kernel)
+        exceeds GPK_HYPER_MAX_N falls back to the host sampler.  "device_blocked" runs the same chain through
+        gpk_sample_hypers_blocked at every N up to GPK_HYPER_BLOCKED_MAX_N, with no fallback.  Both device values raise
+        TypeError for a prior other than None / DefaultPrior / EnvPrior / MTBOPrior or a kernel the device cannot
+        represent."""
+        if hyper_sampler not in HYPER_PATHS:
+            raise ValueError("hyper_sampler must be 'host', 'device' or 'device_blocked', not %r" % (hyper_sampler,))
+        if hyper_sampler != "host":
+            _hyper_prior(prior, value=hyper_sampler)
+            _hyper_kernel(kernel, value=hyper_sampler)
         self.hyper_sampler = hyper_sampler
         self._hyper_handle = None
         self._hyper_fallback_logged = False
@@ -167,8 +179,8 @@ class GaussianProcessMCMC(BaseModel):
         self.gp = DeviceGP(self.kernel, mean=self.mean, device=self.device)
         self.gp.set_data(self.X, self.y)
 
-        on_device = do_optimize and self.hyper_sampler == "device"
-        if on_device and len(self.X) > _lib.HYPER_MAX_N:
+        on_device = do_optimize and self.hyper_sampler != "host"
+        if on_device and self.hyper_sampler == "device" and len(self.X) > _lib.HYPER_MAX_N:
             # the device keeps one factor per SM in shared memory: larger N samples on the host for this train
             if not self._hyper_fallback_logged:
                 logger.info("N = %d exceeds GPK_HYPER_MAX_N = %d: the hyper-parameters are sampled on the host",
@@ -215,9 +227,10 @@ class GaussianProcessMCMC(BaseModel):
 
     def _sample_hypers_device(self):
         """train's MCMC phase on the device: the same p0 / burn-in / chain bookkeeping as the host path, each run_mcmc
-        one gpk_sample_hypers call seeded from self.rng."""
-        prior_kind, prior_par, n_ls, n_lr = _hyper_prior(self.prior)
-        f = _hyper_kernel(self.kernel)
+        one gpk_sample_hypers (or, for "device_blocked", gpk_sample_hypers_blocked) call seeded from self.rng."""
+        prior_kind, prior_par, n_ls, n_lr = _hyper_prior(self.prior, value=self.hyper_sampler)
+        f = _hyper_kernel(self.kernel, value=self.hyper_sampler)
+        sample = _lib.sample_hypers_blocked if self.hyper_sampler == "device_blocked" else _lib.sample_hypers
         dim = len(self.kernel) + 1
         if self._hyper_handle is None:
             self._hyper_handle = _lib.Handle(self.device)
@@ -228,7 +241,7 @@ class GaussianProcessMCMC(BaseModel):
 
         def run(p0, steps):
             seed = int(self.rng.randint(0, 2 ** 63, dtype=np.int64))
-            return _lib.sample_hypers(h, p0, steps, seed)["pos"]
+            return sample(h, p0, steps, seed)["pos"]
         calls = 0
         if not self.burned:
             if self.prior is None:

@@ -170,6 +170,18 @@ print("dngo", _lib.dngo_dims(h), "features", _lib.dngo_features(h, Xs[:3])[0, :2
 r = _lib.maximize_direct([h], _lib.ACQ_EI, [float(y.min())], 0.0, np.zeros(D), np.ones(D), n_func_evals=100)
 print("dngo direct", r["nit"], r["nfev"])
 h.close()
+# hyper-parameters at large N, blocked path: the log-posterior across two 128-row blocks in three chunks of at most two
+# thetas (1 MiB of matrix and P strip each), the sampler and the optimiser
+h = _lib.Handle(0)
+h.set_option("hyper_batch_bytes", 2 * 1100000)
+h.set_data(X[:150], y[:150])
+h.set_kernel(f["family"], f["log_amp"], f["axis"], f["group"], f["log_metric"])
+_lib.set_hyper_model(h, f["slots"], len(f["axis"]), float(y[:150].mean()), 1.25e-12)
+Th = np.c_[rng.uniform(-1, 1, (5, 4)), rng.uniform(-6, -2, 5)]
+print("hyper blocked", _lib.hyper_lnpost_blocked(h, Th)[0][:2],
+      _lib.sample_hypers_blocked(h, Th[[0, 1, 2, 3, 4, 0, 1, 2, 3, 4]], 2, 5)["lnpost"][:2],
+      _lib.optimize_hypers_blocked(h, Th[0], maxiter=3)["f"])
+h.close()
 h = _lib.moments_handle()
 print(h.acq_moments(rng.randn(100), rng.rand(100) + 0.1, _lib.ACQ_LOG_EI, 0.0, 0.0)[0][:3])
 print(h.reduce_models(rng.rand(4, 50), rng.rand(4, 50))[1][:3])
