@@ -46,9 +46,14 @@ constexpr int APP_KC = 512;          // split-K chunk of gpk_fit_append's long c
 
 struct Range { int off = 0, cnt = 0; };
 
+// a device allocation of cap bytes, freed with its owner
 struct DevBuf {
     void* p = nullptr;
     size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() { if (p) cudaFree(p); }
 };
 
 // the model a handle holds: a Gaussian process unless a gpk_*_set_data made it a surrogate, which it stays for life
@@ -56,32 +61,35 @@ enum ModelKind { MODEL_GP, MODEL_BLR, MODEL_RF, MODEL_BNN, MODEL_DNGO };
 
 }  // namespace
 
+// Every CUDA resource of a handle is released with it: the buffers by their DevBuf members, the streams, events and
+// pinned host memory by the destructor.
 struct gpk_handle {
     int device = 0;
     cudaStream_t stream = nullptr;
     cudaStream_t own_stream = nullptr;
     cudaStream_t side_stream = nullptr;     // trailing updates of the look-ahead Cholesky
     std::vector<cudaEvent_t> ev_panel, ev_rest;
-    // variance contraction on the int8 tensor pipe (gpk_ozaki.cuh); 0 = fp64 DMMA kernels
-    int ozaki = 1;
-    DevBuf oz_Pq, oz_Kq, oz_Kq2, oz_eP, oz_emax, oz_pmu2;
-    int oz_last_variant = 0;        // contraction of the last int8 launch: 1 = gpk_oz_vargemm_kernel, + 8 when it walked the tile
+    // variance contraction on the int8 tensor pipe (gpk_ozaki.cuh)
+    struct {
+        int enabled = 1;            // 0 = fp64 DMMA kernels
+        DevBuf Pq, Kq, Kq2, eP, emax, pmu2;
+        int last_variant = 0;       // contraction of the last int8 launch: 1 = gpk_oz_vargemm_kernel, + 8 when it walked the tile
                                     // list persistently, + 16 / + 32 in clusters of 2 / 4 CTAs
-    int oz_cluster = 4;             // CTAs per cluster of the int8 contraction (1, 2 or 4): they share the L^-1 slices by TMA
+        int cluster = 4;            // CTAs per cluster of the int8 contraction (1, 2 or 4): they share the L^-1 slices by TMA
                                     // multicast [default 4: tools/persist_threshold.py and bench.py on an H100, DESIGN 9.5]
-    int oz_map_cs = 0;              // cluster size mapOzP's box was encoded for (0: not encoded)
-    int oz_max_clusters[5] = {0, 0, 0, 0, 0};   // co-resident clusters of the contraction per cluster size (0: not queried)
-    int oz_persist = 3;             // 1: one CTA per SM walks the tile list; 0: one CTA per tile; 3 = automatic [default]: persistent
+        int map_cs = 0;             // cluster size mapP's box was encoded for (0: not encoded)
+        int max_clusters[5] = {0, 0, 0, 0, 0};  // co-resident clusters of the contraction per cluster size (0: not queried)
+        int persist = 3;            // 1: one CTA per SM walks the tile list; 0: one CTA per tile; 3 = automatic [default]: persistent
                                     // for N <= 4096 (tools/persist_threshold.py and bench.py on an H100 with 4-CTA clusters: the
                                     // walk is as fast or faster up to N = 4096, one CTA per tile is faster at 6144)
-    int oz_grid = 0;                // most clusters the persistent walk launches (0: as many as fit at once [default])
-    DevBuf oz_probe;                // scratch of gpk_oz_contract (operands, slices, exponents, partial sums)
-    long oz_linv_serial = -1;       // linv_serial the slices of L^-1 were made for
+        int grid = 0;               // most clusters the persistent walk launches (0: as many as fit at once [default])
+        DevBuf probe;               // scratch of gpk_oz_contract (operands, slices, exponents, partial sums)
+        long linv_serial = -1;      // linv_serial the slices of L^-1 were made for
+        int emax_host = 0;
+        CUtensorMap mapP, mapK, mapK2;
+        double launches = 0;
+    } oz;
     long linv_serial = 0;           // bumped whenever L^-1 is (re)built
-    int oz_emax_host = 0;
-    long oz_rows = 0, oz_rows2 = 0;
-    CUtensorMap mapOzP, mapOzK, mapOzK2;
-    double oz_launches = 0;
     int n_sm = 0;
     char err[1024] = {0};
     long chunk = 16384;
@@ -93,8 +101,6 @@ struct gpk_handle {
     int n = 0, d = 0, NP = 0, nb = 0;
     bool has_data = false, has_spec = false, fitted = false, linv_ready = false, alpha_ready = false;
     KSpec spec;
-    double log_amp = 0.0;
-    std::vector<double> log_metric;
     bool has_bounds = false;
     std::vector<double> task_theta; // gpk_set_task_factor's packed log-entries (the gradient's contraction)
     std::vector<int> col_tasks;     // per input column: 1 + the largest value when every value is an integer >= 0 (the
@@ -103,25 +109,26 @@ struct gpk_handle {
     double y_mean = 0.0, y_std = 1.0, mean = 0.0, diag_add = 0.0;
 
     // device buffers
-    DevBuf Xrow, Xt, y, Kbuf, P, Q, W, lower, upper, logdet_part, scal, status, jobs;
-    DevBuf Kstar2, cand2;
+    DevBuf Xrow, Xt, y, Kbuf, P, Q, W, lower, upper, logdet_part, scal, status;
+    DevBuf Kstar2;
     DevBuf Xts;                     // training inputs, term-major and pre-scaled (operand of gpk_cov_tma_kernel)
     cudaStream_t copy_stream = nullptr;
-    std::vector<cudaEvent_t> ev_copied, ev_scored;
-    std::vector<cudaEvent_t> ev_g0, ev_g1;    // timed pairs around every variance-GEMM launch of the last scoring call
-    int last_nchunks = 0;
+    std::vector<cudaEvent_t> ev_copied;
     DevBuf cand, Kstar, part_mu, part_ssq, out_mu, out_var, out_acq, block_best, best, nneg;
     DevBuf Vt, cov, XsT, tmpjobs, alpha, tmp1, tmp2, tmp3;
     int layout_NP = -1;           // NP the P/Q/W buffers were zeroed for
-    int jobs_nb = -1;
 
-    // job tables
-    std::vector<Range> syrk_r, tri1_r, tri2_r, trsm32_r, pu32_r;
-    std::vector<Range> syrk2_r;     // depth-2 trailing update: columns >= k+2 with panels k-1 and k in one contraction (K = 256)
+    // job tables: the GEMM jobs of the fit, L^-1, K^-1 and gpk_fit_append, and their ranges, built for nb row blocks
+    DevBuf jobs;
+    struct {
+        int nb = -1;
+        std::vector<Range> syrk, tri1, tri2, trsm32, pu32;
+        std::vector<Range> syrk2;       // depth-2 trailing update: columns >= k+2 with panels k-1 and k in one contraction (K = 256)
+        Range kinv;
+        Range app_syrk, app_p;          // gpk_fit_append (last block row only)
+        Range app_row2, app_t2;         // its two long contractions, split-K
+    } ranges;
     int depth2 = 2;                 // 0 / 1, or 2 = automatic: on for nb >= 48 (trailing updates gate the fit only there)
-    Range kinv_r;
-    Range app_row_r, app_syrk_r, app_t_r, app_p_r;      // gpk_fit_append (last block row only)
-    Range app_row2_r, app_t2_r;                         // split-K versions of the two long contractions
 
     // tensor maps
     CUtensorMap mapK, mapP, mapQ, mapW, mapKs, mapVt;
@@ -134,91 +141,121 @@ struct gpk_handle {
     long mapKs_rows = 0, mapVt_rows = 0;
 
     // timing
-    cudaEvent_t ev[16];
+    struct {
+        cudaEvent_t ev[16] = {};
+        std::vector<cudaEvent_t> ev_g0, ev_g1;    // timed pairs around every variance-GEMM launch of the last scoring call
+        int last_nchunks = 0;
+        bool fit_timed = false, score_timed = false;
+        double launches_total = 0, launches_var = 0;
+    } timing;
     cudaEvent_t ev_order = nullptr;
-    bool ev_ok = false;
-    bool fit_timed = false, score_timed = false;
-    double launches_total = 0, launches_var = 0;
-    long last_chunk_rows = 0;
     double* pin = nullptr;        // pinned host: [0..1] z^T z, logdet ; [2] status (as int) for async fits
     double* stage[2] = {nullptr, nullptr};    // pinned staging of pageable candidate batches (gpk_acq)
     size_t stage_cap = 0;
     bool fit_pending = false;
 
-    // several models, one batch (gpk_acq_multi): buffers owned by the first handle of the call
-    DevBuf multi_cand, multi_A, multi_B, multi_out, multi_bb;
-    cudaEvent_t ev_multi = nullptr;
-    // differential evolution (gpk_maximize_de): population, trials, scaled batch, energies, {status, limits, winner},
-    // radix-sort scratch of the LHS initialisation; owned by the first handle of the call
-    DevBuf de_pop, de_trial, de_param, de_E, de_small, de_sort;
-    // multi-start L-BFGS (gpk_maximize_lbfgs): per-start state, pair memory, scored batch, active lists, status record;
-    // owned by the first handle of the call
-    DevBuf lb_buf;
-    // CMA-ES (gpk_maximize_cmaes*): state, status record, constant table, bounds and x0, the Z / Y / G / P rows of a
-    // generation; owned by the first handle of the call (gpk_cmaes_draws uses it as scratch)
-    DevBuf cma_buf;
-    // DIRECT (gpk_maximize_direct*): state, status record, box, rectangle store, row buffer, selection; owned by the
-    // first handle of the call
-    DevBuf dir_buf;
-    DevBuf ep_buf;                  // scratch of gpk_ep_joint_min (operands, raw and renormalised outputs, status)
+    // scratch of the entry points over several handles, owned by the first handle of the call
+    struct {
+        // several models, one batch (gpk_acq_multi)
+        DevBuf cand, A, B, out, bb;
+        cudaEvent_t ev = nullptr;       // fork_join's start of the sub-handles' work
+        // differential evolution (gpk_maximize_de): population, trials, scaled batch, energies, {status, limits, winner},
+        // radix-sort scratch of the LHS initialisation
+        DevBuf de_pop, de_trial, de_param, de_E, de_small, de_sort;
+        // multi-start L-BFGS (gpk_maximize_lbfgs): per-start state, pair memory, scored batch, active lists, status record
+        DevBuf lb_buf;
+        // CMA-ES (gpk_maximize_cmaes*): state, status record, constant table, bounds and x0, the Z / Y / G / P rows of a
+        // generation (gpk_cmaes_draws uses it as scratch)
+        DevBuf cma_buf;
+        // DIRECT (gpk_maximize_direct*): state, status record, box, rectangle store, row buffer, selection
+        DevBuf dir_buf;
+        DevBuf ep_buf;                  // scratch of gpk_ep_joint_min (operands, raw and renormalised outputs, status)
+        // information gain per unit cost (gpk_es_cost_multi): the batch under the objective's and the cost's Fabolas
+        // transform and the configuration bounds; owned by the first objective handle of the call
+        DevBuf fab_in;
+        // representer sampling (gpk_sample_representers): walkers, log-probabilities, proposals, scored batches, bounds,
+        // accept counts, seeds, slots
+        DevBuf rs_buf;
+    } multi;
     // entropy search (gpk_es_update / gpk_es_compute): EP state, W, bounds, scaled zb, U = K^-1 K(X, zb), per-chunk v, sigma
-    DevBuf es_state, es_U, es_work, es_in;
-    // information gain per unit cost (gpk_es_cost_multi): the batch under the objective's and the cost's Fabolas
-    // transform and the configuration bounds; owned by the first objective handle of the call
-    DevBuf fab_in;
-    // representer sampling (gpk_sample_representers): walkers, log-probabilities, proposals, scored batches, bounds,
-    // accept counts, seeds, slots; owned by the first handle of the call
-    DevBuf rs_buf;
-    // hyper-parameter sampling (gpk_sample_hypers): theta -> kernel map and prior, walkers / log-posteriors / accepts
-    bool has_hyper = false;
-    HyperModel hyper;
-    DevBuf hy_buf;
-    // the blocked path (gpk_hyper_blocked.cuh): one chunk's matrices, parameters and block log-sums, released at the end
-    // of every call; the chunk's byte budget ("hyper_batch_bytes")
-    DevBuf hb_buf;
-    GemmJob* hb_jobs = nullptr;     // the chunk's job tables, inside hb_buf
-    long hyper_batch_bytes = GPK_HYPER_BATCH_BYTES;
+    struct {
+        DevBuf state, U, work, in;
+        int nb = 0, np = 0;
+        double sn2 = 0.0, H = 0.0;
+        long linv_serial = -1;          // linv_serial U was built for (-1: no update yet)
+        int kind = 0;                   // which update is current: ES_KIND_EP (gpk_es_update) or ES_KIND_MC (gpk_esmc_update)
+    } es;
+    // sampling-based entropy search (gpk_esmc_update / gpk_esmc_compute): Mb, Vb, W, lmb, scaled zb and the draws F;
+    // the scratch of gpk_mc_pmin / gpk_mc_draws; the two status words of the last pass (gpk_esmc.cuh)
+    struct {
+        DevBuf state, buf, stat;
+        int nf = 0;
+        long last_jitter = 0;
+    } mc;
+    // hyper-parameter sampling (gpk_sample_hypers): theta -> kernel map and prior, walkers / log-posteriors / accepts;
+    // the byte budget of a chunk of the blocked path (gpk_hyper_blocked.cuh, "hyper_batch_bytes")
+    struct {
+        bool has_model = false;
+        HyperModel model;
+        DevBuf buf;
+        long batch_bytes = GPK_HYPER_BATCH_BYTES;
+    } hyper;
     // a surrogate handle serves its own entry points and the scoring ones only; its scoring pass uses block_best, best
     // and nneg as the GP's does
     ModelKind model = MODEL_GP;
-    // Bayesian linear regression (gpk_blr.cuh, gpk_blr_set_data).  blr_data: Phi (n x F), y, G = Phi^T Phi,
-    // b = Phi^T y; blr_post: the fit's M (k x F), L^-1 and S (k x F x F each), 1 / beta (k), failure flags; blr_work:
-    // thetas / walkers and their values
-    bool blr_fitted = false;
-    int blr_basis = 0, blr_F = 0, blr_k = 0;
-    BlrPrior blr_prior;
-    DevBuf blr_data, blr_post, blr_work;
-    // random forest (gpk_rf.cuh, gpk_rf_set_data).  rf_data: X (n x d), y (n), the per-feature row order (d x n ints);
-    // rf_work: the growth's per-tree multiplicities, lists and segments; rf_nodes: the trees (RfNodes)
-    bool rf_fitted = false;
-    int rf_T = 0, rf_total = 0;
-    DevBuf rf_data, rf_work, rf_nodes;
-    // Bayesian neural network (gpk_bnn.cuh, gpk_bnn_set_data).  bnn_data: the scaled X (n x d), y (n), the input mean
-    // and std (d each), with the y statistics in bnn_ymean / bnn_ystd (a DNGO handle keeps its training set there too);
-    // bnn_samples: the kept networks (S x P); bnn_state: the chain's final theta, p, tau, g, vhat (P each)
-    int bnn_P = 0, bnn_S = 0;
-    double bnn_ymean = 0.0, bnn_ystd = 1.0;
-    DevBuf bnn_data, bnn_samples, bnn_state;
-    // DNGO (gpk_dngo.cuh, gpk_dngo_set_data): the training set in bnn_data, the trained net (P), Adam's m and v (P each,
-    // after dngo_t steps; -1: the net was set, not trained), the scoring pack and the collapse's failure flag.  The
-    // Bayesian linear regression over the features lives in the blr_* fields (F = 50, no basis).
-    bool dngo_trained = false, dngo_fitted = false;
-    int dngo_P = 0;
-    long long dngo_t = -1;
-    DevBuf dngo_net, dngo_state, dngo_pack;
-    int es_nb = 0, es_np = 0;
-    double es_sn2 = 0.0, es_H = 0.0;
-    long es_linv_serial = -1;       // linv_serial U was built for (-1: no update yet)
-    int es_kind = 0;                // which update is current: ES_KIND_EP (gpk_es_update) or ES_KIND_MC (gpk_esmc_update)
-    // sampling-based entropy search (gpk_esmc_update / gpk_esmc_compute): Mb, Vb, W, lmb, scaled zb and the draws F;
-    // the scratch of gpk_mc_pmin / gpk_mc_draws; the two status words of the last pass (gpk_esmc.cuh)
-    DevBuf mc_state, mc_buf, mc_stat;
-    int es_nf = 0;
-    long mc_last_jitter = 0;
+    // Bayesian linear regression (gpk_blr.cuh, gpk_blr_set_data).  data: Phi (n x F), y, G = Phi^T Phi, b = Phi^T y;
+    // post: the fit's M (k x F), L^-1 and S (k x F x F each), 1 / beta (k), failure flags; work: thetas / walkers and
+    // their values
+    struct {
+        bool fitted = false;
+        int basis = 0, F = 0, k = 0;
+        BlrPrior prior;
+        DevBuf data, post, work;
+    } blr;
+    // random forest (gpk_rf.cuh, gpk_rf_set_data).  data: X (n x d), y (n), the per-feature row order (d x n ints);
+    // work: the growth's per-tree multiplicities, lists and segments; nodes: the trees (RfNodes)
+    struct {
+        bool fitted = false;
+        int T = 0, total = 0;
+        DevBuf data, work, nodes;
+    } rf;
+    // Bayesian neural network (gpk_bnn.cuh, gpk_bnn_set_data).  data: the scaled X (n x d), y (n), the input mean and
+    // std (d each), with the y statistics in ymean / ystd (a DNGO handle keeps its training set here too); samples: the
+    // kept networks (S x P); state: the chain's final theta, p, tau, g, vhat (P each)
+    struct {
+        int P = 0, S = 0;
+        double ymean = 0.0, ystd = 1.0;
+        DevBuf data, samples, state;
+    } bnn;
+    // DNGO (gpk_dngo.cuh, gpk_dngo_set_data): the training set in bnn.data, the trained net (P), Adam's m and v (P each,
+    // after t steps; -1: the net was set, not trained), the scoring pack and the collapse's failure flag.  The Bayesian
+    // linear regression over the features lives in blr (F = 50, no basis).
+    struct {
+        bool trained = false, fitted = false;
+        int P = 0;
+        long long t = -1;
+        DevBuf net, state, pack;
+    } dngo;
     // multi-GPU (gpk_comm_*): NCCL communicator bound at run time, one 16-byte pair per rank
-    void* comm = nullptr;
-    int rank = 0, world = 1;
-    DevBuf gather, best_global;
+    struct {
+        void* comm = nullptr;
+        int rank = 0, world = 1;
+        DevBuf gather, best_global;
+    } dist;
+
+    // the caller makes the handle's device current; the communicator goes first (gpk_comm_destroy)
+    ~gpk_handle() {
+        for (cudaEvent_t e : timing.ev)
+            if (e) cudaEventDestroy(e);
+        for (cudaEvent_t e : {ev_order, multi.ev})
+            if (e) cudaEventDestroy(e);
+        for (const auto* evs : {&ev_panel, &ev_rest, &ev_cov, &ev_gemm, &ev_copied, &timing.ev_g0, &timing.ev_g1})
+            for (cudaEvent_t e : *evs) cudaEventDestroy(e);
+        for (cudaStream_t s : {copy_stream, side_stream, own_stream})
+            if (s) cudaStreamDestroy(s);
+        for (double* p : {pin, stage[0], stage[1]})
+            if (p) cudaFreeHost(p);
+    }
 };
 
 namespace {
@@ -247,7 +284,7 @@ void set_err(gpk_handle* h, const char* fmt, ...) {
             set_err(h, "kernel launch -> %s (%s:%d)", cudaGetErrorString(e_), __FILE__, __LINE__); \
             return GPK_CUDA_ERROR;                                                               \
         }                                                                                        \
-        h->launches_total += 1;                                                                  \
+        h->timing.launches_total += 1;                                                           \
     } while (0)
 
 #define BAD(...)                           \
@@ -270,6 +307,25 @@ int ensure(gpk_handle* h, DevBuf& b, size_t bytes, bool* grew = nullptr) {
 }
 
 template <typename T> T* ptr(const DevBuf& b) { return reinterpret_cast<T*>(b.p); }
+
+// grows evs to n events created with flags; the handle's destructor releases them
+int grow_events(gpk_handle* h, std::vector<cudaEvent_t>& evs, size_t n, unsigned flags) {
+    while (evs.size() < n) {
+        cudaEvent_t e;
+        CK(cudaEventCreateWithFlags(&e, flags));
+        evs.push_back(e);
+    }
+    return GPK_OK;
+}
+
+// the two timing events of a gpk_measure_* call, released on every return
+struct TimerEvents {
+    cudaEvent_t e0 = nullptr, e1 = nullptr;
+    ~TimerEvents() {
+        if (e0) cudaEventDestroy(e0);
+        if (e1) cudaEventDestroy(e1);
+    }
+};
 
 inline long round_up(long x, long m) { return (x + m - 1) / m * m; }
 
@@ -411,9 +467,9 @@ cudaError_t launch_oz(void (*kernel)(KArgs...), unsigned grid, int cs, size_t sm
 
 // How many clusters of cs contraction CTAs fit on the device at once (the grid of the persistent walk), once per handle
 int oz_max_clusters(gpk_handle* h, int cs, int* out) {
-    if (h->oz_max_clusters[cs] == 0) {
+    if (h->oz.max_clusters[cs] == 0) {
         if (cs == 1) {
-            h->oz_max_clusters[cs] = std::max(h->n_sm, 1);
+            h->oz.max_clusters[cs] = std::max(h->n_sm, 1);
         } else {
             cudaLaunchConfig_t cfg;
             memset(&cfg, 0, sizeof(cfg));
@@ -430,10 +486,10 @@ int oz_max_clusters(gpk_handle* h, int cs, int* out) {
             int n = 0;
             CK(cudaOccupancyMaxActiveClusters(&n, gpk_oz_vargemm_kernel, &cfg));
             if (n < 1) { set_err(h, "no cluster of %d int8 contraction CTAs fits on this device", cs); return GPK_CUDA_ERROR; }
-            h->oz_max_clusters[cs] = n;
+            h->oz.max_clusters[cs] = n;
         }
     }
-    *out = h->oz_max_clusters[cs];
+    *out = h->oz.max_clusters[cs];
     return GPK_OK;
 }
 
@@ -446,20 +502,20 @@ int launch_oz_contraction(gpk_handle* h, const CUtensorMap& mapP, const CUtensor
     o.nb = nb; o.ncb = (int)(rows_padded / OZ_TN); o.NP = (int)NP; o.rows = (int)rows;
     // a group's K* slices take about 24 MB, half of the L2; whole clusters of candidate blocks (ncb = rows_padded / 32 is
     // a multiple of 4, so of every cluster size)
-    const int cs = h->oz_cluster;
+    const int cs = h->oz.cluster;
     o.group = (int)std::min<long>(512, std::max<long>(4, ((long)24 << 20) / ((long)OZ_TN * NP * OZ_S))) / cs * cs;
     o.eP = eP; o.eK = eK;
     o.part_ssq = part_ssq; o.ldpart = ldpart;
-    const int persist = h->oz_persist == 3 ? (nb <= 32 ? 1 : 0) : h->oz_persist;
+    const int persist = h->oz.persist == 3 ? (nb <= 32 ? 1 : 0) : h->oz.persist;
     const int tiles = o.nb * o.ncb;
     int grid = tiles;
     if (persist == 1) {
         int nclusters = 0, rc;
         if ((rc = oz_max_clusters(h, cs, &nclusters))) return rc;
-        if (h->oz_grid > 0) nclusters = std::min(nclusters, h->oz_grid);
+        if (h->oz.grid > 0) nclusters = std::min(nclusters, h->oz.grid);
         grid = cs * std::min(tiles / cs, nclusters);
     }
-    h->oz_last_variant = 1 + (persist == 1 ? 8 : 0) + (cs == 2 ? 16 : cs == 4 ? 32 : 0);
+    h->oz.last_variant = 1 + (persist == 1 ? 8 : 0) + (cs == 2 ? 16 : cs == 4 ? 32 : 0);
     CK(launch_oz(gpk_oz_vargemm_kernel, (unsigned)grid, cs, (size_t)OZ_SMEM, h->stream, mapP, mapK, o));
     CKL();
     return GPK_OK;
@@ -474,7 +530,7 @@ int launch_gemm(gpk_handle* h, const CUtensorMap& mA, const CUtensorMap& mB, con
     if (stream == nullptr) stream = h->stream;
     if constexpr (MI == 2) {
         CK(launch_pdl(gpk_gemm_nt_kernel, dim3(njobs), dim3(GEMM_THREADS), (size_t)GEMM_SMEM_CHAIN, stream, mA, mB, a));
-        h->launches_total += 1;
+        h->timing.launches_total += 1;
         return GPK_OK;
     }
     gpk_gemm_ws_kernel<EPI><<<njobs, WS_THREADS, GEMM_SMEM_TMA, stream>>>(mA, mB, a);
@@ -516,51 +572,51 @@ int build_nodes(int lo, int hi, std::vector<Node>& nodes) {
 
 int build_job_tables(gpk_handle* h) {
     const int nb = h->nb;
-    if (h->jobs_nb == nb) return GPK_OK;
+    if (h->ranges.nb == nb) return GPK_OK;
     std::vector<GemmJob> jobs;
-    h->syrk_r.assign(nb, Range());
+    h->ranges.syrk.assign(nb, Range());
     for (int k = 0; k < nb; ++k) {
-        h->syrk_r[k].off = (int)jobs.size();
+        h->ranges.syrk[k].off = (int)jobs.size();
         for (int j = k + 1; j < nb; ++j)
             for (int i = j; i <= nb; ++i)
                 jobs.push_back({i * BM, j * BM, k * BM, (k + 1) * BM, i * BM, j * BM, 0, 0});
-        h->syrk_r[k].cnt = (int)jobs.size() - h->syrk_r[k].off;
+        h->ranges.syrk[k].cnt = (int)jobs.size() - h->ranges.syrk[k].off;
     }
     // depth-2 trailing update (odd steps k >= 1): tile (i, j), j >= k+2, receives panels k-1 and k in ONE contraction
     // over the 256 columns [(k-1)*128, (k+1)*128): same arithmetic, in the same order, as the two separate updates
-    h->syrk2_r.assign(nb, Range());
+    h->ranges.syrk2.assign(nb, Range());
     for (int k = 1; k < nb; k += 2) {
-        h->syrk2_r[k].off = (int)jobs.size();
+        h->ranges.syrk2[k].off = (int)jobs.size();
         for (int j = k + 2; j < nb; ++j)
             for (int i = j; i <= nb; ++i)
                 jobs.push_back({i * BM, j * BM, (k - 1) * BM, (k + 1) * BM, i * BM, j * BM, 0, 0});
-        h->syrk2_r[k].cnt = (int)jobs.size() - h->syrk2_r[k].off;
+        h->ranges.syrk2[k].cnt = (int)jobs.size() - h->ranges.syrk2[k].off;
     }
     // 32-row versions of the two GEMMs on the critical chain (row split only: the in-place panel solve
     // stays race-free because every CTA reads and writes its own rows)
-    h->trsm32_r.assign(nb, Range());
-    h->pu32_r.assign(nb, Range());
+    h->ranges.trsm32.assign(nb, Range());
+    h->ranges.pu32.assign(nb, Range());
     for (int k = 0; k < nb; ++k) {
-        h->trsm32_r[k].off = (int)jobs.size();
+        h->ranges.trsm32[k].off = (int)jobs.size();
         for (int i = k + 1; i <= nb; ++i)
             for (int q = 0; q < 4; ++q) {
                 if (i == nb && q > 0) break;         // augmented block: only its first rows are non-zero
                 jobs.push_back({i * BM + 32 * q, k * BM, k * BM, (k + 1) * BM, i * BM + 32 * q, k * BM, 0, 0});
             }
-        h->trsm32_r[k].cnt = (int)jobs.size() - h->trsm32_r[k].off;
-        h->pu32_r[k].off = (int)jobs.size();
+        h->ranges.trsm32[k].cnt = (int)jobs.size() - h->ranges.trsm32[k].off;
+        h->ranges.pu32[k].off = (int)jobs.size();
         if (k + 1 < nb)
             for (int i = k + 1; i <= nb; ++i)
                 for (int q = 0; q < 4; ++q) {
                     if (i == nb && q > 0) break;
                     jobs.push_back({i * BM + 32 * q, (k + 1) * BM, k * BM, (k + 1) * BM, i * BM + 32 * q, (k + 1) * BM, 0, 0});
                 }
-        h->pu32_r[k].cnt = (int)jobs.size() - h->pu32_r[k].off;
+        h->ranges.pu32[k].cnt = (int)jobs.size() - h->ranges.pu32[k].off;
     }
     std::vector<Node> nodes;
     int hmax = build_nodes(0, nb, nodes);
-    h->tri1_r.assign(hmax + 1, Range());
-    h->tri2_r.assign(hmax + 1, Range());
+    h->ranges.tri1.assign(hmax + 1, Range());
+    h->ranges.tri2.assign(hmax + 1, Range());
     auto by_len = [](const GemmJob& a, const GemmJob& b) { return (a.k1 - a.k0) > (b.k1 - b.k0); };
     for (int ht = 1; ht <= hmax; ++ht) {
         size_t s1 = jobs.size();
@@ -571,8 +627,8 @@ int build_job_tables(gpk_handle* h) {
                     jobs.push_back({c * BM, i * BM, c * BM, nd.mid * BM, c * BM, i * BM, 0, 0});
         }
         std::stable_sort(jobs.begin() + s1, jobs.end(), by_len);
-        h->tri1_r[ht].off = (int)s1;
-        h->tri1_r[ht].cnt = (int)(jobs.size() - s1);
+        h->ranges.tri1[ht].off = (int)s1;
+        h->ranges.tri1[ht].cnt = (int)(jobs.size() - s1);
         size_t s2 = jobs.size();
         for (const Node& nd : nodes) {
             if (nd.height != ht) continue;
@@ -581,60 +637,49 @@ int build_job_tables(gpk_handle* h) {
                     jobs.push_back({i * BM, c * BM, nd.mid * BM, (i + 1) * BM, i * BM, c * BM, 0, 0});
         }
         std::stable_sort(jobs.begin() + s2, jobs.end(), by_len);
-        h->tri2_r[ht].off = (int)s2;
-        h->tri2_r[ht].cnt = (int)(jobs.size() - s2);
+        h->ranges.tri2[ht].off = (int)s2;
+        h->ranges.tri2[ht].cnt = (int)(jobs.size() - s2);
     }
     // K^-1 = Q Q^T (lower tiles), Q = L^-T upper: K^-1[i][j] = sum_{k >= i} Q[i][k] Q[j][k], i >= j
-    h->kinv_r.off = (int)jobs.size();
+    h->ranges.kinv.off = (int)jobs.size();
     for (int j = 0; j < nb; ++j)
         for (int i = j; i < nb; ++i)
             jobs.push_back({i * BM, j * BM, i * BM, nb * BM, i * BM, j * BM, 0, 0});
-    std::stable_sort(jobs.begin() + h->kinv_r.off, jobs.end(), by_len);
-    h->kinv_r.cnt = (int)jobs.size() - h->kinv_r.off;
+    std::stable_sort(jobs.begin() + h->ranges.kinv.off, jobs.end(), by_len);
+    h->ranges.kinv.cnt = (int)jobs.size() - h->ranges.kinv.off;
     // gpk_fit_append: only block row b = nb-1 changes.  N1 = b*128 leading rows keep their factor L11 and inverse P11.
     {
         const int b = nb - 1, N1 = b * BM;
-        // L_row = K[b, 0:N1] P11^T, 32-row tiles (the contraction is up to N1 long: more, shorter CTAs)
-        h->app_row_r.off = (int)jobs.size();
-        for (int j = b - 1; j >= 0; --j)
-            for (int q = 0; q < 4; ++q)
-                jobs.push_back({N1 + 32 * q, j * BM, 0, (j + 1) * BM, N1 + 32 * q, j * BM, 0, 0});
-        h->app_row_r.cnt = (int)jobs.size() - h->app_row_r.off;
         // partial Gram tiles  T_s = L_row[:, s] L_row[:, s]^T  into the free tiles (s, b) of W; summed in fixed order
-        h->app_syrk_r.off = (int)jobs.size();
+        h->ranges.app_syrk.off = (int)jobs.size();
         for (int sblk = 0; sblk < b; ++sblk)
             jobs.push_back({N1, N1, sblk * BM, (sblk + 1) * BM, sblk * BM, N1, 0, 0});
-        h->app_syrk_r.cnt = (int)jobs.size() - h->app_syrk_r.off;
-        // T = L_row P11 (= L_row Q11^T in NT form), 32-row tiles, stored to P[b, :] and transposed to Q[:, b]
-        h->app_t_r.off = (int)jobs.size();
-        for (int j = 0; j < b; ++j)
-            for (int q = 0; q < 4; ++q)
-                jobs.push_back({N1 + 32 * q, j * BM, j * BM, N1, N1 + 32 * q, j * BM, 0, 0});
-        h->app_t_r.cnt = (int)jobs.size() - h->app_t_r.off;
-        // split-K versions (default): 128-row tiles, the contraction cut into chunks of APP_KC columns, partial tile
-        // (chunk c, column block j) -> scratch tile W(c, j); summed in fixed order by gpk_append_reduce_kernel
-        h->app_row2_r.off = (int)jobs.size();
+        h->ranges.app_syrk.cnt = (int)jobs.size() - h->ranges.app_syrk.off;
+        // L_row = K[b, 0:N1] P11^T and T = L_row P11 (= L_row Q11^T in NT form), split-K: 128-row tiles, the contraction
+        // cut into chunks of APP_KC columns, partial tile (chunk c, column block j) -> scratch tile W(c, j); summed in
+        // fixed order by gpk_append_reduce_kernel
+        h->ranges.app_row2.off = (int)jobs.size();
         for (int j = b - 1; j >= 0; --j)
             for (int c = 0, k0 = 0; k0 < (j + 1) * BM; ++c, k0 += APP_KC)
                 jobs.push_back({N1, j * BM, k0, std::min(k0 + APP_KC, (j + 1) * BM), c * BM, j * BM, 0, 0});
-        h->app_row2_r.cnt = (int)jobs.size() - h->app_row2_r.off;
-        h->app_t2_r.off = (int)jobs.size();
+        h->ranges.app_row2.cnt = (int)jobs.size() - h->ranges.app_row2.off;
+        h->ranges.app_t2.off = (int)jobs.size();
         for (int j = 0; j < b; ++j)
             for (int c = 0, k0 = j * BM; k0 < N1; ++c, k0 += APP_KC)
                 jobs.push_back({N1, j * BM, k0, std::min(k0 + APP_KC, N1), c * BM, j * BM, 0, 0});
-        h->app_t2_r.cnt = (int)jobs.size() - h->app_t2_r.off;
+        h->ranges.app_t2.cnt = (int)jobs.size() - h->ranges.app_t2.off;
         // P[b, j] = -P_bb T[:, j]
-        h->app_p_r.off = (int)jobs.size();
+        h->ranges.app_p.off = (int)jobs.size();
         for (int j = 0; j < b; ++j)
             jobs.push_back({N1, j * BM, N1, nb * BM, N1, j * BM, 0, 0});
-        h->app_p_r.cnt = (int)jobs.size() - h->app_p_r.off;
+        h->ranges.app_p.cnt = (int)jobs.size() - h->ranges.app_p.off;
     }
     if (jobs.empty()) jobs.push_back({0, 0, 0, 0, 0, 0, 0, 0});
     int rc = ensure(h, h->jobs, jobs.size() * sizeof(GemmJob));
     if (rc) return rc;
     CK(cudaMemcpyAsync(h->jobs.p, jobs.data(), jobs.size() * sizeof(GemmJob), cudaMemcpyHostToDevice, h->stream));
     CK(cudaStreamSynchronize(h->stream));
-    h->jobs_nb = nb;
+    h->ranges.nb = nb;
     return GPK_OK;
 }
 
@@ -818,8 +863,8 @@ int require(gpk_handle* h, bool data, bool spec, bool fitted) {
 // the preconditions of the entry points that score any model kind: a fitted GP, or a trained surrogate
 int require_model(gpk_handle* h) {
     if (!h || h->model == MODEL_GP) return require(h, true, true, true);
-    const bool trained = h->model == MODEL_BLR ? h->blr_fitted : h->model == MODEL_RF ? h->rf_fitted
-                       : h->model == MODEL_BNN ? h->bnn_S >= 1 : h->dngo_fitted;
+    const bool trained = h->model == MODEL_BLR ? h->blr.fitted : h->model == MODEL_RF ? h->rf.fitted
+                       : h->model == MODEL_BNN ? h->bnn.S >= 1 : h->dngo.fitted;
     if (!trained) { set_err(h, "%s", MODELS[h->model].not_fitted); return GPK_NOT_FITTED; }
     return GPK_OK;
 }
@@ -827,9 +872,9 @@ int require_model(gpk_handle* h) {
 // L^-1 by recursive block inversion (P lower, Q = P^T upper), after a successful fit.
 int build_linv(gpk_handle* h) {
     if (h->linv_ready) return GPK_OK;
-    CK(cudaEventRecord(h->ev[4], h->stream));
+    CK(cudaEventRecord(h->timing.ev[4], h->stream));
     const long NP = h->NP;
-    const int hmax = (int)h->tri1_r.size() - 1;
+    const int hmax = (int)h->ranges.tri1.size() - 1;
     for (int ht = 1; ht <= hmax; ++ht) {
         GemmArgs a;
         memset(&a, 0, sizeof(a));
@@ -837,9 +882,9 @@ int build_linv(gpk_handle* h) {
         a.B = ptr<double>(h->Kbuf); a.ldb = NP;
         a.C = ptr<double>(h->W); a.ldc = NP;
         a.alpha = 1.0; a.beta = 0;
-        a.jobs = ptr<GemmJob>(h->jobs) + h->tri1_r[ht].off;
+        a.jobs = ptr<GemmJob>(h->jobs) + h->ranges.tri1[ht].off;
         a.job_mode = JOBS_TABLE;
-        int rc = launch_gemm<EPI_STORE>(h, h->mapQ, h->mapK, a, h->tri1_r[ht].cnt);
+        int rc = launch_gemm<EPI_STORE>(h, h->mapQ, h->mapK, a, h->ranges.tri1[ht].cnt);
         if (rc) return rc;
         GemmArgs b;
         memset(&b, 0, sizeof(b));
@@ -848,12 +893,12 @@ int build_linv(gpk_handle* h) {
         b.C = ptr<double>(h->P); b.ldc = NP;
         b.Ct = ptr<double>(h->Q); b.ldct = NP;
         b.alpha = -1.0; b.beta = 0;
-        b.jobs = ptr<GemmJob>(h->jobs) + h->tri2_r[ht].off;
+        b.jobs = ptr<GemmJob>(h->jobs) + h->ranges.tri2[ht].off;
         b.job_mode = JOBS_TABLE;
-        rc = launch_gemm<EPI_STORE>(h, h->mapP, h->mapW, b, h->tri2_r[ht].cnt);
+        rc = launch_gemm<EPI_STORE>(h, h->mapP, h->mapW, b, h->ranges.tri2[ht].cnt);
         if (rc) return rc;
     }
-    CK(cudaEventRecord(h->ev[5], h->stream));
+    CK(cudaEventRecord(h->timing.ev[5], h->stream));
     h->linv_ready = true;
     h->linv_serial += 1;
     h->alpha_ready = false;
@@ -894,36 +939,36 @@ int make_oz_map(gpk_handle* h, CUtensorMap* map, void* base, long rows_total, lo
 // A kernel with a factor is never eligible: the digit split of K* assumes 0 < k <= amp.
 int prepare_ozaki(gpk_handle* h, bool* usable) {
     *usable = false;
-    if (!h->ozaki || h->NP > 16384 || h->spec.factor.kind != GPK_FACTOR_NONE)
+    if (!h->oz.enabled || h->NP > 16384 || h->spec.factor.kind != GPK_FACTOR_NONE)
         return GPK_OK;
     const long NP = h->NP;
-    if (h->oz_linv_serial != h->linv_serial) {
+    if (h->oz.linv_serial != h->linv_serial) {
         int rc;
-        if ((rc = ensure(h, h->oz_Pq, (size_t)OZ_S * NP * NP))) return rc;
-        if ((rc = ensure(h, h->oz_eP, (size_t)NP * 4))) return rc;
-        if ((rc = ensure(h, h->oz_emax, 4))) return rc;
+        if ((rc = ensure(h, h->oz.Pq, (size_t)OZ_S * NP * NP))) return rc;
+        if ((rc = ensure(h, h->oz.eP, (size_t)NP * 4))) return rc;
+        if ((rc = ensure(h, h->oz.emax, 4))) return rc;
         const int lowest = -100000;
-        CK(cudaMemcpyAsync(h->oz_emax.p, &lowest, 4, cudaMemcpyHostToDevice, h->stream));
-        gpk_oz_rowexp_kernel<<<(unsigned)NP, 256, 0, h->stream>>>(ptr<double>(h->P), NP, (int)NP, ptr<int>(h->oz_eP), ptr<int>(h->oz_emax));
+        CK(cudaMemcpyAsync(h->oz.emax.p, &lowest, 4, cudaMemcpyHostToDevice, h->stream));
+        gpk_oz_rowexp_kernel<<<(unsigned)NP, 256, 0, h->stream>>>(ptr<double>(h->P), NP, (int)NP, ptr<int>(h->oz.eP), ptr<int>(h->oz.emax));
         CKL();
-        gpk_oz_split_kernel<<<(unsigned)((NP * NP + 255) / 256), 256, 0, h->stream>>>(ptr<double>(h->P), NP, NP, ptr<int>(h->oz_eP), 0,
-                                                                                   ptr<int8_t>(h->oz_Pq), NP * NP);
+        gpk_oz_split_kernel<<<(unsigned)((NP * NP + 255) / 256), 256, 0, h->stream>>>(ptr<double>(h->P), NP, NP, ptr<int>(h->oz.eP), 0,
+                                                                                   ptr<int8_t>(h->oz.Pq), NP * NP);
         CKL();
         // the mean goes through fp64, mu - mean = K* alpha
         if ((rc = ensure_alpha(h))) return rc;
-        CK(cudaMemcpyAsync(&h->oz_emax_host, h->oz_emax.p, 4, cudaMemcpyDeviceToHost, h->stream));
+        CK(cudaMemcpyAsync(&h->oz.emax_host, h->oz.emax.p, 4, cudaMemcpyDeviceToHost, h->stream));
         CK(cudaStreamSynchronize(h->stream));
-        h->oz_map_cs = 0;
-        h->oz_linv_serial = h->linv_serial;
+        h->oz.map_cs = 0;
+        h->oz.linv_serial = h->linv_serial;
     }
     // each CTA of a cluster loads 128 / CS rows of every L^-1 slice; 64-row (CS = 2) and 32-row (CS = 4) offsets are
     // multiples of the 512-byte SWIZZLE_64B atom, so the multicast pieces form the same swizzled 128-row tile
-    if (h->oz_map_cs != h->oz_cluster) {
+    if (h->oz.map_cs != h->oz.cluster) {
         int rc;
-        if ((rc = make_oz_map(h, &h->mapOzP, h->oz_Pq.p, (long)OZ_S * NP, NP, OZ_TM / h->oz_cluster))) return rc;
-        h->oz_map_cs = h->oz_cluster;
+        if ((rc = make_oz_map(h, &h->oz.mapP, h->oz.Pq.p, (long)OZ_S * NP, NP, OZ_TM / h->oz.cluster))) return rc;
+        h->oz.map_cs = h->oz.cluster;
     }
-    *usable = h->oz_emax_host <= OZ_MAX_EXP;
+    *usable = h->oz.emax_host <= OZ_MAX_EXP;
     return GPK_OK;
 }
 
@@ -983,11 +1028,11 @@ int score_dev(gpk_handle* h, const double* dX, long m, int kind, double eta, dou
     if (use_oz) {
         // slices of K* per chunk buffer: [S][cap][NP] int8; one exponent for the whole matrix (0 < k <= amp)
         // (the tensor maps are re-encoded per call: a few microseconds, and they depend on the buffer, cap and NP)
-        if ((rc = ensure(h, h->oz_Kq, (size_t)OZ_S * cap * NP))) return rc;
-        if (h->overlap && (rc = ensure(h, h->oz_Kq2, (size_t)OZ_S * cap * NP))) return rc;
-        if ((rc = make_oz_map(h, &h->mapOzK, h->oz_Kq.p, (long)OZ_S * cap, NP, OZ_TN))) return rc;
-        if (h->overlap && (rc = make_oz_map(h, &h->mapOzK2, h->oz_Kq2.p, (long)OZ_S * cap, NP, OZ_TN))) return rc;
-        if (h->overlap && (rc = ensure(h, h->oz_pmu2, (size_t)h->nb * cap * 8))) return rc;
+        if ((rc = ensure(h, h->oz.Kq, (size_t)OZ_S * cap * NP))) return rc;
+        if (h->overlap && (rc = ensure(h, h->oz.Kq2, (size_t)OZ_S * cap * NP))) return rc;
+        if ((rc = make_oz_map(h, &h->oz.mapK, h->oz.Kq.p, (long)OZ_S * cap, NP, OZ_TN))) return rc;
+        if (h->overlap && (rc = make_oz_map(h, &h->oz.mapK2, h->oz.Kq2.p, (long)OZ_S * cap, NP, OZ_TN))) return rc;
+        if (h->overlap && (rc = ensure(h, h->oz.pmu2, (size_t)h->nb * cap * 8))) return rc;
         oz_eK = oz_exponent(h->spec.amp);
     }
     if (d_best == nullptr) d_best = ptr<BestPair>(h->best);
@@ -996,29 +1041,19 @@ int score_dev(gpk_handle* h, const double* dX, long m, int kind, double eta, dou
         CK(cudaMemsetAsync(d_best, 0xFF, sizeof(BestPair), h->stream));
         CK(cudaMemsetAsync(d_nneg, 0, 8, h->stream));
     }
-    CK(cudaEventRecord(h->ev[6], h->stream));
+    CK(cudaEventRecord(h->timing.ev[6], h->stream));
     const int nchunks = (int)((m + cap - 1) / cap);
     // With more than one chunk, K* of chunk i+1 is built on the low-priority side stream (8 candidates
     // per thread, ~60 registers: its CTAs fit next to the resident GEMM CTAs and use the FP64 ALUs while
     // the GEMM keeps the DMMA pipe busy); two K* buffers alternate.
     const bool pipelined = h->overlap && nchunks > 1;
-    if (pipelined) {
-        while ((int)h->ev_cov.size() < nchunks) {
-            cudaEvent_t e1, e2;
-            CK(cudaEventCreateWithFlags(&e1, cudaEventDisableTiming));
-            CK(cudaEventCreateWithFlags(&e2, cudaEventDisableTiming));
-            h->ev_cov.push_back(e1);
-            h->ev_gemm.push_back(e2);
-        }
-    }
-    while ((int)h->ev_g0.size() < nchunks) {
-        cudaEvent_t e1, e2;
-        CK(cudaEventCreate(&e1));
-        CK(cudaEventCreate(&e2));
-        h->ev_g0.push_back(e1);
-        h->ev_g1.push_back(e2);
-    }
-    h->last_nchunks = nchunks;
+    if (pipelined && ((rc = grow_events(h, h->ev_cov, nchunks, cudaEventDisableTiming)) ||
+                      (rc = grow_events(h, h->ev_gemm, nchunks, cudaEventDisableTiming))))
+        return rc;
+    if ((rc = grow_events(h, h->timing.ev_g0, nchunks, cudaEventDefault)) ||
+        (rc = grow_events(h, h->timing.ev_g1, nchunks, cudaEventDefault)))
+        return rc;
+    h->timing.last_nchunks = nchunks;
     auto launch_cov = [&](int ci, cudaStream_t st, bool small) -> int {
         const long base = (long)ci * cap;
         const long mc = std::min(cap, m - base);
@@ -1038,8 +1073,8 @@ int score_dev(gpk_handle* h, const double* dX, long m, int kind, double eta, dou
         CUtensorMap map;
         int mrc = make_cov_map(h, &map, h->Xts.p, h->spec.n_terms, NP);
         if (mrc) return mrc;
-        int8_t* qdst = second ? ptr<int8_t>(h->oz_Kq2) : ptr<int8_t>(h->oz_Kq);
-        double* pmu = second ? ptr<double>(h->oz_pmu2) : ptr<double>(h->part_mu);
+        int8_t* qdst = second ? ptr<int8_t>(h->oz.Kq2) : ptr<int8_t>(h->oz.Kq);
+        double* pmu = second ? ptr<double>(h->oz.pmu2) : ptr<double>(h->part_mu);
         const int gx = (int)(NP / 128);
         if (small)
             gpk_cov_oz_kernel<4><<<(unsigned)(gx * (mcp / 16)), 256, cov_oz_smem_bytes(h->spec.n_terms, 4), st>>>(
@@ -1063,7 +1098,7 @@ int score_dev(gpk_handle* h, const double* dX, long m, int kind, double eta, dou
         const long mc = std::min(cap, m - base);
         const long mcp = round_up(mc, BM);
         const bool last = ci == nchunks - 1;
-        if (last) CK(cudaEventRecord(h->ev[8], h->stream));
+        if (last) CK(cudaEventRecord(h->timing.ev[8], h->stream));
         if (pipelined) {
             CK(cudaStreamWaitEvent(h->stream, h->ev_cov[ci], 0));
             if (ci + 1 < nchunks) {
@@ -1086,20 +1121,19 @@ int score_dev(gpk_handle* h, const double* dX, long m, int kind, double eta, dou
         a.part_mu = ptr<double>(h->part_mu);
         a.part_ssq = ptr<double>(h->part_ssq);
         a.ldpart = cap;
-        if (last) CK(cudaEventRecord(h->ev[10], h->stream));
-        CK(cudaEventRecord(h->ev_g0[ci], h->stream));
+        if (last) CK(cudaEventRecord(h->timing.ev[10], h->stream));
+        CK(cudaEventRecord(h->timing.ev_g0[ci], h->stream));
         if (use_oz) {
-            if ((rc = launch_oz_contraction(h, h->mapOzP, second ? h->mapOzK2 : h->mapOzK, h->nb, mcp, NP, cap,
-                                            ptr<int>(h->oz_eP), oz_eK, a.part_ssq, a.ldpart)))
+            if ((rc = launch_oz_contraction(h, h->oz.mapP, second ? h->oz.mapK2 : h->oz.mapK, h->nb, mcp, NP, cap,
+                                            ptr<int>(h->oz.eP), oz_eK, a.part_ssq, a.ldpart)))
                 return rc;
-            h->oz_launches += 1;
+            h->oz.launches += 1;
         } else if ((rc = launch_gemm<EPI_COLREDUCE>(h, h->mapP, second ? h->mapKs2 : h->mapKs, a, h->nb * a.mcb))) return rc;
-        CK(cudaEventRecord(h->ev_g1[ci], h->stream));
-        if (last) CK(cudaEventRecord(h->ev[11], h->stream));
+        CK(cudaEventRecord(h->timing.ev_g1[ci], h->stream));
+        if (last) CK(cudaEventRecord(h->timing.ev[11], h->stream));
         // fp64 path: this parity's K* buffer is free once the contraction has read it
         if (pipelined && !use_oz) CK(cudaEventRecord(h->ev_gemm[ci], h->stream));
-        h->launches_var += 1;
-        h->last_chunk_rows = mcp;
+        h->timing.launches_var += 1;
         FinishArgs f;
         memset(&f, 0, sizeof(f));
         f.part_mu = ptr<double>(h->part_mu); f.part_ssq = ptr<double>(h->part_ssq);
@@ -1111,7 +1145,7 @@ int score_dev(gpk_handle* h, const double* dX, long m, int kind, double eta, dou
         f.up = h->has_bounds ? ptr<double>(h->upper) : nullptr;
         f.norm_out = h->norm_out; f.y_mean = h->y_mean; f.y_std = h->y_std;
         f.o = score_out(h, kind, eta, par, d_out, d_mu, d_var, d_nneg, index_offset + base, global_base);
-        if (use_oz && second) f.part_mu = ptr<double>(h->oz_pmu2);
+        if (use_oz && second) f.part_mu = ptr<double>(h->oz.pmu2);
         const int fb = (int)((mc + 255) / 256);
         gpk_finish_kernel<<<fb, 256, 0, h->stream>>>(f);
         CKL();
@@ -1121,14 +1155,14 @@ int score_dev(gpk_handle* h, const double* dX, long m, int kind, double eta, dou
         }
         // int8 path: the builder also writes this parity's mean partials, which the finish kernel above still reads
         if (pipelined && use_oz) CK(cudaEventRecord(h->ev_gemm[ci], h->stream));
-        if (last) CK(cudaEventRecord(h->ev[12], h->stream));
+        if (last) CK(cudaEventRecord(h->timing.ev[12], h->stream));
     }
-    CK(cudaEventRecord(h->ev[7], h->stream));
-    h->score_timed = true;
+    CK(cudaEventRecord(h->timing.ev[7], h->stream));
+    h->timing.score_timed = true;
     return GPK_OK;
 }
 
-// layout of h->es_state (doubles): logP (nb), lmb (nb), dMu (nb x nb), dSig (nb x T), Hs (nb x T), W (np), lower (d),
+// layout of h->es.state (doubles): logP (nb), lmb (nb), dMu (nb x nb), dSig (nb x T), Hs (nb x T), W (np), lower (d),
 // upper (d), scaled zb (nb x d)
 struct EsLayout {
     size_t logP, lmb, dMu, dSig, Hs, W, lo, up, zb, total;
@@ -1139,7 +1173,7 @@ struct EsLayout {
     }
 };
 
-// layout of h->mc_state (doubles): Mb (nb), Vb (nb x nb), W (np), lmb (nb), scaled zb (nb x d), F (nb x nf)
+// layout of h->mc.state (doubles): Mb (nb), Vb (nb x nb), W (np), lmb (nb), scaled zb (nb x d), F (nb x nf)
 struct McLayout {
     size_t Mb, Vb, W, lmb, zb, F, total;
     McLayout(int nb, int np_, int d, int nf) {
@@ -1187,17 +1221,17 @@ const long ES_CH = 16384;                   // candidates per pass of es_dh_dev;
 
 // es_dh_dev's scratch (variance and sigma of one pass), sized for the handle's current gpk_es_update
 int es_reserve(gpk_handle* h) {
-    return ensure(h, h->es_work, (size_t)ES_CH * (h->es_nb + 1) * 8);
+    return ensure(h, h->es.work, (size_t)ES_CH * (h->es.nb + 1) * 8);
 }
 
 // One pass of es_dh_dev's first half: the predictive variance of rows <= ES_CH candidates X (the scoring pass) into
-// es_work's var (rows) and their clipped covariance to zb into its sig (rows x nb), the two buffers gpk_es_dh_kernel
+// es.work's var (rows) and their clipped covariance to zb into its sig (rows x nb), the two buffers gpk_es_dh_kernel
 // reads.  Asynchronous on the handle's stream; needs es_reserve and a current gpk_es_update.
 int es_moments_pass(gpk_handle* h, const double* X, long rows) {
-    const int nb = h->es_nb, d = h->d;
-    const double* zs = h->es_kind == ES_KIND_MC ? ptr<double>(h->mc_state) + McLayout(nb, h->es_np, d, h->es_nf).zb
-                                                : ptr<double>(h->es_state) + EsLayout(nb, h->es_np, d).zb;
-    double* var = ptr<double>(h->es_work);
+    const int nb = h->es.nb, d = h->d;
+    const double* zs = h->es.kind == ES_KIND_MC ? ptr<double>(h->mc.state) + McLayout(nb, h->es.np, d, h->mc.nf).zb
+                                                : ptr<double>(h->es.state) + EsLayout(nb, h->es.np, d).zb;
+    double* var = ptr<double>(h->es.work);
     double* sig = var + ES_CH;
     const double* lo = h->has_bounds ? ptr<double>(h->lower) : nullptr;
     const double* up = h->has_bounds ? ptr<double>(h->upper) : nullptr;
@@ -1206,7 +1240,7 @@ int es_moments_pass(gpk_handle* h, const double* X, long rows) {
     if ((rc = score_dev(h, X, rows, GPK_ACQ_NONE, 0.0, 0.0, nullptr, nullptr, var, nullptr, nullptr))) return rc;
     gpk_es_sigma_kernel<<<(unsigned)rows, GPK_ES_THREADS, 0, h->stream>>>(h->spec, X, rows, d, lo, up,
                                                                           ptr<double>(h->Xrow), h->n,
-                                                                          ptr<double>(h->es_U), zs, nb,
+                                                                          ptr<double>(h->es.U), zs, nb,
                                                                           out_scale, sig);
     CKL();
     return GPK_OK;
@@ -1216,19 +1250,19 @@ int es_moments_pass(gpk_handle* h, const double* X, long rows) {
 // covariance to zb take, Xb the ones the bounds test of gpk_es_update's [lower, upper] sees (the same array unless the
 // model's inputs were transformed).  Asynchronous on the handle's stream; needs a current gpk_es_update.
 int es_dh_dev(gpk_handle* h, const double* Xm, const double* Xb, long m, double* d_out) {
-    const int nb = h->es_nb, d = h->d;
-    EsLayout L(nb, h->es_np, d);
-    const double* st = ptr<double>(h->es_state);
+    const int nb = h->es.nb, d = h->d;
+    EsLayout L(nb, h->es.np, d);
+    const double* st = ptr<double>(h->es.state);
     const long CH = ES_CH;
     int rc;
     if ((rc = es_reserve(h))) return rc;
-    const double* var = ptr<double>(h->es_work);
+    const double* var = ptr<double>(h->es.work);
     const double* sig = var + CH;
     for (long c0 = 0; c0 < m; c0 += CH) {
         const long rows = std::min(CH, m - c0);
         if ((rc = es_moments_pass(h, Xm + c0 * d, rows))) return rc;
         gpk_es_dh_kernel<<<(unsigned)rows, GPK_ES_THREADS, 0, h->stream>>>(
-            Xb + c0 * d, rows, d, st + L.lo, st + L.up, var, sig, nb, h->es_np, h->es_sn2, h->es_H, st + L.logP,
+            Xb + c0 * d, rows, d, st + L.lo, st + L.up, var, sig, nb, h->es.np, h->es.sn2, h->es.H, st + L.logP,
             st + L.lmb, st + L.dMu, st + L.dSig, st + L.Hs, st + L.W, d_out + c0);
         CKL();
     }
@@ -1241,14 +1275,14 @@ int es_ready(gpk_handle* h, gpk_handle* report, const char* who, int kind = ES_K
     gpk_handle* r = report ? report : h;
     const char* upd = kind == ES_KIND_MC ? "gpk_esmc_update" : "gpk_es_update";
     if (gp_refusal(h)) { set_err(r, "%s: %s", who, gp_refusal(h)); return GPK_BAD_ARG; }
-    if (h->es_linv_serial < 0) { set_err(r, "%s: call %s first", who, upd); return GPK_BAD_ARG; }
-    if (!h->linv_ready || h->es_linv_serial != h->linv_serial) {
+    if (h->es.linv_serial < 0) { set_err(r, "%s: call %s first", who, upd); return GPK_BAD_ARG; }
+    if (!h->linv_ready || h->es.linv_serial != h->linv_serial) {
         set_err(r, "%s: the model changed since %s", who, upd);
         return GPK_BAD_ARG;
     }
-    if (kind != ES_KIND_NONE && h->es_kind != kind) {
+    if (kind != ES_KIND_NONE && h->es.kind != kind) {
         set_err(r, "%s: the current update is %s, not %s", who,
-                h->es_kind == ES_KIND_MC ? "gpk_esmc_update" : "gpk_es_update", upd);
+                h->es.kind == ES_KIND_MC ? "gpk_esmc_update" : "gpk_es_update", upd);
         return GPK_BAD_ARG;
     }
     return GPK_OK;
@@ -1256,7 +1290,7 @@ int es_ready(gpk_handle* h, gpk_handle* report, const char* who, int kind = ES_K
 
 // The zb half of an entropy-search update, shared by gpk_es_update and gpk_esmc_update: the raw representer points zb
 // (nb x d, host) scaled like the model's inputs into zs (device), and U = L^-T (L^-1 K(X, zb)) in fp64 from the handle's
-// L^-1 into h->es_U.  Asynchronous on the handle's stream.
+// L^-1 into h->es.U.  Asynchronous on the handle's stream.
 int es_build_u(gpk_handle* h, const double* zb, int nb, double* zs) {
     const int d = h->d, n = h->n, NP = h->NP;
     const size_t D = (size_t)nb;
@@ -1269,8 +1303,8 @@ int es_build_u(gpk_handle* h, const double* zb, int nb, double* zs) {
     gpk_es_scale_kernel<<<(unsigned)((D * d + 255) / 256), 256, 0, s>>>(ptr<double>(h->tmp1), nb, d, lo, up, zs);
     CKL();
     if (!h->linv_ready && (rc = build_linv(h))) return rc;
-    if ((rc = ensure(h, h->es_U, (size_t)NP * D * 8 * 2))) return rc;
-    double* U = ptr<double>(h->es_U);
+    if ((rc = ensure(h, h->es.U, (size_t)NP * D * 8 * 2))) return rc;
+    double* U = ptr<double>(h->es.U);
     double* tmp = U + (size_t)NP * D;
     CK(cudaMemsetAsync(tmp, 0, (size_t)NP * D * 8, s));
     gpk_es_kxz_kernel<<<(unsigned)(((long)n * nb + 255) / 256), 256, 0, s>>>(h->spec, ptr<double>(h->Xrow), n, d, zs, nb,
@@ -1295,18 +1329,18 @@ int mc_kernel_attrs(gpk_handle* h) {
 // the 2 status words of gpk_mc_pmin_kernel on h (device), zeroed on h's stream
 int mc_stat_reset(gpk_handle* h) {
     int rc;
-    if ((rc = ensure(h, h->mc_stat, 2 * sizeof(int)))) return rc;
-    CK(cudaMemsetAsync(h->mc_stat.p, 0, 2 * sizeof(int), h->stream));
+    if ((rc = ensure(h, h->mc.stat, 2 * sizeof(int)))) return rc;
+    CK(cudaMemsetAsync(h->mc.stat.p, 0, 2 * sizeof(int), h->stream));
     return GPK_OK;
 }
 
 // Waits for h's stream and reads the status words at d_stat: GPK_NOT_PD (numpy.linalg.LinAlgError, mc_part.py:40-41)
-// when a factorisation failed at every rung of the jitter ladder; the jittered count goes to h->mc_last_jitter.
+// when a factorisation failed at every rung of the jitter ladder; the jittered count goes to h->mc.last_jitter.
 int mc_stat_check(gpk_handle* h, const int* d_stat, const char* who) {
     int st[2] = {0, 0};
     CK(cudaMemcpyAsync(st, d_stat, sizeof(st), cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
-    h->mc_last_jitter = st[GPK_MC_STAT_JITTER];
+    h->mc.last_jitter = st[GPK_MC_STAT_JITTER];
     if (st[GPK_MC_STAT_NOT_PD] > 0) {
         set_err(h, "%s: Cholesky decomposition failed. (%d factorisation(s) not positive definite at noise 10000)", who,
                 st[GPK_MC_STAT_NOT_PD]);
@@ -1319,32 +1353,32 @@ int mc_stat_check(gpk_handle* h, const int* d_stat, const char* who) {
 // es_moments_pass, then gpk_mc_pmin_kernel, in passes of ES_CH.  The status words go to d_stat (2 ints, device), which
 // the caller zeroes and reads.  Asynchronous on the handle's stream; needs a current gpk_esmc_update.
 int esmc_dev(gpk_handle* h, const double* X, long m, double* d_out, int* d_stat) {
-    const int nb = h->es_nb, d = h->d;
-    McLayout L(nb, h->es_np, d, h->es_nf);
-    const double* st = ptr<double>(h->mc_state);
+    const int nb = h->es.nb, d = h->d;
+    McLayout L(nb, h->es.np, d, h->mc.nf);
+    const double* st = ptr<double>(h->mc.state);
     int rc;
     if ((rc = es_reserve(h))) return rc;
-    const double* var = ptr<double>(h->es_work);
+    const double* var = ptr<double>(h->es.work);
     const double* sig = var + ES_CH;
     if ((rc = mc_kernel_attrs(h))) return rc;
     for (long c0 = 0; c0 < m; c0 += ES_CH) {
         const long rows = std::min(ES_CH, m - c0);
         if ((rc = es_moments_pass(h, X + c0 * d, rows))) return rc;
         gpk_mc_pmin_kernel<<<(unsigned)rows, GPK_MC_THREADS, GPK_MC_SMEM, h->stream>>>(
-            nullptr, st + L.Mb, st + L.W, h->es_np, st + L.Vb, nb, st + L.F, h->es_nf, var, sig, h->es_sn2, st + L.lmb,
-            h->es_H, d_out + c0, nullptr, nullptr, d_stat);
+            nullptr, st + L.Mb, st + L.W, h->es.np, st + L.Vb, nb, st + L.F, h->mc.nf, var, sig, h->es.sn2, st + L.lmb,
+            h->es.H, d_out + c0, nullptr, nullptr, d_stat);
         CKL();
     }
     return GPK_OK;
 }
 
-// the layout of h->blr_data (doubles): Phi (n x F), y (n), G (F x F), b (F)
-inline double* blr_phi(gpk_handle* h) { return ptr<double>(h->blr_data); }
-inline double* blr_y(gpk_handle* h) { return blr_phi(h) + (size_t)h->n * h->blr_F; }
+// the layout of h->blr.data (doubles): Phi (n x F), y (n), G (F x F), b (F)
+inline double* blr_phi(gpk_handle* h) { return ptr<double>(h->blr.data); }
+inline double* blr_y(gpk_handle* h) { return blr_phi(h) + (size_t)h->n * h->blr.F; }
 inline double* blr_G(gpk_handle* h) { return blr_y(h) + h->n; }
-inline double* blr_b(gpk_handle* h) { return blr_G(h) + (size_t)h->blr_F * h->blr_F; }
+inline double* blr_b(gpk_handle* h) { return blr_G(h) + (size_t)h->blr.F * h->blr.F; }
 
-// the layout of h->blr_post (doubles) for k posteriors: M (k x F), L^-1 (k x F x F), S (k x F x F), 1 / beta (k), then
+// the layout of h->blr.post (doubles) for k posteriors: M (k x F), L^-1 (k x F x F), S (k x F x F), 1 / beta (k), then
 // k int failure flags
 struct BlrPost {
     size_t M, Li, S, ib, fail, total;
@@ -1360,26 +1394,26 @@ int blr_ready(gpk_handle* h, const char* who) {
     int rc;
     if (h && h->model == MODEL_DNGO) {
         if ((rc = model_ready(h, MODEL_DNGO, who))) return rc;
-        if (!h->dngo_trained) { set_err(h, "%s: model is not trained (gpk_dngo_train)", who); return GPK_NOT_FITTED; }
+        if (!h->dngo.trained) { set_err(h, "%s: model is not trained (gpk_dngo_train)", who); return GPK_NOT_FITTED; }
     } else if ((rc = model_ready(h, MODEL_BLR, who))) {
         return rc;
     }
-    const int sm_eval = (int)(gpk_blr_smem_doubles(h->blr_F) * 8);
+    const int sm_eval = (int)(gpk_blr_smem_doubles(h->blr.F) * 8);
     CK(cudaFuncSetAttribute(gpk_blr_eval_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, sm_eval));
     CK(cudaFuncSetAttribute(gpk_blr_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, sm_eval));
     CK(cudaFuncSetAttribute(gpk_blr_fit_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                            sm_eval + h->blr_F * h->blr_F * 8));
+                            sm_eval + h->blr.F * h->blr.F * 8));
     CK(cudaFuncSetAttribute(gpk_blr_score_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                            h->blr_F * GPK_BLR_SCORE_THREADS * 8));
+                            h->blr.F * GPK_BLR_SCORE_THREADS * 8));
     return GPK_OK;
 }
 
-// the layout of h->rf_data: X (n x d doubles), y (n doubles), the per-feature row order (d x n ints)
-inline double* rf_X(gpk_handle* h) { return ptr<double>(h->rf_data); }
+// the layout of h->rf.data: X (n x d doubles), y (n doubles), the per-feature row order (d x n ints)
+inline double* rf_X(gpk_handle* h) { return ptr<double>(h->rf.data); }
 inline double* rf_y(gpk_handle* h) { return rf_X(h) + (size_t)h->n * h->d; }
 inline int* rf_order(gpk_handle* h) { return (int*)(rf_y(h) + h->n); }
 
-// the layout of h->rf_nodes (bytes) for T trees of S = 2 n node slots: feat, left (T x S ints), n_nodes (T ints, padded
+// the layout of h->rf.nodes (bytes) for T trees of S = 2 n node slots: feat, left (T x S ints), n_nodes (T ints, padded
 // to 8 bytes), thr, W, mean, var (T x S doubles each)
 struct RfNodes {
     size_t feat, left, nn, thr, W, mean, var, total;
@@ -1391,8 +1425,8 @@ struct RfNodes {
     }
 };
 
-// the layout of h->bnn_data: the scaled X (n x d), the scaled y (n), the input mean and std (d each)
-inline double* bnn_X(gpk_handle* h) { return ptr<double>(h->bnn_data); }
+// the layout of h->bnn.data: the scaled X (n x d), the scaled y (n), the input mean and std (d each)
+inline double* bnn_X(gpk_handle* h) { return ptr<double>(h->bnn.data); }
 inline double* bnn_y(gpk_handle* h) { return bnn_X(h) + (size_t)h->n * h->d; }
 inline double* bnn_xm(gpk_handle* h) { return bnn_y(h) + h->n; }
 inline double* bnn_xs(gpk_handle* h) { return bnn_xm(h) + h->d; }
@@ -1425,12 +1459,12 @@ int surrogate_score(gpk_handle* h, const double* dX, long m, int kind, double et
     const ScoreOut o = score_out(h, kind, eta, par, d_out, d_mu, d_var, d_nneg, index_offset, global_base);
     switch (h->model) {
     case MODEL_BLR: {
-        const int F = h->blr_F, k = h->blr_k;
+        const int F = h->blr.F, k = h->blr.k;
         const BlrPost L(k, F);
-        const double* post = ptr<double>(h->blr_post);
+        const double* post = ptr<double>(h->blr.post);
         BlrScoreArgs a;
         memset(&a, 0, sizeof(a));
-        a.X = dX; a.m = m; a.D = h->d; a.F = F; a.basis = h->blr_basis; a.k = k;
+        a.X = dX; a.m = m; a.D = h->d; a.F = F; a.basis = h->blr.basis; a.k = k;
         a.M = post + L.M; a.Li = post + L.Li; a.ib = post + L.ib;
         a.o = o;
         gpk_blr_score_kernel<<<(unsigned)nblk, GPK_BLR_SCORE_THREADS, (size_t)F * GPK_BLR_SCORE_THREADS * 8, h->stream>>>(a);
@@ -1438,27 +1472,27 @@ int surrogate_score(gpk_handle* h, const double* dX, long m, int kind, double et
     }
     case MODEL_RF: {
         const long S = 2L * h->n;
-        const RfNodes L(h->rf_T, S);
-        const char* nodes = ptr<char>(h->rf_nodes);
+        const RfNodes L(h->rf.T, S);
+        const char* nodes = ptr<char>(h->rf.nodes);
         RfScoreArgs a;
         memset(&a, 0, sizeof(a));
-        a.X = dX; a.m = m; a.D = h->d; a.T = h->rf_T; a.S = S;
+        a.X = dX; a.m = m; a.D = h->d; a.T = h->rf.T; a.S = S;
         a.feat = (const int*)(nodes + L.feat); a.left = (const int*)(nodes + L.left);
         a.thr = (const double*)(nodes + L.thr); a.mean = (const double*)(nodes + L.mean);
         a.var = (const double*)(nodes + L.var);
-        a.total_var = h->rf_total;
+        a.total_var = h->rf.total;
         a.o = o;
-        gpk_rf_score_kernel<<<(unsigned)nblk, GPK_RF_SCORE_WARPS * 32, gpk_rf_score_smem_doubles(h->rf_T) * 8,
+        gpk_rf_score_kernel<<<(unsigned)nblk, GPK_RF_SCORE_WARPS * 32, gpk_rf_score_smem_doubles(h->rf.T) * 8,
                               h->stream>>>(a);
         break;
     }
     case MODEL_BNN: {
         BnnScoreArgs a;
         memset(&a, 0, sizeof(a));
-        a.X = dX; a.m = m; a.D = h->d; a.P = h->bnn_P; a.S = h->bnn_S;
-        a.samples = ptr<double>(h->bnn_samples);
+        a.X = dX; a.m = m; a.D = h->d; a.P = h->bnn.P; a.S = h->bnn.S;
+        a.samples = ptr<double>(h->bnn.samples);
         a.xm = bnn_xm(h); a.xs = bnn_xs(h);
-        a.y_mean = h->bnn_ymean; a.y_std = h->bnn_ystd;
+        a.y_mean = h->bnn.ymean; a.y_std = h->bnn.ystd;
         a.o = o;
         const size_t smem = (size_t)gpk_bnn_score_smem(h->d);
         CK(cudaFuncSetAttribute(gpk_bnn_score_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -1469,9 +1503,9 @@ int surrogate_score(gpk_handle* h, const double* dX, long m, int kind, double et
         DngoScoreArgs a;
         memset(&a, 0, sizeof(a));
         a.X = dX; a.m = m; a.D = h->d; a.ntiles = (int)ntiles;
-        a.pack = ptr<double>(h->dngo_pack);
+        a.pack = ptr<double>(h->dngo.pack);
         a.xm = bnn_xm(h); a.xs = bnn_xs(h);
-        a.y_mean = h->bnn_ymean; a.y_std = h->bnn_ystd;
+        a.y_mean = h->bnn.ymean; a.y_std = h->bnn.ystd;
         a.o = o;
         const size_t smem = (size_t)gpk_dngo_score_smem(h->d);
         CK(cudaFuncSetAttribute(gpk_dngo_score_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -1520,8 +1554,7 @@ int gpk_create(gpk_handle** out, int device) {
     }
     h->stream = h->own_stream;
     for (int i = 0; i < 16; ++i)
-        if (cudaEventCreate(&h->ev[i]) != cudaSuccess) { delete h; return GPK_CUDA_ERROR; }
-    h->ev_ok = true;
+        if (cudaEventCreate(&h->timing.ev[i]) != cudaSuccess) { delete h; return GPK_CUDA_ERROR; }
     if (cudaEventCreateWithFlags(&h->ev_order, cudaEventDisableTiming) != cudaSuccess) { delete h; return GPK_CUDA_ERROR; }
     int rc = set_kernel_attrs(h);
     if (rc) { fprintf(stderr, "gpk_create: %s\n", h->err); delete h; return rc; }
@@ -1543,34 +1576,6 @@ int gpk_destroy(gpk_handle* h) {
     cudaSetDevice(h->device);
     cudaStreamSynchronize(h->stream);
     gpk_comm_destroy(h);
-    if (h->ev_multi) cudaEventDestroy(h->ev_multi);
-    DevBuf* bufs[] = {&h->Xrow, &h->Xt, &h->y, &h->Kbuf, &h->P, &h->Q, &h->W, &h->lower, &h->upper, &h->logdet_part,
-                      &h->scal, &h->status, &h->jobs, &h->cand, &h->Kstar, &h->Kstar2, &h->cand2, &h->part_mu, &h->part_ssq, &h->out_mu,
-                      &h->out_var, &h->out_acq, &h->block_best, &h->best, &h->nneg, &h->Vt, &h->cov, &h->XsT,
-                      &h->tmpjobs, &h->alpha, &h->tmp1, &h->tmp2, &h->tmp3, &h->dprof, &h->Xts, &h->oz_Pq, &h->oz_Kq, &h->oz_Kq2, &h->oz_eP, &h->oz_emax, &h->oz_pmu2, &h->oz_probe,
-                      &h->multi_cand, &h->multi_A, &h->multi_B, &h->multi_out, &h->multi_bb, &h->gather, &h->best_global,
-                      &h->de_pop, &h->de_trial, &h->de_param, &h->de_E, &h->de_small, &h->de_sort, &h->lb_buf, &h->cma_buf, &h->dir_buf, &h->ep_buf, &h->es_state, &h->es_U, &h->es_work, &h->es_in, &h->mc_state, &h->mc_buf, &h->mc_stat, &h->fab_in, &h->rs_buf, &h->hy_buf, &h->hb_buf,
-                      &h->blr_data, &h->blr_post, &h->blr_work, &h->rf_data, &h->rf_work, &h->rf_nodes,
-                      &h->bnn_data, &h->bnn_samples, &h->bnn_state, &h->dngo_net, &h->dngo_state, &h->dngo_pack};
-    for (DevBuf* b : bufs)
-        if (b->p) cudaFree(b->p);
-    if (h->ev_ok)
-        for (int i = 0; i < 16; ++i) cudaEventDestroy(h->ev[i]);
-    if (h->ev_order) cudaEventDestroy(h->ev_order);
-    for (int i = 0; i < 2; ++i)
-        if (h->stage[i]) cudaFreeHost(h->stage[i]);
-    for (cudaEvent_t e : h->ev_panel) cudaEventDestroy(e);
-    for (cudaEvent_t e : h->ev_rest) cudaEventDestroy(e);
-    for (cudaEvent_t e : h->ev_cov) cudaEventDestroy(e);
-    for (cudaEvent_t e : h->ev_g0) cudaEventDestroy(e);
-    for (cudaEvent_t e : h->ev_g1) cudaEventDestroy(e);
-    for (cudaEvent_t e : h->ev_copied) cudaEventDestroy(e);
-    for (cudaEvent_t e : h->ev_scored) cudaEventDestroy(e);
-    if (h->copy_stream) cudaStreamDestroy(h->copy_stream);
-    for (cudaEvent_t e : h->ev_gemm) cudaEventDestroy(e);
-    if (h->side_stream) cudaStreamDestroy(h->side_stream);
-    if (h->own_stream) cudaStreamDestroy(h->own_stream);
-    if (h->pin) cudaFreeHost(h->pin);
     delete h;
     return GPK_OK;
 }
@@ -1579,24 +1584,24 @@ int gpk_set_option(gpk_handle* h, const char* key, long value) {
     if (!h || !key) return GPK_BAD_ARG;
     if (!strcmp(key, "ozpersist")) {
         if (value != 0 && value != 1 && value != 3) BAD("ozpersist must be 0, 1 or 3");
-        h->oz_persist = (int)value;
+        h->oz.persist = (int)value;
         return GPK_OK;
     }
     if (!strcmp(key, "ozcluster")) {
         if (value != 1 && value != 2 && value != 4) BAD("ozcluster must be 1, 2 or 4");
-        h->oz_cluster = (int)value;
+        h->oz.cluster = (int)value;
         return GPK_OK;
     }
     if (!strcmp(key, "ozgrid")) {
         if (value < 0 || value > (1L << 20)) BAD("ozgrid must be >= 0 (0: as many clusters as fit)");
-        h->oz_grid = (int)value;
+        h->oz.grid = (int)value;
         return GPK_OK;
     }
     if (!strcmp(key, "ozaki")) {
         if (value != 0 && value != 1)
             BAD("ozaki must be 0 (fp64 DMMA) or 1 (int8 tensor pipe, error-free split; kernels with the environment "
                 "factor always take fp64)");
-        h->ozaki = (int)value;
+        h->oz.enabled = (int)value;
         return GPK_OK;
     }
     if (!strcmp(key, "depth2")) {
@@ -1629,7 +1634,7 @@ int gpk_set_option(gpk_handle* h, const char* key, long value) {
     }
     if (!strcmp(key, "hyper_batch_bytes")) {
         if (value < 1) BAD("hyper_batch_bytes must be >= 1 (default %ld)", (long)GPK_HYPER_BATCH_BYTES);
-        h->hyper_batch_bytes = value;
+        h->hyper.batch_bytes = value;
         return GPK_OK;
     }
     if (!strcmp(key, "chunk")) {
@@ -1789,8 +1794,6 @@ int gpk_set_kernel(gpk_handle* h, int family, double log_amp, int n_terms, const
     }
     if (group[0] != 0) BAD("gpk_set_kernel: groups must start at 0");
     h->spec = s;
-    h->log_amp = log_amp;
-    h->log_metric.assign(log_metric, log_metric + n_terms);
     h->has_spec = true;
     h->fitted = false;
     h->linv_ready = false;
@@ -1850,7 +1853,7 @@ int gpk_fit_begin(gpk_handle* h, double diag_add, double mean) {
     h->diag_add = diag_add;
     double* K = ptr<double>(h->Kbuf);
 
-    CK(cudaEventRecord(h->ev[0], h->stream));
+    CK(cudaEventRecord(h->timing.ev[0], h->stream));
     {
         // the pre-scaled operand depends on the hyper-parameters: rebuilt per fit (n_terms x NP)
         if ((rc = ensure(h, h->Xts, (size_t)GPK_MAX_TERMS * NP * 8))) return rc;
@@ -1864,14 +1867,10 @@ int gpk_fit_begin(gpk_handle* h, double diag_add, double mean) {
         CKL();
     }
     CK(cudaMemsetAsync(h->status.p, 0, 4, h->stream));
-    CK(cudaEventRecord(h->ev[1], h->stream));
-    while ((int)h->ev_panel.size() < nb) {
-        cudaEvent_t e1, e2;
-        CK(cudaEventCreateWithFlags(&e1, cudaEventDisableTiming));
-        CK(cudaEventCreateWithFlags(&e2, cudaEventDisableTiming));
-        h->ev_panel.push_back(e1);
-        h->ev_rest.push_back(e2);
-    }
+    CK(cudaEventRecord(h->timing.ev[1], h->stream));
+    if ((rc = grow_events(h, h->ev_panel, nb, cudaEventDisableTiming)) ||
+        (rc = grow_events(h, h->ev_rest, nb, cudaEventDisableTiming)))
+        return rc;
     std::vector<char> rest_recorded(nb, 0);
     // ---- look-ahead schedule: diag(k), then the panel solve and the update of block column k+1 in 32-row tiles on the
     // critical stream; the rest of the trailing update on the side stream
@@ -1894,8 +1893,8 @@ int gpk_fit_begin(gpk_handle* h, double diag_add, double mean) {
         a.alpha = 1.0; a.beta = 0;
         a.job_mode = JOBS_TABLE;
         a.status = ptr<int>(h->status);
-        a.jobs = ptr<GemmJob>(h->jobs) + h->trsm32_r[k].off;
-        if ((rc = launch_gemm<EPI_STORE, 2>(h, h->mapK32, h->mapP, a, h->trsm32_r[k].cnt))) return rc;
+        a.jobs = ptr<GemmJob>(h->jobs) + h->ranges.trsm32[k].off;
+        if ((rc = launch_gemm<EPI_STORE, 2>(h, h->mapK32, h->mapP, a, h->ranges.trsm32[k].cnt))) return rc;
         GemmArgs s;
         memset(&s, 0, sizeof(s));
         s.A = K; s.lda = NP;
@@ -1904,7 +1903,7 @@ int gpk_fit_begin(gpk_handle* h, double diag_add, double mean) {
         s.alpha = -1.0; s.beta = 1;
         s.job_mode = JOBS_TABLE;
         s.status = ptr<int>(h->status);
-        const int off = h->syrk_r[k].off, cnt = h->syrk_r[k].cnt;
+        const int off = h->ranges.syrk[k].off, cnt = h->ranges.syrk[k].cnt;
         if (cnt > 0) {
             // Look-ahead: the first nb-k jobs update column block k+1 (what the next diagonal block
             // and panel solve need) and stay on the critical stream; the rest of the trailing update
@@ -1912,8 +1911,8 @@ int gpk_fit_begin(gpk_handle* h, double diag_add, double mean) {
             const int npu = nb - k;
             CK(cudaEventRecord(h->ev_panel[k], h->stream));                       // panel k solved
             if (k >= 1 && rest_recorded[k - 1]) CK(cudaStreamWaitEvent(h->stream, h->ev_rest[k - 1], 0));
-            s.jobs = ptr<GemmJob>(h->jobs) + h->pu32_r[k].off;
-            if ((rc = launch_gemm<EPI_STORE, 2>(h, h->mapK32, h->mapK, s, h->pu32_r[k].cnt))) return rc;
+            s.jobs = ptr<GemmJob>(h->jobs) + h->ranges.pu32[k].off;
+            if ((rc = launch_gemm<EPI_STORE, 2>(h, h->mapK32, h->mapK, s, h->ranges.pu32[k].cnt))) return rc;
             const bool d2 = h->depth2 == 1 || (h->depth2 == 2 && nb >= 48);
             if (cnt > npu && !d2) {
                 CK(cudaStreamWaitEvent(h->side_stream, h->ev_panel[k], 0));
@@ -1930,8 +1929,8 @@ int gpk_fit_begin(gpk_handle* h, double diag_add, double mean) {
                     s.jobs = ptr<GemmJob>(h->jobs) + off + npu;
                     if ((rc = launch_gemm<EPI_STORE>(h, h->mapK, h->mapK, s, std::min(nb - k - 1, cnt - npu), h->side_stream))) return rc;
                 } else {
-                    s.jobs = ptr<GemmJob>(h->jobs) + h->syrk2_r[k].off;
-                    if ((rc = launch_gemm<EPI_STORE>(h, h->mapK, h->mapK, s, h->syrk2_r[k].cnt, h->side_stream))) return rc;
+                    s.jobs = ptr<GemmJob>(h->jobs) + h->ranges.syrk2[k].off;
+                    if ((rc = launch_gemm<EPI_STORE>(h, h->mapK, h->mapK, s, h->ranges.syrk2[k].cnt, h->side_stream))) return rc;
                 }
                 CK(cudaEventRecord(h->ev_rest[k], h->side_stream));
                 rest_recorded[k] = 1;
@@ -1940,11 +1939,11 @@ int gpk_fit_begin(gpk_handle* h, double diag_add, double mean) {
     }
     gpk_diag_qfill_kernel<<<nb, 256, 0, h->stream>>>(ptr<double>(h->P), ptr<double>(h->Q), (long)NP, ptr<int>(h->status));
     CKL();
-    CK(cudaEventRecord(h->ev[2], h->stream));
+    CK(cudaEventRecord(h->timing.ev[2], h->stream));
     gpk_fit_reduce_kernel<<<1, 256, 0, h->stream>>>(K + NP * NP, h->n, ptr<double>(h->logdet_part), nb,
                                                     ptr<double>(h->scal));
     CKL();
-    CK(cudaEventRecord(h->ev[3], h->stream));
+    CK(cudaEventRecord(h->timing.ev[3], h->stream));
     CK(cudaMemcpyAsync(h->pin, h->scal.p, 16, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaMemcpyAsync(h->pin + 2, h->status.p, 4, cudaMemcpyDeviceToHost, h->stream));
     h->fit_pending = true;
@@ -1960,7 +1959,7 @@ int gpk_fit_end(gpk_handle* h, double* logdet, double* loglik) {
     const double* sc = h->pin;
     int st = 0;
     memcpy(&st, h->pin + 2, 4);
-    h->fit_timed = true;
+    h->timing.fit_timed = true;
     if (st != 0) {
         set_err(h, "matrix is not positive definite: pivot %d <= 0", st - 1);
         return GPK_NOT_PD;
@@ -2015,7 +2014,7 @@ int gpk_fit_append(gpk_handle* h, const double* X, const double* y, int n, int d
     double* Q = ptr<double>(h->Q);
     double* W = ptr<double>(h->W);
     if ((rc = ensure(h, h->tmp1, (size_t)NP * 8))) return rc;
-    CK(cudaEventRecord(h->ev[0], h->stream));
+    CK(cudaEventRecord(h->timing.ev[0], h->stream));
     // inputs (everything is re-uploaded: 8 n (d + 1) bytes; the first h->n rows of X must be the ones already fitted)
     if ((rc = ensure(h, h->Xrow, (size_t)NP * d * 8))) return rc;      // no-op: gpk_set_data sized it for NP rows
     CK(cudaMemcpyAsync(h->Xrow.p, X, (size_t)n * d * 8, cudaMemcpyHostToDevice, h->stream));
@@ -2040,22 +2039,22 @@ int gpk_fit_append(gpk_handle* h, const double* X, const double* y, int n, int d
         CKL();
     }
     CK(cudaMemsetAsync(h->status.p, 0, 4, h->stream));
-    CK(cudaEventRecord(h->ev[1], h->stream));
+    CK(cudaEventRecord(h->timing.ev[1], h->stream));
     GemmArgs a;
     // L_row = K[b, 0:N1] P11^T -> W[b, 0:N1]: split-K partial tiles into the free tiles W(c, j), then a fixed-order sum
     memset(&a, 0, sizeof(a));
     a.A = K; a.lda = NP; a.B = P; a.ldb = NP; a.C = W; a.ldc = NP;
     a.alpha = 1.0; a.beta = 0; a.job_mode = JOBS_TABLE;
-    a.jobs = ptr<GemmJob>(h->jobs) + h->app_row2_r.off;
-    if ((rc = launch_gemm<EPI_STORE>(h, h->mapK, h->mapP, a, h->app_row2_r.cnt))) return rc;
+    a.jobs = ptr<GemmJob>(h->jobs) + h->ranges.app_row2.off;
+    if ((rc = launch_gemm<EPI_STORE>(h, h->mapK, h->mapP, a, h->ranges.app_row2.cnt))) return rc;
     gpk_append_reduce_kernel<<<dim3(b, 64), 256, 0, h->stream>>>(W, NP, b, 0, W + (long)N1 * NP, NP, nullptr, 0, 0);
     CKL();
     // partial Gram tiles, then the Schur complement of the last block
     memset(&a, 0, sizeof(a));
     a.A = W; a.lda = NP; a.B = W; a.ldb = NP; a.C = W; a.ldc = NP;
     a.alpha = 1.0; a.beta = 0; a.job_mode = JOBS_TABLE;
-    a.jobs = ptr<GemmJob>(h->jobs) + h->app_syrk_r.off;
-    if ((rc = launch_gemm<EPI_STORE>(h, h->mapW, h->mapW, a, h->app_syrk_r.cnt))) return rc;
+    a.jobs = ptr<GemmJob>(h->jobs) + h->ranges.app_syrk.off;
+    if ((rc = launch_gemm<EPI_STORE>(h, h->mapW, h->mapW, a, h->ranges.app_syrk.cnt))) return rc;
     gpk_append_schur_kernel<<<64, 256, 0, h->stream>>>(K, W, NP, N1, b);
     CKL();
     // L_row to its final place (rows N1.. of K, columns 0..N1)
@@ -2074,16 +2073,16 @@ int gpk_fit_append(gpk_handle* h, const double* X, const double* y, int n, int d
     memset(&a, 0, sizeof(a));
     a.A = K; a.lda = NP; a.B = Q; a.ldb = NP; a.C = W; a.ldc = NP;
     a.alpha = 1.0; a.beta = 0; a.job_mode = JOBS_TABLE; a.status = ptr<int>(h->status);
-    a.jobs = ptr<GemmJob>(h->jobs) + h->app_t2_r.off;
-    if ((rc = launch_gemm<EPI_STORE>(h, h->mapK, h->mapQ, a, h->app_t2_r.cnt))) return rc;
+    a.jobs = ptr<GemmJob>(h->jobs) + h->ranges.app_t2.off;
+    if ((rc = launch_gemm<EPI_STORE>(h, h->mapK, h->mapQ, a, h->ranges.app_t2.cnt))) return rc;
     gpk_append_reduce_kernel<<<dim3(b, 64), 256, 0, h->stream>>>(W, NP, b, 1, P + (long)N1 * NP, NP, Q, NP, N1);
     CKL();
     // P[b, 0:N1] = -P_bb T (and its transpose into Q)
     memset(&a, 0, sizeof(a));
     a.A = P; a.lda = NP; a.B = Q; a.ldb = NP; a.C = P; a.ldc = NP; a.Ct = Q; a.ldct = NP;
     a.alpha = -1.0; a.beta = 0; a.job_mode = JOBS_TABLE; a.status = ptr<int>(h->status);
-    a.jobs = ptr<GemmJob>(h->jobs) + h->app_p_r.off;
-    if ((rc = launch_gemm<EPI_STORE>(h, h->mapP, h->mapQ, a, h->app_p_r.cnt))) return rc;
+    a.jobs = ptr<GemmJob>(h->jobs) + h->ranges.app_p.off;
+    if ((rc = launch_gemm<EPI_STORE>(h, h->mapP, h->mapQ, a, h->ranges.app_p.cnt))) return rc;
     // z = P (y - mean) into row NP of K, then z^T z and the log-determinant
     gpk_resid_kernel<<<(unsigned)((NP + 255) / 256), 256, 0, h->stream>>>(ptr<double>(h->y), mean, n, (int)NP,
                                                                           ptr<double>(h->tmp1));
@@ -2091,15 +2090,15 @@ int gpk_fit_append(gpk_handle* h, const double* X, const double* y, int n, int d
     gpk_rowdot_kernel<<<(unsigned)((NP + 7) / 8), 256, 0, h->stream>>>(P, NP, NP, (int)NP, 0, ptr<double>(h->tmp1),
                                                                        K + NP * NP);
     CKL();
-    CK(cudaEventRecord(h->ev[2], h->stream));
+    CK(cudaEventRecord(h->timing.ev[2], h->stream));
     gpk_fit_reduce_kernel<<<1, 256, 0, h->stream>>>(K + NP * NP, n, ptr<double>(h->logdet_part), nb, ptr<double>(h->scal));
     CKL();
-    CK(cudaEventRecord(h->ev[3], h->stream));
+    CK(cudaEventRecord(h->timing.ev[3], h->stream));
     CK(cudaMemcpyAsync(h->pin, h->scal.p, 16, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaMemcpyAsync(h->pin + 2, h->status.p, 4, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
-    h->launches_total += 12;
-    h->fit_timed = true;
+    h->timing.launches_total += 12;
+    h->timing.fit_timed = true;
     int st = 0;
     memcpy(&st, h->pin + 2, 4);
     if (st != 0) {                      // the block row of K / P is half updated: the model has to be refitted
@@ -2172,11 +2171,7 @@ struct HostFeeder : Feeder {
         while (next < hi && next < rows) {
             const int i = npieces;
             const long mc = std::min(piece, rows - next);
-            while ((int)h->ev_copied.size() <= i) {
-                cudaEvent_t e1;
-                CK(cudaEventCreateWithFlags(&e1, cudaEventDisableTiming));
-                h->ev_copied.push_back(e1);
-            }
+            if (int rc = grow_events(h, h->ev_copied, i + 1, cudaEventDisableTiming)) return rc;
             const double* src = Xs + next * d;
             if (staged) {
                 if (i >= 2) CK(cudaEventSynchronize(h->ev_copied[i - 2]));   // the DMA out of this staging buffer is done
@@ -2208,7 +2203,7 @@ int gpk_acq(gpk_handle* h, const double* Xs, long m, int kind, double eta, doubl
     if (out && (rc = ensure(h, h->out_acq, (size_t)m * 8))) return rc;
     if (mu && (rc = ensure(h, h->out_mu, (size_t)m * 8))) return rc;
     if (var && (rc = ensure(h, h->out_var, (size_t)m * 8))) return rc;
-    CK(cudaEventRecord(h->ev[14], h->stream));
+    CK(cudaEventRecord(h->timing.ev[14], h->stream));
     const long piece = std::min<long>(chunk_rows(h), round_up(m, BM));       // one H2D piece per scoring chunk
     const bool small = (size_t)m * d * 8 <= ((size_t)1 << 20);
     const bool staged = !small && !host_is_pinned(Xs);
@@ -2240,7 +2235,7 @@ int gpk_acq(gpk_handle* h, const double* Xs, long m, int kind, double eta, doubl
     unsigned long long nn = 0;
     CK(cudaMemcpyAsync(&bp, h->best.p, sizeof(bp), cudaMemcpyDeviceToHost, h->stream));
     CK(cudaMemcpyAsync(&nn, h->nneg.p, 8, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaEventRecord(h->ev[15], h->stream));
+    CK(cudaEventRecord(h->timing.ev[15], h->stream));
     CK(cudaStreamSynchronize(h->stream));
     if (best_val) *best_val = bp.val;
     if (best_idx) *best_idx = (long)bp.idx;
@@ -2570,7 +2565,7 @@ int gpk_set_hyper_model(gpk_handle* h, int n_params, const int* amp_slot, const 
     if (!h) return GPK_BAD_ARG;
     const char* who = "gpk_set_hyper_model";
     if (gp_refusal(h)) BAD("%s: %s", who, gp_refusal(h));
-    h->has_hyper = false;
+    h->hyper.has_model = false;
     if (!h->has_spec) BAD("%s: gpk_set_kernel has not been called", who);
     if (n_params < 1 || n_params + 1 > GPK_HYPER_MAX_DIM || !amp_slot || !term_param)
         BAD("%s: need 1 <= n_params <= %d and the slot table", who, GPK_HYPER_MAX_DIM - 1);
@@ -2627,8 +2622,8 @@ int gpk_set_hyper_model(gpk_handle* h, int n_params, const int* amp_slot, const 
         m.ln_sigma = prior_par[0]; m.ln_loc = prior_par[1]; m.th_lo = prior_par[2]; m.th_hi = prior_par[3];
         m.hs_scale = prior_par[4]; m.nrm_sigma = prior_par[5]; m.nrm_mean = prior_par[6];
     }
-    h->hyper = m;
-    h->has_hyper = true;
+    h->hyper.model = m;
+    h->hyper.has_model = true;
     return GPK_OK;
 }
 
@@ -2638,8 +2633,8 @@ namespace {
 int hyper_check(gpk_handle* h, int dim, const char* who, bool blocked) {
     int rc = require(h, true, true, false);
     if (rc) return rc;
-    if (!h->has_hyper) BAD("%s: gpk_set_hyper_model has not been called", who);
-    const HyperModel& m = h->hyper;
+    if (!h->hyper.has_model) BAD("%s: gpk_set_hyper_model has not been called", who);
+    const HyperModel& m = h->hyper.model;
     const KFactor& f = h->spec.factor;
     if (m.f_kind != f.kind || m.f_axis != f.axis || m.f_n_tasks != f.n_tasks)
         BAD("%s: the kernel structure changed since gpk_set_hyper_model", who);
@@ -2678,13 +2673,13 @@ int gpk_hyper_lnpost(gpk_handle* h, const double* theta, int count, int dim, dou
     int rc = hyper_ready(h, dim, who);
     if (rc) return rc;
     const size_t nT = (size_t)count * dim;
-    if ((rc = ensure(h, h->hy_buf, (nT + 2 * (size_t)count) * 8))) return rc;
-    double* dT = ptr<double>(h->hy_buf);
+    if ((rc = ensure(h, h->hyper.buf, (nT + 2 * (size_t)count) * 8))) return rc;
+    double* dT = ptr<double>(h->hyper.buf);
     double* dll = dT + nT;
     double* dlp = dll + count;
     CK(cudaMemcpyAsync(dT, theta, nT * 8, cudaMemcpyHostToDevice, h->stream));
     gpk_hy_eval_kernel<<<count, GPK_HY_THREADS, gpk_hy_smem_doubles(h->n) * 8, h->stream>>>(
-        h->hyper, ptr<double>(h->Xt), h->NP, ptr<double>(h->y), h->n, dT, dll, dlp, nullptr);
+        h->hyper.model, ptr<double>(h->Xt), h->NP, ptr<double>(h->y), h->n, dT, dll, dlp, nullptr);
     CKL();
     CK(cudaMemcpyAsync(ll, dll, (size_t)count * 8, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaMemcpyAsync(lp, dlp, (size_t)count * 8, cudaMemcpyDeviceToHost, h->stream));
@@ -2705,7 +2700,7 @@ int hy_args(gpk_handle* h, const char* who, const double* p0, int nwalkers, int 
 }
 
 // One EnsembleSampler.run_mcmc on the device, shared by both samplers: P (nwalkers x dim), L (nwalkers) and the accept
-// counts (nwalkers) contiguous in h->hy_buf, so that one copy brings the run back, then `extra` doubles for the caller.
+// counts (nwalkers) contiguous in h->hyper.buf, so that one copy brings the run back, then `extra` doubles for the caller.
 // score(P, L, extra) enqueues the initial log-posteriors, half(s, half, P, L, acc, extra) one half-step; no host
 // synchronisation until the final copy.
 template <class Score, class Half>
@@ -2714,9 +2709,9 @@ int hy_run(gpk_handle* h, const double* p0, int nwalkers, int dim, int steps, si
     static_assert(sizeof(long) == sizeof(long long) && sizeof(long long) == sizeof(double),
                   "the accept counts travel in the walkers' transfer");
     const size_t nP = (size_t)nwalkers * dim, total = nP + 2 * (size_t)nwalkers;
-    int rc = ensure(h, h->hy_buf, (total + extra) * 8);
+    int rc = ensure(h, h->hyper.buf, (total + extra) * 8);
     if (rc) return rc;
-    double* P = ptr<double>(h->hy_buf);
+    double* P = ptr<double>(h->hyper.buf);
     double* L = P + nP;
     long long* acc = (long long*)(L + nwalkers);
     double* ex = P + total;
@@ -2750,7 +2745,7 @@ int ho_args(gpk_handle* h, const char* who, const double* p0, const double* thet
 }
 
 // One L-BFGS-B run on the device, shared by both optimisers: the state record, the work buffer and `extra` doubles for
-// the caller in h->hy_buf; round(dst, work, q, extra) enqueues one round; the host reads the status once per
+// the caller in h->hyper.buf; round(dst, work, q, extra) enqueues one round; the host reads the status once per
 // GPK_HO_CHUNK rounds.
 template <class Round>
 int ho_run(gpk_handle* h, const double* p0, int dim, int maxcor, int maxiter, long maxfun, double ftol, double pgtol,
@@ -2758,10 +2753,10 @@ int ho_run(gpk_handle* h, const double* p0, int dim, int maxcor, int maxiter, lo
            int* status) {
     // the state record, then the work buffer
     const size_t nst = (sizeof(HOState) + 7) / 8, nw = (size_t)gpk_ho_work_doubles(dim, maxcor);
-    int rc = ensure(h, h->hy_buf, (nst + nw + extra) * 8);
+    int rc = ensure(h, h->hyper.buf, (nst + nw + extra) * 8);
     if (rc) return rc;
-    HOState* dst = ptr<HOState>(h->hy_buf);
-    double* work = ptr<double>(h->hy_buf) + nst;
+    HOState* dst = ptr<HOState>(h->hyper.buf);
+    double* work = ptr<double>(h->hyper.buf) + nst;
     const HOWork w = gpk_ho_work(work, dim, maxcor);
     HOState s0;
     memset(&s0, 0, sizeof(s0));
@@ -2805,13 +2800,13 @@ int gpk_sample_hypers(gpk_handle* h, const double* p0, int nwalkers, int dim, in
     const double* Xt = ptr<double>(h->Xt);
     const double* y = ptr<double>(h->y);
     auto score = [&](double* P, double* L, double*) -> int {
-        gpk_hy_eval_kernel<<<nwalkers, GPK_HY_THREADS, smem, h->stream>>>(h->hyper, Xt, h->NP, y, h->n, P, nullptr,
+        gpk_hy_eval_kernel<<<nwalkers, GPK_HY_THREADS, smem, h->stream>>>(h->hyper.model, Xt, h->NP, y, h->n, P, nullptr,
                                                                           nullptr, L);
         CKL();
         return GPK_OK;
     };
     auto half = [&](int s, int hf, double* P, double* L, long long* acc, double*) -> int {
-        gpk_hy_step_kernel<<<nwalkers / 2, GPK_HY_THREADS, smem, h->stream>>>(h->hyper, Xt, h->NP, y, h->n, nwalkers,
+        gpk_hy_step_kernel<<<nwalkers / 2, GPK_HY_THREADS, smem, h->stream>>>(h->hyper.model, Xt, h->NP, y, h->n, nwalkers,
                                                                             s, hf, seed, P, L, acc);
         CKL();
         return GPK_OK;
@@ -2833,7 +2828,7 @@ int gpk_optimize_hypers(gpk_handle* h, const double* p0, int dim, int maxcor, in
     const double* Xt = ptr<double>(h->Xt);
     const double* y = ptr<double>(h->y);
     auto round = [&](HOState* dst, double* work, const HOParams& q, double*) -> int {
-        gpk_ho_round_kernel<<<dim + 1, GPK_HY_THREADS, smem, h->stream>>>(h->hyper, Xt, h->NP, y, h->n, q, work, dst);
+        gpk_ho_round_kernel<<<dim + 1, GPK_HY_THREADS, smem, h->stream>>>(h->hyper.model, Xt, h->NP, y, h->n, q, work, dst);
         CKL();
         return GPK_OK;
     };
@@ -2845,9 +2840,12 @@ int gpk_optimize_hypers(gpk_handle* h, const double* p0, int dim, int maxcor, in
 // kernel and tile engine with job tables that span the chunk
 // ---------------------------------------------------------------------------------------
 namespace {
-// HBM layout of one chunk of B thetas in h->hb_buf: B matrices (one stacked array, tensor map mapA), B P strips
-// (mapP), B HBPar, B x nb block log-sums, B status words and the chunk's skip word
+// One chunk of B thetas, in HBM in buf: B matrices (one stacked array, tensor map mapA), B P strips (mapP), B HBPar,
+// B x nb block log-sums, B status words, the chunk's skip word and the job tables.  Each blocked call holds its own, so
+// the buffer (it can take most of the budget) is released before the call returns, whatever its outcome.
 struct HBChunk {
+    DevBuf buf;
+    GemmJob* jobs = nullptr;
     int B = 0;
     double* A = nullptr;
     double* P = nullptr;
@@ -2866,10 +2864,10 @@ int hb_reserve(gpk_handle* h, int count, const char* who, HBChunk* c) {
     const int n = h->n, nb = gpk_hb_nb(n);
     const long NP = (long)nb * HB_T, R = NP + HB_T;
     const long per = gpk_hb_theta_bytes(n);
-    const long fit = h->hyper_batch_bytes / per;
+    const long fit = h->hyper.batch_bytes / per;
     if (fit < 1)
         BAD("%s: one theta needs %ld bytes at n = %d, more than hyper_batch_bytes = %ld", who, per, n,
-            h->hyper_batch_bytes);
+            h->hyper.batch_bytes);
     c->B = (int)std::min<long>(std::min<long>(fit, count), 32768);
     const int B = c->B;
     const size_t nA = (size_t)B * R * NP, nPs = (size_t)B * HB_T * NP, npar = (size_t)B * ((sizeof(HBPar) + 7) / 8);
@@ -2897,31 +2895,22 @@ int hb_reserve(gpk_handle* h, int count, const char* who, HBChunk* c) {
         }
     }
     const size_t njob = (jobs.size() * sizeof(GemmJob) + 7) / 8;
-    int rc = ensure(h, h->hb_buf, (nA + nPs + npar + nlog + nst + njob) * 8);
+    int rc = ensure(h, c->buf, (nA + nPs + npar + nlog + nst + njob) * 8);
     if (rc) return rc;
-    c->A = ptr<double>(h->hb_buf);
+    c->A = ptr<double>(c->buf);
     c->P = c->A + nA;
     c->par = reinterpret_cast<HBPar*>(c->P + nPs);
     c->logpart = c->P + nPs + npar;
     c->st = reinterpret_cast<int*>(c->logpart + nlog);
     c->skip = c->st + B;
-    GemmJob* djobs = reinterpret_cast<GemmJob*>(c->logpart + nlog + nst);
+    c->jobs = reinterpret_cast<GemmJob*>(c->logpart + nlog + nst);
     if (!jobs.empty())
-        CK(cudaMemcpyAsync(djobs, jobs.data(), jobs.size() * sizeof(GemmJob), cudaMemcpyHostToDevice, h->stream));
+        CK(cudaMemcpyAsync(c->jobs, jobs.data(), jobs.size() * sizeof(GemmJob), cudaMemcpyHostToDevice, h->stream));
     CK(cudaMemsetAsync(c->skip, 0, sizeof(int), h->stream));
     CK(cudaStreamSynchronize(h->stream));         // the host job vector goes out of scope
-    h->hb_jobs = djobs;
     if ((rc = make_map(h, &c->mapA, c->A, (long)B * R, NP, NP))) return rc;
     if ((rc = make_map(h, &c->mapP, c->P, (long)B * HB_T, NP, NP))) return rc;
     return GPK_OK;
-}
-
-// the chunk buffer goes back at the end of every blocked call, whatever its outcome (it can take most of the budget)
-void hb_release(gpk_handle* h) {
-    if (h->hb_buf.p) cudaFree(h->hb_buf.p);
-    h->hb_buf.p = nullptr;
-    h->hb_buf.cap = 0;
-    h->hb_jobs = nullptr;
 }
 
 // The log-posterior parts of the count thetas T (device, count x dim) in chunks of c.B, enqueued on the handle's stream
@@ -2929,7 +2918,7 @@ void hb_release(gpk_handle* h) {
 // the chunk's own zero word): non-zero makes every launch return at once.
 int hb_score(gpk_handle* h, const HBChunk& c, const double* T, int count, const int* skip, double* ll, double* lp,
              double* post, double* fobj) {
-    const int n = h->n, nb = gpk_hb_nb(n), D = h->hyper.n_params + 1;
+    const int n = h->n, nb = gpk_hb_nb(n), D = h->hyper.model.n_params + 1;
     const long NP = (long)nb * HB_T, R = NP + HB_T;
     if (!skip) skip = c.skip;
     auto at = [](double* p, int off) { return p ? p + off : nullptr; };
@@ -2938,9 +2927,9 @@ int hb_score(gpk_handle* h, const HBChunk& c, const double* T, int count, const 
         const int B = std::min(c.B, count - c0);
         // the P strips: zero right of the diagonal 16-blocks, where the diagonal kernel never stores
         CK(cudaMemsetAsync(c.P, 0, (size_t)B * HB_T * NP * 8, h->stream));
-        gpk_hb_prep_kernel<<<B, 32, 0, h->stream>>>(h->hyper, T + (size_t)c0 * D, skip, c.par, c.st);
+        gpk_hb_prep_kernel<<<B, 32, 0, h->stream>>>(h->hyper.model, T + (size_t)c0 * D, skip, c.par, c.st);
         CKL();
-        gpk_hb_build_kernel<<<dim3(nb, nb + 1, B), 256, 0, h->stream>>>(h->hyper, ptr<double>(h->Xt), h->NP,
+        gpk_hb_build_kernel<<<dim3(nb, nb + 1, B), 256, 0, h->stream>>>(h->hyper.model, ptr<double>(h->Xt), h->NP,
                                                                         ptr<double>(h->y), n, c.par, c.A);
         CKL();
         for (int k = 0; k < nb; ++k) {
@@ -2962,23 +2951,25 @@ int hb_score(gpk_handle* h, const HBChunk& c, const double* T, int count, const 
             a.alpha = 1.0; a.beta = 0;
             a.job_mode = JOBS_TABLE;
             a.status = skip;
-            a.jobs = h->hb_jobs + c.panel_r[k].off;
+            a.jobs = c.jobs + c.panel_r[k].off;
             if ((rc = launch_gemm<EPI_STORE>(h, c.mapA, c.mapP, a, B * c.panel_r[k].cnt))) return rc;
             if (c.update_r[k].cnt > 0) {
                 a.B = c.A;
                 a.alpha = -1.0; a.beta = 1;
-                a.jobs = h->hb_jobs + c.update_r[k].off;
+                a.jobs = c.jobs + c.update_r[k].off;
                 if ((rc = launch_gemm<EPI_STORE>(h, c.mapA, c.mapA, a, B * c.update_r[k].cnt))) return rc;
             }
         }
-        gpk_hb_finish_kernel<<<B, GPK_HY_THREADS, 0, h->stream>>>(h->hyper, n, c.par, c.A, c.logpart, c.st, at(ll, c0),
+        gpk_hb_finish_kernel<<<B, GPK_HY_THREADS, 0, h->stream>>>(h->hyper.model, n, c.par, c.A, c.logpart, c.st, at(ll, c0),
                                                                   at(lp, c0), at(post, c0), at(fobj, c0));
         CKL();
     }
     return GPK_OK;
 }
+}  // namespace
 
-int hyper_lnpost_blocked(gpk_handle* h, const double* theta, int count, int dim, double* ll, double* lp) {
+int gpk_hyper_lnpost_blocked(gpk_handle* h, const double* theta, int count, int dim, double* ll, double* lp) {
+    if (!h) return GPK_BAD_ARG;
     const char* who = "gpk_hyper_lnpost_blocked";
     if (count < 1 || !theta || !ll || !lp) BAD("%s: need count >= 1, theta, ll and lp", who);
     int rc = hyper_check(h, dim, who, true);
@@ -2986,8 +2977,8 @@ int hyper_lnpost_blocked(gpk_handle* h, const double* theta, int count, int dim,
     HBChunk c;
     if ((rc = hb_reserve(h, count, who, &c))) return rc;
     const size_t nT = (size_t)count * dim;
-    if ((rc = ensure(h, h->hy_buf, (nT + 2 * (size_t)count) * 8))) return rc;
-    double* dT = ptr<double>(h->hy_buf);
+    if ((rc = ensure(h, h->hyper.buf, (nT + 2 * (size_t)count) * 8))) return rc;
+    double* dT = ptr<double>(h->hyper.buf);
     double* dll = dT + nT;
     double* dlp = dll + count;
     CK(cudaMemcpyAsync(dT, theta, nT * 8, cudaMemcpyHostToDevice, h->stream));
@@ -2998,8 +2989,9 @@ int hyper_lnpost_blocked(gpk_handle* h, const double* theta, int count, int dim,
     return GPK_OK;
 }
 
-int sample_hypers_blocked(gpk_handle* h, const double* p0, int nwalkers, int dim, int steps, unsigned long long seed,
-                          double* pos, double* lnpost, long* n_accepted) {
+int gpk_sample_hypers_blocked(gpk_handle* h, const double* p0, int nwalkers, int dim, int steps, unsigned long long seed,
+                              double* pos, double* lnpost, long* n_accepted) {
+    if (!h) return GPK_BAD_ARG;
     const char* who = "gpk_sample_hypers_blocked";
     int rc = hy_args(h, who, p0, nwalkers, dim, steps, pos, lnpost);
     if (rc) return rc;
@@ -3024,9 +3016,10 @@ int sample_hypers_blocked(gpk_handle* h, const double* p0, int nwalkers, int dim
     return hy_run(h, p0, nwalkers, dim, steps, (size_t)hb * dim + hb, score, half, pos, lnpost, n_accepted);
 }
 
-int optimize_hypers_blocked(gpk_handle* h, const double* p0, int dim, int maxcor, int maxiter, long maxfun, double ftol,
-                            double pgtol, double eps, int maxls, double* theta, double* f, int* nit, long* nfev,
-                            int* status) {
+int gpk_optimize_hypers_blocked(gpk_handle* h, const double* p0, int dim, int maxcor, int maxiter, long maxfun,
+                                double ftol, double pgtol, double eps, int maxls, double* theta, double* f, int* nit,
+                                long* nfev, int* status) {
+    if (!h) return GPK_BAD_ARG;
     const char* who = "gpk_optimize_hypers_blocked";
     int rc = ho_args(h, who, p0, theta, dim, maxcor, maxiter, maxfun, eps, maxls);
     if (rc) return rc;
@@ -3047,32 +3040,6 @@ int optimize_hypers_blocked(gpk_handle* h, const double* p0, int dim, int maxcor
     return ho_run(h, p0, dim, maxcor, maxiter, maxfun, ftol, pgtol, eps, maxls, (size_t)(dim + 1) * dim, round, theta,
                   f, nit, nfev, status);
 }
-}  // namespace
-
-int gpk_hyper_lnpost_blocked(gpk_handle* h, const double* theta, int count, int dim, double* ll, double* lp) {
-    if (!h) return GPK_BAD_ARG;
-    const int rc = hyper_lnpost_blocked(h, theta, count, dim, ll, lp);
-    hb_release(h);
-    return rc;
-}
-
-int gpk_sample_hypers_blocked(gpk_handle* h, const double* p0, int nwalkers, int dim, int steps, unsigned long long seed,
-                              double* pos, double* lnpost, long* n_accepted) {
-    if (!h) return GPK_BAD_ARG;
-    const int rc = sample_hypers_blocked(h, p0, nwalkers, dim, steps, seed, pos, lnpost, n_accepted);
-    hb_release(h);
-    return rc;
-}
-
-int gpk_optimize_hypers_blocked(gpk_handle* h, const double* p0, int dim, int maxcor, int maxiter, long maxfun,
-                                double ftol, double pgtol, double eps, int maxls, double* theta, double* f, int* nit,
-                                long* nfev, int* status) {
-    if (!h) return GPK_BAD_ARG;
-    const int rc = optimize_hypers_blocked(h, p0, dim, maxcor, maxiter, maxfun, ftol, pgtol, eps, maxls, theta, f, nit,
-                                           nfev, status);
-    hb_release(h);
-    return rc;
-}
 
 // ---------------------------------------------------------------------------------------
 // Bayesian linear regression (gpk_blr.cuh; robo/models/bayesian_linear_regression.py)
@@ -3089,10 +3056,10 @@ int gpk_blr_set_data(gpk_handle* h, const double* X, const double* y, int n, int
         BAD("%s: %ld features (d = %d) exceed GPK_BLR_MAX_F = %d", who, F, d, GPK_BLR_MAX_F);
     CK(cudaSetDevice(h->device));
     h->model = MODEL_BLR;
-    h->blr_fitted = false;
-    h->n = n; h->d = d; h->blr_F = (int)F; h->blr_basis = basis;
-    h->blr_prior.ln_sigma = prior_par[0]; h->blr_prior.ln_loc = prior_par[1]; h->blr_prior.hs_scale = prior_par[2];
-    if ((rc = ensure(h, h->blr_data, ((size_t)n * F + n + F * F + F) * 8))) return rc;
+    h->blr.fitted = false;
+    h->n = n; h->d = d; h->blr.F = (int)F; h->blr.basis = basis;
+    h->blr.prior.ln_sigma = prior_par[0]; h->blr.prior.ln_loc = prior_par[1]; h->blr.prior.hs_scale = prior_par[2];
+    if ((rc = ensure(h, h->blr.data, ((size_t)n * F + n + F * F + F) * 8))) return rc;
     if ((rc = ensure(h, h->cand, (size_t)n * d * 8))) return rc;
     CK(cudaMemcpyAsync(h->cand.p, X, (size_t)n * d * 8, cudaMemcpyHostToDevice, h->stream));
     CK(cudaMemcpyAsync(blr_y(h), y, (size_t)n * 8, cudaMemcpyHostToDevice, h->stream));
@@ -3110,12 +3077,12 @@ int gpk_blr_lnpost(gpk_handle* h, const double* thetas, int count, double* out) 
     int rc = blr_ready(h, who);
     if (rc) return rc;
     if (count < 1 || !thetas || !out) BAD("%s: need count >= 1, thetas and out", who);
-    if ((rc = ensure(h, h->blr_work, (size_t)count * 3 * 8))) return rc;
-    double* dT = ptr<double>(h->blr_work);
+    if ((rc = ensure(h, h->blr.work, (size_t)count * 3 * 8))) return rc;
+    double* dT = ptr<double>(h->blr.work);
     double* dv = dT + 2 * (size_t)count;
     CK(cudaMemcpyAsync(dT, thetas, (size_t)count * 2 * 8, cudaMemcpyHostToDevice, h->stream));
-    gpk_blr_eval_kernel<<<count, GPK_BLR_THREADS, gpk_blr_smem_doubles(h->blr_F) * 8, h->stream>>>(
-        blr_phi(h), blr_y(h), blr_G(h), blr_b(h), h->n, h->blr_F, h->blr_prior, dT, dv);
+    gpk_blr_eval_kernel<<<count, GPK_BLR_THREADS, gpk_blr_smem_doubles(h->blr.F) * 8, h->stream>>>(
+        blr_phi(h), blr_y(h), blr_G(h), blr_b(h), h->n, h->blr.F, h->blr.prior, dT, dv);
     CKL();
     CK(cudaMemcpyAsync(out, dv, (size_t)count * 8, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
@@ -3135,20 +3102,20 @@ int gpk_blr_sample(gpk_handle* h, unsigned long long seed, int nwalkers, const d
     if (steps < 0) BAD("%s: need steps >= 0", who);
     // P (nwalkers x 2), L (nwalkers), accept counts (nwalkers): contiguous, so that one copy brings the run back
     const size_t nP = 2 * (size_t)nwalkers, total = nP + 2 * (size_t)nwalkers;
-    if ((rc = ensure(h, h->blr_work, total * 8))) return rc;
-    double* P = ptr<double>(h->blr_work);
+    if ((rc = ensure(h, h->blr.work, total * 8))) return rc;
+    double* P = ptr<double>(h->blr.work);
     double* L = P + nP;
     long long* acc = (long long*)(L + nwalkers);
-    const size_t smem = gpk_blr_smem_doubles(h->blr_F) * 8;
+    const size_t smem = gpk_blr_smem_doubles(h->blr.F) * 8;
     CK(cudaMemcpyAsync(P, p0, nP * 8, cudaMemcpyHostToDevice, h->stream));
     CK(cudaMemsetAsync(acc, 0, (size_t)nwalkers * 8, h->stream));
     gpk_blr_eval_kernel<<<nwalkers, GPK_BLR_THREADS, smem, h->stream>>>(blr_phi(h), blr_y(h), blr_G(h), blr_b(h), h->n,
-                                                                       h->blr_F, h->blr_prior, P, L);
+                                                                       h->blr.F, h->blr.prior, P, L);
     CKL();
     for (int s = 0; s < steps; ++s)
         for (int half = 0; half < 2; ++half) {
             gpk_blr_step_kernel<<<nwalkers / 2, GPK_BLR_THREADS, smem, h->stream>>>(
-                blr_phi(h), blr_y(h), blr_G(h), blr_b(h), h->n, h->blr_F, h->blr_prior, nwalkers, s, half, seed, P, L, acc);
+                blr_phi(h), blr_y(h), blr_G(h), blr_b(h), h->n, h->blr.F, h->blr.prior, nwalkers, s, half, seed, P, L, acc);
             CKL();
         }
     std::vector<double> out(total);
@@ -3167,13 +3134,13 @@ namespace {
 int blr_fit(gpk_handle* h, const double* hypers, int k, const char* who) {
     int rc;
     if (!hypers || k < 1) BAD("%s: need hypers and k >= 1", who);
-    h->blr_fitted = false;
-    const int F = h->blr_F;
+    h->blr.fitted = false;
+    const int F = h->blr.F;
     const BlrPost L(k, F);
-    if ((rc = ensure(h, h->blr_post, L.total))) return rc;
-    if ((rc = ensure(h, h->blr_work, (size_t)k * 2 * 8))) return rc;
-    double* post = ptr<double>(h->blr_post);
-    double* dH = ptr<double>(h->blr_work);
+    if ((rc = ensure(h, h->blr.post, L.total))) return rc;
+    if ((rc = ensure(h, h->blr.work, (size_t)k * 2 * 8))) return rc;
+    double* post = ptr<double>(h->blr.post);
+    double* dH = ptr<double>(h->blr.work);
     CK(cudaMemcpyAsync(dH, hypers, (size_t)k * 2 * 8, cudaMemcpyHostToDevice, h->stream));
     gpk_blr_fit_kernel<<<k, GPK_BLR_THREADS, (gpk_blr_smem_doubles(F) + (size_t)F * F) * 8, h->stream>>>(
         blr_G(h), blr_b(h), F, dH, post + L.M, post + L.Li, post + L.S, post + L.ib, (int*)(post + L.fail));
@@ -3187,8 +3154,8 @@ int blr_fit(gpk_handle* h, const double* hypers, int k, const char* who) {
                     who, i, hypers[2 * i], hypers[2 * i + 1]);
             return GPK_NOT_PD;
         }
-    h->blr_k = k;
-    h->blr_fitted = true;
+    h->blr.k = k;
+    h->blr.fitted = true;
     return GPK_OK;
 }
 }  // namespace
@@ -3207,12 +3174,12 @@ int gpk_blr_get_models(gpk_handle* h, double* m, double* S) {
     const char* who = "gpk_blr_get_models";
     int rc = blr_ready(h, who);
     if (rc) return rc;
-    if (!h->blr_fitted) { set_err(h, "%s: %s", who, MODELS[MODEL_BLR].not_fitted); return GPK_NOT_FITTED; }
-    const BlrPost L(h->blr_k, h->blr_F);
-    const double* post = ptr<double>(h->blr_post);
-    if (m) CK(cudaMemcpyAsync(m, post + L.M, (size_t)h->blr_k * h->blr_F * 8, cudaMemcpyDeviceToHost, h->stream));
+    if (!h->blr.fitted) { set_err(h, "%s: %s", who, MODELS[MODEL_BLR].not_fitted); return GPK_NOT_FITTED; }
+    const BlrPost L(h->blr.k, h->blr.F);
+    const double* post = ptr<double>(h->blr.post);
+    if (m) CK(cudaMemcpyAsync(m, post + L.M, (size_t)h->blr.k * h->blr.F * 8, cudaMemcpyDeviceToHost, h->stream));
     if (S)
-        CK(cudaMemcpyAsync(S, post + L.S, (size_t)h->blr_k * h->blr_F * h->blr_F * 8, cudaMemcpyDeviceToHost, h->stream));
+        CK(cudaMemcpyAsync(S, post + L.S, (size_t)h->blr.k * h->blr.F * h->blr.F * 8, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
     return GPK_OK;
 }
@@ -3221,8 +3188,8 @@ int gpk_blr_dims(gpk_handle* h, int* n, int* F, int* k) {
     int rc = blr_ready(h, "gpk_blr_dims");
     if (rc) return rc;
     if (n) *n = h->n;
-    if (F) *F = h->blr_F;
-    if (k) *k = h->blr_fitted ? h->blr_k : 0;
+    if (F) *F = h->blr.F;
+    if (k) *k = h->blr.fitted ? h->blr.k : 0;
     return GPK_OK;
 }
 
@@ -3253,9 +3220,9 @@ int gpk_rf_set_data(gpk_handle* h, const double* X, const double* y, int n, int 
         });
     }
     h->model = MODEL_RF;
-    h->rf_fitted = false;
+    h->rf.fitted = false;
     h->n = n; h->d = d;
-    if ((rc = ensure(h, h->rf_data, ((size_t)n * d + n) * 8 + (size_t)d * n * 4))) return rc;
+    if ((rc = ensure(h, h->rf.data, ((size_t)n * d + n) * 8 + (size_t)d * n * 4))) return rc;
     CK(cudaMemcpyAsync(rf_X(h), X, (size_t)n * d * 8, cudaMemcpyHostToDevice, h->stream));
     CK(cudaMemcpyAsync(rf_y(h), y, (size_t)n * 8, cudaMemcpyHostToDevice, h->stream));
     CK(cudaMemcpyAsync(rf_order(h), order.data(), (size_t)d * n * 4, cudaMemcpyHostToDevice, h->stream));
@@ -3274,17 +3241,17 @@ int gpk_rf_fit(gpk_handle* h, unsigned long long seed, unsigned counter, int T, 
     const int nt = n_per_tree > 0 ? n_per_tree : n;
     if (!bootstrap && nt > n)
         BAD("%s: without bootstrapping a tree cannot take %d of %d points (n_points_per_tree <= n)", who, nt, n);
-    h->rf_fitted = false;
+    h->rf.fitted = false;
     const long S = 2L * n;
     const RfNodes L(T, S);
-    if ((rc = ensure(h, h->rf_nodes, L.total))) return rc;
+    if ((rc = ensure(h, h->rf.nodes, L.total))) return rc;
     // growth scratch per CTA: multiplicities (n), two list buffers (2 (d + 1) n) and the segments (3 x 2 n), ints;
     // trees are grown in batches that keep it near 512 MB
     const size_t per_tree = (size_t)n * (1 + 2 * (size_t)(d + 1) + 6) * 4;
     const int batch = (int)std::max<size_t>(1, std::min<size_t>((size_t)T, ((size_t)512 << 20) / per_tree));
-    if ((rc = ensure(h, h->rf_work, per_tree * batch))) return rc;
-    char* nodes = ptr<char>(h->rf_nodes);
-    int* work = ptr<int>(h->rf_work);
+    if ((rc = ensure(h, h->rf.work, per_tree * batch))) return rc;
+    char* nodes = ptr<char>(h->rf.nodes);
+    int* work = ptr<int>(h->rf.work);
     RfGrowArgs a;
     memset(&a, 0, sizeof(a));
     a.X = rf_X(h); a.y = rf_y(h); a.order = rf_order(h);
@@ -3302,9 +3269,9 @@ int gpk_rf_fit(gpk_handle* h, unsigned long long seed, unsigned counter, int T, 
         CKL();
     }
     CK(cudaStreamSynchronize(h->stream));
-    h->rf_T = T;
-    h->rf_total = total_variance ? 1 : 0;
-    h->rf_fitted = true;
+    h->rf.T = T;
+    h->rf.total = total_variance ? 1 : 0;
+    h->rf.fitted = true;
     return GPK_OK;
 }
 
@@ -3313,7 +3280,7 @@ int gpk_rf_dims(gpk_handle* h, int* n, int* d, int* T, int* slots) {
     if (rc) return rc;
     if (n) *n = h->n;
     if (d) *d = h->d;
-    if (T) *T = h->rf_fitted ? h->rf_T : 0;
+    if (T) *T = h->rf.fitted ? h->rf.T : 0;
     if (slots) *slots = 2 * h->n;
     return GPK_OK;
 }
@@ -3323,13 +3290,13 @@ int gpk_rf_get_trees(gpk_handle* h, int* n_nodes, int* feat, double* thr, int* l
     const char* who = "gpk_rf_get_trees";
     int rc = model_ready(h, MODEL_RF, who);
     if (rc) return rc;
-    if (!h->rf_fitted) { set_err(h, "%s: %s", who, MODELS[MODEL_RF].not_fitted); return GPK_NOT_FITTED; }
+    if (!h->rf.fitted) { set_err(h, "%s: %s", who, MODELS[MODEL_RF].not_fitted); return GPK_NOT_FITTED; }
     const long S = 2L * h->n;
-    const size_t TS = (size_t)h->rf_T * S;
-    const RfNodes L(h->rf_T, S);
-    const char* nodes = ptr<char>(h->rf_nodes);
+    const size_t TS = (size_t)h->rf.T * S;
+    const RfNodes L(h->rf.T, S);
+    const char* nodes = ptr<char>(h->rf.nodes);
     const struct { void* dst; size_t off, bytes; } parts[] = {
-        {n_nodes, L.nn, (size_t)h->rf_T * 4}, {feat, L.feat, TS * 4}, {thr, L.thr, TS * 8}, {left, L.left, TS * 4},
+        {n_nodes, L.nn, (size_t)h->rf.T * 4}, {feat, L.feat, TS * 4}, {thr, L.thr, TS * 8}, {left, L.left, TS * 4},
         {W, L.W, TS * 8}, {mean, L.mean, TS * 8}, {var, L.var, TS * 8}};
     for (const auto& p : parts)
         if (p.dst) CK(cudaMemcpyAsync(p.dst, nodes + p.off, p.bytes, cudaMemcpyDeviceToHost, h->stream));
@@ -3355,19 +3322,19 @@ int gpk_rf_set_trees(gpk_handle* h, int T, int total_variance, const int* n_node
                 BAD("%s: node %d of tree %d is not a valid split or leaf", who, v, t);
         }
     }
-    h->rf_fitted = false;
+    h->rf.fitted = false;
     const size_t TS = (size_t)T * S;
     const RfNodes L(T, S);
-    if ((rc = ensure(h, h->rf_nodes, L.total))) return rc;
-    char* nodes = ptr<char>(h->rf_nodes);
+    if ((rc = ensure(h, h->rf.nodes, L.total))) return rc;
+    char* nodes = ptr<char>(h->rf.nodes);
     const struct { const void* src; size_t off, bytes; } parts[] = {
         {n_nodes, L.nn, (size_t)T * 4}, {feat, L.feat, TS * 4}, {thr, L.thr, TS * 8}, {left, L.left, TS * 4},
         {W, L.W, TS * 8}, {mean, L.mean, TS * 8}, {var, L.var, TS * 8}};
     for (const auto& p : parts) CK(cudaMemcpyAsync(nodes + p.off, p.src, p.bytes, cudaMemcpyHostToDevice, h->stream));
     CK(cudaStreamSynchronize(h->stream));
-    h->rf_T = T;
-    h->rf_total = total_variance ? 1 : 0;
-    h->rf_fitted = true;
+    h->rf.T = T;
+    h->rf.total = total_variance ? 1 : 0;
+    h->rf.fitted = true;
     return GPK_OK;
 }
 
@@ -3444,11 +3411,11 @@ int gpk_bnn_set_data(gpk_handle* h, const double* X, const double* y, int n, int
     if ((rc = scale_set(h, who, X, y, n, d, true, true, buf, &ym, &ysd))) return rc;
     CK(cudaSetDevice(h->device));
     h->model = MODEL_BNN;
-    h->bnn_S = 0;
+    h->bnn.S = 0;
     h->n = n; h->d = d;
-    h->bnn_P = gpk_bnn_params(d);
-    h->bnn_ymean = ym; h->bnn_ystd = ysd;
-    if ((rc = ensure(h, h->bnn_data, buf.size() * 8))) return rc;
+    h->bnn.P = gpk_bnn_params(d);
+    h->bnn.ymean = ym; h->bnn.ystd = ysd;
+    if ((rc = ensure(h, h->bnn.data, buf.size() * 8))) return rc;
     CK(cudaMemcpyAsync(bnn_X(h), buf.data(), buf.size() * 8, cudaMemcpyHostToDevice, h->stream));
     CK(cudaStreamSynchronize(h->stream));     // the staging vector dies here
     return GPK_OK;
@@ -3467,10 +3434,10 @@ int gpk_bnn_train(gpk_handle* h, unsigned long long seed, unsigned counter, doub
     const long S = num_steps - 1 > burn_in ? (num_steps - 1 - burn_in) / keep_every : 0;
     if (S < 1) BAD("%s: the chain keeps no network (num_steps = %ld, burn_in = %ld, keep_every = %ld)", who, num_steps,
                    burn_in, keep_every);
-    const int P = h->bnn_P;
-    h->bnn_S = 0;
-    if ((rc = ensure(h, h->bnn_samples, (size_t)S * P * 8))) return rc;
-    if ((rc = ensure(h, h->bnn_state, (size_t)5 * P * 8))) return rc;
+    const int P = h->bnn.P;
+    h->bnn.S = 0;
+    if ((rc = ensure(h, h->bnn.samples, (size_t)S * P * 8))) return rc;
+    if ((rc = ensure(h, h->bnn.state, (size_t)5 * P * 8))) return rc;
     const size_t smem = (size_t)gpk_bnn_chain_smem(h->n, h->d, batch);
     CK(cudaFuncSetAttribute(gpk_bnn_chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     BnnChainArgs a;
@@ -3480,12 +3447,12 @@ int gpk_bnn_train(gpk_handle* h, unsigned long long seed, unsigned counter, doub
     a.seed = seed; a.counter = counter;
     a.lr = lr; a.mdecay = mdecay; a.eps = eps;
     a.burn_in = burn_in; a.num_steps = num_steps; a.keep_every = keep_every;
-    a.samples = ptr<double>(h->bnn_samples);
-    a.state = ptr<double>(h->bnn_state);
+    a.samples = ptr<double>(h->bnn.samples);
+    a.state = ptr<double>(h->bnn.state);
     gpk_bnn_chain_kernel<<<1, GPK_BNN_THREADS, smem, h->stream>>>(a);
     CKL();
     CK(cudaStreamSynchronize(h->stream));
-    h->bnn_S = (int)S;
+    h->bnn.S = (int)S;
     return GPK_OK;
 }
 
@@ -3494,8 +3461,8 @@ int gpk_bnn_dims(gpk_handle* h, int* n, int* d, int* P, int* S) {
     if (rc) return rc;
     if (n) *n = h->n;
     if (d) *d = h->d;
-    if (P) *P = h->bnn_P;
-    if (S) *S = h->bnn_S;
+    if (P) *P = h->bnn.P;
+    if (S) *S = h->bnn.S;
     return GPK_OK;
 }
 
@@ -3503,9 +3470,9 @@ int gpk_bnn_get_samples(gpk_handle* h, double* samples) {
     const char* who = "gpk_bnn_get_samples";
     int rc = model_ready(h, MODEL_BNN, who);
     if (rc) return rc;
-    if (h->bnn_S < 1) { set_err(h, "%s: %s", who, MODELS[MODEL_BNN].not_fitted); return GPK_NOT_FITTED; }
+    if (h->bnn.S < 1) { set_err(h, "%s: %s", who, MODELS[MODEL_BNN].not_fitted); return GPK_NOT_FITTED; }
     if (!samples) BAD("%s: need the output array", who);
-    CK(cudaMemcpyAsync(samples, h->bnn_samples.p, (size_t)h->bnn_S * h->bnn_P * 8, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaMemcpyAsync(samples, h->bnn.samples.p, (size_t)h->bnn.S * h->bnn.P * 8, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
     return GPK_OK;
 }
@@ -3515,11 +3482,11 @@ int gpk_bnn_set_samples(gpk_handle* h, int S, const double* samples) {
     int rc = model_ready(h, MODEL_BNN, who);
     if (rc) return rc;
     if (S < 1 || !samples) BAD("%s: need S >= 1 networks", who);
-    h->bnn_S = 0;
-    if ((rc = ensure(h, h->bnn_samples, (size_t)S * h->bnn_P * 8))) return rc;
-    CK(cudaMemcpyAsync(h->bnn_samples.p, samples, (size_t)S * h->bnn_P * 8, cudaMemcpyHostToDevice, h->stream));
+    h->bnn.S = 0;
+    if ((rc = ensure(h, h->bnn.samples, (size_t)S * h->bnn.P * 8))) return rc;
+    CK(cudaMemcpyAsync(h->bnn.samples.p, samples, (size_t)S * h->bnn.P * 8, cudaMemcpyHostToDevice, h->stream));
     CK(cudaStreamSynchronize(h->stream));
-    h->bnn_S = S;
+    h->bnn.S = S;
     return GPK_OK;
 }
 
@@ -3527,11 +3494,11 @@ int gpk_bnn_get_state(gpk_handle* h, double* theta, double* p, double* tau, doub
     const char* who = "gpk_bnn_get_state";
     int rc = model_ready(h, MODEL_BNN, who);
     if (rc) return rc;
-    if (h->bnn_S < 1 || !h->bnn_state.p) { set_err(h, "%s: no chain has run (gpk_bnn_train)", who); return GPK_NOT_FITTED; }
+    if (h->bnn.S < 1 || !h->bnn.state.p) { set_err(h, "%s: no chain has run (gpk_bnn_train)", who); return GPK_NOT_FITTED; }
     double* out[5] = {theta, p, tau, g, vhat};
-    const size_t P = h->bnn_P;
+    const size_t P = h->bnn.P;
     for (int i = 0; i < 5; ++i)
-        if (out[i]) CK(cudaMemcpyAsync(out[i], ptr<double>(h->bnn_state) + i * P, P * 8, cudaMemcpyDeviceToHost, h->stream));
+        if (out[i]) CK(cudaMemcpyAsync(out[i], ptr<double>(h->bnn.state) + i * P, P * 8, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
     return GPK_OK;
 }
@@ -3541,7 +3508,7 @@ int gpk_bnn_draws(gpk_handle* h, unsigned long long seed, unsigned counter, int 
     int rc = model_ready(h, MODEL_BNN, who);
     if (rc) return rc;
     if (ns < 1 || !Z) BAD("%s: need ns >= 1 and an output array", who);
-    const int P = h->bnn_P;
+    const int P = h->bnn.P;
     const size_t bytes = (size_t)ns * P * 8;
     if ((rc = ensure(h, h->tmp1, bytes))) return rc;
     const long threads = (long)ns * (P / 2);
@@ -3566,14 +3533,14 @@ int dngo_gram(gpk_handle* h) {
         blr_phi(h), blr_y(h), h->n, GPK_DNGO_H, blr_G(h), blr_b(h));
     CKL();
     CK(cudaStreamSynchronize(h->stream));
-    h->dngo_trained = true;
+    h->dngo.trained = true;
     return GPK_OK;
 }
 
 int dngo_trained(gpk_handle* h, const char* who) {
     int rc = model_ready(h, MODEL_DNGO, who);
     if (rc) return rc;
-    if (!h->dngo_trained) { set_err(h, "%s: model is not trained (gpk_dngo_train)", who); return GPK_NOT_FITTED; }
+    if (!h->dngo.trained) { set_err(h, "%s: model is not trained (gpk_dngo_train)", who); return GPK_NOT_FITTED; }
     return GPK_OK;
 }
 }  // namespace
@@ -3596,15 +3563,15 @@ int gpk_dngo_set_data(gpk_handle* h, const double* X, const double* y, int n, in
     if ((rc = scale_set(h, who, X, y, n, d, normalize_input != 0, normalize_output != 0, buf, &ym, &ysd))) return rc;
     CK(cudaSetDevice(h->device));
     h->model = MODEL_DNGO;
-    h->dngo_trained = h->dngo_fitted = h->blr_fitted = false;
-    h->dngo_t = -1;
+    h->dngo.trained = h->dngo.fitted = h->blr.fitted = false;
+    h->dngo.t = -1;
     h->n = n; h->d = d;
-    h->dngo_P = gpk_dngo_params(d);
-    h->bnn_ymean = ym; h->bnn_ystd = ysd;
-    h->blr_F = GPK_DNGO_H; h->blr_basis = GPK_BLR_NONE;
-    h->blr_prior.ln_sigma = prior_par[0]; h->blr_prior.ln_loc = prior_par[1]; h->blr_prior.hs_scale = prior_par[2];
-    if ((rc = ensure(h, h->bnn_data, buf.size() * 8))) return rc;
-    if ((rc = ensure(h, h->blr_data, ((size_t)n * GPK_DNGO_H + n + GPK_DNGO_H * GPK_DNGO_H + GPK_DNGO_H) * 8))) return rc;
+    h->dngo.P = gpk_dngo_params(d);
+    h->bnn.ymean = ym; h->bnn.ystd = ysd;
+    h->blr.F = GPK_DNGO_H; h->blr.basis = GPK_BLR_NONE;
+    h->blr.prior.ln_sigma = prior_par[0]; h->blr.prior.ln_loc = prior_par[1]; h->blr.prior.hs_scale = prior_par[2];
+    if ((rc = ensure(h, h->bnn.data, buf.size() * 8))) return rc;
+    if ((rc = ensure(h, h->blr.data, ((size_t)n * GPK_DNGO_H + n + GPK_DNGO_H * GPK_DNGO_H + GPK_DNGO_H) * 8))) return rc;
     CK(cudaMemcpyAsync(bnn_X(h), buf.data(), buf.size() * 8, cudaMemcpyHostToDevice, h->stream));
     CK(cudaMemcpyAsync(blr_y(h), buf.data() + (size_t)n * d, (size_t)n * 8, cudaMemcpyHostToDevice, h->stream));
     CK(cudaStreamSynchronize(h->stream));     // the staging vector dies here
@@ -3620,11 +3587,11 @@ int gpk_dngo_train(gpk_handle* h, unsigned long long seed, unsigned counter, dou
     const int B = std::min(batch, h->n);
     if (B > GPK_DNGO_MAX_BATCH)
         BAD("%s: a batch of min(batch, n) = %d rows exceeds GPK_DNGO_MAX_BATCH = %d", who, B, GPK_DNGO_MAX_BATCH);
-    const int P = h->dngo_P;
-    h->dngo_trained = h->dngo_fitted = h->blr_fitted = false;
-    h->dngo_t = -1;
-    if ((rc = ensure(h, h->dngo_net, (size_t)P * 8))) return rc;
-    if ((rc = ensure(h, h->dngo_state, (size_t)2 * P * 8))) return rc;
+    const int P = h->dngo.P;
+    h->dngo.trained = h->dngo.fitted = h->blr.fitted = false;
+    h->dngo.t = -1;
+    if ((rc = ensure(h, h->dngo.net, (size_t)P * 8))) return rc;
+    if ((rc = ensure(h, h->dngo.state, (size_t)2 * P * 8))) return rc;
     const size_t smem = (size_t)gpk_dngo_train_smem(h->n, h->d, B);
     CK(cudaFuncSetAttribute(gpk_dngo_train_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     DngoTrainArgs a;
@@ -3633,13 +3600,13 @@ int gpk_dngo_train(gpk_handle* h, unsigned long long seed, unsigned counter, dou
     a.n = h->n; a.d = h->d; a.P = P; a.B = B; a.epochs = epochs;
     a.seed = seed; a.counter = counter;
     a.lr = lr;
-    a.state = ptr<double>(h->dngo_state);
-    a.net = ptr<double>(h->dngo_net);
+    a.state = ptr<double>(h->dngo.state);
+    a.net = ptr<double>(h->dngo.net);
     a.Theta = blr_phi(h);
     gpk_dngo_train_kernel<<<1, GPK_DNGO_THREADS, smem, h->stream>>>(a);
     CKL();
     if ((rc = dngo_gram(h))) return rc;
-    h->dngo_t = (long long)epochs * (h->n / B);
+    h->dngo.t = (long long)epochs * (h->n / B);
     return GPK_OK;
 }
 
@@ -3649,15 +3616,15 @@ int gpk_dngo_fit(gpk_handle* h, const double* hypers, int k) {
     if (!rc) rc = blr_ready(h, who);
     if (!rc) rc = blr_fit(h, hypers, k, who);
     if (rc) return rc;
-    h->dngo_fitted = false;
+    h->dngo.fitted = false;
     const DngoPack K(h->d);
-    if ((rc = ensure(h, h->dngo_pack, (size_t)K.total * 8 + 8))) return rc;
-    double* pack = ptr<double>(h->dngo_pack);
+    if ((rc = ensure(h, h->dngo.pack, (size_t)K.total * 8 + 8))) return rc;
+    double* pack = ptr<double>(h->dngo.pack);
     int* fail = (int*)(pack + K.total);
     const BlrPost L(k, GPK_DNGO_H);
-    const double* post = ptr<double>(h->blr_post);
+    const double* post = ptr<double>(h->blr.post);
     gpk_dngo_collapse_kernel<<<1, GPK_BLR_THREADS, gpk_dngo_collapse_doubles() * 8, h->stream>>>(
-        post + L.M, post + L.S, post + L.ib, k, ptr<double>(h->dngo_net), h->d, pack, fail);
+        post + L.M, post + L.S, post + L.ib, k, ptr<double>(h->dngo.net), h->d, pack, fail);
     CKL();
     int f = 0;
     CK(cudaMemcpyAsync(&f, fail, 4, cudaMemcpyDeviceToHost, h->stream));
@@ -3666,7 +3633,7 @@ int gpk_dngo_fit(gpk_handle* h, const double* hypers, int k) {
         set_err(h, "%s: the mixture covariance mean S_i + cov(m_i) of the %d hypers is not positive definite", who, k);
         return GPK_NOT_PD;
     }
-    h->dngo_fitted = true;
+    h->dngo.fitted = true;
     return GPK_OK;
 }
 
@@ -3675,8 +3642,8 @@ int gpk_dngo_dims(gpk_handle* h, int* n, int* d, int* P, int* k) {
     if (rc) return rc;
     if (n) *n = h->n;
     if (d) *d = h->d;
-    if (P) *P = h->dngo_P;
-    if (k) *k = h->dngo_fitted ? h->blr_k : 0;
+    if (P) *P = h->dngo.P;
+    if (k) *k = h->dngo.fitted ? h->blr.k : 0;
     return GPK_OK;
 }
 
@@ -3685,7 +3652,7 @@ int gpk_dngo_get_net(gpk_handle* h, double* net) {
     int rc = dngo_trained(h, who);
     if (rc) return rc;
     if (!net) BAD("%s: need the output array", who);
-    CK(cudaMemcpyAsync(net, h->dngo_net.p, (size_t)h->dngo_P * 8, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaMemcpyAsync(net, h->dngo.net.p, (size_t)h->dngo.P * 8, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
     return GPK_OK;
 }
@@ -3695,15 +3662,15 @@ int gpk_dngo_set_net(gpk_handle* h, const double* net) {
     int rc = model_ready(h, MODEL_DNGO, who);
     if (rc) return rc;
     if (!net) BAD("%s: need the net", who);
-    const int P = h->dngo_P;
+    const int P = h->dngo.P;
     for (int i = 0; i < P; ++i)
         if (!std::isfinite(net[i])) BAD("%s: the net must be finite", who);
-    h->dngo_trained = h->dngo_fitted = h->blr_fitted = false;
-    h->dngo_t = -1;
-    if ((rc = ensure(h, h->dngo_net, (size_t)P * 8))) return rc;
-    CK(cudaMemcpyAsync(h->dngo_net.p, net, (size_t)P * 8, cudaMemcpyHostToDevice, h->stream));
+    h->dngo.trained = h->dngo.fitted = h->blr.fitted = false;
+    h->dngo.t = -1;
+    if ((rc = ensure(h, h->dngo.net, (size_t)P * 8))) return rc;
+    CK(cudaMemcpyAsync(h->dngo.net.p, net, (size_t)P * 8, cudaMemcpyHostToDevice, h->stream));
     gpk_dngo_features_kernel<<<(unsigned)h->n, 64, 0, h->stream>>>(bnn_X(h), h->n, h->d, nullptr, nullptr,
-                                                                   ptr<double>(h->dngo_net), blr_phi(h));
+                                                                   ptr<double>(h->dngo.net), blr_phi(h));
     CKL();
     return dngo_gram(h);
 }
@@ -3719,7 +3686,7 @@ int gpk_dngo_features(gpk_handle* h, const double* X, long m, double* out) {
     double* dO = dX + (size_t)m * h->d;
     CK(cudaMemcpyAsync(dX, X, xb, cudaMemcpyHostToDevice, h->stream));
     gpk_dngo_features_kernel<<<(unsigned)m, 64, 0, h->stream>>>(dX, m, h->d, bnn_xm(h), bnn_xs(h),
-                                                               ptr<double>(h->dngo_net), dO);
+                                                               ptr<double>(h->dngo.net), dO);
     CKL();
     CK(cudaMemcpyAsync(out, dO, ob, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
@@ -3730,11 +3697,11 @@ int gpk_dngo_get_state(gpk_handle* h, double* m, double* v, long long* t) {
     const char* who = "gpk_dngo_get_state";
     int rc = model_ready(h, MODEL_DNGO, who);
     if (rc) return rc;
-    if (h->dngo_t < 0) { set_err(h, "%s: no training has run (gpk_dngo_train)", who); return GPK_NOT_FITTED; }
-    const size_t P = h->dngo_P;
-    if (m) CK(cudaMemcpyAsync(m, ptr<double>(h->dngo_state), P * 8, cudaMemcpyDeviceToHost, h->stream));
-    if (v) CK(cudaMemcpyAsync(v, ptr<double>(h->dngo_state) + P, P * 8, cudaMemcpyDeviceToHost, h->stream));
-    if (t) *t = h->dngo_t;
+    if (h->dngo.t < 0) { set_err(h, "%s: no training has run (gpk_dngo_train)", who); return GPK_NOT_FITTED; }
+    const size_t P = h->dngo.P;
+    if (m) CK(cudaMemcpyAsync(m, ptr<double>(h->dngo.state), P * 8, cudaMemcpyDeviceToHost, h->stream));
+    if (v) CK(cudaMemcpyAsync(v, ptr<double>(h->dngo.state) + P, P * 8, cudaMemcpyDeviceToHost, h->stream));
+    if (t) *t = h->dngo.t;
     CK(cudaStreamSynchronize(h->stream));
     return GPK_OK;
 }
@@ -3791,9 +3758,9 @@ int gpk_nll_grad(gpk_handle* h, double noise_var, double* grad) {
         a.B = ptr<double>(h->Q); a.ldb = NP;
         a.C = ptr<double>(h->W); a.ldc = NP;
         a.alpha = 1.0; a.beta = 0;
-        a.jobs = ptr<GemmJob>(h->jobs) + h->kinv_r.off;
+        a.jobs = ptr<GemmJob>(h->jobs) + h->ranges.kinv.off;
         a.job_mode = JOBS_TABLE;
-        if ((rc = launch_gemm<EPI_STORE>(h, h->mapQ, h->mapQ, a, h->kinv_r.cnt))) return rc;
+        if ((rc = launch_gemm<EPI_STORE>(h, h->mapQ, h->mapQ, a, h->ranges.kinv.cnt))) return rc;
     }
     dim3 tg((unsigned)(NP / 128), (unsigned)(NP / 32));
     const long nblocks = (long)tg.x * tg.y;
@@ -3849,9 +3816,10 @@ int gpk_measure_fp64_peaks(gpk_handle* h, double* dmma_tflops, double* dfma_tflo
     const int blocks = prop.multiProcessorCount, warps = 16, threads = warps * 32, iters = 8000;
     int rc;
     if ((rc = ensure(h, h->tmp1, 64))) return rc;
-    cudaEvent_t e0, e1;
-    CK(cudaEventCreate(&e0));
-    CK(cudaEventCreate(&e1));
+    TimerEvents t;
+    CK(cudaEventCreate(&t.e0));
+    CK(cudaEventCreate(&t.e1));
+    const cudaEvent_t e0 = t.e0, e1 = t.e1;
     double best_mma = 0.0, best_fma = 0.0;
     for (int rep = 0; rep < 3; ++rep) {
         float ms = 0.f;
@@ -3870,8 +3838,6 @@ int gpk_measure_fp64_peaks(gpk_handle* h, double* dmma_tflops, double* dfma_tflo
         CK(cudaEventElapsedTime(&ms, e0, e1));
         best_fma = std::max(best_fma, 2.0 * 8 * (double)iters * threads * blocks / (ms * 1e-3) / 1e12);
     }
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
     if (dmma_tflops) *dmma_tflops = best_mma;
     if (dfma_tflops) *dfma_tflops = best_fma;
     return GPK_OK;
@@ -3883,9 +3849,10 @@ int gpk_measure_int8_peak(gpk_handle* h, double* tops) {
     const int blocks = std::max(h->n_sm, 1), iters = 4000, smem = 2 * 8192 + 1024 + 64;
     int rc;
     if ((rc = ensure(h, h->tmp1, 64))) return rc;
-    cudaEvent_t e0, e1;
-    CK(cudaEventCreate(&e0));
-    CK(cudaEventCreate(&e1));
+    TimerEvents t;
+    CK(cudaEventCreate(&t.e0));
+    CK(cudaEventCreate(&t.e1));
+    const cudaEvent_t e0 = t.e0, e1 = t.e1;
     double best = 0.0;
     for (int rep = 0; rep < 3; ++rep) {
         float ms = 0.f;
@@ -3897,8 +3864,6 @@ int gpk_measure_int8_peak(gpk_handle* h, double* tops) {
         CK(cudaEventElapsedTime(&ms, e0, e1));
         best = std::max(best, 2.0 * 128 * 128 * 32 * 2.0 * iters * blocks / (ms * 1e-3) / 1e12);
     }
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
     *tops = best;
     return GPK_OK;
 }
@@ -3912,9 +3877,10 @@ int gpk_measure_int8_peak_sustained(gpk_handle* h, double seconds, int random_op
     const double ops = 2.0 * 128 * 128 * 32 * 2.0 * iters * blocks;
     int rc;
     if ((rc = ensure(h, h->tmp1, 64))) return rc;
-    cudaEvent_t e0, e1;
-    CK(cudaEventCreate(&e0));
-    CK(cudaEventCreate(&e1));
+    TimerEvents t;
+    CK(cudaEventCreate(&t.e0));
+    CK(cudaEventCreate(&t.e1));
+    const cudaEvent_t e0 = t.e0, e1 = t.e1;
     float ms1 = 0.f;
     CK(cudaEventRecord(e0, h->stream));
     gpk_peak_i8_kernel<<<blocks, 256, smem, h->stream>>>(iters, random_operands, ptr<unsigned>(h->tmp1));
@@ -3931,8 +3897,6 @@ int gpk_measure_int8_peak_sustained(gpk_handle* h, double seconds, int random_op
     CK(cudaEventSynchronize(e1));
     float ms = 0.f;
     CK(cudaEventElapsedTime(&ms, e0, e1));
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
     *tops = ops * n_half / (ms * 1e-3) / 1e12;
     return GPK_OK;
 }
@@ -3989,8 +3953,8 @@ int gpk_oz_contract(gpk_handle* h, const double* P, int n, const double* Ks, lon
     const size_t oK = (size_t)NP * NP * 8, oPq = oK + (size_t)MP * NP * 8, oKq = oPq + (size_t)OZ_S * NP * NP;
     const size_t opart = oKq + (size_t)OZ_S * MP * NP, oe = opart + (size_t)nb * MP * 8, oemax = oe + (size_t)NP * 4;
     int rc;
-    if ((rc = ensure(h, h->oz_probe, oemax + 4))) return rc;
-    char* b = (char*)h->oz_probe.p;
+    if ((rc = ensure(h, h->oz.probe, oemax + 4))) return rc;
+    char* b = (char*)h->oz.probe.p;
     double* dP = (double*)b;
     double* dK = (double*)(b + oK);
     int8_t* dPq = (int8_t*)(b + oPq);
@@ -4012,7 +3976,7 @@ int gpk_oz_contract(gpk_handle* h, const double* P, int n, const double* Ks, lon
     gpk_oz_split_kernel<<<(unsigned)((MP * NP + 255) / 256), 256, 0, st>>>(dK, MP, NP, nullptr, ek, dKq, MP * NP);
     CKL();
     CUtensorMap mapP, mapK;
-    if ((rc = make_oz_map(h, &mapP, dPq, (long)OZ_S * NP, NP, OZ_TM / h->oz_cluster))) return rc;
+    if ((rc = make_oz_map(h, &mapP, dPq, (long)OZ_S * NP, NP, OZ_TM / h->oz.cluster))) return rc;
     if ((rc = make_oz_map(h, &mapK, dKq, (long)OZ_S * MP, NP, OZ_TN))) return rc;
     if ((rc = launch_oz_contraction(h, mapP, mapK, (int)nb, MP, NP, MP, de, ek, dpart, MP))) return rc;
     CK(cudaMemcpy2DAsync(part_ssq, (size_t)m * 8, dpart, (size_t)MP * 8, (size_t)m * 8, (size_t)nb, cudaMemcpyDeviceToHost, st));
@@ -4033,8 +3997,8 @@ int gpk_ep_joint_min(gpk_handle* h, const double* mu, const double* V, int nb, d
     const size_t omu = 0, oV = omu + D, oP = oV + D * D, odM = oP + D, odMM = odM + D * D, odS = odMM + D * D * D;
     const size_t oZm = odS + D * T, oZs = oZm + D, oad = oZs + T, oint = oad + D * D;
     int rc;
-    if ((rc = ensure(h, h->ep_buf, oint * 8 + 2 * D * 4))) return rc;
-    double* b = ptr<double>(h->ep_buf);
+    if ((rc = ensure(h, h->multi.ep_buf, oint * 8 + 2 * D * 4))) return rc;
+    double* b = ptr<double>(h->multi.ep_buf);
     int* dsw = (int*)(b + oint);
     int* dst = dsw + D;
     cudaStream_t st = h->stream;
@@ -4098,8 +4062,8 @@ int gpk_es_update(gpk_handle* h, const double* zb, int nb, const double* lmb, do
                 Hs[i * T + a * (a + 1) / 2 + b] = a == b ? dMuMu[(i * D + a) * D + a]
                                                          : dMuMu[(i * D + a) * D + b] + dMuMu[(i * D + b) * D + a];
     EsLayout L(nb, np_, d);
-    if ((rc = ensure(h, h->es_state, L.total * 8))) return rc;
-    double* st = ptr<double>(h->es_state);
+    if ((rc = ensure(h, h->es.state, L.total * 8))) return rc;
+    double* st = ptr<double>(h->es.state);
     cudaStream_t s = h->stream;
     CK(cudaMemcpyAsync(st + L.logP, lp.data(), D * 8, cudaMemcpyHostToDevice, s));
     CK(cudaMemcpyAsync(st + L.lmb, lmb, D * 8, cudaMemcpyHostToDevice, s));
@@ -4112,12 +4076,12 @@ int gpk_es_update(gpk_handle* h, const double* zb, int nb, const double* lmb, do
     // scaled zb, then U = L^-T (L^-1 K(X, zb)) in fp64 from the handle's L^-1
     if ((rc = es_build_u(h, zb, nb, st + L.zb))) return rc;
     CK(cudaStreamSynchronize(s));
-    h->es_nb = nb;
-    h->es_np = np_;
-    h->es_sn2 = sn2;
-    h->es_H = H;
-    h->es_linv_serial = h->linv_serial;
-    h->es_kind = ES_KIND_EP;
+    h->es.nb = nb;
+    h->es.np = np_;
+    h->es.sn2 = sn2;
+    h->es.H = H;
+    h->es.linv_serial = h->linv_serial;
+    h->es.kind = ES_KIND_EP;
     if (logP) std::copy(lp.begin(), lp.end(), logP);
     if (dlogPdMu) std::copy(dMu.begin(), dMu.end(), dlogPdMu);
     if (dlogPdSigma) std::copy(dSig.begin(), dSig.end(), dlogPdSigma);
@@ -4139,8 +4103,8 @@ int gpk_es_compute(gpk_handle* h, const double* Xs, long m, double* out) {
     if (rc) return rc;
     if (!Xs || !out || m <= 0) BAD("gpk_es_compute: need candidates and out");
     CK(cudaSetDevice(h->device));
-    if ((rc = ensure(h, h->es_in, (size_t)m * (h->d + 1) * 8))) return rc;
-    double* dX = ptr<double>(h->es_in);
+    if ((rc = ensure(h, h->es.in, (size_t)m * (h->d + 1) * 8))) return rc;
+    double* dX = ptr<double>(h->es.in);
     double* dout = dX + (size_t)m * h->d;
     CK(cudaMemcpyAsync(dX, Xs, (size_t)m * h->d * 8, cudaMemcpyHostToDevice, h->stream));
     if ((rc = gpk_es_compute_dev(h, dX, m, dout))) return rc;
@@ -4155,11 +4119,11 @@ int gpk_es_moments(gpk_handle* h, const double* Xs, long m, double* var, double*
     if (!Xs || !var || !sigma || m <= 0) BAD("gpk_es_moments: need candidates, var and sigma");
     if ((rc = es_ready(h, nullptr, "gpk_es_moments", ES_KIND_NONE))) return rc;
     CK(cudaSetDevice(h->device));
-    const int nb = h->es_nb, d = h->d;
+    const int nb = h->es.nb, d = h->d;
     if ((rc = es_reserve(h))) return rc;
-    if ((rc = ensure(h, h->es_in, (size_t)m * d * 8))) return rc;
-    double* dX = ptr<double>(h->es_in);
-    const double* dvar = ptr<double>(h->es_work);
+    if ((rc = ensure(h, h->es.in, (size_t)m * d * 8))) return rc;
+    double* dX = ptr<double>(h->es.in);
+    const double* dvar = ptr<double>(h->es.work);
     const double* dsig = dvar + ES_CH;
     CK(cudaMemcpyAsync(dX, Xs, (size_t)m * d * 8, cudaMemcpyHostToDevice, h->stream));
     for (long c0 = 0; c0 < m; c0 += ES_CH) {          // the passes of es_dh_dev, each read back before the next
@@ -4178,7 +4142,7 @@ int gpk_es_dims(gpk_handle* h, int* n, int* nb) {
     if (!n || !nb) BAD("gpk_es_dims: null output");
     if ((rc = es_ready(h, nullptr, "gpk_es_dims", ES_KIND_NONE))) return rc;
     *n = h->n;
-    *nb = h->es_nb;
+    *nb = h->es.nb;
     return GPK_OK;
 }
 
@@ -4188,7 +4152,7 @@ int gpk_es_get_u(gpk_handle* h, double* U) {
     if (!U) BAD("gpk_es_get_u: null output");
     if ((rc = es_ready(h, nullptr, "gpk_es_get_u", ES_KIND_NONE))) return rc;
     CK(cudaSetDevice(h->device));
-    CK(cudaMemcpyAsync(U, h->es_U.p, (size_t)h->n * h->es_nb * 8, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaMemcpyAsync(U, h->es.U.p, (size_t)h->n * h->es.nb * 8, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
     return GPK_OK;
 }
@@ -4200,11 +4164,11 @@ int gpk_mc_draws(gpk_handle* h, unsigned long long seed, int nb, int nf, double*
     CK(cudaSetDevice(h->device));
     const size_t bytes = (size_t)nb * nf * 8;
     int rc;
-    if ((rc = ensure(h, h->mc_buf, bytes))) return rc;
+    if ((rc = ensure(h, h->mc.buf, bytes))) return rc;
     const long work = (long)nb * ((nf + 1) / 2);
-    gpk_mc_draws_kernel<<<(unsigned)((work + 255) / 256), 256, 0, h->stream>>>(seed, nb, nf, ptr<double>(h->mc_buf));
+    gpk_mc_draws_kernel<<<(unsigned)((work + 255) / 256), 256, 0, h->stream>>>(seed, nb, nf, ptr<double>(h->mc.buf));
     CKL();
-    CK(cudaMemcpyAsync(F, h->mc_buf.p, bytes, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaMemcpyAsync(F, h->mc.buf.p, bytes, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
     return GPK_OK;
 }
@@ -4226,8 +4190,8 @@ int gpk_mc_pmin(gpk_handle* h, const double* m, int np_, const double* V, int nb
     CK(cudaSetDevice(h->device));
     // scratch in doubles: m (nb x np), V (nb x nb), F (nb x nf), pmin (nb), then the status words
     const size_t om = 0, oV = om + (size_t)nb * np_, oF = oV + (size_t)nb * nb, oP = oF + (size_t)nb * nf, oS = oP + nb;
-    if ((rc = ensure(h, h->mc_buf, oS * 8 + 2 * sizeof(int)))) return rc;
-    double* b = ptr<double>(h->mc_buf);
+    if ((rc = ensure(h, h->mc.buf, oS * 8 + 2 * sizeof(int)))) return rc;
+    double* b = ptr<double>(h->mc.buf);
     int* dst = (int*)(b + oS);
     cudaStream_t st = h->stream;
     CK(cudaMemcpyAsync(b + om, m, (size_t)nb * np_ * 8, cudaMemcpyHostToDevice, st));
@@ -4243,7 +4207,7 @@ int gpk_mc_pmin(gpk_handle* h, const double* m, int np_, const double* V, int nb
     CKL();
     CK(cudaMemcpyAsync(pmin, b + oP, (size_t)nb * 8, cudaMemcpyDeviceToHost, st));
     if ((rc = mc_stat_check(h, dst, "gpk_mc_pmin"))) return rc;
-    if (n_jitter) *n_jitter = (int)h->mc_last_jitter;
+    if (n_jitter) *n_jitter = (int)h->mc.last_jitter;
     return GPK_OK;
 }
 
@@ -4257,12 +4221,12 @@ int gpk_esmc_update(gpk_handle* h, const double* zb, int nb, const double* lmb, 
         if (!std::isfinite(lmb[i])) BAD("lmb should not be infinite.");
     const int d = h->d;
     const size_t D = (size_t)nb;
-    h->es_linv_serial = -1;                     // no update is current until this one completes
+    h->es.linv_serial = -1;                     // no update is current until this one completes
     std::vector<double> mu(D), V(D * D), pm(D);
     if ((rc = gpk_predict_cov(h, zb, nb, mu.data(), V.data()))) return rc;          // predict(zb, full_cov=True)
     McLayout L(nb, np_, d, nf);
-    if ((rc = ensure(h, h->mc_state, L.total * 8))) return rc;
-    double* st = ptr<double>(h->mc_state);
+    if ((rc = ensure(h, h->mc.state, L.total * 8))) return rc;
+    double* st = ptr<double>(h->mc.state);
     cudaStream_t s = h->stream;
     CK(cudaMemcpyAsync(st + L.Mb, mu.data(), D * 8, cudaMemcpyHostToDevice, s));
     CK(cudaMemcpyAsync(st + L.Vb, V.data(), D * D * 8, cudaMemcpyHostToDevice, s));
@@ -4272,15 +4236,15 @@ int gpk_esmc_update(gpk_handle* h, const double* zb, int nb, const double* lmb, 
     gpk_mc_draws_kernel<<<(unsigned)((work + 255) / 256), 256, 0, s>>>(seed, nb, nf, st + L.F);
     CKL();
     // pmin = joint_pmin(Mb, Vb, Nf) with Mb as (Nb, 1): one column of innovations
-    if ((rc = ensure(h, h->mc_buf, D * 8))) return rc;
+    if ((rc = ensure(h, h->mc.buf, D * 8))) return rc;
     if ((rc = mc_stat_reset(h))) return rc;
     if ((rc = mc_kernel_attrs(h))) return rc;
     gpk_mc_pmin_kernel<<<1, GPK_MC_THREADS, GPK_MC_SMEM, s>>>(st + L.Mb, nullptr, nullptr, 1, st + L.Vb, nb, st + L.F, nf,
                                                                 nullptr, nullptr, 0.0, nullptr, 0.0, nullptr,
-                                                                ptr<double>(h->mc_buf), nullptr, ptr<int>(h->mc_stat));
+                                                                ptr<double>(h->mc.buf), nullptr, ptr<int>(h->mc.stat));
     CKL();
-    CK(cudaMemcpyAsync(pm.data(), h->mc_buf.p, D * 8, cudaMemcpyDeviceToHost, s));
-    if ((rc = mc_stat_check(h, ptr<int>(h->mc_stat), "gpk_esmc_update"))) return rc;
+    CK(cudaMemcpyAsync(pm.data(), h->mc.buf.p, D * 8, cudaMemcpyDeviceToHost, s));
+    if ((rc = mc_stat_check(h, ptr<int>(h->mc.stat), "gpk_esmc_update"))) return rc;
     // logP = log(pmin); H of the loss (information_gain.py:82), summed in index order
     std::vector<double> lp(D);
     double H = 0.0;
@@ -4291,13 +4255,13 @@ int gpk_esmc_update(gpk_handle* h, const double* zb, int nb, const double* lmb, 
     H = -H;
     if ((rc = es_build_u(h, zb, nb, st + L.zb))) return rc;
     CK(cudaStreamSynchronize(s));
-    h->es_nb = nb;
-    h->es_np = np_;
-    h->es_nf = nf;
-    h->es_sn2 = sn2;
-    h->es_H = H;
-    h->es_linv_serial = h->linv_serial;
-    h->es_kind = ES_KIND_MC;
+    h->es.nb = nb;
+    h->es.np = np_;
+    h->mc.nf = nf;
+    h->es.sn2 = sn2;
+    h->es.H = H;
+    h->es.linv_serial = h->linv_serial;
+    h->es.kind = ES_KIND_MC;
     if (logP) std::copy(lp.begin(), lp.end(), logP);
     if (pmin) std::copy(pm.begin(), pm.end(), pmin);
     return GPK_OK;
@@ -4310,7 +4274,7 @@ int gpk_esmc_compute_dev(gpk_handle* h, const void* d_Xs, long m, void* d_out) {
     if ((rc = es_ready(h, nullptr, "gpk_esmc_compute", ES_KIND_MC))) return rc;
     CK(cudaSetDevice(h->device));
     if ((rc = mc_stat_reset(h))) return rc;
-    return esmc_dev(h, (const double*)d_Xs, m, (double*)d_out, ptr<int>(h->mc_stat));
+    return esmc_dev(h, (const double*)d_Xs, m, (double*)d_out, ptr<int>(h->mc.stat));
 }
 
 int gpk_esmc_compute(gpk_handle* h, const double* Xs, long m, double* out) {
@@ -4319,13 +4283,13 @@ int gpk_esmc_compute(gpk_handle* h, const double* Xs, long m, double* out) {
     if (!Xs || !out || m <= 0) BAD("gpk_esmc_compute: need candidates and out");
     CK(cudaSetDevice(h->device));
     if ((rc = es_ready(h, nullptr, "gpk_esmc_compute", ES_KIND_MC))) return rc;
-    if ((rc = ensure(h, h->es_in, (size_t)m * (h->d + 1) * 8))) return rc;
-    double* dX = ptr<double>(h->es_in);
+    if ((rc = ensure(h, h->es.in, (size_t)m * (h->d + 1) * 8))) return rc;
+    double* dX = ptr<double>(h->es.in);
     double* dout = dX + (size_t)m * h->d;
     CK(cudaMemcpyAsync(dX, Xs, (size_t)m * h->d * 8, cudaMemcpyHostToDevice, h->stream));
     if ((rc = gpk_esmc_compute_dev(h, dX, m, dout))) return rc;
     CK(cudaMemcpyAsync(out, dout, (size_t)m * 8, cudaMemcpyDeviceToHost, h->stream));
-    return mc_stat_check(h, ptr<int>(h->mc_stat), "gpk_esmc_compute");
+    return mc_stat_check(h, ptr<int>(h->mc.stat), "gpk_esmc_compute");
 }
 
 int gpk_esmc_get_draws(gpk_handle* h, double* F) {
@@ -4334,8 +4298,8 @@ int gpk_esmc_get_draws(gpk_handle* h, double* F) {
     if (!F) BAD("gpk_esmc_get_draws: null output");
     if ((rc = es_ready(h, nullptr, "gpk_esmc_get_draws", ES_KIND_MC))) return rc;
     CK(cudaSetDevice(h->device));
-    const McLayout L(h->es_nb, h->es_np, h->d, h->es_nf);
-    CK(cudaMemcpyAsync(F, ptr<double>(h->mc_state) + L.F, (size_t)h->es_nb * h->es_nf * 8, cudaMemcpyDeviceToHost,
+    const McLayout L(h->es.nb, h->es.np, h->d, h->mc.nf);
+    CK(cudaMemcpyAsync(F, ptr<double>(h->mc.state) + L.F, (size_t)h->es.nb * h->mc.nf * 8, cudaMemcpyDeviceToHost,
                        h->stream));
     CK(cudaStreamSynchronize(h->stream));
     return GPK_OK;
@@ -4347,9 +4311,9 @@ int gpk_esmc_get_state(gpk_handle* h, double* Mb, double* Vb) {
     if (!Mb || !Vb) BAD("gpk_esmc_get_state: null output");
     if ((rc = es_ready(h, nullptr, "gpk_esmc_get_state", ES_KIND_MC))) return rc;
     CK(cudaSetDevice(h->device));
-    const int nb = h->es_nb;
-    const McLayout L(nb, h->es_np, h->d, h->es_nf);
-    const double* st = ptr<double>(h->mc_state);
+    const int nb = h->es.nb;
+    const McLayout L(nb, h->es.np, h->d, h->mc.nf);
+    const double* st = ptr<double>(h->mc.state);
     CK(cudaMemcpyAsync(Mb, st + L.Mb, (size_t)nb * 8, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaMemcpyAsync(Vb, st + L.Vb, (size_t)nb * nb * 8, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
@@ -4359,7 +4323,7 @@ int gpk_esmc_get_state(gpk_handle* h, double* Mb, double* Vb) {
 int gpk_esmc_last_jitter(gpk_handle* h, long* n_jitter) {
     if (!h) return GPK_BAD_ARG;
     if (!n_jitter) BAD("gpk_esmc_last_jitter: null output");
-    *n_jitter = h->mc_last_jitter;
+    *n_jitter = h->mc.last_jitter;
     return GPK_OK;
 }
 
@@ -4378,32 +4342,32 @@ int gpk_get_timings(gpk_handle* h, double* out /* 16 */) {
     CK(cudaStreamSynchronize(h->stream));
     for (int i = 0; i < 16; ++i) out[i] = 0.0;
     float ms = 0.f;
-    if (h->fit_timed) {
-        if (cudaEventElapsedTime(&ms, h->ev[0], h->ev[3]) == cudaSuccess) out[0] = ms;
-        if (cudaEventElapsedTime(&ms, h->ev[0], h->ev[1]) == cudaSuccess) out[1] = ms;
-        if (cudaEventElapsedTime(&ms, h->ev[1], h->ev[2]) == cudaSuccess) out[2] = ms;
+    if (h->timing.fit_timed) {
+        if (cudaEventElapsedTime(&ms, h->timing.ev[0], h->timing.ev[3]) == cudaSuccess) out[0] = ms;
+        if (cudaEventElapsedTime(&ms, h->timing.ev[0], h->timing.ev[1]) == cudaSuccess) out[1] = ms;
+        if (cudaEventElapsedTime(&ms, h->timing.ev[1], h->timing.ev[2]) == cudaSuccess) out[2] = ms;
     }
-    if (h->linv_ready && cudaEventElapsedTime(&ms, h->ev[4], h->ev[5]) == cudaSuccess) out[3] = ms;
-    if (h->score_timed) {
-        if (cudaEventElapsedTime(&ms, h->ev[6], h->ev[7]) == cudaSuccess) out[4] = ms;
-        if (cudaEventElapsedTime(&ms, h->ev[8], h->ev[10]) == cudaSuccess) out[5] = ms;    // K* of the last chunk
+    if (h->linv_ready && cudaEventElapsedTime(&ms, h->timing.ev[4], h->timing.ev[5]) == cudaSuccess) out[3] = ms;
+    if (h->timing.score_timed) {
+        if (cudaEventElapsedTime(&ms, h->timing.ev[6], h->timing.ev[7]) == cudaSuccess) out[4] = ms;
+        if (cudaEventElapsedTime(&ms, h->timing.ev[8], h->timing.ev[10]) == cudaSuccess) out[5] = ms;    // K* of the last chunk
         // variance GEMM: mean over the FULL-SIZE chunk launches of the last scoring call (the last chunk
         // is included only when it is the only one)
         double sum = 0.0;
         int cnt = 0;
-        const int nfull = h->last_nchunks > 1 ? h->last_nchunks - 1 : h->last_nchunks;
-        for (int i = 0; i < nfull && i < (int)h->ev_g0.size(); ++i)
-            if (cudaEventElapsedTime(&ms, h->ev_g0[i], h->ev_g1[i]) == cudaSuccess) { sum += ms; ++cnt; }
+        const int nfull = h->timing.last_nchunks > 1 ? h->timing.last_nchunks - 1 : h->timing.last_nchunks;
+        for (int i = 0; i < nfull && i < (int)h->timing.ev_g0.size(); ++i)
+            if (cudaEventElapsedTime(&ms, h->timing.ev_g0[i], h->timing.ev_g1[i]) == cudaSuccess) { sum += ms; ++cnt; }
         if (cnt > 0) out[6] = sum / cnt;
-        if (cudaEventElapsedTime(&ms, h->ev[11], h->ev[12]) == cudaSuccess) out[7] = ms;   // epilogue, last chunk
+        if (cudaEventElapsedTime(&ms, h->timing.ev[11], h->timing.ev[12]) == cudaSuccess) out[7] = ms;   // epilogue, last chunk
     }
     cudaGetLastError();
-    out[8] = h->launches_var;
-    out[9] = h->launches_total;
-    out[10] = h->oz_launches;
-    out[11] = (double)h->oz_emax_host;
+    out[8] = h->timing.launches_var;
+    out[9] = h->timing.launches_total;
+    out[10] = h->oz.launches;
+    out[11] = (double)h->oz.emax_host;
     out[13] = (double)OZ_PAIRS;
-    out[14] = (double)h->oz_last_variant;
+    out[14] = (double)h->oz.last_variant;
     return GPK_OK;
 }
 
